@@ -1,7 +1,7 @@
 """Drop-in for `src.atlas.Atlas` (reference src/atlas.py:42-647): the retrieve-then-read step that
 `train.py` / `evaluate.py` drive, on top of the B200 index, Contriever and FiD of this package.
 
-Same constructor, method names, argument meaning and return types as the reference class (SURVEY.md §8b):
+Same constructor, method names, argument meaning and return types as the reference class:
 `build_index`, `retrieve` / `_retrieve` / `retrieve_with_rerank`, `tokenize` / `retriever_tokenize` /
 `reader_tokenize` / `tokenize_passages`, `forward -> (reader_loss, retriever_loss)`, the four gold-score
 modes, `kldivloss`, `logprob`, `compute_reader_loss_and_logits`, `generate`.  What is different underneath:
@@ -12,10 +12,10 @@ modes, `kldivloss`, `logprob`, `compute_reader_loss_and_logits`, `generate`.  Wh
     no transposed strided write;
   * `_retrieve` embeds the queries with the B200 Contriever kernels and runs the fused scan + top-k
     (`DistributedIndex.search_knn`); the passage dicts come from the node-shared store;
-  * the reader passes run on the tcgen05 FiD kernels (`atlas_b200.fid.FiD`).
+  * the reader passes run on the wgmma FiD kernels (`atlas_b200.fid.FiD`).
 
 Tokenisation, string formatting and the loss arithmetic on `[bsz, n_context]` tensors stay on the host / in
-plain torch exactly as the reference does them: they are not on the measured path (SURVEY.md §8a last column).
+plain torch exactly as the reference does them: they are not on the measured path.
 """
 import math
 import time

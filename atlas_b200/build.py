@@ -1,5 +1,5 @@
-"""In-tree build of `lib/libatlas_b200.so` with nvcc for sm_100a (no JIT cache: the built .so
-travels to the GPU box with the repo snapshot).  Every .cu under csrc/ is compiled to an object file in
+"""In-tree build of `lib/libatlas_b200.so` with nvcc for sm_90a (H100; no JIT cache: the library is built next to the
+sources by `__graft_entry__.build()`).  Every .cu under csrc/ is compiled to an object file in
 parallel (only the stale ones), then linked into one shared library."""
 import glob
 import os
@@ -15,9 +15,9 @@ LIB = os.path.join(LIB_DIR, "libatlas_b200.so")
 
 NVCC_FLAGS = [
     "-Xcompiler", "-fPIC", "-std=c++17", "-O3", "-lineinfo",
-    "-gencode", "arch=compute_100a,code=sm_100a",
+    "-gencode", "arch=compute_90a,code=sm_90a",
 ]
-LINK_FLAGS = ["-shared", "-Xcompiler", "-fPIC", "-cudart", "static", "-gencode", "arch=compute_100a,code=sm_100a"]
+LINK_FLAGS = ["-shared", "-Xcompiler", "-fPIC", "-cudart", "static", "-gencode", "arch=compute_90a,code=sm_90a"]
 
 
 def _nvcc():

@@ -1,26 +1,27 @@
-// Fused multi-head attention (head_dim 64, <= 512 keys per segment) on tcgen05 for the Contriever and
-// FiD encoders and the FiD decoder's self-attention:
+// Fused multi-head attention (head_dim 64, <= 576 keys per segment) on Hopper warpgroup MMAs for the Contriever and FiD
+// encoders and the FiD decoder's self- and cross-attention:
 //     O[b, i, h, :] = softmax_j( scale * Q[b,i,h,:].K[b,j,h,:] + rel_bias[h, j-i] + key_mask[b, j] (+ causal) ) V[b, j, h, :]
 // Replaces, per layer, two batched cuBLAS GEMMs + the materialised [B, H, L, L] score / probability tensors +
 // the ATen softmax / mask / bias kernels of
 //     BertSelfAttention.forward  src/modeling_bert.py:328-366   (scale 1/8, additive key mask, fp32 softmax)
 //     T5Attention.forward        src/modeling_t5.py:478-524      (no scaling, relative-position bias + mask
 //                                                                 added to the scores, fp32 softmax)
-// Q, K, V are read IN PLACE from the fused projection output ([tokens, n_cols] row-major, head h at a
-// column offset) through TMA boxes {64 columns, 128 rows}; nothing is transposed or re-laid-out:
-//   S = Q K^T : A = Q tile (K-major, 128B swizzle), B = K rows (K-major)  -> fp32 S in TMEM, one column per key
-//   P V       : A = P from TENSOR MEMORY (16-bit, two keys per column, written by tcgen05.st over the S columns
-//               it replaces), B = V rows as they lie in memory = MN-major operand (head_dim contiguous)
-// Because a whole segment's keys fit in TMEM (<= 512 columns) the softmax is exact two-pass (row max, then
-// exp / sum) with no online rescaling.  One CTA works on one (segment, head) at a time: K and V are loaded once
-// and reused by all of its 128-row query tiles.
+// Q, K, V are read IN PLACE from the fused projection output ([tokens, n_cols] row-major, head h at a column offset)
+// through TMA boxes of {64 columns, 64 rows} with the 128-byte swizzle; nothing is transposed or re-laid-out:
+//   S = Q K^T : wgmma m64n64k16, A = Q rows (K-major), B = K rows (K-major)          -> fp32 S in registers
+//   O += P V  : wgmma m64n64k16, A = P from REGISTERS (the S fragment rounded to 16 bits),
+//               B = V rows as they lie in memory = MN-major operand (transpose flag)
+// One CTA = one (segment, head, 128-row query tile): the segment's K and V (<= 576 keys, 72 KB each) and the query tile land in
+// shared memory through one mbarrier; two warpgroups own 64 query rows each and sweep the 64-key blocks with an online
+// (flash-attention) softmax in the log2 domain.  Key blocks whose keys are all masked out (key_block_live) are skipped: their
+// probabilities are exactly 0 in fp32.
 //
-// Roles (608 threads): warp 0 TMA producer, warp 1 MMA issuer, warp 2 TMEM allocator + per-item mask / bias
-// tables (double buffered, one item ahead), warps 3-18 softmax + output (four threads per query row = TMEM lane).
-// With <= 384 keys the output of query tile t-1 is written while the tensor pipe runs P.V(t) and S(t+1).
+// Packed layout (seg_tile != nullptr, the padding-compacted FiD encoder): segment b keeps the first popcount(blk_live[b, :]) of
+// its 64-row tiles, stored back to back from row 64 * seg_tile[b * nb] of q / k / v / out; query tiles past them do not exist.
 #include "common.cuh"
 #include "dropout.cuh"
 #include "host_common.h"
+#include "wgmma.cuh"
 
 #include <math.h>
 #include <stdlib.h>
@@ -28,21 +29,15 @@
 namespace attn {
 
 constexpr int D = 64;            // head dim
-constexpr int BLOCK_Q = 128;
-constexpr int MAX_LK = 512;
-constexpr int SPLIT = 4;                       // softmax threads per query row (key chunks part, part+SPLIT, ...)
-constexpr int SM_THREADS = 128 * SPLIT;         // softmax / output threads (warps 4..), 4 warps per SM sub-partition
-constexpr int THREADS = 96 + SM_THREADS;           // 19 warps -> 104 registers per thread
-// attention_split_kernel: 2 softmax threads per query row, each keeping its <= 96 score columns of a key half in
-// registers between the two softmax passes (register files are allocated per 4 warps: 20 warps cap at 96 registers)
-constexpr int SPLIT2 = 2;
-constexpr int SM_THREADS2 = 128 * SPLIT2;
-constexpr int THREADS_SPLIT = 64 + SM_THREADS2;    // producer/aux warp, MMA warp, 8 softmax warps
-constexpr int AUX_THREADS = 32;                 // warp 2: per-item mask / bias tables, one item ahead
-constexpr int Q_BYTES = BLOCK_Q * D * 2;        // 16 KB, double buffered
-constexpr int KV_BYTES = MAX_LK * D * 2;        // 64 KB each
-constexpr int SMEM_BYTES = 2 * Q_BYTES + 2 * KV_BYTES + 1024;
-constexpr int TMEM_COLS = 512;
+constexpr int BQ = 128;          // query rows per CTA (two warpgroups x 64)
+constexpr int BK = 64;           // keys per block
+constexpr int MAX_BLOCKS = 9;
+constexpr int MAX_LK = MAX_BLOCKS * BK;        // 576
+constexpr int THREADS = 256;
+constexpr int TILE_BYTES = BK * D * 2;         // 8 KB: 64 rows x 128 bytes
+constexpr int Q_BYTES = BQ * D * 2;
+constexpr int KV_BYTES = MAX_LK * D * 2;
+constexpr int SMEM_BYTES = 1024 + Q_BYTES + 2 * KV_BYTES;
 constexpr float LOG2E = 1.4426950408889634f;
 
 struct Params {
@@ -60,48 +55,16 @@ struct Params {
     float* o_partial;         // [B*Lq, H*64] fp32 or nullptr
     float* ml_partial;        // [B*Lq, H, 2] fp32
     float* lse_out;           // [B, H, Lq] fp32 row log-sum-exp (natural log) for the backward pass, or nullptr
-    abdrop::Key drop;         // attention-probability dropout (training path, attention_kernel only); thr16 == 0: off
+    abdrop::Key drop;         // attention-probability dropout (training path); thr16 == 0: off
+    const uint8_t* blk_live;  // [B, ceil(Lk / 64)] or nullptr: 0 = every key of the block is masked out
+    const int32_t* seg_tile;  // nullptr, or [B * Lk / 64]: packed layout (see above); needs Lq == Lk and blk_live
+    int n_qt;                 // query tiles per segment (grid.x)
 };
-
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, uint32_t (&r)[16]) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-          "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-        : "r"(taddr));
-}
-
-__device__ __forceinline__ void tmem_st16(uint32_t taddr, const uint32_t (&r)[16]) {
-    asm volatile(
-        "tcgen05.st.sync.aligned.32x32b.x16.b32 [%0], "
-        "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16};" ::"r"(taddr),
-        "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]), "r"(r[8]), "r"(r[9]),
-        "r"(r[10]), "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15])
-        : "memory");
-}
-
-// smem descriptor of an MN-major operand tile stored as rows of 128 bytes (64 x 16-bit along MN) with the 128B
-// swizzle: 8-row (K) groups are 1024 bytes apart (SBO); LBO (stride between 64-element MN blocks) is unused for N = 64.
-__device__ __forceinline__ uint64_t umma_desc_mn_sw128(uint32_t smem_addr) {
-    uint64_t d = 0;
-    d |= static_cast<uint64_t>((smem_addr & 0x3FFFFu) >> 4);
-    d |= static_cast<uint64_t>(1024 >> 4) << 16;
-    d |= static_cast<uint64_t>(1024 >> 4) << 32;
-    d |= static_cast<uint64_t>(1) << 46;
-    d |= static_cast<uint64_t>(2) << 61;
-    return d;
-}
 
 template <bool kBF16>
 __device__ __forceinline__ uint32_t pack2(float a, float b) {
     return ab::pack2_rn<kBF16>(a, b);
 }
-
-__device__ __forceinline__ void sm_bar2() { asm volatile("bar.sync 1, %0;" ::"n"(SM_THREADS2) : "memory"); }
-__device__ __forceinline__ void sm_bar() { asm volatile("bar.sync 1, %0;" ::"n"(SM_THREADS) : "memory"); }
-// the SPLIT warps that share query rows 32*lg .. 32*lg+31
-__device__ __forceinline__ void pair_bar(uint32_t lg) { asm volatile("bar.sync %0, %1;" ::"r"(2u + lg), "n"(32 * SPLIT) : "memory"); }
 
 __device__ __forceinline__ float ex2_approx(float x) {
     float y;
@@ -109,749 +72,258 @@ __device__ __forceinline__ float ex2_approx(float x) {
     return y;
 }
 
-// Pass 1 on one 32-key chunk, IN PLACE: r[jj] <- t = S*scale2 + (mask2[j] + bias2[j + boff]) (log2 domain); returns
-// the chunk maximum.  The key mask is the same for every row: read with 128-bit broadcast loads (8 per chunk); the
-// relative-position bias is one 4-byte load per element (lanes of a warp read 32 consecutive floats).
-template <bool kBias>
-__device__ __forceinline__ float chunk_scores(uint32_t (&r)[32], float scale2, const float* mask2, const float* bias2,
-                                              int j0, int boff) {
-    float mx = -INFINITY;
-    const float4* m4 = reinterpret_cast<const float4*>(mask2 + j0);
-#pragma unroll
-    for (int q = 0; q < 8; ++q) {
-        const float4 m = m4[q];
-        const float add[4] = {m.x, m.y, m.z, m.w};
-#pragma unroll
-        for (int e = 0; e < 4; ++e) {
-            const int jj = 4 * q + e;
-            float a = add[e];
-            if (kBias) a += bias2[j0 + jj + boff];
-            const float t = fmaf(__uint_as_float(r[jj]), scale2, a);
-            r[jj] = __float_as_uint(t);
-            mx = fmaxf(mx, t);
-        }
-    }
-    return mx;
-}
-
-// Pass 2 on one chunk: p = 2^(t - max), returns the partial row sum, packs P to 16 bits.
-template <bool kBF16>
-__device__ __forceinline__ float chunk_probs(const uint32_t (&r)[32], uint32_t (&pk)[16], float mx) {
-    float s0 = 0.f, s1 = 0.f;
-#pragma unroll
-    for (int jj = 0; jj < 32; jj += 2) {
-        const float e0 = ex2_approx(__uint_as_float(r[jj]) - mx), e1 = ex2_approx(__uint_as_float(r[jj + 1]) - mx);
-        s0 += e0;
-        s1 += e1;
-        pk[jj >> 1] = pack2<kBF16>(e0, e1);
-    }
-    return s0 + s1;
-}
-
-// Pass 2 with attention-probability dropout (src/modeling_t5.py:515-516, src/modeling_bert.py:354): the row sum takes every
-// probability, the packed P tile only the kept ones (the 1 / (1 - p) scale is folded into the output normalisation).
-// `R` = (batch * H + h) * Lq + i, `G` = global key column of the chunk / 32 (csrc/dropout.cuh).
-template <bool kBF16>
-__device__ __forceinline__ float chunk_probs_drop(const uint32_t (&r)[32], uint32_t (&pk)[16], float mx, const abdrop::Key& key,
-                                                  uint64_t R, uint32_t G) {
-    float s0 = 0.f, s1 = 0.f;
-#pragma unroll
-    for (int q = 0; q < 4; ++q) {
-        uint32_t w[4];
-        abdrop::attn_words(key, R, G, q, w);
-#pragma unroll
-        for (int t = 0; t < 4; ++t) {
-            const int jj = 8 * t + 2 * q;
-            const float e0 = ex2_approx(__uint_as_float(r[jj]) - mx), e1 = ex2_approx(__uint_as_float(r[jj + 1]) - mx);
-            s0 += e0;
-            s1 += e1;
-            pk[jj >> 1] = pack2<kBF16>(abdrop::keep_lo(key, w[t]) ? e0 : 0.f, abdrop::keep_hi(key, w[t]) ? e1 : 0.f);
-        }
-    }
-    return s0 + s1;
-}
-
+// grid = (query tiles, H, B)
 template <bool kBF16>
 __global__ void __launch_bounds__(THREADS, 1)
 attention_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ CUtensorMap tmap_k,
                  const __grid_constant__ CUtensorMap tmap_v, const Params p) {
     extern __shared__ uint8_t smem_raw[];
-    __shared__ __align__(8) uint64_t k_full, k_empty, v_full, v_empty, q_full[2], q_empty[2], s_full, p_ready, o_full, s_free;
-    __shared__ __align__(8) uint64_t aux_full[2], aux_empty[2];
-    __shared__ uint32_t tmem_base_smem;
-    // per-(segment, head) tables, double buffered: filled by the two auxiliary warps one item ahead of the softmax warps
-    __shared__ float s_bias[2][2 * MAX_LK];               // (bias by (j - i) + (Lq - 1) [+ causal]) * log2e
-    __shared__ __align__(16) float s_mask[2][MAX_LK];     // additive key mask * log2e (-inf beyond Lk)
-    __shared__ float s_red[SPLIT][BLOCK_Q];   // per-row partial max of the SPLIT key parts
-    __shared__ float s_sum[SPLIT][BLOCK_Q];   // per-row partial sums
+    __shared__ __align__(8) uint64_t load_bar;
+    __shared__ float s_mask[MAX_LK];                 // key mask * log2e, -inf past Lk
+    __shared__ float s_bias[2 * MAX_LK + BK];        // (bias by (j - i) + (Lq - 1) [+ causal]) * log2e
+    __shared__ uint32_t s_live;
 
+    const int qt = blockIdx.x, h = blockIdx.y, b = blockIdx.z;
     const uint32_t warp = threadIdx.x >> 5;
     const uint32_t lane = threadIdx.x & 31u;
     const uint32_t smem_base = (ab::smem_u32(smem_raw) + 1023u) & ~1023u;
     uint8_t* smem_gen = smem_raw + (smem_base - ab::smem_u32(smem_raw));
-    uint8_t* sQ = smem_gen;
-    uint8_t* sK = smem_gen + 2 * Q_BYTES;
-    uint8_t* sV = sK + KV_BYTES;
-    const uint32_t aQ = smem_base, aK = smem_base + 2 * Q_BYTES, aV = aK + KV_BYTES;
+    const uint32_t sQ = smem_base, sK = smem_base + Q_BYTES, sV = sK + KV_BYTES;
 
-    const int n_chunks = (p.Lk + 127) / 128;   // 128-key chunks (TMA boxes / S column blocks)
-    const int lk_pad = n_chunks * 128;
-    const int n_qt = (p.Lq + BLOCK_Q - 1) / BLOCK_Q;
-    const int n_items = p.B * p.H;
-    // TMEM columns: S (fp32, one column per key) at [0, lk_pad); P (16-bit) overwrites [0, lk_pad/2).
-    //   lk_pad <= 384 ("pipelined"): two O accumulators at 384 and 448, outside the S columns.  The S = Q.K^T of the
-    //       next query tile is issued as soon as this tile's P.V has retired, and the softmax warps write tile t-1's
-    //       output while the tensor pipe runs P.V(t) and S(t+1).
-    //   lk_pad == 512: one O accumulator at lk_pad/2 (inside the S columns, free once P is packed); the next S waits
-    //       until the softmax warps have read O (s_free).
-    const bool pipelined = lk_pad <= 384;
-    auto o_col_of = [&](int qt_it) -> uint32_t {
-        return pipelined ? static_cast<uint32_t>(384 + 64 * (qt_it & 1)) : static_cast<uint32_t>(lk_pad / 2);
-    };
-
-    if (warp == 0 && lane == 0) {
-        ab::tma_prefetch_desc(&tmap_q);
-        ab::tma_prefetch_desc(&tmap_k);
-        ab::tma_prefetch_desc(&tmap_v);
+    const int nb = (p.Lk + BK - 1) / BK;
+    const bool packed = p.seg_tile != nullptr;
+    // live key blocks (bit j = block j); none flagged live = all live
+    uint32_t live = (1u << nb) - 1u;
+    if (p.blk_live != nullptr) {
+        const bool lv = static_cast<int>(lane) < nb && __ldg(p.blk_live + static_cast<size_t>(b) * nb + lane) != 0;
+        const uint32_t m = __ballot_sync(0xffffffffu, lv);
+        if (m != 0u) live = m;
     }
-    if (warp == 1 && lane == 0) {
-        ab::mbar_init(&k_full, 1);
-        ab::mbar_init(&k_empty, 1);
-        ab::mbar_init(&v_full, 1);
-        ab::mbar_init(&v_empty, 1);
-        for (int i = 0; i < 2; ++i) {
-            ab::mbar_init(&q_full[i], 1);
-            ab::mbar_init(&q_empty[i], 1);
-            ab::mbar_init(&aux_full[i], AUX_THREADS);
-            ab::mbar_init(&aux_empty[i], SM_THREADS);
-        }
-        ab::mbar_init(&s_full, 1);
-        ab::mbar_init(&p_ready, SM_THREADS);
-        ab::mbar_init(&o_full, 1);
-        ab::mbar_init(&s_free, SM_THREADS);
+    // rows of this segment: packed layout = its kept tiles, back to back
+    const int lq = packed ? 64 * __popc(live) : p.Lq;
+    const int lk = packed ? lq : p.Lk;
+    if (qt * BQ >= lq) return;                       // (packed) this query tile does not exist
+    const int q_row0 = packed ? 64 * __ldg(p.seg_tile + static_cast<size_t>(b) * nb) : (b / p.q_div) * p.Lq;
+    const int k_row0 = packed ? q_row0 : b * p.Lk;
+    const int o_row0 = packed ? q_row0 : b * p.Lq;
+    const int nkb = (lk + BK - 1) / BK;
+
+    if (threadIdx.x == 0) {
+        ab::mbar_init(&load_bar, 1);
         ab::fence_barrier_init();
+        s_live = live;
     }
-    if (warp == 2) ab::tmem_alloc<1>(&tmem_base_smem, TMEM_COLS);
-    ab::tc_fence_before();
     __syncthreads();
-    ab::tc_fence_after();
-    const uint32_t tmem_base = tmem_base_smem;
-
-    if (warp == 0) {
-        // ===================== TMA producer =====================
-        // K and V have separate barriers: the next (segment, head)'s K streams in while the current one's last
-        // query tile is still in its softmax / P.V phase, its V while the next S = Q.K^T and softmax run.
-        if (lane == 0) {
-            int item_it = 0, qt_it = 0;
-            const uint32_t kv_bytes = static_cast<uint32_t>(n_chunks * 128 * D * 2);
-            auto load_q = [&](int b, int h, int qt) {
-                const int qb = qt_it & 1;
-                ab::mbar_wait(&q_empty[qb], ((qt_it >> 1) & 1) ^ 1u, 22);
-                ab::mbar_arrive_expect_tx(&q_full[qb], Q_BYTES);
-                ab::tma_load_2d(&tmap_q, &q_full[qb], sQ + qb * Q_BYTES, p.q_col0 + h * D,
-                                (b / p.q_div) * p.Lq + qt * BLOCK_Q, ab::kEvictFirst);
-                ++qt_it;
-            };
-            for (int item = blockIdx.x; item < n_items; item += gridDim.x, ++item_it) {
-                const int b = item / p.H, h = item % p.H;
-                ab::mbar_wait(&k_empty, (item_it & 1) ^ 1u, 21);
-                ab::mbar_arrive_expect_tx(&k_full, kv_bytes);
-                for (int c = 0; c < n_chunks; ++c)
-                    ab::tma_load_2d(&tmap_k, &k_full, sK + c * (128 * D * 2), p.k_col0 + h * D, b * p.Lk + c * 128,
-                                    ab::kEvictNormal);
-                load_q(b, h, 0);
-                ab::mbar_wait(&v_empty, (item_it & 1) ^ 1u, 29);
-                ab::mbar_arrive_expect_tx(&v_full, kv_bytes);
-                for (int c = 0; c < n_chunks; ++c)
-                    ab::tma_load_2d(&tmap_v, &v_full, sV + c * (128 * D * 2), p.v_col0 + h * D, b * p.Lk + c * 128,
-                                    ab::kEvictNormal);
-                for (int qt = 1; qt < n_qt; ++qt) load_q(b, h, qt);
-            }
-        }
-    } else if (warp == 1) {
-        // ===================== MMA issuer =====================
-        if (lane == 0) {
-            constexpr uint32_t idesc_s = ab::umma_idesc_f16(BLOCK_Q, 128, kBF16);
-            // P.V: A from TMEM (K-major), B = V rows = MN-major operand -> b_major bit (16) set
-            constexpr uint32_t idesc_o = ab::umma_idesc_f16(BLOCK_Q, D, kBF16) | (1u << 16);
-            int item_it = 0, qt_it = 0;
-            for (int item = blockIdx.x; item < n_items; item += gridDim.x, ++item_it) {
-                ab::mbar_wait(&k_full, item_it & 1, 23);
-                for (int qt = 0; qt < n_qt; ++qt, ++qt_it) {
-                    const int qb = qt_it & 1;
-                    ab::mbar_wait(&q_full[qb], (qt_it >> 1) & 1, 24);
-                    if (pipelined) {
-                        // S(t) overwrites the columns P(t-1) occupies: wait until P.V(t-1) has retired
-                        if (qt_it > 0) ab::mbar_wait(&o_full, (qt_it - 1) & 1, 31);
-                    } else {
-                        ab::mbar_wait(&s_free, (qt_it & 1) ^ 1u, 25);
-                    }
-                    ab::tc_fence_after();
-                    const uint64_t qdesc = ab::umma_desc_k_sw128(aQ + qb * Q_BYTES);
-                    for (int c = 0; c < n_chunks; ++c) {
-                        const uint64_t kdesc = ab::umma_desc_k_sw128(aK + c * (128 * D * 2));
-#pragma unroll
-                        for (int k = 0; k < D / 16; ++k)
-                            ab::umma_ss<1>(tmem_base + c * 128, qdesc + ((k * 32) >> 4), kdesc + ((k * 32) >> 4), idesc_s,
-                                           k != 0 ? 1u : 0u);
-                    }
-                    ab::umma_commit(&q_empty[qb]);  // Q tile consumed once the S MMAs retire
-                    if (qt == n_qt - 1) ab::umma_commit(&k_empty);
-                    ab::umma_commit(&s_full);
-                    if (qt == 0) ab::mbar_wait(&v_full, item_it & 1, 30);
-                    ab::mbar_wait(&p_ready, qt_it & 1, 26);
-                    ab::tc_fence_after();
-                    const uint64_t vdesc = umma_desc_mn_sw128(aV);
-                    const uint32_t o_tmem = tmem_base + o_col_of(qt_it);
-                    for (int k = 0; k < lk_pad / 16; ++k)
-                        ab::umma_ts<1>(o_tmem, tmem_base + k * 8, vdesc + static_cast<uint64_t>((k * 2048) >> 4), idesc_o,
-                                       k != 0 ? 1u : 0u);
-                    if (qt == n_qt - 1) ab::umma_commit(&v_empty);  // last use of this (segment, head)'s V
-                    ab::umma_commit(&o_full);
-                }
-            }
-        }
-    } else if (warp == 2) {
-        // ===================== auxiliary warp 2: mask / bias tables of the NEXT item =====================
-        const int tid = static_cast<int>(threadIdx.x) - 64;
-        const bool has_bias = (p.bias_delta != nullptr) || (p.causal_value != 0.f);
-        int item_it = 0;
-        for (int item = blockIdx.x; item < n_items; item += gridDim.x, ++item_it) {
-            const int b = item / p.H, h = item % p.H;
-            const int buf = item_it & 1;
-            ab::mbar_wait(&aux_empty[buf], ((item_it >> 1) & 1) ^ 1u, 32);
-#pragma unroll 4
-            for (int j = tid; j < lk_pad; j += AUX_THREADS)
-                s_mask[buf][j] = (j < p.Lk) ? (p.add_mask ? p.add_mask[static_cast<size_t>(b) * p.Lk + j] * LOG2E : 0.f)
-                                            : -INFINITY;
-            if (has_bias)
-#pragma unroll 4
-                for (int d = tid; d < 2 * MAX_LK; d += AUX_THREADS) {   // entries past the valid offsets stay finite (0)
-                    float v = 0.f;
-                    if (d < p.Lq + p.Lk - 1) {
-                        v = p.bias_delta ? p.bias_delta[static_cast<size_t>(h) * (p.Lq + p.Lk - 1) + d] : 0.f;
-                        if (p.causal_value != 0.f && d > p.Lq - 1) v += p.causal_value;   // j > i
-                    }
-                    s_bias[buf][d] = v * LOG2E;
-                }
-            ab::mbar_arrive(&aux_full[buf]);
-        }
-    } else {
-        // ===================== softmax + output: SPLIT threads per query row =====================
-        const uint32_t lg = warp & 3u;
-        const uint32_t part = (warp - 3u) >> 2;                    // key chunks part, part+SPLIT, ...; O columns 16*part..
-        const int row = static_cast<int>(lg * 32 + lane);
-        const uint32_t lane_addr = tmem_base + ((lg * 32u) << 16);
-        const float scale2 = p.scale * LOG2E;
-        const bool has_bias = (p.bias_delta != nullptr) || (p.causal_value != 0.f);
-        const int n32 = lk_pad / 32;
-        constexpr int OC = D / SPLIT;                               // O columns per thread
-
-        // one finished tile's output: O (fp32, TMEM) -> normalised 16-bit rows, or split-KV partials
-        auto emit = [&](int b, int h, int i, float mx, float sum, uint32_t ocol) {
-            uint32_t ro[OC];
-            tmem_ld16(lane_addr + ocol + part * OC, ro);
-            ab::tmem_ld_wait();
-            if (i >= p.Lq) return;
-            if (p.o_partial != nullptr) {
-                // split-KV: un-normalised partial output in fp32 + (max, sum) of this split (natural log units)
-                float* dst = p.o_partial + (static_cast<size_t>(b) * p.Lq + i) * (static_cast<size_t>(p.H) * D) + h * D +
-                             part * OC;
-#pragma unroll
-                const float ik = p.drop.inv_keep;
-                for (int v4 = 0; v4 < OC / 4; ++v4)
-                    reinterpret_cast<float4*>(dst)[v4] =
-                        make_float4(__uint_as_float(ro[4 * v4]) * ik, __uint_as_float(ro[4 * v4 + 1]) * ik,
-                                    __uint_as_float(ro[4 * v4 + 2]) * ik, __uint_as_float(ro[4 * v4 + 3]) * ik);
-                if (part == 0) {
-                    float* ml = p.ml_partial + ((static_cast<size_t>(b) * p.Lq + i) * p.H + h) * 2;
-                    ml[0] = mx * (1.0f / LOG2E);
-                    ml[1] = sum;
-                }
-            } else {
-                const float inv = p.drop.inv_keep / sum;
-                if (p.lse_out != nullptr && part == 0)
-                    p.lse_out[(static_cast<size_t>(b) * p.H + h) * p.Lq + i] = mx * (1.0f / LOG2E) + __logf(sum);
-                uint4* dst = reinterpret_cast<uint4*>(p.O + (static_cast<size_t>(b) * p.Lq + i) * p.ldo + h * D + part * OC);
-#pragma unroll
-                for (int v4 = 0; v4 < OC / 8; ++v4)
-                    dst[v4] = make_uint4(
-                        pack2<kBF16>(__uint_as_float(ro[8 * v4]) * inv, __uint_as_float(ro[8 * v4 + 1]) * inv),
-                        pack2<kBF16>(__uint_as_float(ro[8 * v4 + 2]) * inv, __uint_as_float(ro[8 * v4 + 3]) * inv),
-                        pack2<kBF16>(__uint_as_float(ro[8 * v4 + 4]) * inv, __uint_as_float(ro[8 * v4 + 5]) * inv),
-                        pack2<kBF16>(__uint_as_float(ro[8 * v4 + 6]) * inv, __uint_as_float(ro[8 * v4 + 7]) * inv));
-            }
-        };
-
-        int qt_it = 0, item_it = 0;
-        // pipelined mode: the previous tile, whose output is written while the tensor pipe works on this one
-        bool pend = false;
-        int pend_b = 0, pend_h = 0, pend_i = 0, pend_it = 0;
-        float pend_mx = 0.f, pend_sum = 1.f;
-        for (int item = blockIdx.x; item < n_items; item += gridDim.x, ++item_it) {
-            const int b = item / p.H, h = item % p.H;
-            const int buf = item_it & 1;
-            ab::mbar_wait(&aux_full[buf], (item_it >> 1) & 1, 33);
-            const float* mask2 = s_mask[buf];
-            const float* bias2 = s_bias[buf];
-            for (int qt = 0; qt < n_qt; ++qt, ++qt_it) {
-                const int i = qt * BLOCK_Q + row;                   // query position inside the segment
-                const int boff = min(p.Lq - 1 - i, 2 * MAX_LK - 1 - lk_pad);  // bias index = j + boff (clamped for pad rows)
-                const int boffc = max(boff, 0);
-                ab::mbar_wait(&s_full, qt_it & 1, 27);
-                ab::tc_fence_after();
-                // ---- pass 1: t = scaled score + mask + bias written back over S; partial row max ----
-                float mx = -INFINITY;
-                {
-                    uint32_t ra[32];
-                    for (int c = static_cast<int>(part); c < n32; c += SPLIT) {
-                        ab::tmem_ld32(lane_addr + c * 32, ra);
-                        ab::tmem_ld_wait();
-                        mx = fmaxf(mx, has_bias ? chunk_scores<true>(ra, scale2, mask2, bias2, c * 32, boffc)
-                                                : chunk_scores<false>(ra, scale2, mask2, bias2, c * 32, boffc));
-                        ab::tmem_st32(lane_addr + c * 32, ra);
-                    }
-                }
-                if (qt == n_qt - 1) ab::mbar_arrive(&aux_empty[buf]);   // last read of this item's tables
-                s_red[part][row] = mx;
-                ab::tmem_st_wait();   // this thread re-reads its own t columns in pass 2
-                sm_bar();
-#pragma unroll
-                for (int q = 0; q < SPLIT; ++q) mx = fmaxf(mx, s_red[q][row]);
-                // ---- pass 2: p = 2^(t - max), partial row sum, P (16-bit) written over the S columns it replaces ----
-                float sum = 0.f;
-                {
-                    uint32_t ra[32], pk[16];
-                    for (int c = static_cast<int>(part); c < n32; c += SPLIT) {
-                        ab::tmem_ld32(lane_addr + c * 32, ra);
-                        ab::tmem_ld_wait();
-                        // P of chunks SPLIT*k .. SPLIT*k+SPLIT-1 lands on the columns of S chunks <= SPLIT*k + SPLIT-1:
-                        // every thread of a row must have loaded its chunk of this iteration before any of them stores P
-                        pair_bar(lg);
-                        if (p.drop.thr16 != 0u) {
-                            const uint64_t R = (static_cast<uint64_t>(b / p.q_div) * p.H + h) * p.Lq + min(i, p.Lq - 1);
-                            const uint32_t G = static_cast<uint32_t>(((b % p.q_div) * p.Lk + c * 32) >> 5);
-                            sum += chunk_probs_drop<kBF16>(ra, pk, mx, p.drop, R, G);
-                        } else {
-                            sum += chunk_probs<kBF16>(ra, pk, mx);
-                        }
-                        tmem_st16(lane_addr + c * 16, pk);
-                    }
-                }
-                s_sum[part][row] = sum;
-                ab::tmem_st_wait();
-                ab::tc_fence_before();
-                sm_bar();  // both halves' sums are in smem; all P columns of this warp pair are written
-                ab::mbar_arrive(&p_ready);
-                sum = 0.f;
-#pragma unroll
-                for (int q = 0; q < SPLIT; ++q) sum += s_sum[q][row];
-                if (pipelined) {
-                    // P.V(t-1) retired before S(t) was issued (MMA warp), and S(t) was observed above: O(t-1) is final
-                    if (pend) emit(pend_b, pend_h, pend_i, pend_mx, pend_sum, o_col_of(pend_it));
-                    ab::tc_fence_before();
-                    pend = true;
-                    pend_b = b, pend_h = h, pend_i = i, pend_it = qt_it, pend_mx = mx, pend_sum = sum;
-                } else {
-                    ab::mbar_wait(&o_full, qt_it & 1, 28);
-                    ab::tc_fence_after();
-                    emit(b, h, i, mx, sum, o_col_of(qt_it));
-                    ab::tc_fence_before();
-                    ab::mbar_arrive(&s_free);  // S / P / O columns may be overwritten by the next query tile
-                }
-            }
-        }
-        if (pend) {
-            ab::mbar_wait(&o_full, pend_it & 1, 34);
-            ab::tc_fence_after();
-            emit(pend_b, pend_h, pend_i, pend_mx, pend_sum, o_col_of(pend_it));
-        }
-    }
-
-    ab::tc_fence_before();
-    __syncthreads();
-    if (warp == 2) {
-        ab::tc_fence_after();
-        ab::tmem_dealloc<1>(tmem_base, TMEM_COLS);
-    }
-}
-
-// ---------------------------------------------------------------------------------------------------------------
-// attention_split_kernel: the <= 384-key kernel.  Every 128-query tile is processed as TWO independent key halves
-// (a = keys [0, lk_pad/2), b = the rest), each with its own exact two-pass softmax (row max m_h, row sum l_h) and its
-// own un-normalised accumulator O_h = P_h.V_h; the halves are merged in registers when the tile's output is written:
-//     out = (w_a O_a + w_b O_b) / (w_a l_a + w_b l_b),   w_h = 2^(m_h - max(m_a, m_b))
-// (the split-KV identity, src/fid.py:298-349 semantics unchanged).  This makes the tensor pipe and the softmax warps
-// overlap: while the softmax warps work on half b of tile t the MMA warp runs P_a.V_a(t) and S_a(t+1), and vice versa.
-// TMEM columns: S_a [0, half) | S_b [half, 2*half) (P_h packed over the first half of S_h) | O_a 384 | O_b 448.
-// ---------------------------------------------------------------------------------------------------------------
-__device__ __forceinline__ void tmem_st8(uint32_t taddr, const uint32_t (&r)[8]) {
-    asm volatile("tcgen05.st.sync.aligned.32x32b.x8.b32 [%0], {%1, %2, %3, %4, %5, %6, %7, %8};" ::"r"(taddr), "r"(r[0]),
-                 "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7])
-                 : "memory");
-}
-
-// pass 1 on one 16-key unit, in place: r <- t = S*scale2 + mask2[j] + bias2[j + boff]; returns the unit maximum
-template <bool kBias>
-__device__ __forceinline__ float unit_scores(uint32_t (&r)[16], float scale2, const float* mask2, const float* bias2,
-                                             int j0, int boff) {
-    float mx = -INFINITY;
-    const float4* m4 = reinterpret_cast<const float4*>(mask2 + j0);
-#pragma unroll
-    for (int q = 0; q < 4; ++q) {
-        const float4 m = m4[q];
-        const float add[4] = {m.x, m.y, m.z, m.w};
-#pragma unroll
-        for (int e = 0; e < 4; ++e) {
-            const int jj = 4 * q + e;
-            float a = add[e];
-            if (kBias) a += bias2[j0 + jj + boff];
-            const float t = fmaf(__uint_as_float(r[jj]), scale2, a);
-            r[jj] = __float_as_uint(t);
-            mx = fmaxf(mx, t);
-        }
-    }
-    return mx;
-}
-
-template <bool kBF16>
-__device__ __forceinline__ float unit_probs(const uint32_t (&r)[16], uint32_t (&pk)[8], float mx) {
-    float s0 = 0.f, s1 = 0.f;
-#pragma unroll
-    for (int jj = 0; jj < 16; jj += 2) {
-        const float e0 = ex2_approx(__uint_as_float(r[jj]) - mx), e1 = ex2_approx(__uint_as_float(r[jj + 1]) - mx);
-        s0 += e0;
-        s1 += e1;
-        pk[jj >> 1] = pack2<kBF16>(e0, e1);
-    }
-    return s0 + s1;
-}
-
-template <bool kBF16>
-__global__ void __launch_bounds__(THREADS_SPLIT, 1)   // 10 warps (allocated as 12): up to 168 registers per thread
-attention_split_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ CUtensorMap tmap_k,
-                       const __grid_constant__ CUtensorMap tmap_v, const Params p) {
-    extern __shared__ uint8_t smem_raw[];
-    __shared__ __align__(8) uint64_t k_full[2], k_empty[2], v_full[2], v_empty[2], q_full[2], q_empty[2];
-    __shared__ __align__(8) uint64_t s_full[2], p_ready[2], o_full[2], aux_full[2], aux_empty[2];
-    __shared__ uint32_t tmem_base_smem;
-    __shared__ float s_bias[2][2 * MAX_LK];
-    __shared__ __align__(16) float s_mask[2][MAX_LK];
-    __shared__ float s_red[SPLIT2][BLOCK_Q];
-    __shared__ float s_sum[SPLIT2][BLOCK_Q];
-    __shared__ float s_stat[2][4][BLOCK_Q];   // per tile parity: (m_a, l_a, m_b, l_b) of every row, kept until the output
-
-    const uint32_t warp = threadIdx.x >> 5;
-    const uint32_t lane = threadIdx.x & 31u;
-    const uint32_t smem_base = (ab::smem_u32(smem_raw) + 1023u) & ~1023u;
-    uint8_t* smem_gen = smem_raw + (smem_base - ab::smem_u32(smem_raw));
-    uint8_t* sQ = smem_gen;
-    const int n_chunks = (p.Lk + 127) / 128;
-    const int lk_pad = n_chunks * 128;          // <= 384 (host dispatch)
-    // K and V of <= 256 keys are DOUBLE-buffered inside the same 2 x 64 KB region (4 x 32 KB): the next (segment, head)'s K
-    // and V stream in while this one computes.  The split-KV cross-attention of the FiD decoder is a pure K / V stream
-    // (32 queries against 15 360 keys per (batch, head)); with single buffers every item paid its own load latency
-    // (160 us per layer = 36 % of the HBM roofline, profiles/r02_launches_step_visit_f.csv).
-    const int nbuf = lk_pad <= 256 ? 2 : 1;
-    const uint32_t kvb = static_cast<uint32_t>(lk_pad) * (D * 2);           // bytes of one K (or V) buffer
-    uint8_t* sK = smem_gen + 2 * Q_BYTES;
-    uint8_t* sV = sK + nbuf * kvb;
-    const uint32_t aQ = smem_base, aK = smem_base + 2 * Q_BYTES, aV = aK + nbuf * kvb;
-    const int half = lk_pad / 2;                // keys per half: 64, 128 or 192
-    const int n_qt = (p.Lq + BLOCK_Q - 1) / BLOCK_Q;
-    const int n_items = p.B * p.H;
-    const int my_items = (n_items - static_cast<int>(blockIdx.x) + static_cast<int>(gridDim.x) - 1) / static_cast<int>(gridDim.x);
-    const int n_tiles = my_items * n_qt;        // 128-query tiles this CTA processes, in order (item-major)
-    constexpr uint32_t O_COL0 = 384;
-
-    if (warp == 0 && lane == 0) {
+    if (threadIdx.x == 0) {
         ab::tma_prefetch_desc(&tmap_q);
-        ab::tma_prefetch_desc(&tmap_k);
-        ab::tma_prefetch_desc(&tmap_v);
-    }
-    if (warp == 1 && lane == 0) {
-        for (int i = 0; i < 2; ++i) {
-            ab::mbar_init(&k_full[i], 1);
-            ab::mbar_init(&k_empty[i], 1);
-            ab::mbar_init(&v_full[i], 1);
-            ab::mbar_init(&v_empty[i], 1);
-            ab::mbar_init(&q_full[i], 1);
-            ab::mbar_init(&q_empty[i], 1);
-            ab::mbar_init(&s_full[i], 1);
-            ab::mbar_init(&p_ready[i], SM_THREADS2);
-            ab::mbar_init(&o_full[i], 1);
-            ab::mbar_init(&aux_full[i], AUX_THREADS);
-            ab::mbar_init(&aux_empty[i], SM_THREADS2);
+        int nload = 0;
+        for (int kb = 0; kb < nkb; ++kb) nload += (live >> kb) & 1u;
+        ab::mbar_arrive_expect_tx(&load_bar, static_cast<uint32_t>(2 * TILE_BYTES + 2 * nload * TILE_BYTES));
+        for (int t = 0; t < 2; ++t)
+            ab::tma_load_2d(&tmap_q, &load_bar, smem_gen + t * TILE_BYTES, p.q_col0 + h * D, q_row0 + qt * BQ + t * BK,
+                            ab::kEvictFirst);
+        for (int kb = 0; kb < nkb; ++kb) {
+            if (!((live >> kb) & 1u)) continue;
+            ab::tma_load_2d(&tmap_k, &load_bar, smem_gen + Q_BYTES + kb * TILE_BYTES, p.k_col0 + h * D, k_row0 + kb * BK,
+                            ab::kEvictNormal);
+            ab::tma_load_2d(&tmap_v, &load_bar, smem_gen + Q_BYTES + KV_BYTES + kb * TILE_BYTES, p.v_col0 + h * D,
+                            k_row0 + kb * BK, ab::kEvictNormal);
         }
-        ab::fence_barrier_init();
     }
-    if (warp == 0) ab::tmem_alloc<1>(&tmem_base_smem, TMEM_COLS);
-    ab::tc_fence_before();
+    // mask / bias tables while the loads are in flight
+    const bool has_bias = (p.bias_delta != nullptr) || (p.causal_value != 0.f);
+    for (int j = threadIdx.x; j < nkb * BK; j += THREADS)
+        s_mask[j] = (j < lk) ? (p.add_mask ? p.add_mask[static_cast<size_t>(b) * p.Lk + j] * LOG2E : 0.f) : -INFINITY;
+    if (has_bias) {
+        const int n_valid = p.Lq + p.Lk - 1;
+        for (int d = threadIdx.x; d < 2 * MAX_LK + BK; d += THREADS) {   // entries past the valid offsets stay finite (0)
+            float v = 0.f;
+            if (d < n_valid) {
+                v = p.bias_delta ? p.bias_delta[static_cast<size_t>(h) * n_valid + d] : 0.f;
+                if (p.causal_value != 0.f && d > p.Lq - 1) v += p.causal_value;   // j > i
+            }
+            s_bias[d] = v * LOG2E;
+        }
+    }
     __syncthreads();
-    ab::tc_fence_after();
-    const uint32_t tmem_base = tmem_base_smem;
+    ab::mbar_wait(&load_bar, 0, 40);
 
-    if (warp == 0) {
-        // ===================== warp 0: mask / bias tables (all lanes) + TMA producer (lane 0), one item ahead ========
-        // The tables of item n+1 are filled BEFORE its loads are issued: the fill only waits for item n-1's softmax
-        // (aux_empty), while a Q load can wait on this item's own MMAs.
-        const bool has_bias = (p.bias_delta != nullptr) || (p.causal_value != 0.f);
-        const int tid = static_cast<int>(lane);
-        int item_it = 0, qt_it = 0;
-        const uint32_t kv_bytes = static_cast<uint32_t>(n_chunks * 128 * D * 2);
-        for (int item = blockIdx.x; item < n_items; item += gridDim.x, ++item_it) {
-            const int b = item / p.H, h = item % p.H;
-            const int buf = item_it & 1;
-            ab::mbar_wait(&aux_empty[buf], ((item_it >> 1) & 1) ^ 1u, 52);
-#pragma unroll 4
-            for (int j = tid; j < lk_pad; j += AUX_THREADS)
-                s_mask[buf][j] = (j < p.Lk) ? (p.add_mask ? p.add_mask[static_cast<size_t>(b) * p.Lk + j] * LOG2E : 0.f)
-                                            : -INFINITY;
-            if (has_bias) {
-#pragma unroll 4
-                for (int d = tid; d < 2 * MAX_LK; d += AUX_THREADS) {
-                    float v = 0.f;
-                    if (d < p.Lq + p.Lk - 1) {
-                        v = p.bias_delta ? p.bias_delta[static_cast<size_t>(h) * (p.Lq + p.Lk - 1) + d] : 0.f;
-                        if (p.causal_value != 0.f && d > p.Lq - 1) v += p.causal_value;   // j > i
-                    }
-                    s_bias[buf][d] = v * LOG2E;
-                }
-            }
-            ab::mbar_arrive(&aux_full[buf]);
-            if (lane == 0) {
-                auto load_q = [&](int qt) {
-                    const int qb = qt_it & 1;
-                    ab::mbar_wait(&q_empty[qb], ((qt_it >> 1) & 1) ^ 1u, 42);
-                    ab::mbar_arrive_expect_tx(&q_full[qb], Q_BYTES);
-                    ab::tma_load_2d(&tmap_q, &q_full[qb], sQ + qb * Q_BYTES, p.q_col0 + h * D,
-                                    (b / p.q_div) * p.Lq + qt * BLOCK_Q, ab::kEvictFirst);
-                    ++qt_it;
-                };
-                const int kb = item_it % nbuf;
-                const uint32_t kph = static_cast<uint32_t>(item_it / nbuf) & 1u;
-                ab::mbar_wait(&k_empty[kb], kph ^ 1u, 41);
-                ab::mbar_arrive_expect_tx(&k_full[kb], kv_bytes);
-                for (int c = 0; c < n_chunks; ++c)
-                    ab::tma_load_2d(&tmap_k, &k_full[kb], sK + kb * kvb + c * (128 * D * 2), p.k_col0 + h * D,
-                                    b * p.Lk + c * 128, ab::kEvictNormal);
-                load_q(0);
-                ab::mbar_wait(&v_empty[kb], kph ^ 1u, 49);
-                ab::mbar_arrive_expect_tx(&v_full[kb], kv_bytes);
-                for (int c = 0; c < n_chunks; ++c)
-                    ab::tma_load_2d(&tmap_v, &v_full[kb], sV + kb * kvb + c * (128 * D * 2), p.v_col0 + h * D,
-                                    b * p.Lk + c * 128, ab::kEvictNormal);
-                for (int qt = 1; qt < n_qt; ++qt) load_q(qt);
-            }
-            __syncwarp();
+    // ---- warpgroup g: query rows 64 g .. 64 g + 63 of the tile; this thread: rows r and r + 8, key pairs 8 j + 2 (lane % 4)
+    const uint32_t g = warp >> 2, wl = warp & 3u;
+    const int i0 = qt * BQ + static_cast<int>(g * 64u + wl * 16u + (lane >> 2));   // query index of row r (in the segment)
+    const int cq = static_cast<int>(2u * (lane & 3u));
+    const float scale2 = p.scale * LOG2E;
+    const bool dropping = p.drop.thr16 != 0u;
+    float o[32];
+#pragma unroll
+    for (int x = 0; x < 32; ++x) o[x] = 0.f;
+    float m_run[2] = {-INFINITY, -INFINITY}, l_run[2] = {0.f, 0.f};
+
+    for (int kb = 0; kb < nkb; ++kb) {
+        if (!((live >> kb) & 1u)) continue;
+        float sc[32];
+        ab::wgmma_fence();
+#pragma unroll
+        for (int k = 0; k < D / 16; ++k) {
+            const uint64_t adesc = ab::wgmma_desc_sw128(sQ + g * 8192u + k * 32u);
+            const uint64_t bdesc = ab::wgmma_desc_sw128(sK + kb * TILE_BYTES + k * 32u);
+            ab::wgmma_m64n64k16_ss<kBF16, 0, 0>(sc, adesc, bdesc, k);
         }
-    } else if (warp == 1) {
-        // ===================== MMA issuer: P_a.V_a(t), S_a(t+1), P_b.V_b(t), S_b(t+1), ... =====================
-        if (lane == 0 && n_tiles > 0) {
-            const uint32_t idesc_s = ab::umma_idesc_f16(BLOCK_Q, half, kBF16);
-            constexpr uint32_t idesc_o = ab::umma_idesc_f16(BLOCK_Q, D, kBF16) | (1u << 16);   // B = V rows, MN-major
-            // S_h(g) = Q(g) . K_h^T  -> columns [h*half, h*half + half)
-            auto issue_s = [&](int hh, int g) {
-                const uint64_t qdesc = ab::umma_desc_k_sw128(aQ + (g & 1) * Q_BYTES);
-                const uint64_t kdesc = ab::umma_desc_k_sw128(aK + ((g / n_qt) % nbuf) * kvb + hh * half * (D * 2));
-#pragma unroll
-                for (int k = 0; k < D / 16; ++k)
-                    ab::umma_ss<1>(tmem_base + hh * half, qdesc + ((k * 32) >> 4), kdesc + ((k * 32) >> 4), idesc_s,
-                                   k != 0 ? 1u : 0u);
-            };
-            // O_h(g) = P_h . V_h : A = packed P in TMEM, B = V rows of this half
-            auto issue_pv = [&](int hh, int g) {
-                const uint64_t vdesc = umma_desc_mn_sw128(aV + ((g / n_qt) % nbuf) * kvb + hh * half * (D * 2));
-                for (int k = 0; k < half / 16; ++k)
-                    ab::umma_ts<1>(tmem_base + O_COL0 + 64 * hh, tmem_base + hh * half + k * 8,
-                                   vdesc + static_cast<uint64_t>((k * 2048) >> 4), idesc_o, k != 0 ? 1u : 0u);
-            };
-            // prologue: both halves of tile 0
-            ab::mbar_wait(&k_full[0], 0, 43);
-            ab::mbar_wait(&q_full[0], 0, 44);
-            ab::tc_fence_after();
-            issue_s(0, 0);
-            ab::umma_commit(&s_full[0]);
-            issue_s(1, 0);
-            ab::umma_commit(&q_empty[0]);
-            if (n_qt == 1) ab::umma_commit(&k_empty[0]);
-            ab::umma_commit(&s_full[1]);
-            for (int g = 0; g < n_tiles; ++g) {
-                const int item_it = g / n_qt, qt = g % n_qt;
-                const bool has_next = g + 1 < n_tiles;
-                const int nitem_it = (g + 1) / n_qt, nqt = (g + 1) % n_qt;
-                const int ib = item_it % nbuf, nib = nitem_it % nbuf;
-                if (qt == 0) ab::mbar_wait(&v_full[ib], static_cast<uint32_t>(item_it / nbuf) & 1u, 50);
-                // ---- half a ----
-                ab::mbar_wait(&p_ready[0], g & 1, 46);
-                ab::tc_fence_after();
-                issue_pv(0, g);
-                ab::umma_commit(&o_full[0]);
-                if (has_next) {
-                    if (nqt == 0) ab::mbar_wait(&k_full[nib], static_cast<uint32_t>(nitem_it / nbuf) & 1u, 43);
-                    ab::mbar_wait(&q_full[(g + 1) & 1], ((g + 1) >> 1) & 1, 44);
-                    // S_a(g+1) takes the columns of P_a(g): tcgen05.mma executes in issue order, P_a.V_a(g) above reads them
-                    // first - no completion round trip (round 1 waited for o_full here)
-                    ab::tc_fence_after();
-                    issue_s(0, g + 1);
-                    ab::umma_commit(&s_full[0]);
-                }
-                // ---- half b ----
-                ab::mbar_wait(&p_ready[1], g & 1, 47);
-                ab::tc_fence_after();
-                issue_pv(1, g);
-                if (qt == n_qt - 1) ab::umma_commit(&v_empty[ib]);   // last use of this (segment, head)'s V
-                ab::umma_commit(&o_full[1]);
-                if (has_next) {
-                    issue_s(1, g + 1);
-                    ab::umma_commit(&q_empty[(g + 1) & 1]);
-                    if (nqt == n_qt - 1) ab::umma_commit(&k_empty[nib]);
-                    ab::umma_commit(&s_full[1]);
-                }
-            }
-        }
-    } else {
-        // ===================== softmax + output: SPLIT threads per query row =====================
-        const uint32_t lg = warp & 3u;
-        const uint32_t part = (warp - 2u) >> 2;
-        const int row = static_cast<int>(lg * 32 + lane);
-        const uint32_t lane_addr = tmem_base + ((lg * 32u) << 16);
-        const float scale2 = p.scale * LOG2E;
-        const bool has_bias = (p.bias_delta != nullptr) || (p.causal_value != 0.f);
-        constexpr int MAXU = 6;                                      // 16-key units per thread and half (half <= 192)
-        const int upp = half / 16 / SPLIT2;                          // 2, 4 or 6
-        constexpr int OC = D / SPLIT2;                               // 32 output columns per thread
+        ab::wgmma_commit();
+        ab::wgmma_wait<0>();
+        ab::wgmma_reg_fence(sc);
 
-        // merge the two halves of a finished tile and write its rows
-        auto emit = [&](int gp) {
-            const int item = static_cast<int>(blockIdx.x) + (gp / n_qt) * static_cast<int>(gridDim.x);
-            const int b = item / p.H, h = item % p.H;
-            const int i = (gp % n_qt) * BLOCK_Q + row;
-            const float m0 = s_stat[gp & 1][0][row], l0 = s_stat[gp & 1][1][row];
-            const float m1 = s_stat[gp & 1][2][row], l1 = s_stat[gp & 1][3][row];
-            const float M = fmaxf(m0, m1);
-            const float w0 = ex2_approx(m0 - M), w1 = ex2_approx(m1 - M);
-            const float den = w0 * l0 + w1 * l1;
-            const bool partial = p.o_partial != nullptr;
-            const float c0 = partial ? w0 : w0 / den, c1 = partial ? w1 : w1 / den;
-#pragma unroll 1
-            for (int cc = 0; cc < OC / 16; ++cc) {          // 16 output columns at a time (register pressure)
-                const int col = static_cast<int>(part) * OC + cc * 16;
-                uint32_t ra[16], rb[16];
-                tmem_ld16(lane_addr + O_COL0 + col, ra);
-                tmem_ld16(lane_addr + O_COL0 + 64 + col, rb);
-                ab::tmem_ld_wait();
-                if (i >= p.Lq) continue;
-                float o[16];
+        // t = S * scale2 + (mask + bias) in the log2 domain; new row maxima
+        float mx[2] = {m_run[0], m_run[1]};
 #pragma unroll
-                for (int e = 0; e < 16; ++e) o[e] = c0 * __uint_as_float(ra[e]) + c1 * __uint_as_float(rb[e]);
-                if (partial) {
-                    float* dst = p.o_partial + (static_cast<size_t>(b) * p.Lq + i) * (static_cast<size_t>(p.H) * D) +
-                                 h * D + col;
+        for (int j = 0; j < 8; ++j) {
 #pragma unroll
-                    for (int v4 = 0; v4 < 4; ++v4)
-                        reinterpret_cast<float4*>(dst)[v4] = make_float4(o[4 * v4], o[4 * v4 + 1], o[4 * v4 + 2], o[4 * v4 + 3]);
-                } else {
-                    uint4* dst = reinterpret_cast<uint4*>(p.O + (static_cast<size_t>(b) * p.Lq + i) * p.ldo + h * D + col);
-#pragma unroll
-                    for (int v4 = 0; v4 < 2; ++v4)
-                        dst[v4] = make_uint4(pack2<kBF16>(o[8 * v4], o[8 * v4 + 1]), pack2<kBF16>(o[8 * v4 + 2], o[8 * v4 + 3]),
-                                             pack2<kBF16>(o[8 * v4 + 4], o[8 * v4 + 5]), pack2<kBF16>(o[8 * v4 + 6], o[8 * v4 + 7]));
-                }
-            }
-            if (partial && part == 0 && i < p.Lq) {
-                float* ml = p.ml_partial + ((static_cast<size_t>(b) * p.Lq + i) * p.H + h) * 2;
-                ml[0] = M * (1.0f / LOG2E);
-                ml[1] = den;
-            }
-            if (!partial && p.lse_out != nullptr && part == 0 && i < p.Lq)
-                p.lse_out[(static_cast<size_t>(b) * p.H + h) * p.Lq + i] = M * (1.0f / LOG2E) + __logf(den);
-        };
-
-        int g = 0, item_it = 0;
-        bool pend = false;   // tile g-1 still has to be written out
-        for (int item = blockIdx.x; item < n_items; item += gridDim.x, ++item_it) {
-            const int buf = item_it & 1;
-            ab::mbar_wait(&aux_full[buf], (item_it >> 1) & 1, 53);
-            const float* mask2 = s_mask[buf];
-            const float* bias2 = s_bias[buf];
-            for (int qt = 0; qt < n_qt; ++qt, ++g) {
-                const int i = qt * BLOCK_Q + row;
-                const int boff = min(p.Lq - 1 - i, 2 * MAX_LK - 1 - lk_pad);
-                const int boffc = max(boff, 0);
+            for (int c = 0; c < 2; ++c) {
+                const int key = kb * BK + 8 * j + cq + c;
+                const float mk = s_mask[key];
 #pragma unroll
                 for (int hh = 0; hh < 2; ++hh) {
-                    const uint32_t s_addr = lane_addr + static_cast<uint32_t>(hh * half);
-                    const int key0 = hh * half;
-                    ab::mbar_wait(&s_full[hh], g & 1, 47 + hh);
-                    ab::tc_fence_after();
-                    // ---- pass 1: this thread's (<= 48) score columns are read from TMEM ONCE and stay in registers ----
-                    uint32_t r[MAXU][16];
-#pragma unroll
-                    for (int k = 0; k < MAXU; ++k)
-                        if (k < upp) tmem_ld16(s_addr + (part + k * SPLIT2) * 16, r[k]);
-                    ab::tmem_ld_wait();
-                    float mx = -INFINITY;
-#pragma unroll
-                    for (int k = 0; k < MAXU; ++k)
-                        if (k < upp) {
-                            const int j0 = key0 + static_cast<int>(part + k * SPLIT2) * 16;
-                            mx = fmaxf(mx, has_bias ? unit_scores<true>(r[k], scale2, mask2, bias2, j0, boffc)
-                                                    : unit_scores<false>(r[k], scale2, mask2, bias2, j0, boffc));
-                        }
-                    if (hh == 1 && qt == n_qt - 1) ab::mbar_arrive(&aux_empty[buf]);   // last read of the tables
-                    s_red[part][row] = mx;
-                    sm_bar2();   // also: every thread has finished LOADING S_h, so P may overwrite its columns
-#pragma unroll
-                    for (int q = 0; q < SPLIT2; ++q) mx = fmaxf(mx, s_red[q][row]);
-                    const float mx_use = (mx == -INFINITY) ? 0.f : mx;      // a half made of padding keys only: P = 0
-                    // ---- pass 2: p = 2^(t - max) from registers, packed P over the first half of S_h ----
-                    float sum = 0.f;
-#pragma unroll
-                    for (int k = 0; k < MAXU; ++k)
-                        if (k < upp) {
-                            uint32_t pk[8];
-                            sum += unit_probs<kBF16>(r[k], pk, mx_use);
-                            tmem_st8(s_addr + (part + k * SPLIT2) * 8, pk);
-                        }
-                    s_sum[part][row] = sum;
-                    ab::tmem_st_wait();
-                    if (hh == 0 && pend) {
-                        // O_a(g-1) retired before S_a(g) was issued; O_b(g-1) has its own barrier
-                        ab::mbar_wait(&o_full[1], (g - 1) & 1, 54);
-                        ab::tc_fence_after();
-                        emit(g - 1);
-                        pend = false;
-                    }
-                    ab::tc_fence_before();
-                    sm_bar2();
-                    ab::mbar_arrive(&p_ready[hh]);
-                    sum = 0.f;
-#pragma unroll
-                    for (int q = 0; q < SPLIT2; ++q) sum += s_sum[q][row];
-                    if (part == 0) {
-                        s_stat[g & 1][2 * hh][row] = mx;
-                        s_stat[g & 1][2 * hh + 1][row] = sum;
-                    }
+                    float a = mk;
+                    if (has_bias) a += s_bias[key - min(i0 + 8 * hh, p.Lq - 1) + (p.Lq - 1)];   // rows past Lq are not stored
+                    const float t = fmaf(sc[4 * j + 2 * hh + c], scale2, a);
+                    sc[4 * j + 2 * hh + c] = t;
+                    mx[hh] = fmaxf(mx[hh], t);
                 }
-                pend = true;
             }
         }
-        if (pend) {
-            sm_bar2();   // the last tile's row statistics (written by the part-0 threads) are visible
-            ab::mbar_wait(&o_full[0], (g - 1) & 1, 55);
-            ab::mbar_wait(&o_full[1], (g - 1) & 1, 56);
-            ab::tc_fence_after();
-            emit(g - 1);
+        float corr[2], base[2];
+#pragma unroll
+        for (int hh = 0; hh < 2; ++hh) {
+            mx[hh] = fmaxf(mx[hh], __shfl_xor_sync(0xffffffffu, mx[hh], 1));
+            mx[hh] = fmaxf(mx[hh], __shfl_xor_sync(0xffffffffu, mx[hh], 2));
+            base[hh] = mx[hh] == -INFINITY ? 0.f : mx[hh];
+            corr[hh] = ex2_approx(m_run[hh] - base[hh]);     // 0 for the first block (m_run = -inf)
+            m_run[hh] = mx[hh];
+            l_run[hh] *= corr[hh];
         }
+#pragma unroll
+        for (int j = 0; j < 8; ++j) {
+            o[4 * j] *= corr[0];
+            o[4 * j + 1] *= corr[0];
+            o[4 * j + 2] *= corr[1];
+            o[4 * j + 3] *= corr[1];
+        }
+        // p = 2^(t - m); the row sum takes every probability, the P operand only the kept ones (dropout)
+        uint32_t pa[16];
+#pragma unroll
+        for (int hh = 0; hh < 2; ++hh) {
+            uint32_t w[2][4];
+            if (dropping) {
+                const uint64_t R = (static_cast<uint64_t>(b / p.q_div) * p.H + h) * p.Lq + min(i0 + 8 * hh, p.Lq - 1);
+#pragma unroll
+                for (int gg = 0; gg < 2; ++gg) {
+                    const uint32_t G = static_cast<uint32_t>(((b % p.q_div) * p.Lk + kb * BK + gg * 32) >> 5);
+                    abdrop::attn_words(p.drop, R, G, static_cast<uint32_t>(lane & 3u), w[gg]);
+                }
+            }
+#pragma unroll
+            for (int j = 0; j < 8; ++j) {
+                const float e0 = ex2_approx(sc[4 * j + 2 * hh] - base[hh]);
+                const float e1 = ex2_approx(sc[4 * j + 2 * hh + 1] - base[hh]);
+                l_run[hh] += e0 + e1;
+                float k0 = e0, k1 = e1;
+                if (dropping) {
+                    const uint32_t word = w[j >> 2][j & 3];
+                    k0 = abdrop::keep_lo(p.drop, word) ? e0 : 0.f;
+                    k1 = abdrop::keep_hi(p.drop, word) ? e1 : 0.f;
+                }
+                // A fragment of k16 step j / 2: a0 = (r, keys 0-7), a1 = (r + 8, keys 0-7), a2 / a3 = keys 8-15
+                pa[4 * (j >> 1) + 2 * (j & 1) + hh] = pack2<kBF16>(k0, k1);
+            }
+        }
+        ab::wgmma_fence();
+#pragma unroll
+        for (int k = 0; k < BK / 16; ++k) {
+            const uint32_t a[4] = {pa[4 * k], pa[4 * k + 1], pa[4 * k + 2], pa[4 * k + 3]};
+            const uint64_t bdesc = ab::wgmma_desc_sw128(sV + kb * TILE_BYTES + k * 2048u, 8192);
+            ab::wgmma_m64n64k16_rs<kBF16, 1>(o, a, bdesc, 1);
+        }
+        ab::wgmma_commit();
+        ab::wgmma_wait<0>();
+        ab::wgmma_reg_fence(o);
     }
 
-    ab::tc_fence_before();
-    __syncthreads();
-    if (warp == 0) {
-        ab::tc_fence_after();
-        ab::tmem_dealloc<1>(tmem_base, TMEM_COLS);
+    // ---- output: full row sums across the quad, then normalised 16-bit rows or split-KV partials
+#pragma unroll
+    for (int hh = 0; hh < 2; ++hh) {
+        float l = l_run[hh];
+        l += __shfl_xor_sync(0xffffffffu, l, 1);
+        l += __shfl_xor_sync(0xffffffffu, l, 2);
+        const int i = i0 + 8 * hh;
+        if (i >= lq) continue;
+        const size_t orow = static_cast<size_t>(o_row0) + i;
+        if (p.o_partial != nullptr) {
+            const float ik = p.drop.inv_keep;
+            float* dst = p.o_partial + orow * (static_cast<size_t>(p.H) * D) + h * D + cq;
+#pragma unroll
+            for (int j = 0; j < 8; ++j)
+                *reinterpret_cast<float2*>(dst + 8 * j) = make_float2(o[4 * j + 2 * hh] * ik, o[4 * j + 2 * hh + 1] * ik);
+            if ((lane & 3u) == 0u) {
+                float* ml = p.ml_partial + (orow * p.H + h) * 2;
+                ml[0] = m_run[hh] * (1.0f / LOG2E);
+                ml[1] = l;
+            }
+        } else {
+            const float inv = p.drop.inv_keep / l;
+            if (p.lse_out != nullptr && (lane & 3u) == 0u)
+                p.lse_out[(static_cast<size_t>(b) * p.H + h) * p.Lq + i] = m_run[hh] * (1.0f / LOG2E) + __logf(l);
+            uint16_t* dst = p.O + orow * p.ldo + h * D + cq;
+#pragma unroll
+            for (int j = 0; j < 8; ++j)
+                *reinterpret_cast<uint32_t*>(dst + 8 * j) = pack2<kBF16>(o[4 * j + 2 * hh] * inv, o[4 * j + 2 * hh + 1] * inv);
+        }
     }
+}
+
+template <bool kBF16>
+static int launch(const void* q, int64_t ldq, const void* k, int64_t ldk, const void* v, int64_t ldv, int q_rows, int k_rows,
+                  const Params& p, cudaStream_t s) {
+    CUtensorMap tq, tk, tv;
+    int rc = abh::make_tmap_2d_16bit(&tq, q, static_cast<uint64_t>(q_rows), static_cast<uint64_t>(p.q_col0 + p.H * D),
+                                     static_cast<uint64_t>(ldq), BK, D, kBF16);
+    if (rc) return rc;
+    rc = abh::make_tmap_2d_16bit(&tk, k, static_cast<uint64_t>(k_rows), static_cast<uint64_t>(p.k_col0 + p.H * D),
+                                 static_cast<uint64_t>(ldk), BK, D, kBF16);
+    if (rc) return rc;
+    rc = abh::make_tmap_2d_16bit(&tv, v, static_cast<uint64_t>(k_rows), static_cast<uint64_t>(p.v_col0 + p.H * D),
+                                 static_cast<uint64_t>(ldv), BK, D, kBF16);
+    if (rc) return rc;
+    static bool attr_set = false;
+    if (!attr_set) {
+        AB_CUDA_CHECK(cudaFuncSetAttribute(attention_kernel<kBF16>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES));
+        attr_set = true;
+    }
+    attention_kernel<kBF16><<<dim3(static_cast<unsigned>(p.n_qt), static_cast<unsigned>(p.H), static_cast<unsigned>(p.B)),
+                              THREADS, SMEM_BYTES, s>>>(tq, tk, tv, p);
+    AB_CUDA_CHECK(cudaGetLastError());
+    return ATLAS_B200_OK;
+}
+
+static Params base_params(int B, int H, int Lq, int Lk, int q_col0, int k_col0, int v_col0, void* out, int64_t ldo,
+                          const float* add_mask, const float* bias_delta, float scale, float causal_value) {
+    Params p;
+    p.B = B, p.H = H, p.Lq = Lq, p.Lk = Lk;
+    p.q_col0 = q_col0, p.k_col0 = k_col0, p.v_col0 = v_col0;
+    p.O = static_cast<uint16_t*>(out);
+    p.ldo = ldo;
+    p.add_mask = add_mask;
+    p.bias_delta = bias_delta;
+    p.scale = scale;
+    p.causal_value = causal_value;
+    p.q_div = 1;
+    p.o_partial = nullptr;
+    p.ml_partial = nullptr;
+    p.lse_out = nullptr;
+    p.drop = abdrop::make_key(0.f, 0, 0);
+    p.blk_live = nullptr;
+    p.seg_tile = nullptr;
+    p.n_qt = (Lq + BQ - 1) / BQ;
+    return p;
 }
 
 // out[b, i, h, :] = sum_s w_s O_s / sum_s w_s l_s with w_s = exp(m_s - max_s m_s); one warp per (b, i, h)
@@ -884,19 +356,6 @@ __global__ void combine_splits_kernel(const float* __restrict__ o_partial, const
 
 }  // namespace attn
 
-// csrc/attention_lanes.cu: the three-lane kernel for >= 2 query tiles per (segment, head)
-int atlas_b200_attention_lanes_launch(const void* q, int64_t ldq, int32_t q_col0, const void* k, int64_t ldk, int32_t k_col0,
-                                      const void* v, int64_t ldv, int32_t v_col0, void* out, int64_t ldo,
-                                      const float* add_mask, const float* bias_delta, int32_t B, int32_t H, int32_t Lq,
-                                      int32_t Lk, float scale, float causal_value, float* lse_out, const uint8_t* blk_live,
-                                      const int32_t* seg_tile, const int32_t* seg_work, int32_t is_bf16, cudaStream_t s);
-// csrc/attention_lanes96.cu: the first three-lane kernel (96-key blocks), ATLAS_B200_ATTN_LANES=3
-int atlas_b200_attention_lanes96_launch(const void* q, int64_t ldq, int32_t q_col0, const void* k, int64_t ldk, int32_t k_col0,
-                                       const void* v, int64_t ldv, int32_t v_col0, void* out, int64_t ldo,
-                                       const float* add_mask, const float* bias_delta, int32_t B, int32_t H, int32_t Lq,
-                                       int32_t Lk, float scale, float causal_value, float* lse_out, const uint8_t* blk_live,
-                                       int32_t is_bf16, cudaStream_t s);
-
 extern "C" {
 
 int atlas_b200_attention(const void* q, int64_t ldq, int32_t q_col0, const void* k, int64_t ldk, int32_t k_col0,
@@ -924,15 +383,21 @@ int atlas_b200_attention_packed(const void* qkv, int64_t ld, int32_t q_col0, int
                                 const float* add_mask, const float* bias_delta, const uint8_t* keep, const int32_t* tile_off,
                                 const int32_t* work_prefix, int32_t B, int32_t H, int32_t L, float scale, int32_t is_bf16,
                                 void* stream) {
+    using namespace attn;
+    (void)work_prefix;   // one CTA per (query tile, head, segment): no work-balanced item ranges needed
     AB_REQUIRE(B > 0 && H > 0 && L > 0 && L % 64 == 0 && L <= 384 && keep != nullptr && tile_off != nullptr,
                "attention_packed: 0 < L <= 384, L %% 64 == 0 and the segment tables are required (got L=%d)", L);
     AB_REQUIRE(ld % 8 == 0 && ldo % 8 == 0 && q_col0 % 8 == 0 && k_col0 % 8 == 0 && v_col0 % 8 == 0,
                "attention_packed: strides and column offsets must be multiples of 8 elements");
     cudaStream_t ls = static_cast<cudaStream_t>(stream);
+    Params p = base_params(B, H, L, L, q_col0, k_col0, v_col0, out, ldo, add_mask, bias_delta, scale, 0.f);
+    p.blk_live = keep;
+    p.seg_tile = tile_off;
+    // the packed rows of all segments: at most B * L (the tensor maps only bound the TMA boxes)
+    const int rows = B * L;
     abh::prof_begin(ls, abh::PROF_ATTENTION);
-    const int lrc = atlas_b200_attention_lanes_launch(qkv, ld, q_col0, qkv, ld, k_col0, qkv, ld, v_col0, out, ldo, add_mask,
-                                                      bias_delta, B, H, L, L, scale, 0.f, nullptr, keep, tile_off, work_prefix, is_bf16,
-                                                      ls);
+    const int lrc = is_bf16 ? launch<true>(qkv, ld, qkv, ld, qkv, ld, rows, rows, p, ls)
+                            : launch<false>(qkv, ld, qkv, ld, qkv, ld, rows, rows, p, ls);
     if (lrc) return lrc;
     // dense-equivalent work, like the masked-block skipping of the padded layout
     abh::prof_end(ls, abh::PROF_ATTENTION, 4.0 * B * H * static_cast<double>(L) * L * attn::D);
@@ -962,77 +427,20 @@ int atlas_b200_attention_train(const void* q, int64_t ldq, int32_t q_col0, const
                    v_col0 % 8 == 0,
                "attention: strides and column offsets must be multiples of 8 elements");
     if (B == 0) return ATLAS_B200_OK;
-    // >= 2 query tiles per (segment, head) (encoder self-attention of FiD / Contriever): the three-lane kernel.
-    // ATLAS_B200_ATTN_LANES=0 selects the first-generation kernels for A/B measurements.
-    static const int lanes_sel = getenv("ATLAS_B200_ATTN_LANES") != nullptr ? atoi(getenv("ATLAS_B200_ATTN_LANES")) : 1;
-    if (lanes_sel != 0 && !dropping && o_partial == nullptr && q_div == 1 && Lq > 128 && Lq <= 512 && Lk <= 576) {
-        cudaStream_t ls = static_cast<cudaStream_t>(stream);
-        abh::prof_begin(ls, abh::PROF_ATTENTION);
-        int lrc = lanes_sel == 3
-                      ? atlas_b200_attention_lanes96_launch(q, ldq, q_col0, k, ldk, k_col0, v, ldv, v_col0, out, ldo, add_mask,
-                                                            bias_delta, B, H, Lq, Lk, scale, causal_value, lse_out, key_block_live,
-                                                            is_bf16, ls)
-                      : atlas_b200_attention_lanes_launch(q, ldq, q_col0, k, ldk, k_col0, v, ldv, v_col0, out, ldo, add_mask,
-                                                          bias_delta, B, H, Lq, Lk, scale, causal_value, lse_out, key_block_live,
-                                                          nullptr, nullptr, is_bf16, ls);
-        if (lrc) return lrc;
-        abh::prof_end(ls, abh::PROF_ATTENTION, 4.0 * B * H * static_cast<double>(Lq) * Lk * D);
-        abh::count_launch();
-        return ATLAS_B200_OK;
-    }
-    CUtensorMap tq, tk, tv;
-    int rc = abh::make_tmap_2d_16bit(&tq, q, static_cast<uint64_t>(B / q_div) * Lq, static_cast<uint64_t>(q_col0 + H * D),
-                                     static_cast<uint64_t>(ldq), BLOCK_Q, D, is_bf16 != 0);
-    if (rc) return rc;
-    rc = abh::make_tmap_2d_16bit(&tk, k, static_cast<uint64_t>(B) * Lk, static_cast<uint64_t>(k_col0 + H * D),
-                                 static_cast<uint64_t>(ldk), 128, D, is_bf16 != 0);
-    if (rc) return rc;
-    rc = abh::make_tmap_2d_16bit(&tv, v, static_cast<uint64_t>(B) * Lk, static_cast<uint64_t>(v_col0 + H * D),
-                                 static_cast<uint64_t>(ldv), 128, D, is_bf16 != 0);
-    if (rc) return rc;
-    Params p;
-    p.B = B;
-    p.H = H;
-    p.Lq = Lq;
-    p.Lk = Lk;
-    p.q_col0 = q_col0;
-    p.k_col0 = k_col0;
-    p.v_col0 = v_col0;
-    p.O = static_cast<uint16_t*>(out);
-    p.ldo = ldo;
-    p.add_mask = add_mask;
-    p.bias_delta = bias_delta;
-    p.scale = scale;
-    p.causal_value = causal_value;
+    Params p = base_params(B, H, Lq, Lk, q_col0, k_col0, v_col0, out, ldo, add_mask, bias_delta, scale, causal_value);
     p.q_div = q_div;
     p.o_partial = o_partial;
     p.ml_partial = ml_partial;
     p.lse_out = lse_out;
     p.drop = drop;
+    p.blk_live = key_block_live;
     cudaStream_t s = static_cast<cudaStream_t>(stream);
-    const int items = B * H;
-    const int grid = items < abh::num_sms() ? items : abh::num_sms();
     abh::prof_begin(s, abh::PROF_ATTENTION);
-    static const bool no_split = getenv("ATLAS_B200_ATTN_NO_SPLIT") != nullptr;   // A/B measurements
-    // dropout on the probabilities (training) is implemented in attention_kernel only
-    const bool split = ((Lk + 127) / 128) * 128 <= 384 && !no_split && !dropping;
-    const int threads = split ? THREADS_SPLIT : THREADS;
-    auto launch = [&](auto kernel, bool& attr_done) -> int {
-        if (!attr_done) {
-            AB_CUDA_CHECK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES));
-            attr_done = true;
-        }
-        kernel<<<grid, threads, SMEM_BYTES, s>>>(tq, tk, tv, p);
-        return ATLAS_B200_OK;
-    };
-    static bool attr_set[4] = {false, false, false, false};
-    int lrc;
-    if (split) lrc = is_bf16 ? launch(attention_split_kernel<true>, attr_set[0]) : launch(attention_split_kernel<false>, attr_set[1]);
-    else lrc = is_bf16 ? launch(attention_kernel<true>, attr_set[2]) : launch(attention_kernel<false>, attr_set[3]);
+    const int lrc = is_bf16 ? launch<true>(q, ldq, k, ldk, v, ldv, (B / q_div) * Lq, B * Lk, p, s)
+                            : launch<false>(q, ldq, k, ldk, v, ldv, (B / q_div) * Lq, B * Lk, p, s);
     if (lrc) return lrc;
     abh::prof_end(s, abh::PROF_ATTENTION, 4.0 * B * H * static_cast<double>(Lq) * Lk * D);
     abh::count_launch();
-    AB_CUDA_CHECK(cudaGetLastError());
     return ATLAS_B200_OK;
 }
 

@@ -17,8 +17,7 @@
 //   attn_bwd_dkv2_kernel  CTA = (b, h, 64-key block): the transposed problem, loops over the query blocks, accumulates dK, dV.
 //   attn_bwd_dq_kernel / attn_bwd_dkv_kernel: first-generation kernels, used when no forward lse is passed (pass 1 over
 //                         the keys recomputes it) and for A/B runs (ATLAS_B200_ATTN_BWD_V1).
-// Bound: tensor (legacy warp-MMA path; profile: profiles/r01_train_step_and_backward_kernels.md).  The tcgen05 version of
-// the dQ kernel (attention_bwd_tc.cu, ATLAS_B200_ATTN_BWD_TC=1) is validated but not yet faster, DESIGN.md §8.
+// Bound: tensor (warp-level mma.sync m16n8k16 fragments).
 // FLOPs per call = 2 * B*H*Lq*Lk*64 * 7 with the forward's lse (S + dP + dQ in the first kernel, S + dP + dV + dK in the
 // second), 8 when it is recomputed.
 #include "common.cuh"
@@ -827,21 +826,6 @@ attn_bwd_dkv2_kernel(const Params p) {
 
 }  // namespace attnb
 
-// experimental tcgen05 dQ kernel (attention_bwd_tc.cu), selected with ATLAS_B200_ATTN_BWD_TC=1
-int atlas_b200_attn_bwd_dq_tc(const void* q, int64_t ldq, int32_t q_col0, const void* k, int64_t ldk, int32_t k_col0,
-                              const void* v, int64_t ldv, int32_t v_col0, const void* out, int64_t ldo, const void* dout,
-                              int64_t lddo, void* dq, int64_t lddq, int32_t dq_col0, const float* add_mask,
-                              const float* bias_delta, float* dbias_delta, const float* lse, float* dsum, int32_t B,
-                              int32_t H, int32_t Lq, int32_t Lk, float scale, float causal_value, int32_t is_bf16,
-                              cudaStream_t s);
-
-// ... and its dK / dV twin (attention_bwd_tc_dkv.cu), selected with ATLAS_B200_ATTN_BWD_TC=2
-int atlas_b200_attn_bwd_dkv_tc(const void* q, int64_t ldq, int32_t q_col0, const void* k, int64_t ldk, int32_t k_col0,
-                               const void* v, int64_t ldv, int32_t v_col0, const void* dout, int64_t lddo, void* dk,
-                               int64_t lddk, int32_t dk_col0, void* dv, int64_t lddv, int32_t dv_col0, const float* add_mask,
-                               const float* bias_delta, const float* lse, const float* dsum, const uint8_t* blk_live,
-                               int32_t B, int32_t H, int32_t Lq, int32_t Lk, float scale, float causal_value, int32_t is_bf16,
-                               cudaStream_t s);
 
 extern "C" {
 
@@ -944,35 +928,7 @@ int atlas_b200_attention_bwd_train(const void* q, int64_t ldq, int32_t q_col0, c
         attr_set = true;
     }
     abh::prof_begin(s, abh::PROF_ATTENTION_BWD);
-    // tcgen05 kernels (attention_bwd_tc*.cu), ATLAS_B200_ATTN_BWD_TC: 1 = dQ kernel, 2 = dQ + dK/dV kernels, 3 = dK/dV kernel
-    // only (the dQ kernel is not yet faster than its warp-MMA twin; the dK/dV kernel is: 0.23 vs 0.33 ms at
-    // 80 x 12 x 384 x 384).  The warp-MMA dQ kernel runs first in mode 3: it writes D = rowsum(dO o O), which the
-    // tcgen05 dK/dV kernel reads.
-    // Default (round 2): mode 3 - it passes the backward / training suites and is 16 % faster than the two warp-MMA kernels
-    // at 80 x 12 x 384 x 384 (0.66 vs 0.80 ms, profiles/r02_attention_bwd_tc_ab_visit_h.log); 0 = warp-MMA kernels only.
-    static const int tc_level = getenv("ATLAS_B200_ATTN_BWD_TC") ? atoi(getenv("ATLAS_B200_ATTN_BWD_TC")) : 3;
-    const bool use_tc = tc_level >= 1 && drop.thr16 == 0u;     // the tcgen05 kernels do not implement dropout
-    bool dq_done = false, dkv_done = false;
-    if (v2 && use_tc && dq_accum == nullptr) {
-        if (tc_level != 3) {
-            const int rc = atlas_b200_attn_bwd_dq_tc(q, ldq, q_col0, k, ldk, k_col0, v, ldv, v_col0, out, ldo, dout, lddo, dq,
-                                                     lddq, dq_col0, add_mask, bias_delta, dbias_delta, lse, dsum, B, H, Lq, Lk,
-                                                     scale, causal_value, is_bf16, s);
-            if (rc == ATLAS_B200_OK) dq_done = true;
-            else if (rc != ATLAS_B200_EUNSUPPORTED) return rc;
-        } else if (Lq <= 512 && Lk <= 512) {
-            if (is_bf16) attn_bwd_dq2_kernel<true><<<static_cast<unsigned>(nq_ctas), THREADS, smem_dq, s>>>(p);
-            else attn_bwd_dq2_kernel<false><<<static_cast<unsigned>(nq_ctas), THREADS, smem_dq, s>>>(p);
-            dq_done = true;
-        }
-        if (dq_done && tc_level >= 2) {
-            const int rc2 = atlas_b200_attn_bwd_dkv_tc(q, ldq, q_col0, k, ldk, k_col0, v, ldv, v_col0, dout, lddo, dk, lddk,
-                                                       dk_col0, dv, lddv, dv_col0, add_mask, bias_delta, lse, dsum, key_block_live, B,
-                                                       H, Lq, Lk, scale, causal_value, is_bf16, s);
-            if (rc2 == ATLAS_B200_OK) dkv_done = true;
-            else if (rc2 != ATLAS_B200_EUNSUPPORTED) return rc2;
-        }
-    }
+    const bool dq_done = false, dkv_done = false;
     if (v2) {
         if (is_bf16) {
             if (!dq_done) attn_bwd_dq2_kernel<true><<<static_cast<unsigned>(nq_ctas), THREADS, smem_dq, s>>>(p);

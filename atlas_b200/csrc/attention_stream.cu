@@ -5,12 +5,11 @@
 // combine_splits_kernel.
 //
 // Why a second kernel: the operation is a pure K / V STREAM (377 MB per layer and 8 queries, 12 GFLOP: 32 FLOP/B, far left of
-// the ridge).  The tcgen05 split kernel treats every 384-key segment as a serial load -> S -> softmax -> P.V chain on a
-// 128-row tile of which 32 rows are real, one CTA per SM: 160 us per layer = 36 % of the HBM roofline
-// (profiles/r02_launches_step_visit_f.csv; double-buffering its K / V did not help, the chain - not the load - sets the
-// segment time).  Here: small CTAs (128 threads, 40 KB of shared memory -> 5 per SM), each streaming its key chunk through a
+// the ridge).  A one-CTA-per-segment kernel treats every 384-key segment as a serial load -> S -> softmax -> P.V chain on a
+// 128-row tile of which 32 rows are real: the chain, not the load, sets the segment time.  Here: small CTAs (128 threads,
+// 40 KB of shared memory -> 5 per SM), each streaming its key chunk through a
 // cp.async double buffer of 64-key K / V tiles, flash-attention style online softmax on warp-level mma.sync fragments (the
-// arithmetic is 1 / 6 of what the HBM time allows, so the legacy tensor-core path is the right tool: no TMEM hand-offs, many
+// arithmetic is 1 / 6 of what the HBM time allows, so the legacy tensor-core path is the right tool: many
 // independent CTAs per SM hide each other's latencies).
 // Bound: HBM.  Algorithmic bytes per launch = B x Lk x 2 x H x 64 x 2 (K and V once) + the fp32 partials.
 #include "common.cuh"

@@ -2,7 +2,7 @@
 // derives for the row-wise / elementwise pieces of Contriever (src/modeling_bert.py) and FiD's T5 (src/modeling_t5.py),
 // plus the layout helpers the weight-gradient GEMMs need.  One pass over the rows each, 16-bit activations, fp32 math.
 //
-//   transpose_16bit     [R, C] -> [C, Rpad] (zero padded): dY^T and X^T for dW = dY^T X on the K-major tcgen05 GEMM
+//   transpose_16bit     [R, C] -> [C, Rpad] (zero padded): dY^T and X^T for dW = dY^T X on the K-major wgmma GEMM
 //   colsum_f32          bias gradient: db[n] = sum_m dY[m, n]
 //   norm_bwd            BertLayerNorm (uncentred 2nd moment, modeling_bert.py:104-114) / T5 RMSNorm (modeling_t5.py:244-253)
 //   gated_gelu fwd/bwd  T5DenseGatedGeluDense (modeling_t5.py:281-285) on the interleaved (wi_0 | wi_1) projection

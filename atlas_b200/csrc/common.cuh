@@ -1,7 +1,6 @@
-// Shared device-side building blocks for the sm_100a kernels of atlas_b200:
-// mbarrier, TMA (cp.async.bulk.tensor), tcgen05 (alloc / mma / commit / ld / st) wrappers,
-// UMMA shared-memory and instruction descriptors.  Hand-written inline PTX; the bit layouts
-// follow the PTX ISA "tcgen05 matrix/instruction descriptor" tables.
+// Shared device-side building blocks for the sm_90a kernels of atlas_b200:
+// mbarrier, TMA (cp.async.bulk.tensor) and register re-partitioning (setmaxnreg).  Hand-written inline
+// PTX; the warpgroup MMA wrappers live in wgmma.cuh.
 #pragma once
 
 #include <cuda.h>
@@ -71,15 +70,6 @@ __device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
     asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
 }
 
-// Arrive on the barrier at the same smem offset in CTA `cta` of the cluster.
-__device__ __forceinline__ void mbar_arrive_cluster(uint64_t* bar, uint32_t cta) {
-    uint32_t remote;
-    asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(remote) : "r"(smem_u32(bar)), "r"(cta));
-    // plain (CTA-scope release) arrive on the remote barrier, as CUTLASS' ClusterBarrier::arrive(cta_id) does:
-    // a cluster-scope release here was measured to cost ~2500 cycles per arrive under load.
-    asm volatile("mbarrier.arrive.shared::cluster.b64 _, [%0];" ::"r"(remote) : "memory");
-}
-
 __device__ __forceinline__ bool mbar_try_wait(uint64_t* bar, uint32_t parity) {
     uint32_t ok;
     asm volatile(
@@ -144,19 +134,6 @@ __device__ __forceinline__ void tma_load_2d(const CUtensorMap* map, uint64_t* ba
         : "memory");
 }
 
-// 2-CTA variant: both CTAs of the pair issue it; completion bytes land on the LEADER CTA's barrier
-// (peer bit of the shared::cluster address cleared).
-__device__ __forceinline__ void tma_load_2d_2sm(const CUtensorMap* map, uint64_t* bar, void* smem_dst, int32_t c0,
-                                                int32_t c1, uint64_t cache_hint) {
-    uint32_t bar_addr = smem_u32(bar) & 0xFEFFFFFFu;
-    asm volatile(
-        "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes.L2::cache_hint"
-        " [%0], [%1, {%3, %4}], [%2], %5;"
-        ::"r"(smem_u32(smem_dst)), "l"(reinterpret_cast<uint64_t>(map)), "r"(bar_addr), "r"(c0), "r"(c1),
-        "l"(cache_hint)
-        : "memory");
-}
-
 // TMA store of a shared-memory box (written by this CTA's threads with generic stores: fence_proxy_async_smem first) to
 // global memory through a tensor map; bulk-group completion (commit + wait_group[.read]) by the issuing thread.
 __device__ __forceinline__ void tma_store_2d(const CUtensorMap* map, const void* smem_src, int32_t c0, int32_t c1) {
@@ -177,209 +154,12 @@ __device__ __forceinline__ void tma_prefetch_2d(const CUtensorMap* map, int32_t 
                  : "memory");
 }
 
-// 2-CTA + multicast: the box lands at the same shared-memory offset in every CTA of `cta_mask`; each destination's bytes
-// are counted on the barrier at this offset in the leader of THAT destination's CTA pair.
-__device__ __forceinline__ void tma_load_2d_2sm_mc(const CUtensorMap* map, uint64_t* bar, void* smem_dst, int32_t c0,
-                                                   int32_t c1, uint16_t cta_mask, uint64_t cache_hint) {
-    uint32_t bar_addr = smem_u32(bar) & 0xFEFFFFFFu;
-    asm volatile(
-        "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster"
-        ".L2::cache_hint [%0], [%1, {%4, %5}], [%2], %3, %6;"
-        ::"r"(smem_u32(smem_dst)), "l"(reinterpret_cast<uint64_t>(map)), "r"(bar_addr), "h"(cta_mask), "r"(c0), "r"(c1),
-        "l"(cache_hint)
-        : "memory");
-}
-
-__device__ __forceinline__ void tma_load_3d(const CUtensorMap* map, uint64_t* bar, void* smem_dst, int32_t c0,
-                                            int32_t c1, int32_t c2, uint64_t cache_hint) {
-    asm volatile(
-        "cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes.L2::cache_hint"
-        " [%0], [%1, {%3, %4, %5}], [%2], %6;"
-        ::"r"(smem_u32(smem_dst)), "l"(reinterpret_cast<uint64_t>(map)), "r"(smem_u32(bar)), "r"(c0), "r"(c1),
-        "r"(c2), "l"(cache_hint)
-        : "memory");
-}
-
-__device__ __forceinline__ void tma_load_3d_2sm(const CUtensorMap* map, uint64_t* bar, void* smem_dst, int32_t c0,
-                                                int32_t c1, int32_t c2, uint64_t cache_hint) {
-    uint32_t bar_addr = smem_u32(bar) & 0xFEFFFFFFu;
-    asm volatile(
-        "cp.async.bulk.tensor.3d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes.L2::cache_hint"
-        " [%0], [%1, {%3, %4, %5}], [%2], %6;"
-        ::"r"(smem_u32(smem_dst)), "l"(reinterpret_cast<uint64_t>(map)), "r"(bar_addr), "r"(c0), "r"(c1), "r"(c2),
-        "l"(cache_hint)
-        : "memory");
-}
-
 // ---------------------------------------------------------------------------------------------
-// tcgen05: TMEM allocation
+// register re-partitioning between warpgroups (every warp of a warpgroup executes it)
 // ---------------------------------------------------------------------------------------------
-template <int kCtaGroup>
-__device__ __forceinline__ void tmem_alloc(uint32_t* smem_result, uint32_t ncols) {
-    if constexpr (kCtaGroup == 1) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_result)),
-                     "r"(ncols)
-                     : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    } else {
-        asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_result)),
-                     "r"(ncols)
-                     : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-    }
-}
-
-template <int kCtaGroup>
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-    if constexpr (kCtaGroup == 1) {
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-    } else {
-        asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-    }
-}
-
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-
-// ---------------------------------------------------------------------------------------------
-// tcgen05: descriptors
-// ---------------------------------------------------------------------------------------------
-// Shared-memory matrix descriptor for a K-major operand tile stored as rows of 128 bytes
-// (64 x 16-bit elements) with the 128-byte swizzle, i.e. exactly what a TMA box {64, rows} with
-// CU_TENSOR_MAP_SWIZZLE_128B writes.  8-row groups are 1024 bytes apart (SBO); LBO is unused for
-// swizzled K-major layouts (canonical value 1).  Bits: [0,14) addr>>4, [16,30) LBO>>4,
-// [32,46) SBO>>4, [46,48) version=1 (sm_100), [61,64) layout type (2 = SWIZZLE_128B).
-__device__ __forceinline__ uint64_t umma_desc_k_sw128(uint32_t smem_addr) {
-    uint64_t d = 0;
-    d |= static_cast<uint64_t>((smem_addr & 0x3FFFFu) >> 4);
-    d |= static_cast<uint64_t>(1) << 16;
-    d |= static_cast<uint64_t>(1024 >> 4) << 32;
-    d |= static_cast<uint64_t>(1) << 46;
-    d |= static_cast<uint64_t>(2) << 61;
-    return d;
-}
-
-// Instruction descriptor for kind::f16 (fp16 or bf16 operands, fp32 accumulate), both operands
-// K-major.  Bits: [4,6) D format (1 = f32), [7,10) A format, [10,13) B format (0 = f16, 1 = bf16),
-// bit 15/16 A/B major (0 = K), [17,23) N>>3, [24,29) M>>4.
-__host__ __device__ constexpr uint32_t umma_idesc_f16(int m, int n, bool bf16) {
-    return (1u << 4) | ((bf16 ? 1u : 0u) << 7) | ((bf16 ? 1u : 0u) << 10) | (static_cast<uint32_t>(n >> 3) << 17) |
-           (static_cast<uint32_t>(m >> 4) << 24);
-}
-
-// ---------------------------------------------------------------------------------------------
-// tcgen05: mma / commit
-// ---------------------------------------------------------------------------------------------
-// D[tmem] (+)= A[smem] * B[smem]^T ; one thread issues on behalf of the CTA (pair).
-template <int kCtaGroup>
-__device__ __forceinline__ void umma_ss(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc,
-                                        uint32_t accumulate) {
-    if constexpr (kCtaGroup == 1) {
-        asm volatile(
-            "{\n\t"
-            ".reg .pred p;\n\t"
-            "setp.ne.b32 p, %4, 0;\n\t"
-            "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t"
-            "}\n" ::"r"(d_tmem),
-            "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate)
-            : "memory");
-    } else {
-        asm volatile(
-            "{\n\t"
-            ".reg .pred p;\n\t"
-            "setp.ne.b32 p, %4, 0;\n\t"
-            "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t"
-            "}\n" ::"r"(d_tmem),
-            "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate)
-            : "memory");
-    }
-}
-
-// D[tmem] (+)= A[tmem] * B[smem]^T
-template <int kCtaGroup>
-__device__ __forceinline__ void umma_ts(uint32_t d_tmem, uint32_t a_tmem, uint64_t b_desc, uint32_t idesc,
-                                        uint32_t accumulate) {
-    if constexpr (kCtaGroup == 1) {
-        asm volatile(
-            "{\n\t"
-            ".reg .pred p;\n\t"
-            "setp.ne.b32 p, %4, 0;\n\t"
-            "tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, p;\n\t"
-            "}\n" ::"r"(d_tmem),
-            "r"(a_tmem), "l"(b_desc), "r"(idesc), "r"(accumulate)
-            : "memory");
-    } else {
-        asm volatile(
-            "{\n\t"
-            ".reg .pred p;\n\t"
-            "setp.ne.b32 p, %4, 0;\n\t"
-            "tcgen05.mma.cta_group::2.kind::f16 [%0], [%1], %2, %3, p;\n\t"
-            "}\n" ::"r"(d_tmem),
-            "r"(a_tmem), "l"(b_desc), "r"(idesc), "r"(accumulate)
-            : "memory");
-    }
-}
-
-// Make the mbarrier track completion of all tcgen05 ops issued so far by this thread.
-// (implies tcgen05.fence::before_thread_sync)
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar))
-                 : "memory");
-}
-
-// 2-CTA: signal the barrier at the same offset in every CTA selected by `cta_mask`.
-__device__ __forceinline__ void umma_commit_2sm(uint64_t* bar, uint16_t cta_mask) {
-    asm volatile(
-        "tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(
-            smem_u32(bar)),
-        "h"(cta_mask)
-        : "memory");
-}
-
-// ---------------------------------------------------------------------------------------------
-// tcgen05: TMEM <-> registers.  32x32b shape: thread t of warp w touches lane 32*(w%4)+t,
-// register j <-> column (col0 + j).
-// ---------------------------------------------------------------------------------------------
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t (&r)[32]) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-          "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]),
-          "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]),
-          "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-        : "r"(taddr));
-}
-
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-
-__device__ __forceinline__ void tmem_st32(uint32_t taddr, const uint32_t (&r)[32]) {
-    asm volatile(
-        "tcgen05.st.sync.aligned.32x32b.x32.b32 [%0], "
-        "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, "
-        "%17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32};" ::"r"(taddr),
-        "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]), "r"(r[8]), "r"(r[9]),
-        "r"(r[10]), "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15]), "r"(r[16]), "r"(r[17]), "r"(r[18]),
-        "r"(r[19]), "r"(r[20]), "r"(r[21]), "r"(r[22]), "r"(r[23]), "r"(r[24]), "r"(r[25]), "r"(r[26]), "r"(r[27]),
-        "r"(r[28]), "r"(r[29]), "r"(r[30]), "r"(r[31])
-        : "memory");
-}
-
-__device__ __forceinline__ void tmem_st_wait() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
-
-// ---------------------------------------------------------------------------------------------
-// clusters
-// ---------------------------------------------------------------------------------------------
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-    uint32_t r;
-    asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-    return r;
-}
-
-__device__ __forceinline__ void cluster_sync_all() {
-    asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");
-    asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
+template <int kRegs>
+__device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(kRegs)); }
+template <int kRegs>
+__device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(kRegs)); }
 
 }  // namespace ab

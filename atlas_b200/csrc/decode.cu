@@ -7,7 +7,7 @@
 //                                   generation): block = (key chunk, head, batch); emits un-normalised fp32 partials +
 //                                   (max, sum) that attn::combine_splits_kernel merges (same identity as the split-KV
 //                                   forward).  Algorithmic bytes per (query, layer, step) = Lk * 2 * H*64 * 2 B
-//                                   (FiD-base, Lk = 15 360: 47 MB; SURVEY.md §8a: 566 MB / query / step over 12 layers).
+//                                   (FiD-base, Lk = 15 360: 47 MB).
 //   decode_self_attention_kernel    appends the new token's K | V to the per-layer cache row t (t read from DEVICE memory so
 //                                   the whole step can be replayed from one CUDA graph) and attends over keys 0..t with
 //                                   T5's relative-position bias.

@@ -17,7 +17,7 @@
 //     counter (4 G + q, R_lo, R_hi, offset_lo); element j uses bits [16 (j & 1), +16) of word t = (j % 32) / 8.
 //     One call therefore covers the columns {32 G + 8 t + 2 q + {0, 1} : t = 0..3} of one row: exactly the eight
 //     elements one thread of an mma.sync accumulator fragment holds per row and 32-column group (backward kernels), and
-//     four calls cover a 32-column chunk of a TMEM row (forward kernels, thread = row) - no call is shared or wasted.
+//     four calls cover a 32-key group of the two rows a thread of a wgmma accumulator holds (forward kernel) - no call is shared or wasted.
 #pragma once
 
 #include <stdint.h>

@@ -201,7 +201,7 @@ masked_mean_pool_kernel(const uint16_t* __restrict__ x, const int64_t* __restric
 }
 
 
-// Reader-input assembly from the device-resident passage token bank (SURVEY.md §8f-1; replaces the per-step host work of
+// Reader-input assembly from the device-resident passage token bank (replaces the per-step host work of
 // Atlas.tokenize_passages, src/atlas.py:261-280: bsz x n_context string formats + tokenizer calls):
 //   row (b, j) = (query_ids[b, :qlen[b]] ++ bank_ids[rows[b, j], :bank_lens[...]])[: L - 1] ++ [eos], padded with `pad`
 // and the attention mask of the same shape.  rows[b, j] < 0 is the "" padding passage: EOS only (src/atlas.py:26-39).

@@ -1,14 +1,14 @@
-// Dense linear layers of Contriever (BERT) and FiD (T5) on tcgen05:
+// Dense linear layers of Contriever (BERT) and FiD (T5) on Hopper warpgroup MMAs (wgmma):
 //     C[M, N] = epilogue( A[M, K] . W[N, K]^T )        A, W, C 16-bit (fp16 or bf16), fp32 accumulate
 // W is the nn.Linear weight as stored ([out_features, in_features]), i.e. both operands are K-major
-// and stream through TMA boxes with the 128-byte swizzle straight into UMMA shared-memory descriptors.
+// and stream through TMA boxes with the 128-byte swizzle straight into wgmma shared-memory descriptors.
 //
 // Replaces the cuBLAS GEMM + separate ATen elementwise kernels behind
 //   BertSelfAttention q/k/v, BertSelfOutput.dense, BertIntermediate.dense (+erf-GELU),
 //   BertOutput.dense                                     (src/modeling_bert.py:280-466)
 //   T5Attention q/k/v/o, T5DenseGatedGeluDense wi_0/wi_1 (+gelu_new gate)/wo, lm_head
 //                                                        (src/modeling_t5.py:272-289,418-531,1642-1647)
-// Fused epilogues (runtime-selected, applied to the fp32 accumulator read back from TMEM):
+// Fused epilogues (runtime-selected, applied to the fp32 accumulator registers):
 //   EPI_NONE      C = acc
 //   EPI_BIAS      C = acc + bias[n]
 //   EPI_GELU      C = gelu_erf(acc + bias[n])                      (ACT2FN["gelu"], modeling_bert.py:444)
@@ -16,19 +16,15 @@
 //   EPI_GATED     C[m, j] = gelu_new(acc[m, 2j]) * acc[m, 2j+1]    (W rows interleaved wi_0/wi_1;
 //                                                                   modeling_t5.py:281-285, fp32 GELU)
 //
-// Persistent, warp-specialised, one CTA per SM (grid = #SMs):
-//   warp 0 TMA producer | warp 1 MMA issuer (UMMA K=16) | warp 2 TMEM allocator
-//   warps 4-11 epilogue: TMEM -> registers -> epilogue math -> 16-bit global stores
-// TMEM: 2 accumulator buffers x BLOCK_N columns, so the epilogue of tile i overlaps the MMAs of tile i+1.
-// Two tile shapes:
-//   kPair = true  (large M): a 2-CTA cluster computes a 256 x 256 tile with cta_group::2 MMAs (UMMA M=256, N=256).
-//       Each CTA streams its own 128 rows of A and HALF of the W tile (128 rows) -> 32 KB per 64-wide K block and
-//       CTA instead of 48 KB, which buys a 6-stage ring: the mainloop of the 1-CTA shape was starved by L2 latency
-//       (4 stages x 48 KB in flight ~ latency x bandwidth; tensor pipe 61 % busy, profiles/r01_gemm_v1.md).
-//       The leader CTA issues the MMAs; tcgen05.commit multicasts ring / accumulator barriers to both CTAs.
-//   kPair = false: one CTA, 128 x BLOCK_N tiles (small M: decoder, tails).
+// Persistent, warp-specialised, one CTA per SM (grid = #SMs), 128 x BLOCK_N tiles (BLOCK_N = 256 once there are enough
+// tiles to fill the SMs, else 128):
+//   warpgroup 0  TMA producer (one thread; setmaxnreg gives its registers to the consumers)
+//   warpgroups 1, 2  consumers: 64 rows x BLOCK_N columns each, wgmma m64nBLOCK_Nk16 into registers, then the epilogue
+//                    straight from the accumulator registers to global memory
+// A ring of 64-wide K stages (~200 KB of shared memory) keeps the next tile's loads in flight during the epilogue.
 #include "common.cuh"
 #include "host_common.h"
+#include "wgmma.cuh"
 
 #include <math.h>
 #include <stdlib.h>
@@ -37,26 +33,19 @@ namespace gemm {
 
 constexpr int BLOCK_M = 128;
 constexpr int BLOCK_K = 64;
-constexpr int UMMA_K = 16;
-constexpr int THREADS = 384;
-constexpr int EPI_WARPS = 8;
+constexpr int UMMA_K = 16;      // K of one wgmma
+constexpr int CONSUMERS = 2;    // consumer warpgroups
+constexpr int THREADS = 128 * (1 + CONSUMERS);
 
 enum Epilogue { EPI_NONE = 0, EPI_BIAS = 1, EPI_GELU = 2, EPI_RESIDUAL = 3, EPI_GATED = 4 };
 
-template <int BLOCK_N, bool kPair>
+template <int BLOCK_N>
 struct Cfg {
-    static constexpr int CTAS = kPair ? 2 : 1;
-    static constexpr int A_BYTES = BLOCK_M * BLOCK_K * 2;                 // this CTA's 128 rows of A
-    static constexpr int B_ROWS = BLOCK_N / CTAS;                         // W rows this CTA streams
-    static constexpr int B_BYTES = B_ROWS * BLOCK_K * 2;
+    static constexpr int A_BYTES = BLOCK_M * BLOCK_K * 2;
+    static constexpr int B_BYTES = BLOCK_N * BLOCK_K * 2;
     static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
-    static constexpr int STAGES = (192 * 1024) / STAGE_BYTES;
-    // epilogue staging (BLOCK_N = 256 kernels): 4 KB per epilogue warp = 32 rows x 128 B (64 output columns), 128B swizzle,
-    // the source of the TMA stores of C
-    static constexpr int EPI_STAGE_BYTES = BLOCK_N == 256 ? EPI_WARPS * 4096 : 0;
-    static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + EPI_STAGE_BYTES + 1024;
-    static constexpr int TMEM_COLS = 2 * BLOCK_N;  // 256 or 512 (power of two)
-    static constexpr int UMMA_M = BLOCK_M * CTAS;
+    static constexpr int STAGES = (200 * 1024) / STAGE_BYTES;
+    static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + 1024;
 };
 
 struct Params {
@@ -71,7 +60,7 @@ struct Params {
     //   row_ss  [M] fp32 sum of squares of the A rows (or nullptr): acc[m, :] *= rsqrt(row_ss[m] / K + rs_eps) before the
     //           epilogue, i.e. the GEMM consumes the UN-normalised rows with the norm weight folded into W
     //   out_ss  [M] fp32 (or nullptr): += sum over this launch's columns of (16-bit rounded output)^2, the statistic the
-    //           next RMSNorm needs, accumulated with one atomicAdd per thread and tile
+    //           next RMSNorm needs, accumulated with one atomicAdd per row, quad and tile
     const float* row_ss;
     float* out_ss;
     float rs_eps;
@@ -81,7 +70,6 @@ struct Params {
     int splits, kb_per_split;
     float* C32;
     int l2_prefetch;      // producer prefetches the next work item's A rows into L2 (ATLAS_B200_GEMM_PREFETCH=0: off)
-    int tma_store;        // 16-bit C leaves through shared memory + TMA stores (BLOCK_N = 256 kernels; tmap_c is valid)
     const int32_t* m_dev; // optional: the number of valid rows lives in device memory (<= M): only ceil(*m_dev / tile) row blocks
                           // are computed (compacted activations under a CUDA graph: the launch shape stays static)
 };
@@ -124,155 +112,76 @@ __device__ __forceinline__ float gelu_new(float x) {
     return x * r;
 }
 
-// smem descriptor of an MN-major operand tile: 64-element (128-byte) MN blocks, each [BLOCK_K rows][128 B] with the 128B
-// swizzle exactly as a TMA box {64, BLOCK_K} writes it, consecutive MN blocks `lbo_bytes` apart (LBO), 8-row K groups
-// 1024 bytes apart (SBO); one UMMA_K = 16 step advances the start address by 16 rows = 2048 bytes.
-__device__ __forceinline__ uint64_t umma_desc_mn_sw128(uint32_t smem_addr, uint32_t lbo_bytes) {
-    uint64_t d = 0;
-    d |= static_cast<uint64_t>((smem_addr & 0x3FFFFu) >> 4);
-    d |= static_cast<uint64_t>(lbo_bytes >> 4) << 16;
-    d |= static_cast<uint64_t>(1024 >> 4) << 32;
-    d |= static_cast<uint64_t>(1) << 46;
-    d |= static_cast<uint64_t>(2) << 61;
-    return d;
-}
-
 // kTN = false: C = A[M, K] . W[N, K]^T, both operands K-major (activations x nn.Linear weight).
 // kTN = true : C[M, N] = A[K, M]^T . W[K, N]: both operands MN-major, i.e. the contraction runs over the ROWS of two
 //              row-major matrices - the weight gradient dW[N_out, K_in] = dY[tokens, N_out]^T . X[tokens, K_in] without
 //              transposing either activation matrix (rows past K are zero-filled by TMA: no padding needed).
-// kQuad (with kPair, K-major operands): a cluster of FOUR CTAs = two CTA pairs working on M-adjacent 256 x 256 tiles of the
-//              same column block.  Both pairs need the same W tile, so every CTA fetches only 64 of the 128 W rows its
-//              pair-half consumes and TMA-multicasts them to the CTA with the same rank in the other pair: per 64-wide K
-//              block a CTA pulls 16 KB of A + 8 KB of W from L2 instead of 16 + 16.  The pair kernel is bound by L2 -> SM
-//              throughput (~6.3 KB/clk chip-wide: 148 CTAs x 32 KB per 512-clk K block is already 1.1x that), not by the
-//              tensor pipe (profiles/r02_gemm.md).  Ring stages are shared by the two pairs: a stage is free when BOTH
-//              pairs' MMAs have consumed it (empty barrier counts 2, commits multicast to all four CTAs).
-template <bool kBF16, int BLOCK_N, bool kPair, bool kTN, bool kQuad>
+//              wgmma reads 16-bit MN-major tiles through its transpose flags: boxes of {64 MN elements, 64 K rows}, MN
+//              blocks 8 KB apart (descriptor LBO).
+template <bool kBF16, int BLOCK_N, bool kTN>
 __global__ void __launch_bounds__(THREADS, 1)
-gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
-            const __grid_constant__ CUtensorMap tmap_c, const Params p) {
-    using C = Cfg<BLOCK_N, kPair>;
+gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b, const Params p) {
+    using C = Cfg<BLOCK_N>;
     extern __shared__ uint8_t smem_raw[];
     __shared__ __align__(8) uint64_t full_bar[C::STAGES];
     __shared__ __align__(8) uint64_t empty_bar[C::STAGES];
-    __shared__ __align__(8) uint64_t tmem_full_bar[2];
-    __shared__ __align__(8) uint64_t tmem_empty_bar[2];
-    __shared__ uint32_t tmem_base_smem;
 
     const uint32_t warp = threadIdx.x >> 5;
     const uint32_t lane = threadIdx.x & 31u;
     const uint32_t smem_base = (ab::smem_u32(smem_raw) + 1023u) & ~1023u;
     uint8_t* smem_gen = smem_raw + (smem_base - ab::smem_u32(smem_raw));
 
-    static_assert(!kQuad || (kPair && !kTN), "the 4-CTA cluster builds on the K-major pair kernel");
-    constexpr int CLUSTER = kQuad ? 4 : (kPair ? 2 : 1);
-    const uint32_t cluster_rank = kPair ? ab::cluster_ctarank() : 0u;
-    const uint32_t cta_rank = cluster_rank & 1u;                   // rank inside the CTA pair
-    const uint32_t pair_id = kQuad ? (cluster_rank >> 1) : 0u;     // which pair of the cluster
-    const bool leader = cta_rank == 0;
-    const int group = static_cast<int>(blockIdx.x) / CLUSTER;
-    const int num_groups = static_cast<int>(gridDim.x) / CLUSTER;
-    constexpr int PAIR_M = BLOCK_M * C::CTAS;                      // rows of one (pair) tile
-    constexpr int TILE_M = PAIR_M * (kQuad ? 2 : 1);               // rows one scheduling group covers per work item
-    const int m_rows = p.m_dev != nullptr ? min(p.M, max(__ldg(p.m_dev), 0)) : p.M;     // identical in every role and CTA
-    const int num_m = (m_rows + TILE_M - 1) / TILE_M;
+    const int m_rows = p.m_dev != nullptr ? min(p.M, max(__ldg(p.m_dev), 0)) : p.M;     // identical in every role
+    const int num_m = (m_rows + BLOCK_M - 1) / BLOCK_M;
     const int num_n = (p.N + BLOCK_N - 1) / BLOCK_N;
     const int num_tiles = num_m * num_n * p.splits;     // work items: (tile, split), split fastest
     const int num_kb = (p.K + BLOCK_K - 1) / BLOCK_K;
 
-    if (warp == 0 && lane == 0) {
+    if (threadIdx.x == 0) {
         ab::tma_prefetch_desc(&tmap_a);
         ab::tma_prefetch_desc(&tmap_b);
-    }
-    if (warp == 1 && lane == 0) {
         for (int s = 0; s < C::STAGES; ++s) {
             ab::mbar_init(&full_bar[s], 1);
-            ab::mbar_init(&empty_bar[s], kQuad ? 2 : 1);          // one commit per pair that reads the stage
-        }
-        for (int b = 0; b < 2; ++b) {
-            ab::mbar_init(&tmem_full_bar[b], 1);
-            ab::mbar_init(&tmem_empty_bar[b], EPI_WARPS * C::CTAS);
+            ab::mbar_init(&empty_bar[s], CONSUMERS);          // one arrive per consumer warpgroup
         }
         ab::fence_barrier_init();
     }
-    if (warp == 2) ab::tmem_alloc<C::CTAS>(&tmem_base_smem, C::TMEM_COLS);
-    ab::tc_fence_before();
-    if constexpr (kPair) {
-        ab::cluster_sync_all();
-    } else {
-        __syncthreads();
-    }
-    ab::tc_fence_after();
-    const uint32_t tmem_base = tmem_base_smem;
+    __syncthreads();
 
-    if (warp == 0) {
-        if (lane == 0) {
+    if (warp < 4) {
+        // ===================== producer warpgroup (one thread issues the TMA loads) =====================
+        ab::setmaxnreg_dec<40>();
+        if (warp == 0 && lane == 0) {
             uint32_t stage = 0, phase = 0;
-            for (int t = group; t < num_tiles; t += num_groups) {
+            for (int t = blockIdx.x; t < num_tiles; t += gridDim.x) {
                 const int tile = t / p.splits, split = t % p.splits;
                 const int m_blk = tile / num_n, n_blk = tile % num_n;
-                const int a_row = m_blk * TILE_M + static_cast<int>(pair_id) * PAIR_M + static_cast<int>(cta_rank) * BLOCK_M;
-                const int b_row = n_blk * BLOCK_N + static_cast<int>(cta_rank) * C::B_ROWS;
+                const int a_row = m_blk * BLOCK_M;
+                const int b_row = n_blk * BLOCK_N;
                 const int kb0 = split * p.kb_per_split, kb1 = min(num_kb, kb0 + p.kb_per_split);
-                // L2 prefetch of the A rows of this group's NEXT work item (K-major activations stream from HBM once per
-                // 256-row block; the ring covers ~6 x 512 clk of latency, an HBM miss costs more).  The groups that work on
-                // the column blocks of one row block run side by side: only the one whose next item has n_blk == 0 prefetches.
+                // L2 prefetch of the A rows of this CTA's NEXT work item when it starts a new row block
                 int pf_row = -1;
                 if constexpr (!kTN) {
-                    const int t2 = t + num_groups;
-                    if (p.l2_prefetch && t2 < num_tiles && (t2 / p.splits) % num_n == 0)
-                        pf_row = ((t2 / p.splits) / num_n) * TILE_M + static_cast<int>(pair_id) * PAIR_M +
-                                 static_cast<int>(cta_rank) * BLOCK_M;
+                    const int t2 = t + static_cast<int>(gridDim.x);
+                    if (p.l2_prefetch && t2 < num_tiles && (t2 / p.splits) % num_n == 0) pf_row = ((t2 / p.splits) / num_n) * BLOCK_M;
                 }
                 for (int kb = kb0; kb < kb1; ++kb) {
                     if (pf_row >= 0) ab::tma_prefetch_2d(&tmap_a, kb * BLOCK_K, pf_row);
-                    ab::mbar_wait(&empty_bar[stage], phase ^ 1u, 11);
+                    ab::mbar_wait_nocall(&empty_bar[stage], phase ^ 1u);
                     uint8_t* st = smem_gen + stage * C::STAGE_BYTES;
+                    ab::mbar_arrive_expect_tx(&full_bar[stage], C::STAGE_BYTES);
                     if constexpr (kTN) {
-                        // boxes of {64 columns (one swizzle atom along MN), 64 contraction rows}
-                        if constexpr (kPair) {
-                            if (leader) ab::mbar_arrive_expect_tx(&full_bar[stage], 2 * C::STAGE_BYTES);
-                        } else {
-                            ab::mbar_arrive_expect_tx(&full_bar[stage], C::STAGE_BYTES);
-                        }
 #pragma unroll
-                        for (int j = 0; j < BLOCK_M / 64; ++j) {
-                            if constexpr (kPair)
-                                ab::tma_load_2d_2sm(&tmap_a, &full_bar[stage], st + j * 8192, a_row + 64 * j, kb * BLOCK_K,
-                                                    ab::kEvictNormal);
-                            else
-                                ab::tma_load_2d(&tmap_a, &full_bar[stage], st + j * 8192, a_row + 64 * j, kb * BLOCK_K,
-                                                ab::kEvictNormal);
-                        }
+                        for (int j = 0; j < BLOCK_M / 64; ++j)
+                            ab::tma_load_2d(&tmap_a, &full_bar[stage], st + j * 8192, a_row + 64 * j, kb * BLOCK_K,
+                                            ab::kEvictNormal);
 #pragma unroll
-                        for (int j = 0; j < C::B_ROWS / 64; ++j) {
-                            if constexpr (kPair)
-                                ab::tma_load_2d_2sm(&tmap_b, &full_bar[stage], st + C::A_BYTES + j * 8192, b_row + 64 * j,
-                                                    kb * BLOCK_K, ab::kEvictNormal);
-                            else
-                                ab::tma_load_2d(&tmap_b, &full_bar[stage], st + C::A_BYTES + j * 8192, b_row + 64 * j,
-                                                kb * BLOCK_K, ab::kEvictNormal);
-                        }
-                    } else if constexpr (kQuad) {
-                        // 2 x (A 16 KB + W 2 x 8 KB) land in this pair's shared memory per stage, whoever issued them
-                        if (leader) ab::mbar_arrive_expect_tx(&full_bar[stage], 2 * C::STAGE_BYTES);
-                        ab::tma_load_2d_2sm(&tmap_a, &full_bar[stage], st, kb * BLOCK_K, a_row, ab::kEvictNormal);
-                        // W box = 64 rows: this CTA's quarter of the pair-half, multicast to the same rank of both pairs
-                        ab::tma_load_2d_2sm_mc(&tmap_b, &full_bar[stage], st + C::A_BYTES + pair_id * (64 * BLOCK_K * 2),
-                                               kb * BLOCK_K, b_row + static_cast<int>(pair_id) * 64,
-                                               static_cast<uint16_t>(0x5u << cta_rank), ab::kEvictLast);
-                    } else if constexpr (kPair) {
-                        // the leader's barrier collects the bytes of BOTH CTAs' boxes
-                        if (leader) ab::mbar_arrive_expect_tx(&full_bar[stage], 2 * C::STAGE_BYTES);
-                        ab::tma_load_2d_2sm(&tmap_a, &full_bar[stage], st, kb * BLOCK_K, a_row, ab::kEvictNormal);
-                        ab::tma_load_2d_2sm(&tmap_b, &full_bar[stage], st + C::A_BYTES, kb * BLOCK_K, b_row,
-                                            ab::kEvictLast);
+                        for (int j = 0; j < BLOCK_N / 64; ++j)
+                            ab::tma_load_2d(&tmap_b, &full_bar[stage], st + C::A_BYTES + j * 8192, b_row + 64 * j,
+                                            kb * BLOCK_K, ab::kEvictNormal);
                     } else {
-                        ab::mbar_arrive_expect_tx(&full_bar[stage], C::STAGE_BYTES);
                         ab::tma_load_2d(&tmap_a, &full_bar[stage], st, kb * BLOCK_K, a_row, ab::kEvictNormal);
-                        ab::tma_load_2d(&tmap_b, &full_bar[stage], st + C::A_BYTES, kb * BLOCK_K, b_row,
-                                        ab::kEvictLast);
+                        ab::tma_load_2d(&tmap_b, &full_bar[stage], st + C::A_BYTES, kb * BLOCK_K, b_row, ab::kEvictLast);
                     }
                     if (++stage == C::STAGES) {
                         stage = 0;
@@ -281,394 +190,130 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ 
                 }
             }
         }
-    } else if (warp == 1) {
-        // MMA issuer (leader CTA of a pair only)
-        if (lane == 0 && leader) {
-            // bits 15 / 16: A / B operand is MN-major
-            constexpr uint32_t idesc = ab::umma_idesc_f16(C::UMMA_M, BLOCK_N, kBF16) | (kTN ? ((1u << 15) | (1u << 16)) : 0u);
-            uint32_t stage = 0, phase = 0;
-            int it = 0;
-            for (int t = group; t < num_tiles; t += num_groups, ++it) {
-                const uint32_t buf = it & 1;
-                ab::mbar_wait(&tmem_empty_bar[buf], ((it >> 1) & 1) ^ 1u, 12);
-                ab::tc_fence_after();
-                const uint32_t d_tmem = tmem_base + buf * BLOCK_N;
-                const int kb0 = (t % p.splits) * p.kb_per_split, kb1 = min(num_kb, kb0 + p.kb_per_split);
-                for (int kb = kb0; kb < kb1; ++kb) {
-                    ab::mbar_wait(&full_bar[stage], phase, 13);
-                    ab::tc_fence_after();
-                    if constexpr (kTN) {
-                        const uint64_t adesc0 = umma_desc_mn_sw128(smem_base + stage * C::STAGE_BYTES, 8192);
-                        const uint64_t bdesc0 = umma_desc_mn_sw128(smem_base + stage * C::STAGE_BYTES + C::A_BYTES, 8192);
+        return;
+    }
+
+    // ===================== consumer warpgroups: 64 rows x BLOCK_N columns each =====================
+    ab::setmaxnreg_inc<232>();
+    const uint32_t wg = (warp >> 2) - 1u;              // 0 / 1: rows [64 wg, 64 wg + 64) of the tile
+    const uint32_t wl = warp & 3u;                     // warp inside the warpgroup
+    constexpr int NACC = BLOCK_N / 2;
+    uint32_t stage = 0, phase = 0;
+    for (int t = blockIdx.x; t < num_tiles; t += gridDim.x) {
+        const int tile = t / p.splits, split = t % p.splits;
+        const int m_blk = tile / num_n, n_blk = tile % num_n;
+        const int kb0 = split * p.kb_per_split, kb1 = min(num_kb, kb0 + p.kb_per_split);
+        float acc[NACC];
 #pragma unroll
-                        for (int k = 0; k < BLOCK_K / UMMA_K; ++k) {
-                            ab::umma_ss<C::CTAS>(d_tmem, adesc0 + ((k * UMMA_K * 128) >> 4),
-                                                 bdesc0 + ((k * UMMA_K * 128) >> 4), idesc, ((kb - kb0) | k) != 0 ? 1u : 0u);
-                        }
-                    } else {
-                        const uint64_t adesc0 = ab::umma_desc_k_sw128(smem_base + stage * C::STAGE_BYTES);
-                        const uint64_t bdesc0 = ab::umma_desc_k_sw128(smem_base + stage * C::STAGE_BYTES + C::A_BYTES);
+        for (int i = 0; i < NACC; ++i) acc[i] = 0.f;
+        int prev_stage = -1;
+        for (int kb = kb0; kb < kb1; ++kb) {
+            ab::mbar_wait_nocall(&full_bar[stage], phase);
+            const uint32_t st = smem_base + stage * C::STAGE_BYTES;
+            ab::wgmma_fence();
 #pragma unroll
-                        for (int k = 0; k < BLOCK_K / UMMA_K; ++k) {
-                            ab::umma_ss<C::CTAS>(d_tmem, adesc0 + ((k * UMMA_K * 2) >> 4),
-                                                 bdesc0 + ((k * UMMA_K * 2) >> 4), idesc, ((kb - kb0) | k) != 0 ? 1u : 0u);
-                        }
-                    }
-                    if constexpr (kQuad) {
-                        ab::umma_commit_2sm(&empty_bar[stage], 0xF);        // the stage is shared with the other pair
-                    } else if constexpr (kPair) {
-                        ab::umma_commit_2sm(&empty_bar[stage], 0x3);
-                    } else {
-                        ab::umma_commit(&empty_bar[stage]);
-                    }
-                    if (++stage == C::STAGES) {
-                        stage = 0;
-                        phase ^= 1u;
-                    }
-                }
-                if constexpr (kPair) {
-                    ab::umma_commit_2sm(&tmem_full_bar[buf], static_cast<uint16_t>(0x3u << (2 * pair_id)));
+            for (int k = 0; k < BLOCK_K / UMMA_K; ++k) {
+                uint64_t adesc, bdesc;
+                if constexpr (kTN) {
+                    adesc = ab::wgmma_desc_sw128(st + wg * 8192u + k * 2048u, 8192);
+                    bdesc = ab::wgmma_desc_sw128(st + C::A_BYTES + k * 2048u, 8192);
                 } else {
-                    ab::umma_commit(&tmem_full_bar[buf]);
+                    adesc = ab::wgmma_desc_sw128(st + wg * 8192u + k * 32u);
+                    bdesc = ab::wgmma_desc_sw128(st + C::A_BYTES + k * 32u);
                 }
+                if constexpr (BLOCK_N == 256)
+                    ab::wgmma_m64n256k16_ss<kBF16, kTN ? 1 : 0, kTN ? 1 : 0>(acc, adesc, bdesc, 1);
+                else
+                    ab::wgmma_m64n128k16_ss<kBF16, kTN ? 1 : 0, kTN ? 1 : 0>(acc, adesc, bdesc, 1);
+            }
+            ab::wgmma_commit();
+            // the previous stage's MMAs have retired once at most this stage's group is pending: release it
+            ab::wgmma_wait<1>();
+            ab::wgmma_reg_fence(acc);
+            if (prev_stage >= 0 && wl == 0 && lane == 0) ab::mbar_arrive(&empty_bar[prev_stage]);
+            prev_stage = static_cast<int>(stage);
+            if (++stage == C::STAGES) {
+                stage = 0;
+                phase ^= 1u;
             }
         }
-    } else if (warp >= 4) {
-        // ===================== epilogue =====================
-        const uint32_t lg = warp & 3u;
-        const uint32_t half = (warp - 4u) >> 2;  // which half of the BLOCK_N columns
-        constexpr int CHUNKS = BLOCK_N / 64;     // 32-column chunks per warp
-        int it = 0;
-        for (int t = group; t < num_tiles; t += num_groups, ++it) {
-            const uint32_t buf = it & 1;
-            const int tile = t / p.splits, split = t % p.splits;
-            const int m_blk = tile / num_n, n_blk = tile % num_n;
-            const int row = m_blk * TILE_M + static_cast<int>(pair_id) * PAIR_M + static_cast<int>(cta_rank) * BLOCK_M +
-                            static_cast<int>(lg * 32 + lane);
-            // fused RMSNorm of the A rows: a per-row scale of the accumulator (loaded while the MMAs run)
-            const float rscale = (p.row_ss != nullptr && row < p.M)
+        ab::wgmma_wait<0>();
+        ab::wgmma_reg_fence(acc);
+        if (prev_stage >= 0 && wl == 0 && lane == 0) ab::mbar_arrive(&empty_bar[prev_stage]);
+
+        // ---- epilogue straight from the accumulator registers: rows r0 and r0 + 8, column pairs 8 j + 2 (lane % 4)
+        const int r0 = m_blk * BLOCK_M + static_cast<int>(wg * 64u + wl * 16u + (lane >> 2));
+        const int cq = static_cast<int>(2u * (lane & 3u));
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+            const int row = r0 + 8 * h;
+            const bool row_ok = row < p.M;
+            const float rscale = (p.row_ss != nullptr && row_ok)
                                      ? rsqrtf(__ldg(p.row_ss + row) / static_cast<float>(p.K) + p.rs_eps) : 1.0f;
             float ss_out = 0.f;
-            if constexpr (BLOCK_N == 256) {
-                if (p.tma_store && p.C32 == nullptr) {
-                    // ---- staged epilogue: accumulator rows -> 16-bit -> this warp's swizzled shared tile -> ONE TMA store per
-                    // 64 output columns (full 128-byte lines) instead of 32-row-strided 16-byte stores per thread; the residual
-                    // rows arrive through coalesced 128-byte loads and the same tile (a transpose scratch).
-                    uint8_t* stg = smem_gen + C::STAGES * C::STAGE_BYTES + (warp - 4u) * 4096u;
-                    const uint32_t swz = lane & 7u;
-                    const bool gated = p.epi == EPI_GATED;
-                    const int n_groups = gated ? 1 : 2;                       // groups of 64 OUTPUT columns of this warp
-                    const int row_warp = m_blk * TILE_M + static_cast<int>(pair_id) * PAIR_M + static_cast<int>(cta_rank) * BLOCK_M +
-                                         static_cast<int>(lg * 32);
-                    const int acc_col_w = static_cast<int>(half) * (BLOCK_N / 2);   // first accumulator column of this warp
-                    const int out_col_w = gated ? n_blk * (BLOCK_N / 2) + static_cast<int>(half) * (BLOCK_N / 4)
-                                                : n_blk * BLOCK_N + acc_col_w;
-                    const bool use_res = p.epi == EPI_RESIDUAL;
-                    uint4 rq[8];                                             // residual pieces in flight (coalesced layout)
-                    auto load_res = [&](int g) {
+            if (row_ok) {
 #pragma unroll
-                        for (int i = 0; i < 8; ++i) {
-                            const int rr = row_warp + static_cast<int>(lane >> 3) + 4 * i;
-                            const int cc = out_col_w + g * 64 + static_cast<int>(lane & 7u) * 8;
-                            rq[i] = (rr < p.M && cc < p.N)
-                                        ? __ldg(reinterpret_cast<const uint4*>(p.residual + static_cast<size_t>(rr) * p.ldr + cc))
-                                        : make_uint4(0u, 0u, 0u, 0u);
-                        }
-                    };
-                    if (use_res) load_res(0);                                 // in flight while the MMAs of this tile finish
-                    ab::mbar_wait(&tmem_full_bar[buf], (it >> 1) & 1, 14);
-                    ab::tc_fence_after();
-#pragma unroll 1
-                    for (int g = 0; g < n_groups; ++g) {
-                        if (lane == 0) ab::tma_store_wait_read();              // the previous store has read the tile
-                        __syncwarp();
-                        uint4 rown[8];                                        // this thread's residual row, 64 columns
-                        if (use_res) {
-#pragma unroll
-                            for (int i = 0; i < 8; ++i) {
-                                const uint32_t rr = (lane >> 3) + 4u * i;
-                                *reinterpret_cast<uint4*>(stg + rr * 128u + (((lane & 7u) ^ (rr & 7u)) << 4)) = rq[i];
-                            }
-                            __syncwarp();
-#pragma unroll
-                            for (int k = 0; k < 8; ++k)
-                                rown[k] = *reinterpret_cast<const uint4*>(stg + lane * 128u + ((static_cast<uint32_t>(k) ^ swz) << 4));
-                            if (g + 1 < n_groups) load_res(g + 1);
-                        }
-                        const int chunks_in_group = gated ? 4 : 2;
-#pragma unroll 1
-                        for (int cg = 0; cg < chunks_in_group; ++cg) {
-                            const int c = gated ? cg : g * 2 + cg;            // 32-column accumulator chunk of this warp
-                            const int col_local = acc_col_w + c * 32;
-                            const int col0 = n_blk * BLOCK_N + col_local;
-                            uint32_t r[32];
-                            ab::tmem_ld32(tmem_base + ((lg * 32u) << 16) + buf * BLOCK_N + col_local, r);
-                            ab::tmem_ld_wait();
-                            if (c == CHUNKS - 1) {
-                                ab::tc_fence_before();
-                                __syncwarp();
-                                if (lane == 0) {
-                                    if (leader) ab::mbar_arrive(&tmem_empty_bar[buf]);
-                                    else ab::mbar_arrive_cluster(&tmem_empty_bar[buf], 2 * pair_id);
-                                }
-                            }
-                            float v[32];
-#pragma unroll
-                            for (int j = 0; j < 32; ++j) v[j] = __uint_as_float(r[j]) * rscale;
-                            if (p.epi != EPI_NONE && !gated && p.bias != nullptr) {
-#pragma unroll
-                                for (int j8 = 0; j8 < 4; ++j8) {
-                                    if (col0 + j8 * 8 < p.N) {
-                                        const uint4 b = __ldg(reinterpret_cast<const uint4*>(p.bias + col0 + j8 * 8));
-                                        const uint32_t w[4] = {b.x, b.y, b.z, b.w};
-#pragma unroll
-                                        for (int e = 0; e < 4; ++e) {
-                                            v[j8 * 8 + 2 * e] += to_f32<kBF16>(static_cast<uint16_t>(w[e] & 0xFFFFu));
-                                            v[j8 * 8 + 2 * e + 1] += to_f32<kBF16>(static_cast<uint16_t>(w[e] >> 16));
-                                        }
-                                    }
-                                }
-                            }
-                            if (p.epi == EPI_GELU) {
-#pragma unroll
-                                for (int j = 0; j < 32; ++j) v[j] = gelu_erf(v[j]);
-                            } else if (use_res) {
-#pragma unroll
-                                for (int j8 = 0; j8 < 4; ++j8) {
-                                    const uint4 b = cg ? rown[4 + j8] : rown[j8];     // static register indices
-                                    const uint32_t w[4] = {b.x, b.y, b.z, b.w};
-#pragma unroll
-                                    for (int e = 0; e < 4; ++e) {
-                                        v[j8 * 8 + 2 * e] += to_f32<kBF16>(static_cast<uint16_t>(w[e] & 0xFFFFu));
-                                        v[j8 * 8 + 2 * e + 1] += to_f32<kBF16>(static_cast<uint16_t>(w[e] >> 16));
-                                    }
-                                }
-                            }
-                            if (gated) {
-                                uint32_t o[8];
-#pragma unroll
-                                for (int e = 0; e < 8; ++e)
-                                    o[e] = pack2<kBF16>(gelu_new(v[4 * e]) * v[4 * e + 1], gelu_new(v[4 * e + 2]) * v[4 * e + 3]);
-#pragma unroll
-                                for (int k = 0; k < 2; ++k)
-                                    *reinterpret_cast<uint4*>(stg + lane * 128u + ((static_cast<uint32_t>(cg * 2 + k) ^ swz) << 4)) =
-                                        make_uint4(o[4 * k], o[4 * k + 1], o[4 * k + 2], o[4 * k + 3]);
-                            } else {
-#pragma unroll
-                                for (int j8 = 0; j8 < 4; ++j8) {
-                                    const uint4 o = make_uint4(
-                                        pack2<kBF16>(v[j8 * 8 + 0], v[j8 * 8 + 1]), pack2<kBF16>(v[j8 * 8 + 2], v[j8 * 8 + 3]),
-                                        pack2<kBF16>(v[j8 * 8 + 4], v[j8 * 8 + 5]), pack2<kBF16>(v[j8 * 8 + 6], v[j8 * 8 + 7]));
-                                    *reinterpret_cast<uint4*>(stg + lane * 128u + ((static_cast<uint32_t>(cg * 4 + j8) ^ swz) << 4)) = o;
-                                    if (p.out_ss != nullptr && col0 + j8 * 8 < p.N) {   // squares of the values as STORED
-                                        const uint32_t w[4] = {o.x, o.y, o.z, o.w};
-#pragma unroll
-                                        for (int e = 0; e < 4; ++e) {
-                                            const float a = to_f32<kBF16>(static_cast<uint16_t>(w[e] & 0xFFFFu));
-                                            const float b = to_f32<kBF16>(static_cast<uint16_t>(w[e] >> 16));
-                                            ss_out = fmaf(a, a, fmaf(b, b, ss_out));
-                                        }
-                                    }
-                                }
-                            }
-                        }
-                        ab::fence_proxy_async_smem();                          // generic-proxy writes -> visible to the TMA engine
-                        __syncwarp();
-                        if (lane == 0 && row_warp < p.M) {                     // rows / columns past M / N are clipped by the tensor map
-                            ab::tma_store_2d(&tmap_c, stg, out_col_w + g * 64, row_warp);
-                            ab::tma_store_commit();
-                        }
+                for (int j = 0; j < BLOCK_N / 8; ++j) {
+                    const int col = n_blk * BLOCK_N + 8 * j + cq;
+                    if (col >= p.N) continue;
+                    float v0 = acc[4 * j + 2 * h], v1 = acc[4 * j + 2 * h + 1];
+                    if (p.C32 != nullptr) {   // split-K partial: raw fp32 accumulator
+                        *reinterpret_cast<float2*>(p.C32 + (static_cast<size_t>(split) * p.M + row) * p.N + col) = make_float2(v0, v1);
+                        continue;
                     }
-                    if (p.out_ss != nullptr && row < p.M) atomicAdd(p.out_ss + row, ss_out);
-                    continue;
-                }
-            }
-            ab::mbar_wait(&tmem_full_bar[buf], (it >> 1) & 1, 14);
-            ab::tc_fence_after();
-#pragma unroll 1
-            for (int c = 0; c < CHUNKS; ++c) {
-                const int col_local = static_cast<int>(half) * (BLOCK_N / 2) + c * 32;
-                const int col0 = n_blk * BLOCK_N + col_local;
-                uint32_t r[32];
-                ab::tmem_ld32(tmem_base + ((lg * 32u) << 16) + buf * BLOCK_N + col_local, r);
-                ab::tmem_ld_wait();
-                if (c == CHUNKS - 1) {
-                    // all accumulator columns of this warp are in registers: release the buffer
-                    ab::tc_fence_before();
-                    __syncwarp();
-                    if (lane == 0) {
-                        if (leader) ab::mbar_arrive(&tmem_empty_bar[buf]);
-                        else ab::mbar_arrive_cluster(&tmem_empty_bar[buf], 2 * pair_id);   // the pair's leader issues the next MMAs
+                    v0 *= rscale;
+                    v1 *= rscale;
+                    if (p.epi == EPI_GATED) {
+                        // columns (2c, 2c+1) = (x.wi_0[c], x.wi_1[c]) -> one output
+                        const uint32_t o = pack2<kBF16>(gelu_new(v0) * v1, 0.f);
+                        p.C[static_cast<size_t>(row) * p.ldc + (col >> 1)] = static_cast<uint16_t>(o & 0xFFFFu);
+                        continue;
                     }
-                }
-                if (row >= p.M || col0 >= p.N) continue;
-                if (p.C32 != nullptr) {   // split-K partial: raw fp32 accumulator
-                    float* crow = p.C32 + (static_cast<size_t>(split) * p.M + row) * p.N + col0;
-#pragma unroll
-                    for (int j4 = 0; j4 < 8; ++j4)
-                        if (col0 + j4 * 4 < p.N)
-                            *reinterpret_cast<uint4*>(crow + j4 * 4) = make_uint4(r[4 * j4], r[4 * j4 + 1], r[4 * j4 + 2], r[4 * j4 + 3]);
-                    continue;
-                }
-                float v[32];
-#pragma unroll
-                for (int j = 0; j < 32; ++j) v[j] = __uint_as_float(r[j]) * rscale;
-                if (p.epi != EPI_NONE && p.epi != EPI_GATED && p.bias != nullptr) {
-#pragma unroll
-                    for (int j8 = 0; j8 < 4; ++j8) {
-                        if (col0 + j8 * 8 < p.N) {
-                            const uint4 b = __ldg(reinterpret_cast<const uint4*>(p.bias + col0 + j8 * 8));
-                            const uint32_t w[4] = {b.x, b.y, b.z, b.w};
-#pragma unroll
-                            for (int e = 0; e < 4; ++e) {
-                                v[j8 * 8 + 2 * e] += to_f32<kBF16>(static_cast<uint16_t>(w[e] & 0xFFFFu));
-                                v[j8 * 8 + 2 * e + 1] += to_f32<kBF16>(static_cast<uint16_t>(w[e] >> 16));
-                            }
-                        }
+                    if (p.epi != EPI_NONE && p.bias != nullptr) {
+                        const uint32_t b = __ldg(reinterpret_cast<const uint32_t*>(p.bias + col));
+                        v0 += to_f32<kBF16>(static_cast<uint16_t>(b & 0xFFFFu));
+                        v1 += to_f32<kBF16>(static_cast<uint16_t>(b >> 16));
                     }
-                }
-                if (p.epi == EPI_GELU) {
-#pragma unroll
-                    for (int j = 0; j < 32; ++j) v[j] = gelu_erf(v[j]);
-                } else if (p.epi == EPI_RESIDUAL) {
-                    const uint16_t* rrow = p.residual + static_cast<size_t>(row) * p.ldr + col0;
-#pragma unroll
-                    for (int j8 = 0; j8 < 4; ++j8) {
-                        if (col0 + j8 * 8 < p.N) {
-                            const uint4 b = __ldg(reinterpret_cast<const uint4*>(rrow + j8 * 8));
-                            const uint32_t w[4] = {b.x, b.y, b.z, b.w};
-#pragma unroll
-                            for (int e = 0; e < 4; ++e) {
-                                v[j8 * 8 + 2 * e] += to_f32<kBF16>(static_cast<uint16_t>(w[e] & 0xFFFFu));
-                                v[j8 * 8 + 2 * e + 1] += to_f32<kBF16>(static_cast<uint16_t>(w[e] >> 16));
-                            }
-                        }
+                    if (p.epi == EPI_GELU) {
+                        v0 = gelu_erf(v0);
+                        v1 = gelu_erf(v1);
+                    } else if (p.epi == EPI_RESIDUAL) {
+                        const uint32_t r = __ldg(reinterpret_cast<const uint32_t*>(p.residual + static_cast<size_t>(row) * p.ldr + col));
+                        v0 += to_f32<kBF16>(static_cast<uint16_t>(r & 0xFFFFu));
+                        v1 += to_f32<kBF16>(static_cast<uint16_t>(r >> 16));
                     }
-                }
-                if (p.epi == EPI_GATED) {
-                    // columns (2j, 2j+1) = (x.wi_0[j], x.wi_1[j]) -> 16 outputs
-                    uint16_t* crow = p.C + static_cast<size_t>(row) * p.ldc + (col0 >> 1);
-                    uint32_t o[8];
-#pragma unroll
-                    for (int e = 0; e < 8; ++e)
-                        o[e] = pack2<kBF16>(gelu_new(v[4 * e]) * v[4 * e + 1], gelu_new(v[4 * e + 2]) * v[4 * e + 3]);
-#pragma unroll
-                    for (int j8 = 0; j8 < 2; ++j8)
-                        if (col0 + j8 * 16 < p.N)
-                            *reinterpret_cast<uint4*>(crow + j8 * 8) =
-                                make_uint4(o[4 * j8], o[4 * j8 + 1], o[4 * j8 + 2], o[4 * j8 + 3]);
-                } else {
-                    uint16_t* crow = p.C + static_cast<size_t>(row) * p.ldc + col0;
-#pragma unroll
-                    for (int j8 = 0; j8 < 4; ++j8) {
-                        if (col0 + j8 * 8 < p.N) {
-                            const uint4 o = make_uint4(
-                                pack2<kBF16>(v[j8 * 8 + 0], v[j8 * 8 + 1]), pack2<kBF16>(v[j8 * 8 + 2], v[j8 * 8 + 3]),
-                                pack2<kBF16>(v[j8 * 8 + 4], v[j8 * 8 + 5]), pack2<kBF16>(v[j8 * 8 + 6], v[j8 * 8 + 7]));
-                            *reinterpret_cast<uint4*>(crow + j8 * 8) = o;
-                            if (p.out_ss != nullptr) {   // squares of the values as STORED (what a separate norm would read)
-                                const uint32_t w[4] = {o.x, o.y, o.z, o.w};
-#pragma unroll
-                                for (int e = 0; e < 4; ++e) {
-                                    const float a = to_f32<kBF16>(static_cast<uint16_t>(w[e] & 0xFFFFu));
-                                    const float b = to_f32<kBF16>(static_cast<uint16_t>(w[e] >> 16));
-                                    ss_out = fmaf(a, a, fmaf(b, b, ss_out));
-                                }
-                            }
-                        }
+                    const uint32_t o = pack2<kBF16>(v0, v1);
+                    *reinterpret_cast<uint32_t*>(p.C + static_cast<size_t>(row) * p.ldc + col) = o;
+                    if (p.out_ss != nullptr) {   // squares of the values as STORED (what a separate norm would read)
+                        const float a = to_f32<kBF16>(static_cast<uint16_t>(o & 0xFFFFu));
+                        const float b = to_f32<kBF16>(static_cast<uint16_t>(o >> 16));
+                        ss_out = fmaf(a, a, fmaf(b, b, ss_out));
                     }
                 }
             }
-            if (p.out_ss != nullptr && row < p.M) atomicAdd(p.out_ss + row, ss_out);
+            if (p.out_ss != nullptr) {
+                // the four threads of a quad hold the same row
+                ss_out += __shfl_xor_sync(0xffffffffu, ss_out, 1);
+                ss_out += __shfl_xor_sync(0xffffffffu, ss_out, 2);
+                if (row_ok && (lane & 3u) == 0u) atomicAdd(p.out_ss + row, ss_out);
+            }
         }
-        if constexpr (BLOCK_N == 256) {
-            if (lane == 0) ab::tma_store_wait_all();     // every TMA store of this warp has landed before the CTA exits
-        }
-    }
-
-    ab::tc_fence_before();
-    if constexpr (kPair) {
-        ab::cluster_sync_all();   // the peer's MMAs / multicast commits may still target this CTA's smem and barriers
-    } else {
-        __syncthreads();
-    }
-    if (warp == 2) {
-        ab::tc_fence_after();
-        ab::tmem_dealloc<C::CTAS>(tmem_base, C::TMEM_COLS);
     }
 }
 
-// number of 4-CTA clusters of the quad kernel that can be resident at once (GPC boundaries may leave SMs unused), 0 = unknown
-template <bool kBF16>
-static int quad_clusters() {
-    static int cached = -1;
-    if (cached >= 0) return cached;
-    using C = Cfg<256, true>;
-    auto kernel = gemm_kernel<kBF16, 256, true, false, true>;
-    cached = 0;
-    if (cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, C::SMEM_BYTES) != cudaSuccess) return cached;
-    cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = dim3(static_cast<unsigned>(abh::num_sms() / 4 * 4));
-    cfg.blockDim = dim3(THREADS);
-    cfg.dynamicSmemBytes = C::SMEM_BYTES;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeClusterDimension;
-    attr[0].val.clusterDim.x = 4;
-    attr[0].val.clusterDim.y = 1;
-    attr[0].val.clusterDim.z = 1;
-    cfg.attrs = attr;
-    cfg.numAttrs = 1;
-    int n = 0;
-    if (cudaOccupancyMaxActiveClusters(&n, kernel, &cfg) == cudaSuccess && n > 0) cached = n;
-    else (void)cudaGetLastError();
-    return cached;
-}
-
-template <bool kBF16, int BLOCK_N, bool kPair, bool kTN = false, bool kQuad = false>
-static int launch(const CUtensorMap& ta, const CUtensorMap& tb, const Params& p_in, cudaStream_t s) {
-    using C = Cfg<BLOCK_N, kPair>;
-    // C through shared memory + TMA stores (BLOCK_N = 256 kernels, 16-bit output): box = {64 columns, 32 rows}
-    Params p = p_in;
-    CUtensorMap tc = ta;      // placeholder when the staged epilogue is off
-    static const bool stage_off = getenv("ATLAS_B200_GEMM_TMA_STORE") != nullptr && getenv("ATLAS_B200_GEMM_TMA_STORE")[0] == '0';
-    p.tma_store = 0;
-    if (BLOCK_N == 256 && p.C32 == nullptr && !stage_off) {
-        const int n_out = p.epi == EPI_GATED ? p.N / 2 : p.N;
-        const int rc = abh::make_tmap_2d_16bit(&tc, p.C, static_cast<uint64_t>(p.M), static_cast<uint64_t>(n_out),
-                                               static_cast<uint64_t>(p.ldc), 32, 64, kBF16);
-        if (rc) return rc;
-        p.tma_store = 1;
-    }
+template <bool kBF16, int BLOCK_N, bool kTN = false>
+static int launch(const CUtensorMap& ta, const CUtensorMap& tb, const Params& p, cudaStream_t s) {
+    using C = Cfg<BLOCK_N>;
     static bool attr_set = false;
     if (!attr_set) {
-        AB_CUDA_CHECK(cudaFuncSetAttribute(gemm_kernel<kBF16, BLOCK_N, kPair, kTN, kQuad>,
-                                           cudaFuncAttributeMaxDynamicSharedMemorySize, C::SMEM_BYTES));
+        AB_CUDA_CHECK(cudaFuncSetAttribute(gemm_kernel<kBF16, BLOCK_N, kTN>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                           C::SMEM_BYTES));
         attr_set = true;
     }
-    constexpr int CLUSTER = kQuad ? 4 : C::CTAS;
-    const int tile_m = BLOCK_M * CLUSTER;
-    const int tiles = ((p.M + tile_m - 1) / tile_m) * ((p.N + BLOCK_N - 1) / BLOCK_N) * p.splits;
-    int groups_max = abh::num_sms() / CLUSTER;
-    if constexpr (kQuad) groups_max = quad_clusters<kBF16>();
-    const int grid = (tiles < groups_max ? tiles : groups_max) * CLUSTER;
+    const int tiles = ((p.M + BLOCK_M - 1) / BLOCK_M) * ((p.N + BLOCK_N - 1) / BLOCK_N) * p.splits;
+    const int grid = tiles < abh::num_sms() ? tiles : abh::num_sms();
     abh::prof_begin(s, abh::PROF_LINEAR);
-    if constexpr (kPair) {
-        cudaLaunchConfig_t cfg = {};
-        cfg.gridDim = dim3(static_cast<unsigned>(grid));
-        cfg.blockDim = dim3(THREADS);
-        cfg.dynamicSmemBytes = C::SMEM_BYTES;
-        cfg.stream = s;
-        cudaLaunchAttribute attr[1];
-        attr[0].id = cudaLaunchAttributeClusterDimension;
-        attr[0].val.clusterDim.x = CLUSTER;
-        attr[0].val.clusterDim.y = 1;
-        attr[0].val.clusterDim.z = 1;
-        cfg.attrs = attr;
-        cfg.numAttrs = 1;
-        AB_CUDA_CHECK(cudaLaunchKernelEx(&cfg, gemm_kernel<kBF16, BLOCK_N, kPair, kTN, kQuad>, ta, tb, tc, p));
-    } else {
-        gemm_kernel<kBF16, BLOCK_N, kPair, kTN, kQuad><<<grid, THREADS, C::SMEM_BYTES, s>>>(ta, tb, tc, p);
-    }
+    gemm_kernel<kBF16, BLOCK_N, kTN><<<grid, THREADS, C::SMEM_BYTES, s>>>(ta, tb, p);
     if (p.m_dev != nullptr) abh::prof_end_dyn(s, abh::PROF_LINEAR, 2.0 * static_cast<double>(p.N) * p.K, p.m_dev, p.M);
     else abh::prof_end(s, abh::PROF_LINEAR, 2.0 * p.M * static_cast<double>(p.N) * p.K);
     abh::count_launch();
@@ -769,48 +414,27 @@ int atlas_b200_linear_ex(const void* A, int64_t lda, const void* W, int64_t ldw,
     p.bias = static_cast<const uint16_t*>(bias);
     p.residual = static_cast<const uint16_t*>(residual);
     p.C = static_cast<uint16_t*>(C);
-    const bool wide = N >= 256 && (static_cast<int64_t>((M + 127) / 128) * ((N + 255) / 256) >= abh::num_sms() / 2);
-    // 256 x 256 pair tiles once there are enough of them to fill the 74 CTA pairs (encoder-sized M)
-    const bool pair = N >= 256 && M >= 256 &&
-                      (static_cast<int64_t>((M + 255) / 256) * ((N + 255) / 256) >= abh::num_sms() / 2);
-    // 4-CTA clusters (two pairs sharing the W tile through TMA multicast), opt-in with ATLAS_B200_GEMM_QUAD=1: measured
-    // 3 - 5 % SLOWER than the pair kernel on the FiD-base shapes (profiles/r02_gemm.md) - the mainloop is bound by the
-    // latency of the A stream, not by L2 -> SM throughput, and the two pairs of a cluster run in lockstep.
-    static const bool quad_off = getenv("ATLAS_B200_GEMM_QUAD") == nullptr || getenv("ATLAS_B200_GEMM_QUAD")[0] != '1';
-    static const bool no_pair = getenv("ATLAS_B200_GEMM_NO_PAIR") != nullptr;   // A/B measurements
-    const int qc = (pair && !quad_off && !no_pair && M >= 512) ? (is_bf16 ? quad_clusters<true>() : quad_clusters<false>()) : 0;
-    const bool quad = qc > 0 && (static_cast<int64_t>((M + 511) / 512) * ((N + 255) / 256) >= 2ll * qc);
-    const int block_n = (wide || pair) ? 256 : 128;
-    const int b_box_rows = quad ? 64 : (pair ? 128 : block_n);
+    // 128 x 256 tiles once there are enough of them to fill the SMs (encoder-sized M), else 128 x 128
+    const bool wide = N >= 256 && (static_cast<int64_t>((M + 127) / 128) * ((N + 255) / 256) >= abh::num_sms());
+    const int block_n = wide ? 256 : 128;
     CUtensorMap ta, tb;
     int rc = abh::make_tmap_2d_16bit(&ta, A, static_cast<uint64_t>(M), static_cast<uint64_t>(K),
                                      static_cast<uint64_t>(lda), BLOCK_M, BLOCK_K, is_bf16 != 0);
     if (rc) return rc;
     rc = abh::make_tmap_2d_16bit(&tb, W, static_cast<uint64_t>(N), static_cast<uint64_t>(K), static_cast<uint64_t>(ldw),
-                                 static_cast<uint32_t>(b_box_rows), BLOCK_K, is_bf16 != 0);
+                                 static_cast<uint32_t>(block_n), BLOCK_K, is_bf16 != 0);
     if (rc) return rc;
     cudaStream_t s = static_cast<cudaStream_t>(stream);
-    if (quad)
-        return is_bf16 ? launch<true, 256, true, false, true>(ta, tb, p, s) : launch<false, 256, true, false, true>(ta, tb, p, s);
-    if (pair && !no_pair) return is_bf16 ? launch<true, 256, true>(ta, tb, p, s) : launch<false, 256, true>(ta, tb, p, s);
-    if (pair && no_pair) {   // the 1-CTA kernel needs the full-height W box
-        rc = abh::make_tmap_2d_16bit(&tb, W, static_cast<uint64_t>(N), static_cast<uint64_t>(K),
-                                     static_cast<uint64_t>(ldw), 256, BLOCK_K, is_bf16 != 0);
-        if (rc) return rc;
-        return is_bf16 ? launch<true, 256, false>(ta, tb, p, s) : launch<false, 256, false>(ta, tb, p, s);
-    }
-    if (is_bf16) return wide ? launch<true, 256, false>(ta, tb, p, s) : launch<true, 128, false>(ta, tb, p, s);
-    return wide ? launch<false, 256, false>(ta, tb, p, s) : launch<false, 128, false>(ta, tb, p, s);
+    if (is_bf16) return wide ? launch<true, 256>(ta, tb, p, s) : launch<true, 128>(ta, tb, p, s);
+    return wide ? launch<false, 256>(ta, tb, p, s) : launch<false, 128>(ta, tb, p, s);
 }
 
 // (tile shape, number of K splits) of a weight-gradient GEMM: minimise the number of waves of work items per split
-static void wgrad_plan(int32_t tokens, int32_t N, int32_t K, bool* pair, int* block_n, int* splits, int* kb_per_split) {
+static void wgrad_plan(int32_t tokens, int32_t N, int32_t K, int* block_n, int* splits, int* kb_per_split) {
     using namespace gemm;
-    *pair = K >= 256 && N >= 256;
     *block_n = K >= 256 ? 256 : 128;
-    const int tile_m = *pair ? 256 : 128;
-    const int64_t tiles = static_cast<int64_t>((N + tile_m - 1) / tile_m) * ((K + *block_n - 1) / *block_n);
-    const int groups = abh::num_sms() / (*pair ? 2 : 1);
+    const int64_t tiles = static_cast<int64_t>((N + BLOCK_M - 1) / BLOCK_M) * ((K + *block_n - 1) / *block_n);
+    const int groups = abh::num_sms();
     const int num_kb = (tokens + BLOCK_K - 1) / BLOCK_K;
     int best = 1;
     double best_t = 1e30;
@@ -828,9 +452,8 @@ static void wgrad_plan(int32_t tokens, int32_t N, int32_t K, bool* pair, int* bl
 }
 
 size_t atlas_b200_linear_wgrad_workspace_bytes(int32_t tokens, int32_t N, int32_t K) {
-    bool pair;
     int block_n, splits, per;
-    wgrad_plan(tokens, N, K, &pair, &block_n, &splits, &per);
+    wgrad_plan(tokens, N, K, &block_n, &splits, &per);
     return splits > 1 ? static_cast<size_t>(splits) * N * K * sizeof(float) : 0;
 }
 
@@ -861,9 +484,8 @@ int atlas_b200_linear_wgrad(const void* dY, int64_t lddy, const void* X, int64_t
     p.bias = nullptr;
     p.residual = nullptr;
     p.C = static_cast<uint16_t*>(dW);
-    bool pair;
     int block_n, splits, per;
-    wgrad_plan(tokens, N, K, &pair, &block_n, &splits, &per);
+    wgrad_plan(tokens, N, K, &block_n, &splits, &per);
     const bool wide = block_n == 256;
     static const bool no_splitk = getenv("ATLAS_B200_WGRAD_NO_SPLITK") != nullptr;   // A/B measurements
     const size_t need = static_cast<size_t>(splits) * N * K * sizeof(float);
@@ -883,9 +505,8 @@ int atlas_b200_linear_wgrad(const void* dY, int64_t lddy, const void* X, int64_t
     rc = abh::make_tmap_2d_16bit(&tb, X, static_cast<uint64_t>(tokens), static_cast<uint64_t>(K), static_cast<uint64_t>(ldx),
                                  BLOCK_K, 64, is_bf16 != 0);
     if (rc) return rc;
-    if (pair) rc = is_bf16 ? launch<true, 256, true, true>(ta, tb, p, s) : launch<false, 256, true, true>(ta, tb, p, s);
-    else if (is_bf16) rc = wide ? launch<true, 256, false, true>(ta, tb, p, s) : launch<true, 128, false, true>(ta, tb, p, s);
-    else rc = wide ? launch<false, 256, false, true>(ta, tb, p, s) : launch<false, 128, false, true>(ta, tb, p, s);
+    if (is_bf16) rc = wide ? launch<true, 256, true>(ta, tb, p, s) : launch<true, 128, true>(ta, tb, p, s);
+    else rc = wide ? launch<false, 256, true>(ta, tb, p, s) : launch<false, 128, true>(ta, tb, p, s);
     if (rc || splits == 1) return rc;
     const int64_t vecs = static_cast<int64_t>(N) * (K / 8);
     const int64_t blocks = (vecs + 255) / 256, cap = static_cast<int64_t>(abh::num_sms()) * 8;

@@ -60,36 +60,12 @@ int make_tmap_2d_16bit(CUtensorMap* out, const void* base, uint64_t rows, uint64
     return ATLAS_B200_OK;
 }
 
-int make_tmap_kslabs_16bit(CUtensorMap* out, const void* base, uint64_t rows, uint64_t cols, uint64_t ld,
-                           uint32_t box_rows, uint32_t box_slabs, bool bf16) {
-    EncodeTiledFn fn = get_encode();
-    if (!fn) return ATLAS_B200_ECUDA;
-    if ((reinterpret_cast<uintptr_t>(base) & 15u) != 0 || (ld * 2) % 16 != 0 || cols % 64 != 0) {
-        set_error("tensor map: base must be 16-byte aligned, row stride a multiple of 16 bytes, cols a multiple of 64");
-        return ATLAS_B200_EINVAL;
-    }
-    cuuint64_t gdim[3] = {64, rows, cols / 64};
-    cuuint64_t gstride[2] = {ld * 2, 128};
-    cuuint32_t box[3] = {64, box_rows, box_slabs};
-    cuuint32_t estr[3] = {1, 1, 1};
-    CUresult r = fn(out, bf16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 3,
-                    const_cast<void*>(base), gdim, gstride, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                    CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                    CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (r != CUDA_SUCCESS) {
-        set_error("cuTensorMapEncodeTiled(3d) failed with CUresult %d (rows=%llu cols=%llu ld=%llu box=%ux%u)", (int)r,
-                  (unsigned long long)rows, (unsigned long long)cols, (unsigned long long)ld, box_rows, box_slabs);
-        return ATLAS_B200_ECUDA;
-    }
-    return ATLAS_B200_OK;
-}
-
 int num_sms() {
     static int n = 0;
     if (n == 0) {
         int dev = 0;
-        if (cudaGetDevice(&dev) != cudaSuccess) return 148;
-        if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) n = 148;
+        if (cudaGetDevice(&dev) != cudaSuccess) return 132;
+        if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) n = 132;
     }
     return n;
 }
@@ -215,7 +191,7 @@ int atlas_b200_profile_collect(double* total_ms, int32_t* launches) {
 
 
 const char* atlas_b200_last_error(void) { return abh::g_err; }
-const char* atlas_b200_version(void) { return "atlas_b200 0.1 (sm_100a)"; }
+const char* atlas_b200_version(void) { return "atlas_b200 0.2 (sm_90a)"; }
 uint64_t atlas_b200_launch_count(void) { return abh::g_launches.load(); }
 
 }  // extern "C"

@@ -41,13 +41,6 @@ inline void count_launch(int n = 1) { g_launches.fetch_add(static_cast<uint64_t>
 int make_tmap_2d_16bit(CUtensorMap* out, const void* base, uint64_t rows, uint64_t cols, uint64_t ld,
                        uint32_t box_rows, uint32_t box_cols, bool bf16);
 
-// 3-D view of a row-major [rows, 768]-like matrix of 2-byte elements as (k-in-slab, row, slab):
-// dim0 = 64 elements (128 B), dim1 = rows (stride ld*2 B), dim2 = cols/64 slabs (stride 128 B).
-// A box {64, box_rows, box_slabs} lands in smem as `box_slabs` consecutive K-major slabs of
-// [box_rows][128 B] with the 128-byte swizzle - the layout tcgen05 smem descriptors expect.
-int make_tmap_kslabs_16bit(CUtensorMap* out, const void* base, uint64_t rows, uint64_t cols, uint64_t ld,
-                           uint32_t box_rows, uint32_t box_slabs, bool bf16);
-
 int num_sms();
 
 // Optional CUDA-event bracketing of the dominant kernel (bench.py's roofline measurement): when

@@ -1,4 +1,4 @@
-// Exact max-inner-product search with fused top-k candidate filtering for sm_100a.
+// Exact max-inner-product search with fused top-k candidate filtering for sm_90a.
 //
 // Replaces the reference's `torch.matmul(q.half(), E)` + `torch.topk` (src/index.py:113-120): the
 // [nq, n] score matrix is never written.  Pipeline per block of <= 256 queries:
@@ -7,10 +7,10 @@
 //                       score kept                                   -> candidate lists
 //   (2) select (thr)  : per query, exact k-th best of the sample      -> a VALID lower bound on the
 //                       final k-th best score (k real passages reach it)
-//   (3) main scan     : ONE sweep of the whole bank (the HBM-bound part): tcgen05 GEMM tiles
-//                       [<=256 queries] x [128 passages] x 768, fp32 accumulators in TMEM; the
-//                       epilogue reads them back with tcgen05.ld, and appends (score, id) of the
-//                       few scores >= bound to the per-query candidate list
+//   (3) main scan     : ONE sweep of the whole bank (the HBM-bound part): wgmma GEMM tiles
+//                       [<=256 queries] x [128 passages] x 768, fp32 accumulators in registers;
+//                       the epilogue appends (score, id) of the few scores >= bound to the
+//                       per-query candidate list
 //   (4) select (final): per query, exact radix-select + sort of the candidates with the canonical
 //                       order (fp16 score desc, id asc)               -> [nq, k] scores / ids
 //
@@ -20,12 +20,13 @@
 // is raised and the caller falls back to `atlas_b200_mips_topk_exhaustive` (chunked, no thresholds).
 //
 // Scan kernel roles (384 threads, persistent, 1 CTA / SM):
-//   warp 0      TMA producer   : bank tile + query tile K-blocks -> 4-stage smem ring (128B swizzle)
-//   warp 1      MMA issuer     : tcgen05.mma kind::f16, M=128 (x2 query halves), N=128, K=16
-//   warp 2      TMEM allocator : 512 columns = 2 (double buffer) x 2 (query halves) x 128
-//   warps 4-11  epilogue       : thread <-> query row (TMEM lane); threshold filter + append
+//   warpgroup 0     TMA producer (one thread): bank tile + query tile K-blocks -> 4-stage smem ring (128B swizzle)
+//   warpgroups 1-4  64 queries each (query half h = (wg - 1) / 2, rows 64 ((wg - 1) % 2) ..): one wgmma m64n128k16 per
+//                   K step into 64 accumulator registers per thread, then the threshold filter + append straight from the
+//                   registers
 #include "common.cuh"
 #include "host_common.h"
+#include "wgmma.cuh"
 
 #include <math.h>
 #include <stdlib.h>
@@ -35,17 +36,16 @@ namespace mips {
 constexpr int DIM = ATLAS_B200_EMBEDDINGS_DIM;
 constexpr int BLOCK_K = 64;  // 128 bytes of 16-bit elements = one swizzle row
 constexpr int K_BLOCKS = DIM / BLOCK_K;
-constexpr int UMMA_K = 16;
-constexpr int TILE_N = 128;   // passages per tile (UMMA N)
-constexpr int HALF_M = 128;   // queries per UMMA (M)
+constexpr int UMMA_K = 16;   // K of one wgmma
+constexpr int TILE_N = 128;   // passages per tile (wgmma N)
+constexpr int HALF_M = 128;   // queries per consumer warpgroup
 constexpr int QBLOCK = 256;   // queries per scan launch
 constexpr int STAGES = 4;
 constexpr int A_HALF_BYTES = HALF_M * BLOCK_K * 2;
 constexpr int B_BYTES = TILE_N * BLOCK_K * 2;
 constexpr int STAGE_BYTES = 2 * A_HALF_BYTES + B_BYTES;
 constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + 1024;
-constexpr int NUM_THREADS = 384;
-constexpr int TMEM_COLS = 512;
+constexpr int NUM_THREADS = 640;
 
 static_assert(DIM % BLOCK_K == 0, "");
 
@@ -129,9 +129,6 @@ mips_scan_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_consta
     extern __shared__ uint8_t smem_raw[];
     __shared__ __align__(8) uint64_t full_bar[STAGES];
     __shared__ __align__(8) uint64_t empty_bar[STAGES];
-    __shared__ __align__(8) uint64_t tmem_full_bar[2];
-    __shared__ __align__(8) uint64_t tmem_empty_bar[2];
-    __shared__ uint32_t tmem_base_smem;
 
     const uint32_t warp = threadIdx.x >> 5;
     const uint32_t lane = threadIdx.x & 31u;
@@ -139,38 +136,26 @@ mips_scan_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_consta
     const uint32_t smem_base = (ab::smem_u32(smem_raw) + 1023u) & ~1023u;
     uint8_t* smem_gen = smem_raw + (smem_base - ab::smem_u32(smem_raw));
 
-    if (warp == 0 && lane == 0) {
+    if (threadIdx.x == 0) {
         ab::tma_prefetch_desc(&tmap_q);
         ab::tma_prefetch_desc(&tmap_bank);
-    }
-    if (warp == 1 && lane == 0) {
         for (int s = 0; s < STAGES; ++s) {
             ab::mbar_init(&full_bar[s], 1);
-            ab::mbar_init(&empty_bar[s], 1);
-        }
-        for (int b = 0; b < 2; ++b) {
-            ab::mbar_init(&tmem_full_bar[b], 1);
-            ab::mbar_init(&tmem_empty_bar[b], static_cast<uint32_t>(p.n_halves) * HALF_M);
+            ab::mbar_init(&empty_bar[s], static_cast<uint32_t>(2 * p.n_halves));   // one arrive per active consumer warpgroup
         }
         ab::fence_barrier_init();
     }
-    if (warp == 2) {
-        ab::tmem_alloc<1>(&tmem_base_smem, TMEM_COLS);
-    }
-    ab::tc_fence_before();
     __syncthreads();
-    ab::tc_fence_after();
-    const uint32_t tmem_base = tmem_base_smem;
 
-    if (warp == 0) {
+    if (warp < 4) {
         // ===================== TMA producer =====================
-        if (lane == 0) {
+        if (warp == 0 && lane == 0) {
             uint32_t stage = 0, phase = 0;
             const uint32_t tx_bytes = static_cast<uint32_t>(p.n_halves) * A_HALF_BYTES + B_BYTES;
             for (int i = blockIdx.x; i < p.num_tiles; i += gridDim.x) {
                 const int tile = p.tile_begin + i * p.tile_step;
                 for (int kb = 0; kb < K_BLOCKS; ++kb) {
-                    ab::mbar_wait(&empty_bar[stage], phase ^ 1u, 1);
+                    ab::mbar_wait_nocall(&empty_bar[stage], phase ^ 1u);
                     ab::mbar_arrive_expect_tx(&full_bar[stage], tx_bytes);
                     uint8_t* st = smem_gen + stage * STAGE_BYTES;
                     ab::tma_load_2d(&tmap_q, &full_bar[stage], st, kb * BLOCK_K, 0, ab::kEvictLast);
@@ -186,465 +171,84 @@ mips_scan_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_consta
                 }
             }
         }
-    } else if (warp == 1) {
-        // ===================== MMA issuer =====================
-        if (lane == 0) {
-            constexpr uint32_t idesc = ab::umma_idesc_f16(HALF_M, TILE_N, kBF16);
-            uint32_t stage = 0, phase = 0;
-            int it = 0;
-            for (int i = blockIdx.x; i < p.num_tiles; i += gridDim.x, ++it) {
-                const uint32_t buf = it & 1;
-                ab::mbar_wait(&tmem_empty_bar[buf], ((it >> 1) & 1) ^ 1u, 2);
-                ab::tc_fence_after();
-                for (int kb = 0; kb < K_BLOCKS; ++kb) {
-                    ab::mbar_wait(&full_bar[stage], phase, 3);
-                    ab::tc_fence_after();
-                    const uint32_t st = smem_base + stage * STAGE_BYTES;
-                    for (int h = 0; h < p.n_halves; ++h) {
-                        const uint32_t d_tmem = tmem_base + (buf * 2 + h) * TILE_N;
+        return;
+    }
+
+    // ===================== query half h: MMAs + threshold filter + candidate append =====================
+    const uint32_t cw = (warp >> 2) - 1u;             // consumer warpgroup 0..3
+    const uint32_t half = cw >> 1, sub = cw & 1u;
+    const uint32_t wl = warp & 3u;
+    if (static_cast<int>(half) >= p.n_halves) return;
+    // this thread's two query rows e: r and r + 8
+    int qrow[2];
+    float bnd[2];
 #pragma unroll
-                        for (int k = 0; k < BLOCK_K / UMMA_K; ++k) {
-                            const uint64_t adesc = ab::umma_desc_k_sw128(st + h * A_HALF_BYTES + k * UMMA_K * 2);
-                            const uint64_t bdesc = ab::umma_desc_k_sw128(st + 2 * A_HALF_BYTES + k * UMMA_K * 2);
-                            ab::umma_ss<1>(d_tmem, adesc, bdesc, idesc, (kb | k) != 0 ? 1u : 0u);
-                        }
-                    }
-                    ab::umma_commit(&empty_bar[stage]);
-                    if (++stage == STAGES) {
-                        stage = 0;
-                        phase ^= 1u;
-                    }
-                }
-                ab::umma_commit(&tmem_full_bar[buf]);
+    for (int e = 0; e < 2; ++e) {
+        qrow[e] = static_cast<int>(half * HALF_M + sub * 64 + wl * 16 + (lane >> 2) + e * 8);
+        bnd[e] = qrow[e] < p.nq ? p.bound[qrow[e]] : INFINITY;
+    }
+    const int cq = static_cast<int>(2u * (lane & 3u));
+    uint32_t stage = 0, phase = 0;
+    for (int i = blockIdx.x; i < p.num_tiles; i += gridDim.x) {
+        const int tile = p.tile_begin + i * p.tile_step;
+        float acc[64];
+        int prev_stage = -1;
+        for (int kb = 0; kb < K_BLOCKS; ++kb) {
+            ab::mbar_wait_nocall(&full_bar[stage], phase);
+            const uint32_t st = smem_base + stage * STAGE_BYTES;
+            ab::wgmma_fence();
+#pragma unroll
+            for (int k = 0; k < BLOCK_K / UMMA_K; ++k) {
+                const uint64_t bdesc = ab::wgmma_desc_sw128(st + 2 * A_HALF_BYTES + k * UMMA_K * 2);
+                const uint64_t adesc = ab::wgmma_desc_sw128(st + half * A_HALF_BYTES + sub * 8192 + k * UMMA_K * 2);
+                ab::wgmma_m64n128k16_ss<kBF16, 0, 0>(acc, adesc, bdesc, (kb | k) != 0 ? 1 : 0);
+            }
+            ab::wgmma_commit();
+            // the previous stage's MMAs have retired once at most this stage's group is pending: release it
+            ab::wgmma_wait<1>();
+            ab::wgmma_reg_fence(acc);
+            if (prev_stage >= 0 && wl == 0 && lane == 0) ab::mbar_arrive(&empty_bar[prev_stage]);
+            prev_stage = static_cast<int>(stage);
+            if (++stage == STAGES) {
+                stage = 0;
+                phase ^= 1u;
             }
         }
-    } else if (warp >= 4) {
-        // ===================== epilogue: threshold filter + candidate append =====================
-        const uint32_t half = (warp - 4) >> 2;
-        const uint32_t lg = warp & 3u;  // TMEM lane group this warp may access
-        if (static_cast<int>(half) < p.n_halves) {
-            const uint32_t q = half * HALF_M + lg * 32 + lane;
-            const float bnd = (static_cast<int>(q) < p.nq) ? p.bound[q] : INFINITY;
-            uint64_t* my_cand = p.cand + static_cast<size_t>(q) * p.capq;
-            int it = 0;
-            for (int i = blockIdx.x; i < p.num_tiles; i += gridDim.x, ++it) {
-                const uint32_t buf = it & 1;
-                const int tile = p.tile_begin + i * p.tile_step;
-                ab::mbar_wait(&tmem_full_bar[buf], (it >> 1) & 1, 4);
-                ab::tc_fence_after();
-#pragma unroll 1
-                for (int c = 0; c < TILE_N / 32; ++c) {
-                    uint32_t r[32];
-                    ab::tmem_ld32(tmem_base + ((lg * 32) << 16) + (buf * 2 + half) * TILE_N + c * 32, r);
-                    ab::tmem_ld_wait();
-                    float m = __uint_as_float(r[0]);
+        ab::wgmma_wait<0>();
+        ab::wgmma_reg_fence(acc);
+        if (wl == 0 && lane == 0) ab::mbar_arrive(&empty_bar[prev_stage]);
+
+        // row e of this thread: acc[4 j + 2 e + c] = passage tile * 128 + 8 j + 2 (lane % 4) + c
+        const int id_base = tile * TILE_N + cq;
 #pragma unroll
-                    for (int j = 1; j < 32; ++j) m = fmaxf(m, __uint_as_float(r[j]));
-                    if (__any_sync(0xffffffffu, m >= bnd)) {
-                        const int id0 = tile * TILE_N + c * 32;
-                        uint32_t npass = 0;
+        for (int e = 0; e < 2; ++e) {
+            const float* a = acc + 2 * e;
+            float m = -INFINITY;
 #pragma unroll
-                        for (int j = 0; j < 32; ++j)
-                            npass += (__uint_as_float(r[j]) >= bnd && id0 + j < p.n_rows) ? 1u : 0u;
-                        if (npass) {
-                            uint32_t pos = atomicAdd(&p.count[q], npass);
+            for (int j = 0; j < 32; ++j) m = fmaxf(m, fmaxf(a[4 * j], a[4 * j + 1]));
+            if (!(m >= bnd[e])) continue;
+            uint32_t npass = 0;
 #pragma unroll
-                            for (int j = 0; j < 32; ++j) {
-                                const float v = __uint_as_float(r[j]);
-                                if (v >= bnd && id0 + j < p.n_rows) {
-                                    if (pos < p.capq)
-                                        my_cand[pos] = pack_candidate(bits_to_key(round_to_bits<kBF16>(v)),
-                                                                      static_cast<uint32_t>(id0 + j));
-                                    ++pos;
-                                }
-                            }
-                        }
-                    }
-                }
-                ab::tc_fence_before();
-                ab::mbar_arrive(&tmem_empty_bar[buf]);
-            }
-        }
-    }
-
-    ab::tc_fence_before();
-    __syncthreads();
-    if (warp == 2) {
-        ab::tc_fence_after();
-        ab::tmem_dealloc<1>(tmem_base, TMEM_COLS);
-    }
-}
-
-
-// ---------------------------------------------------------------------------------------------
-// scan kernel v2 ("TS"): the query block stays RESIDENT ON THE SM as the tcgen05 A operand, so the
-// only bytes that cross L2 -> SM are the bank rows.
-//
-//   128 queries x 768 fp16 = 192 KB per CTA: K-blocks 0..7 (512 K) live in TENSOR MEMORY (256 columns,
-//   A-from-TMEM MMAs), K-blocks 8..11 (256 K) in 64 KB of shared memory (A-from-smem MMAs).  That split
-//   leaves 256 TMEM columns for TWO 128 x 128 fp32 accumulator buffers (MMA of tile i+1 overlaps the
-//   epilogue of tile i) at UMMA N = 128 — measured: below N = 128 tcgen05.mma is issue-bound at ~46-50
-//   cycles per instruction, at N >= 128 it runs at the 64/128-cycle peak (tools/umma_bench.cu).
-//   kPair = true : a 2-CTA cluster (cta_group::2, UMMA M=256) covers 256 queries; each CTA owns 128
-//                  query rows and streams HALF of every 128-passage tile (64 full rows = 96 KB contiguous
-//                  in HBM, two 3-D TMA boxes of 48 KB) through its own shared memory, so each bank byte is
-//                  fetched once per SM pair.
-//   kPair = false: one CTA (UMMA M=128) for <= 128 queries, four 48 KB boxes per 128-row tile.
-//   smem: 64 KB resident query K-tail + 3 ring stages x 48 KB (K-major slabs [rows][128 B], 128B swizzle).
-// Roles (384 threads): warp 0 TMA producer, warp 1 MMA issuer (leader CTA), warp 2 TMEM allocator,
-// warps 4-11 load the query K-head into TMEM once (tcgen05.st), then run the threshold-filter epilogue
-// (warp w: TMEM lane group w%4, accumulator columns 64*((w-4)/4) .. +63).
-// ---------------------------------------------------------------------------------------------
-constexpr int TS_TILE_N = 128;
-constexpr int TS_KB_TMEM = 8;                        // K-blocks of the queries kept in TMEM
-constexpr int TS_KB_SMEM = K_BLOCKS - TS_KB_TMEM;    // K-blocks of the queries kept in smem
-constexpr int TS_A_COLS = TS_KB_TMEM * (BLOCK_K / 2);  // 256 TMEM columns
-constexpr int TS_A_SMEM_BYTES = TS_KB_SMEM * HALF_M * 128;  // 64 KB
-constexpr int TS_THREADS = 384;
-constexpr int TS_EPI_WARPS = 8;
-
-template <bool kPair>
-struct TsCfg {
-    static constexpr int ROWS_PER_CTA = kPair ? 64 : 128;
-    static constexpr int SLAB_BYTES = ROWS_PER_CTA * 128;
-    static constexpr int KB_PER_STAGE = kPair ? 6 : 3;
-    static constexpr int STAGE_BYTES = KB_PER_STAGE * SLAB_BYTES;  // 48 KB
-    static constexpr int STAGES_PER_TILE = K_BLOCKS / KB_PER_STAGE;
-    static constexpr int STAGES = 3;
-    static constexpr int UMMA_M = kPair ? 256 : 128;
-    static constexpr int CTAS = kPair ? 2 : 1;
-    static constexpr int SMEM_BYTES = TS_A_SMEM_BYTES + STAGES * STAGE_BYTES + 1024;
-};
-
-__device__ __forceinline__ float max32(const uint32_t (&r)[32]) {
-    float t[16];
+            for (int j = 0; j < 32; ++j)
 #pragma unroll
-    for (int j = 0; j < 16; ++j) t[j] = fmaxf(__uint_as_float(r[j]), __uint_as_float(r[j + 16]));
+                for (int c = 0; c < 2; ++c) npass += (a[4 * j + c] >= bnd[e] && id_base + 8 * j + c < p.n_rows) ? 1u : 0u;
+            if (npass == 0) continue;
+            uint64_t* my_cand = p.cand + static_cast<size_t>(qrow[e]) * p.capq;
+            uint32_t pos = atomicAdd(&p.count[qrow[e]], npass);
 #pragma unroll
-    for (int j = 0; j < 8; ++j) t[j] = fmaxf(t[j], t[j + 8]);
+            for (int j = 0; j < 32; ++j) {
 #pragma unroll
-    for (int j = 0; j < 4; ++j) t[j] = fmaxf(t[j], t[j + 4]);
-    return fmaxf(fmaxf(t[0], t[1]), fmaxf(t[2], t[3]));
-}
-
-// Per-thread slot reservation in a query's candidate list: a thread claims BLOCKS of slots with one
-// atomicAdd (>= 8 at a time) and fills them privately, so the L2 atomic (measured: thousands of cycles
-// of latency while the bank sweep saturates HBM) is paid once or twice per thread per kernel instead of
-// once per hit.  Slots of a block that stay unused are written as 0 = the smallest composite key, which
-// the selection kernel can never pick while k real candidates exist.
-struct SlotBlock {
-    uint32_t pos;
-    uint32_t left;
-};
-
-__device__ __forceinline__ void slots_release(SlotBlock& b, uint32_t capq, uint64_t* my_cand) {
-    while (b.left) {
-        if (b.pos < capq) my_cand[b.pos] = 0ull;
-        ++b.pos;
-        --b.left;
-    }
-}
-
-// r[j] for a run-time j without local memory: a 5-level select tree over the 32 registers.
-__device__ __forceinline__ float mux32(const uint32_t (&r)[32], int j) {
-    uint32_t a[16], b[8], c[4];
-#pragma unroll
-    for (int i = 0; i < 16; ++i) a[i] = (j & 16) ? r[i + 16] : r[i];
-#pragma unroll
-    for (int i = 0; i < 8; ++i) b[i] = (j & 8) ? a[i + 8] : a[i];
-#pragma unroll
-    for (int i = 0; i < 4; ++i) c[i] = (j & 4) ? b[i + 4] : b[i];
-    const uint32_t d0 = (j & 2) ? c[2] : c[0], d1 = (j & 2) ? c[3] : c[1];
-    return __uint_as_float((j & 1) ? d1 : d0);
-}
-
-// Slow path of the threshold filter for one thread (= one query row) that has at least one passing
-// score among 32 accumulator columns: hit bitmask by straight-line compares, then the (few) set bits are
-// walked, each value fetched with the select tree above.  Only lanes with hits run this; there are no
-// warp votes, no chains of dependent branches and no local-memory arrays.
-template <bool kBF16>
-__device__ __forceinline__ void append_hits32(const uint32_t (&r)[32], float bnd, int id0, int n_rows,
-                                              uint32_t* count_q, uint32_t capq, uint64_t* my_cand, SlotBlock& blk) {
-    uint32_t m = 0;
-#pragma unroll
-    for (int j = 0; j < 32; ++j) m |= (__uint_as_float(r[j]) >= bnd) ? (1u << j) : 0u;
-    // columns past the end of the bank (zero-filled by TMA in the last tile) never count
-    const int valid = n_rows - id0;
-    if (valid < 32) m &= (valid <= 0) ? 0u : ((1u << valid) - 1u);
-    const uint32_t npass = __popc(m);
-    if (npass == 0) return;
-    if (npass > blk.left) {
-        slots_release(blk, capq, my_cand);
-        const uint32_t want = (npass + 7u) & ~7u;
-        blk.pos = atomicAdd(count_q, want);
-        blk.left = want;
-    }
-    while (m) {
-        const int j = __ffs(m) - 1;
-        m &= m - 1;
-        const float v = mux32(r, j);
-        if (blk.pos < capq)
-            my_cand[blk.pos] = pack_candidate(bits_to_key(round_to_bits<kBF16>(v)), static_cast<uint32_t>(id0 + j));
-        ++blk.pos;
-        --blk.left;
-    }
-}
-
-template <bool kBF16, bool kPair>
-__global__ void __launch_bounds__(TS_THREADS, 1)
-mips_scan_ts_kernel(const __grid_constant__ CUtensorMap tmap_bank, const __grid_constant__ CUtensorMap tmap_q,
-                    const uint16_t* __restrict__ qstage, const ScanParams p) {
-    using C = TsCfg<kPair>;
-    extern __shared__ uint8_t smem_raw[];
-    __shared__ __align__(8) uint64_t full_bar[C::STAGES];
-    __shared__ __align__(8) uint64_t empty_bar[C::STAGES];
-    __shared__ __align__(8) uint64_t tmem_full_bar[2];
-    __shared__ __align__(8) uint64_t tmem_empty_bar[2];
-    __shared__ __align__(8) uint64_t a_tmem_bar;   // query K-head written to TMEM (all epilogue threads)
-    __shared__ __align__(8) uint64_t a_smem_bar;   // query K-tail landed in smem (TMA)
-    __shared__ uint32_t tmem_base_smem;
-
-    const uint32_t warp = threadIdx.x >> 5;
-    const uint32_t lane = threadIdx.x & 31u;
-    const uint32_t cta_rank = kPair ? ab::cluster_ctarank() : 0u;
-    const bool leader = cta_rank == 0;
-    const int group = kPair ? static_cast<int>(blockIdx.x >> 1) : static_cast<int>(blockIdx.x);
-    const int num_groups = kPair ? static_cast<int>(gridDim.x >> 1) : static_cast<int>(gridDim.x);
-    const uint32_t smem_base = (ab::smem_u32(smem_raw) + 1023u) & ~1023u;   // resident query K-tail
-    const uint32_t ring_base = smem_base + TS_A_SMEM_BYTES;
-    uint8_t* smem_gen = smem_raw + (smem_base - ab::smem_u32(smem_raw));
-    uint8_t* ring_gen = smem_gen + TS_A_SMEM_BYTES;
-
-    if (warp == 0 && lane == 0) {
-        ab::tma_prefetch_desc(&tmap_bank);
-        ab::tma_prefetch_desc(&tmap_q);
-    }
-    if (warp == 1 && lane == 0) {
-        for (int s = 0; s < C::STAGES; ++s) {
-            ab::mbar_init(&full_bar[s], 1);
-            ab::mbar_init(&empty_bar[s], 1);
-        }
-        for (int b = 0; b < 2; ++b) {
-            ab::mbar_init(&tmem_full_bar[b], 1);
-            ab::mbar_init(&tmem_empty_bar[b], static_cast<uint32_t>(TS_EPI_WARPS * C::CTAS));
-        }
-        ab::mbar_init(&a_tmem_bar, static_cast<uint32_t>(TS_EPI_WARPS * 32 * C::CTAS));
-        ab::mbar_init(&a_smem_bar, 1);
-        ab::fence_barrier_init();
-    }
-    if (warp == 2) ab::tmem_alloc<C::CTAS>(&tmem_base_smem, TMEM_COLS);
-    ab::tc_fence_before();
-    if constexpr (kPair) {
-        ab::cluster_sync_all();
-    } else {
-        __syncthreads();
-    }
-    ab::tc_fence_after();
-    const uint32_t tmem_base = tmem_base_smem;
-
-    if (warp == 0) {
-        // ===================== TMA producer (every CTA streams its own rows) =====================
-        if (lane == 0) {
-            // resident query K-tail: K-blocks 8..11 of this CTA's 128 query rows
-            if (leader) ab::mbar_arrive_expect_tx(&a_smem_bar, TS_A_SMEM_BYTES * C::CTAS);
-            for (int s = 0; s < TS_KB_SMEM; ++s) {
-                if constexpr (kPair) {
-                    ab::tma_load_2d_2sm(&tmap_q, &a_smem_bar, smem_gen + s * (HALF_M * 128), (TS_KB_TMEM + s) * BLOCK_K,
-                                        static_cast<int>(cta_rank) * HALF_M, ab::kEvictLast);
-                } else {
-                    ab::tma_load_2d(&tmap_q, &a_smem_bar, smem_gen + s * (HALF_M * 128), (TS_KB_TMEM + s) * BLOCK_K, 0,
-                                    ab::kEvictLast);
-                }
-            }
-            uint32_t stage = 0, phase = 0;
-            long long w_empty = 0;
-            for (int i = group; i < p.num_tiles; i += num_groups) {
-                const int tile = p.tile_begin + i * p.tile_step;
-                const int row0 = tile * TS_TILE_N + static_cast<int>(cta_rank) * C::ROWS_PER_CTA;
-                for (int st = 0; st < C::STAGES_PER_TILE; ++st) {
-                    const long long t0 = clock64();
-                    ab::mbar_wait(&empty_bar[stage], phase ^ 1u, 1);
-                    w_empty += clock64() - t0;
-                    uint8_t* dst = ring_gen + stage * C::STAGE_BYTES;
-                    if constexpr (kPair) {
-                        // the leader's barrier collects the bytes of BOTH CTAs' boxes
-                        if (leader) ab::mbar_arrive_expect_tx(&full_bar[stage], 2 * C::STAGE_BYTES);
-                        ab::tma_load_3d_2sm(&tmap_bank, &full_bar[stage], dst, 0, row0, st * C::KB_PER_STAGE,
-                                            ab::kEvictFirst);
-                    } else {
-                        ab::mbar_arrive_expect_tx(&full_bar[stage], C::STAGE_BYTES);
-                        ab::tma_load_3d(&tmap_bank, &full_bar[stage], dst, 0, row0, st * C::KB_PER_STAGE,
-                                        ab::kEvictFirst);
-                    }
-                    if (++stage == C::STAGES) {
-                        stage = 0;
-                        phase ^= 1u;
+                for (int c = 0; c < 2; ++c) {
+                    const float v = a[4 * j + c];
+                    const int id = id_base + 8 * j + c;
+                    if (v >= bnd[e] && id < p.n_rows) {
+                        if (pos < p.capq)
+                            my_cand[pos] = pack_candidate(bits_to_key(round_to_bits<kBF16>(v)), static_cast<uint32_t>(id));
+                        ++pos;
                     }
                 }
             }
-            if (p.dbg) p.dbg[blockIdx.x * 16 + 0] = w_empty;
         }
-    } else if (warp == 1) {
-        // ===================== MMA issuer (leader CTA only) =====================
-        if (lane == 0 && leader) {
-            constexpr uint32_t idesc = ab::umma_idesc_f16(C::UMMA_M, TS_TILE_N, kBF16);
-            const long long tstart = clock64();
-            long long w_te = 0, w_full = 0;
-            ab::mbar_wait(&a_tmem_bar, 0, 5);
-            ab::mbar_wait(&a_smem_bar, 0, 6);
-            const long long w_a = clock64() - tstart;
-            ab::tc_fence_after();
-            const uint64_t adesc0 = ab::umma_desc_k_sw128(smem_base);
-            uint32_t stage = 0, phase = 0;
-            int it = 0;
-            for (int i = group; i < p.num_tiles; i += num_groups, ++it) {
-                const uint32_t buf = it & 1;
-                const long long t0 = clock64();
-                ab::mbar_wait(&tmem_empty_bar[buf], ((it >> 1) & 1) ^ 1u, 2);
-                w_te += clock64() - t0;
-                ab::tc_fence_after();
-                const uint32_t d_tmem = tmem_base + TS_A_COLS + buf * TS_TILE_N;
-#pragma unroll
-                for (int st = 0; st < C::STAGES_PER_TILE; ++st) {
-                    const long long t1 = clock64();
-                    ab::mbar_wait(&full_bar[stage], phase, 3);
-                    w_full += clock64() - t1;
-                    ab::tc_fence_after();
-                    const uint64_t desc0 = ab::umma_desc_k_sw128(ring_base + stage * C::STAGE_BYTES);
-#pragma unroll
-                    for (int kbl = 0; kbl < C::KB_PER_STAGE; ++kbl) {
-                        const int kb = st * C::KB_PER_STAGE + kbl;
-#pragma unroll
-                        for (int k = 0; k < BLOCK_K / UMMA_K; ++k) {
-                            const uint64_t bdesc =
-                                desc0 + static_cast<uint64_t>((kbl * C::SLAB_BYTES + k * UMMA_K * 2) >> 4);
-                            if (kb < TS_KB_TMEM) {
-                                ab::umma_ts<C::CTAS>(d_tmem, tmem_base + kb * (BLOCK_K / 2) + k * (UMMA_K / 2), bdesc,
-                                                     idesc, (kb | k) != 0 ? 1u : 0u);
-                            } else {
-                                const uint64_t adesc =
-                                    adesc0 +
-                                    static_cast<uint64_t>(((kb - TS_KB_TMEM) * (HALF_M * 128) + k * UMMA_K * 2) >> 4);
-                                ab::umma_ss<C::CTAS>(d_tmem, adesc, bdesc, idesc, 1u);
-                            }
-                        }
-                    }
-                    if constexpr (kPair) {
-                        ab::umma_commit_2sm(&empty_bar[stage], 0x3);
-                    } else {
-                        ab::umma_commit(&empty_bar[stage]);
-                    }
-                    if (++stage == C::STAGES) {
-                        stage = 0;
-                        phase ^= 1u;
-                    }
-                }
-                if constexpr (kPair) {
-                    ab::umma_commit_2sm(&tmem_full_bar[buf], 0x3);
-                } else {
-                    ab::umma_commit(&tmem_full_bar[buf]);
-                }
-            }
-            if (p.dbg) {
-                p.dbg[blockIdx.x * 16 + 1] = w_te;
-                p.dbg[blockIdx.x * 16 + 2] = w_full;
-                p.dbg[blockIdx.x * 16 + 3] = w_a;
-                p.dbg[blockIdx.x * 16 + 4] = clock64() - tstart;
-                p.dbg[blockIdx.x * 16 + 5] = it;
-            }
-        }
-    } else if (warp >= 4) {
-        // ===================== query K-head into TMEM, then the filter epilogue =====================
-        const uint32_t lg = warp & 3u;
-        const uint32_t half = (warp - 4u) >> 2;                 // which 64 accumulator columns
-        const uint32_t q = cta_rank * 128u + lg * 32u + lane;   // row of the staged query block
-        const uint32_t lane_addr = tmem_base + ((lg * 32u) << 16);
-        {
-            const uint4* src = reinterpret_cast<const uint4*>(qstage + static_cast<size_t>(q) * DIM);
-#pragma unroll 1
-            for (int kb = static_cast<int>(half) * (TS_KB_TMEM / 2); kb < static_cast<int>(half + 1) * (TS_KB_TMEM / 2);
-                 ++kb) {
-                uint32_t r[32];
-#pragma unroll
-                for (int v = 0; v < 8; ++v) {
-                    const uint4 x = __ldg(src + kb * 8 + v);
-                    r[4 * v + 0] = x.x;
-                    r[4 * v + 1] = x.y;
-                    r[4 * v + 2] = x.z;
-                    r[4 * v + 3] = x.w;
-                }
-                ab::tmem_st32(lane_addr + kb * (BLOCK_K / 2), r);
-            }
-            ab::tmem_st_wait();
-            ab::tc_fence_before();
-            if (leader) {
-                ab::mbar_arrive(&a_tmem_bar);
-            } else {
-                ab::mbar_arrive_cluster(&a_tmem_bar, 0);
-            }
-        }
-        const float bnd = (static_cast<int>(q) < p.nq) ? p.bound[q] : INFINITY;
-        uint64_t* my_cand = p.cand + static_cast<size_t>(q) * p.capq;
-        int it = 0;
-        long long w_tf = 0, w_ld = 0, w_arr = 0, w_max = 0, w_slow = 0;
-        SlotBlock blk = {0u, 0u};
-        for (int i = group; i < p.num_tiles; i += num_groups, ++it) {
-            const uint32_t buf = it & 1;
-            const int tile = p.tile_begin + i * p.tile_step;
-            const long long t0 = clock64();
-            ab::mbar_wait(&tmem_full_bar[buf], (it >> 1) & 1, 4);
-            const long long t1 = clock64();
-            w_tf += t1 - t0;
-            ab::tc_fence_after();
-            const uint32_t d_addr = lane_addr + TS_A_COLS + buf * TS_TILE_N + half * 64u;
-            uint32_t r0[32], r1[32];
-            ab::tmem_ld32(d_addr, r0);
-            ab::tmem_ld32(d_addr + 32, r1);
-            ab::tmem_ld_wait();
-            const long long t2 = clock64();
-            w_ld += t2 - t1;
-            // the accumulator columns are in registers: hand the buffer back before filtering
-            ab::tc_fence_before();
-            __syncwarp();
-            if (lane == 0) {
-                if (leader) {
-                    ab::mbar_arrive(&tmem_empty_bar[buf]);
-                } else {
-                    ab::mbar_arrive_cluster(&tmem_empty_bar[buf], 0);
-                }
-            }
-            const long long t3 = clock64();
-            w_arr += t3 - t2;
-            const int id0 = tile * TS_TILE_N + static_cast<int>(half) * 64;
-            // lane-divergent on purpose: only rows with a hit pay for the slow path
-            const float mx0 = max32(r0), mx1 = max32(r1);
-            asm volatile("" ::"f"(mx0), "f"(mx1));
-            const long long t4 = clock64();
-            w_max += t4 - t3;
-            if (mx0 >= bnd) append_hits32<kBF16>(r0, bnd, id0, p.n_rows, &p.count[q], p.capq, my_cand, blk);
-            if (mx1 >= bnd) append_hits32<kBF16>(r1, bnd, id0 + 32, p.n_rows, &p.count[q], p.capq, my_cand, blk);
-            __syncwarp();
-            w_slow += clock64() - t4;
-        }
-        slots_release(blk, p.capq, my_cand);
-        if (p.dbg && warp == 4 && lane == 0) {
-            p.dbg[blockIdx.x * 16 + 7] = w_ld;
-            p.dbg[blockIdx.x * 16 + 8] = w_arr;
-            p.dbg[blockIdx.x * 16 + 9] = w_max;
-            p.dbg[blockIdx.x * 16 + 10] = w_slow;
-        }
-        if (p.dbg && warp == 4 && lane == 0) p.dbg[blockIdx.x * 16 + 6] = w_tf;
-    }
-
-    ab::tc_fence_before();
-    if constexpr (kPair) {
-        ab::cluster_sync_all();
-    } else {
-        __syncthreads();
-    }
-    if (warp == 2) {
-        ab::tc_fence_after();
-        ab::tmem_dealloc<C::CTAS>(tmem_base, TMEM_COLS);
     }
 }
 
@@ -942,46 +546,7 @@ static int launch_scan(const CUtensorMap& tq, const CUtensorMap& tb, const ScanP
     return ATLAS_B200_OK;
 }
 
-// 0 = SS kernel (queries streamed through smem), 1 = TS kernel (queries resident in TMEM)
-static int g_kernel_mode = -1;
-static unsigned long long* g_dbg = nullptr;  // device buffer for wait-cycle counters of the main scan
-static int kernel_mode() {
-    if (g_kernel_mode < 0) {
-        const char* e = getenv("ATLAS_B200_MIPS_KERNEL");
-        g_kernel_mode = (e && (e[0] == 's' || e[0] == 'S')) ? 0 : 1;
-    }
-    return g_kernel_mode;
-}
-
-template <bool kBF16, bool kPair>
-static int launch_scan_ts(const CUtensorMap& tb, const CUtensorMap& tq, const uint16_t* qstage, const ScanParams& p,
-                          cudaStream_t s) {
-    using C = TsCfg<kPair>;
-    static bool attr_set = false;
-    if (!attr_set) {
-        AB_CUDA_CHECK(cudaFuncSetAttribute(mips_scan_ts_kernel<kBF16, kPair>,
-                                           cudaFuncAttributeMaxDynamicSharedMemorySize, C::SMEM_BYTES));
-        attr_set = true;
-    }
-    if (p.num_tiles <= 0) return ATLAS_B200_OK;
-    const int max_groups = abh::num_sms() / C::CTAS;
-    const int groups = p.num_tiles < max_groups ? p.num_tiles : max_groups;
-    cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = dim3(static_cast<unsigned>(groups * C::CTAS));
-    cfg.blockDim = dim3(TS_THREADS);
-    cfg.dynamicSmemBytes = C::SMEM_BYTES;
-    cfg.stream = s;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeClusterDimension;
-    attr[0].val.clusterDim.x = C::CTAS;
-    attr[0].val.clusterDim.y = 1;
-    attr[0].val.clusterDim.z = 1;
-    cfg.attrs = attr;
-    cfg.numAttrs = 1;
-    AB_CUDA_CHECK(cudaLaunchKernelEx(&cfg, mips_scan_ts_kernel<kBF16, kPair>, tb, tq, qstage, p));
-    abh::count_launch();
-    return ATLAS_B200_OK;
-}
+static unsigned long long* g_dbg = nullptr;  // device buffer for wait-cycle counters of the main scan (unused by this kernel)
 
 static int check_common(const void* bank, int64_t n, int64_t ld, const void* queries, int nq, int k) {
     AB_REQUIRE(nq >= 0 && k >= 1, "nq must be >= 0 and k >= 1 (nq=%d k=%d)", nq, k);
@@ -1010,24 +575,13 @@ static int topk_impl(const void* bank, int64_t n, int64_t ld, const void* querie
         abh::set_error("workspace too small: have %zu need %zu", workspace_bytes, need);
         return ATLAS_B200_EWORKSPACE;
     }
-    const bool ts = kernel_mode() == 1;
-    const int tile_n = ts ? TS_TILE_N : TILE_N;
-    // tensor maps: SS = query block + 128-row bank boxes; TS = 64-row (single CTA) / 32-row (CTA pair) boxes
-    CUtensorMap tq, tb, tb_pair;
+    const int tile_n = TILE_N;
+    // tensor maps: query block (128-row boxes) + 128-row bank boxes
+    CUtensorMap tq, tb;
     rc = abh::make_tmap_2d_16bit(&tq, w.qstage, QBLOCK, DIM, DIM, HALF_M, BLOCK_K, kBF16);
     if (rc) return rc;
-    if (!ts) {
-        rc = abh::make_tmap_2d_16bit(&tb, bank, static_cast<uint64_t>(n), DIM, static_cast<uint64_t>(ld), TILE_N,
-                                     BLOCK_K, kBF16);
-        if (rc) return rc;
-    } else {
-        rc = abh::make_tmap_kslabs_16bit(&tb, bank, static_cast<uint64_t>(n), DIM, static_cast<uint64_t>(ld),
-                                         TsCfg<false>::ROWS_PER_CTA, TsCfg<false>::KB_PER_STAGE, kBF16);
-        if (rc) return rc;
-        rc = abh::make_tmap_kslabs_16bit(&tb_pair, bank, static_cast<uint64_t>(n), DIM, static_cast<uint64_t>(ld),
-                                         TsCfg<true>::ROWS_PER_CTA, TsCfg<true>::KB_PER_STAGE, kBF16);
-        if (rc) return rc;
-    }
+    rc = abh::make_tmap_2d_16bit(&tb, bank, static_cast<uint64_t>(n), DIM, static_cast<uint64_t>(ld), TILE_N, BLOCK_K, kBF16);
+    if (rc) return rc;
 
     const int total_tiles = static_cast<int>((n + tile_n - 1) / tile_n);
     const uint16_t* q16 = static_cast<const uint16_t*>(queries);
@@ -1048,11 +602,7 @@ static int topk_impl(const void* bank, int64_t n, int64_t ld, const void* querie
         p.dbg = nullptr;
         uint16_t* os_b = os + static_cast<size_t>(q0) * k;
         int64_t* oi_b = out_ids + static_cast<size_t>(q0) * k;
-        auto scan = [&](const ScanParams& sp) -> int {
-            if (!ts) return launch_scan<kBF16>(tq, tb, sp, s);
-            if (sp.n_halves == 2) return launch_scan_ts<kBF16, true>(tb_pair, tq, w.qstage, sp, s);
-            return launch_scan_ts<kBF16, false>(tb, tq, w.qstage, sp, s);
-        };
+        auto scan = [&](const ScanParams& sp) -> int { return launch_scan<kBF16>(tq, tb, sp, s); };
 
         if (!exhaustive) {
             int first_tile = 0;
@@ -1061,7 +611,7 @@ static int topk_impl(const void* bank, int64_t n, int64_t ld, const void* querie
                 // Sample size: the bound-only select costs O(m) per query and the sweep that follows keeps ~k*n_next/m
                 // candidates per query.  With the refinement sweep over the first tenth of the bank (below) the next part
                 // is n/10 rows, so m = sqrt(k*n/10) balances the two selects (4 Mi rows, k = 40: m = 4096 instead of the
-                // 26 k of the one-stage bound 2*sqrt(k*n): the 256-query threshold select drops from ~220 us to ~35 us);
+                // 26 k of the one-stage bound 2*sqrt(k*n): the 256-query threshold select does ~6 x less work);
                 // without a refinement stage the one-stage optimum is kept.
                 double m_two_stage = sqrt(static_cast<double>(k) * static_cast<double>(n) / 10.0);
                 if (m_two_stage < 4096) m_two_stage = 4096;
@@ -1138,7 +688,8 @@ static int topk_impl(const void* bank, int64_t n, int64_t ld, const void* querie
 
 extern "C" {
 
-void atlas_b200_mips_set_kernel(int32_t mode) { mips::g_kernel_mode = mode ? 1 : 0; }
+// one scan kernel on sm_90a: the mode switch is accepted and ignored
+void atlas_b200_mips_set_kernel(int32_t mode) { (void)mode; }
 void atlas_b200_mips_set_debug_counters(void* device_u64_buffer) {
     mips::g_dbg = static_cast<unsigned long long*>(device_u64_buffer);
 }

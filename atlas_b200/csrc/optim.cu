@@ -1,4 +1,4 @@
-// Multi-tensor optimiser / gradient-statistics kernels of the training step (SURVEY.md §8 f3):
+// Multi-tensor optimiser / gradient-statistics kernels of the training step:
 //   adamw_fp32copy_kernel   one launch updates EVERY parameter of an `AdamWFP32Copy` group (src/AdamWFP32Copy.py:79-169: fp32
 //                           master copy + torch.optim AdamW math on it + copy back into the 16-bit / fp32 parameter), instead
 //                           of ~10 foreach launches per dtype bucket plus one `p.copy_` per parameter;

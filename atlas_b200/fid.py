@@ -3,7 +3,7 @@ Fusion-in-Decoder on B200 kernels: the no-grad forward (evaluation / scoring / g
 CUDA graph), the with-grad forward + hand-written backward kernels of the training step (`_forward_train`, grad_ops.py),
 and the cross-attention score capture used for retriever distillation (src/fid.py:126-235,333-343).
 
-Surface kept (SURVEY.md §8b): `FiD(config)`, `forward(input_ids [B, n*L], attention_mask, decoder_input_ids,
+Surface kept: `FiD(config)`, `forward(input_ids [B, n*L], attention_mask, decoder_input_ids,
 labels, encoder_outputs=None, use_cache=False)` -> output indexable as `out[0]` = loss, `out[1]` = logits with
 `.logits`, `.loss`, `.encoder_last_hidden_state`; `encoder.config.{n_context,bsz}` are read like the reference's
 `FiDStack` (src/fid.py:47-49,66-76); `_shift_right`; `generate` (greedy); parameter names identical to HF T5
@@ -11,7 +11,7 @@ labels, encoder_outputs=None, use_cache=False)` -> output indexable as `out[0]` 
 `layer.1.EncDecAttention`, `DenseReluDense.{wi_0,wi_1,wo}`, `lm_head`) so reference checkpoints load.
 
 What runs where (all in csrc/): RMSNorm (T5LayerNorm, modeling_t5.py:244-253); q/k/v/o and FF projections on the
-tcgen05 GEMM with fused residual and gated-GELU epilogues (modeling_t5.py:281-289); encoder self-attention as
+wgmma GEMM with fused residual and gated-GELU epilogues (modeling_t5.py:281-289); encoder self-attention as
 B*n independent L-token segments with the relative-position bias added on the fly from a [H, 2L-1] table
 (modeling_t5.py:352-416,478-524) - the [B*n, H, L, L] bias / probability tensors are never materialised;
 decoder cross-attention over the n*L concatenated keys as split-KV + combine (fid.py:298-349).
@@ -462,10 +462,8 @@ class FiD(nn.Module):
         B, T = decoder_input_ids.shape
         d, H = c.d_model, c.num_heads
         Lk = enc.shape[1]
-        # key segments of the split-KV cross-attention: the largest divisor of Lk up to 384 keys (the two-half kernel,
-        # attention_split_kernel), else up to 512 (single-accumulator kernel).  256-key segments (K / V double-buffered by
-        # that kernel) were measured SLOWER for the FiD decoder: 2.32 vs 1.92 ms per 8-query step - the per-segment
-        # softmax / MMA chain, not the load latency, sets the segment time (profiles/r02_launches_step_visit_i.csv)
+        # key segments of the split-KV cross-attention: the largest divisor of Lk up to 384 keys, else up to 512 (the
+        # attention kernel keeps a whole segment's K / V in shared memory)
         split = next((s for s in range(min(384, Lk), 63, -1) if Lk % s == 0), None) or \
             next(s for s in range(min(512, Lk), 0, -1) if Lk % s == 0)
         if split < 64 and Lk > 512:

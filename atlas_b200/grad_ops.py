@@ -3,7 +3,7 @@
 (ops.py); torch.autograd only chains them and accumulates into the parameters' `.grad`.
 
 What autograd would derive through the reference's modules is implemented by hand:
-  Linear           y = x W^T (+ b) (+ residual)      dX = dY W (tcgen05 GEMM on W^T), dW = dY^T X (tcgen05 GEMM with both
+  Linear           y = x W^T (+ b) (+ residual)      dX = dY W (wgmma GEMM on W^T), dW = dY^T X (wgmma GEMM with both
                                                      operands MN-major: no transposes; split-K, fp32 accumulation over
                                                      the tokens), db = column sums
   Norm             BertLayerNorm / T5 RMSNorm        src/modeling_bert.py:104-114, src/modeling_t5.py:244-253

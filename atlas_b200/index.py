@@ -1,11 +1,11 @@
 """Drop-in for `src.index.DistributedIndex` (reference src/index.py:43-160) on B200.
 
-Same public surface (SURVEY.md §8b): `embeddings` ([768, N] fp16 CUDA, slice-assignable on dim 1),
+Same public surface: `embeddings` ([768, N] fp16 CUDA, slice-assignable on dim 1),
 `doc_map`, `is_in_gpu`, `init_embeddings`, `search_knn`, `save_index`, `load_index`,
 `is_index_trained`, `train_index`.  What changes underneath:
 
   * the bank is stored passage-major, `[N, 768]` row-major (1536 contiguous bytes per passage, what
-    TMA / tcgen05 want); `embeddings` is the transposed VIEW, so `index.embeddings[:, a:b] = emb.T`
+    TMA / wgmma want); `embeddings` is the transposed VIEW, so `index.embeddings[:, a:b] = emb.T`
     (src/atlas.py:79) and `embeddings[:, s:e]` (src/index.py:85) keep working and write through;
   * `_compute_scores_and_indices` is ONE fused scan (csrc/mips.cu) instead of matmul + topk: the
     [nq, N] score matrix is never materialised;

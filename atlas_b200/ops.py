@@ -164,7 +164,7 @@ EPI_NONE, EPI_BIAS, EPI_GELU, EPI_RESIDUAL, EPI_GATED = 0, 1, 2, 3, 4
 
 
 def linear(x, weight, bias=None, residual=None, epilogue=None, out=None, row_ss=None, out_ss=None, rs_eps=1e-6, rows=None):
-    """y = epilogue(x @ weight.T) on tcgen05.  x [..., K], weight [N, K] (nn.Linear layout), 16-bit.
+    """y = epilogue(x @ weight.T) on wgmma.  x [..., K], weight [N, K] (nn.Linear layout), 16-bit.
 
     epilogue: EPI_NONE / EPI_BIAS / EPI_GELU / EPI_RESIDUAL / EPI_GATED (see include/atlas_b200.h);
     default: EPI_RESIDUAL if `residual` is given, else EPI_BIAS if `bias` is given, else EPI_NONE.
@@ -494,12 +494,12 @@ def colsum(x):
 
 
 def linear_dgrad(dy, weight):
-    """dX [M, K] = dY [M, N] . W [N, K]: the same tcgen05 GEMM on W^T (a weight-sized transpose per call)."""
+    """dX [M, K] = dY [M, N] . W [N, K]: the same wgmma GEMM on W^T (a weight-sized transpose per call)."""
     return linear(dy, transpose(weight))
 
 
 def linear_wgrad(dy, x):
-    """dW [N, K] = dY^T [N, M] . X [M, K] (contraction over the M tokens, fp32 accumulation, 16-bit result): the tcgen05
+    """dW [N, K] = dY^T [N, M] . X [M, K] (contraction over the M tokens, fp32 accumulation, 16-bit result): the wgmma
     GEMM with both operands MN-major (no transposes).  ATLAS_B200_WGRAD_TRANSPOSE=1 selects the first-generation path
     (two explicit transposes + the K-major GEMM), kept for A/B measurements."""
     require_cuda(dy, "dy")

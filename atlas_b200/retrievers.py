@@ -9,7 +9,7 @@ src/modeling_bert.py:190-648,872-1045), so `load_state_dict` of a Contriever che
     embeddings.{word,position,token_type}_embeddings.weight, embeddings.LayerNorm.{weight,bias},
     encoder.layer.N.attention.self.{query,key,value}.{weight,bias}, attention.output.dense / LayerNorm,
     intermediate.dense, output.dense / LayerNorm.
-The arithmetic runs in `csrc/`: tcgen05 GEMMs with fused bias / erf-GELU / residual epilogues, fused attention
+The arithmetic runs in `csrc/`: wgmma GEMMs with fused bias / erf-GELU / residual epilogues, fused attention
 reading Q/K/V in place from one [tokens, 2304] projection buffer, the reference's non-standard BertLayerNorm
 (uncentred second moment, src/modeling_bert.py:104-114), masked mean pooling that can write straight into
 the passage bank rows.  16-bit only on the device: fp32 parameters (the live query encoder without
@@ -248,7 +248,7 @@ class Contriever(nn.Module):
         # transformers==4.18 get_extended_attention_mask: (1 - mask) * -10000 (src/modeling_bert.py:993)
         add_mask = (1.0 - attention_mask.to(torch.float32)) * -10000.0
         live = ops.key_block_live(add_mask)       # all-padding 64-key blocks (queries are padded to text_maxlength): skipped
-        # Padding-compacted encoder (DESIGN.md 3.10, same scheme as FiD._encode_rows): every sequence keeps its 64-row tiles up
+        # Padding-compacted encoder (same scheme as FiD._encode_rows): every sequence keeps its 64-row tiles up
         # to its last live key, packed back to back; projections run over the device-side row count, the attention on the
         # packed rows.  Padded positions never influence live ones and every consumer of the result masks them (mean pooling)
         # or reads position 0 (cls pooling): the returned rows of dropped tiles are 0.

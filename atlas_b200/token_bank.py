@@ -1,4 +1,4 @@
-"""Device-resident reader token bank (SURVEY.md §8f-1).
+"""Device-resident reader token bank.
 
 `Atlas.tokenize_passages` (src/atlas.py:261-280) formats and tokenises bsz x n_context "query + passage" strings of
 ~text_maxlength tokens on the host EVERY step and copies [bsz, n, L] int64 ids + mask to the device; at

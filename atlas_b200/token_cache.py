@@ -1,4 +1,4 @@
-"""Retriever-side passage token cache for index refresh (SURVEY.md §8f-1).
+"""Retriever-side passage token cache for index refresh.
 
 `Atlas.build_index` (src/atlas.py:61-88) formats and tokenises EVERY local passage again on every index refresh
 (`fstr.format(**p)` + a tokenizer call per 512-passage batch, src/atlas.py:69-76): 4 Mi tokenizer calls' worth of host

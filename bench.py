@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py — the driver's measurement contract for atlas_b200 (see DESIGN.md §6).
+"""bench.py — the measurement of atlas_b200's flagship workload.
 
 Metric (BASELINE.json): end-to-end queries/sec of the retrieve-then-read step — Contriever query embedding,
 exact top-40 search over the GPU-resident 768-d fp16 passage bank (BASELINE configs[1]: 4 Mi passages per GPU,
@@ -9,7 +9,7 @@ text_maxlength 384, 32 target tokens) — plus the MIPS scan against the HBM roo
   value         queries/s of the whole job, step inputs already resident in HBM, CUDA events, max over ranks
   e2e           the same step with HOST inputs: pinned token ids are copied H2D and the retrieved ids / scores and the
                 loss are copied D2H inside the timed region
-  roofline      the dominant kernel of the step (tcgen05 GEMM): FLOPs / CUDA-event time, against the measured bf16 peak
+  roofline      the dominant kernel of the step (wgmma GEMM): FLOPs / CUDA-event time, against the measured bf16 peak
   mips          the retrieval kernel alone at its BASELINE batch (256 queries): queries/s, C-ABI e2e with host buffers,
                 and the bank sweep against the measured HBM peak (`mips.roofline`)
   train         supplementary: FiD-base forward + BACKWARD step (the training path's kernels), reader tokens/s
@@ -42,7 +42,7 @@ TOPK = 40
 CPU_SAMPLE_ROWS = 1 << 20   # bounded CPU sample: 1 Mi of the 4 Mi rows (scaled linearly, stated)
 METRIC = "end-to-end queries/sec (retrieve top-40 + FiD-base fwd)"
 N_DOCS, TEXT_LEN, TARGET_LEN, QUERY_TOKENS = 40, 384, 32, 20   # BASELINE configs[3] / finetune_qa defaults
-FID_FLOPS_PER_QUERY = 3.29e12                                   # SURVEY.md §8(d)
+FID_FLOPS_PER_QUERY = 3.29e12                                   # forward FLOPs of one query (encoder 2.83 T, cross-attention K/V projections 0.435 T, rest 0.03 T)
 PASSAGE_TOKENS = 256                                            # token-bank row width (passage part of the reader input)
 
 
@@ -59,6 +59,9 @@ def parse():
     ap.add_argument("--no-xl", action="store_true", help="skip the Atlas-xl training leg (BASELINE configs[4])")
     ap.add_argument("--ref-budget-s", type=float, default=150.0,
                     help="--impl reference: wall-clock budget of the timed CPU steps (each step = one query)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write what the last timed step returned (loss, retrieved ids and scores, "
+                         "reader logits) as DIR/<name>.npy in float32 / float64, at most 64 MB in all")
     ap.add_argument("--profile-step", action="store_true",
                     help="run warm-up + the timed steps inside an NVTX range 'atlas_b200_timed' and exit (for ncu "
                          "--nvtx --nvtx-include 'atlas_b200_timed/'; no JSON line is printed)")
@@ -75,12 +78,12 @@ def peaks(kind="hbm"):
             d = json.load(f)
         if key in d:
             return float(d[key]), f"measured (MEASURED_PEAKS.json {key})"
-    return (6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)") if kind == "hbm" else \
-        (1500.0, "fallback (B200_PROFILING.md dense bf16)")
+    return (3350.0, "fallback (H100 SXM data sheet, 3.35 TB/s)") if kind == "hbm" else \
+        (989.0, "fallback (H100 SXM data sheet, dense bf16)")
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons sampled DURING the timed region (B200_PROFILING.md):
+    """nvidia-smi clocks / throttle reasons sampled DURING the timed region:
     one `nvidia-smi -lms 20` process is started before the region and stopped after it."""
 
     QUERY = ("clocks.sm,clocks.max.sm,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,"
@@ -273,10 +276,10 @@ def workload_config(args):
                              f"id (lengths U[{PASSAGE_TOKENS // 2}, {PASSAGE_TOKENS}]), spliced behind the query tokens "
                              "on the GPU (atlas_b200_splice_tokens); no tokenizer vocabulary offline",
             "padding": "every reader passage is padded to text_maxlength like src/atlas.py:261-270 pads (148 - 276 of 384 positions "
-                       "real); the repo arm encodes each passage's 64-position tiles up to its last real token (same logits / loss, "
-                       "DESIGN.md 3.10) and also reports the step with every padded position encoded (`padded_encoder`)",
+                       "real); the repo arm encodes each passage's 64-position tiles up to its last real token (same logits / loss) "
+                       "and also reports the step with every padded position encoded (`padded_encoder`)",
             "weights": "random init (Contriever-base / T5-v1.1-base shapes), bf16 reader + retriever, fp16 bank",
-            "l2": "bank (6.4 GB) and per-step activations (> 1 GB) exceed the 126 MB L2; no explicit flush"}
+            "l2": "bank (6.4 GB) and per-step activations (> 1 GB) exceed the 50 MB L2; no explicit flush"}
 
 
 def run_reference(args):
@@ -605,7 +608,7 @@ def run_ours(args):
             tok = bank_tokens.splice(gids, TEXT_LEN, rq_ids, rq_lens)
             out = reader(input_ids=tok["input_ids"].view(B, -1), attention_mask=tok["attention_mask"].view(B, -1),
                          decoder_input_ids=dec, labels=labels)
-        return out[0], gids, scores
+        return out[0], gids, scores, out[1]
 
     def step_api():
         """The same step through the module surface train.py / evaluate.py call, HOST inputs and outputs: query strings
@@ -642,7 +645,7 @@ def run_ours(args):
         torch.cuda.nvtx.range_push("atlas_b200_timed")
         e0.record()
         for _ in range(args.steps):
-            loss, gids, _ = step_device()
+            loss, gids, scores, logits = step_device()
         e1.record()
         barrier_sync()
         torch.cuda.nvtx.range_pop()
@@ -650,6 +653,8 @@ def run_ours(args):
         if world > 1:
             dist.destroy_process_group()
         return
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, {"loss": loss, "retrieved_ids": gids, "retrieved_scores": scores, "logits": logits})
     total_ms = max_over_ranks(e0.elapsed_time(e1))
     launches_eager = None
     ms_per_step = total_ms / args.steps
@@ -781,15 +786,7 @@ def run_ours(args):
         return
 
     peak, peak_src = peaks("tensor")
-    gemm_traffic, gemm_traffic_note = None, None
-    tpath = os.path.join(ROOT, "profiles", "r02_gemm_traffic.json")
-    if not os.path.exists(tpath):
-        tpath = os.path.join(ROOT, "profiles", "r01_gemm_traffic.json")
-    if os.path.exists(tpath):     # dram bytes of ONE representative launch from the committed `ncu --set full` capture
-        with open(tpath) as f:
-            tj = json.load(f)
-        gemm_traffic = tj.get("dram_bytes_per_launch")
-        gemm_traffic_note = f"{tj.get('launch')}: algorithmic {tj.get('algorithmic_bytes_per_launch')} B; {tj.get('source')}"
+    gemm_traffic, gemm_traffic_note = None, None    # no stored capture of a launch's DRAM bytes
     g_ms, g_n, g_flops = prof["gemm"]
     a_ms, a_n, a_flops = prof["attention"]
     all_gemm = {"ms_per_step": g_ms, "launches_per_step": g_n, "flops_per_step": g_flops,
@@ -825,7 +822,7 @@ def run_ours(args):
                      "model_flops_utilisation_note": "dense-model FLOPs (every padded position counted) over the step time; "
                                                      "`achieved` / `frac` above count only the rows the GEMMs computed"},
         "encoder": "padding-compacted: each passage keeps its 64-row tiles up to its last real token "
-                   "(FiD._encode_rows, DESIGN.md 3.10); `padded_encoder` = the same step with ATLAS_B200_ENC_PACKED=0"
+                   "(FiD._encode_rows); `padded_encoder` = the same step with ATLAS_B200_ENC_PACKED=0"
                    if _ops._ENC_PACKED else "every padded position (ATLAS_B200_ENC_PACKED=0)",
         "padded_encoder": padded_encoder,
         "e2e": {"value": B * world / (e2e_ms * 1e-3), "unit": "queries/s", "h2d_bytes_per_step": h2d,
@@ -950,7 +947,7 @@ def xl_train_leg(args, atlas_base, index, bank_tokens, dev, world, rank, L, barr
     384) retrieve + reader forward + backward + retriever distillation (`Atlas.forward(train_retriever=True)`,
     gold_score_mode ppmean, src/atlas.py:399-550, dropout 0), per GPU 1 query per step, gradient checkpointing on both
     models, followed at N > 1 by one NCCL all-reduce of the flattened gradients (what DDP does in train.py).  Reader input
-    tokens/s (B * n_docs * text_maxlength per step, SURVEY.md §8d C5's unit) over all ranks."""
+    tokens/s (B * n_docs * text_maxlength per step) over all ranks."""
     import ctypes
 
     import torch
@@ -1031,7 +1028,7 @@ def refresh_leg(args, retriever, index, dev, world, L, barrier_sync, max_over_ra
     """Index refresh (`Atlas.build_index`, src/atlas.py:61-88): one embedder batch of 512 synthetic passages (lengths
     U[64, 192] tokens, padded to the longest like the reference's tokenizer call) through Contriever-base with fp16
     weight copies, pooled rows written straight into bank rows (`Contriever.embed_into`).  Passages/s over all ranks (no
-    communication: every rank rewrites its own shard) and the tensor-roofline fraction with SURVEY.md §8(d)'s FLOPs per
+    communication: every rank rewrites its own shard) and the tensor-roofline fraction with the FLOPs per
     token (169.9 MFLOP + 36 864 L).  Runs last: it overwrites the first 512 rows of the synthetic bank."""
     import torch
 
@@ -1060,7 +1057,7 @@ def refresh_leg(args, retriever, index, dev, world, L, barrier_sync, max_over_ra
     ms = max_over_ranks(e0.elapsed_time(e1)) / steps
     assert bool(torch.isfinite(rows.float()).all()), "non-finite embeddings in the refresh leg"
     flops_dense = nb * lmax * (169.9e6 + 36864.0 * lmax)
-    # the encoder runs on each passage's 64-row tiles up to its last real token (DESIGN.md 3.10): FLOPs of the rows computed
+    # the encoder runs on each passage's 64-row tiles up to its last real token: FLOPs of the rows computed
     from atlas_b200 import ops as _ops
 
     flops = flops_dense
@@ -1083,7 +1080,7 @@ def refresh_leg(args, retriever, index, dev, world, L, barrier_sync, max_over_ra
 def train_leg(args, reader, dev, world, L, barrier_sync, max_over_ranks, steps=3, warmup=2):
     """FiD-base forward + backward (`loss.backward()` through grad_ops.py's kernels; at N > 1 followed by one NCCL
     all-reduce of the flattened gradients, what DDP does in train.py) on `train_batch` queries x 40 passages x 384 tokens
-    per GPU: reader tokens/s (B * n_docs * text_maxlength per step, SURVEY.md §8d C5's unit) and the share of the GEMM /
+    per GPU: reader tokens/s (B * n_docs * text_maxlength per step) and the share of the GEMM /
     attention-backward kernels.  Supplementary to the headline metric (which is the forward step)."""
     import ctypes
 
@@ -1213,11 +1210,7 @@ def mips_leg(args, index, dev, world, rank, L, barrier_sync, max_over_ranks):
     kernel_ms = kms.value / steps
     alg_bytes = args.rows * DIM * 2
     achieved = alg_bytes / (kernel_ms * 1e-3) / 1e9 if kernel_ms > 0 else 0.0
-    traffic = None
-    tpath = os.path.join(ROOT, "profiles", "r01_mips_scan_traffic.json")
-    if os.path.exists(tpath):     # dram bytes of the sweep from the committed `ncu --set full` capture (see profiles/)
-        with open(tpath) as f:
-            traffic = json.load(f).get("dram_bytes_per_search")
+    traffic = None                # no stored capture of the sweep's DRAM bytes
     return {
         "metric": "retrieve queries/sec (exact top-40 search_knn, 256-query batches)", "value": NQ / (ms_per_step * 1e-3),
         "unit": "queries/s", "ms_per_step": ms_per_step, "steps": steps, "queries_per_step": NQ,
@@ -1238,6 +1231,33 @@ def mips_leg(args, index, dev, world, rank, L, barrier_sync, max_over_ranks):
 
 
 _JSON_FD = None
+
+
+DUMP_BUDGET_BYTES = 64 * 1024 * 1024
+
+
+def dump_outputs(out_dir, arrays):
+    """Write the arrays of the last timed step as out_dir/<name>.npy: floating outputs as float32, integer ids as float64
+    (exact below 2^53).  An array that would take the total past DUMP_BUDGET_BYTES is replaced by a fixed, seeded sample of
+    its flattened elements (same positions in every run), stored with the sampled flat indices as <name>_index.npy."""
+    import numpy as np
+    import torch
+
+    os.makedirs(out_dir, exist_ok=True)
+    used = 0
+    for name, t in arrays.items():
+        t = t.detach()
+        a = t.double() if not torch.is_floating_point(t) else t.float()
+        a = a.cpu().numpy()
+        room = DUMP_BUDGET_BYTES - used
+        if a.nbytes > room:
+            n = max(1, room // (a.itemsize + 8))
+            idx = np.sort(np.random.default_rng(0).choice(a.size, size=n, replace=False))
+            np.save(os.path.join(out_dir, f"{name}_index.npy"), idx.astype(np.float64))
+            a = a.reshape(-1)[idx]
+            used += idx.size * 8
+        np.save(os.path.join(out_dir, f"{name}.npy"), a)
+        used += a.nbytes
 
 
 def emit(line):

@@ -1,7 +1,7 @@
 /* atlas_b200 — C ABI of the B200-native retrieve-then-read hot path.
  *
  * The reference (facebookresearch/atlas) is pure Python and has no FFI; its boundary for this path
- * is the Python module surface (SURVEY.md §8b).  This header is the C-ABI layer underneath our
+ * is the Python module surface.  This header is the C-ABI layer underneath our
  * drop-in Python modules (`atlas_b200/index.py` etc.): plain pointers and sizes, no torch types.
  * Every entry point cites the reference code it replaces.
  *
@@ -68,9 +68,8 @@ int atlas_b200_mips_topk(const void* bank, int64_t n, int64_t ld, int32_t is_bf1
                          void* out_scores, int64_t* out_ids, int64_t id_base, int64_t id_stride,
                          int32_t* status, void* workspace, size_t workspace_bytes, void* stream);
 
-/* Selects the scan kernel: 1 (default) = queries resident in TMEM (tcgen05 A-from-TMEM, CTA pairs);
- * 0 = queries streamed through shared memory next to the bank tiles (first-generation kernel, kept for
- * A/B measurements).  Also settable with the environment variable ATLAS_B200_MIPS_KERNEL=ss|ts. */
+/* Kept for ABI compatibility: there is one scan kernel (queries and bank tiles streamed through shared memory);
+ * the mode is ignored. */
 void atlas_b200_mips_set_kernel(int32_t mode);
 
 /* Development aid: when a device buffer of gridDim*8 uint64 is registered, the main TS scan kernel
@@ -108,7 +107,7 @@ int atlas_b200_search_host(const void* bank, int64_t n, int64_t ld, int32_t is_b
                            void* workspace, size_t workspace_bytes, void* stream);
 
 /* --------------------------------------------------------------------------------------------
- * Dense linear layer with a fused epilogue on tcgen05 (csrc/gemm.cu):
+ * Dense linear layer with a fused epilogue on wgmma (csrc/gemm.cu):
  *     C[M, N] = epilogue( A[M, K] . W[N, K]^T )     A, W, C, bias, residual: fp16 (is_bf16 = 0) or bf16
  * W is the nn.Linear weight as stored by torch ([out_features, in_features]).  fp32 accumulation.
  * Replaces cuBLAS GEMM + ATen elementwise kernels behind the Linear layers of the Contriever encoder
@@ -182,7 +181,7 @@ int atlas_b200_decode_argmax(const void* logits, int64_t ld, int32_t V, int64_t*
                              uint8_t* done, int32_t* t_dev, int32_t eos_id, int32_t pad_id, int32_t min_length, int32_t B,
                              int32_t is_bf16, void* stream);
 
-/* Reader-input assembly from a device-resident passage token bank (SURVEY.md 8f-1).  Replaces the per-step host work of
+/* Reader-input assembly from a device-resident passage token bank.  Replaces the per-step host work of
  * Atlas.tokenize_passages (src/atlas.py:261-280: bsz * n_context string formats + tokenizer calls, then H2D of
  * [bsz, n, L] int64 ids + mask):
  *   out_ids[b, j, :]  = (query_ids[b, :query_lens[b]] ++ bank_ids[rows[b*n + j], :bank_lens[..]])[: L-1] ++ [eos_id],
@@ -264,7 +263,7 @@ int atlas_b200_cross_attention_stats(const void* q, int64_t ldq, int32_t q_col0,
                                      float* out_scores, float* out_probs, float* out_norms, int32_t B, int32_t H, int32_t T,
                                      int32_t Lk, float scale, int32_t is_bf16, void* stream);
 
-/* Weight gradient of a Linear layer on tcgen05 (csrc/gemm.cu, MN-major operand descriptors):
+/* Weight gradient of a Linear layer on wgmma (csrc/gemm.cu, MN-major operand descriptors):
  *     dW[N, K] = dY[tokens, N]^T . X[tokens, K]        16-bit operands, fp32 accumulation over the tokens
  * Both activations are read as they lie in memory (no transposes); dW is written in 16 bits like the reference's
  * bf16 gradients (`--precision bf16`, src/model_io.py:94-98).
@@ -364,7 +363,7 @@ int atlas_b200_attention_bwd_train(const void* q, int64_t ldq, int32_t q_col0, c
                                    int32_t Lk, float scale, float causal_value, float dropout_p, uint64_t seed,
                                    uint64_t offset, const uint8_t* key_block_live, int32_t is_bf16, void* stream);
 
-/* Multi-tensor optimiser step and gradient statistics of the training loop (SURVEY.md §8 f3).  The work list is a device
+/* Multi-tensor optimiser step and gradient statistics of the training loop.  The work list is a device
  * table of (tensor index, chunk index) int32 pairs, `chunk_elems` elements per chunk (multiple of 4).
  *   atlas_b200_adamw_fp32copy: src/AdamWFP32Copy.py:79-169 for one param group - per element, on the fp32 master copy:
  *     g = grad * inv_scale; p *= decay; m = lerp(m, g, one_minus_beta1); v = beta2*v + one_minus_beta2*g*g;
@@ -470,7 +469,7 @@ int atlas_b200_expand_packed_tiles(const void* src, int64_t lds, const int32_t* 
 /* Measurement hook for bench.py's roofline: while enabled, every launch of ONE kind of kernel is bracketed
  * with CUDA events on its launching stream:
  *   kind 1  the bank sweep of atlas_b200_mips_topk (work = algorithmic bytes swept)
- *   kind 2  the tcgen05 GEMM of atlas_b200_linear   (work = 2*M*N*K FLOPs)
+ *   kind 2  the wgmma GEMM of atlas_b200_linear   (work = 2*M*N*K FLOPs)
  *   kind 3  the attention kernel                     (work = 4*B*H*Lq*Lk*64 FLOPs)
  *   kind 4  the attention backward kernels           (work = 16*B*H*Lq*Lk*64 FLOPs)
  *   kind 0  off (default).

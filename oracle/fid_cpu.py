@@ -14,7 +14,7 @@ Follows (file:line under /root/reference/src):
   T5DenseGatedGeluDense           modeling_t5.py:272-289    gelu_new(x W0) * (x W1) -> Wo
   T5ForConditionalGeneration.forward  modeling_t5.py:1523-1669   lm_head (untied for v1.1), CE(ignore_index=-100)
   masks: transformers==4.18 get_extended_attention_mask ((1-m)*-10000; causal product for the decoder) and
-         invert_attention_mask ((1-m)*-1e9 in fp32) - SURVEY.md Appendix A items 5, 6.
+         invert_attention_mask ((1-m)*-1e9 in fp32).
   Contriever.forward              retrievers.py:22-60; BertLayerNorm modeling_bert.py:104-114 (UNCENTRED 2nd moment);
   BertSelfAttention               modeling_bert.py:328-366  (1/sqrt(64), additive mask, fp32 softmax); erf-GELU.
 """

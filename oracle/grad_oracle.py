@@ -1,4 +1,4 @@
-"""Gradients of the CPU restatements (oracle/fid_cpu.py) by torch.autograd: the checker for the B200 training path.
+"""Gradients of the CPU restatements (oracle/fid_cpu.py) by torch.autograd: the checker for the GPU training path.
 
 TEST INFRASTRUCTURE (only tests/, smoke() and bench.py's CPU legs may import oracle/).  Pinned against the UNMODIFIED
 reference's own gradients in tests/test_oracle_golden.py (tests/golden/grads_tiny.npz, oracle/make_golden_grads.py):

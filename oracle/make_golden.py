@@ -11,7 +11,7 @@ For every case we record
                               returned passage dicts); tie order is torch.topk's, i.e. unspecified
   canon_ids    [nq,k] int64 - canonical pick: reference fp16 score matrix
                               (`torch.matmul(q.half(), E)`, src/index.py:117) + stable sort by
-                              (score desc, global id asc)            (SURVEY.md §8c)
+                              (score desc, global id asc)           
 Multi-rank cases run the reference under a real `torch.distributed` gloo group on CPU
 (`Tensor.cuda` patched to a no-op: the reference hard-codes `.cuda()` at src/index.py:35).
 """

@@ -6,7 +6,7 @@ TEST / BENCH INFRASTRUCTURE.  `/root/reference` does not exist on the GPU box; `
 `gpu_reference` leg import `oracle/_ref/src/*` there (through `oracle/ref_shims.py`, which only patches the library
 symbols that transformers 5.x / the missing faiss removed - the reference files themselves are byte-identical copies;
 `MANIFEST.json` records their sha256).  The reference has no setup.py, so the base contract's
-`pip install ... /root/reference` does not apply (DESIGN.md §6); this copy is the tier's `oracle/_ref` equivalent.
+`pip install ... /root/reference` does not apply; this copy is the tier's `oracle/_ref` equivalent.
 
 Run in the build container:  python oracle/make_ref.py      (also called by __graft_entry__.build()).
 """

@@ -15,7 +15,7 @@ Restated reference code (numpy, no torch):
                               (`torch.matmul(allqueries.half(), self.embeddings)`: fp16 operands,
                               fp32 accumulation, ONE rounding of the result to fp16)
   * `canonical_topk`       <- `torch.topk(scores, topk, dim=1)`, src/index.py:118, with the tie
-                              order pinned (SURVEY.md §8c): stable sort by (score desc, id asc).
+                              order pinned: stable sort by (score desc, id asc).
   * `search_knn_oracle`    <- `DistributedIndex.search_knn`, src/index.py:122-157, for a world of
                               W ranks holding round-robin shards (src/index_io.py:41).
 """
@@ -104,7 +104,7 @@ def search_knn_oracle(bank, queries_per_rank, k):
 def ids_match_tie_aware(scores_row, ids_a, ids_b):
     """True if two id lists for one query agree at every position whose score is unique in the
     row's top-k and differs from the k-th score (positions where torch.topk's unspecified tie order
-    or the k-boundary cannot matter).  SURVEY.md §8c gate (iii)."""
+    or the k-boundary cannot matter)."""
     s = np.asarray(scores_row, dtype=np.float32)
     ok = True
     for p in range(len(s)):

@@ -6,7 +6,7 @@ produce the committed fixtures under `tests/golden/`.  `/root/reference` does no
 on the GPU box, so nothing in `tests/`, `bench.py` or `__graft_entry__.py` imports this
 module at run time on the GPU; the product package `atlas_b200/` never imports it.
 
-What is patched and why (SURVEY.md Appendix A, verified by running it):
+What is patched and why (verified by running it):
   1. `faiss`, `faiss.contrib.torch_utils` are absent -> stub modules carrying the class
      names that `src/index.py:18-28` evaluates at import time.
   2. `transformers.modeling_utils` lost `apply_chunking_to_forward`,

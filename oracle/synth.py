@@ -5,11 +5,11 @@ TEST/BENCH INFRASTRUCTURE (numpy only, no reference code).  Everything is genera
 that writes `tests/golden/` and the GPU box that replays them build bit-identical inputs;
 each fixture also stores a sha256 of the generated arrays.
 
-Distributions (SURVEY.md §8c/§8d):
+Distributions:
   * "grid"  : clamp(round(8*N(0,1))/8, -4, 4).  Every product is a multiple of 2^-6 and every
               partial sum of 768 products fits in 18 bits, so fp32 accumulation is exact in ANY
               order -> the fp16-rounded score matrix is identical on CPU BLAS, cuBLAS and
-              tcgen05.  This is the bit-exact gate.
+              wgmma.  This is the bit-exact gate.
   * "gauss" : N(0,1)/sqrt(768)-scaled passages and unit-scale queries ("realistic"); scores may
               differ by 1 fp16 ulp between accumulation orders -> tolerance gate, tie-aware ids.
 """

@@ -2,7 +2,7 @@
 generate) against outputs of the UNMODIFIED reference `src.atlas.Atlas` run on CPU in fp32
 (oracle/make_golden_atlas.py -> tests/golden/atlas_tiny.npz), same seeded weights, corpus and fake tokenizers.
 
-The B200 modules compute in 16 bits (fp16 Contriever, bf16 / fp16 FiD), the golden run in fp32 (fp16 for the bank,
+The atlas_b200 modules compute in 16 bits (fp16 Contriever, bf16 / fp16 FiD), the golden run in fp32 (fp16 for the bank,
 as the reference does): every tolerance below is stated next to the reference's own 16-bit drift stored in the golden
 files."""
 import os

@@ -313,7 +313,7 @@ def test_cross_attention_backward(dev, dtype, B, H, T, Lk, split):
 @pytest.mark.parametrize("tokens,N,K", [(1000, 768, 768), (77, 128, 64), (4096, 512, 2048), (30720, 2304, 768),
                                         (5, 64, 256), (129, 2048, 768)])
 def test_wgrad_mn_major_gemm_exact(dev, dtype, tokens, N, K):
-    """dW = dY^T X on the MN-major tcgen05 path: exact-grid inputs (multiples of 1/8 in [-2, 2]) make every partial sum
+    """dW = dY^T X on the MN-major wgmma path: exact-grid inputs (multiples of 1/8 in [-2, 2]) make every partial sum
     exact in fp32 whatever the accumulation order, so the result must equal the fp32 product rounded once - bit for bit,
     and so must the first-generation path (explicit transposes + K-major GEMM)."""
     import os

@@ -4,8 +4,8 @@ reference on CPU (oracle/make_golden_fullsize.py: fp32 outputs plus the referenc
 CPU oracle restatement (oracle/fid_cpu.py, itself pinned to the reference's goldens) where the golden holds a sample.
 
 Accuracy budget: a 16-bit run here may sit as far from the reference's fp32 outputs as the reference's OWN 16-bit run does
-(x 2 on the maximum, x 1.5 on the mean).  The measured numbers are printed (pytest -s) and recorded in DESIGN.md §5;
-north_star's "1e-3 fp16" is below the reference's own fp16 drift at this depth (4.1e-2 on the logits), see DESIGN.md.
+(x 2 on the maximum, x 1.5 on the mean).  The measured numbers are printed (pytest -s); north_star's "1e-3 fp16" is below
+the reference's own fp16 drift at this depth (4.1e-2 on the logits).
 Also here: the untied dual encoder (src/retrievers.py:108-135) against the reference's embeddings and gradient norms."""
 import os
 from types import SimpleNamespace

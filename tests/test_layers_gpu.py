@@ -252,7 +252,7 @@ def test_fid_fp16_overflow_is_clamped_like_the_reference(dev):
 @pytest.mark.parametrize("B,H,T,Lk", [(2, 3, 32, 4000), (1, 12, 7, 15360), (3, 2, 64, 1088), (2, 1, 1, 2048)])
 def test_cross_attention_stream_kernel(dev, dtype, B, H, T, Lk):
     """csrc/attention_stream.cu (few target tokens against the concatenated encoder keys, src/fid.py:298-349): against an fp32
-    restatement, ragged key counts, masked keys, and against the tcgen05 split-KV path where that one applies."""
+    restatement, ragged key counts, masked keys, and against the split-KV path where that one applies."""
     from atlas_b200 import ops
 
     g = torch.Generator().manual_seed(B * 1000 + T)

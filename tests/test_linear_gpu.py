@@ -1,4 +1,4 @@
-"""GPU numerics of the tcgen05 linear layer (csrc/gemm.cu) against a plain PyTorch fp32 reference of the
+"""GPU numerics of the wgmma linear layer (csrc/gemm.cu) against a plain PyTorch fp32 reference of the
 same op (inputs rounded to the 16-bit type first, fp32 math, one rounding of the result).  Tolerance:
 the result must be within 1 ulp(16-bit) + 1e-3*|ref| of the correctly rounded fp32 reference — what a
 different fp32 accumulation order can cost — and bit-exact on exact-grid inputs."""

@@ -1,4 +1,4 @@
-"""CPU: why the padding-compacted encoder (DESIGN.md §3.10) computes what the reference computes - shown on the oracle's restatement
+"""CPU: why the padding-compacted encoder computes what the reference computes - shown on the oracle's restatement
 of the reference's algorithm (oracle/fid_cpu.py, pinned to the unmodified reference's outputs by tests/test_oracle_golden.py).
 
 1. A passage's encoder states at the positions of its kept 64-position tiles do not depend on the padded positions behind them:

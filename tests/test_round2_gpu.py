@@ -1,4 +1,4 @@
-"""GPU tests of the round-2 additions: the device token bank + splice kernel (SURVEY.md §8f-1), the KV-cached greedy decode
+"""GPU tests of the round-2 additions: the device token bank + splice kernel, the KV-cached greedy decode
 (§8f-2), the in-place 16-bit weight cache (ADVICE r1), the sync-free search entry points."""
 import numpy as np
 import pytest

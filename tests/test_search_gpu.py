@@ -170,7 +170,7 @@ def test_merge_kernel_matches_oracle(dev):
 
 
 def test_index_module_drop_in(dev, tmp_path):
-    """The reference-shaped surface (SURVEY.md §8b): slice-assign into `embeddings`, search, save/load."""
+    """The reference-shaped surface: slice-assign into `embeddings`, search, save/load."""
     from atlas_b200.index import DistributedIndex
 
     g = load_golden("c1_grid")
@@ -215,7 +215,7 @@ def test_bf16_bank_variant(dev):
 
 def test_full_size_properties(dev):
     """BASELINE.json configs[1]: 4 Mi x 768 fp16 bank, 256 queries, top-40.  Exact-grid bank so that
-    cuBLAS and tcgen05 accumulation agree bit-for-bit; checked against torch on the GPU in chunks."""
+    cuBLAS and wgmma accumulation agree bit-for-bit; checked against torch on the GPU in chunks."""
     from atlas_b200 import ops
 
     n, nq, k = 4 * 1024 * 1024, 256, 40
@@ -246,7 +246,7 @@ def test_full_size_properties(dev):
     assert torch.all((full > s[sub, -1:]).sum(dim=1) <= k - 1)
 
 
-@pytest.mark.skipif(torch.cuda.device_count() < 2, reason="needs >= 2 GPUs (gpurun --gpus 2)")
+@pytest.mark.skipif(torch.cuda.device_count() < 2, reason="needs >= 2 GPUs")
 def test_distributed_search_nccl(tmp_path):
     """NCCL world of 2: sharded bank, query all-gather, packed result all-gather, merge kernel."""
     import subprocess

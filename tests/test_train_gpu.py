@@ -7,7 +7,7 @@ Accuracy budget: the golden also holds the reference's own bf16-parameter run; i
 norm (projection) from its fp32 run.  The kernels compute in 16 bits with fp32 accumulation, so the bars are 3 % on the
 norm, 15 % of the norm on the projection (a random projection of an error vector e is ~ N(0, |e|): over the ~50
 parameters of a model the largest |z| is ~2.5, so this corresponds to |e| / |g| ~ 6 %) and 8 % relative L2 per tensor
-(bf16; half of each for fp16, which has 3 more mantissa bits).  Measured on B200: see tools/perf_train.py diag."""
+(bf16; half of each for fp16, which has 3 more mantissa bits)."""
 import os
 
 import numpy as np

@@ -52,7 +52,7 @@ def run_case(n, nq, k, dist="grid", bseed=1, qseed=2, exhaustive=False, verbose=
 from atlas_b200._lib import lib
 MODE = int(sys.argv[1]) if len(sys.argv) > 1 else 1
 lib().atlas_b200_mips_set_kernel(MODE)
-print("kernel mode", MODE, "(1 = TS/TMEM-resident queries, 0 = SS)", flush=True)
+print("kernel mode", MODE, "(ignored: one scan kernel)", flush=True)
 results = {}
 try:
     results["single_small"] = run_case(128, 4, 128)

@@ -1,4 +1,4 @@
-"""Training-step diagnostics on one B200: (1) per-parameter relative L2 error of the kernels' gradients against the CPU
+"""Training-step diagnostics on one GPU: (1) per-parameter relative L2 error of the kernels' gradients against the CPU
 gradient oracle on the tiny models, (2) FiD-base forward + backward time at n_context 40 x 384 tokens with the share of
 the GEMM / attention-backward kernels, (3) single-op timings of the backward kernels at FiD-base shapes.
     python tools/perf_train.py [diag] [step] [ops]"""

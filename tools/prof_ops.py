@@ -145,4 +145,4 @@ elif what == "wgrad":
     dy = torch.randn(M, N, device=dev).bfloat16() * 0.1
     fn = lambda: ops.linear_wgrad(dy, x)
     ms = timed(fn, reps)
-    print(f"wgrad tokens={M} N={N} K={K} (MN-major tcgen05): {ms:.3f} ms = {2 * M * N * K / ms / 1e9:.0f} TFLOP/s")
+    print(f"wgrad tokens={M} N={N} K={K} (MN-major wgmma): {ms:.3f} ms = {2 * M * N * K / ms / 1e9:.0f} TFLOP/s")
