@@ -184,6 +184,17 @@ def lib():
     L.atlas_b200_attention_packed.argtypes = [vp, i64, i32, i32, i32, vp, i64, vp, vp, vp, vp, vp, i32, i32, i32, f32, i32, vp]
     L.atlas_b200_expand_packed_tiles.restype = c.c_int
     L.atlas_b200_expand_packed_tiles.argtypes = [vp, i64, vp, i32, vp, i64, i32, vp]
+    L.atlas_b200_pq_workspace_bytes.restype = c.c_size_t
+    L.atlas_b200_pq_workspace_bytes.argtypes = [i32, i64, i32, i32, i32]
+    L.atlas_b200_pq_train.restype = c.c_int
+    L.atlas_b200_pq_train.argtypes = [vp, i64, i32, i32, i32, vp, vp, vp, c.c_size_t, vp]
+    L.atlas_b200_pq_encode.restype = c.c_int
+    L.atlas_b200_pq_encode.argtypes = [vp, i64, i32, vp, vp, i32, vp, vp, vp, c.c_size_t, vp]
+    L.atlas_b200_pq_topk.restype = c.c_int
+    L.atlas_b200_pq_topk.argtypes = [vp, vp, i64, i32, vp, vp, i32, vp, i32, i32, vp, vp, i64, i64, vp, vp, c.c_size_t, vp]
+    L.atlas_b200_pq_topk_exhaustive.restype = c.c_int
+    L.atlas_b200_pq_topk_exhaustive.argtypes = [vp, vp, i64, i32, vp, vp, i32, vp, i32, i32, vp, vp, i64, i64, vp, c.c_size_t,
+                                                vp]
     _lib = L
     return L
 
@@ -249,6 +260,11 @@ EXPORTED_SYMBOLS = [
     "atlas_b200_linear_rows",
     "atlas_b200_attention_packed",
     "atlas_b200_expand_packed_tiles",
+    "atlas_b200_pq_workspace_bytes",
+    "atlas_b200_pq_train",
+    "atlas_b200_pq_encode",
+    "atlas_b200_pq_topk",
+    "atlas_b200_pq_topk_exhaustive",
 ]
 
 

@@ -118,7 +118,9 @@ class Atlas(nn.Module):
     @torch.no_grad()
     def build_index(self, index, passages, gpu_embedder_batch_size, logger=None):
         """(Re)embed the local passage shard into the bank IN PLACE (src/atlas.py:61-88).  No communication:
-        every rank rewrites its own rows; one barrier at the end like the reference."""
+        every rank rewrites its own rows; one barrier at the end like the reference.
+        An index with host-resident rows (`is_in_gpu = False`, DistributedFAISSIndex) gets every batch embedded into one
+        of two device staging buffers and copied to its rows asynchronously; it is then marked stale and retrained."""
         tower = self._passage_tower()
         bank = getattr(index, "_bank", None)
         if bank is None or not hasattr(tower, "embed_into"):
@@ -136,6 +138,9 @@ class Atlas(nn.Module):
         cache = self._token_cache if (use_cache and self._token_cache_key == key and self._token_cache is not None
                                       and self._token_cache.complete) else None
         record = None
+        host = not getattr(index, "is_in_gpu", True)
+        stage = [torch.empty((gpu_embedder_batch_size, EMBEDDINGS_DIM), dtype=torch.float16, device=_device())
+                 for _ in range(2)] if host else None
         if use_cache and cache is None:
             record = token_cache.RetrieverTokenCache(len(passages), max_len, device=getattr(self.opt, "token_cache_device", "cpu"))
         for i in range(n_batch):
@@ -150,13 +155,18 @@ class Atlas(nn.Module):
                 if record is not None:
                     record.append(enc["input_ids"], enc["attention_mask"])
                 enc = _to_cuda(enc)
-            rows = bank[total:total + (b - a)]
+            rows = stage[i & 1][:b - a] if host else bank[total:total + (b - a)]
             tower.embed_into(enc["input_ids"], enc["attention_mask"], rows, dtype=torch.float16)
+            if host:    # stream-ordered: the staging buffer is rewritten two batches later, after this copy
+                bank[total:total + (b - a)].copy_(rows, non_blocking=True)
             total += b - a
             if logger is not None and i % 500 == 0 and i > 0:
                 logger.info(f"Number of passages encoded: {total}")
         if record is not None and record.complete:
             self._token_cache, self._token_cache_key = record, key
+        if host:
+            torch.cuda.current_stream().synchronize()
+            index.mark_stale()
         dist_utils.barrier()
         if logger is not None:
             logger.info(f"{total} passages encoded on process: {dist_utils.get_rank()}")

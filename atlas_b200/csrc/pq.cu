@@ -1,0 +1,844 @@
+// Product-quantized passage index (`--index_mode faiss`, types pq and ivfpq) for sm_90a.
+//
+// Replaces faiss's IndexPQ / GpuIndexIVFPQ behind `DistributedFAISSIndex` (src/index.py:163-381):
+//   pq     a row x [768] is stored as M one-byte codes; code m is the nearest (L2) of 256 centroids of the m-th
+//          sub-vector x[m*dsub, (m+1)*dsub), dsub = 768 / M.  score(q, x) = sum_m <q_m, cb_m[code_m]>.
+//   ivfpq  n_list coarse centroids (inner-product assignment); the residual x - c_list is product-quantized.
+//          score(q, x) = sum_m <q_m, cb_m[code_m]> + <q, c_list>.  The reference probes every list
+//          (nprobe = n_list, src/index.py:212,269), so the search is a full scan of these scores.
+//
+// Training (one call, both quantizers): faiss's k-means defaults - the caller passes a training sample in a seeded random
+// order (<= 256 points per centroid), the first k rows are the initial centroids, `iters` Lloyd iterations, an empty
+// cluster is re-seeded by splitting the largest one with a symmetric 1/1024 perturbation.  Deterministic: assignments are
+// argmin / argmax with the lowest index on ties, centroid sums run over the members in sample order (no float atomics).
+//   coarse assignment  the wgmma GEMM atlas_b200_linear (fp16 rows x fp16 copy of the centroids) + a row argmax
+//   PQ assignment      ||c||^2 - 2 <r, c> in fp32 on CUDA cores (pq_subdot_kernel + pq_argmin_kernel), residuals in fp32
+//
+// Search per block of <= 256 queries: fp32 lookup tables LUT[q][m][256] (and coarse terms T[q][list] for ivfpq) from the
+// fp16 queries, then mips.cu's exact top-k pipeline on the scores of a code sweep:
+//   sample sweep -> bound (mips_select_kernel) -> full sweep with the bound -> select + emit, `status` on overflow,
+//   and the chunked exhaustive variant.  Scores accumulate in fp32 over m = 0..M-1, then + T, and are rounded ONCE to fp16.
+// Scan kernel: one row per thread, QPC queries per CTA whose LUTs (and coarse terms) sit in shared memory for the whole
+// sweep; a row's codes are read once per query group.
+#include "mips_select.cuh"
+
+#include <math.h>
+
+namespace pq {
+
+constexpr int DIM = ATLAS_B200_EMBEDDINGS_DIM;
+constexpr int KSUB = 256;             // 8-bit codes
+constexpr int QBLOCK = 256;           // queries per select block (mips.cu's candidate layout)
+constexpr int PQ_TRAIN_MAX = 256 * KSUB;
+constexpr int SCAN_THREADS = 512;     // rows per scan tile
+constexpr int SCAN_SMEM_MAX = 200 * 1024;
+constexpr size_t CHUNK_BUDGET = 128ull << 20;   // per-chunk scratch of training / encoding
+constexpr float SPLIT_EPS = 1.0f / 1024.0f;
+
+inline bool valid_m(int M) { return M >= 1 && DIM % M == 0 && DIM / M >= 8; }
+inline int pad8(int x) { return (x + 7) / 8 * 8; }
+
+// ---------------------------------------------------------------------------------------------
+// elementwise helpers
+// ---------------------------------------------------------------------------------------------
+// out[i, :] = float(x[i, :]) - (coarse ? coarse[assign[i], :] : 0)
+__global__ void pq_residual_kernel(const __half* __restrict__ x, int64_t n, const float* __restrict__ coarse,
+                                   const int32_t* __restrict__ assign, float* __restrict__ out) {
+    const int64_t total = n * DIM;
+    for (int64_t e = blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x; e < total;
+         e += static_cast<int64_t>(gridDim.x) * blockDim.x) {
+        const int64_t i = e / DIM;
+        const int d = static_cast<int>(e - i * DIM);
+        float v = __half2float(x[e]);
+        if (coarse) v -= coarse[static_cast<int64_t>(assign[i]) * DIM + d];
+        out[e] = v;
+    }
+}
+
+// dst[r, :] = src[r, :] for r < rows (fp32 rows of width `width`, source stride lds, destination stride ldd)
+__global__ void pq_copy_rows_kernel(const float* __restrict__ src, int64_t lds, float* __restrict__ dst, int64_t ldd,
+                                    int rows, int width, int src_col_step, int64_t dst_block_step) {
+    // grid.y = block m: dst block m (dst + m * dst_block_step) takes columns [m * src_col_step, + width) of src
+    const int m = blockIdx.y;
+    for (int e = blockIdx.x * blockDim.x + threadIdx.x; e < rows * width; e += gridDim.x * blockDim.x) {
+        const int r = e / width, d = e - r * width;
+        dst[m * dst_block_step + static_cast<int64_t>(r) * ldd + d] = src[static_cast<int64_t>(r) * lds + m * src_col_step + d];
+    }
+}
+
+__global__ void pq_half_to_float_kernel(const __half* __restrict__ x, int64_t count, float* __restrict__ out) {
+    for (int64_t e = blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x; e < count;
+         e += static_cast<int64_t>(gridDim.x) * blockDim.x)
+        out[e] = __half2float(x[e]);
+}
+
+// norms[b] = sum_d c[b, d]^2 over nb rows of width D
+__global__ void pq_norms_kernel(const float* __restrict__ c, int nb, int D, float* __restrict__ norms) {
+    const int b = blockIdx.x * blockDim.x + threadIdx.x;
+    if (b >= nb) return;
+    float s = 0.f;
+    for (int d = 0; d < D; ++d) s = fmaf(c[static_cast<int64_t>(b) * D + d], c[static_cast<int64_t>(b) * D + d], s);
+    norms[b] = s;
+}
+
+// ---------------------------------------------------------------------------------------------
+// out[i][m][j] = sum_{d < dsub} A[i, m*dsub + d] * B[m][j][d]   (fp32, d ascending, fmaf)
+// 64 x 64 output tile per CTA, 4 x 4 per thread.  Serves the LUTs (B = codebooks), the coarse terms (M = 1, B = centroids)
+// and the PQ distances of training / encoding.
+// ---------------------------------------------------------------------------------------------
+constexpr int SD_T = 64, SD_KC = 16;
+
+__global__ void __launch_bounds__(256) pq_subdot_kernel(const float* __restrict__ A, int64_t lda, int rows,
+                                                        const float* __restrict__ B, int nb, int dsub, int M,
+                                                        float* __restrict__ out) {
+    __shared__ float As[SD_KC][SD_T];
+    __shared__ float Bs[SD_KC][SD_T + 1];
+    const int m = blockIdx.z;
+    const int i0 = blockIdx.y * SD_T, j0 = blockIdx.x * SD_T;
+    const int tx = threadIdx.x & 15, ty = threadIdx.x >> 4;
+    const float* Bm = B + static_cast<int64_t>(m) * nb * dsub;
+    float acc[4][4];
+#pragma unroll
+    for (int r = 0; r < 4; ++r)
+#pragma unroll
+        for (int c = 0; c < 4; ++c) acc[r][c] = 0.f;
+    for (int d0 = 0; d0 < dsub; d0 += SD_KC) {
+        for (int e = threadIdx.x; e < SD_T * SD_KC; e += 256) {
+            const int r = e / SD_KC, kk = e % SD_KC;
+            const int d = d0 + kk;
+            const int i = i0 + r, j = j0 + r;
+            As[kk][r] = (i < rows && d < dsub) ? A[static_cast<int64_t>(i) * lda + m * dsub + d] : 0.f;
+            Bs[kk][r] = (j < nb && d < dsub) ? Bm[static_cast<int64_t>(j) * dsub + d] : 0.f;
+        }
+        __syncthreads();
+        const int kmax = min(SD_KC, dsub - d0);
+        for (int kk = 0; kk < kmax; ++kk) {
+            float a[4], b[4];
+#pragma unroll
+            for (int r = 0; r < 4; ++r) a[r] = As[kk][ty + 16 * r];
+#pragma unroll
+            for (int c = 0; c < 4; ++c) b[c] = Bs[kk][tx + 16 * c];
+#pragma unroll
+            for (int r = 0; r < 4; ++r)
+#pragma unroll
+                for (int c = 0; c < 4; ++c) acc[r][c] = fmaf(a[r], b[c], acc[r][c]);
+        }
+        __syncthreads();
+    }
+#pragma unroll
+    for (int r = 0; r < 4; ++r) {
+        const int i = i0 + ty + 16 * r;
+        if (i >= rows) continue;
+#pragma unroll
+        for (int c = 0; c < 4; ++c) {
+            const int j = j0 + tx + 16 * c;
+            if (j < nb) out[(static_cast<int64_t>(i) * M + m) * nb + j] = acc[r][c];
+        }
+    }
+}
+
+// codes[i, m] = argmin_j (norms[m][j] - 2 dots[i][m][j]), lowest j on ties.  One warp per (i, m), grid-stride.
+__global__ void pq_argmin_kernel(const float* __restrict__ dots, const float* __restrict__ norms, int64_t rows, int M,
+                                 uint8_t* __restrict__ codes) {
+    const int lane = threadIdx.x & 31;
+    const int64_t warps = (static_cast<int64_t>(gridDim.x) * blockDim.x) >> 5;
+    for (int64_t w = (blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x) >> 5; w < rows * M; w += warps) {
+        const int m = static_cast<int>(w % M);
+        const float* dv = dots + w * KSUB;
+        float best = INFINITY;
+        int bj = KSUB;
+#pragma unroll
+        for (int t = 0; t < KSUB / 32; ++t) {
+            const int j = lane + 32 * t;
+            const float v = norms[m * KSUB + j] - 2.0f * dv[j];
+            if (v < best) { best = v; bj = j; }
+        }
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) {
+            const float ob = __shfl_xor_sync(0xffffffffu, best, o);
+            const int oj = __shfl_xor_sync(0xffffffffu, bj, o);
+            if (ob < best || (ob == best && oj < bj)) { best = ob; bj = oj; }
+        }
+        if (lane == 0) codes[w] = static_cast<uint8_t>(bj < KSUB ? bj : 0);
+    }
+}
+
+// assign[i] = argmax_{l < n_list} scores[i, l] (16-bit GEMM output, row stride ld), lowest l on ties; one warp per row.
+// Optionally also writes the list id in its storage type (uint16 when n_list <= 65535, else int32).  Grid-stride.
+__global__ void pq_argmax_rows_kernel(const __half* __restrict__ scores, int64_t ld, int64_t rows, int n_list,
+                                      int32_t* __restrict__ assign, void* __restrict__ lists, int list_u16) {
+    const int lane = threadIdx.x & 31;
+    const int64_t warps = (static_cast<int64_t>(gridDim.x) * blockDim.x) >> 5;
+    for (int64_t i = (blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x) >> 5; i < rows; i += warps) {
+        const __half* s = scores + i * ld;
+        float best = -INFINITY;
+        int bl = n_list;
+        for (int l = lane; l < n_list; l += 32) {
+            const float v = __half2float(s[l]);
+            if (bl == n_list || v > best) { best = v; bl = l; }
+        }
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) {
+            const float ob = __shfl_xor_sync(0xffffffffu, best, o);
+            const int ol = __shfl_xor_sync(0xffffffffu, bl, o);
+            if (ol < n_list && (bl >= n_list || ob > best || (ob == best && ol < bl))) { best = ob; bl = ol; }
+        }
+        if (lane == 0) {
+            if (bl >= n_list) bl = 0;
+            if (assign) assign[i] = bl;
+            if (lists) {
+                if (list_u16) static_cast<uint16_t*>(lists)[i] = static_cast<uint16_t>(bl);
+                else static_cast<int32_t*>(lists)[i] = bl;
+            }
+        }
+    }
+}
+
+// ---------------------------------------------------------------------------------------------
+// k-means update: one CTA per (cluster c, block m).  Members are collected in sample order 256 rows at a time and summed
+// in that order, so the centroids are bitwise reproducible.  Empty clusters keep their centroid (split below).
+//   X rows of width D at column m * D (row stride ldx); assign[i * lda + m] = cluster of row i in block m.
+// ---------------------------------------------------------------------------------------------
+template <typename XT, typename AT>
+__global__ void __launch_bounds__(256) pq_update_kernel(const XT* __restrict__ X, int64_t ldx, const AT* __restrict__ assign,
+                                                        int lda, int S, int K, int D, float* __restrict__ cent,
+                                                        int32_t* __restrict__ counts) {
+    __shared__ int32_t s_idx[256];
+    __shared__ int32_t s_warp[8];
+    const int c = blockIdx.x, m = blockIdx.y;
+    const int t = threadIdx.x, lane = t & 31, w = t >> 5;
+    constexpr int PER = (DIM + 255) / 256;
+    float acc[PER];
+#pragma unroll
+    for (int r = 0; r < PER; ++r) acc[r] = 0.f;
+    int cnt = 0;
+    for (int base = 0; base < S; base += 256) {
+        const int i = base + t;
+        const bool flag = i < S && static_cast<int>(assign[static_cast<int64_t>(i) * lda + m]) == c;
+        const uint32_t bal = __ballot_sync(0xffffffffu, flag);
+        if (lane == 0) s_warp[w] = __popc(bal);
+        __syncthreads();
+        int off = 0, tot = 0;
+#pragma unroll
+        for (int w2 = 0; w2 < 8; ++w2) {
+            off += w2 < w ? s_warp[w2] : 0;
+            tot += s_warp[w2];
+        }
+        if (flag) s_idx[off + __popc(bal & ((1u << lane) - 1u))] = i;
+        __syncthreads();
+        for (int j = 0; j < tot; ++j) {
+            const XT* row = X + static_cast<int64_t>(s_idx[j]) * ldx + static_cast<int64_t>(m) * D;
+#pragma unroll
+            for (int r = 0; r < PER; ++r) {
+                const int d = t + 256 * r;
+                if (d < D) acc[r] += static_cast<float>(row[d]);
+            }
+        }
+        cnt += tot;
+        __syncthreads();
+    }
+    float* cc = cent + (static_cast<int64_t>(m) * K + c) * D;
+    if (cnt > 0) {
+        const float inv = 1.0f / static_cast<float>(cnt);
+#pragma unroll
+        for (int r = 0; r < PER; ++r) {
+            const int d = t + 256 * r;
+            if (d < D) cc[d] = acc[r] * inv;
+        }
+    }
+    if (t == 0) counts[static_cast<int64_t>(m) * K + c] = cnt;
+}
+
+// Empty clusters of block m = blockIdx.x, in index order: copy the currently largest cluster (lowest index on ties) with a
+// symmetric perturbation (even dims *(1 + eps) / *(1 - eps), odd dims the other way round) and split its count.
+__global__ void __launch_bounds__(256) pq_split_kernel(float* __restrict__ cent, int32_t* __restrict__ counts, int K, int D) {
+    __shared__ int32_t s_best[256], s_bidx[256];
+    const int m = blockIdx.x, t = threadIdx.x;
+    float* cm = cent + static_cast<int64_t>(m) * K * D;
+    int32_t* nm = counts + static_cast<int64_t>(m) * K;
+    for (int c = 0; c < K; ++c) {
+        __syncthreads();
+        if (nm[c] != 0) continue;
+        int best = -1, bidx = K;
+        for (int j = t; j < K; j += 256)
+            if (nm[j] > best) { best = nm[j]; bidx = j; }
+        s_best[t] = best;
+        s_bidx[t] = bidx;
+        __syncthreads();
+        for (int o = 128; o > 0; o >>= 1) {
+            if (t < o) {
+                const int ob = s_best[t + o], oi = s_bidx[t + o];
+                if (ob > s_best[t] || (ob == s_best[t] && oi < s_bidx[t])) { s_best[t] = ob; s_bidx[t] = oi; }
+            }
+            __syncthreads();
+        }
+        const int cj = s_bidx[0];
+        if (cj >= K || s_best[0] <= 0) continue;
+        for (int d = t; d < D; d += 256) {
+            const float v = cm[static_cast<int64_t>(cj) * D + d];
+            const float up = v * (1.0f + SPLIT_EPS), dn = v * (1.0f - SPLIT_EPS);
+            cm[static_cast<int64_t>(c) * D + d] = (d % 2 == 0) ? up : dn;
+            cm[static_cast<int64_t>(cj) * D + d] = (d % 2 == 0) ? dn : up;
+        }
+        __syncthreads();
+        if (t == 0) {
+            const int half = nm[cj] / 2;
+            nm[c] = half;
+            nm[cj] -= half;
+        }
+    }
+}
+
+// ---------------------------------------------------------------------------------------------
+// scan: one row per thread; LUTs (+ coarse terms) of QPC queries in shared memory; candidates in mips.cu's format
+// ---------------------------------------------------------------------------------------------
+struct ScanParams {
+    const uint8_t* codes;    // [n, M]
+    const void* lists;       // [n] uint16 / int32 (ivfpq) or nullptr (pq)
+    int list_u16;
+    int n_rows;
+    int M;
+    const float* lut;        // [QBLOCK][M][256]
+    const float* cterm;      // [QBLOCK][n_list] or nullptr
+    int n_list;
+    int cterm_smem;          // coarse terms staged in shared memory
+    int nq;                  // valid queries in this block
+    int tile_begin, tile_step, num_tiles;
+    const float* bound;
+    uint32_t* count;
+    uint64_t* cand;
+    uint32_t capq;
+};
+
+template <int QPC>
+__global__ void __launch_bounds__(SCAN_THREADS) pq_scan_kernel(const ScanParams p) {
+    extern __shared__ float s_tab[];
+    __shared__ float s_bnd[QPC];
+    const int t = threadIdx.x, lane = t & 31;
+    const int q0 = blockIdx.y * QPC;
+    const int nqg = min(QPC, p.nq - q0);
+    const int M = p.M;
+    const int lut_q = M * KSUB;
+    for (int e = t; e < nqg * lut_q; e += SCAN_THREADS) s_tab[e] = p.lut[static_cast<int64_t>(q0) * lut_q + e];
+    float* s_ct = s_tab + QPC * lut_q;
+    if (p.cterm && p.cterm_smem)
+        for (int e = t; e < nqg * p.n_list; e += SCAN_THREADS) s_ct[e] = p.cterm[static_cast<int64_t>(q0) * p.n_list + e];
+    if (t < QPC) s_bnd[t] = t < nqg ? p.bound[q0 + t] : INFINITY;
+    __syncthreads();
+
+    for (int it = blockIdx.x; it < p.num_tiles; it += gridDim.x) {
+        const int tile = p.tile_begin + it * p.tile_step;
+        const int row = tile * SCAN_THREADS + t;
+        const bool live = row < p.n_rows;
+        float acc[QPC];
+#pragma unroll
+        for (int q = 0; q < QPC; ++q) acc[q] = 0.f;
+        if (live) {
+            const uint8_t* c = p.codes + static_cast<int64_t>(row) * M;
+            if ((M & 3) == 0) {
+                const uint32_t* cw = reinterpret_cast<const uint32_t*>(c);
+                for (int wi = 0; wi < M / 4; ++wi) {
+                    const uint32_t word = __ldg(cw + wi);
+#pragma unroll
+                    for (int b = 0; b < 4; ++b) {
+                        const int off = (4 * wi + b) * KSUB + ((word >> (8 * b)) & 0xFFu);
+#pragma unroll
+                        for (int q = 0; q < QPC; ++q) acc[q] += s_tab[q * lut_q + off];
+                    }
+                }
+            } else {
+                for (int m = 0; m < M; ++m) {
+                    const int off = m * KSUB + __ldg(c + m);
+#pragma unroll
+                    for (int q = 0; q < QPC; ++q) acc[q] += s_tab[q * lut_q + off];
+                }
+            }
+            if (p.cterm) {
+                const int l = p.list_u16 ? static_cast<int>(static_cast<const uint16_t*>(p.lists)[row])
+                                         : static_cast<const int32_t*>(p.lists)[row];
+#pragma unroll
+                for (int q = 0; q < QPC; ++q)
+                    if (q < nqg)
+                        acc[q] += p.cterm_smem ? s_ct[q * p.n_list + l]
+                                               : p.cterm[static_cast<int64_t>(q0 + q) * p.n_list + l];
+            }
+        }
+#pragma unroll
+        for (int q = 0; q < QPC; ++q) {
+            if (q >= nqg) break;
+            const bool pass = live && acc[q] >= s_bnd[q];
+            const uint32_t bal = __ballot_sync(0xffffffffu, pass);
+            if (bal == 0) continue;
+            const int leader = __ffs(bal) - 1;
+            uint32_t base = 0;
+            if (lane == leader) base = atomicAdd(&p.count[q0 + q], static_cast<uint32_t>(__popc(bal)));
+            base = __shfl_sync(0xffffffffu, base, leader);
+            if (pass) {
+                const uint32_t pos = base + __popc(bal & ((1u << lane) - 1u));
+                if (pos < p.capq)
+                    p.cand[static_cast<size_t>(q0 + q) * p.capq + pos] =
+                        mips::pack_candidate(mips::bits_to_key(mips::round_to_bits<false>(acc[q])), static_cast<uint32_t>(row));
+            }
+        }
+    }
+}
+
+__global__ void pq_prep_kernel(uint32_t* __restrict__ count, float* __restrict__ bound) {
+    if (threadIdx.x < QBLOCK) {
+        count[threadIdx.x] = 0;
+        bound[threadIdx.x] = -INFINITY;
+    }
+}
+
+// ---------------------------------------------------------------------------------------------
+// host side
+// ---------------------------------------------------------------------------------------------
+static int grid_1d(int64_t work, int threads) {
+    int64_t b = (work + threads - 1) / threads;
+    if (b > 8192) b = 8192;
+    return static_cast<int>(b < 1 ? 1 : b);
+}
+
+struct Carver {
+    uint8_t* base;
+    size_t off = 0;
+    template <typename T>
+    T* take(size_t count) {
+        const size_t o = off;
+        off = abh::align_up(off + count * sizeof(T), 256);
+        return base ? reinterpret_cast<T*>(base + o) : nullptr;
+    }
+};
+
+// rows per chunk of training / encoding: GEMM scores + assignment + residuals + PQ distances of one chunk in the budget
+static int64_t chunk_rows(int M, int n_list) {
+    const size_t per_row = static_cast<size_t>(M) * KSUB * 4 + static_cast<size_t>(pad8(n_list)) * 2 + DIM * 4 + 4;
+    int64_t r = static_cast<int64_t>(CHUNK_BUDGET / per_row);
+    if (r > 65536) r = 65536;
+    r = r / 64 * 64;
+    return r < 64 ? 64 : r;
+}
+
+struct ChunkWs {
+    __half* gemm;      // [R][pad8(n_list)]
+    int32_t* assign;   // [R]
+    float* resid;      // [R][768]
+    float* dots;       // [R][M][256]
+    __half* coarse16;  // [pad8(n_list)][768]
+    float* norms;      // [M][256]
+};
+
+static void carve_chunk(Carver& cv, ChunkWs& w, int M, int n_list) {
+    const int64_t R = chunk_rows(M, n_list);
+    const int nlp = pad8(n_list);
+    w.gemm = cv.take<__half>(n_list > 0 ? static_cast<size_t>(R) * nlp : 0);
+    w.assign = cv.take<int32_t>(R);
+    w.resid = cv.take<float>(static_cast<size_t>(R) * DIM);
+    w.dots = cv.take<float>(static_cast<size_t>(R) * M * KSUB);
+    w.coarse16 = cv.take<__half>(static_cast<size_t>(nlp) * DIM);
+    w.norms = cv.take<float>(static_cast<size_t>(M) * KSUB);
+}
+
+static size_t train_bytes(int64_t S, int M, int n_list, ChunkWs* w, float** resid_all, uint8_t** codes_t, int32_t** counts,
+                          int32_t** assign_all, void* base) {
+    Carver cv{static_cast<uint8_t*>(base)};
+    ChunkWs tmp;
+    carve_chunk(cv, w ? *w : tmp, M, n_list);
+    const int64_t sp = S < PQ_TRAIN_MAX ? S : PQ_TRAIN_MAX;
+    float* r = cv.take<float>(static_cast<size_t>(sp) * DIM);
+    uint8_t* c = cv.take<uint8_t>(static_cast<size_t>(sp) * M);
+    int32_t* n = cv.take<int32_t>(static_cast<size_t>(M) * KSUB > static_cast<size_t>(n_list) ? static_cast<size_t>(M) * KSUB
+                                                                                            : static_cast<size_t>(n_list));
+    int32_t* a = cv.take<int32_t>(static_cast<size_t>(S));
+    if (resid_all) *resid_all = r;
+    if (codes_t) *codes_t = c;
+    if (counts) *counts = n;
+    if (assign_all) *assign_all = a;
+    return cv.off;
+}
+
+static size_t encode_bytes(int M, int n_list, ChunkWs* w, void* base) {
+    Carver cv{static_cast<uint8_t*>(base)};
+    ChunkWs tmp;
+    carve_chunk(cv, w ? *w : tmp, M, n_list);
+    return cv.off;
+}
+
+struct SearchWs {
+    uint32_t* count;
+    float* bound;
+    uint64_t* cand;
+    uint32_t capq;
+    float* qf32;   // [QBLOCK][768]
+    float* lut;    // [QBLOCK][M][256]
+    float* cterm;  // [QBLOCK][n_list]
+};
+
+static size_t search_bytes(int64_t n, int M, int n_list, int k, SearchWs* w, void* base) {
+    Carver cv{static_cast<uint8_t*>(base)};
+    const uint32_t capq = mips::capq_for(n, k);
+    uint32_t* count = cv.take<uint32_t>(QBLOCK);
+    float* bound = cv.take<float>(QBLOCK);
+    uint64_t* cand = cv.take<uint64_t>(static_cast<size_t>(QBLOCK) * capq);
+    float* qf = cv.take<float>(static_cast<size_t>(QBLOCK) * DIM);
+    float* lut = cv.take<float>(static_cast<size_t>(QBLOCK) * M * KSUB);
+    float* ct = cv.take<float>(static_cast<size_t>(QBLOCK) * (n_list > 0 ? n_list : 0));
+    if (w) *w = SearchWs{count, bound, cand, capq, qf, lut, ct};
+    return cv.off;
+}
+
+static int subdot(const float* A, int64_t lda, int rows, const float* B, int nb, int dsub, int M, float* out, cudaStream_t s) {
+    if (rows <= 0) return ATLAS_B200_OK;
+    dim3 grid((nb + SD_T - 1) / SD_T, (rows + SD_T - 1) / SD_T, M);
+    pq_subdot_kernel<<<grid, 256, 0, s>>>(A, lda, rows, B, nb, dsub, M, out);
+    abh::count_launch();
+    AB_CUDA_CHECK(cudaGetLastError());
+    return ATLAS_B200_OK;
+}
+
+static int residual(const __half* x, int64_t n, const float* coarse, const int32_t* assign, float* out, cudaStream_t s) {
+    if (n <= 0) return ATLAS_B200_OK;
+    pq_residual_kernel<<<grid_1d(n * DIM, 256), 256, 0, s>>>(x, n, coarse, assign, out);
+    abh::count_launch();
+    AB_CUDA_CHECK(cudaGetLastError());
+    return ATLAS_B200_OK;
+}
+
+// fp16 copy of the coarse centroids for the GEMM, zero rows up to a multiple of 8
+static int coarse_to_half(const float* coarse, int n_list, __half* out, cudaStream_t s) {
+    const int nlp = pad8(n_list);
+    if (nlp > n_list)
+        AB_CUDA_CHECK(cudaMemsetAsync(out + static_cast<size_t>(n_list) * DIM, 0, static_cast<size_t>(nlp - n_list) * DIM * 2, s));
+    return atlas_b200_cast_f32(coarse, out, static_cast<int64_t>(n_list) * DIM, 0, s);
+}
+
+// coarse assignment of rows [n] (inner product, GEMM + argmax), in chunks of R rows
+static int coarse_assign(const __half* x, int64_t n, const __half* coarse16, int n_list, const ChunkWs& w, int64_t R,
+                         int32_t* assign, void* lists, int list_u16, cudaStream_t s) {
+    const int nlp = pad8(n_list);
+    for (int64_t r0 = 0; r0 < n; r0 += R) {
+        const int rows = static_cast<int>(n - r0 < R ? n - r0 : R);
+        int rc = atlas_b200_linear(x + r0 * DIM, DIM, coarse16, DIM, nullptr, nullptr, 0, w.gemm, nlp, rows, nlp, DIM, 0, 0, s);
+        if (rc) return rc;
+        pq_argmax_rows_kernel<<<grid_1d(static_cast<int64_t>(rows) * 32, 256), 256, 0, s>>>(
+            w.gemm, nlp, rows, n_list, assign ? assign + r0 : nullptr,
+            lists ? static_cast<void*>(static_cast<uint8_t*>(lists) + r0 * (list_u16 ? 2 : 4)) : nullptr, list_u16);
+        abh::count_launch();
+        AB_CUDA_CHECK(cudaGetLastError());
+    }
+    return ATLAS_B200_OK;
+}
+
+// PQ codes of fp32 rows [n][768] (residuals), in chunks of R rows; norms must hold the codebook norms
+static int pq_assign(const float* rows32, int64_t n, int M, const float* codebooks, const ChunkWs& w, int64_t R, uint8_t* codes,
+                     cudaStream_t s) {
+    const int dsub = DIM / M;
+    for (int64_t r0 = 0; r0 < n; r0 += R) {
+        const int rows = static_cast<int>(n - r0 < R ? n - r0 : R);
+        int rc = subdot(rows32 + r0 * DIM, DIM, rows, codebooks, KSUB, dsub, M, w.dots, s);
+        if (rc) return rc;
+        pq_argmin_kernel<<<grid_1d(static_cast<int64_t>(rows) * M * 32, 256), 256, 0, s>>>(w.dots, w.norms, rows, M,
+                                                                                          codes + r0 * M);
+        abh::count_launch();
+        AB_CUDA_CHECK(cudaGetLastError());
+    }
+    return ATLAS_B200_OK;
+}
+
+static int codebook_norms(const float* codebooks, int M, float* norms, cudaStream_t s) {
+    pq_norms_kernel<<<(M * KSUB + 255) / 256, 256, 0, s>>>(codebooks, M * KSUB, DIM / M, norms);
+    abh::count_launch();
+    AB_CUDA_CHECK(cudaGetLastError());
+    return ATLAS_B200_OK;
+}
+
+static int check_shape(int M, int n_list) {
+    AB_REQUIRE(valid_m(M), "code_size M=%d is not supported: M must divide 768 with 768 / M >= 8 "
+               "(1, 2, 3, 4, 6, 8, 12, 16, 24, 32, 48, 64, 96)", M);
+    AB_REQUIRE(n_list >= 0, "n_list=%d must be >= 0 (0 = pq without a coarse quantizer)", n_list);
+    return ATLAS_B200_OK;
+}
+
+static int train(const __half* sample, int64_t S, int M, int n_list, int iters, float* codebooks, float* coarse, void* ws,
+                 size_t ws_bytes, cudaStream_t s) {
+    int rc = check_shape(M, n_list);
+    if (rc) return rc;
+    AB_REQUIRE(sample != nullptr && codebooks != nullptr && (n_list == 0 || coarse != nullptr), "null pointer argument");
+    AB_REQUIRE(S >= KSUB && S >= n_list && S < (1ll << 31), "training needs at least max(256, n_list) rows (got %lld)",
+               (long long)S);
+    AB_REQUIRE(iters >= 0, "iters=%d must be >= 0", iters);
+    ChunkWs w;
+    float* resid;
+    uint8_t* codes_t;
+    int32_t* counts;
+    int32_t* assign;
+    const size_t need = train_bytes(S, M, n_list, &w, &resid, &codes_t, &counts, &assign, ws);
+    if (ws == nullptr || ws_bytes < need) {
+        abh::set_error("workspace too small: have %zu need %zu", ws_bytes, need);
+        return ATLAS_B200_EWORKSPACE;
+    }
+    const int64_t R = chunk_rows(M, n_list);
+    const int dsub = DIM / M;
+
+    // ---- coarse quantizer: inner-product k-means on the first min(S, 256 n_list) rows
+    if (n_list > 0) {
+        const int64_t sc = S < static_cast<int64_t>(n_list) * KSUB ? S : static_cast<int64_t>(n_list) * KSUB;
+        pq_half_to_float_kernel<<<grid_1d(static_cast<int64_t>(n_list) * DIM, 256), 256, 0, s>>>(
+            sample, static_cast<int64_t>(n_list) * DIM, coarse);
+        abh::count_launch();
+        for (int it = 0; it < iters; ++it) {
+            if ((rc = coarse_to_half(coarse, n_list, w.coarse16, s))) return rc;
+            if ((rc = coarse_assign(sample, sc, w.coarse16, n_list, w, R, assign, nullptr, 0, s))) return rc;
+            pq_update_kernel<__half, int32_t><<<dim3(n_list, 1), 256, 0, s>>>(sample, DIM, assign, 1, static_cast<int>(sc),
+                                                                            n_list, DIM, coarse, counts);
+            pq_split_kernel<<<1, 256, 0, s>>>(coarse, counts, n_list, DIM);
+            abh::count_launch(2);
+            AB_CUDA_CHECK(cudaGetLastError());
+        }
+        if ((rc = coarse_to_half(coarse, n_list, w.coarse16, s))) return rc;
+    }
+
+    // ---- product quantizer: L2 k-means per sub-space on the residuals of the first min(S, 65536) rows
+    const int64_t sp = S < PQ_TRAIN_MAX ? S : PQ_TRAIN_MAX;
+    if (n_list > 0 && (rc = coarse_assign(sample, sp, w.coarse16, n_list, w, R, assign, nullptr, 0, s))) return rc;
+    if ((rc = residual(sample, sp, n_list > 0 ? coarse : nullptr, assign, resid, s))) return rc;
+    // initial centroids: rows 0..255 of the (randomly ordered) sample
+    pq_copy_rows_kernel<<<dim3(grid_1d(static_cast<int64_t>(KSUB) * dsub, 256), M), 256, 0, s>>>(
+        resid, DIM, codebooks, dsub, KSUB, dsub, dsub, static_cast<int64_t>(KSUB) * dsub);
+    abh::count_launch();
+    for (int it = 0; it < iters; ++it) {
+        if ((rc = codebook_norms(codebooks, M, w.norms, s))) return rc;
+        if ((rc = pq_assign(resid, sp, M, codebooks, w, R, codes_t, s))) return rc;
+        pq_update_kernel<float, uint8_t><<<dim3(KSUB, M), 256, 0, s>>>(resid, DIM, codes_t, M, static_cast<int>(sp), KSUB,
+                                                                      dsub, codebooks, counts);
+        pq_split_kernel<<<M, 256, 0, s>>>(codebooks, counts, KSUB, dsub);
+        abh::count_launch(2);
+        AB_CUDA_CHECK(cudaGetLastError());
+    }
+    return ATLAS_B200_OK;
+}
+
+static int encode(const __half* rows, int64_t n, int M, const float* codebooks, const float* coarse, int n_list,
+                  uint8_t* codes, void* lists, void* ws, size_t ws_bytes, cudaStream_t s) {
+    int rc = check_shape(M, n_list);
+    if (rc) return rc;
+    AB_REQUIRE(n >= 0, "n=%lld must be >= 0", (long long)n);
+    if (n == 0) return ATLAS_B200_OK;
+    AB_REQUIRE(rows != nullptr && codebooks != nullptr && codes != nullptr &&
+               (n_list == 0 || (coarse != nullptr && lists != nullptr)), "null pointer argument");
+    ChunkWs w;
+    const size_t need = encode_bytes(M, n_list, &w, ws);
+    if (ws == nullptr || ws_bytes < need) {
+        abh::set_error("workspace too small: have %zu need %zu", ws_bytes, need);
+        return ATLAS_B200_EWORKSPACE;
+    }
+    const int64_t R = chunk_rows(M, n_list);
+    const int list_u16 = n_list <= 65535 ? 1 : 0;
+    if ((rc = codebook_norms(codebooks, M, w.norms, s))) return rc;
+    if (n_list > 0 && (rc = coarse_to_half(coarse, n_list, w.coarse16, s))) return rc;
+    for (int64_t r0 = 0; r0 < n; r0 += R) {
+        const int64_t cn = n - r0 < R ? n - r0 : R;
+        const __half* x = rows + r0 * DIM;
+        if (n_list > 0) {
+            void* l = static_cast<uint8_t*>(lists) + r0 * (list_u16 ? 2 : 4);
+            if ((rc = coarse_assign(x, cn, w.coarse16, n_list, w, R, w.assign, l, list_u16, s))) return rc;
+        }
+        if ((rc = residual(x, cn, n_list > 0 ? coarse : nullptr, w.assign, w.resid, s))) return rc;
+        if ((rc = pq_assign(w.resid, cn, M, codebooks, w, R, codes + r0 * M, s))) return rc;
+    }
+    return ATLAS_B200_OK;
+}
+
+// queries per scan CTA: the largest power of two <= 16 (and not above the block's query count) whose tables fit
+static int choose_qpc(int M, int n_list, int nq, bool* cterm_smem) {
+    int cap = 1;
+    while (cap < nq && cap < 16) cap <<= 1;
+    for (int with_ct = (n_list > 0); with_ct >= 0; --with_ct) {
+        for (int qpc = cap; qpc >= 1; qpc >>= 1) {
+            const size_t bytes = static_cast<size_t>(qpc) * (static_cast<size_t>(M) * KSUB * 4 + (with_ct ? n_list * 4ull : 0));
+            if (bytes <= SCAN_SMEM_MAX) {
+                *cterm_smem = with_ct != 0;
+                return qpc;
+            }
+        }
+    }
+    *cterm_smem = false;
+    return 1;
+}
+
+template <int QPC>
+static int launch_scan_q(const ScanParams& p, size_t smem, cudaStream_t s) {
+    static bool attr_set = false;
+    if (!attr_set) {
+        AB_CUDA_CHECK(cudaFuncSetAttribute(pq_scan_kernel<QPC>, cudaFuncAttributeMaxDynamicSharedMemorySize, SCAN_SMEM_MAX));
+        attr_set = true;
+    }
+    const int groups = (p.nq + QPC - 1) / QPC;
+    const int per_sm = static_cast<int>((228 * 1024) / (smem + 2048)) > 0 ? static_cast<int>((228 * 1024) / (smem + 2048)) : 1;
+    const int resident = abh::num_sms() * (per_sm < 4 ? per_sm : 4);
+    int gx = (resident + groups - 1) / groups;
+    if (gx > p.num_tiles) gx = p.num_tiles;
+    if (gx < 1) gx = 1;
+    pq_scan_kernel<QPC><<<dim3(gx, groups), SCAN_THREADS, smem, s>>>(p);
+    abh::count_launch();
+    AB_CUDA_CHECK(cudaGetLastError());
+    return ATLAS_B200_OK;
+}
+
+static int launch_scan(int qpc, const ScanParams& p, size_t smem, cudaStream_t s) {
+    if (p.num_tiles <= 0) return ATLAS_B200_OK;
+    switch (qpc) {
+        case 16: return launch_scan_q<16>(p, smem, s);
+        case 8: return launch_scan_q<8>(p, smem, s);
+        case 4: return launch_scan_q<4>(p, smem, s);
+        case 2: return launch_scan_q<2>(p, smem, s);
+        default: return launch_scan_q<1>(p, smem, s);
+    }
+}
+
+static int topk(const uint8_t* codes, const void* lists, int64_t n, int M, const float* codebooks, const float* coarse,
+                int n_list, const __half* queries, int nq, int k, __half* out_scores, int64_t* out_ids, int64_t id_base,
+                int64_t id_stride, int32_t* status, void* ws, size_t ws_bytes, cudaStream_t s, bool exhaustive) {
+    int rc = check_shape(M, n_list);
+    if (rc) return rc;
+    AB_REQUIRE(nq >= 0 && k >= 1, "nq must be >= 0 and k >= 1 (nq=%d k=%d)", nq, k);
+    AB_REQUIRE(k <= ATLAS_B200_MAX_TOPK, "k=%d exceeds ATLAS_B200_MAX_TOPK=%d", k, ATLAS_B200_MAX_TOPK);
+    AB_REQUIRE(n >= 1 && n < (1ll << 31) - SCAN_THREADS, "rows n=%lld out of range", (long long)n);
+    AB_REQUIRE(k <= n, "selected index k out of range: k=%d > n=%lld", k, (long long)n);
+    AB_REQUIRE(codes != nullptr && codebooks != nullptr && (n_list == 0 || (coarse != nullptr && lists != nullptr)),
+               "null pointer argument");
+    AB_REQUIRE((M & 3) != 0 || (reinterpret_cast<uintptr_t>(codes) & 3u) == 0, "codes must be 4-byte aligned");
+    AB_REQUIRE(nq == 0 || queries != nullptr, "queries is null");
+    if (status) AB_CUDA_CHECK(cudaMemsetAsync(status, 0, sizeof(int32_t), s));
+    if (nq == 0) return ATLAS_B200_OK;
+    SearchWs w;
+    const size_t need = search_bytes(n, M, n_list, k, &w, ws);
+    if (ws == nullptr || ws_bytes < need) {
+        abh::set_error("workspace too small: have %zu need %zu", ws_bytes, need);
+        return ATLAS_B200_EWORKSPACE;
+    }
+    const int dsub = DIM / M;
+    const int total_tiles = static_cast<int>((n + SCAN_THREADS - 1) / SCAN_THREADS);
+    for (int q0 = 0; q0 < nq; q0 += QBLOCK) {
+        const int nqb = nq - q0 < QBLOCK ? nq - q0 : QBLOCK;
+        if ((rc = residual(queries + static_cast<int64_t>(q0) * DIM, nqb, nullptr, nullptr, w.qf32, s))) return rc;
+        if ((rc = subdot(w.qf32, DIM, nqb, codebooks, KSUB, dsub, M, w.lut, s))) return rc;
+        if (n_list > 0 && (rc = subdot(w.qf32, DIM, nqb, coarse, n_list, DIM, 1, w.cterm, s))) return rc;
+        pq_prep_kernel<<<1, QBLOCK, 0, s>>>(w.count, w.bound);
+        abh::count_launch();
+        bool cterm_smem = false;
+        const int qpc = choose_qpc(M, n_list, nqb, &cterm_smem);
+        const size_t smem = static_cast<size_t>(qpc) * (static_cast<size_t>(M) * KSUB * 4 + (cterm_smem ? n_list * 4ull : 0));
+        ScanParams p;
+        p.codes = codes;
+        p.lists = lists;
+        p.list_u16 = n_list <= 65535 ? 1 : 0;
+        p.n_rows = static_cast<int>(n);
+        p.M = M;
+        p.lut = w.lut;
+        p.cterm = n_list > 0 ? w.cterm : nullptr;
+        p.n_list = n_list;
+        p.cterm_smem = cterm_smem ? 1 : 0;
+        p.nq = nqb;
+        p.bound = w.bound;
+        p.count = w.count;
+        p.cand = w.cand;
+        p.capq = w.capq;
+        __half* os_b = out_scores + static_cast<size_t>(q0) * k;
+        int64_t* oi_b = out_ids + static_cast<size_t>(q0) * k;
+        uint16_t* os16 = reinterpret_cast<uint16_t*>(os_b);
+        if (!exhaustive) {
+            if (n > static_cast<int64_t>(w.capq)) {
+                // bound from a strided sample of ~2 sqrt(k n) rows (every score kept), as in mips.cu's one-stage sample
+                double m = 2.0 * sqrt(static_cast<double>(k) * static_cast<double>(n));
+                if (m < 4096) m = 4096;
+                if (m > w.capq / 2) m = w.capq / 2;
+                int sample_tiles = static_cast<int>(m / SCAN_THREADS);
+                if (sample_tiles < 1) sample_tiles = 1;
+                if (sample_tiles > total_tiles) sample_tiles = total_tiles;
+                p.tile_begin = 0;
+                p.tile_step = total_tiles / sample_tiles;
+                p.num_tiles = sample_tiles;
+                if ((rc = launch_scan(qpc, p, smem, s))) return rc;
+                mips::mips_select_kernel<false><<<nqb, mips::SEL_THREADS, 0, s>>>(
+                    w.cand, w.count, w.capq, k, mips::SEL_WRITE_BOUND, w.bound, nullptr, nullptr, 0, 0, nullptr);
+                abh::count_launch();
+            }
+            p.tile_begin = 0;
+            p.tile_step = 1;
+            p.num_tiles = total_tiles;
+            abh::prof_begin(s, abh::PROF_SCAN);
+            rc = launch_scan(qpc, p, smem, s);
+            abh::prof_end(s, abh::PROF_SCAN, static_cast<double>(n) * M * ((nqb + qpc - 1) / qpc));
+            if (rc) return rc;
+            mips::mips_select_kernel<false><<<nqb, mips::SEL_THREADS, 0, s>>>(
+                w.cand, w.count, w.capq, k, mips::SEL_EMIT, w.bound, os16, oi_b, id_base, id_stride, status);
+            abh::count_launch();
+        } else {
+            // chunked exact scan: every score of a chunk is a candidate, winners are carried forward
+            int chunk_tiles = static_cast<int>((w.capq - static_cast<uint32_t>(k)) / SCAN_THREADS);
+            if (chunk_tiles < 1) chunk_tiles = 1;
+            for (int t0 = 0; t0 < total_tiles; t0 += chunk_tiles) {
+                const bool last = t0 + chunk_tiles >= total_tiles;
+                p.tile_begin = t0;
+                p.tile_step = 1;
+                p.num_tiles = last ? total_tiles - t0 : chunk_tiles;
+                if ((rc = launch_scan(qpc, p, smem, s))) return rc;
+                mips::mips_select_kernel<false><<<nqb, mips::SEL_THREADS, 0, s>>>(
+                    w.cand, w.count, w.capq, k, last ? mips::SEL_EMIT : mips::SEL_CARRY, w.bound, os16, oi_b, id_base,
+                    id_stride, nullptr);
+                abh::count_launch();
+            }
+        }
+    }
+    AB_CUDA_CHECK(cudaGetLastError());
+    return ATLAS_B200_OK;
+}
+
+}  // namespace pq
+
+extern "C" {
+
+size_t atlas_b200_pq_workspace_bytes(int32_t op, int64_t n, int32_t M, int32_t n_list, int32_t k) {
+    if (!pq::valid_m(M) || n_list < 0) return 0;
+    if (n < 1) n = 1;
+    if (k < 1) k = 1;
+    switch (op) {
+        case ATLAS_B200_PQ_OP_TRAIN: return pq::train_bytes(n, M, n_list, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr);
+        case ATLAS_B200_PQ_OP_ENCODE: return pq::encode_bytes(M, n_list, nullptr, nullptr);
+        case ATLAS_B200_PQ_OP_SEARCH: return pq::search_bytes(n, M, n_list, k, nullptr, nullptr);
+        default: return 0;
+    }
+}
+
+int atlas_b200_pq_train(const void* sample, int64_t n_sample, int32_t M, int32_t n_list, int32_t iters, float* codebooks,
+                        float* coarse, void* workspace, size_t workspace_bytes, void* stream) {
+    return pq::train(static_cast<const __half*>(sample), n_sample, M, n_list, iters, codebooks, coarse, workspace,
+                     workspace_bytes, static_cast<cudaStream_t>(stream));
+}
+
+int atlas_b200_pq_encode(const void* rows, int64_t n, int32_t M, const float* codebooks, const float* coarse, int32_t n_list,
+                         uint8_t* codes, void* list_ids, void* workspace, size_t workspace_bytes, void* stream) {
+    return pq::encode(static_cast<const __half*>(rows), n, M, codebooks, coarse, n_list, codes, list_ids, workspace,
+                      workspace_bytes, static_cast<cudaStream_t>(stream));
+}
+
+int atlas_b200_pq_topk(const uint8_t* codes, const void* list_ids, int64_t n, int32_t M, const float* codebooks,
+                       const float* coarse, int32_t n_list, const void* queries, int32_t nq, int32_t k, void* out_scores,
+                       int64_t* out_ids, int64_t id_base, int64_t id_stride, int32_t* status, void* workspace,
+                       size_t workspace_bytes, void* stream) {
+    return pq::topk(codes, list_ids, n, M, codebooks, coarse, n_list, static_cast<const __half*>(queries), nq, k,
+                    static_cast<__half*>(out_scores), out_ids, id_base, id_stride, status, workspace, workspace_bytes,
+                    static_cast<cudaStream_t>(stream), false);
+}
+
+int atlas_b200_pq_topk_exhaustive(const uint8_t* codes, const void* list_ids, int64_t n, int32_t M, const float* codebooks,
+                                  const float* coarse, int32_t n_list, const void* queries, int32_t nq, int32_t k,
+                                  void* out_scores, int64_t* out_ids, int64_t id_base, int64_t id_stride, void* workspace,
+                                  size_t workspace_bytes, void* stream) {
+    return pq::topk(codes, list_ids, n, M, codebooks, coarse, n_list, static_cast<const __half*>(queries), nq, k,
+                    static_cast<__half*>(out_scores), out_ids, id_base, id_stride, nullptr, workspace, workspace_bytes,
+                    static_cast<cudaStream_t>(stream), true);
+}
+
+}  // extern "C"

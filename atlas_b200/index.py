@@ -14,9 +14,11 @@ Same public surface: `embeddings` ([768, N] fp16 CUDA, slice-assignable on dim 1
     store (atlas_b200/passage_store.py);
   * ties are ordered canonically: score descending, then global passage id ascending.
 
-There is no CPU path: `is_in_gpu = False` (the reference's FAISS-only mode) raises.
+There is no CPU path: `is_in_gpu = False` raises here.  `DistributedFAISSIndex` (below) is the reference's
+`--index_mode faiss` with host-resident rows and a product-quantized device index (csrc/pq.cu).
 """
 import ctypes
+import logging
 import math
 import os
 import pickle
@@ -28,6 +30,8 @@ import torch
 from . import dist_utils, ops
 from ._lib import MAX_TOPK, AtlasB200Error, check, lib
 from .passage_store import make_store
+
+logger = logging.getLogger(__name__)
 
 EMBEDDINGS_DIM: int = 768  # src/retrievers.py:13
 
@@ -138,23 +142,32 @@ class DistributedIndex(object):
                 n_passages += 1
         device = self._device()
         files = [self._get_saved_embedding_path(path, s) for s in shard_ids]
-        if device.type == "cuda":
-            self._bank = self._load_bank_streamed(files, device)
-        else:       # CPU test doubles of this class (tests/test_index_gloo.py)
-            rows = [torch.load(f, map_location="cpu").t().to(torch.float16) for f in files]
-            self._bank = torch.cat(rows, dim=0).contiguous().to(device)
-        sizes = dist_utils.get_varsize(self._bank)
+        self._bank = self._load_rows(files, device)
+        sizes = dist_utils.get_varsize(torch.empty((self._bank.shape[0], 0), device=self._query_device()))
         self._offsets = np.concatenate([[0], np.cumsum(sizes)]).astype(np.int64)
         self._id_base, self._id_stride = int(self._offsets[rank]), 1
         self._reset_store()
 
+    def _load_rows(self, files, device):
+        if device.type == "cuda":
+            return self._load_bank_streamed(files, device)
+        # CPU test doubles of this class (tests/test_index_gloo.py)
+        rows = [torch.load(f, map_location="cpu").t().to(torch.float16) for f in files]
+        return torch.cat(rows, dim=0).contiguous().to(device)
+
+    def _query_device(self):
+        """Where the query rows of a search live (the bank's device)."""
+        return self._bank.device
+
     @staticmethod
-    def _load_bank_streamed(files, device, chunk_cols=262144):
+    def _load_bank_streamed(files, device, chunk_cols=262144, host=False):
         """The shard files (`embeddings.{s}.pt` = [768, n_s] fp16, src/index.py:75-87) straight into the device bank
         [sum n_s, 768]: every file is memory-mapped (`torch.load(mmap=True)`: no host copy of the whole tensor), column
         chunks are staged through two pinned buffers, copied H2D asynchronously and transposed into their bank rows by
         `atlas_b200_transpose` on the GPU.  The reference (and round 1 here) reads every shard into host memory,
-        transposes it on ONE CPU core (`.t()` + `cat` -> a strided 2-byte copy, ~1 GB/s) and only then uploads it."""
+        transposes it on ONE CPU core (`.t()` + `cat` -> a strided 2-byte copy, ~1 GB/s) and only then uploads it.
+        host=True: the rows go to a pinned HOST tensor instead (DistributedFAISSIndex): every chunk is transposed into a
+        device staging buffer and copied back asynchronously."""
         shards = []
         for f in files:
             try:
@@ -165,9 +178,13 @@ class DistributedIndex(object):
                 raise AtlasB200Error(f"{f}: expected a [{EMBEDDINGS_DIM}, n] embedding shard, got {tuple(t.shape)}")
             shards.append(t)
         total = sum(int(t.shape[1]) for t in shards)
-        bank = torch.empty((total, EMBEDDINGS_DIM), dtype=torch.float16, device=device)
         width = max(8, min(chunk_cols, max((int(t.shape[1]) for t in shards), default=8)))
         width = (width + 7) // 8 * 8
+        if host:
+            bank = torch.empty((total, EMBEDDINGS_DIM), dtype=torch.float16).pin_memory()
+            tstage = [torch.empty((width, EMBEDDINGS_DIM), dtype=torch.float16, device=device) for _ in range(2)]
+        else:
+            bank = torch.empty((total, EMBEDDINGS_DIM), dtype=torch.float16, device=device)
         stage = [torch.empty((EMBEDDINGS_DIM, width), dtype=torch.float16).pin_memory() for _ in range(2)]
         dstage = [torch.empty((EMBEDDINGS_DIM, width), dtype=torch.float16, device=device) for _ in range(2)]
         done = [torch.cuda.Event(), torch.cuda.Event()]
@@ -187,12 +204,14 @@ class DistributedIndex(object):
                 done[k].record(stream)
                 used[k] = True
                 view = dstage[k][:, :w]
+                target = tstage[k][:w] if host else bank[row0 + a:row0 + a + w]
                 if w % 2 == 0:
-                    dst = bank.data_ptr() + (row0 + a) * bank.stride(0) * 2
-                    check(lib().atlas_b200_transpose(view.data_ptr(), view.stride(0), dst, bank.stride(0), EMBEDDINGS_DIM, w,
-                                                     EMBEDDINGS_DIM, ctypes.c_void_p(stream.cuda_stream)))
+                    check(lib().atlas_b200_transpose(view.data_ptr(), view.stride(0), target.data_ptr(), target.stride(0),
+                                                     EMBEDDINGS_DIM, w, EMBEDDINGS_DIM, ctypes.c_void_p(stream.cuda_stream)))
                 else:   # odd tail width: the transpose kernel moves 2-column words
-                    bank[row0 + a:row0 + a + w].copy_(view.t())
+                    target.copy_(view.t())
+                if host:
+                    bank[row0 + a:row0 + a + w].copy_(target, non_blocking=True)
                 it += 1
             row0 += n
         torch.cuda.current_stream(device).synchronize()
@@ -245,7 +264,7 @@ class DistributedIndex(object):
             s, i, status = self._local_search(queries, topk, exhaustive)
             status = status.to(torch.int64).reshape(())
         else:
-            q16 = queries.to(self._bank.device).to(torch.float16)                  # `.half()`, src/index.py:117
+            q16 = queries.to(self._query_device()).to(torch.float16)                  # `.half()`, src/index.py:117
             cap = self.max_queries_per_rank
             if cap:
                 if nq_local > cap:
@@ -299,11 +318,181 @@ class DistributedIndex(object):
 
 
 class DistributedFAISSIndex(DistributedIndex):
-    """src/index.py:163-381 wraps faiss-gpu IVF/PQ indices.  Out of scope here (north_star: "No FAISS");
-    the exact flat index above is the supported mode and is what the README recommends."""
+    """`--index_mode faiss` (src/index.py:163-381) with a product-quantized index on the device (csrc/pq.cu).
+
+    index_type "pq": `code_size` one-byte sub-quantizer codes per passage; "ivfpq": floor(sqrt(N_local)) coarse centroids
+    (inner-product assignment) and PQ codes of the residuals.  The reference probes every inverted list
+    (nprobe = n_list, src/index.py:212,269), so a search scores every row: sum_m LUT[m][code_m] (+ <q, c_list>), fp32,
+    rounded once to fp16 - the same scores faiss's IndexPQ / IVFPQ produce, up to the fp32 summation order.
+
+    Memory: the full-precision rows stay in pinned HOST memory as [N, 768] fp16 (`embeddings` is the reference's
+    [768, N] view of them, `is_in_gpu = False`).  The device holds M bytes of codes (plus 2 bytes of list id for ivfpq)
+    per passage, the codebooks and the coarse centroids; training and encoding stage host chunks through a transient
+    device buffer.
+
+    Training: `train_index()` retrains both quantizers (k-means, faiss's defaults, deterministic) on the current rows and
+    re-encodes every row.  After writing rows by hand (`index.embeddings[:, a:b] = ...`) call `train_index()` again;
+    `Atlas.build_index` does this itself (it marks the index stale, as the reference's inverted `is_index_trained`
+    makes it do after every refresh, src/atlas.py:86-88).  Searching an untrained index raises.
+
+    Persistence: `save_index` writes the reference's `embeddings.{s}.pt` / `passages.{s}.pt` shards and, per rank,
+    `index{type}_{code_size}_rank_{r}.atlas_b200.pt` (format version, type, M, n_list, row count, codebooks, coarse
+    centroids, codes, list ids).  `load_index` uses that file when type, M and row count match and retrains otherwise;
+    a reference `.faiss` file is not read (faiss's format is not reproduced here)."""
+
+    SUPPORTED_TYPES = ("pq", "ivfpq")
+    FILE_FORMAT = 1
+    TRAIN_SEED = 1234
+    STAGE_ROWS = 65536
 
     def __init__(self, index_type: str = "flat", code_size: Optional[int] = None):
-        raise AtlasB200Error(
-            "DistributedFAISSIndex is not provided by atlas_b200: use --index_mode flat "
-            "(exact search, atlas_b200.index.DistributedIndex)"
-        )
+        if index_type not in self.SUPPORTED_TYPES:
+            raise AtlasB200Error(
+                f"DistributedFAISSIndex: index_type={index_type!r} is not provided by atlas_b200; supported types are "
+                f"{', '.join(self.SUPPORTED_TYPES)}.  For exact search use --index_mode flat "
+                "(atlas_b200.index.DistributedIndex): flat and ivfflat with nprobe = n_list are exact anyway")
+        if code_size is None:
+            raise AtlasB200Error(f"DistributedFAISSIndex({index_type!r}) needs a code_size (--faiss_code_size)")
+        ops.pq_check_code_size(code_size)
+        super().__init__()
+        self._device()                 # no CUDA device: raise here, like the flat index (no CPU path)
+        self.index_type = index_type
+        self.code_size = int(code_size)
+        self.is_in_gpu = False
+        self._pq = None                # dict(codebooks, coarse, codes, list_ids, n_list) of the trained index
+
+    # ------------------------------------------------------------------ host rows
+    @property
+    def embeddings(self):
+        return None if self._bank is None else self._bank.t()
+
+    @embeddings.setter
+    def embeddings(self, value):
+        if value is None:
+            self._bank = None
+        else:
+            if value.dim() != 2 or value.shape[0] != EMBEDDINGS_DIM:
+                raise ValueError(f"embeddings must be [{EMBEDDINGS_DIM}, N], got {tuple(value.shape)}")
+            self._bank = self._host_rows(value.shape[1])
+            self._bank.copy_(value.t())
+        self._pq = None
+
+    def _host_rows(self, n):
+        rows = torch.zeros((n, EMBEDDINGS_DIM), dtype=torch.float16)
+        return rows.pin_memory() if torch.cuda.is_available() else rows
+
+    def _query_device(self):
+        return self._device()
+
+    def init_embeddings(self, passages, dim: Optional[int] = EMBEDDINGS_DIM):
+        if dim != EMBEDDINGS_DIM:
+            raise ValueError(f"only dim={EMBEDDINGS_DIM} is supported (src/retrievers.py:13)")
+        self.doc_map = {i: doc for i, doc in enumerate(passages)}
+        self._bank = self._host_rows(len(passages))
+        self._id_base, self._id_stride = dist_utils.get_rank(), dist_utils.get_world_size()
+        self._offsets = None
+        self._pq = None
+        self._reset_store()
+
+    def _load_rows(self, files, device):
+        if device.type == "cuda":
+            return self._load_bank_streamed(files, device, host=True)
+        rows = [torch.load(f, map_location="cpu").t().to(torch.float16) for f in files]
+        return torch.cat(rows, dim=0).contiguous()
+
+    # ------------------------------------------------------------------ training
+    def is_index_trained(self) -> bool:
+        return self._pq is not None
+
+    def mark_stale(self):
+        """The rows changed: the next `is_index_trained()` is False and searching raises until `train_index()`."""
+        self._pq = None
+
+    def n_list(self, n_rows=None):
+        n = self._bank.shape[0] if n_rows is None else n_rows
+        return int(math.floor(math.sqrt(n))) if self.index_type == "ivfpq" else 0
+
+    def train_index(self):
+        """Train the quantizers on the current rows and encode every row (src/index.py:352-381 trains + adds)."""
+        if self._bank is None:
+            raise AtlasB200Error("train_index before init_embeddings/load_index")
+        n = self._bank.shape[0]
+        if n < ops.PQ_KSUB:
+            raise AtlasB200Error(f"train_index: {n} rows on this rank; product quantization needs at least "
+                                 f"{ops.PQ_KSUB} training points (faiss raises the same way)")
+        self._pq = None
+        self._pq = self._train_and_encode(self._bank, n)
+
+    def _train_and_encode(self, rows, n):
+        device = self._device()
+        n_list = self.n_list(n)
+        n_sample = min(n, max(ops.PQ_KSUB * ops.PQ_KSUB, ops.PQ_KSUB * n_list))
+        perm = np.random.default_rng(self.TRAIN_SEED).permutation(n)[:n_sample]
+        sample = rows[torch.from_numpy(perm)].to(device)
+        codebooks, coarse = ops.pq_train(sample, self.code_size, n_list)
+        del sample
+        codes = torch.empty((n, self.code_size), dtype=torch.uint8, device=device)
+        list_ids = torch.empty(n, dtype=ops.pq_list_dtype(n_list), device=device) if n_list else None
+        ws = ops.Workspace()
+        width = min(self.STAGE_ROWS, n)
+        stage = [torch.empty((width, EMBEDDINGS_DIM), dtype=torch.float16, device=device) for _ in range(2)]
+        for it, a in enumerate(range(0, n, width)):
+            b = min(n, a + width)
+            st = stage[it & 1][: b - a]
+            st.copy_(rows[a:b], non_blocking=True)       # pinned source; the stream orders the reuse of `st`
+            ops.pq_encode(st, codebooks, coarse, codes[a:b], list_ids[a:b] if n_list else None, ws)
+        torch.cuda.current_stream(device).synchronize()
+        return dict(codebooks=codebooks, coarse=coarse, codes=codes, list_ids=list_ids, n_list=n_list)
+
+    # ------------------------------------------------------------------ search
+    def _trained(self):
+        if self._pq is None:
+            raise AtlasB200Error("search_knn on an untrained DistributedFAISSIndex: call train_index() after writing rows")
+        return self._pq
+
+    def _local_search(self, allqueries, topk, exhaustive=False):
+        p = self._trained()
+        return ops.pq_topk(p["codes"], p["list_ids"], p["codebooks"], p["coarse"], allqueries, topk, self._id_base,
+                           self._id_stride, self._workspace, exhaustive=exhaustive)
+
+    # ------------------------------------------------------------------ persistence
+    def _get_index_filename(self, path: str) -> str:
+        """src/index.py:175-183 names `index{type}_{code_size}_rank_{r}.faiss`; this format gets its own suffix."""
+        return os.path.join(path, f"index{self.index_type}_{self.code_size}_rank_{dist_utils.get_rank()}.atlas_b200.pt")
+
+    def _get_faiss_index_filename(self, path: str) -> str:
+        return os.path.join(path, f"index{self.index_type}_{self.code_size}_rank_{dist_utils.get_rank()}.faiss")
+
+    def save_index(self, path: str, total_saved_shards: int, overwrite_saved_passages: bool = False) -> None:
+        super().save_index(path, total_saved_shards, overwrite_saved_passages)
+        if self._pq is None:
+            return
+        p = self._pq
+        cpu = lambda t: None if t is None else t.cpu()
+        torch.save(dict(format=self.FILE_FORMAT, index_type=self.index_type, code_size=self.code_size, n_list=p["n_list"],
+                        n_rows=int(self._bank.shape[0]), codebooks=cpu(p["codebooks"]), coarse=cpu(p["coarse"]),
+                        codes=cpu(p["codes"]), list_ids=cpu(p["list_ids"])),
+                   self._get_index_filename(path))
+
+    def load_index(self, path: str, total_saved_shards: int):
+        """Loads the shards into the host rows, then the index file if it matches (type, M, row count); else retrains."""
+        super().load_index(path, total_saved_shards)
+        self._pq = None
+        f = self._get_index_filename(path)
+        n = int(self._bank.shape[0])
+        if os.path.exists(f):
+            d = torch.load(f, map_location="cpu")
+            if (d.get("format") == self.FILE_FORMAT and d.get("index_type") == self.index_type
+                    and d.get("code_size") == self.code_size and d.get("n_rows") == n
+                    and d.get("n_list") == self.n_list(n)):
+                dev = self._device()
+                to = lambda t: None if t is None else t.to(dev)
+                self._pq = dict(codebooks=to(d["codebooks"]), coarse=to(d["coarse"]), codes=to(d["codes"]),
+                                list_ids=to(d["list_ids"]), n_list=int(d["n_list"]))
+                return
+            logger.info(f"{f} does not match this index (type {self.index_type}, code_size {self.code_size}, {n} rows): "
+                        "retraining")
+        elif os.path.exists(self._get_faiss_index_filename(path)):
+            logger.info(f"{self._get_faiss_index_filename(path)} is a faiss file, which atlas_b200 does not read: retraining")
+        if n >= ops.PQ_KSUB:
+            self.train_index()

@@ -158,6 +158,88 @@ def topk_merge_blob(blob_all, ids_off, world, nq_total, k, q_begin, nq_out, dtyp
 
 
 # ---------------------------------------------------------------------------------------------
+# product-quantized index (csrc/pq.cu)
+# ---------------------------------------------------------------------------------------------
+PQ_OP_TRAIN, PQ_OP_ENCODE, PQ_OP_SEARCH = 0, 1, 2
+PQ_KSUB = 256
+PQ_ITERS = 25   # faiss's k-means default
+
+
+def pq_check_code_size(code_size):
+    """code_size M: sub-quantizers of 8 bits; M must divide 768 with 768 / M >= 8."""
+    if not isinstance(code_size, int) or code_size < 1 or DIM % code_size or DIM // code_size < 8:
+        ok = [m for m in range(1, DIM + 1) if DIM % m == 0 and DIM // m >= 8]
+        raise AtlasB200Error(f"code_size={code_size!r} is not supported: it must divide {DIM} into sub-vectors of at "
+                             f"least 8 dimensions, one of {ok}")
+
+
+def pq_list_dtype(n_list):
+    """Storage type of the list ids: uint16 while every id fits, else int32."""
+    return torch.uint16 if n_list <= 65535 else torch.int32
+
+
+def pq_train(sample, code_size, n_list, iters=PQ_ITERS):
+    """k-means on the device (atlas_b200_pq_train).  sample: CUDA fp16 [S, 768], rows in a seeded random order.
+    Returns (codebooks fp32 [M, 256, 768 / M], coarse centroids fp32 [n_list, 768] or None)."""
+    require_cuda(sample, "sample")
+    pq_check_code_size(code_size)
+    s = sample.reshape(-1, DIM).to(torch.float16).contiguous()
+    dev = s.device
+    cb = torch.empty((code_size, PQ_KSUB, DIM // code_size), dtype=torch.float32, device=dev)
+    coarse = torch.empty((n_list, DIM), dtype=torch.float32, device=dev) if n_list else None
+    ws = torch.empty(int(lib().atlas_b200_pq_workspace_bytes(PQ_OP_TRAIN, s.shape[0], code_size, n_list, 1)),
+                     dtype=torch.uint8, device=dev)
+    check(lib().atlas_b200_pq_train(_ptr(s), s.shape[0], code_size, n_list, iters, _ptr(cb),
+                                    _ptr(coarse) if coarse is not None else None, _ptr(ws), ws.numel(),
+                                    current_stream_ptr()))
+    return cb, coarse
+
+
+def pq_encode(rows, codebooks, coarse, codes, list_ids=None, workspace=None):
+    """Codes (and list ids) of CUDA fp16 rows [n, 768] into `codes` uint8 [n, M] (and `list_ids` [n])."""
+    require_cuda(rows, "rows")
+    r = rows.reshape(-1, DIM)
+    if r.dtype != torch.float16 or not r.is_contiguous():
+        raise AtlasB200Error("pq_encode: rows must be contiguous fp16 [n, 768]")
+    M = codebooks.shape[0]
+    n_list = 0 if coarse is None else coarse.shape[0]
+    if codes.shape != (r.shape[0], M) or codes.dtype != torch.uint8 or (n_list and list_ids is None):
+        raise AtlasB200Error("pq_encode: codes must be uint8 [n, M] (and list ids are needed with a coarse quantizer)")
+    buf = (workspace or _default_ws).get(lib().atlas_b200_pq_workspace_bytes(PQ_OP_ENCODE, r.shape[0], M, n_list, 1),
+                                         r.device)
+    check(lib().atlas_b200_pq_encode(_ptr(r), r.shape[0], M, _ptr(codebooks), _ptr(coarse) if n_list else None, n_list,
+                                     _ptr(codes), _ptr(list_ids) if n_list else None, _ptr(buf), buf.numel(),
+                                     current_stream_ptr()))
+    return codes, list_ids
+
+
+def pq_topk(codes, list_ids, codebooks, coarse, queries, k, id_base=0, id_stride=1, workspace=None, exhaustive=False):
+    """Top-k of the PQ / IVF-PQ scores of `queries` [nq, 768] over one shard's codes (atlas_b200_pq_topk).
+
+    Returns (scores [nq, k] fp16 desc, ids [nq, k] int64, status int32[1] device tensor) like `mips_topk`."""
+    require_cuda(codes, "codes")
+    n, M = codes.shape
+    n_list = 0 if coarse is None else coarse.shape[0]
+    q = cast_queries(queries.reshape(-1, DIM).to(codes.device), torch.float16)
+    nq = q.shape[0]
+    buf = (workspace or _default_ws).get(lib().atlas_b200_pq_workspace_bytes(PQ_OP_SEARCH, n, M, n_list, k), codes.device)
+    out_s = torch.empty((nq, k), dtype=torch.float16, device=codes.device)
+    out_i = torch.empty((nq, k), dtype=torch.int64, device=codes.device)
+    status = torch.zeros(1, dtype=torch.int32, device=codes.device)
+    lp = _ptr(list_ids) if n_list else None
+    cp = _ptr(coarse) if n_list else None
+    if exhaustive:
+        check(lib().atlas_b200_pq_topk_exhaustive(_ptr(codes), lp, n, M, _ptr(codebooks), cp, n_list, _ptr(q), nq, k,
+                                                  _ptr(out_s), _ptr(out_i), id_base, id_stride, _ptr(buf), buf.numel(),
+                                                  current_stream_ptr()))
+    else:
+        check(lib().atlas_b200_pq_topk(_ptr(codes), lp, n, M, _ptr(codebooks), cp, n_list, _ptr(q), nq, k, _ptr(out_s),
+                                       _ptr(out_i), id_base, id_stride, _ptr(status), _ptr(buf), buf.numel(),
+                                       current_stream_ptr()))
+    return out_s, out_i, status
+
+
+# ---------------------------------------------------------------------------------------------
 # dense layers (csrc/gemm.cu)
 # ---------------------------------------------------------------------------------------------
 EPI_NONE, EPI_BIAS, EPI_GELU, EPI_RESIDUAL, EPI_GATED = 0, 1, 2, 3, 4

@@ -107,6 +107,47 @@ int atlas_b200_search_host(const void* bank, int64_t n, int64_t ld, int32_t is_b
                            void* workspace, size_t workspace_bytes, void* stream);
 
 /* --------------------------------------------------------------------------------------------
+ * Product-quantized passage index (csrc/pq.cu): `DistributedFAISSIndex` with index_type pq / ivfpq
+ * (src/index.py:163-381; faiss IndexPQ / GpuIndexIVFPQ with 8-bit codes and nprobe = n_list).
+ *
+ *   M          code_size: sub-quantizers of 256 centroids each; M divides 768 and dsub = 768 / M >= 8.
+ *   n_list     coarse centroids (ivfpq), 0 = pq.  The reference probes every list, so a search scans all rows.
+ *   codebooks  device fp32 [M][256][dsub];  coarse: device fp32 [n_list][768] (NULL for pq).
+ *   codes      device uint8 [n, M] (4-byte aligned when M % 4 == 0);  list_ids: device [n] uint16 when
+ *              n_list <= 65535, else int32 (NULL for pq).
+ *   scores     fp32 LUTs <q_m, cb_m[j]> and coarse terms <q, c_l> from the fp16 queries; each row's score is
+ *              sum_m LUT[m][code_m] (m ascending, fp32) + <q, c_list>, rounded ONCE to fp16.
+ *
+ * atlas_b200_pq_train: k-means with faiss's defaults on the device.  `sample` [n_sample, 768] fp16 holds the
+ *   training rows in a seeded random order: the coarse quantizer (inner-product assignment, plain means) is trained
+ *   on the first min(n_sample, 256 n_list) rows, the product quantizer (L2 per sub-space) on the residuals of the
+ *   first min(n_sample, 65536); the first rows are the initial centroids; empty clusters are split off the largest
+ *   one.  Bitwise deterministic.  n_sample >= max(256, n_list).
+ * atlas_b200_pq_encode: codes (and list ids) of n fp16 rows [n, 768] - call it chunk by chunk.
+ * atlas_b200_pq_topk / _exhaustive: atlas_b200_mips_topk's contract (fp16 scores desc, ids = id_base +
+ *   id_stride * row, canonical tie order, `status` overflow flag and the exhaustive retry) over these scores.
+ * Workspace: atlas_b200_pq_workspace_bytes(op, n, M, n_list, k) with n = n_sample (train), unused (encode) or the
+ *   row count (search); 0 for an unsupported M.
+ * -------------------------------------------------------------------------------------------- */
+#define ATLAS_B200_PQ_OP_TRAIN 0
+#define ATLAS_B200_PQ_OP_ENCODE 1
+#define ATLAS_B200_PQ_OP_SEARCH 2
+size_t atlas_b200_pq_workspace_bytes(int32_t op, int64_t n, int32_t M, int32_t n_list, int32_t k);
+int atlas_b200_pq_train(const void* sample, int64_t n_sample, int32_t M, int32_t n_list, int32_t iters,
+                        float* codebooks, float* coarse, void* workspace, size_t workspace_bytes, void* stream);
+int atlas_b200_pq_encode(const void* rows, int64_t n, int32_t M, const float* codebooks, const float* coarse,
+                         int32_t n_list, uint8_t* codes, void* list_ids, void* workspace, size_t workspace_bytes,
+                         void* stream);
+int atlas_b200_pq_topk(const uint8_t* codes, const void* list_ids, int64_t n, int32_t M, const float* codebooks,
+                       const float* coarse, int32_t n_list, const void* queries, int32_t nq, int32_t k,
+                       void* out_scores, int64_t* out_ids, int64_t id_base, int64_t id_stride, int32_t* status,
+                       void* workspace, size_t workspace_bytes, void* stream);
+int atlas_b200_pq_topk_exhaustive(const uint8_t* codes, const void* list_ids, int64_t n, int32_t M,
+                                  const float* codebooks, const float* coarse, int32_t n_list, const void* queries,
+                                  int32_t nq, int32_t k, void* out_scores, int64_t* out_ids, int64_t id_base,
+                                  int64_t id_stride, void* workspace, size_t workspace_bytes, void* stream);
+
+/* --------------------------------------------------------------------------------------------
  * Dense linear layer with a fused epilogue on wgmma (csrc/gemm.cu):
  *     C[M, N] = epilogue( A[M, K] . W[N, K]^T )     A, W, C, bias, residual: fp16 (is_bf16 = 0) or bf16
  * W is the nn.Linear weight as stored by torch ([out_features, in_features]).  fp32 accumulation.
