@@ -8,7 +8,7 @@
 //   BertOutput.dense                                     (src/modeling_bert.py:280-466)
 //   T5Attention q/k/v/o, T5DenseGatedGeluDense wi_0/wi_1 (+gelu_new gate)/wo, lm_head
 //                                                        (src/modeling_t5.py:272-289,418-531,1642-1647)
-// Fused epilogues (runtime-selected, applied to the fp32 accumulator registers):
+// Fused epilogues (a template parameter of the kernel, applied to the fp32 accumulator registers):
 //   EPI_NONE      C = acc
 //   EPI_BIAS      C = acc + bias[n]
 //   EPI_GELU      C = gelu_erf(acc + bias[n])                      (ACT2FN["gelu"], modeling_bert.py:444)
@@ -20,7 +20,8 @@
 // tiles to fill the SMs, else 128):
 //   warpgroup 0  TMA producer (one thread; setmaxnreg gives its registers to the consumers)
 //   warpgroups 1, 2  consumers: 64 rows x BLOCK_N columns each, wgmma m64nBLOCK_Nk16 into registers, then the epilogue
-//                    straight from the accumulator registers to global memory
+//                    straight from the accumulator registers to global memory (EPI_RESIDUAL: the tile's residual rows are
+//                    prefetched into L2 before its mainloop and read in batches of independent loads)
 // A ring of 64-wide K stages (~200 KB of shared memory) keeps the next tile's loads in flight during the epilogue.
 #include "common.cuh"
 #include "host_common.h"
@@ -52,7 +53,6 @@ struct Params {
     int M, N, K;
     int ldc;              // elements; for EPI_GATED C has N/2 columns
     int ldr;              // residual row stride
-    int epi;
     const uint16_t* bias;      // [N] 16-bit or nullptr
     const uint16_t* residual;  // [M, ldr] 16-bit or nullptr
     uint16_t* C;
@@ -118,7 +118,8 @@ __device__ __forceinline__ float gelu_new(float x) {
 //              transposing either activation matrix (rows past K are zero-filled by TMA: no padding needed).
 //              wgmma reads 16-bit MN-major tiles through its transpose flags: boxes of {64 MN elements, 64 K rows}, MN
 //              blocks 8 KB apart (descriptor LBO).
-template <bool kBF16, int BLOCK_N, bool kTN>
+// kEpi: the epilogue (EPI_*), a compile-time choice; the MN-major path runs EPI_NONE (or the split-K partial store).
+template <bool kBF16, int BLOCK_N, bool kTN, int kEpi>
 __global__ void __launch_bounds__(THREADS, 1)
 gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b, const Params p) {
     using C = Cfg<BLOCK_N>;
@@ -198,11 +199,25 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ 
     const uint32_t wg = (warp >> 2) - 1u;              // 0 / 1: rows [64 wg, 64 wg + 64) of the tile
     const uint32_t wl = warp & 3u;                     // warp inside the warpgroup
     constexpr int NACC = BLOCK_N / 2;
+    constexpr int RES_BATCH = 8;                       // residual loads in flight per thread
     uint32_t stage = 0, phase = 0;
     for (int t = blockIdx.x; t < num_tiles; t += gridDim.x) {
         const int tile = t / p.splits, split = t % p.splits;
         const int m_blk = tile / num_n, n_blk = tile % num_n;
         const int kb0 = split * p.kb_per_split, kb1 = min(num_kb, kb0 + p.kb_per_split);
+        const int r0 = m_blk * BLOCK_M + static_cast<int>(wg * 64u + wl * 16u + (lane >> 2));
+        const int cq = static_cast<int>(2u * (lane & 3u));
+        if constexpr (kEpi == EPI_RESIDUAL) {
+            // pull this thread's residual rows into L2 while the mainloop runs: the activations are larger than L2, and the
+            // epilogue would otherwise wait out DRAM latency on them (each lane of a quad takes a quarter of the row segment)
+            const int col = n_blk * BLOCK_N + static_cast<int>(lane & 3u) * (BLOCK_N / 4);
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+                const int row = r0 + 8 * h;
+                if (row < p.M && col < p.N)
+                    asm volatile("prefetch.global.L2 [%0];" ::"l"(p.residual + static_cast<size_t>(row) * p.ldr + col));
+            }
+        }
         float acc[NACC];
 #pragma unroll
         for (int i = 0; i < NACC; ++i) acc[i] = 0.f;
@@ -242,8 +257,6 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ 
         if (prev_stage >= 0 && wl == 0 && lane == 0) ab::mbar_arrive(&empty_bar[prev_stage]);
 
         // ---- epilogue straight from the accumulator registers: rows r0 and r0 + 8, column pairs 8 j + 2 (lane % 4)
-        const int r0 = m_blk * BLOCK_M + static_cast<int>(wg * 64u + wl * 16u + (lane >> 2));
-        const int cq = static_cast<int>(2u * (lane & 3u));
 #pragma unroll
         for (int h = 0; h < 2; ++h) {
             const int row = r0 + 8 * h;
@@ -253,34 +266,51 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ 
             float ss_out = 0.f;
             if (row_ok) {
 #pragma unroll
-                for (int j = 0; j < BLOCK_N / 8; ++j) {
+              for (int jb = 0; jb < BLOCK_N / 8; jb += RES_BATCH) {
+                // a batch of independent residual loads issued together, ahead of the batch's stores.  Plain (coherent) loads:
+                // the compiler treats them as possibly aliasing the stores and keeps them in place, whereas read-only (.nc)
+                // loads get sunk to their uses, one dependent memory latency per column pair.
+                uint32_t res[RES_BATCH];
+                if constexpr (kEpi == EPI_RESIDUAL) {
+#pragma unroll
+                    for (int jj = 0; jj < RES_BATCH; ++jj) {
+                        const int col = n_blk * BLOCK_N + 8 * (jb + jj) + cq;
+                        res[jj] = col < p.N ? *reinterpret_cast<const uint32_t*>(p.residual + static_cast<size_t>(row) * p.ldr + col)
+                                            : 0u;
+                    }
+                }
+#pragma unroll
+                for (int jj = 0; jj < RES_BATCH; ++jj) {
+                    const int j = jb + jj;
                     const int col = n_blk * BLOCK_N + 8 * j + cq;
                     if (col >= p.N) continue;
                     float v0 = acc[4 * j + 2 * h], v1 = acc[4 * j + 2 * h + 1];
-                    if (p.C32 != nullptr) {   // split-K partial: raw fp32 accumulator
-                        *reinterpret_cast<float2*>(p.C32 + (static_cast<size_t>(split) * p.M + row) * p.N + col) = make_float2(v0, v1);
-                        continue;
+                    if constexpr (kTN) {
+                        if (p.C32 != nullptr) {   // split-K partial: raw fp32 accumulator
+                            *reinterpret_cast<float2*>(p.C32 + (static_cast<size_t>(split) * p.M + row) * p.N + col) =
+                                make_float2(v0, v1);
+                            continue;
+                        }
                     }
                     v0 *= rscale;
                     v1 *= rscale;
-                    if (p.epi == EPI_GATED) {
+                    if constexpr (kEpi == EPI_GATED) {
                         // columns (2c, 2c+1) = (x.wi_0[c], x.wi_1[c]) -> one output
                         const uint32_t o = pack2<kBF16>(gelu_new(v0) * v1, 0.f);
                         p.C[static_cast<size_t>(row) * p.ldc + (col >> 1)] = static_cast<uint16_t>(o & 0xFFFFu);
                         continue;
                     }
-                    if (p.epi != EPI_NONE && p.bias != nullptr) {
+                    if (kEpi != EPI_NONE && p.bias != nullptr) {
                         const uint32_t b = __ldg(reinterpret_cast<const uint32_t*>(p.bias + col));
                         v0 += to_f32<kBF16>(static_cast<uint16_t>(b & 0xFFFFu));
                         v1 += to_f32<kBF16>(static_cast<uint16_t>(b >> 16));
                     }
-                    if (p.epi == EPI_GELU) {
+                    if constexpr (kEpi == EPI_GELU) {
                         v0 = gelu_erf(v0);
                         v1 = gelu_erf(v1);
-                    } else if (p.epi == EPI_RESIDUAL) {
-                        const uint32_t r = __ldg(reinterpret_cast<const uint32_t*>(p.residual + static_cast<size_t>(row) * p.ldr + col));
-                        v0 += to_f32<kBF16>(static_cast<uint16_t>(r & 0xFFFFu));
-                        v1 += to_f32<kBF16>(static_cast<uint16_t>(r >> 16));
+                    } else if constexpr (kEpi == EPI_RESIDUAL) {
+                        v0 += to_f32<kBF16>(static_cast<uint16_t>(res[jj] & 0xFFFFu));
+                        v1 += to_f32<kBF16>(static_cast<uint16_t>(res[jj] >> 16));
                     }
                     const uint32_t o = pack2<kBF16>(v0, v1);
                     *reinterpret_cast<uint32_t*>(p.C + static_cast<size_t>(row) * p.ldc + col) = o;
@@ -290,6 +320,7 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ 
                         ss_out = fmaf(a, a, fmaf(b, b, ss_out));
                     }
                 }
+              }
             }
             if (p.out_ss != nullptr) {
                 // the four threads of a quad hold the same row
@@ -301,24 +332,31 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ 
     }
 }
 
-template <bool kBF16, int BLOCK_N, bool kTN = false>
+template <bool kBF16, int BLOCK_N, bool kTN, int kEpi>
 static int launch(const CUtensorMap& ta, const CUtensorMap& tb, const Params& p, cudaStream_t s) {
     using C = Cfg<BLOCK_N>;
     static bool attr_set = false;
     if (!attr_set) {
-        AB_CUDA_CHECK(cudaFuncSetAttribute(gemm_kernel<kBF16, BLOCK_N, kTN>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+        AB_CUDA_CHECK(cudaFuncSetAttribute(gemm_kernel<kBF16, BLOCK_N, kTN, kEpi>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                            C::SMEM_BYTES));
         attr_set = true;
     }
     const int tiles = ((p.M + BLOCK_M - 1) / BLOCK_M) * ((p.N + BLOCK_N - 1) / BLOCK_N) * p.splits;
     const int grid = tiles < abh::num_sms() ? tiles : abh::num_sms();
     abh::prof_begin(s, abh::PROF_LINEAR);
-    gemm_kernel<kBF16, BLOCK_N, kTN><<<grid, THREADS, C::SMEM_BYTES, s>>>(ta, tb, p);
+    gemm_kernel<kBF16, BLOCK_N, kTN, kEpi><<<grid, THREADS, C::SMEM_BYTES, s>>>(ta, tb, p);
     if (p.m_dev != nullptr) abh::prof_end_dyn(s, abh::PROF_LINEAR, 2.0 * static_cast<double>(p.N) * p.K, p.m_dev, p.M);
     else abh::prof_end(s, abh::PROF_LINEAR, 2.0 * p.M * static_cast<double>(p.N) * p.K);
     abh::count_launch();
     AB_CUDA_CHECK(cudaGetLastError());
     return ATLAS_B200_OK;
+}
+
+// K-major launch of one epilogue: 16-bit type and tile width chosen at run time
+template <int kEpi>
+static int launch_n(bool bf16, bool wide, const CUtensorMap& ta, const CUtensorMap& tb, const Params& p, cudaStream_t s) {
+    if (bf16) return wide ? launch<true, 256, false, kEpi>(ta, tb, p, s) : launch<true, 128, false, kEpi>(ta, tb, p, s);
+    return wide ? launch<false, 256, false, kEpi>(ta, tb, p, s) : launch<false, 128, false, kEpi>(ta, tb, p, s);
 }
 
 // out[i] = round16(sum_s part[s][i]) for the M*N outputs of a split-K GEMM (8 outputs per thread)
@@ -410,7 +448,6 @@ int atlas_b200_linear_ex(const void* A, int64_t lda, const void* W, int64_t ldw,
     p.K = K;
     p.ldc = static_cast<int>(ldc);
     p.ldr = static_cast<int>(ldr);
-    p.epi = epilogue;
     p.bias = static_cast<const uint16_t*>(bias);
     p.residual = static_cast<const uint16_t*>(residual);
     p.C = static_cast<uint16_t*>(C);
@@ -425,8 +462,13 @@ int atlas_b200_linear_ex(const void* A, int64_t lda, const void* W, int64_t ldw,
                                  static_cast<uint32_t>(block_n), BLOCK_K, is_bf16 != 0);
     if (rc) return rc;
     cudaStream_t s = static_cast<cudaStream_t>(stream);
-    if (is_bf16) return wide ? launch<true, 256>(ta, tb, p, s) : launch<true, 128>(ta, tb, p, s);
-    return wide ? launch<false, 256>(ta, tb, p, s) : launch<false, 128>(ta, tb, p, s);
+    switch (epilogue) {
+        case EPI_NONE: return launch_n<EPI_NONE>(is_bf16 != 0, wide, ta, tb, p, s);
+        case EPI_BIAS: return launch_n<EPI_BIAS>(is_bf16 != 0, wide, ta, tb, p, s);
+        case EPI_GELU: return launch_n<EPI_GELU>(is_bf16 != 0, wide, ta, tb, p, s);
+        case EPI_RESIDUAL: return launch_n<EPI_RESIDUAL>(is_bf16 != 0, wide, ta, tb, p, s);
+        default: return launch_n<EPI_GATED>(is_bf16 != 0, wide, ta, tb, p, s);
+    }
 }
 
 // (tile shape, number of K splits) of a weight-gradient GEMM: minimise the number of waves of work items per split
@@ -480,7 +522,6 @@ int atlas_b200_linear_wgrad(const void* dY, int64_t lddy, const void* X, int64_t
     p.K = tokens;       // contraction  = tokens
     p.ldc = static_cast<int>(lddw);
     p.ldr = 0;
-    p.epi = EPI_NONE;
     p.bias = nullptr;
     p.residual = nullptr;
     p.C = static_cast<uint16_t*>(dW);
@@ -505,8 +546,8 @@ int atlas_b200_linear_wgrad(const void* dY, int64_t lddy, const void* X, int64_t
     rc = abh::make_tmap_2d_16bit(&tb, X, static_cast<uint64_t>(tokens), static_cast<uint64_t>(K), static_cast<uint64_t>(ldx),
                                  BLOCK_K, 64, is_bf16 != 0);
     if (rc) return rc;
-    if (is_bf16) rc = wide ? launch<true, 256, true>(ta, tb, p, s) : launch<true, 128, true>(ta, tb, p, s);
-    else rc = wide ? launch<false, 256, true>(ta, tb, p, s) : launch<false, 128, true>(ta, tb, p, s);
+    if (is_bf16) rc = wide ? launch<true, 256, true, EPI_NONE>(ta, tb, p, s) : launch<true, 128, true, EPI_NONE>(ta, tb, p, s);
+    else rc = wide ? launch<false, 256, true, EPI_NONE>(ta, tb, p, s) : launch<false, 128, true, EPI_NONE>(ta, tb, p, s);
     if (rc || splits == 1) return rc;
     const int64_t vecs = static_cast<int64_t>(N) * (K / 8);
     const int64_t blocks = (vecs + 255) / 256, cap = static_cast<int64_t>(abh::num_sms()) * 8;

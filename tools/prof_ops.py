@@ -34,25 +34,36 @@ elif what == "gemm":
     ms = timed(fn, reps)
     print(f"gemm M={M} N={N} K={K} gated: {ms:.3f} ms = {2 * M * N * K / ms / 1e9:.0f} TFLOP/s")
 elif what == "gemm4":
-    # the four linear-layer shapes of a FiD-base encoder block at 4 queries x 40 passages x 384 tokens, next to cuBLAS
-    # (torch.matmul of the same shape, plain epilogue): ATLAS_B200_GEMM_QUAD=0 selects the 2-CTA pair kernel for A/B runs
-    M = 61440
-    for name, N, K, epi in (("qkv", 2304, 768, None), ("o-proj+res", 768, 768, "res"), ("wi gated", 4096, 768, "gated"),
-                            ("wo+res", 768, 2048, "res")):
+    # the four linear-layer shapes of a FiD-base encoder block at 4 queries x 40 passages x 384 tokens with their fused
+    # epilogues, then the wo projection of the padding-compacted encoder (8 queries x 40 passages, U[148, 276] real tokens
+    # padded to 384, as in `packed`): only the first `count` rows (device-side row count), residual + out_ss; each next to
+    # cuBLAS (torch.matmul of the same computed rows, plain epilogue)
+    S, L = 320, 384
+    lens = torch.randint(148, 277, (S,), device=dev)
+    mask = (torch.arange(L, device=dev)[None, :] >= lens[:, None]).float() * -10000.0
+    count = ops.segment_tile_scan(ops.key_block_live(mask))[3]
+    rows = int(count)
+    for name, M, N, K, epi in (("qkv", 61440, 2304, 768, None), ("o-proj+res", 61440, 768, 768, "res"),
+                               ("wi gated", 61440, 4096, 768, "gated"), ("wo+res", 61440, 768, 2048, "res"),
+                               ("wo+res m_dev", S * L, 768, 2048, "res_rows")):
         x = torch.randn(M, K, device=dev).bfloat16() * 0.1
         w = torch.randn(N, K, device=dev).bfloat16() * 0.03
-        r = torch.randn(M, N, device=dev).bfloat16() if epi == "res" else None
+        r = torch.randn(M, N, device=dev).bfloat16() if epi in ("res", "res_rows") else None
+        ss = torch.zeros(M, device=dev)
         if epi == "gated":
             fn = lambda: ops.linear(x, w, epilogue=ops.EPI_GATED)
         elif epi == "res":
             fn = lambda: ops.linear(x, w, None, residual=r, epilogue=ops.EPI_RESIDUAL)
+        elif epi == "res_rows":
+            fn = lambda: ops.linear(x, w, None, residual=r, epilogue=ops.EPI_RESIDUAL, out_ss=ss, rows=count)
         else:
             fn = lambda: ops.linear(x, w)
         ms = timed(fn, reps)
-        wt = w.t().contiguous()
-        ms_ref = timed(lambda: torch.matmul(x, wt), reps)
-        fl = 2 * M * N * K
-        print(f"gemm {name:12s} M={M} N={N} K={K}: {ms:.3f} ms = {fl / ms / 1e9:.0f} TFLOP/s   cuBLAS plain: {ms_ref:.3f} ms = "
+        m = rows if epi == "res_rows" else M
+        xm, wt = x[:m], w.t().contiguous()
+        ms_ref = timed(lambda: torch.matmul(xm, wt), reps)
+        fl = 2 * m * N * K
+        print(f"gemm {name:12s} M={m} N={N} K={K}: {ms:.3f} ms = {fl / ms / 1e9:.0f} TFLOP/s   cuBLAS plain: {ms_ref:.3f} ms = "
               f"{fl / ms_ref / 1e9:.0f} TFLOP/s")
 elif what == "mips":
     # one 256-query top-40 search over a 4 Mi x 768 fp16 bank (BASELINE configs[1]): for `ncu --metrics gpu__time_duration.sum`
