@@ -84,6 +84,21 @@ __device__ __forceinline__ bool mbar_try_wait(uint64_t* bar, uint32_t parity) {
     return ok != 0;
 }
 
+// non-blocking probe (try_wait may suspend the thread for a while before it reports false)
+__device__ __forceinline__ bool mbar_test_wait(uint64_t* bar, uint32_t parity) {
+    uint32_t ok;
+    asm volatile(
+        "{\n\t"
+        ".reg .pred P;\n\t"
+        "mbarrier.test_wait.parity.shared::cta.b64 P, [%1], %2;\n\t"
+        "selp.u32 %0, 1, 0, P;\n\t"
+        "}\n"
+        : "=r"(ok)
+        : "r"(smem_u32(bar)), "r"(parity)
+        : "memory");
+    return ok != 0;
+}
+
 // Bounded spin: a protocol bug must surface as a trapped launch with a diagnostic, not as a hung GPU.
 // ~2^28 failed probes is several seconds; every wait site passes a distinct `tag`.
 #ifndef AB_WATCHDOG_SPINS
@@ -152,6 +167,17 @@ __device__ __forceinline__ void tma_prefetch_2d(const CUtensorMap* map, int32_t 
     asm volatile("cp.async.bulk.prefetch.tensor.2d.L2.global [%0, {%1, %2}];" ::"l"(reinterpret_cast<uint64_t>(map)), "r"(c0),
                  "r"(c1)
                  : "memory");
+}
+
+// ---------------------------------------------------------------------------------------------
+// named CTA barriers (ids 1..15; 0 is __syncthreads): `count` threads take part, a multiple of 32.  The non-aligned
+// forms, so a warp that just left a single-thread branch may execute them.
+// ---------------------------------------------------------------------------------------------
+__device__ __forceinline__ void named_bar_sync(uint32_t id, uint32_t count) {
+    asm volatile("barrier.sync %0, %1;" ::"r"(id), "r"(count) : "memory");
+}
+__device__ __forceinline__ void named_bar_arrive(uint32_t id, uint32_t count) {
+    asm volatile("barrier.arrive %0, %1;" ::"r"(id), "r"(count) : "memory");
 }
 
 // ---------------------------------------------------------------------------------------------

@@ -16,13 +16,22 @@
 //   EPI_GATED     C[m, j] = gelu_new(acc[m, 2j]) * acc[m, 2j+1]    (W rows interleaved wi_0/wi_1;
 //                                                                   modeling_t5.py:281-285, fp32 GELU)
 //
-// Persistent, warp-specialised, one CTA per SM (grid = #SMs), 128 x BLOCK_N tiles (BLOCK_N = 256 once there are enough
-// tiles to fill the SMs, else 128):
-//   warpgroup 0  TMA producer (one thread; setmaxnreg gives its registers to the consumers)
-//   warpgroups 1, 2  consumers: 64 rows x BLOCK_N columns each, wgmma m64nBLOCK_Nk16 into registers, then the epilogue
-//                    straight from the accumulator registers to global memory (EPI_RESIDUAL: the tile's residual rows are
-//                    prefetched into L2 before its mainloop and read in batches of independent loads)
-// A ring of 64-wide K stages (~200 KB of shared memory) keeps the next tile's loads in flight during the epilogue.
+// Persistent, warp-specialised, one CTA per SM (grid = #SMs): warpgroup 0 is the TMA producer (one thread; setmaxnreg
+// gives its registers to the consumers), warpgroups 1 and 2 are consumers.  Two schedules:
+//   ping-pong (gemm_pp_kernel; K-major launches of at least 2 x #SMs 128 x 128 tiles, i.e. the encoder projections, the
+//     cross-attention K|V projection and the LM head at 256 rows x 32128): each consumer owns whole 128 x 128 tiles, two wgmma m64n128k16 per k16 step
+//     sharing the W descriptor; a CTA's work items alternate between the consumers, which take turns in the mainloop, so
+//     one consumer's epilogue runs under the other's MMAs.  The epilogue goes through a per-consumer 32 KB staging buffer
+//     (128-byte swizzle) and a TMA store; EPI_RESIDUAL's residual tile is loaded into that buffer by the producer during
+//     the item's mainloop.  5 stages of 32 KB.
+//   cooperative (gemm_kernel; smaller launches - the decoder's other 256-row GEMMs, Contriever's query batch - and
+//     the MN-major weight-gradient / split-K path): both consumers share one 128 x BLOCK_N tile (BLOCK_N = 256 once there
+//     are enough tiles to fill the SMs, else 128), 64 rows each, wgmma m64nBLOCK_Nk16, then the epilogue straight from the
+//     accumulator registers to global memory (EPI_RESIDUAL: the tile's residual rows are prefetched into L2 before its
+//     mainloop and read in batches of independent loads).  A ring of 64-wide K stages (~200 KB).
+// The choice depends only on the shape (and, for EPI_RESIDUAL, on a 16-byte aligned residual, which its tensor map needs).
+// Both schedules run each output element through the same sequence of k16 MMAs and the same epilogue arithmetic
+// (epilogue_pair), so they give bit-identical results.
 #include "common.cuh"
 #include "host_common.h"
 #include "wgmma.cuh"
@@ -110,6 +119,46 @@ __device__ __forceinline__ float gelu_new(float x) {
     asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(e) : "f"(-1.4426950408889634f * u2));
     asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(r) : "f"(1.0f + e));
     return x * r;
+}
+
+// ---- the fused epilogue, shared by both schedules: the same fp32 operations in the same order, one rounding to 16 bits
+// rsqrt(row_ss / K + eps) of output row `row` (fused RMSNorm), or 1
+__device__ __forceinline__ float row_scale(const Params& p, int row, bool row_ok) {
+    return (p.row_ss != nullptr && row_ok) ? rsqrtf(__ldg(p.row_ss + row) / static_cast<float>(p.K) + p.rs_eps) : 1.0f;
+}
+// accumulators (v0, v1) of columns (col, col + 1) -> the packed 16-bit pair to store; `res` is the packed residual pair
+// (EPI_RESIDUAL).  EPI_GATED: columns (2c, 2c+1) = (x.wi_0[c], x.wi_1[c]) -> one output, in the low half.
+template <bool kBF16, int kEpi>
+__device__ __forceinline__ uint32_t epilogue_pair(const Params& p, float v0, float v1, float rscale, int col, uint32_t res) {
+    v0 *= rscale;
+    v1 *= rscale;
+    if constexpr (kEpi == EPI_GATED) return pack2<kBF16>(gelu_new(v0) * v1, 0.f);
+    if (kEpi != EPI_NONE && p.bias != nullptr) {
+        const uint32_t b = __ldg(reinterpret_cast<const uint32_t*>(p.bias + col));
+        v0 += to_f32<kBF16>(static_cast<uint16_t>(b & 0xFFFFu));
+        v1 += to_f32<kBF16>(static_cast<uint16_t>(b >> 16));
+    }
+    if constexpr (kEpi == EPI_GELU) {
+        v0 = gelu_erf(v0);
+        v1 = gelu_erf(v1);
+    } else if constexpr (kEpi == EPI_RESIDUAL) {
+        v0 += to_f32<kBF16>(static_cast<uint16_t>(res & 0xFFFFu));
+        v1 += to_f32<kBF16>(static_cast<uint16_t>(res >> 16));
+    }
+    return pack2<kBF16>(v0, v1);
+}
+// out_ss: squares of the values as STORED (what a separate norm would read)
+template <bool kBF16>
+__device__ __forceinline__ float add_sq_pair(uint32_t o, float ss) {
+    const float a = to_f32<kBF16>(static_cast<uint16_t>(o & 0xFFFFu));
+    const float b = to_f32<kBF16>(static_cast<uint16_t>(o >> 16));
+    return fmaf(a, a, fmaf(b, b, ss));
+}
+// the four threads of a quad hold the same row: one atomicAdd per row and quad (every lane of the warp calls this)
+__device__ __forceinline__ void out_ss_add(const Params& p, int row, bool row_ok, uint32_t lane, float ss) {
+    ss += __shfl_xor_sync(0xffffffffu, ss, 1);
+    ss += __shfl_xor_sync(0xffffffffu, ss, 2);
+    if (row_ok && (lane & 3u) == 0u) atomicAdd(p.out_ss + row, ss);
 }
 
 // kTN = false: C = A[M, K] . W[N, K]^T, both operands K-major (activations x nn.Linear weight).
@@ -261,8 +310,7 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ 
         for (int h = 0; h < 2; ++h) {
             const int row = r0 + 8 * h;
             const bool row_ok = row < p.M;
-            const float rscale = (p.row_ss != nullptr && row_ok)
-                                     ? rsqrtf(__ldg(p.row_ss + row) / static_cast<float>(p.K) + p.rs_eps) : 1.0f;
+            const float rscale = row_scale(p, row, row_ok);
             float ss_out = 0.f;
             if (row_ok) {
 #pragma unroll
@@ -284,7 +332,7 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ 
                     const int j = jb + jj;
                     const int col = n_blk * BLOCK_N + 8 * j + cq;
                     if (col >= p.N) continue;
-                    float v0 = acc[4 * j + 2 * h], v1 = acc[4 * j + 2 * h + 1];
+                    const float v0 = acc[4 * j + 2 * h], v1 = acc[4 * j + 2 * h + 1];
                     if constexpr (kTN) {
                         if (p.C32 != nullptr) {   // split-K partial: raw fp32 accumulator
                             *reinterpret_cast<float2*>(p.C32 + (static_cast<size_t>(split) * p.M + row) * p.N + col) =
@@ -292,44 +340,230 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ 
                             continue;
                         }
                     }
-                    v0 *= rscale;
-                    v1 *= rscale;
+                    const uint32_t o = epilogue_pair<kBF16, kEpi>(p, v0, v1, rscale, col,
+                                                                  kEpi == EPI_RESIDUAL ? res[jj] : 0u);
                     if constexpr (kEpi == EPI_GATED) {
-                        // columns (2c, 2c+1) = (x.wi_0[c], x.wi_1[c]) -> one output
-                        const uint32_t o = pack2<kBF16>(gelu_new(v0) * v1, 0.f);
                         p.C[static_cast<size_t>(row) * p.ldc + (col >> 1)] = static_cast<uint16_t>(o & 0xFFFFu);
                         continue;
                     }
-                    if (kEpi != EPI_NONE && p.bias != nullptr) {
-                        const uint32_t b = __ldg(reinterpret_cast<const uint32_t*>(p.bias + col));
-                        v0 += to_f32<kBF16>(static_cast<uint16_t>(b & 0xFFFFu));
-                        v1 += to_f32<kBF16>(static_cast<uint16_t>(b >> 16));
-                    }
-                    if constexpr (kEpi == EPI_GELU) {
-                        v0 = gelu_erf(v0);
-                        v1 = gelu_erf(v1);
-                    } else if constexpr (kEpi == EPI_RESIDUAL) {
-                        v0 += to_f32<kBF16>(static_cast<uint16_t>(res[jj] & 0xFFFFu));
-                        v1 += to_f32<kBF16>(static_cast<uint16_t>(res[jj] >> 16));
-                    }
-                    const uint32_t o = pack2<kBF16>(v0, v1);
                     *reinterpret_cast<uint32_t*>(p.C + static_cast<size_t>(row) * p.ldc + col) = o;
-                    if (p.out_ss != nullptr) {   // squares of the values as STORED (what a separate norm would read)
-                        const float a = to_f32<kBF16>(static_cast<uint16_t>(o & 0xFFFFu));
-                        const float b = to_f32<kBF16>(static_cast<uint16_t>(o >> 16));
-                        ss_out = fmaf(a, a, fmaf(b, b, ss_out));
-                    }
+                    if (p.out_ss != nullptr) ss_out = add_sq_pair<kBF16>(o, ss_out);
                 }
               }
             }
-            if (p.out_ss != nullptr) {
-                // the four threads of a quad hold the same row
-                ss_out += __shfl_xor_sync(0xffffffffu, ss_out, 1);
-                ss_out += __shfl_xor_sync(0xffffffffu, ss_out, 2);
-                if (row_ok && (lane & 3u) == 0u) atomicAdd(p.out_ss + row, ss_out);
-            }
+            if (p.out_ss != nullptr) out_ss_add(p, row, row_ok, lane, ss_out);
         }
     }
+}
+
+// ===================== ping-pong schedule (K-major, 128 x 128 tiles, encoder-sized launches) =====================
+namespace pp {
+constexpr int BLOCK_N = 128;
+constexpr int STAGE_BYTES = (BLOCK_M + BLOCK_N) * BLOCK_K * 2;      // 32 KB: A 128 x 64, W 128 x 64
+constexpr int EPI_BYTES = BLOCK_M * BLOCK_N * 2;                    // 32 KB staging tile per consumer: two 128 x 64 boxes
+constexpr int STAGES = (227 * 1024 - 1024 - CONSUMERS * EPI_BYTES) / STAGE_BYTES;    // 5
+constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + CONSUMERS * EPI_BYTES + 1024;
+// named barriers: consumer c waits on ORDER_BAR + c for its turn in the mainloop; EPI_BAR + c syncs its 128 threads
+constexpr uint32_t ORDER_BAR = 1, EPI_BAR = 3;
+// byte offset of element (r, c) in a 128-row box of 64 16-bit columns written with the 128-byte swizzle (what TMA
+// reads and writes): 16-byte chunk c / 8 of row r lands at chunk (c / 8) ^ (r % 8)
+__device__ __forceinline__ uint32_t sw128_offset(int r, int c) {
+    return static_cast<uint32_t>(r * 128 + ((((c >> 3) ^ r) & 7) << 4) + ((c & 7) << 1));
+}
+}  // namespace pp
+
+// Each consumer warpgroup owns whole 128 x 128 tiles: the CTA's work items alternate between the consumers (item i ->
+// consumer i % 2).  The producer loads the stages of every item in order into one ring; the consumers take turns in the
+// mainloop (named barriers), so one consumer's epilogue runs while the other issues MMAs.  The epilogue writes the tile
+// into the consumer's shared-memory staging buffer, and one thread stores it with TMA through the tensor map of C, whose
+// extent clips ragged edges (and keeps a strided view's neighbouring columns untouched).  EPI_RESIDUAL: the producer
+// loads the residual tile into that buffer with TMA during the item's mainloop; the epilogue adds it in place.
+template <bool kBF16, int kEpi>
+__global__ void __launch_bounds__(THREADS, 1)
+gemm_pp_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
+               const __grid_constant__ CUtensorMap tmap_c, const __grid_constant__ CUtensorMap tmap_r, const Params p) {
+    using namespace pp;
+    extern __shared__ uint8_t smem_raw[];
+    __shared__ __align__(8) uint64_t full_bar[STAGES];
+    __shared__ __align__(8) uint64_t empty_bar[STAGES];
+    __shared__ __align__(8) uint64_t res_full[CONSUMERS];     // residual tile landed in the staging buffer
+    __shared__ __align__(8) uint64_t res_empty[CONSUMERS];    // staging buffer read out by the previous TMA store
+
+    const uint32_t warp = threadIdx.x >> 5;
+    const uint32_t lane = threadIdx.x & 31u;
+    const uint32_t smem_base = (ab::smem_u32(smem_raw) + 1023u) & ~1023u;
+    uint8_t* smem_gen = smem_raw + (smem_base - ab::smem_u32(smem_raw));
+    uint8_t* epi_gen = smem_gen + STAGES * STAGE_BYTES;
+
+    const int m_rows = p.m_dev != nullptr ? min(p.M, max(__ldg(p.m_dev), 0)) : p.M;     // identical in every role
+    const int num_m = (m_rows + BLOCK_M - 1) / BLOCK_M;
+    const int num_n = (p.N + BLOCK_N - 1) / BLOCK_N;
+    const int num_tiles = num_m * num_n;
+    const int num_kb = (p.K + BLOCK_K - 1) / BLOCK_K;
+
+    if (threadIdx.x == 0) {
+        ab::tma_prefetch_desc(&tmap_a);
+        ab::tma_prefetch_desc(&tmap_b);
+        ab::tma_prefetch_desc(&tmap_c);
+        if constexpr (kEpi == EPI_RESIDUAL) ab::tma_prefetch_desc(&tmap_r);
+        for (int s = 0; s < STAGES; ++s) {
+            ab::mbar_init(&full_bar[s], 1);
+            ab::mbar_init(&empty_bar[s], 1);                  // one consumer per stage
+        }
+        for (int c = 0; c < CONSUMERS; ++c) {
+            ab::mbar_init(&res_full[c], 1);
+            ab::mbar_init(&res_empty[c], 1);
+        }
+        ab::fence_barrier_init();
+    }
+    __syncthreads();
+
+    if (warp < 4) {
+        // ===================== producer warpgroup (one thread issues the TMA loads) =====================
+        ab::setmaxnreg_dec<40>();
+        if (warp == 0 && lane == 0) {
+            uint32_t stage = 0, phase = 0;
+            int i = 0;
+            for (int t = blockIdx.x; t < num_tiles; t += gridDim.x, ++i) {
+                const int m_blk = t / num_n, n_blk = t % num_n;
+                const int a_row = m_blk * BLOCK_M;
+                const int b_row = n_blk * BLOCK_N;
+                // L2 prefetch of the A rows of this CTA's NEXT work item when it starts a new row block
+                int pf_row = -1;
+                const int t2 = t + static_cast<int>(gridDim.x);
+                if (p.l2_prefetch && t2 < num_tiles && t2 % num_n == 0) pf_row = (t2 / num_n) * BLOCK_M;
+                bool res_issued = false;
+                for (int kb = 0; kb < num_kb; ++kb) {
+                    if (pf_row >= 0) ab::tma_prefetch_2d(&tmap_a, kb * BLOCK_K, pf_row);
+                    ab::mbar_wait_nocall(&empty_bar[stage], phase ^ 1u);
+                    uint8_t* st = smem_gen + stage * STAGE_BYTES;
+                    ab::mbar_arrive_expect_tx(&full_bar[stage], STAGE_BYTES);
+                    ab::tma_load_2d(&tmap_a, &full_bar[stage], st, kb * BLOCK_K, a_row, ab::kEvictNormal);
+                    ab::tma_load_2d(&tmap_b, &full_bar[stage], st + BLOCK_M * BLOCK_K * 2, kb * BLOCK_K, b_row,
+                                    ab::kEvictLast);
+                    if (++stage == STAGES) {
+                        stage = 0;
+                        phase ^= 1u;
+                    }
+                    if constexpr (kEpi == EPI_RESIDUAL) {
+                        // the residual tile, as early in the item's mainloop as its consumer's staging buffer is free (the
+                        // store of that consumer's previous tile has read it).  The buffer is probed after each k-block
+                        // and waited for only after the last one, so the stage loads never stall on it.
+                        const int c = i & 1;
+                        const uint32_t par = ((static_cast<uint32_t>(i >> 1)) & 1u) ^ 1u;
+                        if (!res_issued && (kb == num_kb - 1 || ab::mbar_test_wait(&res_empty[c], par))) {
+                            ab::mbar_wait_nocall(&res_empty[c], par);
+                            res_issued = true;
+                            uint8_t* buf = epi_gen + c * EPI_BYTES;
+                            ab::mbar_arrive_expect_tx(&res_full[c], EPI_BYTES);
+                            ab::tma_load_2d(&tmap_r, &res_full[c], buf, b_row, a_row, ab::kEvictFirst);
+                            ab::tma_load_2d(&tmap_r, &res_full[c], buf + EPI_BYTES / 2, b_row + 64, a_row, ab::kEvictFirst);
+                        }
+                    }
+                }
+            }
+        }
+        return;
+    }
+
+    // ===================== consumer warpgroups: whole 128 x 128 tiles, alternating =====================
+    ab::setmaxnreg_inc<232>();
+    const uint32_t wg = (warp >> 2) - 1u;              // consumer 0 / 1
+    const uint32_t wl = warp & 3u;                     // warp inside the warpgroup
+    const uint32_t ctid = threadIdx.x & 127u;
+    uint8_t* buf = epi_gen + wg * EPI_BYTES;
+    const int cq = static_cast<int>(2u * (lane & 3u));
+    const int stride = static_cast<int>(gridDim.x);
+    int i = static_cast<int>(wg);
+    for (int t = blockIdx.x + i * stride; t < num_tiles; t += 2 * stride, i += 2) {
+        const int m_blk = t / num_n, n_blk = t % num_n;
+        // this item's first stage: every item has num_kb k-blocks, loaded in item order
+        const int pos = i * num_kb;
+        uint32_t stage = static_cast<uint32_t>(pos % STAGES), phase = static_cast<uint32_t>((pos / STAGES) & 1);
+        // wait for the other consumer to have issued the previous item's mainloop.  Consumer 0's first item has no
+        // predecessor.  This barrier also covers the previous store of this consumer's staging buffer: the thread that
+        // issued it arrives here only after waiting for the store to have read the buffer.
+        if (i > 0) ab::named_bar_sync(ORDER_BAR + wg, 256);
+        float acc[2][64];
+#pragma unroll
+        for (int h = 0; h < 2; ++h)
+#pragma unroll
+            for (int q = 0; q < 64; ++q) acc[h][q] = 0.f;
+        int prev_stage = -1;
+        for (int kb = 0; kb < num_kb; ++kb) {
+            ab::mbar_wait_nocall(&full_bar[stage], phase);
+            const uint32_t st = smem_base + stage * STAGE_BYTES;
+            ab::wgmma_fence();
+#pragma unroll
+            for (int k = 0; k < BLOCK_K / UMMA_K; ++k) {
+                const uint64_t bdesc = ab::wgmma_desc_sw128(st + BLOCK_M * BLOCK_K * 2 + k * 32u);
+                ab::wgmma_m64n128k16_ss<kBF16, 0, 0>(acc[0], ab::wgmma_desc_sw128(st + k * 32u), bdesc, 1);
+                ab::wgmma_m64n128k16_ss<kBF16, 0, 0>(acc[1], ab::wgmma_desc_sw128(st + 8192u + k * 32u), bdesc, 1);
+            }
+            ab::wgmma_commit();
+            // the previous stage's MMAs have retired once at most this stage's group is pending: release it
+            ab::wgmma_wait<1>();
+            ab::wgmma_reg_fence(acc[0]);
+            ab::wgmma_reg_fence(acc[1]);
+            if (prev_stage >= 0 && ctid == 0) ab::mbar_arrive(&empty_bar[prev_stage]);
+            prev_stage = static_cast<int>(stage);
+            if (++stage == STAGES) {
+                stage = 0;
+                phase ^= 1u;
+            }
+        }
+        // the other consumer's turn (if it has a next item)
+        if (t + stride < num_tiles) ab::named_bar_arrive(ORDER_BAR + (wg ^ 1u), 256);
+        ab::wgmma_wait<0>();
+        ab::wgmma_reg_fence(acc[0]);
+        ab::wgmma_reg_fence(acc[1]);
+        if (prev_stage >= 0 && ctid == 0) ab::mbar_arrive(&empty_bar[prev_stage]);
+
+        // ---- epilogue into the staging buffer: rows 64 mh + 16 wl + lane / 4 (+ 8), column pairs 8 j + 2 (lane % 4)
+        if constexpr (kEpi == EPI_RESIDUAL) ab::mbar_wait_nocall(&res_full[wg], static_cast<uint32_t>((i >> 1) & 1));
+#pragma unroll
+        for (int mh = 0; mh < 2; ++mh) {
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+                const int r = mh * 64 + static_cast<int>(wl * 16u + (lane >> 2)) + 8 * h;    // row in the tile
+                const int row = m_blk * BLOCK_M + r;
+                const bool row_ok = row < p.M;
+                const float rscale = row_scale(p, row, row_ok);
+                float ss_out = 0.f;
+#pragma unroll
+                for (int j = 0; j < BLOCK_N / 8; ++j) {
+                    const int c = 8 * j + cq;                                                  // column in the tile
+                    const int col = n_blk * BLOCK_N + c;
+                    if (col >= p.N) continue;                  // past the edge: the TMA store clips it
+                    uint8_t* dst = buf + (c >> 6) * (EPI_BYTES / 2) + sw128_offset(r, c & 63);
+                    const uint32_t res = kEpi == EPI_RESIDUAL ? *reinterpret_cast<const uint32_t*>(dst) : 0u;
+                    const uint32_t o = epilogue_pair<kBF16, kEpi>(p, acc[mh][4 * j + 2 * h], acc[mh][4 * j + 2 * h + 1],
+                                                                  rscale, col, res);
+                    if constexpr (kEpi == EPI_GATED) {
+                        *reinterpret_cast<uint16_t*>(buf + sw128_offset(r, c >> 1)) = static_cast<uint16_t>(o & 0xFFFFu);
+                    } else {
+                        *reinterpret_cast<uint32_t*>(dst) = o;
+                        if (p.out_ss != nullptr) ss_out = add_sq_pair<kBF16>(o, ss_out);
+                    }
+                }
+                if (kEpi != EPI_GATED && p.out_ss != nullptr) out_ss_add(p, row, row_ok, lane, ss_out);
+            }
+        }
+        ab::fence_proxy_async_smem();                  // generic-proxy writes -> visible to the TMA store
+        ab::named_bar_sync(EPI_BAR + wg, 128);
+        if (ctid == 0) {
+            if constexpr (kEpi == EPI_GATED) {
+                ab::tma_store_2d(&tmap_c, buf, n_blk * (BLOCK_N / 2), m_blk * BLOCK_M);
+            } else {
+                ab::tma_store_2d(&tmap_c, buf, n_blk * BLOCK_N, m_blk * BLOCK_M);
+                ab::tma_store_2d(&tmap_c, buf + EPI_BYTES / 2, n_blk * BLOCK_N + 64, m_blk * BLOCK_M);
+            }
+            ab::tma_store_commit();
+            ab::tma_store_wait_read();
+            if constexpr (kEpi == EPI_RESIDUAL) ab::mbar_arrive(&res_empty[wg]);
+        }
+    }
+    if (ctid == 0) ab::tma_store_wait_all();
 }
 
 template <bool kBF16, int BLOCK_N, bool kTN, int kEpi>
@@ -357,6 +591,32 @@ template <int kEpi>
 static int launch_n(bool bf16, bool wide, const CUtensorMap& ta, const CUtensorMap& tb, const Params& p, cudaStream_t s) {
     if (bf16) return wide ? launch<true, 256, false, kEpi>(ta, tb, p, s) : launch<true, 128, false, kEpi>(ta, tb, p, s);
     return wide ? launch<false, 256, false, kEpi>(ta, tb, p, s) : launch<false, 128, false, kEpi>(ta, tb, p, s);
+}
+
+template <bool kBF16, int kEpi>
+static int launch_pp(const CUtensorMap& ta, const CUtensorMap& tb, const CUtensorMap& tc, const CUtensorMap& tr, const Params& p,
+                     cudaStream_t s) {
+    static bool attr_set = false;
+    if (!attr_set) {
+        AB_CUDA_CHECK(cudaFuncSetAttribute(gemm_pp_kernel<kBF16, kEpi>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                           pp::SMEM_BYTES));
+        attr_set = true;
+    }
+    const int tiles = ((p.M + BLOCK_M - 1) / BLOCK_M) * ((p.N + pp::BLOCK_N - 1) / pp::BLOCK_N);
+    const int grid = tiles < abh::num_sms() ? tiles : abh::num_sms();
+    abh::prof_begin(s, abh::PROF_LINEAR);
+    gemm_pp_kernel<kBF16, kEpi><<<grid, THREADS, pp::SMEM_BYTES, s>>>(ta, tb, tc, tr, p);
+    if (p.m_dev != nullptr) abh::prof_end_dyn(s, abh::PROF_LINEAR, 2.0 * static_cast<double>(p.N) * p.K, p.m_dev, p.M);
+    else abh::prof_end(s, abh::PROF_LINEAR, 2.0 * p.M * static_cast<double>(p.N) * p.K);
+    abh::count_launch();
+    AB_CUDA_CHECK(cudaGetLastError());
+    return ATLAS_B200_OK;
+}
+
+template <int kEpi>
+static int launch_pp_t(bool bf16, const CUtensorMap& ta, const CUtensorMap& tb, const CUtensorMap& tc, const CUtensorMap& tr,
+                       const Params& p, cudaStream_t s) {
+    return bf16 ? launch_pp<true, kEpi>(ta, tb, tc, tr, p, s) : launch_pp<false, kEpi>(ta, tb, tc, tr, p, s);
 }
 
 // out[i] = round16(sum_s part[s][i]) for the M*N outputs of a split-K GEMM (8 outputs per thread)
@@ -451,8 +711,15 @@ int atlas_b200_linear_ex(const void* A, int64_t lda, const void* W, int64_t ldw,
     p.bias = static_cast<const uint16_t*>(bias);
     p.residual = static_cast<const uint16_t*>(residual);
     p.C = static_cast<uint16_t*>(C);
-    // 128 x 256 tiles once there are enough of them to fill the SMs (encoder-sized M), else 128 x 128
-    const bool wide = N >= 256 && (static_cast<int64_t>((M + 127) / 128) * ((N + 255) / 256) >= abh::num_sms());
+    cudaStream_t s = static_cast<cudaStream_t>(stream);
+    // ping-pong once every consumer warpgroup has at least one 128 x 128 tile (encoder-sized M, or the 32128-column LM
+    // head); the residual goes
+    // through a tensor map, which needs a 16-byte aligned base
+    const int64_t tiles128 = static_cast<int64_t>((M + 127) / 128) * ((N + 127) / 128);
+    const bool pingpong = tiles128 >= 2 * abh::num_sms() &&
+                          (epilogue != EPI_RESIDUAL || (reinterpret_cast<uintptr_t>(residual) & 15u) == 0);
+    // cooperative: 128 x 256 tiles once there are enough of them to fill the SMs, else 128 x 128
+    const bool wide = !pingpong && N >= 256 && (static_cast<int64_t>((M + 127) / 128) * ((N + 255) / 256) >= abh::num_sms());
     const int block_n = wide ? 256 : 128;
     CUtensorMap ta, tb;
     int rc = abh::make_tmap_2d_16bit(&ta, A, static_cast<uint64_t>(M), static_cast<uint64_t>(K),
@@ -461,7 +728,28 @@ int atlas_b200_linear_ex(const void* A, int64_t lda, const void* W, int64_t ldw,
     rc = abh::make_tmap_2d_16bit(&tb, W, static_cast<uint64_t>(N), static_cast<uint64_t>(K), static_cast<uint64_t>(ldw),
                                  static_cast<uint32_t>(block_n), BLOCK_K, is_bf16 != 0);
     if (rc) return rc;
-    cudaStream_t s = static_cast<cudaStream_t>(stream);
+    if (pingpong) {
+        // C (N / 2 columns for EPI_GATED) and the residual in 128-row boxes of 64 columns
+        CUtensorMap tc, tr;
+        const uint64_t n_out = static_cast<uint64_t>(epilogue == EPI_GATED ? N / 2 : N);
+        rc = abh::make_tmap_2d_16bit(&tc, C, static_cast<uint64_t>(M), n_out, static_cast<uint64_t>(ldc), BLOCK_M, 64,
+                                     is_bf16 != 0);
+        if (rc) return rc;
+        if (epilogue == EPI_RESIDUAL) {
+            rc = abh::make_tmap_2d_16bit(&tr, residual, static_cast<uint64_t>(M), static_cast<uint64_t>(N),
+                                         static_cast<uint64_t>(ldr), BLOCK_M, 64, is_bf16 != 0);
+            if (rc) return rc;
+        } else {
+            tr = tc;                                   // unused
+        }
+        switch (epilogue) {
+            case EPI_NONE: return launch_pp_t<EPI_NONE>(is_bf16 != 0, ta, tb, tc, tr, p, s);
+            case EPI_BIAS: return launch_pp_t<EPI_BIAS>(is_bf16 != 0, ta, tb, tc, tr, p, s);
+            case EPI_GELU: return launch_pp_t<EPI_GELU>(is_bf16 != 0, ta, tb, tc, tr, p, s);
+            case EPI_RESIDUAL: return launch_pp_t<EPI_RESIDUAL>(is_bf16 != 0, ta, tb, tc, tr, p, s);
+            default: return launch_pp_t<EPI_GATED>(is_bf16 != 0, ta, tb, tc, tr, p, s);
+        }
+    }
     switch (epilogue) {
         case EPI_NONE: return launch_n<EPI_NONE>(is_bf16 != 0, wide, ta, tb, p, s);
         case EPI_BIAS: return launch_n<EPI_BIAS>(is_bf16 != 0, wide, ta, tb, p, s);

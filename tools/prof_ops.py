@@ -1,4 +1,4 @@
-"""Single-op drivers for ncu captures: python tools/prof_ops.py attention|gemm|contriever|fid [reps]."""
+"""Single-op drivers for ncu captures: python tools/prof_ops.py attention|gemm|gemm4|gemm_small|contriever|fid [reps]."""
 import os, sys
 import torch
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -17,6 +17,19 @@ def timed(fn, n=10, warm=3):
     for _ in range(n): fn()
     e1.record(); torch.cuda.synchronize()
     return e0.elapsed_time(e1) / n
+
+def graph_timed(fn, n=20, reps=10):
+    """Device time of one fn() call: n calls captured into a CUDA graph, replayed `reps` times (a launch that takes a few
+    microseconds on the GPU takes longer than that to issue from Python, so timing eager calls measures the host)."""
+    s = torch.cuda.Stream()
+    s.wait_stream(torch.cuda.current_stream())
+    with torch.cuda.stream(s):
+        for _ in range(3): fn()
+    torch.cuda.current_stream().wait_stream(s)
+    g = torch.cuda.CUDAGraph()
+    with torch.cuda.graph(g):
+        for _ in range(n): fn()
+    return timed(g.replay, reps) / n
 
 if what == "attention":
     S, H, L = 160, 12, 384      # FiD-base encoder, 4 queries x 40 passages
@@ -65,6 +78,45 @@ elif what == "gemm4":
         fl = 2 * m * N * K
         print(f"gemm {name:12s} M={m} N={N} K={K}: {ms:.3f} ms = {fl / ms / 1e9:.0f} TFLOP/s   cuBLAS plain: {ms_ref:.3f} ms = "
               f"{fl / ms_ref / 1e9:.0f} TFLOP/s")
+elif what == "gemm_small":
+    # both sides of the schedule selection (ping-pong from 2 x #SMs 128 x 128 tiles): the decoder's cross-attention K|V
+    # projection over the packed encoder rows (linear_dynm, device-side row count, ping-pong), then 256-row decoder-sized
+    # launches (8 queries x 32 target tokens) with each epilogue: cooperative, except the LM head (2 x 251 tiles of
+    # 128 x 128: ping-pong); each next to cuBLAS plain on the same rows, all timed inside CUDA graphs
+    S, L = 320, 384
+    lens = torch.randint(148, 277, (S,), device=dev)
+    mask = (torch.arange(L, device=dev)[None, :] >= lens[:, None]).float() * -10000.0
+    count = ops.segment_tile_scan(ops.key_block_live(mask))[3]
+    rows = int(count)
+    shapes = [("cross K|V", S * L, 1536, 768, "dynm")]
+    shapes += [(f"dec {nm}", 256, N, K, epi) for nm, N, K, epi in
+               (("qkv", 2304, 768, None), ("o+res", 768, 768, "res"), ("wi gated", 4096, 768, "gated"),
+                ("wo+res", 768, 2048, "res"), ("bias", 768, 768, "bias"), ("gelu", 3072, 768, "gelu"),
+                ("lm_head", 32128, 768, None))]
+    for name, M, N, K, epi in shapes:
+        x = torch.randn(M, K, device=dev).bfloat16() * 0.1
+        w = torch.randn(N, K, device=dev).bfloat16() * 0.03
+        b = torch.randn(N, device=dev).bfloat16() * 0.1
+        r = torch.randn(M, N, device=dev).bfloat16() if epi == "res" else None
+        if epi == "dynm":
+            fn = lambda: ops.linear_dynm(x, w, count)
+        elif epi == "gated":
+            fn = lambda: ops.linear(x, w, epilogue=ops.EPI_GATED)
+        elif epi == "res":
+            fn = lambda: ops.linear(x, w, b, residual=r, epilogue=ops.EPI_RESIDUAL)
+        elif epi == "bias":
+            fn = lambda: ops.linear(x, w, b, epilogue=ops.EPI_BIAS)
+        elif epi == "gelu":
+            fn = lambda: ops.linear(x, w, b, epilogue=ops.EPI_GELU)
+        else:
+            fn = lambda: ops.linear(x, w)
+        ms = graph_timed(fn, reps=reps)
+        m = rows if epi == "dynm" else M
+        xm, wt = x[:m], w.t().contiguous()
+        ms_ref = graph_timed(lambda: torch.matmul(xm, wt), reps=reps)
+        fl = 2 * m * N * K
+        print(f"gemm {name:12s} M={m} N={N} K={K}: {ms * 1e3:.1f} us = {fl / ms / 1e9:.0f} TFLOP/s   cuBLAS plain: "
+              f"{ms_ref * 1e3:.1f} us = {fl / ms_ref / 1e9:.0f} TFLOP/s")
 elif what == "mips":
     # one 256-query top-40 search over a 4 Mi x 768 fp16 bank (BASELINE configs[1]): for `ncu --metrics gpu__time_duration.sum`
     n, nq, k = 4 * 1024 * 1024, 256, 40
