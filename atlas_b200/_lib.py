@@ -59,8 +59,6 @@ def lib():
     ]
     L.atlas_b200_cast_f32.restype = c.c_int
     L.atlas_b200_cast_f32.argtypes = [c.c_void_p, c.c_void_p, c.c_int64, c.c_int32, c.c_void_p]
-    L.atlas_b200_mips_set_kernel.restype = None
-    L.atlas_b200_mips_set_kernel.argtypes = [c.c_int32]
     L.atlas_b200_linear.restype = c.c_int
     L.atlas_b200_linear.argtypes = [c.c_void_p, c.c_int64, c.c_void_p, c.c_int64, c.c_void_p, c.c_void_p, c.c_int64,
                                     c.c_void_p, c.c_int64, c.c_int32, c.c_int32, c.c_int32, c.c_int32, c.c_int32,
@@ -86,8 +84,6 @@ def lib():
     L.atlas_b200_attention_combine.restype = c.c_int
     L.atlas_b200_attention_combine.argtypes = [c.c_void_p, c.c_void_p, c.c_int32, c.c_int32, c.c_int32, c.c_int32,
                                                c.c_void_p, c.c_int64, c.c_int32, c.c_void_p]
-    L.atlas_b200_mips_set_debug_counters.restype = None
-    L.atlas_b200_mips_set_debug_counters.argtypes = [c.c_void_p]
     L.atlas_b200_profile_enable.restype = None
     L.atlas_b200_profile_enable.argtypes = [c.c_int32]
     L.atlas_b200_profile_work.restype = c.c_double
@@ -175,13 +171,13 @@ def lib():
     L.atlas_b200_attention_dropout_mask.restype = c.c_int
     L.atlas_b200_attention_dropout_mask.argtypes = [vp, i64, i32, f32, u64, u64, vp]
     L.atlas_b200_segment_tile_scan.restype = c.c_int
-    L.atlas_b200_segment_tile_scan.argtypes = [vp, i32, i32, vp, vp, vp, vp, vp, vp]
+    L.atlas_b200_segment_tile_scan.argtypes = [vp, i32, i32, vp, vp, vp, vp, vp]
     L.atlas_b200_embed_packed_tiles.restype = c.c_int
     L.atlas_b200_embed_packed_tiles.argtypes = [vp, vp, i64, i32, vp, i32, vp, i64, i32, vp]
     L.atlas_b200_linear_rows.restype = c.c_int
     L.atlas_b200_linear_rows.argtypes = [vp, i64, vp, i64, vp, vp, i64, vp, i64, i32, i32, i32, i32, i32, vp, vp, f32, vp, vp]
     L.atlas_b200_attention_packed.restype = c.c_int
-    L.atlas_b200_attention_packed.argtypes = [vp, i64, i32, i32, i32, vp, i64, vp, vp, vp, vp, vp, i32, i32, i32, f32, i32, vp]
+    L.atlas_b200_attention_packed.argtypes = [vp, i64, i32, i32, i32, vp, i64, vp, vp, vp, vp, i32, i32, i32, f32, i32, vp]
     L.atlas_b200_expand_packed_tiles.restype = c.c_int
     L.atlas_b200_expand_packed_tiles.argtypes = [vp, i64, vp, i32, vp, i64, i32, vp]
     L.atlas_b200_pq_workspace_bytes.restype = c.c_size_t
@@ -216,8 +212,6 @@ EXPORTED_SYMBOLS = [
     "atlas_b200_masked_mean_pool",
     "atlas_b200_attention",
     "atlas_b200_attention_combine",
-    "atlas_b200_mips_set_kernel",
-    "atlas_b200_mips_set_debug_counters",
     "atlas_b200_profile_enable",
     "atlas_b200_profile_work",
     "atlas_b200_profile_collect",

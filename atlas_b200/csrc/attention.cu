@@ -381,10 +381,8 @@ int atlas_b200_attention_ex(const void* q, int64_t ldq, int32_t q_col0, const vo
 // first popcount(keep[b, :]) of its L / 64 tiles, stored back to back from row 64 * tile_off[b * (L / 64)] of qkv / out.
 int atlas_b200_attention_packed(const void* qkv, int64_t ld, int32_t q_col0, int32_t k_col0, int32_t v_col0, void* out, int64_t ldo,
                                 const float* add_mask, const float* bias_delta, const uint8_t* keep, const int32_t* tile_off,
-                                const int32_t* work_prefix, int32_t B, int32_t H, int32_t L, float scale, int32_t is_bf16,
-                                void* stream) {
+                                int32_t B, int32_t H, int32_t L, float scale, int32_t is_bf16, void* stream) {
     using namespace attn;
-    (void)work_prefix;   // one CTA per (query tile, head, segment): no work-balanced item ranges needed
     AB_REQUIRE(B > 0 && H > 0 && L > 0 && L % 64 == 0 && L <= 384 && keep != nullptr && tile_off != nullptr,
                "attention_packed: 0 < L <= 384, L %% 64 == 0 and the segment tables are required (got L=%d)", L);
     AB_REQUIRE(ld % 8 == 0 && ldo % 8 == 0 && q_col0 % 8 == 0 && k_col0 % 8 == 0 && v_col0 % 8 == 0,

@@ -15,17 +15,13 @@
 //                         (cp.async double-buffered K / V tiles); dbias through a staged dS tile + diagonal sums.  A long
 //                         few-query key range (FiD cross-attention) is split over key chunks with fp32 dQ atomics.
 //   attn_bwd_dkv2_kernel  CTA = (b, h, 64-key block): the transposed problem, loops over the query blocks, accumulates dK, dV.
-//   attn_bwd_dq_kernel / attn_bwd_dkv_kernel: first-generation kernels, used when no forward lse is passed (pass 1 over
-//                         the keys recomputes it) and for A/B runs (ATLAS_B200_ATTN_BWD_V1).
 // Bound: tensor (warp-level mma.sync m16n8k16 fragments).
-// FLOPs per call = 2 * B*H*Lq*Lk*64 * 7 with the forward's lse (S + dP + dQ in the first kernel, S + dP + dV + dK in the
-// second), 8 when it is recomputed.
+// FLOPs per call = 2 * B*H*Lq*Lk*64 * 7 (S + dP + dQ in the first kernel, S + dP + dV + dK in the second).
 #include "common.cuh"
 #include "dropout.cuh"
 #include "host_common.h"
 
 #include <math.h>
-#include <stdlib.h>
 
 namespace attnb {
 
@@ -45,15 +41,16 @@ struct Params {
     const float* add_mask;    // [B, Lk] or nullptr
     const float* bias_delta;  // [H, Lq + Lk - 1] or nullptr
     float* dbias;             // [H, Lq + Lk - 1] (+=, atomics) or nullptr
-    float* lse;               // [B, H, Lq]  (input when lse_given: written by the forward kernels)
+    float* lse;               // [B, H, Lq]  (input: written by the forward kernels)
     float* dsum;              // [B, H, Lq]
     float* dq_accum;          // [B*Lq, H*64] fp32 (+=, atomics) when the keys are split over `key_chunks` CTAs, else nullptr
-    int lse_given, key_chunks;
+    int key_chunks, pad_;     // pad_ keeps the fields below at 8-byte aligned offsets: without it ptxas allocates the
+                              // kernels' registers differently (other spills) for the same source
     int B, H, Lq, Lk;
     float scale, causal_value;
-    abdrop::Key drop;         // attention-probability dropout of the forward (second-generation kernels only); thr16 == 0: off
+    abdrop::Key drop;         // attention-probability dropout of the forward; thr16 == 0: off
     const uint8_t* blk_live;  // [B, ceil(Lk / 64)] or nullptr: 64-key blocks whose keys are all masked out (softmax weight exactly
-                              // 0 in fp32, so dS = 0, dK = dV = 0 there): skipped by the second-generation kernels
+                              // 0 in fp32, so dS = 0, dK = dV = 0 there): skipped
 };
 
 // ---- shared-memory tiles: 64 rows x 128 bytes, 16-byte chunks XOR-swizzled by the row ------------------------------
@@ -99,27 +96,6 @@ __device__ __forceinline__ void mma16816(float (&d)[4], const uint32_t (&a)[4], 
     }
 }
 
-// A fragments (16 rows x 64 k, four k-steps) of the warp's rows [row0, row0 + 16) of a tile
-__device__ __forceinline__ void load_a_frags(uint32_t (&a)[4][4], uint32_t tile, int row0, int lane) {
-#pragma unroll
-    for (int ks = 0; ks < 4; ++ks) ldsm_x4(a[ks], tile + tile_off(row0 + (lane & 15), ks * 2 + (lane >> 4)));
-}
-
-// acc[nt][.] (16 x 64, eight n-tiles) += A(16 x 64 over d) . T^T, T = tile of 64 rows x 64 d: B[k = d][n = tile row]
-template <bool kBF16>
-__device__ __forceinline__ void mma_a_tileT(float (&acc)[8][4], const uint32_t (&a)[4][4], uint32_t tile, int lane) {
-#pragma unroll
-    for (int ks = 0; ks < 4; ++ks) {
-#pragma unroll
-        for (int np = 0; np < 4; ++np) {
-            uint32_t b[4];
-            ldsm_x4(b, tile + tile_off(np * 16 + (lane & 7) + ((lane >> 4) << 3), ks * 2 + ((lane >> 3) & 1)));
-            mma16816<kBF16>(acc[2 * np], a[ks], b[0], b[1]);
-            mma16816<kBF16>(acc[2 * np + 1], a[ks], b[2], b[3]);
-        }
-    }
-}
-
 // acc[nt][.] (16 x 64 over d) += P(16 x 64 over the tile rows, as accumulator-layout fp32 values) . T,
 // T = tile of 64 rows x 64 d: B[k = tile row][n = d] (transposing ldmatrix)
 template <bool kBF16>
@@ -139,18 +115,6 @@ __device__ __forceinline__ void mma_p_tile(float (&acc)[8][4], const float (&p)[
             mma16816<kBF16>(acc[2 * dp + 1], a, b[2], b[3]);
         }
     }
-}
-
-// the score of (query i, key j) from the raw dot product; identical in both kernels and both passes
-__device__ __forceinline__ float score(float dot, int i, int j, const Params& p, const float* bias_s,
-                                       const float* mask_row) {
-    if (j >= p.Lk) return -INFINITY;
-    const int ic = i < p.Lq ? i : p.Lq - 1;
-    float s = dot * p.scale;
-    if (bias_s != nullptr) s += bias_s[j - ic + p.Lq - 1];
-    if (mask_row != nullptr) s += __ldg(mask_row + j);
-    if (p.causal_value != 0.f && j > ic) s += p.causal_value;
-    return s;
 }
 
 template <bool kBF16>
@@ -177,280 +141,9 @@ __device__ __forceinline__ void store_acc(const float (&acc)[8][4], float mul, u
 }
 
 // ======================================================================================================================
-// dQ kernel (+ log-sum-exp, D, dbias)
-// ======================================================================================================================
-template <bool kBF16>
-__global__ void __launch_bounds__(THREADS)
-attn_bwd_dq_kernel(const Params p) {
-    extern __shared__ __align__(128) uint8_t smem[];
-    uint8_t* sQ = smem;
-    uint8_t* sdO = smem + TILE_BYTES;
-    uint8_t* sK = smem + 2 * TILE_BYTES;
-    uint8_t* sV = smem + 3 * TILE_BYTES;
-    const int ntab = p.Lq + p.Lk - 1;
-    float* bias_s = p.bias_delta ? reinterpret_cast<float*>(smem + 4 * TILE_BYTES) : nullptr;
-    float* dbias_s = p.dbias ? reinterpret_cast<float*>(smem + 4 * TILE_BYTES) + (p.bias_delta ? ntab : 0) : nullptr;
-
-    const int nqb = (p.Lq + BM - 1) / BM;
-    const int chunk = static_cast<int>(blockIdx.x) % p.key_chunks;     // this CTA's share of the keys (cross-attention)
-    const int item = static_cast<int>(blockIdx.x) / p.key_chunks;
-    const int qb = item % nqb;
-    const int h = (item / nqb) % p.H;
-    const int b = item / (nqb * p.H);
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, g = lane >> 2, t = lane & 3;
-    const int q0 = qb * BM;
-    const int64_t qrow_base = static_cast<int64_t>(b) * p.Lq, krow_base = static_cast<int64_t>(b) * p.Lk;
-    const float* mask_row = p.add_mask ? p.add_mask + static_cast<int64_t>(b) * p.Lk : nullptr;
-
-    for (int x = threadIdx.x; x < ntab; x += THREADS) {
-        if (bias_s) bias_s[x] = __ldg(p.bias_delta + static_cast<int64_t>(h) * ntab + x);
-        if (dbias_s) dbias_s[x] = 0.f;
-    }
-    load_tile(sQ, p.q, p.ldq, p.q_col0 + h * D, qrow_base, q0, p.Lq);
-    load_tile(sdO, p.dout, p.lddo, h * D, qrow_base, q0, p.Lq);
-
-    // D_i = sum_d dO[i, d] * O[i, d]: two lanes per row, 32 columns each, straight from global memory
-    float drow[2];
-    {
-        const int r = q0 + warp * 16 + (lane >> 1);
-        float acc = 0.f;
-        if (r < p.Lq) {
-            const uint16_t* po = p.o + (qrow_base + r) * p.ldo + h * D + (lane & 1) * 32;
-            const uint16_t* pd = p.dout + (qrow_base + r) * p.lddo + h * D + (lane & 1) * 32;
-#pragma unroll
-            for (int c = 0; c < 4; ++c) {
-                const uint4 a = __ldg(reinterpret_cast<const uint4*>(po) + c);
-                const uint4 d = __ldg(reinterpret_cast<const uint4*>(pd) + c);
-                const uint32_t aw[4] = {a.x, a.y, a.z, a.w}, dw[4] = {d.x, d.y, d.z, d.w};
-#pragma unroll
-                for (int e = 0; e < 4; ++e) {
-                    acc = fmaf(to_f32<kBF16>(aw[e] & 0xFFFFu), to_f32<kBF16>(dw[e] & 0xFFFFu), acc);
-                    acc = fmaf(to_f32<kBF16>(aw[e] >> 16), to_f32<kBF16>(dw[e] >> 16), acc);
-                }
-            }
-        }
-        acc += __shfl_xor_sync(0xffffffffu, acc, 1);
-        // the row (lane >> 1) total now sits in lanes 2r and 2r + 1; this thread needs rows g and g + 8
-        drow[0] = __shfl_sync(0xffffffffu, acc, 2 * g);
-        drow[1] = __shfl_sync(0xffffffffu, acc, 2 * (g + 8));
-        if ((lane & 1) == 0 && r < p.Lq) p.dsum[(static_cast<int64_t>(b) * p.H + h) * p.Lq + r] = acc;
-    }
-    __syncthreads();
-
-    const uint32_t sQ_a = ab::smem_u32(sQ), sdO_a = ab::smem_u32(sdO), sK_a = ab::smem_u32(sK), sV_a = ab::smem_u32(sV);
-    uint32_t qa[4][4], doa[4][4];
-    load_a_frags(qa, sQ_a, warp * 16, lane);
-    load_a_frags(doa, sdO_a, warp * 16, lane);
-
-    const int nkb = (p.Lk + BN - 1) / BN;
-    const int i_lo = q0 + warp * 16 + g;   // this thread's rows: i_lo and i_lo + 8
-
-    // ---- pass 1: row max / sum of exp -> log-sum-exp (skipped when the forward kernel saved it) ----------------------
-    float m_run[2] = {-INFINITY, -INFINITY}, l_run[2] = {0.f, 0.f};
-    for (int kb = 0; kb < (p.lse_given ? 0 : nkb); ++kb) {
-        __syncthreads();
-        load_tile(sK, p.k, p.ldk, p.k_col0 + h * D, krow_base, kb * BN, p.Lk);
-        __syncthreads();
-        float acc[8][4];
-#pragma unroll
-        for (int nt = 0; nt < 8; ++nt)
-#pragma unroll
-            for (int e = 0; e < 4; ++e) acc[nt][e] = 0.f;
-        mma_a_tileT<kBF16>(acc, qa, sK_a, lane);
-        float tmax[2] = {-INFINITY, -INFINITY};
-#pragma unroll
-        for (int nt = 0; nt < 8; ++nt)
-#pragma unroll
-            for (int e = 0; e < 4; ++e) {
-                const float s = score(acc[nt][e], i_lo + (e >> 1) * 8, kb * BN + nt * 8 + 2 * t + (e & 1), p, bias_s, mask_row);
-                acc[nt][e] = s;
-                tmax[e >> 1] = fmaxf(tmax[e >> 1], s);
-            }
-#pragma unroll
-        for (int r = 0; r < 2; ++r) {
-            tmax[r] = fmaxf(tmax[r], __shfl_xor_sync(0xffffffffu, tmax[r], 1));
-            tmax[r] = fmaxf(tmax[r], __shfl_xor_sync(0xffffffffu, tmax[r], 2));
-        }
-        float m_new[2], tsum[2] = {0.f, 0.f};
-#pragma unroll
-        for (int r = 0; r < 2; ++r) m_new[r] = fmaxf(m_run[r], tmax[r]);
-#pragma unroll
-        for (int nt = 0; nt < 8; ++nt)
-#pragma unroll
-            for (int e = 0; e < 4; ++e) tsum[e >> 1] += __expf(acc[nt][e] - m_new[e >> 1]);
-#pragma unroll
-        for (int r = 0; r < 2; ++r) {
-            tsum[r] += __shfl_xor_sync(0xffffffffu, tsum[r], 1);
-            tsum[r] += __shfl_xor_sync(0xffffffffu, tsum[r], 2);
-            l_run[r] = l_run[r] * __expf(m_run[r] - m_new[r]) + tsum[r];
-            m_run[r] = m_new[r];
-        }
-    }
-    float lse[2];
-#pragma unroll
-    for (int r = 0; r < 2; ++r) {
-        const int i = i_lo + r * 8;
-        if (p.lse_given) {
-            // padding rows: +inf makes every probability 0 (their dO rows are zero as well)
-            lse[r] = i < p.Lq ? __ldg(p.lse + (static_cast<int64_t>(b) * p.H + h) * p.Lq + i) : INFINITY;
-        } else {
-            lse[r] = m_run[r] + __logf(l_run[r]);
-            if (t == 0 && i < p.Lq) p.lse[(static_cast<int64_t>(b) * p.H + h) * p.Lq + i] = lse[r];
-        }
-    }
-    const int per_chunk = (nkb + p.key_chunks - 1) / p.key_chunks;
-    const int kb_begin = chunk * per_chunk;
-    const int kb_end = min(nkb, kb_begin + per_chunk);
-
-    // ---- pass 2: dQ = scale * (P o (dO V^T - D)) K --------------------------------------------------------------------
-    float dqacc[8][4];
-#pragma unroll
-    for (int nt = 0; nt < 8; ++nt)
-#pragma unroll
-        for (int e = 0; e < 4; ++e) dqacc[nt][e] = 0.f;
-    for (int kb = kb_begin; kb < kb_end; ++kb) {
-        __syncthreads();
-        load_tile(sK, p.k, p.ldk, p.k_col0 + h * D, krow_base, kb * BN, p.Lk);
-        load_tile(sV, p.v, p.ldv, p.v_col0 + h * D, krow_base, kb * BN, p.Lk);
-        __syncthreads();
-        float acc[8][4], dp[8][4];
-#pragma unroll
-        for (int nt = 0; nt < 8; ++nt)
-#pragma unroll
-            for (int e = 0; e < 4; ++e) {
-                acc[nt][e] = 0.f;
-                dp[nt][e] = 0.f;
-            }
-        mma_a_tileT<kBF16>(acc, qa, sK_a, lane);
-        mma_a_tileT<kBF16>(dp, doa, sV_a, lane);
-#pragma unroll
-        for (int nt = 0; nt < 8; ++nt)
-#pragma unroll
-            for (int e = 0; e < 4; ++e) {
-                const int i = i_lo + (e >> 1) * 8, j = kb * BN + nt * 8 + 2 * t + (e & 1);
-                const float s = score(acc[nt][e], i, j, p, bias_s, mask_row);
-                const float pr = __expf(s - lse[e >> 1]);
-                const float ds = pr * (dp[nt][e] - drow[e >> 1]);
-                acc[nt][e] = ds;
-                if (dbias_s != nullptr && i < p.Lq && j < p.Lk) atomicAdd(&dbias_s[j - i + p.Lq - 1], ds);
-            }
-        mma_p_tile<kBF16>(dqacc, acc, sK_a, lane);
-    }
-    if (p.dq_accum != nullptr) {
-        // keys split over several CTAs: fp32 partial sums, converted to 16 bits by the caller afterwards
-#pragma unroll
-        for (int half = 0; half < 2; ++half) {
-            const int i = i_lo + half * 8;
-            if (i >= p.Lq) continue;
-            float* row = p.dq_accum + (qrow_base + i) * (static_cast<int64_t>(p.H) * D) + h * D;
-#pragma unroll
-            for (int nt = 0; nt < 8; ++nt) {
-                atomicAdd(row + nt * 8 + 2 * t, dqacc[nt][2 * half] * p.scale);
-                atomicAdd(row + nt * 8 + 2 * t + 1, dqacc[nt][2 * half + 1] * p.scale);
-            }
-        }
-    } else {
-        store_acc<kBF16>(dqacc, p.scale, p.dq, p.lddq, p.dq_col0 + h * D, qrow_base, q0 + warp * 16, p.Lq, lane);
-    }
-    if (dbias_s != nullptr) {
-        __syncthreads();
-        for (int x = threadIdx.x; x < ntab; x += THREADS) {
-            const float v = dbias_s[x];
-            if (v != 0.f) atomicAdd(p.dbias + static_cast<int64_t>(h) * ntab + x, v);
-        }
-    }
-}
-
-// ======================================================================================================================
-// dK / dV kernel: everything transposed (rows = keys, columns = queries)
-// ======================================================================================================================
-template <bool kBF16>
-__global__ void __launch_bounds__(THREADS)
-attn_bwd_dkv_kernel(const Params p) {
-    extern __shared__ __align__(128) uint8_t smem[];
-    uint8_t* sK = smem;
-    uint8_t* sV = smem + TILE_BYTES;
-    uint8_t* sQ = smem + 2 * TILE_BYTES;
-    uint8_t* sdO = smem + 3 * TILE_BYTES;
-    float* lse_s = reinterpret_cast<float*>(smem + 4 * TILE_BYTES);
-    float* d_s = lse_s + BN;
-    const int ntab = p.Lq + p.Lk - 1;
-    float* bias_s = p.bias_delta ? d_s + BN : nullptr;
-
-    const int nkb = (p.Lk + BM - 1) / BM;
-    const int kb = static_cast<int>(blockIdx.x) % nkb;
-    const int h = (static_cast<int>(blockIdx.x) / nkb) % p.H;
-    const int b = static_cast<int>(blockIdx.x) / (nkb * p.H);
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, g = lane >> 2, t = lane & 3;
-    const int k0 = kb * BM;
-    const int64_t qrow_base = static_cast<int64_t>(b) * p.Lq, krow_base = static_cast<int64_t>(b) * p.Lk;
-    const float* mask_row = p.add_mask ? p.add_mask + static_cast<int64_t>(b) * p.Lk : nullptr;
-
-    if (bias_s)
-        for (int x = threadIdx.x; x < ntab; x += THREADS) bias_s[x] = __ldg(p.bias_delta + static_cast<int64_t>(h) * ntab + x);
-    load_tile(sK, p.k, p.ldk, p.k_col0 + h * D, krow_base, k0, p.Lk);
-    load_tile(sV, p.v, p.ldv, p.v_col0 + h * D, krow_base, k0, p.Lk);
-    __syncthreads();
-    const uint32_t sQ_a = ab::smem_u32(sQ), sdO_a = ab::smem_u32(sdO), sK_a = ab::smem_u32(sK), sV_a = ab::smem_u32(sV);
-    uint32_t ka[4][4], va[4][4];
-    load_a_frags(ka, sK_a, warp * 16, lane);
-    load_a_frags(va, sV_a, warp * 16, lane);
-
-    float dkacc[8][4], dvacc[8][4];
-#pragma unroll
-    for (int nt = 0; nt < 8; ++nt)
-#pragma unroll
-        for (int e = 0; e < 4; ++e) {
-            dkacc[nt][e] = 0.f;
-            dvacc[nt][e] = 0.f;
-        }
-    const int j_lo = k0 + warp * 16 + g;   // this thread's keys: j_lo and j_lo + 8
-    const int nqb = (p.Lq + BN - 1) / BN;
-    const float* lse_g = p.lse + (static_cast<int64_t>(b) * p.H + h) * p.Lq;
-    const float* d_g = p.dsum + (static_cast<int64_t>(b) * p.H + h) * p.Lq;
-    for (int qb = 0; qb < nqb; ++qb) {
-        __syncthreads();
-        load_tile(sQ, p.q, p.ldq, p.q_col0 + h * D, qrow_base, qb * BN, p.Lq);
-        load_tile(sdO, p.dout, p.lddo, h * D, qrow_base, qb * BN, p.Lq);
-        if (threadIdx.x < BN) {
-            const int i = qb * BN + static_cast<int>(threadIdx.x);
-            lse_s[threadIdx.x] = i < p.Lq ? lse_g[i] : INFINITY;   // exp(s - inf) = 0 for the padding queries
-            d_s[threadIdx.x] = i < p.Lq ? d_g[i] : 0.f;
-        }
-        __syncthreads();
-        float acc[8][4], dp[8][4];
-#pragma unroll
-        for (int nt = 0; nt < 8; ++nt)
-#pragma unroll
-            for (int e = 0; e < 4; ++e) {
-                acc[nt][e] = 0.f;
-                dp[nt][e] = 0.f;
-            }
-        mma_a_tileT<kBF16>(acc, ka, sQ_a, lane);     // S^T  = K Q^T
-        mma_a_tileT<kBF16>(dp, va, sdO_a, lane);     // dP^T = V dO^T
-#pragma unroll
-        for (int nt = 0; nt < 8; ++nt)
-#pragma unroll
-            for (int e = 0; e < 4; ++e) {
-                const int il = nt * 8 + 2 * t + (e & 1);
-                const float s = score(acc[nt][e], qb * BN + il, j_lo + (e >> 1) * 8, p, bias_s, mask_row);
-                const float pr = __expf(s - lse_s[il]);
-                acc[nt][e] = pr;
-                dp[nt][e] = pr * (dp[nt][e] - d_s[il]);
-            }
-        mma_p_tile<kBF16>(dvacc, acc, sdO_a, lane);  // dV += P^T dO
-        mma_p_tile<kBF16>(dkacc, dp, sQ_a, lane);    // dK += dS^T Q
-    }
-    store_acc<kBF16>(dkacc, p.scale, p.dk, p.lddk, p.dk_col0 + h * D, krow_base, k0 + warp * 16, p.Lk, lane);
-    store_acc<kBF16>(dvacc, 1.0f, p.dv, p.lddv, p.dv_col0 + h * D, krow_base, k0 + warp * 16, p.Lk, lane);
-}
-
-
-// ======================================================================================================================
-// Second-generation kernels (default when the forward's log-sum-exp is available): same arithmetic, but
-//   - the streamed tiles are double-buffered with cp.async (the next key / query block lands while this one is computed),
-//   - the resident operand's A fragments are re-read from shared memory per k-step instead of living in 32 registers and
-//     the additive mask / bias come from (padded) shared-memory tables, so three CTAs (12 warps) fit per SM instead of two.
+// The kernels: the streamed tiles are double-buffered with cp.async (the next key / query block lands while this one is
+// computed); the resident operand's A fragments are re-read from shared memory per k-step instead of living in 32 registers
+// and the additive mask / bias come from (padded) shared-memory tables, so that three CTAs (12 warps) fit per SM.
 // ======================================================================================================================
 __device__ __forceinline__ void cp_async16(uint32_t dst, const void* src, int src_bytes) {
     asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(dst), "l"(src), "r"(src_bytes) : "memory");
@@ -852,16 +545,16 @@ int atlas_b200_attention_bwd_train(const void* q, int64_t ldq, int32_t q_col0, c
                                    uint64_t offset, const uint8_t* key_block_live, int32_t is_bf16, void* stream) {
     using namespace attnb;
     AB_REQUIRE(dropout_p >= 0.f && dropout_p < 1.f, "attention_bwd: need 0 <= dropout_p < 1 (got %f)", dropout_p);
+    AB_REQUIRE(lse_given != 0, "attention_bwd: the forward's log-sum-exp is required in lse (lse_given != 0)");
     const abdrop::Key drop = abdrop::make_key(dropout_p, seed, offset);
-    AB_REQUIRE(drop.thr16 == 0u || lse_given != 0, "attention_bwd: dropout needs the forward's log-sum-exp (lse_given)");
-    AB_REQUIRE(dq_accum == nullptr || (lse_given != 0 && dbias_delta == nullptr),
-               "attention_bwd: dq_accum (keys split over CTAs) needs the forward's lse and no dbias");
+    AB_REQUIRE(dq_accum == nullptr || dbias_delta == nullptr,
+               "attention_bwd: dq_accum (keys split over CTAs) cannot be combined with dbias_delta");
     AB_REQUIRE(B >= 0 && H > 0 && Lq > 0 && Lk > 0, "attention_bwd: bad shape B=%d H=%d Lq=%d Lk=%d", B, H, Lq, Lk);
     AB_REQUIRE(ldq % 8 == 0 && ldk % 8 == 0 && ldv % 8 == 0 && ldo % 8 == 0 && lddo % 8 == 0 && lddq % 8 == 0 &&
                    lddk % 8 == 0 && lddv % 8 == 0 && q_col0 % 8 == 0 && k_col0 % 8 == 0 && v_col0 % 8 == 0 &&
                    dq_col0 % 8 == 0 && dk_col0 % 8 == 0 && dv_col0 % 8 == 0,
                "attention_bwd: strides and column offsets must be multiples of 8 elements");
-    AB_REQUIRE(lse != nullptr && dsum != nullptr, "attention_bwd: lse / dsum scratch ([B, H, Lq] fp32 each) is required");
+    AB_REQUIRE(lse != nullptr && dsum != nullptr, "attention_bwd: lse and dsum ([B, H, Lq] fp32 each) are required");
     AB_REQUIRE(dbias_delta == nullptr || bias_delta != nullptr, "attention_bwd: dbias_delta without bias_delta");
     const int64_t ntab = static_cast<int64_t>(Lq) + Lk - 1;
     AB_REQUIRE(bias_delta == nullptr || ntab <= 8192, "attention_bwd: Lq + Lk - 1 = %lld exceeds the bias table (8192)",
@@ -899,7 +592,6 @@ int atlas_b200_attention_bwd_train(const void* q, int64_t ldq, int32_t q_col0, c
     p.lse = lse;
     p.dsum = dsum;
     p.dq_accum = dq_accum;
-    p.lse_given = lse_given;
     p.key_chunks = key_chunks;
     p.B = B; p.H = H; p.Lq = Lq; p.Lk = Lk;
     p.scale = scale;
@@ -907,13 +599,9 @@ int atlas_b200_attention_bwd_train(const void* q, int64_t ldq, int32_t q_col0, c
     p.drop = drop;
     p.blk_live = key_block_live;
     cudaStream_t s = static_cast<cudaStream_t>(stream);
-    static const bool force_v1 = getenv("ATLAS_B200_ATTN_BWD_V1") != nullptr;   // A/B measurements
-    const bool v2 = lse_given != 0 && (!force_v1 || drop.thr16 != 0u);
-    const int smem_dq = v2 ? 7 * TILE_BYTES + 2 * BN * 4 +
-                                 static_cast<int>(((bias_delta ? ntab + 2 * BIAS_PAD : 0) + (dbias_delta ? ntab : 0)) * 4)
-                           : 4 * TILE_BYTES + static_cast<int>(((bias_delta ? ntab : 0) + (dbias_delta ? ntab : 0)) * 4);
-    const int smem_dkv = v2 ? 6 * TILE_BYTES + 4 * BN * 4 + static_cast<int>((bias_delta ? ntab + 2 * BIAS_PAD : 0) * 4)
-                            : 4 * TILE_BYTES + 2 * BN * 4 + static_cast<int>((bias_delta ? ntab : 0) * 4);
+    const int smem_dq = 7 * TILE_BYTES + 2 * BN * 4 +
+                        static_cast<int>(((bias_delta ? ntab + 2 * BIAS_PAD : 0) + (dbias_delta ? ntab : 0)) * 4);
+    const int smem_dkv = 6 * TILE_BYTES + 4 * BN * 4 + static_cast<int>((bias_delta ? ntab + 2 * BIAS_PAD : 0) * 4);
     constexpr int SMEM_MAX = 7 * TILE_BYTES + 4 * BN * 4 + 2 * (8192 + 2 * BIAS_PAD) * 4;
     static bool attr_set = false;
     if (!attr_set) {
@@ -921,28 +609,15 @@ int atlas_b200_attention_bwd_train(const void* q, int64_t ldq, int32_t q_col0, c
         AB_CUDA_CHECK(cudaFuncSetAttribute(attn_bwd_dq2_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_MAX));
         AB_CUDA_CHECK(cudaFuncSetAttribute(attn_bwd_dkv2_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_MAX));
         AB_CUDA_CHECK(cudaFuncSetAttribute(attn_bwd_dkv2_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_MAX));
-        AB_CUDA_CHECK(cudaFuncSetAttribute(attn_bwd_dq_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_MAX));
-        AB_CUDA_CHECK(cudaFuncSetAttribute(attn_bwd_dq_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_MAX));
-        AB_CUDA_CHECK(cudaFuncSetAttribute(attn_bwd_dkv_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_MAX));
-        AB_CUDA_CHECK(cudaFuncSetAttribute(attn_bwd_dkv_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_MAX));
         attr_set = true;
     }
     abh::prof_begin(s, abh::PROF_ATTENTION_BWD);
-    const bool dq_done = false, dkv_done = false;
-    if (v2) {
-        if (is_bf16) {
-            if (!dq_done) attn_bwd_dq2_kernel<true><<<static_cast<unsigned>(nq_ctas), THREADS, smem_dq, s>>>(p);
-            if (!dkv_done) attn_bwd_dkv2_kernel<true><<<static_cast<unsigned>(nk_ctas), THREADS, smem_dkv, s>>>(p);
-        } else {
-            if (!dq_done) attn_bwd_dq2_kernel<false><<<static_cast<unsigned>(nq_ctas), THREADS, smem_dq, s>>>(p);
-            if (!dkv_done) attn_bwd_dkv2_kernel<false><<<static_cast<unsigned>(nk_ctas), THREADS, smem_dkv, s>>>(p);
-        }
-    } else if (is_bf16) {
-        attn_bwd_dq_kernel<true><<<static_cast<unsigned>(nq_ctas), THREADS, smem_dq, s>>>(p);
-        attn_bwd_dkv_kernel<true><<<static_cast<unsigned>(nk_ctas), THREADS, smem_dkv, s>>>(p);
+    if (is_bf16) {
+        attn_bwd_dq2_kernel<true><<<static_cast<unsigned>(nq_ctas), THREADS, smem_dq, s>>>(p);
+        attn_bwd_dkv2_kernel<true><<<static_cast<unsigned>(nk_ctas), THREADS, smem_dkv, s>>>(p);
     } else {
-        attn_bwd_dq_kernel<false><<<static_cast<unsigned>(nq_ctas), THREADS, smem_dq, s>>>(p);
-        attn_bwd_dkv_kernel<false><<<static_cast<unsigned>(nk_ctas), THREADS, smem_dkv, s>>>(p);
+        attn_bwd_dq2_kernel<false><<<static_cast<unsigned>(nq_ctas), THREADS, smem_dq, s>>>(p);
+        attn_bwd_dkv2_kernel<false><<<static_cast<unsigned>(nk_ctas), THREADS, smem_dkv, s>>>(p);
     }
     abh::prof_end(s, abh::PROF_ATTENTION_BWD, 16.0 * B * H * static_cast<double>(Lq) * Lk * D);
     abh::count_launch(2);

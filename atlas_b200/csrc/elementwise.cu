@@ -353,14 +353,13 @@ live_tile_copy_kernel(const uint16_t* __restrict__ src, int64_t lds, const int32
 // that holds a live key; the kept tiles of all segments are packed back to back ------------------------------------------------
 // One block.  live [S, nb] -> keep [S, nb] (1 for tiles 0 .. last live tile of the segment; all nb tiles if none is live),
 // tile_off [S * nb] (index of a kept tile in the packed order, -1 = dropped), tile_src [S * nb] (inverse: source tile of packed
-// tile o, -1 past the end), *count_rows = 64 x (number of kept tiles), work_prefix [S + 1] (optional): exclusive prefix of the
-// attention work of a segment, kept tiles x kept 128-row query tiles (the packed attention kernel splits its items by it).
+// tile o, -1 past the end), *count_rows = 64 x (number of kept tiles).
 __global__ void __launch_bounds__(1024)
 segment_tile_scan_kernel(const uint8_t* __restrict__ live, int S, int nb, uint8_t* __restrict__ keep, int32_t* __restrict__ tile_off,
-                         int32_t* __restrict__ tile_src, int32_t* __restrict__ count_rows, int32_t* __restrict__ work_prefix) {
-    __shared__ int s_warp[32], s_warp_w[32];
-    __shared__ int s_base, s_base_w;
-    if (threadIdx.x == 0) s_base = 0, s_base_w = 0;
+                         int32_t* __restrict__ tile_src, int32_t* __restrict__ count_rows) {
+    __shared__ int s_warp[32];
+    __shared__ int s_base;
+    if (threadIdx.x == 0) s_base = 0;
     __syncthreads();
     for (int s0 = 0; s0 < S; s0 += 1024) {
         const int sg = s0 + static_cast<int>(threadIdx.x);
@@ -370,31 +369,25 @@ segment_tile_scan_kernel(const uint8_t* __restrict__ live, int S, int nb, uint8_
                 if (live[static_cast<size_t>(sg) * nb + j] != 0) f = j + 1;
             if (f == 0) f = nb;
         }
-        const int fw = f * ((f + 1) / 2);                    // key blocks x query tiles
-        int x = f, xw = fw;
+        int x = f;
 #pragma unroll
         for (int o = 1; o < 32; o <<= 1) {
             const int y = __shfl_up_sync(0xffffffffu, x, o);
-            const int yw = __shfl_up_sync(0xffffffffu, xw, o);
-            if (static_cast<int>(threadIdx.x & 31u) >= o) x += y, xw += yw;
+            if (static_cast<int>(threadIdx.x & 31u) >= o) x += y;
         }
-        if ((threadIdx.x & 31u) == 31u) s_warp[threadIdx.x >> 5] = x, s_warp_w[threadIdx.x >> 5] = xw;
+        if ((threadIdx.x & 31u) == 31u) s_warp[threadIdx.x >> 5] = x;
         __syncthreads();
         if (threadIdx.x < 32) {
-            int w = s_warp[threadIdx.x], ww = s_warp_w[threadIdx.x];
+            int w = s_warp[threadIdx.x];
 #pragma unroll
             for (int o = 1; o < 32; o <<= 1) {
                 const int y = __shfl_up_sync(0xffffffffu, w, o);
-                const int yw = __shfl_up_sync(0xffffffffu, ww, o);
-                if (static_cast<int>(threadIdx.x) >= o) w += y, ww += yw;
+                if (static_cast<int>(threadIdx.x) >= o) w += y;
             }
             s_warp[threadIdx.x] = w;
-            s_warp_w[threadIdx.x] = ww;
         }
         __syncthreads();
         const int before = s_base + (threadIdx.x >= 32 ? s_warp[(threadIdx.x >> 5) - 1] : 0) + x - f;
-        if (sg < S && work_prefix != nullptr)
-            work_prefix[sg] = s_base_w + (threadIdx.x >= 32 ? s_warp_w[(threadIdx.x >> 5) - 1] : 0) + xw - fw;
         if (sg < S) {
             for (int j = 0; j < nb; ++j) {
                 const int t = sg * nb + j;
@@ -404,15 +397,12 @@ segment_tile_scan_kernel(const uint8_t* __restrict__ live, int S, int nb, uint8_
             }
         }
         __syncthreads();
-        if (threadIdx.x == 0) s_base += s_warp[31], s_base_w += s_warp_w[31];
+        if (threadIdx.x == 0) s_base += s_warp[31];
         __syncthreads();
     }
     const int total = s_base;
     for (int o = total + static_cast<int>(threadIdx.x); o < S * nb; o += 1024) tile_src[o] = -1;
-    if (threadIdx.x == 0) {
-        *count_rows = total * 64;
-        if (work_prefix != nullptr) work_prefix[S] = s_base_w;
-    }
+    if (threadIdx.x == 0) *count_rows = total * 64;
 }
 
 // block o writes packed tile o: the embedding rows of the 64 token ids of its source tile, zeros past the end
@@ -454,11 +444,10 @@ expand_packed_tiles_kernel(const uint16_t* __restrict__ src, int64_t lds, const 
 extern "C" {
 
 int atlas_b200_segment_tile_scan(const uint8_t* live, int32_t S, int32_t nb, uint8_t* keep, int32_t* tile_off, int32_t* tile_src,
-                                 int32_t* count_rows, int32_t* work_prefix, void* stream) {
+                                 int32_t* count_rows, void* stream) {
     AB_REQUIRE(S > 0 && nb > 0 && nb <= 64 && live != nullptr && keep != nullptr && tile_off != nullptr && tile_src != nullptr &&
                    count_rows != nullptr, "segment_tile_scan: S > 0, 0 < nb <= 64, all tables required");
-    ew::segment_tile_scan_kernel<<<1, 1024, 0, static_cast<cudaStream_t>(stream)>>>(live, S, nb, keep, tile_off, tile_src, count_rows,
-                                                                                    work_prefix);
+    ew::segment_tile_scan_kernel<<<1, 1024, 0, static_cast<cudaStream_t>(stream)>>>(live, S, nb, keep, tile_off, tile_src, count_rows);
     abh::count_launch(1);
     AB_CUDA_CHECK(cudaGetLastError());
     return ATLAS_B200_OK;

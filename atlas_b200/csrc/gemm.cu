@@ -816,10 +816,8 @@ int atlas_b200_linear_wgrad(const void* dY, int64_t lddy, const void* X, int64_t
     int block_n, splits, per;
     wgrad_plan(tokens, N, K, &block_n, &splits, &per);
     const bool wide = block_n == 256;
-    static const bool no_splitk = getenv("ATLAS_B200_WGRAD_NO_SPLITK") != nullptr;   // A/B measurements
     const size_t need = static_cast<size_t>(splits) * N * K * sizeof(float);
-    if (splits > 1 && (no_splitk || workspace == nullptr || workspace_bytes < need ||
-                       (reinterpret_cast<uintptr_t>(workspace) & 15u) != 0)) {
+    if (splits > 1 && (workspace == nullptr || workspace_bytes < need || (reinterpret_cast<uintptr_t>(workspace) & 15u) != 0)) {
         splits = 1;                                      // no (usable) scratch: one CTA group walks the whole contraction
         per = (tokens + BLOCK_K - 1) / BLOCK_K;
     }

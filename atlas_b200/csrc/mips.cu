@@ -64,7 +64,6 @@ struct ScanParams {
     uint32_t* count;      // [QBLOCK]
     uint64_t* cand;       // [QBLOCK][capq]
     uint32_t capq;
-    unsigned long long* dbg;  // optional [gridDim.x][8] cycle counters (nullptr = off)
 };
 
 template <bool kBF16>
@@ -342,8 +341,6 @@ static int launch_scan(const CUtensorMap& tq, const CUtensorMap& tb, const ScanP
     return ATLAS_B200_OK;
 }
 
-static unsigned long long* g_dbg = nullptr;  // device buffer for wait-cycle counters of the main scan (unused by this kernel)
-
 static int check_common(const void* bank, int64_t n, int64_t ld, const void* queries, int nq, int k) {
     AB_REQUIRE(nq >= 0 && k >= 1, "nq must be >= 0 and k >= 1 (nq=%d k=%d)", nq, k);
     AB_REQUIRE(k <= ATLAS_B200_MAX_TOPK, "k=%d exceeds ATLAS_B200_MAX_TOPK=%d", k, ATLAS_B200_MAX_TOPK);
@@ -395,7 +392,6 @@ static int topk_impl(const void* bank, int64_t n, int64_t ld, const void* querie
         p.count = w.count;
         p.cand = w.cand;
         p.capq = w.capq;
-        p.dbg = nullptr;
         uint16_t* os_b = os + static_cast<size_t>(q0) * k;
         int64_t* oi_b = out_ids + static_cast<size_t>(q0) * k;
         auto scan = [&](const ScanParams& sp) -> int { return launch_scan<kBF16>(tq, tb, sp, s); };
@@ -449,11 +445,9 @@ static int topk_impl(const void* bank, int64_t n, int64_t ld, const void* querie
             p.tile_begin = first_tile;
             p.tile_step = 1;
             p.num_tiles = total_tiles - first_tile;
-            p.dbg = g_dbg;
             abh::prof_begin(s, abh::PROF_SCAN);
             rc = scan(p);
             abh::prof_end(s, abh::PROF_SCAN, static_cast<double>(total_tiles - first_tile) * tile_n * DIM * 2.0);
-            p.dbg = nullptr;
             if (rc) return rc;
             mips_select_kernel<kBF16><<<nqb, SEL_THREADS, 0, s>>>(w.cand, w.count, w.capq, k, SEL_EMIT, w.bound, os_b,
                                                                  oi_b, id_base, id_stride, status);
@@ -483,12 +477,6 @@ static int topk_impl(const void* bank, int64_t n, int64_t ld, const void* querie
 }  // namespace mips
 
 extern "C" {
-
-// one scan kernel on sm_90a: the mode switch is accepted and ignored
-void atlas_b200_mips_set_kernel(int32_t mode) { (void)mode; }
-void atlas_b200_mips_set_debug_counters(void* device_u64_buffer) {
-    mips::g_dbg = static_cast<unsigned long long*>(device_u64_buffer);
-}
 
 size_t atlas_b200_mips_workspace_bytes(int64_t n, int32_t nq, int32_t k) {
     if (n < 1) n = 1;

@@ -405,13 +405,11 @@ def compact_live_tiles(x, tile_live):
 
 _ENC_PACKED = os.environ.get("ATLAS_B200_ENC_PACKED", "1") != "0"          # A/B switch of the padding-compacted FiD encoder
 _BERT_PACKED = os.environ.get("ATLAS_B200_BERT_PACKED", "1") != "0"        # ... of the Contriever encoder (needs _ENC_PACKED too)
-_PACKED_BALANCE = os.environ.get("ATLAS_B200_PACKED_BALANCE", "1") != "0"  # A/B: packed attention CTAs split by work, not count
 
 
 def segment_tile_scan(live):
     """live uint8 [S, nb] (key_block_live) -> (keep uint8 [S, nb], tile_off int32 [S * nb], tile_src int32 [S * nb], count_rows
-    int32 [1]): the packed layout of the padding-compacted encoder (include/atlas_b200.h).  No host synchronisation.
-    `keep` carries the work prefix of the segments (`keep._atlas_work`, int32 [S + 1]) that attention_packed balances its CTAs by."""
+    int32 [1]): the packed layout of the padding-compacted encoder (include/atlas_b200.h).  No host synchronisation."""
     require_cuda(live, "live")
     S, nb = live.shape
     live = live.contiguous()
@@ -419,10 +417,8 @@ def segment_tile_scan(live):
     tile_off = torch.empty(S * nb, dtype=torch.int32, device=live.device)
     tile_src = torch.empty(S * nb, dtype=torch.int32, device=live.device)
     count = torch.empty(1, dtype=torch.int32, device=live.device)
-    work = torch.empty(S + 1, dtype=torch.int32, device=live.device)
     check(lib().atlas_b200_segment_tile_scan(_ptr(live), S, nb, _ptr(keep), _ptr(tile_off), _ptr(tile_src), _ptr(count),
-                                             _ptr(work), current_stream_ptr()))
-    keep._atlas_work = work
+                                             current_stream_ptr()))
     return keep, tile_off, tile_src, count
 
 
@@ -451,11 +447,9 @@ def attention_packed(qkv, keep, tile_off, S, H, L, add_mask, bias_delta, scale=1
         out = torch.empty((qkv.shape[0], H * 64), dtype=qkv.dtype, device=qkv.device)
     am = add_mask.float().contiguous()
     bd = bias_delta.float().contiguous() if bias_delta is not None else None
-    work = getattr(keep, "_atlas_work", None) if _PACKED_BALANCE else None
     check(lib().atlas_b200_attention_packed(_ptr(qkv), qkv.stride(0), 0, H * 64, 2 * H * 64, _ptr(out), out.stride(0), _ptr(am),
-                                            _ptr(bd) if bd is not None else None, _ptr(keep), _ptr(tile_off),
-                                            _ptr(work) if work is not None else None, S, H, L, float(scale), _bf(qkv),
-                                            current_stream_ptr()))
+                                            _ptr(bd) if bd is not None else None, _ptr(keep), _ptr(tile_off), S, H, L,
+                                            float(scale), _bf(qkv), current_stream_ptr()))
     return out
 
 
@@ -582,11 +576,8 @@ def linear_dgrad(dy, weight):
 
 def linear_wgrad(dy, x):
     """dW [N, K] = dY^T [N, M] . X [M, K] (contraction over the M tokens, fp32 accumulation, 16-bit result): the wgmma
-    GEMM with both operands MN-major (no transposes).  ATLAS_B200_WGRAD_TRANSPOSE=1 selects the first-generation path
-    (two explicit transposes + the K-major GEMM), kept for A/B measurements."""
+    GEMM with both operands MN-major (no transposes)."""
     require_cuda(dy, "dy")
-    if os.environ.get("ATLAS_B200_WGRAD_TRANSPOSE") == "1":
-        return linear(transpose(dy), transpose(x))
     dy2, x2 = _rows2d(dy), _rows2d(x)
     if dy2.shape[0] != x2.shape[0] or dy2.dtype != x2.dtype:
         raise AtlasB200Error(f"linear_wgrad: dy {tuple(dy2.shape)} and x {tuple(x2.shape)} do not match")
@@ -762,27 +753,29 @@ def attention_bwd(q, q_col0, k, k_col0, v, v_col0, out, dout, dq, dq_col0, dk, d
                   split_keys=False, dropout=None, block_live=None):
     """Backward of `attention` / `cross_attention_split` (un-split key range).  dq / dk / dv are written in place at
     their column offsets; returns dbias_delta fp32 [H, Lq+Lk-1] (or None).  `lse` = the forward's log-sum-exp
-    (return_lse=True) saves the recomputation pass; split_keys (needs lse, no dbias; dq must be a whole contiguous
-    [B*Lq, H*64] tensor) spreads a long key range over many CTAs (FiD cross-attention)."""
+    (return_lse=True), required; split_keys (no dbias; dq must be a whole contiguous [B*Lq, H*64] tensor) spreads a long
+    key range over many CTAs (FiD cross-attention)."""
+    if lse is None:
+        raise AtlasB200Error("attention_bwd: needs the forward's log-sum-exp (lse, from return_lse=True)")
     require_cuda(q, "q")
     am = add_mask.float().contiguous() if add_mask is not None else None
     bd = bias_delta.float().contiguous() if bias_delta is not None else None
     dbias = torch.zeros((H, Lq + Lk - 1), dtype=torch.float32, device=q.device) if (need_dbias and bd is not None) else None
     dsum = torch.empty((B, H, Lq), dtype=torch.float32, device=q.device)
-    lse_buf = lse.contiguous() if lse is not None else torch.empty((B, H, Lq), dtype=torch.float32, device=q.device)
+    lse = lse.contiguous()
     o2 = out if out.stride(-1) == 1 else out.contiguous()
     do2 = _rows2d(dout)
     accum = None
     if split_keys:
-        if lse is None or dbias is not None or dq_col0 != 0 or not dq.is_contiguous() or dq.shape[1] != H * 64:
-            raise AtlasB200Error("attention_bwd: split_keys needs the forward's lse, no dbias and a contiguous dq")
+        if dbias is not None or dq_col0 != 0 or not dq.is_contiguous() or dq.shape[1] != H * 64:
+            raise AtlasB200Error("attention_bwd: split_keys needs no dbias and a contiguous dq")
         accum = torch.zeros((B * Lq, H * 64), dtype=torch.float32, device=q.device)
     dp, dseed, doff = dropout if dropout is not None else (0.0, 0, 0)
     check(lib().atlas_b200_attention_bwd_train(
         _ptr(q), q.stride(0), q_col0, _ptr(k), k.stride(0), k_col0, _ptr(v), v.stride(0), v_col0, _ptr(o2), o2.stride(0),
         _ptr(do2), do2.stride(0), _ptr(dq), dq.stride(0), dq_col0, _ptr(dk), dk.stride(0), dk_col0, _ptr(dv),
         dv.stride(0), dv_col0, _ptr(am) if am is not None else None, _ptr(bd) if bd is not None else None,
-        _ptr(dbias) if dbias is not None else None, _ptr(lse_buf), 1 if lse is not None else 0, _ptr(dsum),
+        _ptr(dbias) if dbias is not None else None, _ptr(lse), 1, _ptr(dsum),
         _ptr(accum) if accum is not None else None, B, H, Lq, Lk, float(scale), float(causal_value), float(dp),
         int(dseed), int(doff), _ptr(block_live) if block_live is not None else None, _bf(q), current_stream_ptr()))
     if accum is not None:

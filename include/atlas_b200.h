@@ -1,4 +1,4 @@
-/* atlas_b200 — C ABI of the B200-native retrieve-then-read hot path.
+/* atlas_b200 — C ABI of the H100-native (sm_90a) retrieve-then-read hot path.
  *
  * The reference (facebookresearch/atlas) is pure Python and has no FFI; its boundary for this path
  * is the Python module surface.  This header is the C-ABI layer underneath our
@@ -67,14 +67,6 @@ int atlas_b200_mips_topk(const void* bank, int64_t n, int64_t ld, int32_t is_bf1
                          const void* queries, int32_t nq, int32_t k,
                          void* out_scores, int64_t* out_ids, int64_t id_base, int64_t id_stride,
                          int32_t* status, void* workspace, size_t workspace_bytes, void* stream);
-
-/* Kept for ABI compatibility: there is one scan kernel (queries and bank tiles streamed through shared memory);
- * the mode is ignored. */
-void atlas_b200_mips_set_kernel(int32_t mode);
-
-/* Development aid: when a device buffer of gridDim*8 uint64 is registered, the main TS scan kernel
- * accumulates per-CTA cycle counters (producer wait, MMA waits, epilogue wait, total).  NULL = off. */
-void atlas_b200_mips_set_debug_counters(void* device_u64_buffer);
 
 /* Same contract, exact for ANY input (chunked scan, no thresholds); slower.  Used as the fallback
  * when `status` reports overflow.  Synchronous with respect to nothing: enqueued on `stream`. */
@@ -271,18 +263,18 @@ int atlas_b200_attention_combine_ex(const float* o_partial, const float* ml_part
 /* --------------------------------------------------------------------------------------------
  * Backward pass (training): what autograd derives in the reference's train.py step
  * (`Atlas.forward` -> `loss.backward()`, src/atlas.py:399-550) for the kernels above.  Weight and
- * input gradients of the linear layers are atlas_b200_linear calls on transposed operands
- * (dX = dY . W via W^T, dW = dY^T . X via atlas_b200_transpose); the entry points below are the rest.
+ * input gradients of the linear layers are wgmma GEMMs (dX = dY . W: atlas_b200_linear on W^T;
+ * dW = dY^T . X: atlas_b200_linear_wgrad); the entry points below are the rest.
  * -------------------------------------------------------------------------------------------- */
 
 /* Backward of atlas_b200_attention (any Lq / Lk, head_dim 64; csrc/attention_bwd.cu).  q / k / v / out as in the
  * forward (out = the forward's result [B*Lq, H*64]); dout [B*Lq, H*64]; dq / dk / dv are written at column offsets
  * d?_col0 + 64h of [B*L, ld] buffers (so one [tokens, 3*H*64] buffer can receive dQ | dK | dV for a fused projection).
  * dbias_delta [H, Lq+Lk-1] fp32 is INCREMENTED (zero it first; NULL = not needed); lse / dsum are [B, H, Lq] fp32:
- * with lse_given != 0, `lse` holds the forward's log-sum-exp (atlas_b200_attention_ex / _combine_ex) and is only read,
- * otherwise it is recomputed (one more pass over the keys) and written.  For FiD's cross-attention
+ * `lse` holds the forward's log-sum-exp (atlas_b200_attention_ex / _train / _combine_ex) and is only read; lse_given must
+ * be non-zero (ATLAS_B200_EINVAL otherwise), `dsum` is scratch.  For FiD's cross-attention
  * (src/fid.py:298-349) pass the un-split key range: B = batch, Lk = n_ctx * L; with dq_accum [B*Lq, H*64] fp32 (zeroed,
- * needs lse_given, no dbias) the keys are split over several CTAs that add their partial dQ into dq_accum instead of
+ * no dbias) the keys are split over several CTAs that add their partial dQ into dq_accum instead of
  * writing `dq` - the caller converts it to 16 bits (atlas_b200_cast_f32).
  * Replaces autograd through BertSelfAttention.forward (src/modeling_bert.py:328-366) and T5Attention.forward
  * (src/modeling_t5.py:478-524). */
@@ -386,7 +378,7 @@ int atlas_b200_attention_dropout_mask(uint8_t* out, int64_t rows, int32_t Lk, fl
  * keep[b, h, i, j] is a function of (seed, offset, (b * H + h) * Lq + i, j) (csrc/dropout.cuh; j = key index over the whole
  * key range when the keys are split: segment s of `q_div` covers j = s * Lk ..., Lk % 32 == 0 required then);
  * atlas_b200_attention_bwd_train re-derives the same mask.  dropout_p == 0 is atlas_b200_attention_ex.
- * key_block_live (optional, uint8 [B, ceil(Lk / 64)], used by the three-lane encoder kernel): 0 marks a 64-key block whose keys
+ * key_block_live (optional, uint8 [B, ceil(Lk / 64)]): 0 marks a 64-key block whose keys
  * are ALL masked out (additive mask <= -5000, softmax weight exactly 0 in fp32): it is neither loaded nor computed - identical
  * results; every row keeps at least one live block (see atlas_b200_cross_attention_stream). */
 int atlas_b200_attention_train(const void* q, int64_t ldq, int32_t q_col0, const void* k, int64_t ldk, int32_t k_col0,
@@ -482,8 +474,7 @@ int atlas_b200_cross_attention_stream_compact(const void* q, int64_t ldq, int32_
  * the packed row count lives in device memory.
  *   atlas_b200_segment_tile_scan: live uint8 [S, nb] (key_block_live) -> keep [S, nb] (tiles 0 .. last live tile of the segment;
  *     all nb if none is live), tile_off int32 [S * nb] (packed index of a kept tile, -1 = dropped), tile_src int32 [S * nb] (source
- *     tile of packed tile o, -1 past the end), *count_rows = 64 x #kept; work_prefix int32 [S + 1] (optional): exclusive prefix
- *     of kept tiles x kept 128-row query tiles per segment - atlas_b200_attention_packed balances its CTAs by it.
+ *     tile of packed tile o, -1 past the end), *count_rows = 64 x #kept.
  *   atlas_b200_embed_packed_tiles: dst[64 o + r, :] = table[ids[64 tile_src[o] + r], :] (zeros past the end): T5Stack's
  *     embed_tokens (src/modeling_t5.py:930-934) straight into the packed layout.
  *   atlas_b200_linear_rows: atlas_b200_linear_ex over the first *m_dev rows (row blocks past it are not computed; rows of the
@@ -494,7 +485,7 @@ int atlas_b200_cross_attention_stream_compact(const void* q, int64_t ldq, int32_
  *   atlas_b200_expand_packed_tiles: back to the padded layout [S * nb * 64, d] (zeros at dropped tiles - the positions the
  *     reference fills with values nothing reads). */
 int atlas_b200_segment_tile_scan(const uint8_t* live, int32_t S, int32_t nb, uint8_t* keep, int32_t* tile_off, int32_t* tile_src,
-                                 int32_t* count_rows, int32_t* work_prefix, void* stream);
+                                 int32_t* count_rows, void* stream);
 int atlas_b200_embed_packed_tiles(const int64_t* ids, const void* table, int64_t ldt, int32_t vocab, const int32_t* tile_src,
                                   int32_t n_tiles, void* dst, int64_t ldd, int32_t d, void* stream);
 int atlas_b200_linear_rows(const void* A, int64_t lda, const void* W, int64_t ldw, const void* bias, const void* residual,
@@ -502,8 +493,7 @@ int atlas_b200_linear_rows(const void* A, int64_t lda, const void* W, int64_t ld
                            int32_t is_bf16, const float* row_ss, float* out_ss, float rs_eps, const int32_t* m_dev, void* stream);
 int atlas_b200_attention_packed(const void* qkv, int64_t ld, int32_t q_col0, int32_t k_col0, int32_t v_col0, void* out, int64_t ldo,
                                 const float* add_mask, const float* bias_delta, const uint8_t* keep, const int32_t* tile_off,
-                                const int32_t* work_prefix, int32_t B, int32_t H, int32_t L, float scale, int32_t is_bf16,
-                                void* stream);
+                                int32_t B, int32_t H, int32_t L, float scale, int32_t is_bf16, void* stream);
 int atlas_b200_expand_packed_tiles(const void* src, int64_t lds, const int32_t* tile_off, int32_t n_tiles, void* dst, int64_t ldd,
                                    int32_t d, void* stream);
 

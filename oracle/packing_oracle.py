@@ -25,10 +25,9 @@ def live_tiles(attention_mask, tile=TILE):
 
 
 def segment_tables(live):
-    """live uint8 [S, nb] -> (keep [S, nb], tile_off int32 [S * nb], tile_src int32 [S * nb], count_rows, work_prefix int32
-    [S + 1]).  keep: tiles 0 .. last live tile of the segment (all nb when none is live).  tile_off: index of a kept tile in
-    the packed order, -1 for a dropped one; tile_src: its inverse, -1 past the end; count_rows = 64 x #kept;
-    work_prefix: exclusive prefix of kept tiles x kept 128-row query tiles per segment."""
+    """live uint8 [S, nb] -> (keep [S, nb], tile_off int32 [S * nb], tile_src int32 [S * nb], count_rows).  keep: tiles
+    0 .. last live tile of the segment (all nb when none is live).  tile_off: index of a kept tile in the packed order, -1 for
+    a dropped one; tile_src: its inverse, -1 past the end; count_rows = 64 x #kept."""
     live = np.asarray(live).astype(bool)
     S, nb = live.shape
     keep = np.zeros((S, nb), dtype=np.uint8)
@@ -40,6 +39,4 @@ def segment_tables(live):
     off = np.where(flat, np.cumsum(flat) - 1, -1).astype(np.int32)
     src = np.full(S * nb, -1, dtype=np.int32)
     src[: int(flat.sum())] = np.flatnonzero(flat).astype(np.int32)
-    f = keep.sum(1).astype(np.int64)
-    work = np.concatenate([[0], np.cumsum(f * ((f + 1) // 2))]).astype(np.int32)
-    return keep, off, src, TILE * int(flat.sum()), work
+    return keep, off, src, TILE * int(flat.sum())

@@ -44,3 +44,19 @@ def test_no_cpu_fallback():
     bank = torch.zeros(64, 768, dtype=torch.float16)
     with pytest.raises(AtlasB200Error):
         ops.mips_topk(bank, torch.zeros(1, 768), 4)
+
+
+def test_attention_bwd_requires_forward_lse():
+    """atlas_b200_attention_bwd_train with lse_given = 0 is rejected during argument validation, before any CUDA call:
+    the backward reads the log-sum-exp the forward wrote and has no path that recomputes it."""
+    from atlas_b200 import _lib
+
+    L = _lib.lib()
+    B, H, Lq, Lk, ld = 2, 4, 64, 64, 3 * 4 * 64
+    buf = (ctypes.c_float * (B * H * Lq))()
+    p = ctypes.cast(buf, ctypes.c_void_p)     # non-null stand-in for q, k, v, out, dout, dq, dk, dv, lse and dsum
+    rc = L.atlas_b200_attention_bwd_train(p, ld, 0, p, ld, 64 * H, p, ld, 128 * H, p, 64 * H, p, 64 * H, p, ld, 0, p, ld,
+                                          64 * H, p, ld, 128 * H, None, None, None, p, 0, p, None, B, H, Lq, Lk,
+                                          0.125, 0.0, 0.0, 0, 0, None, 1, None)
+    assert rc == 1, rc                                             # ATLAS_B200_EINVAL
+    assert b"log-sum-exp" in L.atlas_b200_last_error() and b"lse" in L.atlas_b200_last_error()

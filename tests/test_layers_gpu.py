@@ -143,7 +143,7 @@ def test_attention_matches_fp32_reference(dev, dtype, B, H, L, mode):
 @pytest.mark.parametrize("B,H,L,mode", [(3, 12, 384, "nomask"), (2, 4, 200, "causal"), (2, 12, 384, "ramp"),
                                         (3, 12, 256, "bert_nomask"), (37, 12, 384, "t5enc"), (2, 12, 480, "t5enc")])
 def test_attention_lanes_kernel_cases(dev, dtype, B, H, L, mode):
-    """The three-lane kernel (csrc/attention_lanes.cu, >= 2 query tiles per segment) on the cases the generic test does not
+    """The attention kernel (csrc/attention.cu) with >= 2 query tiles per segment on the cases the generic test does not
     reach: no key mask at all (the bench's shape), causal + bias with several query tiles, a bias RAMP that makes every
     later key block exceed the lazy reference maximum by more than 2^8 (the in-place rescale of O runs on every block),
     more (segment, head) items than SMs x 3 with the bias table changing inside a CTA's item range, and 5 key blocks."""
@@ -294,7 +294,7 @@ def test_cross_attention_stream_kernel(dev, dtype, B, H, T, Lk):
 @pytest.mark.parametrize("S,H,L,use_bias", [(7, 3, 384, True), (5, 2, 200, True), (4, 12, 512, False), (3, 1, 512, True)])
 def test_masked_key_blocks_are_skipped_without_changing_the_result(dev, dtype, S, H, L, use_bias):
     """ops.key_block_live: 64-key blocks made of masked keys only (padding to text_maxlength) are neither loaded nor computed
-    by the three-lane encoder kernel.  Their softmax weights are exactly 0 in fp32, so the output must be BIT-identical to
+    by the attention kernel.  Their softmax weights are exactly 0 in fp32, so the output must be BIT-identical to
     the run that computes every block - and equal to the fp32 restatement."""
     from atlas_b200 import ops
 

@@ -91,11 +91,10 @@ def test_segment_table_rule_on_hand_written_cases():
     mask[2, 130:140] = 1
     live = packing_oracle.live_tiles(mask)          # row 3: no real token at all -> every tile live
     assert live.tolist() == [[1, 1, 0, 0], [1, 1, 1, 1], [1, 0, 1, 0], [1, 1, 1, 1]]
-    keep, off, src, rows, work = packing_oracle.segment_tables(live)
+    keep, off, src, rows = packing_oracle.segment_tables(live)
     assert keep.tolist() == [[1, 1, 0, 0], [1, 1, 1, 1], [1, 1, 1, 0], [1, 1, 1, 1]]
     assert off.tolist() == [0, 1, -1, -1, 2, 3, 4, 5, 6, 7, 8, -1, 9, 10, 11, 12]
     assert src.tolist() == [0, 1, 4, 5, 6, 7, 8, 9, 10, 12, 13, 14, 15, -1, -1, -1]
     assert rows == 13 * 64
-    assert work.tolist() == [0, 2, 10, 16, 24]          # kept x ceil(kept / 2): 2*1, 4*2, 3*2, 4*2
     # ragged length: the last tile is partial
     assert packing_oracle.live_tiles(np.ones((1, 100), dtype=np.int64)).tolist() == [[1, 1]]

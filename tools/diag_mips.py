@@ -1,4 +1,4 @@
-"""GPU diagnostic for the MIPS path (run under gpurun).  Prints detailed mismatch information."""
+"""GPU diagnostic for the MIPS path.  Prints detailed mismatch information."""
 import os, sys, time, json
 import numpy as np
 import torch
@@ -49,10 +49,6 @@ def run_case(n, nq, k, dist="grid", bseed=1, qseed=2, exhaustive=False, verbose=
     return ok_s and ok_i
 
 
-from atlas_b200._lib import lib
-MODE = int(sys.argv[1]) if len(sys.argv) > 1 else 1
-lib().atlas_b200_mips_set_kernel(MODE)
-print("kernel mode", MODE, "(ignored: one scan kernel)", flush=True)
 results = {}
 try:
     results["single_small"] = run_case(128, 4, 128)

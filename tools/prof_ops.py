@@ -129,7 +129,7 @@ elif what == "mips":
     print(f"mips n={n} nq={nq} k={k}: {ms:.3f} ms = {n * 768 * 2 / ms / 1e6:.0f} GB/s over the bank")
 elif what == "packed":
     # the padding-compacted FiD-base encoder ops at the bench's length distribution (8 queries x 40 passages, U[148, 276] real
-    # tokens padded to 384): packed three-lane attention vs the padded kernel with block skipping vs no skipping, and the gated
+    # tokens padded to 384): packed attention vs the padded kernel with block skipping vs no skipping, and the gated
     # projection over the packed rows (device-side row count) vs all rows
     S, H, L = 320, 12, 384
     lens = torch.randint(148, 277, (S,), device=dev)
