@@ -192,9 +192,17 @@ decode_self_attention_kernel(const uint16_t* __restrict__ qkv, int64_t ldqkv, ui
     out[static_cast<int64_t>(b) * ldo + h * D + d] = r;
 }
 
+// (x, i) ranks above (y, j) in torch.argmax's order: NaN above every number, then the larger value; among equal values or
+// among NaNs the lower index.  Plain `x > y` would skip NaNs, and an all-NaN row would keep the "no index" sentinel.
+__device__ __forceinline__ bool argmax_better(float x, int i, float y, int j) {
+    const bool xn = isnan(x), yn = isnan(y);
+    if (xn != yn) return xn;
+    return x > y || ((xn || x == y) && i < j);
+}
+
 // next[b] = done[b] ? pad : argmax_v(logits[b, v] + (v == eos && t + 1 < min_length ? -inf : 0)); seq[b, t + 1] = next;
 // done |= next == eos; tok_in[b] = next (the next step's decoder input); t += 1 (thread 0 of block 0).
-// grid = B, block = 256.  Ties resolve to the LOWEST index like torch.argmax.
+// grid = B, block = 256.  Same pick as torch.argmax: the first NaN if any, else the lowest index of the maximum.
 template <bool kBF16>
 __global__ void __launch_bounds__(256)
 decode_argmax_kernel(const uint16_t* __restrict__ logits, int64_t ld, int V, int64_t* __restrict__ seq, int64_t ld_seq,
@@ -212,7 +220,7 @@ decode_argmax_kernel(const uint16_t* __restrict__ logits, int64_t ld, int V, int
     for (int v = threadIdx.x; v < V; v += blockDim.x) {
         float x = ld16(logits[static_cast<int64_t>(b) * ld + v]);
         if (ban_eos && v == eos) x = -INFINITY;
-        if (x > best || (x == best && v < idx)) best = x, idx = v;
+        if (argmax_better(x, v, best, idx)) best = x, idx = v;
     }
     __shared__ float s_b[256];
     __shared__ int s_i[256];
@@ -223,7 +231,7 @@ decode_argmax_kernel(const uint16_t* __restrict__ logits, int64_t ld, int V, int
         if (threadIdx.x < s) {
             const float ob = s_b[threadIdx.x + s];
             const int oi = s_i[threadIdx.x + s];
-            if (ob > s_b[threadIdx.x] || (ob == s_b[threadIdx.x] && oi < s_i[threadIdx.x])) s_b[threadIdx.x] = ob, s_i[threadIdx.x] = oi;
+            if (argmax_better(ob, oi, s_b[threadIdx.x], s_i[threadIdx.x])) s_b[threadIdx.x] = ob, s_i[threadIdx.x] = oi;
         }
         __syncthreads();
     }

@@ -9,6 +9,11 @@
 // three [B, T, n*L] fp32 maps are written once.
 //
 // Block = 32 consecutive keys of one batch element, 8 warps x 4 keys; lane = query position (t = lane + 32 c).
+//
+// Precision: S and the given lse are fp32, so a key's S carries the rounding of its mask term (up to |mask| * 2^-24).  In a row
+// whose keys are ALL masked with -1e9 that rounding (32) swallows the logits, and the fp32 lse loses log(Lk) the same way, so
+// P = exp(S - lse) comes out near 1 per key instead of the reference's uniform 1 / Lk.  FiD never builds such a row (every
+// passage holds the question tokens); at -1e4 (fp16) a fully masked row keeps about 3 significant digits.
 #include "common.cuh"
 #include "host_common.h"
 

@@ -816,8 +816,6 @@ def decode_cross_attention(q, kv, B, H, Lk, add_mask=None, scale=1.0, chunk=256,
     """q [B, H*64] against kv [B*Lk, 2*H*64] (k | v): chunked partials + the split-KV combine -> ctx [B, H*64].
     tile_live = key_block_live(add_mask): 64-key tiles of masked keys only are not read (identical result)."""
     require_cuda(q, "q")
-    if tile_live is not None and chunk % 64 != 0:
-        tile_live = None
     chunks = (Lk + chunk - 1) // chunk
     o_part = torch.empty((B * chunks, H * 64), dtype=torch.float32, device=q.device)
     ml = torch.empty((B * chunks, H, 2), dtype=torch.float32, device=q.device)

@@ -195,14 +195,15 @@ int atlas_b200_masked_mean_pool(const void* x, const int64_t* mask, void* out, i
  *  decode_self_attention   appends the new token's K | V (columns H*64.. of qkv [B, 3*H*64]) to cache [B, Tmax, 2*H*64] at
  *      row *t_dev and attends over keys 0..*t_dev with bias_delta [H, 2*Tmax-1] (T5 relative bias by offset, NULL = none).
  *      The step index lives in DEVICE memory so that one captured CUDA graph serves every step.
- *  decode_argmax           greedy pick (lowest index among ties, EOS banned while *t_dev + 1 < min_length, finished rows
- *      emit pad_id): seq[b, *t_dev + 1] = tok_in[b] = next; done[b] |= next == eos; then *t_dev += 1. */
+ *  decode_argmax           greedy pick as torch.argmax (a NaN beats every number; among equal values or among NaNs the lowest
+ *      index wins; EOS banned while *t_dev + 1 < min_length, finished rows emit pad_id):
+ *      seq[b, *t_dev + 1] = tok_in[b] = next; done[b] |= next == eos; then *t_dev += 1. */
 int atlas_b200_decode_cross_attention(const void* q, int64_t ldq, const void* kv, int64_t ldkv, int32_t k_col0,
                                       int32_t v_col0, const float* add_mask, int32_t B, int32_t H, int32_t Lk,
                                       int32_t chunk, float scale, float* o_partial, float* ml_partial, int32_t is_bf16,
                                       void* stream);
 /* ... with the live-tile flags of atlas_b200_cross_attention_stream (uint8 [B, ceil(Lk / 64)], NULL = all live): 64-key tiles of
- * masked keys only are not read.  chunk must be a multiple of 64 when flags are given. */
+ * masked keys only are not read.  chunk is a multiple of 16 as without flags: a warp's 16-key group never straddles a tile. */
 int atlas_b200_decode_cross_attention_live(const void* q, int64_t ldq, const void* kv, int64_t ldkv, int32_t k_col0,
                                       int32_t v_col0, const float* add_mask, const uint8_t* tile_live, int32_t B, int32_t H, int32_t Lk,
                                       int32_t chunk, float scale, float* o_partial, float* ml_partial, int32_t is_bf16,
