@@ -138,6 +138,13 @@ def lib():
     L.atlas_b200_decode_self_attention.argtypes = [vp, i64, vp, i32, vp, vp, f32, vp, i64, i32, i32, i32, vp]
     L.atlas_b200_decode_argmax.restype = c.c_int
     L.atlas_b200_decode_argmax.argtypes = [vp, i64, i32, vp, i64, vp, vp, vp, i32, i32, i32, i32, i32, vp]
+    L.atlas_b200_decode_self_attention_beam.restype = c.c_int
+    L.atlas_b200_decode_self_attention_beam.argtypes = [vp, i64, vp, i32, vp, vp, vp, f32, vp, i64, i32, i32, i32, vp]
+    L.atlas_b200_beam_topk.restype = c.c_int
+    L.atlas_b200_beam_topk.argtypes = [vp, i64, i32, vp, i64, vp, vp, i32, i32, i32, i32, vp, vp, vp, i32, i32, vp]
+    L.atlas_b200_beam_select.restype = c.c_int
+    L.atlas_b200_beam_select.argtypes = [vp, vp, i32, i32, i32, vp, vp, vp, vp, vp, vp, i32, vp, vp, vp, vp, vp, vp, vp,
+                                         i32, i32, c.c_double, vp]
     L.atlas_b200_splice_tokens.restype = c.c_int
     L.atlas_b200_splice_tokens.argtypes = [vp, vp, i64, i64, vp, vp, vp, i64, i32, i32, i32, i32, i32, vp, vp, vp]
     u64 = c.c_uint64
@@ -236,6 +243,9 @@ EXPORTED_SYMBOLS = [
     "atlas_b200_decode_cross_attention",
     "atlas_b200_decode_self_attention",
     "atlas_b200_decode_argmax",
+    "atlas_b200_decode_self_attention_beam",
+    "atlas_b200_beam_topk",
+    "atlas_b200_beam_select",
     "atlas_b200_dropout",
     "atlas_b200_dropout_mask",
     "atlas_b200_attention_dropout_mask",

@@ -149,15 +149,22 @@ decode_cross_attention_kernel(const uint16_t* __restrict__ q, int64_t ldq, const
 
 // grid = (H, B); block = 64 (thread = head dim).  qkv [B, 3*H*64] = (q | k | v) of the NEW token; cache [B, Tmax, 2*H*64]
 // (k | v); step t is read from device memory.  bias_delta [H, 2*Tmax - 1]: entry (j - i) + (Tmax - 1) (nullptr = none).
-template <bool kBF16>
+// kAnc (beam search): anc [2, B, Tmax], buffer (t & 1): key / value j of row b is cache row (anc[b, j], j) instead of (b, j);
+// the new token still lands in (b, t) (anc[b, t] == b).  Same arithmetic in the same order as without kAnc.
+template <bool kBF16, bool kAnc = false>
 __global__ void __launch_bounds__(D)
 decode_self_attention_kernel(const uint16_t* __restrict__ qkv, int64_t ldqkv, uint16_t* __restrict__ cache, int Tmax,
                              const int32_t* __restrict__ t_dev, const float* __restrict__ bias_delta, float scale,
-                             uint16_t* __restrict__ out, int64_t ldo, int H) {
+                             uint16_t* __restrict__ out, int64_t ldo, int H, const int32_t* __restrict__ anc = nullptr) {
     const int h = blockIdx.x, b = blockIdx.y, d = threadIdx.x;
     const int t = min(max(*t_dev, 0), Tmax - 1);
     const int64_t ldc = static_cast<int64_t>(2) * H * D;
     uint16_t* crow = cache + (static_cast<int64_t>(b) * Tmax) * ldc;
+    const int32_t* arow = kAnc ? anc + (static_cast<int64_t>(t & 1) * gridDim.y + b) * Tmax : nullptr;
+    auto key_row = [&](int j) -> const uint16_t* {
+        if constexpr (kAnc) return cache + (static_cast<int64_t>(__ldg(arow + j)) * Tmax + j) * ldc;
+        return crow + static_cast<int64_t>(j) * ldc;
+    };
     const uint16_t* tok = qkv + static_cast<int64_t>(b) * ldqkv;
     // append this token's K | V (the reference concatenates past_key_value with the new states, modeling_t5.py:459-470)
     crow[static_cast<int64_t>(t) * ldc + h * D + d] = tok[H * D + h * D + d];
@@ -171,7 +178,8 @@ decode_self_attention_kernel(const uint16_t* __restrict__ qkv, int64_t ldqkv, ui
     float m = -INFINITY, l = 0.f, acc = 0.f;
     __syncthreads();     // the appended row is visible to the block
     for (int j = 0; j <= t; ++j) {
-        float s = qd * ld16(crow[static_cast<int64_t>(j) * ldc + h * D + d]);
+        const uint16_t* kvrow = key_row(j);
+        float s = qd * ld16(kvrow[h * D + d]);
 #pragma unroll
         for (int off = 16; off > 0; off >>= 1) s += __shfl_xor_sync(0xffffffffu, s, off);
         if ((d & 31) == 0) s_part[d >> 5] = s;
@@ -182,7 +190,7 @@ decode_self_attention_kernel(const uint16_t* __restrict__ qkv, int64_t ldqkv, ui
         const float m_new = fmaxf(m, s);
         const float corr = __expf(m - m_new), p = __expf(s - m_new);
         l = l * corr + p;
-        acc = acc * corr + p * ld16(crow[static_cast<int64_t>(j) * ldc + H * D + h * D + d]);
+        acc = acc * corr + p * ld16(kvrow[H * D + h * D + d]);
         m = m_new;
     }
     const float o = acc / l;
@@ -301,6 +309,27 @@ int atlas_b200_decode_self_attention(const void* qkv, int64_t ldqkv, void* cache
         dec::decode_self_attention_kernel<false><<<grid, dec::D, 0, s>>>(static_cast<const uint16_t*>(qkv), ldqkv,
                                                                          static_cast<uint16_t*>(cache), Tmax, t_dev, bias_delta,
                                                                          scale, static_cast<uint16_t*>(out), ldo, H);
+    abh::count_launch();
+    AB_CUDA_CHECK(cudaGetLastError());
+    return ATLAS_B200_OK;
+}
+
+int atlas_b200_decode_self_attention_beam(const void* qkv, int64_t ldqkv, void* cache, int32_t Tmax, const int32_t* t_dev,
+                                          const int32_t* anc, const float* bias_delta, float scale, void* out, int64_t ldo,
+                                          int32_t R, int32_t H, int32_t is_bf16, void* stream) {
+    AB_REQUIRE(R >= 0 && H > 0 && Tmax > 0 && t_dev != nullptr && anc != nullptr, "decode_self_attention_beam: bad shape");
+    AB_REQUIRE(R <= 65535 && H <= 65535, "decode_self_attention_beam: grid too large");
+    if (R == 0) return ATLAS_B200_OK;
+    cudaStream_t s = static_cast<cudaStream_t>(stream);
+    dim3 grid(H, R);
+    if (is_bf16)
+        dec::decode_self_attention_kernel<true, true><<<grid, dec::D, 0, s>>>(
+            static_cast<const uint16_t*>(qkv), ldqkv, static_cast<uint16_t*>(cache), Tmax, t_dev, bias_delta, scale,
+            static_cast<uint16_t*>(out), ldo, H, anc);
+    else
+        dec::decode_self_attention_kernel<false, true><<<grid, dec::D, 0, s>>>(
+            static_cast<const uint16_t*>(qkv), ldqkv, static_cast<uint16_t*>(cache), Tmax, t_dev, bias_delta, scale,
+            static_cast<uint16_t*>(out), ldo, H, anc);
     abh::count_launch();
     AB_CUDA_CHECK(cudaGetLastError());
     return ATLAS_B200_OK;

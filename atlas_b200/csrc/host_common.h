@@ -45,7 +45,14 @@ int num_sms();
 
 // Optional CUDA-event bracketing of the dominant kernel (bench.py's roofline measurement): when
 // enabled, callers wrap that launch with prof_begin/prof_end on the launching stream.
-enum ProfKind { PROF_SCAN = 1, PROF_LINEAR = 2, PROF_ATTENTION = 3, PROF_ATTENTION_BWD = 4, PROF_DECODE_CROSS = 5 };
+enum ProfKind {
+    PROF_SCAN = 1,
+    PROF_LINEAR = 2,
+    PROF_ATTENTION = 3,
+    PROF_ATTENTION_BWD = 4,
+    PROF_DECODE_CROSS = 5,
+    PROF_BEAM_SELECT = 6,     // beam_topk + beam_select (csrc/beam.cu); work = bytes read
+};
 void prof_begin(cudaStream_t s, int kind);
 void prof_end(cudaStream_t s, int kind, double work);   // work = algorithmic bytes (scan) or FLOPs of this launch
 // ... of a launch whose row count lives in device memory: work = work_per_row * min(m_max, *m_dev), resolved when read

@@ -803,18 +803,26 @@ class FiD(nn.Module):
         H = c.num_heads
         eps = c.layer_norm_epsilon
         B, Lk = st.B, st.Lk
-        h = W["shared.weight"][st.tok_in]                                          # [B, d]
+        nb = getattr(st, "nb", 1)           # beam search: B * nb rows, the nb beams of a batch element consecutive
+        h = W["shared.weight"][st.tok_in]                                          # [B * nb, d]
         for i in range(c.num_decoder_layers):
             p = f"decoder.block.{i}.layer.0."
             n = ops.layernorm(h, W[p + "layer_norm.weight"], None, eps, kind=1)
             qkv = ops.linear(n, G[p + "SelfAttention.qkv"])
-            ctx = ops.decode_self_attention(qkv, st.self_kv[i], st.t_dev, H, bias_delta=st.bias, scale=1.0)
+            if nb > 1:      # history gathered through the beams' ancestry table: the cache is never reordered
+                ctx = ops.decode_self_attention_beam(qkv, st.self_kv[i], st.t_dev, st.anc, H, bias_delta=st.bias, scale=1.0)
+            else:
+                ctx = ops.decode_self_attention(qkv, st.self_kv[i], st.t_dev, H, bias_delta=st.bias, scale=1.0)
             h = ops.clamp_inf_(ops.linear(ctx, W[p + "SelfAttention.o.weight"], None, residual=h, epilogue=ops.EPI_RESIDUAL))
             p = f"decoder.block.{i}.layer.1."
             n = ops.layernorm(h, W[p + "layer_norm.weight"], None, eps, kind=1)
             q = ops.linear(n, W[p + "EncDecAttention.q.weight"])
-            ctx = ops.decode_cross_attention(q, st.cross_kv[i], B, H, Lk, add_mask=st.cross_mask, scale=1.0,
-                                             chunk=st.chunk, tile_live=st.cross_live)
+            if nb > 1:      # the nb beams share their batch element's cross K | V, streamed once per step
+                ctx = ops.decode_cross_attention_beams(q, st.cross_kv[i], B, nb, H, Lk, st.cross_mask, st.chunk,
+                                                       tile_live=st.cross_live)
+            else:
+                ctx = ops.decode_cross_attention(q, st.cross_kv[i], B, H, Lk, add_mask=st.cross_mask, scale=1.0,
+                                                 chunk=st.chunk, tile_live=st.cross_live)
             h = ops.clamp_inf_(ops.linear(ctx, W[p + "EncDecAttention.o.weight"], None, residual=h,
                                           epilogue=ops.EPI_RESIDUAL))
             h = self._ff(W, G, f"decoder.block.{i}.layer.2.", h, eps)
@@ -823,38 +831,79 @@ class FiD(nn.Module):
             h = (h.float() * (c.d_model ** -0.5)).to(dt)
         return ops.linear(h, W["lm_head.weight"])
 
-    def _decode_state(self, B, Lk, Tmax, dt, dev):
-        key = (B, Lk, Tmax, dt, dev)
+    class _BeamState:
+        """Static buffers of one (batch, beams, keys, max_length, dtype) beam-search shape (csrc/beam.cu): the per-layer
+        self K|V caches of the R = B * nb beam rows, ONE cross K|V per batch element, the ancestry and token tables, the beam
+        scores and the hypothesis slots, all read and written on the device so that one captured graph serves every step."""
+
+        def __init__(self, model, B, nb, Lk, Tmax, dt, dev):
+            c = model.config
+            H = c.num_heads
+            nl = c.num_decoder_layers
+            R = B * nb
+            self.B, self.nb, self.R, self.Lk, self.Tmax = B, nb, R, Lk, Tmax
+            self.self_kv = [torch.zeros((R, Tmax, 2 * H * 64), dtype=dt, device=dev) for _ in range(nl)]
+            self.cross_kv = [torch.empty((B * Lk, 2 * H * 64), dtype=dt, device=dev) for _ in range(nl)]
+            self.cross_mask = torch.zeros((B, Lk), dtype=torch.float32, device=dev)
+            self.tok_in = torch.zeros(R, dtype=torch.int64, device=dev)
+            self.t_dev = torch.zeros(1, dtype=torch.int32, device=dev)
+            self.anc = torch.zeros((2, R, Tmax), dtype=torch.int32, device=dev)
+            self.tok = torch.zeros((R, Tmax), dtype=torch.int32, device=dev)
+            self.parent = torch.zeros(R, dtype=torch.int32, device=dev)
+            self.beam_scores = torch.zeros(R, dtype=torch.float32, device=dev)
+            self.done = torch.zeros(B, dtype=torch.uint8, device=dev)
+            self.hyp_score = torch.zeros((B, nb), dtype=torch.float64, device=dev)
+            self.hyp_len = torch.zeros((B, nb), dtype=torch.int32, device=dev)
+            self.hyp_ins = torch.zeros((B, nb), dtype=torch.int32, device=dev)
+            self.hyp_tok = torch.zeros((B, nb, Tmax), dtype=torch.int32, device=dev)
+            self.hyp_state = torch.zeros((B, 2), dtype=torch.int32, device=dev)
+            self.hyp_worst = torch.zeros(B, dtype=torch.float64, device=dev)
+            self.cand_score = torch.empty((R, 2 * nb), dtype=torch.float32, device=dev)
+            self.cand_tok = torch.empty((R, 2 * nb), dtype=torch.int32, device=dev)
+            self.graph = None
+            self.cross_live = None
+
+        def reset(self, start, pad):
+            """beam_search's start: every row holds the decoder start token, beam 0 scores 0 and the others -1e9."""
+            self.anc.copy_(torch.arange(self.R, dtype=torch.int32, device=self.anc.device)[None, :, None].expand_as(self.anc))
+            self.tok.fill_(pad)
+            self.tok[:, 0] = start
+            self.tok_in.fill_(start)
+            self.t_dev.zero_()
+            self.done.zero_()
+            self.beam_scores.fill_(-1e9)
+            self.beam_scores.view(self.B, self.nb)[:, 0] = 0.0
+            self.hyp_state.zero_()
+            self.hyp_worst.fill_(1e9)
+
+        def select_buffers(self):
+            """The tensors ops.beam_select reads and writes, in its argument order."""
+            return (self.beam_scores, self.tok_in, self.parent, self.done, self.anc, self.tok, self.t_dev, self.hyp_score,
+                    self.hyp_len, self.hyp_ins, self.hyp_tok, self.hyp_state, self.hyp_worst)
+
+        def sequences(self, t):
+            """The rows' tokens at positions 0..t, gathered through the ancestry of step t -> int64 [R, t + 1]."""
+            pos = torch.arange(t + 1, device=self.tok.device)
+            return self.tok[self.anc[t & 1, :, : t + 1].long(), pos[None, :]].long()
+
+    def _decode_state(self, B, Lk, Tmax, dt, dev, nb=1):
+        key = (B, Lk, Tmax, dt, dev) if nb == 1 else (B, Lk, Tmax, dt, dev, nb)
         states = self.__dict__.setdefault("_decode_states", {})
         st = states.get(key)
         if st is None:
             if len(states) >= 2:
                 states.pop(next(iter(states)))
-            st = FiD._DecodeState(self, B, Lk, Tmax, dt, dev)
+            st = FiD._DecodeState(self, B, Lk, Tmax, dt, dev) if nb == 1 else FiD._BeamState(self, B, nb, Lk, Tmax, dt, dev)
             # keys per block of the cross-attention sweep: ~4 blocks per SM keep every SM streaming
             st.chunk = 256 if Lk >= 2048 else 64
             states[key] = st
         return st
 
-    @torch.no_grad()
-    def generate(self, input_ids=None, attention_mask=None, max_length=32, min_length=1, num_beams=1,
-                 num_return_sequences=1, length_penalty=1.0, forced_bos_token_id=None, prefix_allowed_tokens_fn=None,
-                 use_cache=True, **unused):
-        """Greedy decoding (what `Atlas.generate` requests with num_beams=1, src/atlas.py:592-619; transformers 4.18
-        `greedy_search` with `use_cache`): the encoder and the cross-attention K|V projections run once; every step
-        decodes ONE token per sequence against the per-layer self K|V cache and the cached cross K|V (csrc/decode.cu),
-        picks the next token on the device and - without a `prefix_allowed_tokens_fn` - is replayed from a single CUDA
-        graph with no host synchronisation except an all-done poll every 8 steps.  use_cache=False runs the
-        first-generation path (the decoder prefix re-run every step), kept as the parity reference of the tests."""
-        if num_beams != 1 or num_return_sequences != 1:
-            raise AtlasB200Error("only greedy generation (num_beams=1) is implemented")
-        if not use_cache:
-            return self._generate_prefix_rerun(input_ids, attention_mask, max_length, min_length, prefix_allowed_tokens_fn)
+    def _prepare_decode(self, st, enc, attention_mask, W, dt):
+        """Per generation: the cross K|V projections, the cross-attention mask and its live 64-key tiles, the self-attention
+        bias table - all into the state's fixed buffers (a captured step graph reads them)."""
         c = self.config
-        enc = self.encode(input_ids, attention_mask)
-        B, Lk = enc.shape[0], enc.shape[1]
-        W, G, dt = self._weights()
-        st = self._decode_state(B, Lk, int(max_length), dt, enc.device)
+        B, Lk = st.B, st.Lk
         self.cross_kv(enc, out=st.cross_kv)
         neg = -1e4 if dt == torch.float16 else -1e9                                 # invert_attention_mask (4.18)
         st.cross_mask.copy_((1.0 - attention_mask.reshape(B, Lk).to(torch.float32)) * neg)
@@ -875,6 +924,34 @@ class FiD(nn.Module):
             if getattr(st, "wgen", None) != wkey[0]:                                # buffers re-allocated: re-capture
                 st.graph, st.wgen = None, wkey[0]
             st.wkey = wkey
+
+    @torch.no_grad()
+    def generate(self, input_ids=None, attention_mask=None, max_length=32, min_length=1, num_beams=1,
+                 num_return_sequences=1, length_penalty=1.0, forced_bos_token_id=None, prefix_allowed_tokens_fn=None,
+                 use_cache=True, **unused):
+        """Greedy decoding (what `Atlas.generate` requests with num_beams=1, src/atlas.py:592-619; transformers 4.18
+        `greedy_search` with `use_cache`): the encoder and the cross-attention K|V projections run once; every step
+        decodes ONE token per sequence against the per-layer self K|V cache and the cached cross K|V (csrc/decode.cu),
+        picks the next token on the device and - without a `prefix_allowed_tokens_fn` - is replayed from a single CUDA
+        graph with no host synchronisation except an all-done poll every 8 steps.  use_cache=False runs the
+        first-generation path (the decoder prefix re-run every step), kept as the parity reference of the tests.
+        num_beams > 1: beam search (`_generate_beams`).  min_length=None means no EOS ban (the config's min_length, 0)."""
+        if num_return_sequences != 1:
+            raise AtlasB200Error(f"num_return_sequences={num_return_sequences} is not implemented (only 1)")
+        if min_length is None:
+            min_length = getattr(self.config, "min_length", 0) or 0
+        if num_beams is not None and num_beams > 1:
+            return self._generate_beams(input_ids, attention_mask, max_length, min_length, int(num_beams),
+                                        1.0 if length_penalty is None else float(length_penalty), prefix_allowed_tokens_fn,
+                                        unused)
+        if not use_cache:
+            return self._generate_prefix_rerun(input_ids, attention_mask, max_length, min_length, prefix_allowed_tokens_fn)
+        c = self.config
+        enc = self.encode(input_ids, attention_mask)
+        B, Lk = enc.shape[0], enc.shape[1]
+        W, G, dt = self._weights()
+        st = self._decode_state(B, Lk, int(max_length), dt, enc.device)
+        self._prepare_decode(st, enc, attention_mask, W, dt)
         st.seq.fill_(c.pad_token_id)
         st.seq[:, 0] = c.decoder_start_token_id
         st.tok_in.fill_(c.decoder_start_token_id)
@@ -927,6 +1004,111 @@ class FiD(nn.Module):
             first = is_eos.float().argmax(dim=1) + 1
             seq = seq[:, : int(first.max()) + 1]
         return seq
+
+    @torch.no_grad()
+    def _generate_beams(self, input_ids, attention_mask, max_length, min_length, nb, length_penalty,
+                        prefix_allowed_tokens_fn, unused):
+        """Beam search: transformers 4.18 `beam_search` with `BeamSearchScorer` (early_stopping=False, one returned
+        sequence).  The encoder and the cross K|V projections run once on the B unexpanded rows; each step decodes the
+        B * nb beam rows with the KV-cached decoder (self-attention through the ancestry table, the nb beams of a batch
+        element sharing its cross K|V), then csrc/beam.cu selects the next beams and updates the hypotheses on the device.
+        Without a `prefix_allowed_tokens_fn` the step is replayed from one CUDA graph (all-done poll every 8 steps); with
+        one, the steps run eagerly and the function sees every row's sequence rebuilt through the ancestry.  `finalize`
+        runs on the host from one copy of the hypotheses and the running beams.  use_cache has no effect here."""
+        if nb > ops.MAX_BEAMS:
+            raise AtlasB200Error(f"num_beams={nb} exceeds the beam kernels' limit of {ops.MAX_BEAMS}")
+        for name in ("do_sample", "early_stopping"):
+            if unused.get(name):
+                raise AtlasB200Error(f"{name}=True is not implemented with beam search (only early_stopping=False, no sampling)")
+        if (unused.get("num_beam_groups") or 1) > 1 or unused.get("diversity_penalty"):
+            raise AtlasB200Error("diverse / grouped beam search is not implemented")
+        c = self.config
+        max_length, min_length = int(max_length), int(min_length)
+        V = c.vocab_size
+        if V < 2:
+            raise AtlasB200Error("beam search needs a vocabulary of at least 2 tokens")
+        enc = self.encode(input_ids, attention_mask)
+        B, Lk = enc.shape[0], enc.shape[1]
+        W, G, dt = self._weights()
+        st = self._decode_state(B, Lk, max_length, dt, enc.device, nb=nb)
+        self._prepare_decode(st, enc, attention_mask, W, dt)
+        # 4.18's log_softmax returns the logits' dtype: 16-bit parameters round the log-probs, fp32 ones keep them fp32
+        round_lp = self.shared.weight.dtype in (torch.float16, torch.bfloat16)
+        eos, pad = c.eos_token_id, c.pad_token_id
+        st.reset(c.decoder_start_token_id, pad)
+        n_steps = max_length - 1
+
+        def step(mask=None):
+            logits = self._decode_step_logits(st)
+            ops.beam_topk(logits, st.beam_scores, st.t_dev, 2 * nb, eos, min_length, round_lp, add_mask=mask,
+                          cand_score=st.cand_score, cand_tok=st.cand_tok)
+            ops.beam_select(st.cand_score, st.cand_tok, nb, V, *st.select_buffers(), eos, pad, length_penalty)
+
+        use_graph = self.cuda_graphs and prefix_allowed_tokens_fn is None and n_steps > 0
+        gkey = (min_length, length_penalty, round_lp)
+        if use_graph and (st.graph is None or getattr(st, "gkey", None) != gkey):
+            side = torch.cuda.Stream()
+            side.wait_stream(torch.cuda.current_stream())
+            with torch.cuda.stream(side):                    # eager warm-up step on scratch state (then reset below)
+                step()
+            torch.cuda.current_stream().wait_stream(side)
+            st.graph = torch.cuda.CUDAGraph()
+            with torch.cuda.graph(st.graph):
+                step()
+            st.gkey = gkey
+            st.reset(c.decoder_start_token_id, pad)
+        for s_i in range(n_steps):
+            if use_graph:
+                st.graph.replay()
+            elif prefix_allowed_tokens_fn is None:
+                step()
+            else:
+                seqs = st.sequences(s_i)                     # host synchronisation: the callback needs the sequences
+                allowed = torch.full((st.R, V), -float("inf"), dtype=torch.float32, device=enc.device)
+                for r in range(st.R):
+                    allowed[r, prefix_allowed_tokens_fn(r // nb, seqs[r])] = 0
+                step(allowed)
+            if (s_i % 8 == 7 or s_i == n_steps - 1) and bool(st.done.all()):      # the only host synchronisation
+                break
+        return self._finalize_beams(st, max_length, length_penalty)
+
+    def _finalize_beams(self, st, max_length, length_penalty):
+        """BeamSearchScorer.finalize (4.18) on the host: the running beams of unfinished batch elements join their
+        hypotheses, the best (the last of a stable sort by score: among equal scores the last inserted) is returned, padded
+        with pad only when the lengths differ and closed by EOS where it is shorter than max_length."""
+        c = self.config
+        B, nb = st.B, st.nb
+        t = int(st.t_dev)
+        run = st.sequences(t).cpu().tolist()
+        scores = st.beam_scores.cpu().tolist()
+        done = st.done.cpu().tolist()
+        h_score, h_len, h_ins = st.hyp_score.cpu().tolist(), st.hyp_len.cpu().tolist(), st.hyp_ins.cpu().tolist()
+        h_tok, h_state, h_worst = st.hyp_tok.cpu(), st.hyp_state.cpu().tolist(), st.hyp_worst.cpu().tolist()
+        best = []
+        for b in range(B):
+            slots = sorted(range(h_state[b][0]), key=lambda j: h_ins[b][j])            # list order = insertion order
+            beams = [(h_score[b][j], h_tok[b, j, : h_len[b][j]].tolist()) for j in slots]
+            worst = h_worst[b]
+            if not done[b]:
+                for k in range(nb):                           # BeamHypotheses.add of the running beam
+                    hyp = run[b * nb + k]
+                    score = scores[b * nb + k] / (len(hyp) ** length_penalty)
+                    if len(beams) < nb or score > worst:
+                        beams.append((score, hyp))
+                        if len(beams) > nb:
+                            order = sorted([(s, i) for i, (s, _) in enumerate(beams)])
+                            del beams[order[0][1]]
+                            worst = order[1][0]
+                        else:
+                            worst = min(score, worst)
+            best.append(sorted(beams, key=lambda x: x[0]).pop()[1])
+        lens = [len(h) for h in best]
+        out = torch.full((B, min(max(lens) + 1, max_length)), c.pad_token_id, dtype=torch.int64)
+        for b, h in enumerate(best):
+            out[b, : len(h)] = torch.tensor(h, dtype=torch.int64)
+            if len(h) < max_length:
+                out[b, len(h)] = c.eos_token_id
+        return out.to(st.tok.device)
 
     @torch.no_grad()
     def _generate_prefix_rerun(self, input_ids, attention_mask, max_length, min_length, prefix_allowed_tokens_fn):

@@ -838,3 +838,95 @@ def decode_argmax(logits, seq, tok_in, done, t_dev, eos_id, pad_id, min_length):
     check(lib().atlas_b200_decode_argmax(_ptr(logits), logits.stride(0), V, _ptr(seq), seq.stride(0), _ptr(tok_in),
                                          _ptr(done), _ptr(t_dev), int(eos_id), int(pad_id), int(min_length), B, _bf(logits),
                                          current_stream_ptr()))
+
+
+# ---------------------------------------------------------------------------------------------
+# beam search (csrc/beam.cu, the ancestry-gathered self-attention of csrc/decode.cu)
+# ---------------------------------------------------------------------------------------------
+MAX_BEAMS = 16      # ATLAS_B200_MAX_BEAMS
+
+
+def decode_self_attention_beam(qkv, cache, t_dev, anc, H, bias_delta=None, scale=1.0, out=None):
+    """decode_self_attention over R = B * nb beam rows whose history is gathered through anc int32 [2, R, Tmax] (buffer
+    t_dev[0] & 1): the new K | V lands in cache row (r, t), keys / values j come from (anc[r, j], j)."""
+    require_cuda(qkv, "qkv")
+    R, Tmax = cache.shape[0], cache.shape[1]
+    if anc.shape != (2, R, Tmax) or anc.dtype != torch.int32 or not anc.is_contiguous():
+        raise AtlasB200Error(f"decode_self_attention_beam: anc must be contiguous int32 [2, {R}, {Tmax}]")
+    if out is None:
+        out = torch.empty((R, H * 64), dtype=qkv.dtype, device=qkv.device)
+    bd = bias_delta.float().contiguous() if bias_delta is not None else None
+    check(lib().atlas_b200_decode_self_attention_beam(_ptr(qkv), qkv.stride(0), _ptr(cache), Tmax, _ptr(t_dev), _ptr(anc),
+                                                      _ptr(bd) if bd is not None else None, float(scale), _ptr(out),
+                                                      out.stride(0), R, H, _bf(qkv), current_stream_ptr()))
+    return out
+
+
+def decode_cross_attention_beams(q, kv, B, nb, H, Lk, add_mask, chunk, tile_live=None):
+    """The nb beams of a batch element (consecutive rows of q [B * nb, H*64]) against its ONE cross K | V kv [B * Lk, 2*H*64]:
+    the Lq = nb shape of the cross-attention stream kernel (live-tile skipping) + the split combine -> ctx [B * nb, H*64].
+    The K | V bytes read per step do not grow with nb."""
+    require_cuda(q, "q")
+    if chunk % 64 != 0:
+        raise AtlasB200Error(f"decode_cross_attention_beams: chunk {chunk} must be a multiple of 64")
+    chunks = (Lk + chunk - 1) // chunk
+    o_part = torch.empty((B * chunks * nb, H * 64), dtype=torch.float32, device=q.device)
+    ml = torch.empty((B * chunks * nb, H, 2), dtype=torch.float32, device=q.device)
+    am = add_mask.float().contiguous() if add_mask is not None else None
+    check(lib().atlas_b200_cross_attention_stream(_ptr(q), q.stride(0), 0, _ptr(kv), kv.stride(0), 0, H * 64,
+                                                  _ptr(am) if am is not None else None,
+                                                  _ptr(tile_live) if tile_live is not None else None, B, H, nb, Lk, chunk,
+                                                  1.0, _ptr(o_part), _ptr(ml), _bf(q), current_stream_ptr()))
+    out = torch.empty((B * nb, H * 64), dtype=q.dtype, device=q.device)
+    check(lib().atlas_b200_attention_combine_ex(_ptr(o_part), _ptr(ml), B, chunks, nb, H, _ptr(out), out.stride(0), None,
+                                                _bf(q), current_stream_ptr()))
+    return out
+
+
+def beam_topk(logits, beam_scores, t_dev, k, eos_id, min_length, round_lp, add_mask=None, cand_score=None, cand_tok=None,
+              lp_out=None):
+    """Per-row log-softmax + EOS ban + mask + beam score -> the row's top-k (cand_score fp32, cand_tok int32 [R, k])."""
+    require_cuda(logits, "logits")
+    R, V = logits.shape
+    if cand_score is None:
+        cand_score = torch.empty((R, k), dtype=torch.float32, device=logits.device)
+        cand_tok = torch.empty((R, k), dtype=torch.int32, device=logits.device)
+    if add_mask is not None and (add_mask.dtype != torch.float32 or add_mask.shape != (R, V) or add_mask.stride(1) != 1):
+        raise AtlasB200Error(f"beam_topk: add_mask must be fp32 [{R}, {V}] with unit inner stride")
+    if lp_out is not None and (lp_out.dtype != torch.float32 or lp_out.shape != (R, V) or not lp_out.is_contiguous()):
+        raise AtlasB200Error(f"beam_topk: lp_out must be contiguous fp32 [{R}, {V}]")
+    check(lib().atlas_b200_beam_topk(_ptr(logits), logits.stride(0), V,
+                                     _ptr(add_mask) if add_mask is not None else None,
+                                     add_mask.stride(0) if add_mask is not None else 0, _ptr(beam_scores), _ptr(t_dev),
+                                     int(eos_id), int(min_length), int(bool(round_lp)), int(k), _ptr(cand_score),
+                                     _ptr(cand_tok), _ptr(lp_out) if lp_out is not None else None, R, _bf(logits),
+                                     current_stream_ptr()))
+    return cand_score, cand_tok
+
+
+def beam_select(cand_score, cand_tok, nb, V, beam_scores, tok_in, parent, done, anc, tok, t_dev, hyp_score, hyp_len, hyp_ins,
+                hyp_tok, hyp_state, hyp_worst, eos_id, pad_id, length_penalty):
+    """Scorer step on the device over the candidates of beam_topk (k = 2 * nb), for B = done.numel() batch elements and
+    R = B * nb rows: beam_scores fp32 [R], tok_in int64 [R], parent int32 [R], done uint8 [B], anc int32 [2, R, Tmax],
+    tok int32 [R, Tmax], t_dev int32 [1], hyp_score fp64 [B, nb], hyp_len / hyp_ins int32 [B, nb], hyp_tok int32
+    [B, nb, Tmax], hyp_state int32 [B, 2], hyp_worst fp64 [B] (include/atlas_b200.h).  Advances t_dev."""
+    require_cuda(cand_score, "cand_score")
+    B = done.numel()
+    R, Tmax = tok.shape
+    want = {"cand_score": (cand_score, torch.float32, (R, 2 * nb)), "cand_tok": (cand_tok, torch.int32, (R, 2 * nb)),
+            "beam_scores": (beam_scores, torch.float32, (R,)), "tok_in": (tok_in, torch.int64, (R,)),
+            "parent": (parent, torch.int32, (R,)), "done": (done, torch.uint8, (B,)), "anc": (anc, torch.int32, (2, R, Tmax)),
+            "tok": (tok, torch.int32, (R, Tmax)), "t_dev": (t_dev, torch.int32, (1,)),
+            "hyp_score": (hyp_score, torch.float64, (B, nb)), "hyp_len": (hyp_len, torch.int32, (B, nb)),
+            "hyp_ins": (hyp_ins, torch.int32, (B, nb)), "hyp_tok": (hyp_tok, torch.int32, (B, nb, Tmax)),
+            "hyp_state": (hyp_state, torch.int32, (B, 2)), "hyp_worst": (hyp_worst, torch.float64, (B,))}
+    for name, (t, dtype, shape) in want.items():
+        if t.dtype != dtype or tuple(t.shape) != shape or not t.is_contiguous():
+            raise AtlasB200Error(f"beam_select: {name} must be contiguous {dtype} {list(shape)} (B={B}, nb={nb}), got "
+                                 f"{t.dtype} {list(t.shape)}")
+    if R != B * nb:
+        raise AtlasB200Error(f"beam_select: {R} rows for B={B} x nb={nb}")
+    check(lib().atlas_b200_beam_select(_ptr(cand_score), _ptr(cand_tok), B, nb, V, _ptr(beam_scores), _ptr(tok_in),
+                                       _ptr(parent), _ptr(done), _ptr(anc), _ptr(tok), Tmax, _ptr(t_dev), _ptr(hyp_score),
+                                       _ptr(hyp_len), _ptr(hyp_ins), _ptr(hyp_tok), _ptr(hyp_state), _ptr(hyp_worst),
+                                       int(eos_id), int(pad_id), float(length_penalty), current_stream_ptr()))

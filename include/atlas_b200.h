@@ -215,6 +215,43 @@ int atlas_b200_decode_argmax(const void* logits, int64_t ld, int32_t V, int64_t*
                              uint8_t* done, int32_t* t_dev, int32_t eos_id, int32_t pad_id, int32_t min_length, int32_t B,
                              int32_t is_bf16, void* stream);
 
+/* Beam-search decoding of FiD.generate(num_beams = nb > 1) (csrc/beam.cu; reference: transformers 4.18 `beam_search`,
+ * `BeamSearchScorer`, `BeamHypotheses` with early_stopping = False).  R = B * nb rows, row r = b * nb + beam; the step index
+ * t = *t_dev (cur_len = t + 1) lives in device memory so one captured CUDA graph serves every step.
+ * Ancestry table anc int32 [2, R, Tmax], buffer (t & 1) current at step t: entry (r, j) is the cache slot row holding row r's
+ * position j - its self K | V is cache[anc[r, j], j] and its token tok[anc[r, j], j] (tok int32 [R, Tmax]).  Beams are
+ * reordered by rewriting this table, never by copying the K | V cache.
+ *  decode_self_attention_beam  decode_self_attention over R rows with the history gathered through the ancestry: writes the new
+ *      K | V at cache row (r, t), reads keys / values (anc[r, j], j) for j <= t.  Same arithmetic as decode_self_attention on the
+ *      explicitly gathered cache (bit-identical).
+ *  beam_topk    per row: log-prob = log_softmax(logits) in fp32 (rounded to the logits' 16-bit type when round_lp != 0),
+ *      EOS -> -inf while t + 1 < min_length, + add_mask [R, ld_mask] fp32 (NULL = none; the prefix constraint, 0 / -inf),
+ *      + beam_scores[r] in fp32 -> the row's top k candidates, cand_score fp32 / cand_tok int32 [R, k] (k <= 32).  Order: the
+ *      larger score first, NaN above every number, among equal scores (or NaNs) the lower index; a token is always in [0, V)
+ *      for V >= k.  lp_out (fp32 [R, V], NULL = not written) receives the processed log-probs before the beam score.
+ *  beam_select  per batch element: merges its nb rows' candidates (k = 2 * nb, flat index beam * V + token, the same order)
+ *      into the top 2 * nb and applies BeamSearchScorer.process: an EOS candidate at rank < nb becomes a hypothesis of length
+ *      cur_len and score sum_logprob / cur_len ** length_penalty (fp64), one at rank >= nb is skipped, the others fill the nb
+ *      beams -> beam_scores, tok_in int64 [R], parent int32 [R] (global row), tok[r, t + 1], anc buffer ((t + 1) & 1).
+ *      Hypotheses (at most nb per batch element, list order = insertion number): hyp_score fp64 [B, nb], hyp_len, hyp_ins
+ *      int32 [B, nb], hyp_tok int32 [B, nb, Tmax], hyp_state int32 [B, 2] = (count, next insertion number), hyp_worst fp64 [B]
+ *      (initially 0, 0 and 1e9).  On overflow the lowest score goes (ties: the earliest inserted).  done[b] |= count == nb and
+ *      worst >= best / cur_len ** length_penalty.  A finished batch element emits pad_id with score 0 and keeps its rows in
+ *      place.  Then *t_dev += 1.  Requires 1 <= nb <= ATLAS_B200_MAX_BEAMS and V >= 2. */
+#define ATLAS_B200_MAX_BEAMS 16
+int atlas_b200_decode_self_attention_beam(const void* qkv, int64_t ldqkv, void* cache, int32_t Tmax, const int32_t* t_dev,
+                                          const int32_t* anc, const float* bias_delta, float scale, void* out, int64_t ldo,
+                                          int32_t R, int32_t H, int32_t is_bf16, void* stream);
+int atlas_b200_beam_topk(const void* logits, int64_t ld, int32_t V, const float* add_mask, int64_t ld_mask,
+                         const float* beam_scores, const int32_t* t_dev, int32_t eos_id, int32_t min_length, int32_t round_lp,
+                         int32_t k, float* cand_score, int32_t* cand_tok, float* lp_out, int32_t R, int32_t is_bf16,
+                         void* stream);
+int atlas_b200_beam_select(const float* cand_score, const int32_t* cand_tok, int32_t B, int32_t nb, int32_t V,
+                           float* beam_scores, int64_t* tok_in, int32_t* parent, uint8_t* done, int32_t* anc, int32_t* tok,
+                           int32_t Tmax, int32_t* t_dev, double* hyp_score, int32_t* hyp_len, int32_t* hyp_ins,
+                           int32_t* hyp_tok, int32_t* hyp_state, double* hyp_worst, int32_t eos_id, int32_t pad_id,
+                           double length_penalty, void* stream);
+
 /* Reader-input assembly from a device-resident passage token bank.  Replaces the per-step host work of
  * Atlas.tokenize_passages (src/atlas.py:261-280: bsz * n_context string formats + tokenizer calls, then H2D of
  * [bsz, n, L] int64 ids + mask):
