@@ -119,6 +119,8 @@ def lib():
     L.atlas_b200_gated_gelu.argtypes = [vp, i64, vp, i64, vp, i64, i64, i32, i32, vp]
     L.atlas_b200_gelu_erf.restype = c.c_int
     L.atlas_b200_gelu_erf.argtypes = [vp, i64, vp, i64, vp, i64, i64, i32, i32, vp]
+    L.atlas_b200_relu_bwd.restype = c.c_int
+    L.atlas_b200_relu_bwd.argtypes = [vp, i64, vp, i64, vp, i64, i64, i32, i32, vp]
     L.atlas_b200_bert_embed_sum.restype = c.c_int
     L.atlas_b200_bert_embed_sum.argtypes = [vp, vp, vp, vp, vp, vp, i32, i32, i32, i32, vp]
     L.atlas_b200_scatter_add_rows.restype = c.c_int
@@ -234,6 +236,7 @@ EXPORTED_SYMBOLS = [
     "atlas_b200_layernorm_bwd",
     "atlas_b200_gated_gelu",
     "atlas_b200_gelu_erf",
+    "atlas_b200_relu_bwd",
     "atlas_b200_bert_embed_sum",
     "atlas_b200_scatter_add_rows",
     "atlas_b200_masked_mean_pool_bwd",

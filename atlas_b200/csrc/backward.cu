@@ -7,6 +7,7 @@
 //   norm_bwd            BertLayerNorm (uncentred 2nd moment, modeling_bert.py:104-114) / T5 RMSNorm (modeling_t5.py:244-253)
 //   gated_gelu fwd/bwd  T5DenseGatedGeluDense (modeling_t5.py:281-285) on the interleaved (wi_0 | wi_1) projection
 //   gelu_erf fwd/bwd    BertIntermediate (modeling_bert.py:444)
+//   relu_bwd            T5DenseReluDense (modeling_t5.py:263-265, T5 v1.0) from the saved ReLU output
 //   bert_embed_sum      word + token_type + position (modeling_bert.py:236-243) without the LayerNorm (training keeps the sum)
 //   scatter_add_rows    embedding gradients (fp32 accumulation by row index)
 //   masked_mean_pool_bwd  Contriever pooling (src/retrievers.py:50-53)
@@ -283,6 +284,30 @@ gelu_erf_kernel(const uint16_t* __restrict__ z, int64_t ldz, const uint16_t* __r
     }
 }
 
+// dU = dG * [G > 0] from the saved forward output G = relu(U) (the ReLU's own output decides, as torch's
+// threshold_backward does): a pure select of 16-bit values, eight columns per thread
+template <bool kBF16>
+__global__ void __launch_bounds__(256)
+relu_bwd_kernel(const uint16_t* __restrict__ g, int64_t ldg, const uint16_t* __restrict__ dg, int64_t lddg,
+                uint16_t* __restrict__ du, int64_t lddu, int64_t M, int N) {
+    const int64_t vecs = M * (N / 8);
+    for (int64_t idx = blockIdx.x * 256ll + threadIdx.x; idx < vecs; idx += gridDim.x * 256ll) {
+        const int64_t m = idx / (N / 8);
+        const int c = static_cast<int>(idx % (N / 8)) * 8;
+        const uint4 gv = __ldg(reinterpret_cast<const uint4*>(g + m * ldg + c));
+        const uint4 dv = __ldg(reinterpret_cast<const uint4*>(dg + m * lddg + c));
+        const uint32_t gw[4] = {gv.x, gv.y, gv.z, gv.w}, dw[4] = {dv.x, dv.y, dv.z, dv.w};
+        uint32_t o[4];
+#pragma unroll
+        for (int q = 0; q < 4; ++q) {
+            const uint32_t lo = f32<kBF16>(gw[q]) > 0.f ? 0x0000FFFFu : 0u;
+            const uint32_t hi = f32<kBF16>(gw[q] >> 16) > 0.f ? 0xFFFF0000u : 0u;
+            o[q] = dw[q] & (lo | hi);
+        }
+        *reinterpret_cast<uint4*>(du + m * lddu + c) = make_uint4(o[0], o[1], o[2], o[3]);
+    }
+}
+
 // ---- embeddings -----------------------------------------------------------------------------------------------------
 // y[row] = r16(r16(word[id] + type[tt]) + pos[row % L])   (16-bit adds in the reference's order)
 template <bool kBF16>
@@ -519,6 +544,24 @@ int atlas_b200_gelu_erf(const void* z, int64_t ldz, const void* dy, int64_t lddy
     else
         bw::gelu_erf_kernel<false><<<grid, 256, 0, s>>>(static_cast<const uint16_t*>(z), ldz, static_cast<const uint16_t*>(dy),
                                                          lddy, static_cast<uint16_t*>(out), ldo, M, N);
+    abh::count_launch();
+    AB_CUDA_CHECK(cudaGetLastError());
+    return ATLAS_B200_OK;
+}
+
+int atlas_b200_relu_bwd(const void* g, int64_t ldg, const void* dg, int64_t lddg, void* du, int64_t lddu, int64_t M, int32_t N,
+                        int32_t is_bf16, void* stream) {
+    AB_REQUIRE(M >= 0 && N > 0 && N % 8 == 0 && ldg % 8 == 0 && lddg % 8 == 0 && lddu % 8 == 0,
+               "relu_bwd: N and the strides must be multiples of 8");
+    AB_REQUIRE(((reinterpret_cast<uintptr_t>(g) | reinterpret_cast<uintptr_t>(dg) | reinterpret_cast<uintptr_t>(du)) & 15u) == 0,
+               "relu_bwd: g, dg and du must be 16-byte aligned");
+    if (M == 0) return ATLAS_B200_OK;
+    cudaStream_t s = static_cast<cudaStream_t>(stream);
+    const int grid = bw::grid_for(M * (N / 8));
+    const uint16_t *gp = static_cast<const uint16_t*>(g), *dp = static_cast<const uint16_t*>(dg);
+    uint16_t* op = static_cast<uint16_t*>(du);
+    if (is_bf16) bw::relu_bwd_kernel<true><<<grid, 256, 0, s>>>(gp, ldg, dp, lddg, op, lddu, M, N);
+    else bw::relu_bwd_kernel<false><<<grid, 256, 0, s>>>(gp, ldg, dp, lddg, op, lddu, M, N);
     abh::count_launch();
     AB_CUDA_CHECK(cudaGetLastError());
     return ATLAS_B200_OK;

@@ -6,8 +6,8 @@
 // Replaces the cuBLAS GEMM + separate ATen elementwise kernels behind
 //   BertSelfAttention q/k/v, BertSelfOutput.dense, BertIntermediate.dense (+erf-GELU),
 //   BertOutput.dense                                     (src/modeling_bert.py:280-466)
-//   T5Attention q/k/v/o, T5DenseGatedGeluDense wi_0/wi_1 (+gelu_new gate)/wo, lm_head
-//                                                        (src/modeling_t5.py:272-289,418-531,1642-1647)
+//   T5Attention q/k/v/o, T5DenseGatedGeluDense wi_0/wi_1 (+gelu_new gate)/wo, T5DenseReluDense wi (+ReLU)/wo, lm_head
+//                                                        (src/modeling_t5.py:256-289,418-531,1642-1647)
 // Fused epilogues (a template parameter of the kernel, applied to the fp32 accumulator registers):
 //   EPI_NONE      C = acc
 //   EPI_BIAS      C = acc + bias[n]
@@ -15,6 +15,8 @@
 //   EPI_RESIDUAL  C = acc + bias[n] + R[m, n]                      (dense + residual, LN follows)
 //   EPI_GATED     C[m, j] = gelu_new(acc[m, 2j]) * acc[m, 2j+1]    (W rows interleaved wi_0/wi_1;
 //                                                                   modeling_t5.py:281-285, fp32 GELU)
+//   EPI_RELU      C = max(acc + bias[n], 0)                        (T5 v1.0 T5DenseReluDense, modeling_t5.py:263-265;
+//                                                                   with row_ss the row scale comes first: relu(s acc))
 //
 // Persistent, warp-specialised, one CTA per SM (grid = #SMs): warpgroup 0 is the TMA producer (one thread; setmaxnreg
 // gives its registers to the consumers), warpgroups 1 and 2 are consumers.  Two schedules:
@@ -47,7 +49,7 @@ constexpr int UMMA_K = 16;      // K of one wgmma
 constexpr int CONSUMERS = 2;    // consumer warpgroups
 constexpr int THREADS = 128 * (1 + CONSUMERS);
 
-enum Epilogue { EPI_NONE = 0, EPI_BIAS = 1, EPI_GELU = 2, EPI_RESIDUAL = 3, EPI_GATED = 4 };
+enum Epilogue { EPI_NONE = 0, EPI_BIAS = 1, EPI_GELU = 2, EPI_RESIDUAL = 3, EPI_GATED = 4, EPI_RELU = 5 };
 
 template <int BLOCK_N>
 struct Cfg {
@@ -144,6 +146,10 @@ __device__ __forceinline__ uint32_t epilogue_pair(const Params& p, float v0, flo
     } else if constexpr (kEpi == EPI_RESIDUAL) {
         v0 += to_f32<kBF16>(static_cast<uint16_t>(res & 0xFFFFu));
         v1 += to_f32<kBF16>(static_cast<uint16_t>(res >> 16));
+    } else if constexpr (kEpi == EPI_RELU) {
+        // written as a select so that NaN propagates like torch.relu (fmaxf would return 0)
+        v0 = v0 < 0.f ? 0.f : v0;
+        v1 = v1 < 0.f ? 0.f : v1;
     }
     return pack2<kBF16>(v0, v1);
 }
@@ -687,7 +693,7 @@ int atlas_b200_linear_ex(const void* A, int64_t lda, const void* W, int64_t ldw,
     if (M == 0) return ATLAS_B200_OK;
     AB_REQUIRE(N % 8 == 0 && K % 8 == 0 && lda % 8 == 0 && ldw % 8 == 0 && ldc % 8 == 0,
                "N, K and the leading dimensions must be multiples of 8 (16-byte rows)");
-    AB_REQUIRE(epilogue >= EPI_NONE && epilogue <= EPI_GATED, "unknown epilogue %d", epilogue);
+    AB_REQUIRE(epilogue >= EPI_NONE && epilogue <= EPI_RELU, "unknown epilogue %d", epilogue);
     AB_REQUIRE(epilogue != EPI_RESIDUAL || (residual != nullptr && ldr % 8 == 0), "EPI_RESIDUAL needs a residual");
     AB_REQUIRE(epilogue != EPI_GATED || N % 32 == 0, "EPI_GATED needs N %% 32 == 0");
     AB_REQUIRE((reinterpret_cast<uintptr_t>(C) & 15u) == 0, "C must be 16-byte aligned");
@@ -747,6 +753,7 @@ int atlas_b200_linear_ex(const void* A, int64_t lda, const void* W, int64_t ldw,
             case EPI_BIAS: return launch_pp_t<EPI_BIAS>(is_bf16 != 0, ta, tb, tc, tr, p, s);
             case EPI_GELU: return launch_pp_t<EPI_GELU>(is_bf16 != 0, ta, tb, tc, tr, p, s);
             case EPI_RESIDUAL: return launch_pp_t<EPI_RESIDUAL>(is_bf16 != 0, ta, tb, tc, tr, p, s);
+            case EPI_RELU: return launch_pp_t<EPI_RELU>(is_bf16 != 0, ta, tb, tc, tr, p, s);
             default: return launch_pp_t<EPI_GATED>(is_bf16 != 0, ta, tb, tc, tr, p, s);
         }
     }
@@ -755,6 +762,7 @@ int atlas_b200_linear_ex(const void* A, int64_t lda, const void* W, int64_t ldw,
         case EPI_BIAS: return launch_n<EPI_BIAS>(is_bf16 != 0, wide, ta, tb, p, s);
         case EPI_GELU: return launch_n<EPI_GELU>(is_bf16 != 0, wide, ta, tb, p, s);
         case EPI_RESIDUAL: return launch_n<EPI_RESIDUAL>(is_bf16 != 0, wide, ta, tb, p, s);
+        case EPI_RELU: return launch_n<EPI_RELU>(is_bf16 != 0, wide, ta, tb, p, s);
         default: return launch_n<EPI_GATED>(is_bf16 != 0, wide, ta, tb, p, s);
     }
 }

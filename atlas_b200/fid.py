@@ -1,4 +1,4 @@
-"""Drop-in for `src.fid.FiD` (reference src/fid.py:28-357 over the vendored T5 v1.1, src/modeling_t5.py):
+"""Drop-in for `src.fid.FiD` (reference src/fid.py:28-357 over the vendored T5, src/modeling_t5.py; v1.1 and v1.0):
 Fusion-in-Decoder on B200 kernels: the no-grad forward (evaluation / scoring / greedy generation, replayed from a
 CUDA graph), the with-grad forward + hand-written backward kernels of the training step (`_forward_train`, grad_ops.py),
 and the cross-attention score capture used for retriever distillation (src/fid.py:126-235,333-343).
@@ -8,10 +8,12 @@ labels, encoder_outputs=None, use_cache=False)` -> output indexable as `out[0]` 
 `.logits`, `.loss`, `.encoder_last_hidden_state`; `encoder.config.{n_context,bsz}` are read like the reference's
 `FiDStack` (src/fid.py:47-49,66-76); `_shift_right`; `generate` (greedy); parameter names identical to HF T5
 (`shared`, `encoder.block.N.layer.0.SelfAttention.{q,k,v,o}`, `relative_attention_bias` on block 0,
-`layer.1.EncDecAttention`, `DenseReluDense.{wi_0,wi_1,wo}`, `lm_head`) so reference checkpoints load.
+`layer.1.EncDecAttention`, `DenseReluDense.{wi_0,wi_1,wo}` (v1.1) or `DenseReluDense.{wi,wo}` (v1.0), `lm_head`) so
+reference checkpoints load.  T5 v1.0 (t5-small / -base / -large: `feed_forward_proj="relu"`, LM head tied to `shared` and
+applied to the final hidden state scaled by d_model^-0.5) runs the same kernels with the ReLU fused into the wi GEMM.
 
 What runs where (all in csrc/): RMSNorm (T5LayerNorm, modeling_t5.py:244-253); q/k/v/o and FF projections on the
-wgmma GEMM with fused residual and gated-GELU epilogues (modeling_t5.py:281-289); encoder self-attention as
+wgmma GEMM with fused residual, gated-GELU and ReLU epilogues (modeling_t5.py:256-289); encoder self-attention as
 B*n independent L-token segments with the relative-position bias added on the fly from a [H, 2L-1] table
 (modeling_t5.py:352-416,478-524) - the [B*n, H, L, L] bias / probability tensors are never materialised;
 decoder cross-attention over the n*L concatenated keys as split-KV + combine (fid.py:298-349).
@@ -75,10 +77,15 @@ class _CrossAttnLayer(nn.Module):
 
 
 class _FF(nn.Module):
+    """T5DenseGatedGeluDense (wi_0, wi_1, wo) or, for feed_forward_proj="relu", T5DenseReluDense (wi, wo)."""
+
     def __init__(self, c):
         super().__init__()
-        self.wi_0 = nn.Linear(c.d_model, c.d_ff, bias=False)
-        self.wi_1 = nn.Linear(c.d_model, c.d_ff, bias=False)
+        if c.feed_forward_proj == "relu":
+            self.wi = nn.Linear(c.d_model, c.d_ff, bias=False)
+        else:
+            self.wi_0 = nn.Linear(c.d_model, c.d_ff, bias=False)
+            self.wi_1 = nn.Linear(c.d_model, c.d_ff, bias=False)
         self.wo = nn.Linear(c.d_ff, c.d_model, bias=False)
 
 
@@ -175,15 +182,21 @@ class FiD(nn.Module):
         super().__init__()
         config = config or T5ConfigLite()
         if config.d_kv != 64:
-            raise AtlasB200Error("atlas_b200 attention kernels need d_kv = 64 (all T5 v1.1 sizes)")
-        if getattr(config, "feed_forward_proj", "gated-gelu") != "gated-gelu":
-            raise AtlasB200Error("only T5 v1.1 (gated-gelu) is implemented")
+            raise AtlasB200Error(f"head dimension d_kv = {config.d_kv} is not implemented: the attention kernels need d_kv = 64 "
+                                 "(t5-small / -base / -large and every T5 v1.1 size; t5-3b and t5-11b have d_kv = 128)")
+        if not hasattr(config, "feed_forward_proj"):
+            config.feed_forward_proj = "gated-gelu"
+        if config.feed_forward_proj not in ("gated-gelu", "relu"):
+            raise AtlasB200Error(f"feed_forward_proj={config.feed_forward_proj!r} is not implemented (gated-gelu: T5 v1.1, "
+                                 "relu: T5 v1.0)")
         self.config = config
         self.model_dim = config.d_model
         self.shared = nn.Embedding(config.vocab_size, config.d_model)
         self.encoder = FiDStack(config, self.shared, is_decoder=False)
         self.decoder = FiDStack(config, self.shared, is_decoder=True)
         self.lm_head = nn.Linear(config.d_model, config.vocab_size, bias=False)
+        if getattr(config, "tie_word_embeddings", False):
+            self.lm_head.weight = self.shared.weight            # T5 v1.0: one table for the embedding and the LM head
         self.encoder.config.n_context = 1
         self.encoder.config.bsz = 1
         self._half = HalfCache()
@@ -195,10 +208,18 @@ class FiD(nn.Module):
 
     @classmethod
     def from_pretrained(cls, path, **kw):
-        """Local HF-layout directory (config.json + weights) of a T5 v1.1 checkpoint, src/model_io.py:77."""
+        """Local HF-layout directory (config.json + weights) of a T5 checkpoint, src/model_io.py:77.  A config.json without
+        `feed_forward_proj` (the original t5-small / -base / -large) is read as T5 v1.0 when the weights hold
+        `DenseReluDense.wi` instead of `wi_0` / `wi_1`: ReLU feed-forward and, unless stated, a tied LM head
+        (transformers' defaults for those fields)."""
         from ._pretrained import load_pretrained
 
-        return load_pretrained(cls, T5ConfigLite, path, **kw)
+        def infer(raw, sd):
+            if "feed_forward_proj" in raw or not any(k.endswith("DenseReluDense.wi.weight") for k in sd):
+                return {}
+            return {"feed_forward_proj": "relu", "tie_word_embeddings": raw.get("tie_word_embeddings", True)}
+
+        return load_pretrained(cls, T5ConfigLite, path, infer_config=infer, **kw)
 
     # ---- reference surface that is configuration only -------------------------------------
     def set_checkpoint(self, use_checkpoint):
@@ -319,6 +340,12 @@ class FiD(nn.Module):
         return W, self._half.derived(dt, self._fuse), dt
 
     @staticmethod
+    def _head(W):
+        """The LM-head matrix: `lm_head.weight`, or `shared.weight` when the two are tied (named_parameters() lists a tied
+        parameter once, under its first name)."""
+        return W["lm_head.weight"] if "lm_head.weight" in W else W["shared.weight"]
+
+    @staticmethod
     def _fuse(W):
         """Weights derived once per parameter version: interleaved wi_0/wi_1, fused q|k|v and cross k|v."""
         g = {}
@@ -342,16 +369,29 @@ class FiD(nn.Module):
             else:
                 continue
             g[name + "_n"] = (g[name].float() * ln.float()[None, :]).to(g[name].dtype).contiguous()
-        for name in list(W):        # decoder cross-attention query projection behind layer.1's norm
+        for name in list(W):        # decoder cross-attention query projection behind layer.1's norm; T5 v1.0's wi
             if name.endswith("EncDecAttention.q.weight"):
                 ln = W[name.replace("EncDecAttention.q.weight", "layer_norm.weight")]
                 g[name + "_n"] = (W[name].float() * ln.float()[None, :]).to(W[name].dtype).contiguous()
+            elif name.endswith("DenseReluDense.wi.weight"):
+                ln = W[name.replace("DenseReluDense.wi.weight", "layer_norm.weight")]
+                g[name.replace("wi.weight", "wi_n")] = (W[name].float() * ln.float()[None, :]).to(W[name].dtype).contiguous()
         return g
 
     # ---- encoder ---------------------------------------------------------------------------
+    def _ff_in(self, W, G, prefix, x, rows=None, row_ss=None, eps=1e-6):
+        """The feed-forward's input GEMM with its activation in the epilogue: ReLU on wi (T5 v1.0) or the gated GELU on the
+        interleaved wi_0 | wi_1 (v1.1).  row_ss: x is the UN-normalised hidden state and the norm is fused (see encode)."""
+        p = prefix + "DenseReluDense."
+        if self.config.feed_forward_proj == "relu":
+            w, epi = (G[p + "wi_n"] if row_ss is not None else W[p + "wi.weight"]), ops.EPI_RELU
+        else:
+            w, epi = (G[p + "wi_01_n"] if row_ss is not None else G[p + "wi_01"]), ops.EPI_GATED
+        return ops.linear(x, w, epilogue=epi, row_ss=row_ss, rs_eps=eps, rows=rows)
+
     def _ff(self, W, G, prefix, h, eps, rows=None):
         n = ops.layernorm(h, W[prefix + "layer_norm.weight"], None, eps, kind=1)
-        g = ops.linear(n, G[prefix + "DenseReluDense.wi_01"], epilogue=ops.EPI_GATED, rows=rows)
+        g = self._ff_in(W, G, prefix, n, rows=rows)
         # + the fp16 overflow clamp the reference applies after every sub-layer (src/modeling_t5.py:657-708; no-op in bf16)
         return ops.clamp_inf_(ops.linear(g, W[prefix + "DenseReluDense.wo.weight"], None, residual=h,
                                          epilogue=ops.EPI_RESIDUAL, rows=rows))
@@ -421,8 +461,7 @@ class FiD(nn.Module):
                                out_ss=ss[2 * i], rows=rows)
                 ops.clamp_inf_(h, row_ss=ss[2 * i])
                 p = f"encoder.block.{i}.layer.1."
-                g = ops.linear(h, G[p + "DenseReluDense.wi_01_n"], epilogue=ops.EPI_GATED, row_ss=ss[2 * i], rs_eps=eps,
-                               rows=rows)
+                g = self._ff_in(W, G, p, h, rows=rows, row_ss=ss[2 * i], eps=eps)
                 h = ops.linear(g, W[p + "DenseReluDense.wo.weight"], None, residual=h, epilogue=ops.EPI_RESIDUAL,
                                out_ss=ss[2 * i + 1], rows=rows)
                 ops.clamp_inf_(h, row_ss=ss[2 * i + 1])
@@ -531,14 +570,14 @@ class FiD(nn.Module):
                                out_ss=ss[3 * i + 1])
                 ops.clamp_inf_(h, row_ss=ss[3 * i + 1])
                 p = f"decoder.block.{i}.layer.2."
-                g = ops.linear(h, G[p + "DenseReluDense.wi_01_n"], epilogue=ops.EPI_GATED, row_ss=ss[3 * i + 1], rs_eps=eps)
+                g = self._ff_in(W, G, p, h, row_ss=ss[3 * i + 1], eps=eps)
                 h = ops.linear(g, W[p + "DenseReluDense.wo.weight"], None, residual=h, epilogue=ops.EPI_RESIDUAL,
                                out_ss=ss[3 * i + 2])
                 ops.clamp_inf_(h, row_ss=ss[3 * i + 2])
             h = ops.layernorm(h, W["decoder.final_layer_norm.weight"], None, eps, kind=1)
             if getattr(c, "tie_word_embeddings", False):
                 h = (h.float() * (d ** -0.5)).to(dt)                              # src/modeling_t5.py:1642-1645
-            return ops.linear(h, W["lm_head.weight"]).view(B, T, -1)
+            return ops.linear(h, self._head(W)).view(B, T, -1)
         for i in range(c.num_decoder_layers):
             p = f"decoder.block.{i}.layer.0."
             n = ops.layernorm(h, W[p + "layer_norm.weight"], None, c.layer_norm_epsilon, kind=1)
@@ -561,7 +600,7 @@ class FiD(nn.Module):
         h = ops.layernorm(h, W["decoder.final_layer_norm.weight"], None, c.layer_norm_epsilon, kind=1)
         if getattr(c, "tie_word_embeddings", False):
             h = (h.float() * (d ** -0.5)).to(dt)                                  # src/modeling_t5.py:1642-1645
-        logits = ops.linear(h, W["lm_head.weight"])
+        logits = ops.linear(h, self._head(W))
         return logits.view(B, T, -1)
 
     # ---- training path (autograd through the kernels, grad_ops.py) ---------------------------------------
@@ -584,6 +623,21 @@ class FiD(nn.Module):
 
     def _check_trainable(self):
         return None
+
+    def _embed_train(self, W, dt, ids):
+        """The token embedding with autograd.  Tied (T5 v1.0): gathered from the parameter itself (cast to `dt` per row), so
+        its fp32 scatter-add gradient reaches an fp32 `shared.weight` without a 16-bit rounding and is summed there with
+        the LM head's weight gradient in fp32."""
+        if "lm_head.weight" in W:
+            return grad_ops.embedding(W["shared.weight"], ids)
+        return grad_ops.embedding(self.shared.weight, ids, out_dtype=dt)
+
+    def _ff_train(self, W, G, prefix, n):
+        """wi -> activation of the feed-forward with autograd (the dropout and wo follow in the caller)."""
+        p = prefix + "DenseReluDense."
+        if self.config.feed_forward_proj == "relu":
+            return grad_ops.linear_relu(n, W[p + "wi.weight"])
+        return grad_ops.gated_gelu(grad_ops.linear(n, G[p + "wi_01"]))
 
     def _dropout_p(self):
         """config.dropout_rate in training mode (nn.Dropout / F.dropout of src/modeling_t5.py:266,286,310,515,561,597,
@@ -609,7 +663,7 @@ class FiD(nn.Module):
         d, H = c.d_model, c.num_heads
         eps = c.layer_norm_epsilon
         pdrop = self._dropout_p()
-        h = g.dropout(g.embedding(W["shared.weight"], ids), pdrop)
+        h = g.dropout(self._embed_train(W, dt, ids), pdrop)
         add_mask = (1.0 - mask.to(torch.float32)) * -10000.0
         add_mask._atlas_block_live = ops.key_block_live(add_mask)     # read by grad_ops._SelfAttention (all layers share it)
 
@@ -631,8 +685,7 @@ class FiD(nn.Module):
             h = lin_res(ctx, W[p + "SelfAttention.o.weight"], h)
             p = f"encoder.block.{i}.layer.1."
             n = g.layernorm(h, W[p + "layer_norm.weight"], None, eps, kind=1)
-            u = g.linear(n, G[p + "DenseReluDense.wi_01"])
-            return lin_res(g.dropout(g.gated_gelu(u), pdrop), W[p + "DenseReluDense.wo.weight"], h)
+            return lin_res(g.dropout(self._ff_train(W, G, p, n), pdrop), W[p + "DenseReluDense.wo.weight"], h)
 
         for i in range(c.num_layers):
             h = self._maybe_ckpt(block, i, h, bias)
@@ -661,7 +714,7 @@ class FiD(nn.Module):
         if pdrop and split % 32 != 0 and split != Lk:
             raise AtlasB200Error(f"dropout on the cross-attention probabilities needs a key split that is a multiple of 32 "
                                  f"(n_context*text_maxlength = {Lk} gave {split})")
-        h = g.dropout(g.embedding(W["shared.weight"], decoder_input_ids), pdrop)
+        h = g.dropout(self._embed_train(W, dt, decoder_input_ids), pdrop)
 
         def lin_res(x, w, res):
             if pdrop:
@@ -690,15 +743,14 @@ class FiD(nn.Module):
             h = lin_res(ctx, W[p + "EncDecAttention.o.weight"], h)
             p = f"decoder.block.{i}.layer.2."
             n = g.layernorm(h, W[p + "layer_norm.weight"], None, eps, kind=1)
-            u = g.linear(n, G[p + "DenseReluDense.wi_01"])
-            return lin_res(g.dropout(g.gated_gelu(u), pdrop), W[p + "DenseReluDense.wo.weight"], h)
+            return lin_res(g.dropout(self._ff_train(W, G, p, n), pdrop), W[p + "DenseReluDense.wo.weight"], h)
 
         for i in range(c.num_decoder_layers):
             h = self._maybe_ckpt(block, i, h, bias, flat)
         h = g.dropout(g.layernorm(h, W["decoder.final_layer_norm.weight"], None, eps, kind=1), pdrop)
         if getattr(c, "tie_word_embeddings", False):
-            raise AtlasB200Error("tied LM head (T5 v1.0) is not supported on the training path (T5 v1.1 is untied)")
-        logits = g.linear(h, W["lm_head.weight"])
+            h = h * (d ** -0.5)                                      # src/modeling_t5.py:1642-1645
+        logits = g.linear(h, self._head(W))
         return logits.view(B, T, -1)
 
     def _forward_train(self, input_ids, attention_mask, decoder_input_ids, labels, encoder_outputs):
@@ -829,7 +881,7 @@ class FiD(nn.Module):
         h = ops.layernorm(h, W["decoder.final_layer_norm.weight"], None, eps, kind=1)
         if getattr(c, "tie_word_embeddings", False):
             h = (h.float() * (c.d_model ** -0.5)).to(dt)
-        return ops.linear(h, W["lm_head.weight"])
+        return ops.linear(h, self._head(W))
 
     class _BeamState:
         """Static buffers of one (batch, beams, keys, max_length, dtype) beam-search shape (csrc/beam.cu): the per-layer

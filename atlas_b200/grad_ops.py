@@ -10,6 +10,7 @@ What autograd would derive through the reference's modules is implemented by han
   Attention        fused attention, saved O only     src/modeling_bert.py:328-366, src/modeling_t5.py:478-524
   CrossAttention   FiD decoder over n*L keys         src/fid.py:298-349
   GatedGelu / Gelu T5DenseGatedGeluDense / BERT FF   src/modeling_t5.py:281-285, src/modeling_bert.py:444
+  Relu, LinearRelu T5DenseReluDense (T5 v1.0)        src/modeling_t5.py:256-270; the mask comes from the saved output
   Embedding, BertEmbedSum, MaskedMeanPool, CrossEntropy
 Weights arrive as 16-bit tensors that require grad (the caller derives them from the fp32 / bf16 parameters with
 differentiable casts / concatenations, so autograd routes dW back to the reference-named parameters).
@@ -208,6 +209,51 @@ def gated_gelu(u):
     return _GatedGelu.apply(u)
 
 
+class _Relu(torch.autograd.Function):
+    """Saves the OUTPUT: the reference applies dropout after the ReLU (wi -> relu -> dropout -> wo), so the mask of the
+    backward is the pre-dropout activation's.  The forward is the same select kernel with u as its own mask (u > 0 ? u :
+    0); the feed-forward of the model uses `linear_relu`, which needs no separate pass."""
+
+    @staticmethod
+    def forward(ctx, u):
+        g = ops.relu_bwd(u, u)
+        ctx.save_for_backward(g)
+        return g
+
+    @staticmethod
+    def backward(ctx, dg):
+        (g,) = ctx.saved_tensors
+        return ops.relu_bwd(g, dg)
+
+
+def relu(u):
+    return _Relu.apply(u)
+
+
+class _LinearRelu(torch.autograd.Function):
+    """g = relu(x @ weight.T) with the ReLU in the GEMM epilogue (EPI_RELU): no pre-activation tensor is written; the
+    backward masks dG with the saved output, then runs the Linear's dgrad / wgrad on the masked gradient."""
+
+    @staticmethod
+    def forward(ctx, x, weight):
+        g = ops.linear(x, weight, epilogue=ops.EPI_RELU)
+        ctx.save_for_backward(x, weight, g)
+        return g
+
+    @staticmethod
+    def backward(ctx, dg):
+        x, weight, g = ctx.saved_tensors
+        du = ops.relu_bwd(g, dg).reshape(-1, g.shape[-1])
+        dx = ops.linear_dgrad(du, weight).reshape(x.shape) if _need(ctx, 0) else None
+        dw = ops.linear_wgrad(du, x.reshape(-1, x.shape[-1])) if _need(ctx, 1) else None
+        return dx, dw
+
+
+def linear_relu(x, weight):
+    """relu(x @ weight.T), differentiable in x and weight (T5DenseReluDense's wi, src/modeling_t5.py:263-264)."""
+    return _LinearRelu.apply(x, weight)
+
+
 class _GeluErf(torch.autograd.Function):
     @staticmethod
     def forward(ctx, z):
@@ -225,24 +271,26 @@ def gelu_erf(z):
 
 
 class _Embedding(torch.autograd.Function):
-    """rows = table[ids]; backward = fp32 scatter-add of the row gradients (csrc/backward.cu), `padding_idx` rows dropped."""
+    """rows = table[ids] (cast to out_dtype); backward = fp32 scatter-add of the row gradients (csrc/backward.cu),
+    `padding_idx` rows dropped, returned in the table's dtype."""
 
     @staticmethod
-    def forward(ctx, table, ids, padding_idx):
+    def forward(ctx, table, ids, padding_idx, out_dtype):
         ctx.save_for_backward(ids)
         ctx.shape, ctx.dtype, ctx.padding_idx = table.shape, table.dtype, padding_idx
-        return table[ids.reshape(-1)]
+        rows = table[ids.reshape(-1)]
+        return rows if out_dtype is None else rows.to(out_dtype)
 
     @staticmethod
     def backward(ctx, dy):
         (ids,) = ctx.saved_tensors
         dt = ops.scatter_add_rows(dy.contiguous(), ctx.shape[0], index=ids, skip_index=ctx.padding_idx)
-        return dt.to(ctx.dtype), None, None
+        return dt.to(ctx.dtype), None, None, None
 
 
-def embedding(table, ids, padding_idx=-1):
-    """[n, H] rows of a 16-bit table (the gather itself is a torch index: plumbing)."""
-    return _Embedding.apply(table, ids, padding_idx)
+def embedding(table, ids, padding_idx=-1, out_dtype=None):
+    """[n, H] rows of a 16-bit table, or of an fp32 one cast to out_dtype (the gather itself is a torch index: plumbing)."""
+    return _Embedding.apply(table, ids, padding_idx, out_dtype)
 
 
 class _BertEmbedSum(torch.autograd.Function):

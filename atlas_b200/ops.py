@@ -242,13 +242,13 @@ def pq_topk(codes, list_ids, codebooks, coarse, queries, k, id_base=0, id_stride
 # ---------------------------------------------------------------------------------------------
 # dense layers (csrc/gemm.cu)
 # ---------------------------------------------------------------------------------------------
-EPI_NONE, EPI_BIAS, EPI_GELU, EPI_RESIDUAL, EPI_GATED = 0, 1, 2, 3, 4
+EPI_NONE, EPI_BIAS, EPI_GELU, EPI_RESIDUAL, EPI_GATED, EPI_RELU = 0, 1, 2, 3, 4, 5
 
 
 def linear(x, weight, bias=None, residual=None, epilogue=None, out=None, row_ss=None, out_ss=None, rs_eps=1e-6, rows=None):
     """y = epilogue(x @ weight.T) on wgmma.  x [..., K], weight [N, K] (nn.Linear layout), 16-bit.
 
-    epilogue: EPI_NONE / EPI_BIAS / EPI_GELU / EPI_RESIDUAL / EPI_GATED (see include/atlas_b200.h);
+    epilogue: EPI_NONE / EPI_BIAS / EPI_GELU / EPI_RESIDUAL / EPI_GATED / EPI_RELU (see include/atlas_b200.h);
     default: EPI_RESIDUAL if `residual` is given, else EPI_BIAS if `bias` is given, else EPI_NONE.
     Fused T5 RMSNorm (atlas_b200_linear_ex): `row_ss` fp32 [M] = sum of squares of the rows of x -> accumulator rows are
     scaled by rsqrt(row_ss / K + rs_eps) (x is the UN-normalised hidden state, the norm weight is folded into `weight`);
@@ -624,6 +624,18 @@ def gated_gelu(u, dg=None):
     check(lib().atlas_b200_gated_gelu(_ptr(u2), u2.stride(0), _ptr(d2), d2.stride(0), _ptr(out), out.stride(0), M, F,
                                       _bf(u), current_stream_ptr()))
     return out.reshape(u.shape)
+
+
+def relu_bwd(g, dg):
+    """du = dg * [g > 0] from the ReLU's saved output g (T5 v1.0 feed-forward, linear(..., epilogue=EPI_RELU))."""
+    require_cuda(g, "g")
+    if g.shape != dg.shape or g.dtype != dg.dtype or g.dtype not in (torch.float16, torch.bfloat16):
+        raise AtlasB200Error(f"relu_bwd: g {tuple(g.shape)} {g.dtype} and dg {tuple(dg.shape)} {dg.dtype} must match, 16-bit")
+    g2, d2 = _rows2d(g).contiguous(), _rows2d(dg).contiguous()
+    out = torch.empty_like(g2)
+    check(lib().atlas_b200_relu_bwd(_ptr(g2), g2.stride(0), _ptr(d2), d2.stride(0), _ptr(out), out.stride(0), g2.shape[0],
+                                    g2.shape[1], _bf(g), current_stream_ptr()))
+    return out.reshape(g.shape)
 
 
 def gelu_erf(z, dy=None):

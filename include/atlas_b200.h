@@ -149,8 +149,10 @@ int atlas_b200_pq_topk_exhaustive(const uint8_t* codes, const void* list_ids, in
  *             | 3 +bias +residual[M, ldr] (dense + residual before LayerNorm)
  *             | 4 gated: C[m, j] = gelu_new(acc[m, 2j]) * acc[m, 2j+1], C has N/2 columns; W rows are
  *               wi_0 / wi_1 interleaved (modeling_t5.py:281-285; GELU evaluated in fp32 as at :283)
+ *             | 5 relu: C = max(acc +bias, 0) (T5 v1.0 T5DenseReluDense wi, modeling_t5.py:256-270; with
+ *               atlas_b200_linear_ex's row_ss the row scale is applied first, then the bias and the ReLU)
  * lda / ldw / ldc / ldr are row strides in elements (multiples of 8); N and K multiples of 8.
- * bias may be NULL (no bias added) for epilogues 1-3. */
+ * bias may be NULL (no bias added) for epilogues 1-3 and 5. */
 int atlas_b200_linear(const void* A, int64_t lda, const void* W, int64_t ldw, const void* bias,
                       const void* residual, int64_t ldr, void* C, int64_t ldc,
                       int32_t M, int32_t N, int32_t K, int32_t epilogue, int32_t is_bf16, void* stream);
@@ -370,6 +372,11 @@ int atlas_b200_gated_gelu(const void* u, int64_t ldu, const void* dg, int64_t ld
 /* erf GELU (src/modeling_bert.py:444) on z [M, N]: dy == NULL: out = gelu(z); else out = dy * gelu'(z). */
 int atlas_b200_gelu_erf(const void* z, int64_t ldz, const void* dy, int64_t lddy, void* out, int64_t ldo, int64_t M,
                         int32_t N, int32_t is_bf16, void* stream);
+
+/* Backward of the T5 v1.0 ReLU (src/modeling_t5.py:264) from its saved OUTPUT g [M, N] (what linear's epilogue 5 wrote):
+ * du = g > 0 ? dg : 0, a pure select (bit-exact).  N and the strides multiples of 8, pointers 16-byte aligned. */
+int atlas_b200_relu_bwd(const void* g, int64_t ldg, const void* dg, int64_t lddg, void* du, int64_t lddu, int64_t M, int32_t N,
+                        int32_t is_bf16, void* stream);
 
 /* word + token_type + position embeddings WITHOUT the LayerNorm (src/modeling_bert.py:236-243): the training forward
  * keeps the sum for the LayerNorm backward. */
