@@ -189,6 +189,14 @@ def lib():
     L.atlas_b200_attention_packed.argtypes = [vp, i64, i32, i32, i32, vp, i64, vp, vp, vp, vp, i32, i32, i32, f32, i32, vp]
     L.atlas_b200_expand_packed_tiles.restype = c.c_int
     L.atlas_b200_expand_packed_tiles.argtypes = [vp, i64, vp, i32, vp, i64, i32, vp]
+    L.atlas_b200_quantize_kv_e4m3.restype = c.c_int
+    L.atlas_b200_quantize_kv_e4m3.argtypes = [vp, i64, i64, i32, vp, i64, vp, i64, i32, vp]
+    L.atlas_b200_decode_cross_attention_e4m3.restype = c.c_int
+    L.atlas_b200_decode_cross_attention_e4m3.argtypes = [vp, i64, vp, i64, vp, i64, i32, i32, vp, vp, i32, i32, i32, i32, f32, vp,
+                                                         vp, i32, vp]
+    L.atlas_b200_cross_attention_stream_e4m3.restype = c.c_int
+    L.atlas_b200_cross_attention_stream_e4m3.argtypes = [vp, i64, i32, vp, i64, vp, i64, i32, i32, vp, vp, i32, i32, i32, i32, i32,
+                                                         f32, vp, vp, i32, vp]
     L.atlas_b200_pq_workspace_bytes.restype = c.c_size_t
     L.atlas_b200_pq_workspace_bytes.argtypes = [i32, i64, i32, i32, i32]
     L.atlas_b200_pq_train.restype = c.c_int
@@ -272,6 +280,9 @@ EXPORTED_SYMBOLS = [
     "atlas_b200_pq_encode",
     "atlas_b200_pq_topk",
     "atlas_b200_pq_topk_exhaustive",
+    "atlas_b200_quantize_kv_e4m3",
+    "atlas_b200_decode_cross_attention_e4m3",
+    "atlas_b200_cross_attention_stream_e4m3",
 ]
 
 

@@ -546,7 +546,8 @@ class Atlas(nn.Module):
                                     min_length=self.opt.generation_min_length,
                                     num_beams=self.opt.generation_num_beams,
                                     length_penalty=self.opt.generation_length_penalty, forced_bos_token_id=None,
-                                    prefix_allowed_tokens_fn=allowed_fn)
+                                    prefix_allowed_tokens_fn=allowed_fn,
+                                    cross_kv_dtype=getattr(self.opt, "generation_cross_kv_dtype", None))
 
     def get_prefix_allowed_tokens_fn(self, prefix_str: Optional[List[str]] = None):
         """Force the decoder prompt: while the generated prefix is shorter than the prompt only the next prompt

@@ -8,13 +8,17 @@
 //                                   (max, sum) that attn::combine_splits_kernel merges (same identity as the split-KV
 //                                   forward).  Algorithmic bytes per (query, layer, step) = Lk * 2 * H*64 * 2 B
 //                                   (FiD-base, Lk = 15 360: 47 MB).
+//                                   <kFP8>: the same over the e4m3 cross K|V cache of csrc/kv_fp8.cu (0.53x the bytes).
 //   decode_self_attention_kernel    appends the new token's K | V to the per-layer cache row t (t read from DEVICE memory so
 //                                   the whole step can be replayed from one CUDA graph) and attends over keys 0..t with
 //                                   T5's relative-position bias.
 #include "common.cuh"
 #include "host_common.h"
+#include "kv_fp8.cuh"
 
 #include <math.h>
+
+#include <type_traits>
 
 namespace dec {
 
@@ -40,90 +44,120 @@ __device__ __forceinline__ void unpack8(const uint4& w, float (&f)[8]) {
 }
 
 // grid = (chunks, H, B); block = 128.  Keys [c*chunk, min(Lk, (c+1)*chunk)) of batch b, head h.
-template <bool kBF16>
+// kFP8: kv holds e4m3 codes (uint8, csrc/kv_fp8.cu) and kv_scale one fp32 scale per (key row, 64-column block): the score
+// is kscale_j * (q . k8_j), the value weight p_j * vscale_j.  A lane then reads 16 codes (16 bytes) of a row, 4 lanes per
+// row; a warp still covers 16 keys per iteration, so its key group never straddles a 64-key tile either.
+template <bool kBF16, bool kFP8 = false>
 __global__ void __launch_bounds__(CROSS_THREADS)
-decode_cross_attention_kernel(const uint16_t* __restrict__ q, int64_t ldq, const uint16_t* __restrict__ kv, int64_t ldkv,
+decode_cross_attention_kernel(const uint16_t* __restrict__ q, int64_t ldq,
+                              const std::conditional_t<kFP8, uint8_t, uint16_t>* __restrict__ kv, int64_t ldkv,
                               int k_col0, int v_col0, const float* __restrict__ add_mask, const uint8_t* __restrict__ tile_live,
                               int Lk, int chunk, float scale, float* __restrict__ o_partial, float* __restrict__ ml_partial,
-                              int H) {
+                              int H, const float* __restrict__ kv_scale = nullptr, int64_t ld_scale = 0) {
+    using T = std::conditional_t<kFP8, uint8_t, uint16_t>;
+    constexpr int RL = kFP8 ? 4 : 8;    // lanes per key row (16 bytes of K and 16 of V each)
+    constexpr int DL = D / RL;          // head dims per lane
+    constexpr int ROWS = 32 / RL;       // key rows per warp instruction
     const int c = blockIdx.x, h = blockIdx.y, b = blockIdx.z;
     const int chunks = gridDim.x;
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    const int sub = lane >> 3;          // which of the 4 key rows of this warp instruction
-    const int seg = lane & 7;           // which 8 of the 64 head dims
+    const int sub = lane / RL;          // which of the ROWS key rows of this warp instruction
+    const int seg = lane % RL;          // which DL of the 64 head dims
     __shared__ float s_o[CROSS_THREADS / 32][D];
     __shared__ float s_m[CROSS_THREADS / 32], s_l[CROSS_THREADS / 32];
 
-    float qf[8];
-    {
+    float qf[DL];
+    if constexpr (kFP8) {
+#pragma unroll
+        for (int i = 0; i < DL / 8; ++i) {
+            float f8[8];
+            unpack8<kBF16>(*reinterpret_cast<const uint4*>(q + static_cast<int64_t>(b) * ldq + h * D + seg * DL + i * 8), f8);
+#pragma unroll
+            for (int e = 0; e < 8; ++e) qf[i * 8 + e] = f8[e] * (scale * LOG2E);   // scores in the log2 domain
+        }
+    } else {
         const uint4 qw = *reinterpret_cast<const uint4*>(q + static_cast<int64_t>(b) * ldq + h * D + seg * 8);
-        unpack8<kBF16>(qw, qf);
+        unpack8<kBF16>(qw, *reinterpret_cast<float(*)[8]>(qf));
 #pragma unroll
         for (int e = 0; e < 8; ++e) qf[e] *= scale * LOG2E;          // scores in the log2 domain
     }
     const int j_begin = c * chunk, j_end = min(Lk, (c + 1) * chunk);
-    const uint16_t* base = kv + (static_cast<int64_t>(b) * Lk) * ldkv + h * D + seg * 8;
+    const T* base = kv + (static_cast<int64_t>(b) * Lk) * ldkv + h * D + seg * DL;
     const float* mrow = add_mask ? add_mask + static_cast<int64_t>(b) * Lk : nullptr;
+    // kFP8: scale of key row j = sbase[j * ld_scale] (K), sbase[j * ld_scale + (v_col0 - k_col0) / 64] (V)
+    const float* sbase = kFP8 ? kv_scale + (static_cast<int64_t>(b) * Lk) * ld_scale + k_col0 / D + h : nullptr;
+    const int vs_off = (v_col0 - k_col0) / D;
     // 64-key tiles whose keys are all masked out weigh exactly 0 in the softmax (see atlas_b200_cross_attention_stream): skipped.
     // A warp's 16-key group never straddles a tile (chunk and the group offsets are multiples of 16, tiles of 64).
     const uint8_t* live_row = tile_live ? tile_live + static_cast<int64_t>(b) * ((Lk + 63) / 64) : nullptr;
 
-    float m = -INFINITY, l = 0.f, acc[8];
+    float m = -INFINITY, l = 0.f, acc[DL];
 #pragma unroll
-    for (int e = 0; e < 8; ++e) acc[e] = 0.f;
-    constexpr int UNROLL = 4;                                        // 4 x (K row + V row) 16-byte loads in flight per lane
-    for (int j0 = j_begin + warp * 4 * UNROLL; j0 < j_end; j0 += (CROSS_THREADS / 32) * 4 * UNROLL) {
+    for (int e = 0; e < DL; ++e) acc[e] = 0.f;
+    constexpr int UNROLL = 16 / ROWS;                                // UNROLL x (K row + V row) 16-byte loads in flight per lane
+    for (int j0 = j_begin + warp * ROWS * UNROLL; j0 < j_end; j0 += (CROSS_THREADS / 32) * ROWS * UNROLL) {
         if (live_row != nullptr && __ldg(live_row + (j0 >> 6)) == 0) continue;
         uint4 kw[UNROLL], vw[UNROLL];
-        float madd[UNROLL];
+        float madd[UNROLL], ksc[UNROLL], vsc[UNROLL];
 #pragma unroll
         for (int u = 0; u < UNROLL; ++u) {
-            const int j = j0 + u * 4 + sub;
+            const int j = j0 + u * ROWS + sub;
             const bool ok = j < j_end;
-            const uint16_t* row = base + static_cast<int64_t>(ok ? j : j_begin) * ldkv;
+            const T* row = base + static_cast<int64_t>(ok ? j : j_begin) * ldkv;
             kw[u] = *reinterpret_cast<const uint4*>(row + k_col0);
             vw[u] = *reinterpret_cast<const uint4*>(row + v_col0);
             madd[u] = ok ? (mrow ? mrow[j] * LOG2E : 0.f) : -INFINITY;
+            if constexpr (kFP8) {           // a key past the chunk weighs 0 whatever its (possibly NaN) scale
+                const float* srow = sbase + static_cast<int64_t>(ok ? j : j_begin) * ld_scale;
+                ksc[u] = ok ? __ldg(srow) : 0.f;
+                vsc[u] = ok ? __ldg(srow + vs_off) : 0.f;
+            }
         }
 #pragma unroll
         for (int u = 0; u < UNROLL; ++u) {
-            float kf[8], vf[8];
-            unpack8<kBF16>(kw[u], kf);
-            unpack8<kBF16>(vw[u], vf);
+            float kf[DL], vf[DL];
+            if constexpr (kFP8) {
+                kv8::unpack16(kw[u], kf);
+                kv8::unpack16(vw[u], vf);
+            } else {
+                unpack8<kBF16>(kw[u], kf);
+                unpack8<kBF16>(vw[u], vf);
+            }
             float s = 0.f;
 #pragma unroll
-            for (int e = 0; e < 8; ++e) s = fmaf(qf[e], kf[e], s);
-            s += __shfl_xor_sync(0xffffffffu, s, 1);
-            s += __shfl_xor_sync(0xffffffffu, s, 2);
-            s += __shfl_xor_sync(0xffffffffu, s, 4);                 // all 8 lanes of the row hold its score
+            for (int e = 0; e < DL; ++e) s = fmaf(qf[e], kf[e], s);
+#pragma unroll
+            for (int off = 1; off < RL; off <<= 1) s += __shfl_xor_sync(0xffffffffu, s, off);   // all RL lanes of the row
+            if constexpr (kFP8) s *= ksc[u];
             s += madd[u];
             const float m_new = fmaxf(m, s);
             if (m_new > -INFINITY) {
                 const float corr = exp2f(m - m_new), p = exp2f(s - m_new);
                 l = l * corr + p;
+                const float pv = kFP8 ? p * vsc[u] : p;
 #pragma unroll
-                for (int e = 0; e < 8; ++e) acc[e] = fmaf(acc[e], corr, p * vf[e]);
+                for (int e = 0; e < DL; ++e) acc[e] = fmaf(acc[e], corr, pv * vf[e]);
                 m = m_new;
             }
         }
     }
-    // merge the 4 key rows of the warp (lanes seg, seg+8, seg+16, seg+24), then the warps
+    // merge the ROWS key rows of the warp (lanes seg, seg+RL, ...), then the warps
 #pragma unroll
-    for (int off = 8; off < 32; off <<= 1) {
+    for (int off = RL; off < 32; off <<= 1) {
         const float m2 = __shfl_xor_sync(0xffffffffu, m, off), l2 = __shfl_xor_sync(0xffffffffu, l, off);
         const float mn = fmaxf(m, m2);
         const float c1 = mn > -INFINITY ? exp2f(m - mn) : 0.f, c2 = mn > -INFINITY ? exp2f(m2 - mn) : 0.f;
 #pragma unroll
-        for (int e = 0; e < 8; ++e) {
+        for (int e = 0; e < DL; ++e) {
             const float a2 = __shfl_xor_sync(0xffffffffu, acc[e], off);
             acc[e] = acc[e] * c1 + a2 * c2;
         }
         l = l * c1 + l2 * c2;
         m = mn;
     }
-    if (lane < 8) {
+    if (lane < RL) {
 #pragma unroll
-        for (int e = 0; e < 8; ++e) s_o[warp][lane * 8 + e] = acc[e];
+        for (int e = 0; e < DL; ++e) s_o[warp][lane * DL + e] = acc[e];
         if (lane == 0) s_m[warp] = m, s_l[warp] = l;
     }
     __syncthreads();
@@ -289,6 +323,39 @@ int atlas_b200_decode_cross_attention_live(const void* q, int64_t ldq, const voi
             static_cast<const uint16_t*>(q), ldq, static_cast<const uint16_t*>(kv), ldkv, k_col0, v_col0, add_mask, tile_live, Lk,
             chunk, scale, o_partial, ml_partial, H);
     abh::prof_end(s, abh::PROF_DECODE_CROSS, 4.0 * B * H * static_cast<double>(Lk) * dec::D);   // = K | V bytes read
+    abh::count_launch();
+    AB_CUDA_CHECK(cudaGetLastError());
+    return ATLAS_B200_OK;
+}
+
+int atlas_b200_decode_cross_attention_e4m3(const void* q, int64_t ldq, const uint8_t* kv8, int64_t ldkv, const float* kv_scale,
+                                           int64_t ld_scale, int32_t k_col0, int32_t v_col0, const float* add_mask,
+                                           const uint8_t* tile_live, int32_t B, int32_t H, int32_t Lk, int32_t chunk, float scale,
+                                           float* o_partial, float* ml_partial, int32_t is_bf16, void* stream) {
+    AB_REQUIRE(B >= 0 && H > 0 && Lk > 0 && chunk > 0 && chunk % 16 == 0, "decode_cross_attention_e4m3: bad shape");
+    AB_REQUIRE(ldq % 8 == 0 && ldkv % 16 == 0 && k_col0 % 64 == 0 && v_col0 % 64 == 0 && ld_scale > 0,
+               "decode_cross_attention_e4m3: ldq must be a multiple of 8 elements, ldkv of 16 bytes, the K and V column "
+               "offsets multiples of 64");
+    AB_REQUIRE(kv8 != nullptr && kv_scale != nullptr, "decode_cross_attention_e4m3: null K|V codes or scales");
+    AB_REQUIRE((reinterpret_cast<uintptr_t>(q) & 15) == 0 && (reinterpret_cast<uintptr_t>(kv8) & 15) == 0 &&
+                   (reinterpret_cast<uintptr_t>(kv_scale) & 3) == 0,
+               "decode_cross_attention_e4m3: q and kv8 must be 16-byte aligned (16-byte loads)");
+    if (B == 0) return ATLAS_B200_OK;
+    const int chunks = (Lk + chunk - 1) / chunk;
+    AB_REQUIRE(chunks <= 65535 && H <= 65535 && B <= 65535, "decode_cross_attention_e4m3: grid too large");
+    cudaStream_t s = static_cast<cudaStream_t>(stream);
+    dim3 grid(chunks, H, B);
+    abh::prof_begin(s, abh::PROF_DECODE_CROSS);
+    if (is_bf16)
+        dec::decode_cross_attention_kernel<true, true><<<grid, dec::CROSS_THREADS, 0, s>>>(
+            static_cast<const uint16_t*>(q), ldq, kv8, ldkv, k_col0, v_col0, add_mask, tile_live, Lk, chunk, scale, o_partial,
+            ml_partial, H, kv_scale, ld_scale);
+    else
+        dec::decode_cross_attention_kernel<false, true><<<grid, dec::CROSS_THREADS, 0, s>>>(
+            static_cast<const uint16_t*>(q), ldq, kv8, ldkv, k_col0, v_col0, add_mask, tile_live, Lk, chunk, scale, o_partial,
+            ml_partial, H, kv_scale, ld_scale);
+    // = K | V codes + their two scales read
+    abh::prof_end(s, abh::PROF_DECODE_CROSS, 2.0 * B * H * static_cast<double>(Lk) * (dec::D + 4));
     abh::count_launch();
     AB_CUDA_CHECK(cudaGetLastError());
     return ATLAS_B200_OK;

@@ -479,15 +479,23 @@ class FiD(nn.Module):
 
     # ---- decoder ---------------------------------------------------------------------------
     @torch.no_grad()
-    def cross_kv(self, enc, out=None):
+    def cross_kv(self, enc, out=None, sink=None):
         """K/V projections of the encoder output for every decoder layer ([B*n*L, 2*H*64] each), computed once
         per forward / per generation (the reference recomputes them every decoding step without use_cache).
-        `out`: list of pre-allocated buffers (the static cross K|V cache of the decode graph)."""
+        `out`: list of pre-allocated buffers (the static cross K|V cache of the decode graph).
+        `sink(i, kv)`: instead, hand layer i's projection to `sink` as soon as it is computed; every layer is projected into
+        ONE reused scratch buffer (peak memory: one layer), nothing is returned."""
         c = self.config
         W, G, dt = self._weights()
         flat = enc.reshape(-1, c.d_model)
         if flat.dtype != dt:
             flat = flat.to(dt)
+        if sink is not None:
+            scratch = None
+            for i in range(c.num_decoder_layers):
+                scratch = ops.linear(flat, G[f"decoder.block.{i}.layer.1.EncDecAttention.kv"], out=scratch)
+                sink(i, scratch)
+            return None
         return [ops.linear(flat, G[f"decoder.block.{i}.layer.1.EncDecAttention.kv"], out=None if out is None else out[i])
                 for i in range(c.num_decoder_layers)]
 
@@ -830,13 +838,13 @@ class FiD(nn.Module):
         K|V cache, the token / sequence / done / step tensors the step reads and writes on the device, and (optionally)
         the captured CUDA graph of ONE decode step that every step replays (the step index lives in device memory)."""
 
-        def __init__(self, model, B, Lk, Tmax, dt, dev):
+        def __init__(self, model, B, Lk, Tmax, dt, dev, xkv=None):
             c = model.config
             H, d = c.num_heads, c.d_model
             nl = c.num_decoder_layers
             self.B, self.Lk, self.Tmax = B, Lk, Tmax
             self.self_kv = [torch.zeros((B, Tmax, 2 * H * 64), dtype=dt, device=dev) for _ in range(nl)]
-            self.cross_kv = [torch.empty((B * Lk, 2 * H * 64), dtype=dt, device=dev) for _ in range(nl)]
+            self.cross_kv, self.cross_scale = FiD._cross_kv_buffers(B * Lk, H, nl, dt, dev, xkv)
             self.cross_mask = torch.zeros((B, Lk), dtype=torch.float32, device=dev)
             self.tok_in = torch.zeros(B, dtype=torch.int64, device=dev)
             self.seq = torch.zeros((B, Tmax), dtype=torch.int64, device=dev)
@@ -845,6 +853,15 @@ class FiD(nn.Module):
             self.logits = None
             self.graph = None
             self.cross_live = None
+
+    @staticmethod
+    def _cross_kv_buffers(rows, H, nl, dt, dev, xkv):
+        """The cross K|V cache of a decode state: per layer [rows, 2*H*64] in the run's 16-bit dtype (xkv None), or for
+        xkv == "fp8" the e4m3 codes uint8 [rows, 2*H*64] plus one fp32 scale per (row, 64-column block) [rows, 2*H]."""
+        if xkv is None:
+            return [torch.empty((rows, 2 * H * 64), dtype=dt, device=dev) for _ in range(nl)], None
+        return ([torch.empty((rows, 2 * H * 64), dtype=torch.uint8, device=dev) for _ in range(nl)],
+                [torch.empty((rows, 2 * H), dtype=torch.float32, device=dev) for _ in range(nl)])
 
     @torch.no_grad()
     def _decode_step_logits(self, st):
@@ -869,7 +886,14 @@ class FiD(nn.Module):
             p = f"decoder.block.{i}.layer.1."
             n = ops.layernorm(h, W[p + "layer_norm.weight"], None, eps, kind=1)
             q = ops.linear(n, W[p + "EncDecAttention.q.weight"])
-            if nb > 1:      # the nb beams share their batch element's cross K | V, streamed once per step
+            if st.cross_scale is not None:      # opt-in e4m3 cross K|V cache (cross_kv_dtype="fp8")
+                if nb > 1:
+                    ctx = ops.decode_cross_attention_beams_e4m3(q, st.cross_kv[i], st.cross_scale[i], B, nb, H, Lk, st.cross_mask,
+                                                                st.chunk, tile_live=st.cross_live)
+                else:
+                    ctx = ops.decode_cross_attention_e4m3(q, st.cross_kv[i], st.cross_scale[i], B, H, Lk, add_mask=st.cross_mask,
+                                                          scale=1.0, chunk=st.chunk, tile_live=st.cross_live)
+            elif nb > 1:    # the nb beams share their batch element's cross K | V, streamed once per step
                 ctx = ops.decode_cross_attention_beams(q, st.cross_kv[i], B, nb, H, Lk, st.cross_mask, st.chunk,
                                                        tile_live=st.cross_live)
             else:
@@ -888,14 +912,14 @@ class FiD(nn.Module):
         self K|V caches of the R = B * nb beam rows, ONE cross K|V per batch element, the ancestry and token tables, the beam
         scores and the hypothesis slots, all read and written on the device so that one captured graph serves every step."""
 
-        def __init__(self, model, B, nb, Lk, Tmax, dt, dev):
+        def __init__(self, model, B, nb, Lk, Tmax, dt, dev, xkv=None):
             c = model.config
             H = c.num_heads
             nl = c.num_decoder_layers
             R = B * nb
             self.B, self.nb, self.R, self.Lk, self.Tmax = B, nb, R, Lk, Tmax
             self.self_kv = [torch.zeros((R, Tmax, 2 * H * 64), dtype=dt, device=dev) for _ in range(nl)]
-            self.cross_kv = [torch.empty((B * Lk, 2 * H * 64), dtype=dt, device=dev) for _ in range(nl)]
+            self.cross_kv, self.cross_scale = FiD._cross_kv_buffers(B * Lk, H, nl, dt, dev, xkv)
             self.cross_mask = torch.zeros((B, Lk), dtype=torch.float32, device=dev)
             self.tok_in = torch.zeros(R, dtype=torch.int64, device=dev)
             self.t_dev = torch.zeros(1, dtype=torch.int32, device=dev)
@@ -938,14 +962,17 @@ class FiD(nn.Module):
             pos = torch.arange(t + 1, device=self.tok.device)
             return self.tok[self.anc[t & 1, :, : t + 1].long(), pos[None, :]].long()
 
-    def _decode_state(self, B, Lk, Tmax, dt, dev, nb=1):
+    def _decode_state(self, B, Lk, Tmax, dt, dev, nb=1, xkv=None):
         key = (B, Lk, Tmax, dt, dev) if nb == 1 else (B, Lk, Tmax, dt, dev, nb)
+        if xkv is not None:
+            key = key + (xkv,)
         states = self.__dict__.setdefault("_decode_states", {})
         st = states.get(key)
         if st is None:
             if len(states) >= 2:
                 states.pop(next(iter(states)))
-            st = FiD._DecodeState(self, B, Lk, Tmax, dt, dev) if nb == 1 else FiD._BeamState(self, B, nb, Lk, Tmax, dt, dev)
+            st = FiD._DecodeState(self, B, Lk, Tmax, dt, dev, xkv) if nb == 1 else \
+                FiD._BeamState(self, B, nb, Lk, Tmax, dt, dev, xkv)
             # keys per block of the cross-attention sweep: ~4 blocks per SM keep every SM streaming
             st.chunk = 256 if Lk >= 2048 else 64
             states[key] = st
@@ -956,7 +983,12 @@ class FiD(nn.Module):
         bias table - all into the state's fixed buffers (a captured step graph reads them)."""
         c = self.config
         B, Lk = st.B, st.Lk
-        self.cross_kv(enc, out=st.cross_kv)
+        if st.cross_scale is None:
+            self.cross_kv(enc, out=st.cross_kv)
+        else:
+            # e4m3 cache: each layer's 16-bit projection (one reused scratch buffer) is quantized into the state's fixed
+            # buffers (the captured step graph reads them)
+            self.cross_kv(enc, sink=lambda i, kv: ops.quantize_kv_e4m3(kv, out=st.cross_kv[i], scale_out=st.cross_scale[i]))
         neg = -1e4 if dt == torch.float16 else -1e9                                 # invert_attention_mask (4.18)
         st.cross_mask.copy_((1.0 - attention_mask.reshape(B, Lk).to(torch.float32)) * neg)
         live = ops.key_block_live(st.cross_mask)              # padded 64-key tiles: not read by the decode steps
@@ -980,14 +1012,19 @@ class FiD(nn.Module):
     @torch.no_grad()
     def generate(self, input_ids=None, attention_mask=None, max_length=32, min_length=1, num_beams=1,
                  num_return_sequences=1, length_penalty=1.0, forced_bos_token_id=None, prefix_allowed_tokens_fn=None,
-                 use_cache=True, **unused):
+                 use_cache=True, cross_kv_dtype=None, **unused):
         """Greedy decoding (what `Atlas.generate` requests with num_beams=1, src/atlas.py:592-619; transformers 4.18
         `greedy_search` with `use_cache`): the encoder and the cross-attention K|V projections run once; every step
         decodes ONE token per sequence against the per-layer self K|V cache and the cached cross K|V (csrc/decode.cu),
         picks the next token on the device and - without a `prefix_allowed_tokens_fn` - is replayed from a single CUDA
         graph with no host synchronisation except an all-done poll every 8 steps.  use_cache=False runs the
         first-generation path (the decoder prefix re-run every step), kept as the parity reference of the tests.
-        num_beams > 1: beam search (`_generate_beams`).  min_length=None means no EOS ban (the config's min_length, 0)."""
+        num_beams > 1: beam search (`_generate_beams`).  min_length=None means no EOS ban (the config's min_length, 0).
+        cross_kv_dtype: None (default) keeps the cross K|V cache in the run's 16-bit dtype; "fp8" stores it as e4m3 with one
+        fp32 scale per (key, K or V, head) (csrc/kv_fp8.cu): 0.53x the cache bytes, which every step streams once.  LOSSY
+        (the decoder attends over the dequantized keys and values): tokens may differ from the 16-bit run."""
+        if cross_kv_dtype is not None and cross_kv_dtype != "fp8":
+            raise AtlasB200Error(f"cross_kv_dtype={cross_kv_dtype!r} is not supported (None = the run's 16-bit dtype, or \"fp8\")")
         if num_return_sequences != 1:
             raise AtlasB200Error(f"num_return_sequences={num_return_sequences} is not implemented (only 1)")
         if min_length is None:
@@ -995,14 +1032,17 @@ class FiD(nn.Module):
         if num_beams is not None and num_beams > 1:
             return self._generate_beams(input_ids, attention_mask, max_length, min_length, int(num_beams),
                                         1.0 if length_penalty is None else float(length_penalty), prefix_allowed_tokens_fn,
-                                        unused)
+                                        unused, cross_kv_dtype)
         if not use_cache:
+            if cross_kv_dtype is not None:
+                raise AtlasB200Error("cross_kv_dtype='fp8' needs the KV-cached decode (use_cache=True): the use_cache=False "
+                                     "path re-runs the decoder prefix on the 16-bit cross K|V")
             return self._generate_prefix_rerun(input_ids, attention_mask, max_length, min_length, prefix_allowed_tokens_fn)
         c = self.config
         enc = self.encode(input_ids, attention_mask)
         B, Lk = enc.shape[0], enc.shape[1]
         W, G, dt = self._weights()
-        st = self._decode_state(B, Lk, int(max_length), dt, enc.device)
+        st = self._decode_state(B, Lk, int(max_length), dt, enc.device, xkv=cross_kv_dtype)
         self._prepare_decode(st, enc, attention_mask, W, dt)
         st.seq.fill_(c.pad_token_id)
         st.seq[:, 0] = c.decoder_start_token_id
@@ -1059,7 +1099,7 @@ class FiD(nn.Module):
 
     @torch.no_grad()
     def _generate_beams(self, input_ids, attention_mask, max_length, min_length, nb, length_penalty,
-                        prefix_allowed_tokens_fn, unused):
+                        prefix_allowed_tokens_fn, unused, cross_kv_dtype=None):
         """Beam search: transformers 4.18 `beam_search` with `BeamSearchScorer` (early_stopping=False, one returned
         sequence).  The encoder and the cross K|V projections run once on the B unexpanded rows; each step decodes the
         B * nb beam rows with the KV-cached decoder (self-attention through the ancestry table, the nb beams of a batch
@@ -1082,7 +1122,7 @@ class FiD(nn.Module):
         enc = self.encode(input_ids, attention_mask)
         B, Lk = enc.shape[0], enc.shape[1]
         W, G, dt = self._weights()
-        st = self._decode_state(B, Lk, max_length, dt, enc.device, nb=nb)
+        st = self._decode_state(B, Lk, max_length, dt, enc.device, nb=nb, xkv=cross_kv_dtype)
         self._prepare_decode(st, enc, attention_mask, W, dt)
         # 4.18's log_softmax returns the logits' dtype: 16-bit parameters round the log-probs, fp32 ones keep them fp32
         round_lp = self.shared.weight.dtype in (torch.float16, torch.bfloat16)

@@ -895,6 +895,100 @@ def decode_cross_attention_beams(q, kv, B, nb, H, Lk, add_mask, chunk, tile_live
     return out
 
 
+# ---------------------------------------------------------------------------------------------
+# opt-in FP8 (e4m3) cross K|V cache of KV-cached generation (csrc/kv_fp8.cu): lossy, off by default
+# ---------------------------------------------------------------------------------------------
+def _check_2d(t, name, dtype, shape, ld_mult=1):
+    require_cuda(t, name)
+    if t.dtype != dtype or t.dim() != 2 or tuple(t.shape) != tuple(shape) or t.stride(1) != 1 or \
+            t.stride(0) % ld_mult != 0 or (shape[0] > 1 and t.stride(0) < shape[1]):
+        raise AtlasB200Error(f"{name} must be {dtype} {list(shape)} with unit inner stride and a row stride that is a multiple of "
+                             f"{ld_mult}, got {t.dtype} {list(t.shape)} strides {t.stride()}")
+
+
+def _check_e4m3_cache(q, kv8, kv_scale, Bq, B, H, Lk, add_mask, tile_live, what):
+    if q.dtype not in (torch.float16, torch.bfloat16):
+        raise AtlasB200Error(f"{what}: q must be fp16 or bf16 (got {q.dtype})")
+    _check_2d(q, "q", q.dtype, (Bq, H * 64), 8)
+    _check_2d(kv8, "kv8", torch.uint8, (B * Lk, 2 * H * 64), 16)
+    _check_2d(kv_scale, "kv_scale", torch.float32, (B * Lk, 2 * H))
+    if any(t is not None and t.device != q.device for t in (kv8, kv_scale, add_mask, tile_live)):
+        raise AtlasB200Error(f"{what}: q, kv8, kv_scale, add_mask and tile_live must be on one device")
+    if q.data_ptr() % 16 != 0 or kv8.data_ptr() % 16 != 0:
+        raise AtlasB200Error(f"{what}: q and kv8 must start 16-byte aligned (16-byte loads)")
+    if add_mask is not None and tuple(add_mask.shape) != (B, Lk):
+        raise AtlasB200Error(f"{what}: add_mask must be [{B}, {Lk}] (got {list(add_mask.shape)})")
+    if tile_live is not None and (tile_live.dtype != torch.uint8 or tuple(tile_live.shape) != (B, (Lk + 63) // 64)
+                                  or not tile_live.is_contiguous()):
+        raise AtlasB200Error(f"{what}: tile_live must be contiguous uint8 [{B}, {(Lk + 63) // 64}]")
+
+
+def quantize_kv_e4m3(x, out=None, scale_out=None):
+    """x [rows, C*64] fp16 / bf16 (unit inner stride) -> (codes uint8 [rows, C*64] e4m3fn, scales fp32 [rows, C]): one scale
+    per 64-value block, amax / 448 (see include/atlas_b200.h).  `out` / `scale_out`: pre-allocated (possibly strided) buffers."""
+    require_cuda(x, "x")
+    if x.dtype not in (torch.float16, torch.bfloat16) or x.dim() != 2 or x.shape[1] % 64 != 0 or x.shape[1] == 0:
+        raise AtlasB200Error(f"quantize_kv_e4m3: x must be fp16 / bf16 [rows, C*64] (got {x.dtype} {list(x.shape)})")
+    rows, C = x.shape[0], x.shape[1] // 64
+    _check_2d(x, "x", x.dtype, (rows, C * 64), 8)
+    if out is None:
+        out = torch.empty((rows, C * 64), dtype=torch.uint8, device=x.device)
+    if scale_out is None:
+        scale_out = torch.empty((rows, C), dtype=torch.float32, device=x.device)
+    _check_2d(out, "out", torch.uint8, (rows, C * 64), 8)
+    _check_2d(scale_out, "scale_out", torch.float32, (rows, C))
+    if out.device != x.device or scale_out.device != x.device:
+        raise AtlasB200Error("quantize_kv_e4m3: x, out and scale_out must be on one device")
+    if x.data_ptr() % 16 != 0 or out.data_ptr() % 8 != 0:
+        raise AtlasB200Error("quantize_kv_e4m3: x must start 16-byte aligned (16-byte loads), out 8-byte aligned")
+    check(lib().atlas_b200_quantize_kv_e4m3(_ptr(x), max(x.stride(0), C * 64), rows, C, _ptr(out), max(out.stride(0), C * 64),
+                                            _ptr(scale_out), max(scale_out.stride(0), C), _bf(x), current_stream_ptr()))
+    return out, scale_out
+
+
+def decode_cross_attention_e4m3(q, kv8, kv_scale, B, H, Lk, add_mask=None, scale=1.0, chunk=256, out=None, tile_live=None):
+    """decode_cross_attention over the e4m3 cache: q [B, H*64] against codes kv8 uint8 [B*Lk, 2*H*64] (k | v) and their scales
+    kv_scale fp32 [B*Lk, 2*H] (quantize_kv_e4m3) -> ctx [B, H*64] in q's dtype."""
+    _check_e4m3_cache(q, kv8, kv_scale, B, B, H, Lk, add_mask, tile_live, "decode_cross_attention_e4m3")
+    if chunk <= 0 or chunk % 16 != 0:
+        raise AtlasB200Error(f"decode_cross_attention_e4m3: chunk {chunk} must be a positive multiple of 16")
+    chunks = (Lk + chunk - 1) // chunk
+    o_part = torch.empty((B * chunks, H * 64), dtype=torch.float32, device=q.device)
+    ml = torch.empty((B * chunks, H, 2), dtype=torch.float32, device=q.device)
+    am = add_mask.float().contiguous() if add_mask is not None else None
+    check(lib().atlas_b200_decode_cross_attention_e4m3(_ptr(q), q.stride(0), _ptr(kv8), max(kv8.stride(0), 2 * H * 64),
+                                                       _ptr(kv_scale), max(kv_scale.stride(0), 2 * H), 0, H * 64,
+                                                       _ptr(am) if am is not None else None,
+                                                       _ptr(tile_live) if tile_live is not None else None, B, H, Lk, chunk,
+                                                       float(scale), _ptr(o_part), _ptr(ml), _bf(q), current_stream_ptr()))
+    if out is None:
+        out = torch.empty((B, H * 64), dtype=q.dtype, device=q.device)
+    check(lib().atlas_b200_attention_combine_ex(_ptr(o_part), _ptr(ml), B, chunks, 1, H, _ptr(out), out.stride(0), None,
+                                                _bf(q), current_stream_ptr()))
+    return out
+
+
+def decode_cross_attention_beams_e4m3(q, kv8, kv_scale, B, nb, H, Lk, add_mask, chunk, tile_live=None, scale=1.0):
+    """decode_cross_attention_beams over the e4m3 cache (the stream kernel's e4m3 path, Lq = nb <= 64): q [B * nb, H*64], codes
+    kv8 uint8 [B*Lk, 2*H*64], scales kv_scale fp32 [B*Lk, 2*H] -> ctx [B * nb, H*64]."""
+    _check_e4m3_cache(q, kv8, kv_scale, B * nb, B, H, Lk, add_mask, tile_live, "decode_cross_attention_beams_e4m3")
+    if chunk <= 0 or chunk % 64 != 0:
+        raise AtlasB200Error(f"decode_cross_attention_beams_e4m3: chunk {chunk} must be a positive multiple of 64")
+    chunks = (Lk + chunk - 1) // chunk
+    o_part = torch.empty((B * chunks * nb, H * 64), dtype=torch.float32, device=q.device)
+    ml = torch.empty((B * chunks * nb, H, 2), dtype=torch.float32, device=q.device)
+    am = add_mask.float().contiguous() if add_mask is not None else None
+    check(lib().atlas_b200_cross_attention_stream_e4m3(_ptr(q), q.stride(0), 0, _ptr(kv8), max(kv8.stride(0), 2 * H * 64),
+                                                       _ptr(kv_scale), max(kv_scale.stride(0), 2 * H), 0, H * 64,
+                                                       _ptr(am) if am is not None else None,
+                                                       _ptr(tile_live) if tile_live is not None else None, B, H, nb, Lk, chunk,
+                                                       float(scale), _ptr(o_part), _ptr(ml), _bf(q), current_stream_ptr()))
+    out = torch.empty((B * nb, H * 64), dtype=q.dtype, device=q.device)
+    check(lib().atlas_b200_attention_combine_ex(_ptr(o_part), _ptr(ml), B, chunks, nb, H, _ptr(out), out.stride(0), None,
+                                                _bf(q), current_stream_ptr()))
+    return out
+
+
 def beam_topk(logits, beam_scores, t_dev, k, eos_id, min_length, round_lp, add_mask=None, cand_score=None, cand_tok=None,
               lp_out=None):
     """Per-row log-softmax + EOS ban + mask + beam score -> the row's top-k (cand_score fp32, cand_tok int32 [R, k])."""

@@ -213,6 +213,34 @@ int atlas_b200_decode_cross_attention_live(const void* q, int64_t ldq, const voi
 int atlas_b200_decode_self_attention(const void* qkv, int64_t ldqkv, void* cache, int32_t Tmax, const int32_t* t_dev,
                                      const float* bias_delta, float scale, void* out, int64_t ldo, int32_t B, int32_t H,
                                      int32_t is_bf16, void* stream);
+
+/* Opt-in FP8 (e4m3) cross K | V cache of KV-cached generation (csrc/kv_fp8.cu; FiD.generate(cross_kv_dtype="fp8")).  LOSSY:
+ * the decoder attends over dequantized keys and values.  Format: codes kv8 uint8 [rows, ldkv8] holding e4m3fn (OCP, no inf,
+ * max 448) in the columns of the 16-bit layout, and kv_scale fp32 [rows, ld_scale], one scale per (row, 64-column block):
+ * block c = columns [64 c, 64 c + 64) (K of head h = block h, V of head h = block H + h in the 2*H*64-wide cross K | V).
+ *  quantize_kv_e4m3  x [rows, ldx] 16-bit, n_blocks blocks of 64 values per row.  Per block, in fp32 with IEEE rounding:
+ *      amax = max |x|, inv = 448 / amax, code = e4m3(x * inv) (round to nearest even, saturating), scale = amax / 448;
+ *      amax == 0 -> scale 0 and codes 0; a NaN or inf in the block -> scale NaN and codes 0.  Dequantized value =
+ *      float(e4m3(code)) * scale.  ldx and ldkv8 multiples of 8 elements.
+ *  decode_cross_attention_e4m3  atlas_b200_decode_cross_attention_live over the codes: score_j = kscale_j * (q . k8_j) * scale
+ *      + mask, value weight p_j * vscale_j (fp32).  k_col0 / v_col0 (multiples of 64) index kv8's columns; the scales of key
+ *      row j are kv_scale[j * ld_scale + k_col0 / 64 + h] and [.. + v_col0 / 64 + h].  ldkv a multiple of 16 bytes.  Same
+ *      partials and chunk rules.  Reads Lk * 2 * H * (64 + 4) bytes per query and layer (0.53x the 16-bit cache).
+ *  cross_attention_stream_e4m3  atlas_b200_cross_attention_stream (Lq <= 64; the nb beams of a batch element in beam search)
+ *      over the codes, same scale columns and alignment as above: the codes are converted exactly to the 16-bit type of q,
+ *      kscale scales each column of S, vscale is folded into P before P is rounded to 16 bits (fp16: vscale <= 65504 / 448,
+ *      as quantize_kv_e4m3 of an fp16 K | V yields). */
+int atlas_b200_quantize_kv_e4m3(const void* x, int64_t ldx, int64_t rows, int32_t n_blocks, uint8_t* kv8, int64_t ldkv8,
+                                float* kv_scale, int64_t ld_scale, int32_t is_bf16, void* stream);
+int atlas_b200_decode_cross_attention_e4m3(const void* q, int64_t ldq, const uint8_t* kv8, int64_t ldkv, const float* kv_scale,
+                                           int64_t ld_scale, int32_t k_col0, int32_t v_col0, const float* add_mask,
+                                           const uint8_t* tile_live, int32_t B, int32_t H, int32_t Lk, int32_t chunk, float scale,
+                                           float* o_partial, float* ml_partial, int32_t is_bf16, void* stream);
+int atlas_b200_cross_attention_stream_e4m3(const void* q, int64_t ldq, int32_t q_col0, const uint8_t* kv8, int64_t ldkv,
+                                           const float* kv_scale, int64_t ld_scale, int32_t k_col0, int32_t v_col0,
+                                           const float* add_mask, const uint8_t* tile_live, int32_t B, int32_t H, int32_t Lq,
+                                           int32_t Lk, int32_t chunk, float scale, float* o_partial, float* ml_partial,
+                                           int32_t is_bf16, void* stream);
 int atlas_b200_decode_argmax(const void* logits, int64_t ld, int32_t V, int64_t* seq, int64_t ld_seq, int64_t* tok_in,
                              uint8_t* done, int32_t* t_dev, int32_t eos_id, int32_t pad_id, int32_t min_length, int32_t B,
                              int32_t is_bf16, void* stream);

@@ -12,6 +12,9 @@ steps, and the script reports:
     cross K|V bytes one step reads (live 64-key tiles x 64 keys x 2 (K, V) x H*64 x 2 B x layers: independent of nb) and
     both the kernel's and the whole step's achieved GB/s;
   - the card name and power limit, read in the same run.
+--xkv 16,fp8 runs every case with the 16-bit and with the opt-in e4m3 cross K|V cache (FiD.generate(cross_kv_dtype="fp8"))
+back to back (the fp8 bytes per step count the codes and the two fp32 scales per key and head), and prints the decode
+state's cross K|V bytes at FiD-base and Atlas-xl dimensions (computed from the shapes).
 One JSON line per case (and all of them to --out)."""
 import argparse
 import json
@@ -77,6 +80,7 @@ def main():
     ap.add_argument("--length", type=int, default=32)
     ap.add_argument("--repeats", type=int, default=5)
     ap.add_argument("--gens", type=int, default=10, help="generations per timed window")
+    ap.add_argument("--xkv", default="16", help="cross K|V cache types to compare, e.g. 16,fp8")
     ap.add_argument("--out", default=None)
     args = ap.parse_args()
     assert torch.cuda.is_available(), "perf_generate measures the GPU: no device found"
@@ -97,9 +101,11 @@ def main():
         mask = torch.ones(B, Lk, dtype=torch.bool, device=dev)
         model.encoder.config.n_context, model.encoder.config.bsz = args.n_ctx, B
         live_tiles = int(ops.key_block_live(((1.0 - mask.float()) * -1e9)).sum()) if ops._SKIP_MASKED else B * ((Lk + 63) // 64)
-        xkv_bytes = live_tiles * 64 * 2 * H * 64 * 2 * nl
-        for nb in [int(x) for x in args.beams.split(",")]:
-            kw = dict(max_length=args.length, min_length=args.length, num_beams=nb)
+        for nb, xkv in [(int(x), k) for x in args.beams.split(",") for k in args.xkv.split(",")]:
+            xkv = None if xkv == "16" else xkv
+            # bytes of one key row per head: K and V, 64 values of 2 B each, or 64 e4m3 codes + a fp32 scale each
+            xkv_bytes = live_tiles * 64 * 2 * H * (64 * 2 if xkv is None else 64 + 4) * nl
+            kw = dict(max_length=args.length, min_length=args.length, num_beams=nb, cross_kv_dtype=xkv)
 
             def gen():
                 with torch.no_grad():
@@ -110,6 +116,7 @@ def main():
             torch.cuda.synchronize()
             states = model.__dict__["_decode_states"]
             key = (B, Lk, args.length, torch.bfloat16, dev) if nb == 1 else (B, Lk, args.length, torch.bfloat16, dev, nb)
+            key = key + ((xkv,) if xkv is not None else ())
             st = states[key]
             def reset():
                 if nb == 1:
@@ -140,7 +147,7 @@ def main():
             sel_ms, sel_n = profiled_ms(L, PROF_BEAM_SELECT, gen, 2 * steps) if nb > 1 else (0.0, 0)
             x_ms, x_n = profiled_ms(L, PROF_ATTENTION if nb > 1 else PROF_DECODE_CROSS, gen, nl * steps)
             model.cuda_graphs = True
-            row = dict(B=B, nb=nb, n_ctx=args.n_ctx, text_len=args.text_len, steps=steps, ms_per_step=round(ms_step, 4),
+            row = dict(B=B, nb=nb, xkv=xkv or "16", n_ctx=args.n_ctx, text_len=args.text_len, steps=steps, ms_per_step=round(ms_step, 4),
                        ms_per_step_spread=[round(times[0], 4), round(times[-1], 4)],
                        tokens_per_s=round(B / (ms_step * 1e-3), 1), sequences_per_s=round(B / (ms_step * 1e-3 * steps), 2),
                        select_ms_per_step=round(sel_ms / steps, 4), select_launches=sel_n,
@@ -150,17 +157,26 @@ def main():
                        card=name, power_limit=power)
             rows.append(row)
             print(json.dumps(row), flush=True)
-    greedy = {r["B"]: r["ms_per_step"] for r in rows if r["nb"] == 1}
+    greedy = {(r["B"], r["xkv"]): r["ms_per_step"] for r in rows if r["nb"] == 1}
     for r in rows:
-        if r["B"] in greedy:
-            r["step_vs_greedy"] = round(r["ms_per_step"] / greedy[r["B"]], 3)
+        if (r["B"], r["xkv"]) in greedy:
+            r["step_vs_greedy"] = round(r["ms_per_step"] / greedy[(r["B"], r["xkv"])], 3)
     print(f"{name}, power limit {power}")
-    print(f"{'B':>3} {'nb':>3} {'ms/step':>8} {'x greedy':>8} {'tok/s':>9} {'select ms':>9} {'xattn ms':>8} {'xKV MB':>8} "
-          f"{'xattn GB/s':>10} {'step GB/s':>9}")
+    print(f"{'B':>3} {'nb':>3} {'xKV':>4} {'ms/step':>8} {'x greedy':>8} {'tok/s':>9} {'select ms':>9} {'xattn ms':>8} "
+          f"{'xKV MB':>8} {'xattn GB/s':>10} {'step GB/s':>9}")
     for r in rows:
-        print(f"{r['B']:>3} {r['nb']:>3} {r['ms_per_step']:>8.3f} {r.get('step_vs_greedy', 0):>8.2f} {r['tokens_per_s']:>9.1f} "
+        print(f"{r['B']:>3} {r['nb']:>3} {r['xkv']:>4} {r['ms_per_step']:>8.3f} {r.get('step_vs_greedy', 0):>8.2f} "
+              f"{r['tokens_per_s']:>9.1f} "
               f"{r['select_ms_per_step']:>9.4f} {r['xattn_ms_per_step']:>8.3f} {r['xkv_bytes_per_step'] / 1e6:>8.1f} "
               f"{r['xattn_kernel_GBps']:>10.1f} {r['step_GBps']:>9.1f}")
+    if "fp8" in args.xkv.split(","):
+        # the decode state's cross K|V at B = 8, n_context 40 x 384 keys: FiD-base (12 layers, 12 heads) and Atlas-xl
+        # dimensions (24 layers, d 2048 = 32 heads of 64)
+        for label, layers, heads in (("FiD-base", 12, 12), ("Atlas-xl", 24, 32)):
+            rows_kv = 8 * args.n_ctx * args.text_len
+            b16 = rows_kv * 2 * heads * 64 * 2 * layers
+            b8 = rows_kv * 2 * heads * (64 + 4) * layers
+            print(f"decode-state cross K|V, {label} B=8: 16-bit {b16 / 1e9:.2f} GB, fp8 {b8 / 1e9:.2f} GB ({b8 / b16:.4f}x)")
     if args.out:
         os.makedirs(os.path.dirname(os.path.abspath(args.out)), exist_ok=True)
         with open(args.out, "w") as f:
