@@ -67,6 +67,8 @@ def lib():
     L.atlas_b200_linear_ex.argtypes = [c.c_void_p, c.c_int64, c.c_void_p, c.c_int64, c.c_void_p, c.c_void_p, c.c_int64,
                                        c.c_void_p, c.c_int64, c.c_int32, c.c_int32, c.c_int32, c.c_int32, c.c_int32,
                                        c.c_void_p, c.c_void_p, c.c_float, c.c_void_p]
+    L.atlas_b200_linear_schedule.restype = c.c_int
+    L.atlas_b200_linear_schedule.argtypes = [c.c_int32, c.c_int32, c.c_int32, c.c_int32]
     L.atlas_b200_layernorm.restype = c.c_int
     L.atlas_b200_layernorm.argtypes = [c.c_void_p, c.c_int64, c.c_void_p, c.c_void_p, c.c_void_p, c.c_int64, c.c_int32,
                                        c.c_int32, c.c_float, c.c_int32, c.c_int32, c.c_void_p]
@@ -224,6 +226,7 @@ EXPORTED_SYMBOLS = [
     "atlas_b200_cast_f32",
     "atlas_b200_linear",
     "atlas_b200_linear_ex",
+    "atlas_b200_linear_schedule",
     "atlas_b200_layernorm",
     "atlas_b200_bert_embed_ln",
     "atlas_b200_masked_mean_pool",

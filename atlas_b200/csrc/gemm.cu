@@ -19,9 +19,15 @@
 //                                                                   with row_ss the row scale comes first: relu(s acc))
 //
 // Persistent, warp-specialised, one CTA per SM (grid = #SMs): warpgroup 0 is the TMA producer (one thread; setmaxnreg
-// gives its registers to the consumers), warpgroups 1 and 2 are consumers.  Two schedules:
-//   ping-pong (gemm_pp_kernel; K-major launches of at least 2 x #SMs 128 x 128 tiles, i.e. the encoder projections, the
-//     cross-attention K|V projection and the LM head at 256 rows x 32128): each consumer owns whole 128 x 128 tiles, two wgmma m64n128k16 per k16 step
+// gives its registers to the consumers), warpgroups 1 and 2 are consumers.  Three schedules:
+//   wide (gemm_wide_kernel; the encoder-sized K-major launches with the plain epilogue: the q|k|v projection, the
+//     cross-attention K|V projection, the input-gradient GEMMs of training): both consumers share one 128 x 256 tile,
+//     64 rows each, one wgmma m64n256k16 per k16 step on a shared W block, then a TMA-store epilogue through a 32 KB
+//     staging buffer per consumer that overlaps the next tile's mainloop.  3 stages of 48 KB.  It implements every
+//     epilogue (ATLAS_B200_GEMM_SCHEDULE=wide runs it for all encoder-sized launches); the rule sends it only the plain one.
+//   ping-pong (gemm_pp_kernel; the other K-major launches of at least 2 x #SMs 128 x 128 tiles, i.e. the encoder
+//     projections with a fused bias / activation / residual / gate, and the LM head at 256 rows x 32128, whose 251
+//     column tiles would pad to 252 at 256 wide): each consumer owns whole 128 x 128 tiles, two wgmma m64n128k16 per k16 step
 //     sharing the W descriptor; a CTA's work items alternate between the consumers, which take turns in the mainloop, so
 //     one consumer's epilogue runs under the other's MMAs.  The epilogue goes through a per-consumer 32 KB staging buffer
 //     (128-byte swizzle) and a TMA store; EPI_RESIDUAL's residual tile is loaded into that buffer by the producer during
@@ -31,15 +37,16 @@
 //     are enough tiles to fill the SMs, else 128), 64 rows each, wgmma m64nBLOCK_Nk16, then the epilogue straight from the
 //     accumulator registers to global memory (EPI_RESIDUAL: the tile's residual rows are prefetched into L2 before its
 //     mainloop and read in batches of independent loads).  A ring of 64-wide K stages (~200 KB).
-// The choice depends only on the shape (and, for EPI_RESIDUAL, on a 16-byte aligned residual, which its tensor map needs).
-// Both schedules run each output element through the same sequence of k16 MMAs and the same epilogue arithmetic
-// (epilogue_pair), so they give bit-identical results.
+// The choice depends only on the shape and epilogue (and, for EPI_RESIDUAL, on a 16-byte aligned residual, which its
+// tensor map needs): select_schedule, reported by atlas_b200_linear_schedule.  All schedules run each output element
+// through the same sequence of k16 MMAs and the same epilogue arithmetic (epilogue_pair), so they give bit-identical results.
 #include "common.cuh"
 #include "host_common.h"
 #include "wgmma.cuh"
 
 #include <math.h>
 #include <stdlib.h>
+#include <string.h>
 
 namespace gemm {
 
@@ -572,6 +579,217 @@ gemm_pp_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant
     if (ctid == 0) ab::tma_store_wait_all();
 }
 
+// ===================== wide schedule (K-major, 128 x 256 tiles, encoder-sized launches) =====================
+namespace wd {
+constexpr int BLOCK_N = 256;
+constexpr int A_BYTES = BLOCK_M * BLOCK_K * 2;                      // 16 KB
+constexpr int STAGE_BYTES = (BLOCK_M + BLOCK_N) * BLOCK_K * 2;      // 48 KB: A 128 x 64, W 256 x 64
+constexpr int BOX_BYTES = 64 * 64 * 2;                              // one 64-row x 64-column box of C / the residual
+constexpr int EPI_BYTES = 64 * BLOCK_N * 2;                         // 32 KB staging per consumer: its 64 rows, four boxes
+constexpr int STAGES = (227 * 1024 - 1024 - CONSUMERS * EPI_BYTES) / STAGE_BYTES;    // 3
+constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + CONSUMERS * EPI_BYTES + 1024;
+constexpr uint32_t EPI_BAR = 1;                                     // EPI_BAR + c syncs consumer c's 128 threads
+}  // namespace wd
+
+// Both consumers work on the same 128 x 256 tile: each stage holds one A block (128 x 64) and one W block (256 x 64), and
+// consumer c runs one wgmma m64n256k16 per k16 step on A rows [64 c, 64 c + 64) against the whole W block.  Per FLOP this
+// reads half the W bytes from shared memory that a 128 x 128 tile (two m64n128 sharing a W slice) does, and fills half
+// as many bytes per FLOP by TMA.  Each consumer releases a stage on its own (empty_bar counts two arrivals).  The epilogue
+// writes the consumer's 64 x 256 slice into its own 32 KB staging buffer (four 64 x 64 boxes, 128-byte swizzle) and one
+// thread stores it with TMA; the consumer starts the next tile's mainloop without waiting for the store, and waits for it
+// to have read the buffer only during that mainloop.  EPI_RESIDUAL: the producer loads the consumer's residual slice into
+// the staging buffer during the tile's mainloop, as soon as the previous store has read it.  The two consumers reach their
+// epilogues together; starting consumer 1 two k-blocks after consumer 0 (all the 3-stage ring allows) was measured and
+// did not shorten any encoder shape (see select_schedule), so they run in step.
+template <bool kBF16, int kEpi>
+__global__ void __launch_bounds__(THREADS, 1)
+gemm_wide_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
+                 const __grid_constant__ CUtensorMap tmap_c, const __grid_constant__ CUtensorMap tmap_r, const Params p) {
+    using namespace wd;
+    using pp::sw128_offset;
+    extern __shared__ uint8_t smem_raw[];
+    __shared__ __align__(8) uint64_t full_bar[STAGES];
+    __shared__ __align__(8) uint64_t empty_bar[STAGES];
+    __shared__ __align__(8) uint64_t res_full[CONSUMERS];     // residual slice landed in the staging buffer
+    __shared__ __align__(8) uint64_t res_empty[CONSUMERS];    // staging buffer read out by the previous TMA store
+
+    const uint32_t warp = threadIdx.x >> 5;
+    const uint32_t lane = threadIdx.x & 31u;
+    const uint32_t smem_base = (ab::smem_u32(smem_raw) + 1023u) & ~1023u;
+    uint8_t* smem_gen = smem_raw + (smem_base - ab::smem_u32(smem_raw));
+    uint8_t* epi_gen = smem_gen + STAGES * STAGE_BYTES;
+
+    const int m_rows = p.m_dev != nullptr ? min(p.M, max(__ldg(p.m_dev), 0)) : p.M;     // identical in every role
+    const int num_m = (m_rows + BLOCK_M - 1) / BLOCK_M;
+    const int num_n = (p.N + BLOCK_N - 1) / BLOCK_N;
+    const int num_tiles = num_m * num_n;
+    const int num_kb = (p.K + BLOCK_K - 1) / BLOCK_K;
+    const int n_out = kEpi == EPI_GATED ? p.N / 2 : p.N;                 // columns of C
+    constexpr int OUT_BOXES = kEpi == EPI_GATED ? 2 : 4;                // 64-column boxes of C per tile
+
+    if (threadIdx.x == 0) {
+        ab::tma_prefetch_desc(&tmap_a);
+        ab::tma_prefetch_desc(&tmap_b);
+        ab::tma_prefetch_desc(&tmap_c);
+        if constexpr (kEpi == EPI_RESIDUAL) ab::tma_prefetch_desc(&tmap_r);
+        for (int s = 0; s < STAGES; ++s) {
+            ab::mbar_init(&full_bar[s], 1);
+            ab::mbar_init(&empty_bar[s], CONSUMERS);          // one arrive per consumer warpgroup
+        }
+        for (int c = 0; c < CONSUMERS; ++c) {
+            ab::mbar_init(&res_full[c], 1);
+            ab::mbar_init(&res_empty[c], 1);
+        }
+        ab::fence_barrier_init();
+    }
+    __syncthreads();
+
+    if (warp < 4) {
+        // ===================== producer warpgroup (one thread issues the TMA loads) =====================
+        ab::setmaxnreg_dec<40>();
+        if (warp == 0 && lane == 0) {
+            uint32_t stage = 0, phase = 0;
+            int i = 0;
+            for (int t = blockIdx.x; t < num_tiles; t += gridDim.x, ++i) {
+                const int m_blk = t / num_n, n_blk = t % num_n;
+                const int a_row = m_blk * BLOCK_M;
+                const int b_row = n_blk * BLOCK_N;
+                // L2 prefetch of the A rows of this CTA's NEXT work item when it starts a new row block
+                int pf_row = -1;
+                const int t2 = t + static_cast<int>(gridDim.x);
+                if (p.l2_prefetch && t2 < num_tiles && t2 % num_n == 0) pf_row = (t2 / num_n) * BLOCK_M;
+                bool res_issued[CONSUMERS] = {false, false};
+                for (int kb = 0; kb < num_kb; ++kb) {
+                    if (pf_row >= 0) ab::tma_prefetch_2d(&tmap_a, kb * BLOCK_K, pf_row);
+                    ab::mbar_wait_nocall(&empty_bar[stage], phase ^ 1u);
+                    uint8_t* st = smem_gen + stage * STAGE_BYTES;
+                    ab::mbar_arrive_expect_tx(&full_bar[stage], STAGE_BYTES);
+                    ab::tma_load_2d(&tmap_a, &full_bar[stage], st, kb * BLOCK_K, a_row, ab::kEvictNormal);
+                    ab::tma_load_2d(&tmap_b, &full_bar[stage], st + A_BYTES, kb * BLOCK_K, b_row, ab::kEvictLast);
+                    if (++stage == STAGES) {
+                        stage = 0;
+                        phase ^= 1u;
+                    }
+                    if constexpr (kEpi == EPI_RESIDUAL) {
+                        // each consumer's residual slice, as early in the tile's mainloop as its staging buffer is free.
+                        // The buffer is probed after each k-block and waited for only after the last one, so the stage
+                        // loads never stall on it.  Boxes wholly past the edge of R are not loaded (their columns are
+                        // skipped by the epilogue, their rows clipped by the store).
+                        const uint32_t par = (static_cast<uint32_t>(i) & 1u) ^ 1u;
+                        for (int c = 0; c < CONSUMERS; ++c) {
+                            if (res_issued[c] || !(kb == num_kb - 1 || ab::mbar_test_wait(&res_empty[c], par))) continue;
+                            ab::mbar_wait_nocall(&res_empty[c], par);
+                            res_issued[c] = true;
+                            uint8_t* buf = epi_gen + c * EPI_BYTES;
+                            const int r_row = a_row + 64 * c;
+                            int boxes = 0;
+                            if (r_row < p.M)
+                                for (int b = 0; b < 4 && b_row + 64 * b < p.N; ++b) ++boxes;
+                            ab::mbar_arrive_expect_tx(&res_full[c], boxes * BOX_BYTES);
+                            for (int b = 0; b < boxes; ++b)
+                                ab::tma_load_2d(&tmap_r, &res_full[c], buf + b * BOX_BYTES, b_row + 64 * b, r_row,
+                                                ab::kEvictFirst);
+                        }
+                    }
+                }
+            }
+        }
+        return;
+    }
+
+    // ===================== consumer warpgroups: 64 rows x 256 columns each of every tile =====================
+    ab::setmaxnreg_inc<232>();
+    const uint32_t wg = (warp >> 2) - 1u;              // rows [64 wg, 64 wg + 64) of the tile
+    const uint32_t wl = warp & 3u;                     // warp inside the warpgroup
+    const uint32_t ctid = threadIdx.x & 127u;
+    uint8_t* buf = epi_gen + wg * EPI_BYTES;
+    const int cq = static_cast<int>(2u * (lane & 3u));
+    uint32_t stage = 0, phase = 0;
+    int i = 0;
+    for (int t = blockIdx.x; t < num_tiles; t += gridDim.x, ++i) {
+        const int m_blk = t / num_n, n_blk = t % num_n;
+        float acc[BLOCK_N / 2];
+#pragma unroll
+        for (int q = 0; q < BLOCK_N / 2; ++q) acc[q] = 0.f;
+        int prev_stage = -1;
+        for (int kb = 0; kb < num_kb; ++kb) {
+            ab::mbar_wait_nocall(&full_bar[stage], phase);
+            const uint32_t st = smem_base + stage * STAGE_BYTES;
+            ab::wgmma_fence();
+#pragma unroll
+            for (int k = 0; k < BLOCK_K / UMMA_K; ++k)
+                ab::wgmma_m64n256k16_ss<kBF16, 0, 0>(acc, ab::wgmma_desc_sw128(st + wg * 8192u + k * 32u),
+                                                     ab::wgmma_desc_sw128(st + A_BYTES + k * 32u), 1);
+            ab::wgmma_commit();
+            // the previous tile's TMA store has had this tile's first k-block to read the staging buffer: wait for it
+            // here, under the MMAs just issued, and hand the buffer to the residual load
+            if (kb == 0 && i > 0 && ctid == 0) {
+                ab::tma_store_wait_read();
+                if constexpr (kEpi == EPI_RESIDUAL) ab::mbar_arrive(&res_empty[wg]);
+            }
+            // the previous stage's MMAs have retired once at most this stage's group is pending: release it
+            ab::wgmma_wait<1>();
+            ab::wgmma_reg_fence(acc);
+            if (prev_stage >= 0 && ctid == 0) ab::mbar_arrive(&empty_bar[prev_stage]);
+            prev_stage = static_cast<int>(stage);
+            if (++stage == STAGES) {
+                stage = 0;
+                phase ^= 1u;
+            }
+        }
+        ab::wgmma_wait<0>();
+        ab::wgmma_reg_fence(acc);
+        if (prev_stage >= 0 && ctid == 0) ab::mbar_arrive(&empty_bar[prev_stage]);
+
+        // ---- epilogue into the staging buffer: rows 16 wl + lane / 4 (+ 8) of the slice, column pairs 8 j + 2 (lane % 4)
+        if constexpr (kEpi == EPI_RESIDUAL) ab::mbar_wait_nocall(&res_full[wg], static_cast<uint32_t>(i & 1));
+        else if (i > 0) ab::named_bar_sync(EPI_BAR + wg, 128);    // the previous store has read the buffer
+        const int row0 = m_blk * BLOCK_M + static_cast<int>(wg) * 64;
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+            const int r = static_cast<int>(wl * 16u + (lane >> 2)) + 8 * h;                   // row in the slice
+            const int row = row0 + r;
+            const bool row_ok = row < p.M;
+            const float rscale = row_scale(p, row, row_ok);
+            // out_ss: one partial sum per 128 columns, the same sums in the same order as the 128 x 128 schedules
+#pragma unroll
+            for (int half = 0; half < 2; ++half) {
+                float ss_out = 0.f;
+#pragma unroll
+                for (int j = 16 * half; j < 16 * half + 16; ++j) {
+                    const int c = 8 * j + cq;                                                  // column in the tile
+                    const int col = n_blk * BLOCK_N + c;
+                    if (col >= p.N) continue;                  // past the edge: the TMA store clips it
+                    uint8_t* dst = buf + (c >> 6) * BOX_BYTES + sw128_offset(r, c & 63);
+                    const uint32_t res = kEpi == EPI_RESIDUAL ? *reinterpret_cast<const uint32_t*>(dst) : 0u;
+                    const uint32_t o = epilogue_pair<kBF16, kEpi>(p, acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1], rscale,
+                                                                  col, res);
+                    if constexpr (kEpi == EPI_GATED) {
+                        const int co = c >> 1;
+                        *reinterpret_cast<uint16_t*>(buf + (co >> 6) * BOX_BYTES + sw128_offset(r, co & 63)) =
+                            static_cast<uint16_t>(o & 0xFFFFu);
+                    } else {
+                        *reinterpret_cast<uint32_t*>(dst) = o;
+                        if (p.out_ss != nullptr) ss_out = add_sq_pair<kBF16>(o, ss_out);
+                    }
+                }
+                if (kEpi != EPI_GATED && p.out_ss != nullptr) out_ss_add(p, row, row_ok, lane, ss_out);
+            }
+        }
+        ab::fence_proxy_async_smem();                  // generic-proxy writes -> visible to the TMA store
+        ab::named_bar_sync(EPI_BAR + wg, 128);
+        if (ctid == 0) {
+            // boxes wholly past the edge of C are not stored (the tensor map clips the rest)
+            const int c0 = n_blk * (BLOCK_N / (kEpi == EPI_GATED ? 2 : 1));
+            if (row0 < p.M)
+                for (int b = 0; b < OUT_BOXES && c0 + 64 * b < n_out; ++b)
+                    ab::tma_store_2d(&tmap_c, buf + b * BOX_BYTES, c0 + 64 * b, row0);
+            ab::tma_store_commit();
+        }
+    }
+    if (ctid == 0) ab::tma_store_wait_all();
+}
+
 template <bool kBF16, int BLOCK_N, bool kTN, int kEpi>
 static int launch(const CUtensorMap& ta, const CUtensorMap& tb, const Params& p, cudaStream_t s) {
     using C = Cfg<BLOCK_N>;
@@ -623,6 +841,60 @@ template <int kEpi>
 static int launch_pp_t(bool bf16, const CUtensorMap& ta, const CUtensorMap& tb, const CUtensorMap& tc, const CUtensorMap& tr,
                        const Params& p, cudaStream_t s) {
     return bf16 ? launch_pp<true, kEpi>(ta, tb, tc, tr, p, s) : launch_pp<false, kEpi>(ta, tb, tc, tr, p, s);
+}
+
+template <bool kBF16, int kEpi>
+static int launch_wide(const CUtensorMap& ta, const CUtensorMap& tb, const CUtensorMap& tc, const CUtensorMap& tr,
+                       const Params& p, cudaStream_t s) {
+    static bool attr_set = false;
+    if (!attr_set) {
+        AB_CUDA_CHECK(cudaFuncSetAttribute(gemm_wide_kernel<kBF16, kEpi>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                           wd::SMEM_BYTES));
+        attr_set = true;
+    }
+    const int tiles = ((p.M + BLOCK_M - 1) / BLOCK_M) * ((p.N + wd::BLOCK_N - 1) / wd::BLOCK_N);
+    const int grid = tiles < abh::num_sms() ? tiles : abh::num_sms();
+    abh::prof_begin(s, abh::PROF_LINEAR);
+    gemm_wide_kernel<kBF16, kEpi><<<grid, THREADS, wd::SMEM_BYTES, s>>>(ta, tb, tc, tr, p);
+    if (p.m_dev != nullptr) abh::prof_end_dyn(s, abh::PROF_LINEAR, 2.0 * static_cast<double>(p.N) * p.K, p.m_dev, p.M);
+    else abh::prof_end(s, abh::PROF_LINEAR, 2.0 * p.M * static_cast<double>(p.N) * p.K);
+    abh::count_launch();
+    AB_CUDA_CHECK(cudaGetLastError());
+    return ATLAS_B200_OK;
+}
+
+template <int kEpi>
+static int launch_wide_t(bool bf16, const CUtensorMap& ta, const CUtensorMap& tb, const CUtensorMap& tc, const CUtensorMap& tr,
+                         const Params& p, cudaStream_t s) {
+    return bf16 ? launch_wide<true, kEpi>(ta, tb, tc, tr, p, s) : launch_wide<false, kEpi>(ta, tb, tc, tr, p, s);
+}
+
+// The schedule of a K-major launch (values of atlas_b200_linear_schedule).  res_aligned: EPI_RESIDUAL's residual base is
+// 16-byte aligned, which the TMA-staged schedules need for its tensor map.  Measured at the bench's encoder sizes (77,696
+// packed rows, H100 SXM 80 GB at 700 W, tools/prof_ops.py gemm_sched; wide vs ping-pong, two runs each):
+//   plain      q|k|v N 2304 K 768   401 vs 472-480 us    cross K|V N 1536   286-293 vs 344-376 us
+//              mainloop N 2304 K 4096 (M 61,440)   1675-1682 vs 2160-2218 us                       -> wide
+//   residual   o-proj N 768 K 768   262 vs 226-230 us    wo N 768 K 2048 + out_ss   490-495 vs 427-434 us -> ping-pong
+//   gated      N 4096 K 768         891-893 vs 875-901 us                                           -> ping-pong
+//   bias       N 2304 K 768         624-676 vs 626-632 us                                           -> ping-pong
+//   GELU       N 3072 K 768         1023-1034 vs 978-1022 us                                        -> ping-pong
+//   ReLU       N 3072 K 768         860-871 vs 865-891 us                                           -> ping-pong
+// A fused epilogue is as fast or faster on ping-pong, which hides it under the other consumer's MMAs; wide only wins where
+// the epilogue is a plain store.  Wide also needs the 256-wide tiles to pad no more columns than 128-wide ones
+// (N % 256 == 0 or > 128).
+// ATLAS_B200_GEMM_SCHEDULE=pingpong|wide overrides the choice between the two for every launch that may run either (for
+// timing them against each other on the same shapes: tools/prof_ops.py gemm_sched).
+static int select_schedule(int64_t M, int64_t N, int64_t K, int epilogue, bool res_aligned) {
+    (void)K;
+    static const char* force = getenv("ATLAS_B200_GEMM_SCHEDULE");
+    const int64_t tiles128 = ((M + 127) / 128) * ((N + 127) / 128);
+    if (tiles128 >= 2 * abh::num_sms() && (epilogue != EPI_RESIDUAL || res_aligned)) {
+        if (force != nullptr && strcmp(force, "pingpong") == 0) return ATLAS_B200_GEMM_PINGPONG;
+        if (force != nullptr && strcmp(force, "wide") == 0) return ATLAS_B200_GEMM_WIDE;
+        return epilogue == EPI_NONE && (N + 255) / 256 * 2 == (N + 127) / 128 ? ATLAS_B200_GEMM_WIDE : ATLAS_B200_GEMM_PINGPONG;
+    }
+    if (N >= 256 && ((M + 127) / 128) * ((N + 255) / 256) >= abh::num_sms()) return ATLAS_B200_GEMM_COOPERATIVE_256;
+    return ATLAS_B200_GEMM_COOPERATIVE_128;
 }
 
 // out[i] = round16(sum_s part[s][i]) for the M*N outputs of a split-K GEMM (8 outputs per thread)
@@ -718,15 +990,10 @@ int atlas_b200_linear_ex(const void* A, int64_t lda, const void* W, int64_t ldw,
     p.residual = static_cast<const uint16_t*>(residual);
     p.C = static_cast<uint16_t*>(C);
     cudaStream_t s = static_cast<cudaStream_t>(stream);
-    // ping-pong once every consumer warpgroup has at least one 128 x 128 tile (encoder-sized M, or the 32128-column LM
-    // head); the residual goes
-    // through a tensor map, which needs a 16-byte aligned base
-    const int64_t tiles128 = static_cast<int64_t>((M + 127) / 128) * ((N + 127) / 128);
-    const bool pingpong = tiles128 >= 2 * abh::num_sms() &&
-                          (epilogue != EPI_RESIDUAL || (reinterpret_cast<uintptr_t>(residual) & 15u) == 0);
-    // cooperative: 128 x 256 tiles once there are enough of them to fill the SMs, else 128 x 128
-    const bool wide = !pingpong && N >= 256 && (static_cast<int64_t>((M + 127) / 128) * ((N + 255) / 256) >= abh::num_sms());
-    const int block_n = wide ? 256 : 128;
+    const int sched = select_schedule(M, N, K, epilogue, (reinterpret_cast<uintptr_t>(residual) & 15u) == 0);
+    const bool pingpong = sched == ATLAS_B200_GEMM_PINGPONG;
+    const bool wide = sched == ATLAS_B200_GEMM_COOPERATIVE_256;
+    const int block_n = (wide || sched == ATLAS_B200_GEMM_WIDE) ? 256 : 128;
     CUtensorMap ta, tb;
     int rc = abh::make_tmap_2d_16bit(&ta, A, static_cast<uint64_t>(M), static_cast<uint64_t>(K),
                                      static_cast<uint64_t>(lda), BLOCK_M, BLOCK_K, is_bf16 != 0);
@@ -734,19 +1001,31 @@ int atlas_b200_linear_ex(const void* A, int64_t lda, const void* W, int64_t ldw,
     rc = abh::make_tmap_2d_16bit(&tb, W, static_cast<uint64_t>(N), static_cast<uint64_t>(K), static_cast<uint64_t>(ldw),
                                  static_cast<uint32_t>(block_n), BLOCK_K, is_bf16 != 0);
     if (rc) return rc;
-    if (pingpong) {
-        // C (N / 2 columns for EPI_GATED) and the residual in 128-row boxes of 64 columns
+    if (pingpong || sched == ATLAS_B200_GEMM_WIDE) {
+        // C (N / 2 columns for EPI_GATED) and the residual in boxes of 64 columns: 128 rows (ping-pong: a whole tile per
+        // consumer) or 64 rows (wide: a consumer's slice of the tile)
         CUtensorMap tc, tr;
         const uint64_t n_out = static_cast<uint64_t>(epilogue == EPI_GATED ? N / 2 : N);
-        rc = abh::make_tmap_2d_16bit(&tc, C, static_cast<uint64_t>(M), n_out, static_cast<uint64_t>(ldc), BLOCK_M, 64,
+        const uint32_t box_rows = pingpong ? BLOCK_M : 64;
+        rc = abh::make_tmap_2d_16bit(&tc, C, static_cast<uint64_t>(M), n_out, static_cast<uint64_t>(ldc), box_rows, 64,
                                      is_bf16 != 0);
         if (rc) return rc;
         if (epilogue == EPI_RESIDUAL) {
             rc = abh::make_tmap_2d_16bit(&tr, residual, static_cast<uint64_t>(M), static_cast<uint64_t>(N),
-                                         static_cast<uint64_t>(ldr), BLOCK_M, 64, is_bf16 != 0);
+                                         static_cast<uint64_t>(ldr), box_rows, 64, is_bf16 != 0);
             if (rc) return rc;
         } else {
             tr = tc;                                   // unused
+        }
+        if (!pingpong) {
+            switch (epilogue) {
+                case EPI_NONE: return launch_wide_t<EPI_NONE>(is_bf16 != 0, ta, tb, tc, tr, p, s);
+                case EPI_BIAS: return launch_wide_t<EPI_BIAS>(is_bf16 != 0, ta, tb, tc, tr, p, s);
+                case EPI_GELU: return launch_wide_t<EPI_GELU>(is_bf16 != 0, ta, tb, tc, tr, p, s);
+                case EPI_RESIDUAL: return launch_wide_t<EPI_RESIDUAL>(is_bf16 != 0, ta, tb, tc, tr, p, s);
+                case EPI_RELU: return launch_wide_t<EPI_RELU>(is_bf16 != 0, ta, tb, tc, tr, p, s);
+                default: return launch_wide_t<EPI_GATED>(is_bf16 != 0, ta, tb, tc, tr, p, s);
+            }
         }
         switch (epilogue) {
             case EPI_NONE: return launch_pp_t<EPI_NONE>(is_bf16 != 0, ta, tb, tc, tr, p, s);
@@ -765,6 +1044,10 @@ int atlas_b200_linear_ex(const void* A, int64_t lda, const void* W, int64_t ldw,
         case EPI_RELU: return launch_n<EPI_RELU>(is_bf16 != 0, wide, ta, tb, p, s);
         default: return launch_n<EPI_GATED>(is_bf16 != 0, wide, ta, tb, p, s);
     }
+}
+
+int atlas_b200_linear_schedule(int32_t M, int32_t N, int32_t K, int32_t epilogue) {
+    return gemm::select_schedule(M, N, K, epilogue, true);
 }
 
 // (tile shape, number of K splits) of a weight-gradient GEMM: minimise the number of waves of work items per split

@@ -169,6 +169,18 @@ int atlas_b200_linear_ex(const void* A, int64_t lda, const void* W, int64_t ldw,
                          int32_t epilogue, int32_t is_bf16, const float* row_ss, float* out_ss, float rs_eps,
                          void* stream);
 
+/* Which kernel schedule atlas_b200_linear / _ex / _rows run for an (M, N, K, epilogue) launch, with a 16-byte aligned
+ * residual (an unaligned one falls back to a cooperative schedule):
+ *   0  cooperative, 128 x 128 tiles       1  cooperative, 128 x 256 tiles      (decoder-sized launches)
+ *   2  ping-pong, 128 x 128 tiles         3  wide, 128 x 256 tiles, TMA-store  (encoder-sized launches)
+ * The environment variable ATLAS_B200_GEMM_SCHEDULE=pingpong|wide (read once per process) forces one of the two
+ * encoder-sized schedules wherever either may run, to time them against each other. */
+#define ATLAS_B200_GEMM_COOPERATIVE_128 0
+#define ATLAS_B200_GEMM_COOPERATIVE_256 1
+#define ATLAS_B200_GEMM_PINGPONG 2
+#define ATLAS_B200_GEMM_WIDE 3
+int atlas_b200_linear_schedule(int32_t M, int32_t N, int32_t K, int32_t epilogue);
+
 /* Row-wise normalisation of 16-bit activations (csrc/elementwise.cu), one rounding point per torch op:
  *   kind 0  BertLayerNorm (src/modeling_bert.py:104-114): y = w * r16((x - mean) * rsqrt(mean(x^2) + eps)) + b
  *           — note the UNCENTRED second moment; callers pass the residual sum already rounded to 16 bits.

@@ -117,6 +117,53 @@ elif what == "gemm_small":
         fl = 2 * m * N * K
         print(f"gemm {name:12s} M={m} N={N} K={K}: {ms * 1e3:.1f} us = {fl / ms / 1e9:.0f} TFLOP/s   cuBLAS plain: "
               f"{ms_ref * 1e3:.1f} us = {fl / ms_ref / 1e9:.0f} TFLOP/s")
+elif what == "gemm_sched":
+    # every encoder-sized GEMM shape of the bench step and of the index refresh, timed on the schedule the rule picks and on
+    # both encoder-sized schedules forced (ATLAS_B200_GEMM_SCHEDULE, read once per process: one child process each)
+    import subprocess
+    for force in ("", "pingpong", "wide"):
+        env = dict(os.environ, ATLAS_B200_GEMM_SCHEDULE=force)
+        print(f"-- schedule: {force or 'selected by the rule'}", flush=True)
+        subprocess.run([sys.executable, os.path.abspath(__file__), "gemm_sched1", str(reps)], env=env, check=True)
+elif what == "gemm_sched1":
+    # one process of gemm_sched: each shape at its bench size (8 queries x 40 passages x 384 tokens = 122,880 rows; the
+    # packed encoder's launches run over the first `count` of them, a device-side row count) with its fused epilogue, the
+    # schedule atlas_b200_linear_schedule reports for it, and cuBLAS plain on the same rows; then the mainloop alone
+    # (K = 4096, plain epilogue), all timed inside CUDA graphs
+    from atlas_b200._lib import lib
+    names = {0: "coop128", 1: "coop256", 2: "pingpong", 3: "wide"}
+    S, L = 320, 384
+    lens = torch.randint(148, 277, (S,), device=dev)
+    mask = (torch.arange(L, device=dev)[None, :] >= lens[:, None]).float() * -10000.0
+    count = ops.segment_tile_scan(ops.key_block_live(mask))[3]
+    rows = int(count)
+    for name, M, N, K, epi in (("qkv", S * L, 2304, 768, "rows"), ("o-proj+res", S * L, 768, 768, "res"),
+                               ("wi gated", S * L, 4096, 768, "gated"), ("wo+res+ss", S * L, 768, 2048, "res_ss"),
+                               ("cross K|V", S * L, 1536, 768, "dynm"), ("qkv+bias", S * L, 2304, 768, "bias"),
+                               ("wi+gelu", S * L, 3072, 768, "gelu"), ("wi+relu", S * L, 3072, 768, "relu"),
+                               ("mainloop", 61440, 2304, 4096, None)):
+        x = torch.randn(M, K, device=dev).bfloat16() * 0.1
+        w = torch.randn(N, K, device=dev).bfloat16() * 0.03
+        b = torch.randn(N, device=dev).bfloat16() * 0.1
+        r = torch.randn(M, N, device=dev).bfloat16() if epi in ("res", "res_ss") else None
+        ss = torch.zeros(M, device=dev)
+        e = {"gated": ops.EPI_GATED, "res": ops.EPI_RESIDUAL, "res_ss": ops.EPI_RESIDUAL, "bias": ops.EPI_BIAS,
+             "gelu": ops.EPI_GELU, "relu": ops.EPI_RELU}.get(epi, ops.EPI_NONE)
+        if epi == "dynm":
+            fn = lambda: ops.linear_dynm(x, w, count)
+        elif epi is None:
+            fn = lambda: ops.linear(x, w)
+        else:
+            fn = lambda: ops.linear(x, w, b if epi in ("bias", "gelu", "relu") else None, residual=r, epilogue=e,
+                                    out_ss=ss if epi == "res_ss" else None, rows=count)
+        m = M if epi is None else rows
+        sched = names[lib().atlas_b200_linear_schedule(M, N, K, e)]
+        ms = graph_timed(fn, n=5, reps=reps)
+        xm, wt = x[:m], w.t().contiguous()
+        ms_ref = graph_timed(lambda: torch.matmul(xm, wt), n=5, reps=reps)
+        fl = 2 * m * N * K
+        print(f"gemm {name:11s} M={m} N={N} K={K} {sched:8s}: {ms * 1e3:.1f} us = {fl / ms / 1e9:.0f} TFLOP/s   "
+              f"cuBLAS plain: {ms_ref * 1e3:.1f} us = {fl / ms_ref / 1e9:.0f} TFLOP/s", flush=True)
 elif what == "mips":
     # one 256-query top-40 search over a 4 Mi x 768 fp16 bank (BASELINE configs[1]): for `ncu --metrics gpu__time_duration.sum`
     n, nq, k = 4 * 1024 * 1024, 256, 40
