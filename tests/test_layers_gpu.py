@@ -90,104 +90,6 @@ def test_masked_mean_pool_into_bank_rows(dev):
     assert float(bank[:4].abs().max()) == 0 and float(bank[4 + B:].abs().max()) == 0
 
 
-def _attn_ref(qkv, B, H, L, add_mask, bias_delta, scale, causal_value):
-    """fp32 reference: scores = scale*QK^T + bias + mask, softmax, PV (inputs are the 16-bit values)."""
-    d = 64
-    q = qkv[:, : H * d].float().view(B, L, H, d).permute(0, 2, 1, 3)
-    k = qkv[:, H * d: 2 * H * d].float().view(B, L, H, d).permute(0, 2, 1, 3)
-    v = qkv[:, 2 * H * d:].float().view(B, L, H, d).permute(0, 2, 1, 3)
-    s = torch.matmul(q, k.transpose(-1, -2)) * scale
-    if bias_delta is not None:
-        i = torch.arange(L, device=qkv.device)
-        idx = i[None, :] - i[:, None] + (L - 1)              # [i, j] -> j - i + L - 1
-        s = s + bias_delta[:, idx][None]
-    if add_mask is not None:
-        s = s + add_mask[:, None, None, :]
-    if causal_value != 0.0:
-        i = torch.arange(L, device=qkv.device)
-        s = s + (i[None, :] > i[:, None]).float() * causal_value
-    p = torch.softmax(s, dim=-1)
-    return torch.matmul(p, v).permute(0, 2, 1, 3).reshape(B * L, H * d)
-
-
-@pytest.mark.parametrize("dtype", [torch.float16, torch.bfloat16])
-@pytest.mark.parametrize("B,H,L,mode", [(3, 12, 384, "t5enc"), (2, 12, 128, "bert"), (5, 12, 173, "bert"),
-                                        (2, 12, 512, "bert"), (4, 12, 32, "t5dec"), (1, 32, 384, "t5enc")])
-def test_attention_matches_fp32_reference(dev, dtype, B, H, L, mode):
-    from atlas_b200 import ops
-
-    g = torch.Generator(device="cpu").manual_seed(B * 100 + L)
-    qkv = (torch.randn(B * L, 3 * H * 64, generator=g) * (0.35 if mode == "bert" else 0.12)).to(dtype).to(dev)
-    lens = torch.randint(max(1, L // 3), L + 1, (B,), generator=g)
-    keep = (torch.arange(L)[None] < lens[:, None]).float().to(dev)
-    add_mask = (1.0 - keep) * -10000.0
-    bias = None
-    scale, causal = 1.0, 0.0
-    if mode == "bert":
-        scale = 1.0 / 8.0
-    else:
-        bias = (torch.randn(H, 2 * L - 1, generator=g) * 0.5).to(dev)
-    if mode == "t5dec":
-        causal = -10000.0
-    out = ops.attention(qkv, 0, qkv, H * 64, qkv, 2 * H * 64, B, H, L, L, add_mask=add_mask, bias_delta=bias, scale=scale,
-                        causal_value=causal)
-    ref = _attn_ref(qkv, B, H, L, add_mask, bias, scale, causal)
-    err = (out.float() - ref).abs()
-    tol = 2e-3 if dtype == torch.float16 else 1.2e-2   # P and O are rounded to the 16-bit type (8 / 11 mantissa bits)
-    assert float(err.max()) <= tol * max(1.0, float(ref.abs().max())), float(err.max())
-    # valid rows only matter, but every row must be finite
-    assert torch.isfinite(out.float()).all()
-
-
-@pytest.mark.parametrize("dtype", [torch.float16, torch.bfloat16])
-@pytest.mark.parametrize("B,H,L,mode", [(3, 12, 384, "nomask"), (2, 4, 200, "causal"), (2, 12, 384, "ramp"),
-                                        (3, 12, 256, "bert_nomask"), (37, 12, 384, "t5enc"), (2, 12, 480, "t5enc")])
-def test_attention_lanes_kernel_cases(dev, dtype, B, H, L, mode):
-    """The attention kernel (csrc/attention.cu) with >= 2 query tiles per segment on the cases the generic test does not
-    reach: no key mask at all (the bench's shape), causal + bias with several query tiles, a bias RAMP that makes every
-    later key block exceed the lazy reference maximum by more than 2^8 (the in-place rescale of O runs on every block),
-    more (segment, head) items than SMs x 3 with the bias table changing inside a CTA's item range, and 5 key blocks."""
-    from atlas_b200 import ops
-
-    g = torch.Generator(device="cpu").manual_seed(B * 1000 + L + len(mode))
-    bert = mode.startswith("bert")
-    qkv = (torch.randn(B * L, 3 * H * 64, generator=g) * (0.35 if bert else 0.12)).to(dtype).to(dev)
-    add_mask, bias, scale, causal = None, None, 1.0, 0.0
-    if mode in ("t5enc", "ramp", "causal"):
-        lens = torch.randint(max(1, L // 3), L + 1, (B,), generator=g)
-        add_mask = ((1.0 - (torch.arange(L)[None] < lens[:, None]).float()) * -10000.0).to(dev)
-    if bert:
-        scale = 1.0 / 8.0
-    else:
-        bias = (torch.randn(H, 2 * L - 1, generator=g) * 0.5)
-        if mode == "ramp":
-            bias = bias + 0.15 * torch.arange(2 * L - 1)[None, :].float()      # +14 (natural log units) per 96-key block
-        bias = bias.to(dev)
-    if mode == "causal":
-        causal = -10000.0
-    out, lse = ops.attention(qkv, 0, qkv, H * 64, qkv, 2 * H * 64, B, H, L, L, add_mask=add_mask, bias_delta=bias,
-                             scale=scale, causal_value=causal, return_lse=True)
-    ref = _attn_ref(qkv, B, H, L, add_mask, bias, scale, causal)
-    err = (out.float() - ref).abs()
-    tol = 2e-3 if dtype == torch.float16 else 1.2e-2
-    assert torch.isfinite(out.float()).all()
-    assert float(err.max()) <= tol * max(1.0, float(ref.abs().max())), float(err.max())
-    # the saved log-sum-exp (backward pass input) against the fp32 scores
-    d = 64
-    q = qkv[:, : H * d].float().view(B, L, H, d).permute(0, 2, 1, 3)
-    k = qkv[:, H * d: 2 * H * d].float().view(B, L, H, d).permute(0, 2, 1, 3)
-    s = torch.matmul(q, k.transpose(-1, -2)) * scale
-    if bias is not None:
-        idx = torch.arange(L, device=dev)[None, :] - torch.arange(L, device=dev)[:, None] + (L - 1)
-        s = s + bias[:, idx][None]
-    if add_mask is not None:
-        s = s + add_mask[:, None, None, :]
-    if causal != 0.0:
-        i = torch.arange(L, device=dev)
-        s = s + (i[None, :] > i[:, None]).float() * causal
-    assert float((lse - torch.logsumexp(s, dim=-1)).abs().max()) <= 2e-3
-
-
 def test_fp16_inf_clamp(dev):
     """ops.clamp_inf_ = the reference's `if dtype == fp16 and isinf(h).any(): h = clamp(h, +-(65504 - 1000))`
     (src/modeling_t5.py:657-708) decided on the device: untouched without an inf, torch.clamp's values with one."""
@@ -251,8 +153,9 @@ def test_fid_fp16_overflow_is_clamped_like_the_reference(dev):
 @pytest.mark.parametrize("dtype", [torch.bfloat16, torch.float16])
 @pytest.mark.parametrize("B,H,T,Lk", [(2, 3, 32, 4000), (1, 12, 7, 15360), (3, 2, 64, 1088), (2, 1, 1, 2048)])
 def test_cross_attention_stream_kernel(dev, dtype, B, H, T, Lk):
-    """csrc/attention_stream.cu (few target tokens against the concatenated encoder keys, src/fid.py:298-349): against an fp32
-    restatement, ragged key counts, masked keys, and against the split-KV path where that one applies."""
+    """csrc/attention_stream.cu (few target tokens against the concatenated encoder keys, src/fid.py:298-349): skipping the
+    fully masked 64-key tiles does not change a bit, with ragged key counts and a long fully masked tail.  The values are
+    held against the fp64 oracle in tests/test_attention_fwd_gpu.py (test_stream_kernel, same shapes)."""
     from atlas_b200 import ops
 
     g = torch.Generator().manual_seed(B * 1000 + T)
@@ -264,30 +167,14 @@ def test_cross_attention_stream_kernel(dev, dtype, B, H, T, Lk):
     neg = -1e4 if dtype == torch.float16 else -1e9
     mask = ((~valid).float() * neg).to(dev)
     assert ops._XATTN_STREAM
-    out, lse = ops.cross_attention_split(q, 0, kv, 0, H * 64, B, H, T, Lk, add_mask=mask, scale=1.0, split=Lk, return_lse=True)
-    qf = q.float().reshape(B, T, H, 64)
-    kf, vf = (t.reshape(B, Lk, H, 64) for t in kv.float().split(H * 64, dim=1))
-    s = torch.einsum("bihd,bjhd->bhij", qf, kf) + mask[:, None, None, :]
-    ref = torch.einsum("bhij,bjhd->bihd", torch.softmax(s, -1), vf).reshape(B * T, H * 64)
-    tol = 2e-2 if dtype == torch.bfloat16 else 3e-3
-    err = float((out.float() - ref).abs().max())
-    assert err <= tol * max(1.0, float(ref.abs().max())), err
-    assert torch.allclose(lse, torch.logsumexp(s, -1), rtol=1e-3, atol=2e-3)
-    # skipping the fully masked 64-key tiles (the default above) does not change a bit
+    out = ops.cross_attention_split(q, 0, kv, 0, H * 64, B, H, T, Lk, add_mask=mask, scale=1.0, split=Lk)
+    assert torch.isfinite(out.float()).all()
     ops._SKIP_MASKED = False
     try:
         full = ops.cross_attention_split(q, 0, kv, 0, H * 64, B, H, T, Lk, add_mask=mask, scale=1.0, split=Lk)
     finally:
         ops._SKIP_MASKED = True
     assert torch.equal(full, out)
-    split = next((x for x in range(384, 63, -1) if Lk % x == 0), None)
-    if split is not None:
-        ops._XATTN_STREAM = False
-        try:
-            old = ops.cross_attention_split(q, 0, kv, 0, H * 64, B, H, T, Lk, add_mask=mask, scale=1.0, split=split)
-        finally:
-            ops._XATTN_STREAM = True
-        assert float((old.float() - out.float()).abs().max()) <= tol * max(1.0, float(ref.abs().max()))
 
 
 @pytest.mark.parametrize("dtype", [torch.bfloat16, torch.float16])
@@ -295,7 +182,8 @@ def test_cross_attention_stream_kernel(dev, dtype, B, H, T, Lk):
 def test_masked_key_blocks_are_skipped_without_changing_the_result(dev, dtype, S, H, L, use_bias):
     """ops.key_block_live: 64-key blocks made of masked keys only (padding to text_maxlength) are neither loaded nor computed
     by the attention kernel.  Their softmax weights are exactly 0 in fp32, so the output must be BIT-identical to
-    the run that computes every block - and equal to the fp32 restatement."""
+    the run that computes every block.  The values are held against the fp64 oracle in tests/test_attention_fwd_gpu.py
+    (test_masked_segments_and_holes, same shapes)."""
     from atlas_b200 import ops
 
     g = torch.Generator().manual_seed(S * 100 + L)
@@ -311,15 +199,7 @@ def test_masked_key_blocks_are_skipped_without_changing_the_result(dev, dtype, S
     a = ops.attention(qkv, 0, qkv, H * 64, qkv, 2 * H * 64, S, H, L, L, add_mask=mask, bias_delta=bias, block_live=live)
     b = ops.attention(qkv, 0, qkv, H * 64, qkv, 2 * H * 64, S, H, L, L, add_mask=mask, bias_delta=bias)
     assert torch.equal(a, b), float((a.float() - b.float()).abs().max())
-    q, k, v = (t.float().reshape(S, L, H, 64) for t in qkv.split(H * 64, dim=1))
-    s = torch.einsum("bihd,bjhd->bhij", q, k) + mask[:, None, None, :]
-    if use_bias:
-        i = torch.arange(L, device=dev)[:, None]
-        j = torch.arange(L, device=dev)[None, :]
-        s = s + bias[:, (j - i + L - 1)][None]
-    ref = torch.einsum("bhij,bjhd->bihd", torch.softmax(s, -1), v).reshape(S * L, H * 64)
-    tol = 2e-2 if dtype == torch.bfloat16 else 3e-3
-    assert float((a.float() - ref).abs().max()) <= tol * max(1.0, float(ref.abs().max()))
+    assert torch.isfinite(a.float()).all()
     # a fully masked segment keeps every block (uniform-over-masked-keys softmax like the reference)
     allm = torch.full((2, L), -10000.0, device=dev)
     assert bool(ops.key_block_live(allm).all())
