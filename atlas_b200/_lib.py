@@ -159,6 +159,9 @@ def lib():
     L.atlas_b200_attention_train.restype = c.c_int
     L.atlas_b200_attention_train.argtypes = [vp, i64, i32, vp, i64, i32, vp, i64, i32, vp, i64, vp, vp, i32, i32, i32, i32,
                                              f32, f32, i32, vp, vp, vp, f32, u64, u64, vp, i32, vp]
+    L.atlas_b200_attention_long.restype = c.c_int
+    L.atlas_b200_attention_long.argtypes = [vp, i64, i32, vp, i64, i32, vp, i64, i32, vp, i64, vp, vp, i32, i32, i32, i32, f32,
+                                            f32, vp, f32, u64, u64, vp, i32, vp]
     L.atlas_b200_attention_bwd_train.restype = c.c_int
     L.atlas_b200_attention_bwd_train.argtypes = [vp, i64, i32, vp, i64, i32, vp, i64, i32, vp, i64, vp, i64, vp, i64, i32,
                                                  vp, i64, i32, vp, i64, i32, vp, vp, vp, vp, i32, vp, vp, i32, i32, i32,
@@ -264,6 +267,7 @@ EXPORTED_SYMBOLS = [
     "atlas_b200_dropout_mask",
     "atlas_b200_attention_dropout_mask",
     "atlas_b200_attention_train",
+    "atlas_b200_attention_long",
     "atlas_b200_attention_bwd_train",
     "atlas_b200_adamw_fp32copy",
     "atlas_b200_grad_stats",

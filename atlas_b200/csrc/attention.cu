@@ -16,6 +16,12 @@
 // (flash-attention) softmax in the log2 domain.  Key blocks whose keys are all masked out (key_block_live) are skipped: their
 // probabilities are exactly 0 in fp32.
 //
+// Segments of 577 to 4096 keys (the FiD encoder on long passages) run on attention_long_kernel below: the same per-block
+// arithmetic, with K and V streamed through a ring of shared-memory slots instead of held resident.  Its per-block code
+// (attend_block) is a copy of attention_kernel's loop body rather than shared with it: calling one inlined function from both
+// kernels changes how ptxas allocates attention_kernel (124 -> 122 registers, different SASS), so attention_kernel keeps
+// its own loop and stays instruction-for-instruction what it was.
+//
 // Packed layout (seg_tile != nullptr, the padding-compacted FiD encoder): segment b keeps the first popcount(blk_live[b, :]) of
 // its 64-row tiles, stored back to back from row 64 * seg_tile[b * nb] of q / k / v / out; query tiles past them do not exist.
 #include "common.cuh"
@@ -70,6 +76,104 @@ __device__ __forceinline__ float ex2_approx(float x) {
     float y;
     asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
     return y;
+}
+
+// attention_long_kernel's step over one live 64-key block kb, the loop body of attention_kernel (see the header): for this
+// thread's query rows i0 and i0 + 8 (warpgroup g of the 128-row tile at sQ; the block's K and V in slot `slot` of sK / sV),
+// S = Q K^T, t = S * scale2 + mask + bias in the log2 domain, the online-softmax update of (m_run, l_run, o) and O += P V
+// with P from registers.  s_mask is indexed by key, s_bias by key - min(i, Lq - 1) + bias_off.
+template <bool kBF16>
+__device__ __forceinline__ void attend_block(float (&o)[32], float (&m_run)[2], float (&l_run)[2], const uint32_t sQ,
+                                             const uint32_t g, const uint32_t sK, const uint32_t sV, const int slot,
+                                             const float* s_mask, const float* s_bias,
+                                             const int bias_off, const bool has_bias, const int kb, const int i0, const int cq,
+                                             const float scale2, const bool dropping, const Params& p, const int b, const int h,
+                                             const uint32_t lane) {
+    float sc[32];
+    ab::wgmma_fence();
+#pragma unroll
+    for (int k = 0; k < D / 16; ++k) {
+        const uint64_t adesc = ab::wgmma_desc_sw128(sQ + g * 8192u + k * 32u);
+        const uint64_t bdesc = ab::wgmma_desc_sw128(sK + slot * TILE_BYTES + k * 32u);
+        ab::wgmma_m64n64k16_ss<kBF16, 0, 0>(sc, adesc, bdesc, k);
+    }
+    ab::wgmma_commit();
+    ab::wgmma_wait<0>();
+    ab::wgmma_reg_fence(sc);
+
+    // t = S * scale2 + (mask + bias) in the log2 domain; new row maxima
+    float mx[2] = {m_run[0], m_run[1]};
+#pragma unroll
+    for (int j = 0; j < 8; ++j) {
+#pragma unroll
+        for (int c = 0; c < 2; ++c) {
+            const int key = kb * BK + 8 * j + cq + c;
+            const float mk = s_mask[key];
+#pragma unroll
+            for (int hh = 0; hh < 2; ++hh) {
+                float a = mk;
+                if (has_bias) a += s_bias[key - min(i0 + 8 * hh, p.Lq - 1) + bias_off];   // rows past Lq are not stored
+                const float t = fmaf(sc[4 * j + 2 * hh + c], scale2, a);
+                sc[4 * j + 2 * hh + c] = t;
+                mx[hh] = fmaxf(mx[hh], t);
+            }
+        }
+    }
+    float corr[2], base[2];
+#pragma unroll
+    for (int hh = 0; hh < 2; ++hh) {
+        mx[hh] = fmaxf(mx[hh], __shfl_xor_sync(0xffffffffu, mx[hh], 1));
+        mx[hh] = fmaxf(mx[hh], __shfl_xor_sync(0xffffffffu, mx[hh], 2));
+        base[hh] = mx[hh] == -INFINITY ? 0.f : mx[hh];
+        corr[hh] = ex2_approx(m_run[hh] - base[hh]);     // 0 for the first block (m_run = -inf)
+        m_run[hh] = mx[hh];
+        l_run[hh] *= corr[hh];
+    }
+#pragma unroll
+    for (int j = 0; j < 8; ++j) {
+        o[4 * j] *= corr[0];
+        o[4 * j + 1] *= corr[0];
+        o[4 * j + 2] *= corr[1];
+        o[4 * j + 3] *= corr[1];
+    }
+    // p = 2^(t - m); the row sum takes every probability, the P operand only the kept ones (dropout)
+    uint32_t pa[16];
+#pragma unroll
+    for (int hh = 0; hh < 2; ++hh) {
+        uint32_t w[2][4];
+        if (dropping) {
+            const uint64_t R = (static_cast<uint64_t>(b / p.q_div) * p.H + h) * p.Lq + min(i0 + 8 * hh, p.Lq - 1);
+#pragma unroll
+            for (int gg = 0; gg < 2; ++gg) {
+                const uint32_t G = static_cast<uint32_t>(((b % p.q_div) * p.Lk + kb * BK + gg * 32) >> 5);
+                abdrop::attn_words(p.drop, R, G, static_cast<uint32_t>(lane & 3u), w[gg]);
+            }
+        }
+#pragma unroll
+        for (int j = 0; j < 8; ++j) {
+            const float e0 = ex2_approx(sc[4 * j + 2 * hh] - base[hh]);
+            const float e1 = ex2_approx(sc[4 * j + 2 * hh + 1] - base[hh]);
+            l_run[hh] += e0 + e1;
+            float k0 = e0, k1 = e1;
+            if (dropping) {
+                const uint32_t word = w[j >> 2][j & 3];
+                k0 = abdrop::keep_lo(p.drop, word) ? e0 : 0.f;
+                k1 = abdrop::keep_hi(p.drop, word) ? e1 : 0.f;
+            }
+            // A fragment of k16 step j / 2: a0 = (r, keys 0-7), a1 = (r + 8, keys 0-7), a2 / a3 = keys 8-15
+            pa[4 * (j >> 1) + 2 * (j & 1) + hh] = pack2<kBF16>(k0, k1);
+        }
+    }
+    ab::wgmma_fence();
+#pragma unroll
+    for (int k = 0; k < BK / 16; ++k) {
+        const uint32_t a[4] = {pa[4 * k], pa[4 * k + 1], pa[4 * k + 2], pa[4 * k + 3]};
+        const uint64_t bdesc = ab::wgmma_desc_sw128(sV + slot * TILE_BYTES + k * 2048u, 8192);
+        ab::wgmma_m64n64k16_rs<kBF16, 1>(o, a, bdesc, 1);
+    }
+    ab::wgmma_commit();
+    ab::wgmma_wait<0>();
+    ab::wgmma_reg_fence(o);
 }
 
 // grid = (query tiles, H, B)
@@ -280,18 +384,178 @@ attention_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_consta
     }
 }
 
+// ---- attention_long_kernel: the same contract for Lk up to LONG_MAX_LK keys (no split-KV partials, no packed layout).  K and V
+// stream through a LONG_STAGES-deep ring of 64-key tiles: one producer warp issues their TMA loads (full / empty mbarriers),
+// the two consumer warpgroups of attention_kernel sweep the live blocks with attend_block.  The CTA's slice of the bias table
+// (offsets of its 128 query rows to every key) and the key mask are staged in shared memory once.
+constexpr int LONG_MAX_LK = 4096;              // Lq + Lk - 1 <= 8192: the bias table of the backward (attention_bwd.cu)
+constexpr int LONG_STAGES = 4;
+constexpr int LONG_THREADS = THREADS + 32;     // two consumer warpgroups + one producer warp
+constexpr int LONG_BIAS = LONG_MAX_LK + BQ;    // >= (keys rounded up to 64) + 127 offsets
+constexpr int LONG_SMEM_BYTES = 1024 + Q_BYTES + 2 * LONG_STAGES * TILE_BYTES + (LONG_MAX_LK + LONG_BIAS) * 4;
+
+// grid = (query tiles, H, B)
 template <bool kBF16>
-static int launch(const void* q, int64_t ldq, const void* k, int64_t ldk, const void* v, int64_t ldv, int q_rows, int k_rows,
-                  const Params& p, cudaStream_t s) {
-    CUtensorMap tq, tk, tv;
+__global__ void __launch_bounds__(LONG_THREADS, 1)
+attention_long_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ CUtensorMap tmap_k,
+                      const __grid_constant__ CUtensorMap tmap_v, const Params p) {
+    extern __shared__ uint8_t smem_raw[];
+    __shared__ __align__(8) uint64_t q_bar, full_bar[LONG_STAGES], empty_bar[LONG_STAGES];
+    __shared__ uint8_t s_live[LONG_MAX_LK / BK];
+
+    const int qt = blockIdx.x, h = blockIdx.y, b = blockIdx.z;
+    const uint32_t warp = threadIdx.x >> 5;
+    const uint32_t lane = threadIdx.x & 31u;
+    const uint32_t smem_base = (ab::smem_u32(smem_raw) + 1023u) & ~1023u;
+    uint8_t* smem_gen = smem_raw + (smem_base - ab::smem_u32(smem_raw));
+    // Q | K ring | V ring | key mask | bias slice
+    const uint32_t sQ = smem_base, sK = smem_base + Q_BYTES, sV = sK + LONG_STAGES * TILE_BYTES;
+    float* s_mask = reinterpret_cast<float*>(smem_gen + Q_BYTES + 2 * LONG_STAGES * TILE_BYTES);
+    float* s_bias = s_mask + LONG_MAX_LK;
+
+    const int nkb = (p.Lk + BK - 1) / BK;
+    const bool producer = warp == THREADS / 32;
+    if (threadIdx.x == 0) {
+        ab::mbar_init(&q_bar, 1);
+        for (int s = 0; s < LONG_STAGES; ++s) {
+            ab::mbar_init(&full_bar[s], 1);
+            ab::mbar_init(&empty_bar[s], THREADS / 32);     // one arrival per consumer warp
+        }
+        ab::fence_barrier_init();
+    }
+    // live key blocks; none flagged live = all live
+    bool lv = false;
+    if (static_cast<int>(threadIdx.x) < nkb) {
+        lv = p.blk_live == nullptr || __ldg(p.blk_live + static_cast<size_t>(b) * nkb + threadIdx.x) != 0;
+        s_live[threadIdx.x] = lv;
+    }
+    const bool all_live = __syncthreads_or(lv) == 0;
+
+    // producer: the query tile, then the live K / V blocks; the first LONG_STAGES go out before the tables are staged
+    int next_kb = 0, n_issued = 0;
+    auto produce = [&](int max_issued) {
+        for (; next_kb < nkb && n_issued < max_issued; ++next_kb) {
+            if (!all_live && !s_live[next_kb]) continue;
+            const int s = n_issued % LONG_STAGES;
+            if (n_issued >= LONG_STAGES) ab::mbar_wait(&empty_bar[s], ((n_issued / LONG_STAGES) & 1) ^ 1, 51);
+            ab::mbar_arrive_expect_tx(&full_bar[s], static_cast<uint32_t>(2 * TILE_BYTES));
+            const int row = b * p.Lk + next_kb * BK;
+            ab::tma_load_2d(&tmap_k, &full_bar[s], smem_gen + Q_BYTES + s * TILE_BYTES, p.k_col0 + h * D, row,
+                            ab::kEvictNormal);
+            ab::tma_load_2d(&tmap_v, &full_bar[s], smem_gen + Q_BYTES + (LONG_STAGES + s) * TILE_BYTES, p.v_col0 + h * D,
+                            row, ab::kEvictNormal);
+            ++n_issued;
+        }
+    };
+    if (producer && lane == 0) {
+        ab::tma_prefetch_desc(&tmap_q);
+        ab::mbar_arrive_expect_tx(&q_bar, static_cast<uint32_t>(2 * TILE_BYTES));
+        for (int t = 0; t < 2; ++t)
+            ab::tma_load_2d(&tmap_q, &q_bar, smem_gen + t * TILE_BYTES, p.q_col0 + h * D, b * p.Lq + qt * BQ + t * BK,
+                            ab::kEvictFirst);
+        produce(LONG_STAGES);
+    }
+    // mask and the bias slice: offsets d_lo .. d_lo + 64 nkb + 126 of the [H, Lq + Lk - 1] table, d_lo = that of the tile's
+    // last (clamped) row to key 0; entries past the valid offsets stay finite (0)
+    const bool has_bias = (p.bias_delta != nullptr) || (p.causal_value != 0.f);
+    for (int j = threadIdx.x; j < nkb * BK; j += LONG_THREADS)
+        s_mask[j] = (j < p.Lk) ? (p.add_mask ? p.add_mask[static_cast<size_t>(b) * p.Lk + j] * LOG2E : 0.f) : -INFINITY;
+    const int bias_off = min(qt * BQ + BQ - 1, p.Lq - 1);
+    if (has_bias) {
+        const int n_valid = p.Lq + p.Lk - 1;
+        const int d_lo = (p.Lq - 1) - bias_off;
+        for (int t = threadIdx.x; t < nkb * BK + BQ - 1; t += LONG_THREADS) {
+            const int d = d_lo + t;
+            float v = 0.f;
+            if (d < n_valid) {
+                v = p.bias_delta ? p.bias_delta[static_cast<size_t>(h) * n_valid + d] : 0.f;
+                if (p.causal_value != 0.f && d > p.Lq - 1) v += p.causal_value;   // j > i
+            }
+            s_bias[t] = v * LOG2E;
+        }
+    }
+    __syncthreads();
+    if (producer) {
+        if (lane == 0) produce(nkb);
+        return;
+    }
+    ab::mbar_wait(&q_bar, 0, 50);
+
+    const uint32_t g = warp >> 2, wl = warp & 3u;
+    const int i0 = qt * BQ + static_cast<int>(g * 64u + wl * 16u + (lane >> 2));
+    const int cq = static_cast<int>(2u * (lane & 3u));
+    const float scale2 = p.scale * LOG2E;
+    const bool dropping = p.drop.thr16 != 0u;
+    float o[32];
+#pragma unroll
+    for (int x = 0; x < 32; ++x) o[x] = 0.f;
+    float m_run[2] = {-INFINITY, -INFINITY}, l_run[2] = {0.f, 0.f};
+
+    int n_used = 0;
+    for (int kb = 0; kb < nkb; ++kb) {
+        if (!all_live && !s_live[kb]) continue;
+        const int s = n_used % LONG_STAGES;
+        ab::mbar_wait(&full_bar[s], (n_used / LONG_STAGES) & 1, 52);
+        attend_block<kBF16>(o, m_run, l_run, sQ, g, sK, sV, s, s_mask, s_bias, bias_off, has_bias, kb, i0, cq, scale2,
+                            dropping, p, b, h, lane);
+        __syncwarp();
+        if (lane == 0) ab::mbar_arrive(&empty_bar[s]);     // this warp's MMAs on the slot have completed
+        ++n_used;
+    }
+
+#pragma unroll
+    for (int hh = 0; hh < 2; ++hh) {
+        float l = l_run[hh];
+        l += __shfl_xor_sync(0xffffffffu, l, 1);
+        l += __shfl_xor_sync(0xffffffffu, l, 2);
+        const int i = i0 + 8 * hh;
+        if (i >= p.Lq) continue;
+        const float inv = p.drop.inv_keep / l;
+        if (p.lse_out != nullptr && (lane & 3u) == 0u)
+            p.lse_out[(static_cast<size_t>(b) * p.H + h) * p.Lq + i] = m_run[hh] * (1.0f / LOG2E) + __logf(l);
+        uint16_t* dst = p.O + (static_cast<size_t>(b) * p.Lq + i) * p.ldo + h * D + cq;
+#pragma unroll
+        for (int j = 0; j < 8; ++j)
+            *reinterpret_cast<uint32_t*>(dst + 8 * j) = pack2<kBF16>(o[4 * j + 2 * hh] * inv, o[4 * j + 2 * hh + 1] * inv);
+    }
+}
+
+template <bool kBF16>
+static int make_tmaps(CUtensorMap& tq, CUtensorMap& tk, CUtensorMap& tv, const void* q, int64_t ldq, const void* k, int64_t ldk,
+                      const void* v, int64_t ldv, int q_rows, int k_rows, const Params& p) {
     int rc = abh::make_tmap_2d_16bit(&tq, q, static_cast<uint64_t>(q_rows), static_cast<uint64_t>(p.q_col0 + p.H * D),
                                      static_cast<uint64_t>(ldq), BK, D, kBF16);
     if (rc) return rc;
     rc = abh::make_tmap_2d_16bit(&tk, k, static_cast<uint64_t>(k_rows), static_cast<uint64_t>(p.k_col0 + p.H * D),
                                  static_cast<uint64_t>(ldk), BK, D, kBF16);
     if (rc) return rc;
-    rc = abh::make_tmap_2d_16bit(&tv, v, static_cast<uint64_t>(k_rows), static_cast<uint64_t>(p.v_col0 + p.H * D),
-                                 static_cast<uint64_t>(ldv), BK, D, kBF16);
+    return abh::make_tmap_2d_16bit(&tv, v, static_cast<uint64_t>(k_rows), static_cast<uint64_t>(p.v_col0 + p.H * D),
+                                   static_cast<uint64_t>(ldv), BK, D, kBF16);
+}
+
+template <bool kBF16>
+static int launch_long(const void* q, int64_t ldq, const void* k, int64_t ldk, const void* v, int64_t ldv, const Params& p,
+                       cudaStream_t s) {
+    CUtensorMap tq, tk, tv;
+    const int rc = make_tmaps<kBF16>(tq, tk, tv, q, ldq, k, ldk, v, ldv, p.B * p.Lq, p.B * p.Lk, p);
+    if (rc) return rc;
+    static bool attr_set = false;
+    if (!attr_set) {
+        AB_CUDA_CHECK(cudaFuncSetAttribute(attention_long_kernel<kBF16>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                           LONG_SMEM_BYTES));
+        attr_set = true;
+    }
+    attention_long_kernel<kBF16><<<dim3(static_cast<unsigned>(p.n_qt), static_cast<unsigned>(p.H), static_cast<unsigned>(p.B)),
+                                   LONG_THREADS, LONG_SMEM_BYTES, s>>>(tq, tk, tv, p);
+    AB_CUDA_CHECK(cudaGetLastError());
+    return ATLAS_B200_OK;
+}
+
+template <bool kBF16>
+static int launch(const void* q, int64_t ldq, const void* k, int64_t ldk, const void* v, int64_t ldv, int q_rows, int k_rows,
+                  const Params& p, cudaStream_t s) {
+    CUtensorMap tq, tk, tv;
+    const int rc = make_tmaps<kBF16>(tq, tk, tv, q, ldq, k, ldk, v, ldv, q_rows, k_rows, p);
     if (rc) return rc;
     static bool attr_set = false;
     if (!attr_set) {
@@ -436,6 +700,36 @@ int atlas_b200_attention_train(const void* q, int64_t ldq, int32_t q_col0, const
     abh::prof_begin(s, abh::PROF_ATTENTION);
     const int lrc = is_bf16 ? launch<true>(q, ldq, k, ldk, v, ldv, (B / q_div) * Lq, B * Lk, p, s)
                             : launch<false>(q, ldq, k, ldk, v, ldv, (B / q_div) * Lq, B * Lk, p, s);
+    if (lrc) return lrc;
+    abh::prof_end(s, abh::PROF_ATTENTION, 4.0 * B * H * static_cast<double>(Lq) * Lk * D);
+    abh::count_launch();
+    return ATLAS_B200_OK;
+}
+
+int atlas_b200_attention_long(const void* q, int64_t ldq, int32_t q_col0, const void* k, int64_t ldk, int32_t k_col0,
+                              const void* v, int64_t ldv, int32_t v_col0, void* out, int64_t ldo, const float* add_mask,
+                              const float* bias_delta, int32_t B, int32_t H, int32_t Lq, int32_t Lk, float scale,
+                              float causal_value, float* lse_out, float dropout_p, uint64_t seed, uint64_t offset,
+                              const uint8_t* key_block_live, int32_t is_bf16, void* stream) {
+    using namespace attn;
+    AB_REQUIRE(dropout_p >= 0.f && dropout_p < 1.f, "attention_long: need 0 <= dropout_p < 1 (got %f)", dropout_p);
+    AB_REQUIRE(B >= 0 && H > 0 && Lq > 0 && Lk > 0 && Lk <= LONG_MAX_LK, "attention_long: need 0 < Lk <= %d (got Lq=%d Lk=%d)",
+               LONG_MAX_LK, Lq, Lk);
+    AB_REQUIRE(Lq + Lk - 1 <= 2 * LONG_MAX_LK, "attention_long: Lq + Lk - 1 = %d exceeds the bias table (%d)", Lq + Lk - 1,
+               2 * LONG_MAX_LK);
+    AB_REQUIRE(ldq % 8 == 0 && ldk % 8 == 0 && ldv % 8 == 0 && ldo % 8 == 0 && q_col0 % 8 == 0 && k_col0 % 8 == 0 &&
+                   v_col0 % 8 == 0,
+               "attention_long: strides and column offsets must be multiples of 8 elements");
+    AB_REQUIRE(static_cast<int64_t>(B) * Lq < (1ll << 31) && static_cast<int64_t>(B) * Lk < (1ll << 31),
+               "attention_long: more than 2^31 rows");
+    if (B == 0) return ATLAS_B200_OK;
+    Params p = base_params(B, H, Lq, Lk, q_col0, k_col0, v_col0, out, ldo, add_mask, bias_delta, scale, causal_value);
+    p.lse_out = lse_out;
+    p.drop = abdrop::make_key(dropout_p, seed, offset);
+    p.blk_live = key_block_live;
+    cudaStream_t s = static_cast<cudaStream_t>(stream);
+    abh::prof_begin(s, abh::PROF_ATTENTION);
+    const int lrc = is_bf16 ? launch_long<true>(q, ldq, k, ldk, v, ldv, p, s) : launch_long<false>(q, ldq, k, ldk, v, ldv, p, s);
     if (lrc) return lrc;
     abh::prof_end(s, abh::PROF_ATTENTION, 4.0 * B * H * static_cast<double>(Lq) * Lk * D);
     abh::count_launch();

@@ -168,6 +168,12 @@ class _GraphRunner:
         return self.static_out
 
 
+def _check_passage_length(L):
+    if L > ops.ATTENTION_LONG_MAX_LK:
+        raise AtlasB200Error(f"text_maxlength = {L} is not supported: the encoder self-attention takes passages of at most "
+                             f"{ops.ATTENTION_LONG_MAX_LK} tokens")
+
+
 class FiDOutput(tuple):
     """(loss, logits, encoder_last_hidden_state) with the attribute names Atlas reads (src/atlas.py:292-300,583-590)."""
 
@@ -420,6 +426,7 @@ class FiD(nn.Module):
         ids = input_ids.reshape(input_ids.size(0) * n_ctx, -1)
         mask = attention_mask.reshape(attention_mask.size(0) * n_ctx, -1)
         S, L = ids.shape
+        _check_passage_length(L)
         d, H = c.d_model, c.num_heads
         add_mask = (1.0 - mask.to(torch.float32)) * -10000.0                      # 4.18 get_extended_attention_mask
         # 64-key blocks made of padding only (every passage is padded to text_maxlength) weigh exactly 0 in the softmax:
@@ -438,9 +445,11 @@ class FiD(nn.Module):
         else:
             h = W["shared.weight"][ids.reshape(-1)]                              # embedding gather, [S*L, d]
 
+            fwd = ops.encoder_attention(L)
+
             def attn(qkv):
-                return ops.attention(qkv, 0, qkv, H * 64, qkv, 2 * H * 64, S, H, L, L, add_mask=add_mask, bias_delta=bias,
-                                     scale=1.0, block_live=live)
+                return fwd(qkv, 0, qkv, H * 64, qkv, 2 * H * 64, S, H, L, L, add_mask=add_mask, bias_delta=bias, scale=1.0,
+                           block_live=live)
         qkv = torch.empty((S * L, 3 * H * 64), dtype=dt, device=h.device)
         eps = c.layer_norm_epsilon
         if self.fuse_norm:
@@ -668,6 +677,7 @@ class FiD(nn.Module):
         ids = input_ids.reshape(input_ids.size(0) * n_ctx, -1)
         mask = attention_mask.reshape(attention_mask.size(0) * n_ctx, -1)
         S, L = ids.shape
+        _check_passage_length(L)
         d, H = c.d_model, c.num_heads
         eps = c.layer_norm_epsilon
         pdrop = self._dropout_p()
@@ -689,7 +699,8 @@ class FiD(nn.Module):
             p = f"encoder.block.{i}.layer.0."
             n = g.layernorm(h, W[p + "layer_norm.weight"], None, eps, kind=1)
             qkv = g.linear(n, G[p + "SelfAttention.qkv"])
-            ctx = g.self_attention(qkv, S, H, L, add_mask=add_mask, bias_delta=bias, scale=1.0, dropout_p=pdrop)
+            ctx = g.self_attention(qkv, S, H, L, add_mask=add_mask, bias_delta=bias, scale=1.0, dropout_p=pdrop,
+                                   long_segments=True)
             h = lin_res(ctx, W[p + "SelfAttention.o.weight"], h)
             p = f"encoder.block.{i}.layer.1."
             n = g.layernorm(h, W[p + "layer_norm.weight"], None, eps, kind=1)

@@ -81,11 +81,12 @@ class _SelfAttention(torch.autograd.Function):
     """qkv [B*L, 3*H*64] (q | k | v as written by the fused projection) -> ctx [B*L, H*64]."""
 
     @staticmethod
-    def forward(ctx, qkv, bias_delta, add_mask, B, H, L, scale, causal_value, dropout_p):
+    def forward(ctx, qkv, bias_delta, add_mask, B, H, L, scale, causal_value, dropout_p, long_segments):
         ctx.drop = (dropout_p,) + next_dropout_key(qkv.device) if dropout_p else None
-        out, lse = ops.attention(qkv, 0, qkv, H * 64, qkv, 2 * H * 64, B, H, L, L, add_mask=add_mask,
-                                 bias_delta=bias_delta, scale=scale, causal_value=causal_value, return_lse=True,
-                                 dropout=ctx.drop, block_live=getattr(add_mask, "_atlas_block_live", None))
+        fwd = ops.encoder_attention(L) if long_segments else ops.attention
+        out, lse = fwd(qkv, 0, qkv, H * 64, qkv, 2 * H * 64, B, H, L, L, add_mask=add_mask, bias_delta=bias_delta, scale=scale,
+                       causal_value=causal_value, return_lse=True, dropout=ctx.drop,
+                       block_live=getattr(add_mask, "_atlas_block_live", None))
         ctx.save_for_backward(qkv, out, bias_delta, add_mask, lse)
         ctx.dims = (B, H, L, scale, causal_value)
         return out
@@ -100,12 +101,15 @@ class _SelfAttention(torch.autograd.Function):
                                   need_dbias=bias_delta is not None and _need(ctx, 1), scale=scale,
                                   causal_value=causal_value, lse=lse, dropout=ctx.drop,
                                   block_live=getattr(add_mask, "_atlas_block_live", None))
-        return dqkv, dbias, None, None, None, None, None, None, None
+        return dqkv, dbias, None, None, None, None, None, None, None, None
 
 
-def self_attention(qkv, B, H, L, add_mask=None, bias_delta=None, scale=1.0, causal_value=0.0, dropout_p=0.0):
-    """dropout_p: nn.Dropout on the attention probabilities (training), inside the kernels."""
-    return _SelfAttention.apply(qkv, bias_delta, add_mask, B, H, L, scale, causal_value, float(dropout_p or 0.0))
+def self_attention(qkv, B, H, L, add_mask=None, bias_delta=None, scale=1.0, causal_value=0.0, dropout_p=0.0,
+                   long_segments=False):
+    """dropout_p: nn.Dropout on the attention probabilities (training), inside the kernels.  long_segments: segments longer
+    than ops.ATTENTION_MAX_LK run on ops.attention_long (the FiD encoder's passages; the backward takes any length)."""
+    return _SelfAttention.apply(qkv, bias_delta, add_mask, B, H, L, scale, causal_value, float(dropout_p or 0.0),
+                                long_segments)
 
 
 class _CrossAttention(torch.autograd.Function):

@@ -359,6 +359,35 @@ def attention(q, q_col0, k, k_col0, v, v_col0, B, H, Lq, Lk, add_mask=None, bias
     return (out, lse) if return_lse else out
 
 
+ATTENTION_MAX_LK = 576          # keys per segment of `attention` (its K and V stay resident in shared memory)
+ATTENTION_LONG_MAX_LK = 4096    # ... of `attention_long`; Lq + Lk - 1 <= 8192 as well (the bias table of attention_bwd)
+
+
+def attention_long(q, q_col0, k, k_col0, v, v_col0, B, H, Lq, Lk, add_mask=None, bias_delta=None, scale=1.0,
+                   causal_value=0.0, out=None, return_lse=False, dropout=None, block_live=None):
+    """`attention` for key ranges up to ATTENTION_LONG_MAX_LK: K and V stream through shared memory (atlas_b200_attention_long).
+    Same arguments and results; its lse and dropout masks are those `attention_bwd` expects."""
+    require_cuda(q, "q")
+    if out is None:
+        out = torch.empty((B * Lq, H * 64), dtype=q.dtype, device=q.device)
+    am = add_mask.float().contiguous() if add_mask is not None else None
+    bd = bias_delta.float().contiguous() if bias_delta is not None else None
+    lse = torch.empty((B, H, Lq), dtype=torch.float32, device=q.device) if return_lse else None
+    dp, dseed, doff = dropout if dropout is not None else (0.0, 0, 0)
+    check(lib().atlas_b200_attention_long(_ptr(q), q.stride(0), q_col0, _ptr(k), k.stride(0), k_col0, _ptr(v), v.stride(0),
+                                          v_col0, _ptr(out), out.stride(0), _ptr(am) if am is not None else None,
+                                          _ptr(bd) if bd is not None else None, B, H, Lq, Lk, float(scale),
+                                          float(causal_value), _ptr(lse) if lse is not None else None, float(dp),
+                                          int(dseed), int(doff), _ptr(block_live) if block_live is not None else None,
+                                          _bf(q), current_stream_ptr()))
+    return (out, lse) if return_lse else out
+
+
+def encoder_attention(L):
+    """The self-attention forward for segments of L tokens: `attention` up to ATTENTION_MAX_LK, `attention_long` above."""
+    return attention if L <= ATTENTION_MAX_LK else attention_long
+
+
 _SKIP_MASKED = os.environ.get("ATLAS_B200_ATTN_SKIP_MASKED", "1") != "0"    # A/B switch of the masked-key-block skipping
 
 

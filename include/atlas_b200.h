@@ -472,6 +472,17 @@ int atlas_b200_attention_train(const void* q, int64_t ldq, int32_t q_col0, const
                                float causal_value, int32_t q_div, float* o_partial, float* ml_partial, float* lse_out,
                                float dropout_p, uint64_t seed, uint64_t offset, const uint8_t* key_block_live,
                                int32_t is_bf16, void* stream);
+/* atlas_b200_attention_train for long key ranges: 0 < Lk <= 4096 keys per segment and Lq + Lk - 1 <= 8192 (the bias table
+ * of atlas_b200_attention_bwd_train), same arguments and results except that there are no split-KV partials (q_div = 1).
+ * K and V stream through shared memory in 64-key blocks instead of staying resident (csrc/attention.cu,
+ * attention_long_kernel), so the key count is not bounded by shared memory.  The FiD encoder takes it for passages longer
+ * than the 576 keys of atlas_b200_attention.  Strides and column offsets must be multiples of 8 elements; any violated
+ * limit returns ATLAS_B200_EINVAL before a launch. */
+int atlas_b200_attention_long(const void* q, int64_t ldq, int32_t q_col0, const void* k, int64_t ldk, int32_t k_col0,
+                              const void* v, int64_t ldv, int32_t v_col0, void* out, int64_t ldo, const float* add_mask,
+                              const float* bias_delta, int32_t B, int32_t H, int32_t Lq, int32_t Lk, float scale,
+                              float causal_value, float* lse_out, float dropout_p, uint64_t seed, uint64_t offset,
+                              const uint8_t* key_block_live, int32_t is_bf16, void* stream);
 int atlas_b200_attention_bwd_train(const void* q, int64_t ldq, int32_t q_col0, const void* k, int64_t ldk, int32_t k_col0,
                                    const void* v, int64_t ldv, int32_t v_col0, const void* out, int64_t ldo,
                                    const void* dout, int64_t lddo, void* dq, int64_t lddq, int32_t dq_col0, void* dk,
