@@ -213,6 +213,10 @@ def lib():
     L.atlas_b200_pq_topk_exhaustive.restype = c.c_int
     L.atlas_b200_pq_topk_exhaustive.argtypes = [vp, vp, i64, i32, vp, vp, i32, vp, i32, i32, vp, vp, i64, i64, vp, c.c_size_t,
                                                 vp]
+    L.atlas_b200_pq_refine_workspace_bytes.restype = c.c_size_t
+    L.atlas_b200_pq_refine_workspace_bytes.argtypes = [i32, i32]
+    L.atlas_b200_pq_refine_topk.restype = c.c_int
+    L.atlas_b200_pq_refine_topk.argtypes = [vp, i64, vp, i32, vp, i32, i32, vp, vp, i64, i64, vp, c.c_size_t, vp]
     _lib = L
     return L
 
@@ -287,6 +291,8 @@ EXPORTED_SYMBOLS = [
     "atlas_b200_pq_encode",
     "atlas_b200_pq_topk",
     "atlas_b200_pq_topk_exhaustive",
+    "atlas_b200_pq_refine_workspace_bytes",
+    "atlas_b200_pq_refine_topk",
     "atlas_b200_quantize_kv_e4m3",
     "atlas_b200_decode_cross_attention_e4m3",
     "atlas_b200_cross_attention_stream_e4m3",

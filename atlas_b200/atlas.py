@@ -194,6 +194,10 @@ class Atlas(nn.Module):
             # every rank runs the same options: the per-GPU batch size bounds the queries of any rank, which lets the
             # distributed search skip its size exchange (index.py: `max_queries_per_rank`)
             index.max_queries_per_rank = int(cap)
+        refine = getattr(self.opt, "faiss_refine_factor", None)
+        if refine is not None and hasattr(index, "refine_factor"):
+            # --index_mode faiss: re-rank refine * topk PQ candidates per rank by exact score (the flat index is exact)
+            index.refine_factor = int(refine)
         if filtering_fun is not None:
             passages, scores = index.search_knn(query_emb, topk * self.opt.filtering_overretrieve_ratio)
             passages, scores = filtering_fun(batch_metadata, passages, scores, topk, training=self.training)

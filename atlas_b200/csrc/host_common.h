@@ -52,6 +52,7 @@ enum ProfKind {
     PROF_ATTENTION_BWD = 4,
     PROF_DECODE_CROSS = 5,
     PROF_BEAM_SELECT = 6,     // beam_topk + beam_select (csrc/beam.cu); work = bytes read
+    PROF_PQ_REFINE = 7,       // pq_refine_kernel (csrc/pq_refine.cu); work = host-row bytes read
 };
 void prof_begin(cudaStream_t s, int kind);
 void prof_end(cudaStream_t s, int kind, double work);   // work = algorithmic bytes (scan) or FLOPs of this launch

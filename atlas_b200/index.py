@@ -338,14 +338,23 @@ class DistributedFAISSIndex(DistributedIndex):
     Persistence: `save_index` writes the reference's `embeddings.{s}.pt` / `passages.{s}.pt` shards and, per rank,
     `index{type}_{code_size}_rank_{r}.atlas_b200.pt` (format version, type, M, n_list, row count, codebooks, coarse
     centroids, codes, list ids).  `load_index` uses that file when type, M and row count match and retrains otherwise;
-    a reference `.faiss` file is not read (faiss's format is not reproduced here)."""
+    a reference `.faiss` file is not read (faiss's format is not reproduced here).
+
+    Refinement (faiss IndexRefineFlat / `k_factor`, opt-in): with `refine_factor` R > 1 (a constructor keyword and a plain
+    attribute that may be set at any time; Atlas sets it from `--faiss_refine_factor`) each rank takes its top
+    k' = min(k * R, N_local) rows by PQ score, re-scores them against their full-precision host rows (read zero-copy over
+    the host link, csrc/pq_refine.cu) and keeps its top k by that exact score; the ranks' lists are then merged as
+    before, which gives the exact top k of the union of the candidates.  The scores returned are then the exact inner
+    products rounded once to fp16 (the flat index's scores up to the fp32 summation order), not PQ scores.  k' must
+    not exceed MAX_TOPK.  No per-passage device memory is added; nothing is added to the index files.  `status` and the
+    exhaustive retry refer to the candidate search; the retry refines too.  R = 1 (default) runs the PQ search alone."""
 
     SUPPORTED_TYPES = ("pq", "ivfpq")
     FILE_FORMAT = 1
     TRAIN_SEED = 1234
     STAGE_ROWS = 65536
 
-    def __init__(self, index_type: str = "flat", code_size: Optional[int] = None):
+    def __init__(self, index_type: str = "flat", code_size: Optional[int] = None, refine_factor: int = 1):
         if index_type not in self.SUPPORTED_TYPES:
             raise AtlasB200Error(
                 f"DistributedFAISSIndex: index_type={index_type!r} is not provided by atlas_b200; supported types are "
@@ -360,6 +369,8 @@ class DistributedFAISSIndex(DistributedIndex):
         self.code_size = int(code_size)
         self.is_in_gpu = False
         self._pq = None                # dict(codebooks, coarse, codes, list_ids, n_list) of the trained index
+        self.refine_factor = refine_factor
+        self._refine_factor()
 
     # ------------------------------------------------------------------ host rows
     @property
@@ -450,10 +461,34 @@ class DistributedFAISSIndex(DistributedIndex):
             raise AtlasB200Error("search_knn on an untrained DistributedFAISSIndex: call train_index() after writing rows")
         return self._pq
 
+    def _refine_factor(self):
+        r = self.refine_factor
+        if isinstance(r, bool) or not isinstance(r, int) or r < 1:
+            raise AtlasB200Error(f"DistributedFAISSIndex: refine_factor={r!r} must be an integer >= 1 (1 = no refinement)")
+        return r
+
     def _local_search(self, allqueries, topk, exhaustive=False):
+        r = self._refine_factor()
+        if r == 1:
+            return self._candidate_search(allqueries, topk, self._id_base, self._id_stride, exhaustive)
+        k_cand = min(topk * r, int(self._bank.shape[0]))
+        if k_cand > MAX_TOPK:
+            raise AtlasB200Error(f"DistributedFAISSIndex: refine_factor={r} x topk={topk} = {topk * r} candidates per "
+                                 f"query exceed MAX_TOPK={MAX_TOPK}; lower refine_factor or topk")
+        _, cand, status = self._candidate_search(allqueries, k_cand, 0, 1, exhaustive)
+        s, i = self._refine(allqueries, cand, topk)
+        return s, i, status
+
+    def _candidate_search(self, allqueries, k, id_base, id_stride, exhaustive):
+        """Top k by PQ score: (scores, ids = id_base + id_stride * row, device status word)."""
         p = self._trained()
-        return ops.pq_topk(p["codes"], p["list_ids"], p["codebooks"], p["coarse"], allqueries, topk, self._id_base,
-                           self._id_stride, self._workspace, exhaustive=exhaustive)
+        return ops.pq_topk(p["codes"], p["list_ids"], p["codebooks"], p["coarse"], allqueries, k, id_base, id_stride,
+                           self._workspace, exhaustive=exhaustive)
+
+    def _refine(self, allqueries, cand_local, topk):
+        """Top `topk` of the candidate rows `cand_local` [nq, k'] by exact score: (scores, global ids)."""
+        return ops.pq_refine_topk(self._bank, allqueries, cand_local, topk, self._id_base, self._id_stride,
+                                  self._workspace)
 
     # ------------------------------------------------------------------ persistence
     def _get_index_filename(self, path: str) -> str:

@@ -239,6 +239,45 @@ def pq_topk(codes, list_ids, codebooks, coarse, queries, k, id_base=0, id_stride
     return out_s, out_i, status
 
 
+def pq_refine_topk(rows_host, queries, cand_local, k, id_base=0, id_stride=1, workspace=None):
+    """Exact re-ranking of PQ candidates (atlas_b200_pq_refine_topk, faiss IndexRefineFlat).
+
+    rows_host: PINNED CPU fp16 [n, 768] (the index's host rows), read zero-copy by the kernel; queries: [nq, 768], moved
+    to cand_local's device and rounded to fp16 like `pq_topk`; cand_local: CUDA int64 [nq, k'] local row numbers
+    (`pq_topk(..., k', 0, 1)`), distinct within a row; entries outside [0, n) are skipped.
+    Returns (scores fp16 [nq, k] desc, ids int64 [nq, k] = id_base + id_stride * row) as CUDA tensors: the top k of the
+    candidates by their exact inner product, accumulated in fp32 and rounded once to fp16."""
+    if rows_host.is_cuda or rows_host.dtype != torch.float16 or rows_host.dim() != 2 or rows_host.shape[1] != DIM \
+            or not rows_host.is_contiguous():
+        raise AtlasB200Error(f"pq_refine_topk: rows_host must be a contiguous CPU fp16 [n, {DIM}] tensor, got "
+                             f"{rows_host.dtype} {tuple(rows_host.shape)} on {rows_host.device}")
+    if not rows_host.is_pinned():
+        raise AtlasB200Error("pq_refine_topk: rows_host must be pinned host memory (tensor.pin_memory()): the kernel "
+                             "reads it over the host link")
+    require_cuda(cand_local, "cand_local")
+    q = cast_queries(queries.reshape(-1, DIM).to(cand_local.device), torch.float16)
+    nq = q.shape[0]
+    if cand_local.dtype != torch.int64 or cand_local.dim() != 2 or cand_local.shape[0] != nq:
+        raise AtlasB200Error(f"pq_refine_topk: cand_local must be int64 [nq={nq}, k'], got {cand_local.dtype} "
+                             f"{tuple(cand_local.shape)}")
+    cand = cand_local.contiguous()
+    k_cand = cand.shape[1]
+    if not 1 <= k <= k_cand:
+        raise AtlasB200Error(f"pq_refine_topk: need 1 <= k <= k' (k={k}, k'={k_cand})")
+    if k_cand > _lib.MAX_TOPK:
+        raise AtlasB200Error(f"pq_refine_topk: k'={k_cand} candidates exceed MAX_TOPK={_lib.MAX_TOPK}")
+    dev = q.device
+    out_s = torch.empty((nq, k), dtype=torch.float16, device=dev)
+    out_i = torch.empty((nq, k), dtype=torch.int64, device=dev)
+    if nq == 0:
+        return out_s, out_i
+    buf = (workspace or _default_ws).get(lib().atlas_b200_pq_refine_workspace_bytes(nq, k_cand), dev)
+    check(lib().atlas_b200_pq_refine_topk(_ptr(rows_host), rows_host.shape[0], _ptr(q), nq, _ptr(cand), k_cand, k,
+                                          _ptr(out_s), _ptr(out_i), id_base, id_stride, _ptr(buf), buf.numel(),
+                                          current_stream_ptr()))
+    return out_s, out_i
+
+
 # ---------------------------------------------------------------------------------------------
 # dense layers (csrc/gemm.cu)
 # ---------------------------------------------------------------------------------------------

@@ -139,6 +139,24 @@ int atlas_b200_pq_topk_exhaustive(const uint8_t* codes, const void* list_ids, in
                                   int32_t nq, int32_t k, void* out_scores, int64_t* out_ids, int64_t id_base,
                                   int64_t id_stride, void* workspace, size_t workspace_bytes, void* stream);
 
+/* Exact re-ranking of PQ search candidates (csrc/pq_refine.cu; faiss IndexRefineFlat, `k_factor`): for every query,
+ * the k_cand candidate rows are re-scored against their full-precision rows and the top k are returned.
+ *   rows_host   PINNED host memory, [n, 768] fp16 row-major, 16-byte aligned.  Read zero-copy by the kernel through
+ *               cudaHostGetDevicePointer (ATLAS_B200_ECUDA if that fails); each candidate row is read once.
+ *   queries     device fp16 [nq, 768], 16-byte aligned.
+ *   cand_local  device int64 [nq, k_cand]: local row numbers (atlas_b200_pq_topk with id_base = 0, id_stride = 1),
+ *               distinct within a query; entries outside [0, n) are skipped.  1 <= k <= k_cand <= ATLAS_B200_MAX_TOPK.
+ *   scores      fp16( sum_d fp32(q_d) fp32(x_d) ): fp32 accumulation in a fixed order, rounded ONCE to fp16, i.e. the
+ *               flat index's score up to the fp32 summation order; bitwise reproducible.
+ *   out_scores  device fp16 [nq, k], descending;  out_ids: device int64 [nq, k] = id_base + id_stride * row, canonical
+ *               tie order (score desc, id asc; id_stride >= 1).  Fewer than k valid candidates: -inf / -1 tail.
+ *   workspace   device scratch of atlas_b200_pq_refine_workspace_bytes(nq, k_cand) bytes (at most 256 queries' worth).
+ * nq == 0 is a no-op.  Reads of rows_host are ordered on `stream` after earlier work on it (e.g. copies into the rows). */
+size_t atlas_b200_pq_refine_workspace_bytes(int32_t nq, int32_t k_cand);
+int atlas_b200_pq_refine_topk(const void* rows_host, int64_t n, const void* queries, int32_t nq, const int64_t* cand_local,
+                              int32_t k_cand, int32_t k, void* out_scores, int64_t* out_ids, int64_t id_base,
+                              int64_t id_stride, void* workspace, size_t workspace_bytes, void* stream);
+
 /* --------------------------------------------------------------------------------------------
  * Dense linear layer with a fused epilogue on wgmma (csrc/gemm.cu):
  *     C[M, N] = epilogue( A[M, K] . W[N, K]^T )     A, W, C, bias, residual: fp16 (is_bf16 = 0) or bf16
@@ -599,6 +617,7 @@ int atlas_b200_expand_packed_tiles(const void* src, int64_t lds, const int32_t* 
  *   kind 2  the wgmma GEMM of atlas_b200_linear   (work = 2*M*N*K FLOPs)
  *   kind 3  the attention kernel                     (work = 4*B*H*Lq*Lk*64 FLOPs)
  *   kind 4  the attention backward kernels           (work = 16*B*H*Lq*Lk*64 FLOPs)
+ *   kind 7  the refine kernel of atlas_b200_pq_refine_topk (work = host-row bytes read, nq * k_cand * 1536)
  *   kind 0  off (default).
  * atlas_b200_profile_work() returns the work summed over the bracketed launches so far;
  * atlas_b200_profile_collect() synchronises the events, returns the summed kernel time and the number of

@@ -7,7 +7,12 @@ of bench.py (4 Mi passages of 768-d fp16 per GPU, BASELINE configs[1]).  Prints 
                               HBM peak
   device_bytes_per_passage    codes + list ids + codebooks + coarse centroids, over the rows
   recall_at_40                against the exact flat search, on a synthetic Gaussian bank: says little about real embeddings
+  refine                      with --refine-factor R > 1 only: the same search re-ranked by exact score over the top
+                              k' = 40 R PQ candidates (refine_factor = R): queries/s, recall_at_40 refined vs unrefined, the
+                              refine kernel's time and the host-row bytes it reads per search (nq k' 1536, from shapes) over
+                              that time
     python tools/perf_pq_index.py [--index-type ivfpq] [--code-size 16] [--rows N] [--steps 20] [--warmup 3]
+                                  [--refine-factor 1]
 Writes nothing."""
 import argparse
 import json
@@ -72,13 +77,32 @@ def measure(args):
     L.atlas_b200_profile_enable(0)
     assert int(st.item()) == 0, "fast search path overflowed"
     ids = ids.cpu().numpy()
-    recall = float(sum(len(set(a) & set(b)) for a, b in zip(ids.tolist(), exact.tolist())) / (NQ * TOPK))
+    recall_of = lambda ids: float(sum(len(set(a) & set(b)) for a, b in zip(ids.tolist(), exact.tolist())) / (NQ * TOPK))
+    recall = recall_of(ids)
     list_bytes = 0 if p["list_ids"] is None else p["list_ids"].element_size()
     groups = kn.value // (steps + warmup) if kn.value else 0
     kernel_ms = kms.value / (steps + warmup)
     sweep_bytes = rows * (M + list_bytes)
     peak, peak_src = peaks("hbm")
     achieved = sweep_bytes / (kernel_ms * 1e-3) / 1e9 if kernel_ms > 0 else 0.0
+    refine = None
+    if args.refine_factor > 1:
+        index.refine_factor = args.refine_factor
+        k_cand = min(TOPK * args.refine_factor, rows)
+        rms, (_, rids, st) = timed(lambda: index.search_device(q, TOPK, return_status=True))
+        assert int(st.item()) == 0, "fast search path overflowed"
+        L.atlas_b200_profile_enable(7)     # the refine kernel (csrc/pq_refine.cu)
+        timed(lambda: index.search_device(q, TOPK, return_status=True))
+        L.atlas_b200_profile_collect(ctypes.byref(kms), ctypes.byref(kn))
+        L.atlas_b200_profile_enable(0)
+        refine_kernel_ms = kms.value / (steps + warmup)
+        host_bytes = NQ * k_cand * DIM * 2
+        refine = {"refine_factor": args.refine_factor, "candidates_per_query": k_cand,
+                  "value": NQ / (rms * 1e-3), "unit": "queries/s", "ms_per_search": rms,
+                  "recall_at_40": recall_of(rids.cpu().numpy()), "recall_at_40_unrefined": recall,
+                  "kernel": "pq_refine_kernel (zero-copy reads of the pinned host rows)",
+                  "kernel_ms_per_search": refine_kernel_ms, "host_bytes_per_search": host_bytes,
+                  "host_link_GBps": host_bytes / (refine_kernel_ms * 1e-3) / 1e9 if refine_kernel_ms > 0 else 0.0}
     try:
         smi = subprocess.run(["nvidia-smi", "--id=0", "--query-gpu=name,power.limit", "--format=csv,noheader"],
                              capture_output=True, text=True, timeout=30).stdout.strip()
@@ -99,7 +123,7 @@ def measure(args):
         "recall_at_40": recall, "recall_note": "against the exact flat search on a synthetic Gaussian bank; not "
                                                "representative of real embeddings",
         "gpu": smi,
-    }
+    } | ({"refine": refine} if refine else {})
 
 
 def main():
@@ -109,6 +133,8 @@ def main():
     ap.add_argument("--rows", type=int, default=N_LOCAL)
     ap.add_argument("--steps", type=int, default=20)
     ap.add_argument("--warmup", type=int, default=3)
+    ap.add_argument("--refine-factor", type=int, default=1,
+                    help="also time the search re-ranked over refine-factor x 40 PQ candidates (1 = off)")
     print(json.dumps(measure(ap.parse_args())))
 
 
