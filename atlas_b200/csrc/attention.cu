@@ -22,13 +22,14 @@
 // kernels changes how ptxas allocates attention_kernel (124 -> 122 registers, different SASS), so attention_kernel keeps
 // its own loop and stays instruction-for-instruction what it was.
 //
-// Packed layout (seg_tile != nullptr, the padding-compacted FiD encoder): segment b keeps the first popcount(blk_live[b, :]) of
-// its 64-row tiles, stored back to back from row 64 * seg_tile[b * nb] of q / k / v / out; query tiles past them do not exist.
+// The padding-compacted encoders (segment b keeps the first n_b of its 64-row tiles, stored back to back) run on
+// attention_packed_kernel below: a persistent kernel over (segment, head) items with the same per-block arithmetic.
 #include "common.cuh"
 #include "dropout.cuh"
 #include "host_common.h"
 #include "wgmma.cuh"
 
+#include <algorithm>
 #include <math.h>
 #include <stdlib.h>
 
@@ -63,7 +64,6 @@ struct Params {
     float* lse_out;           // [B, H, Lq] fp32 row log-sum-exp (natural log) for the backward pass, or nullptr
     abdrop::Key drop;         // attention-probability dropout (training path); thr16 == 0: off
     const uint8_t* blk_live;  // [B, ceil(Lk / 64)] or nullptr: 0 = every key of the block is masked out
-    const int32_t* seg_tile;  // nullptr, or [B * Lk / 64]: packed layout (see above); needs Lq == Lk and blk_live
     int n_qt;                 // query tiles per segment (grid.x)
 };
 
@@ -194,23 +194,17 @@ attention_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_consta
     uint8_t* smem_gen = smem_raw + (smem_base - ab::smem_u32(smem_raw));
     const uint32_t sQ = smem_base, sK = smem_base + Q_BYTES, sV = sK + KV_BYTES;
 
-    const int nb = (p.Lk + BK - 1) / BK;
-    const bool packed = p.seg_tile != nullptr;
+    const int nkb = (p.Lk + BK - 1) / BK;
     // live key blocks (bit j = block j); none flagged live = all live
-    uint32_t live = (1u << nb) - 1u;
+    uint32_t live = (1u << nkb) - 1u;
     if (p.blk_live != nullptr) {
-        const bool lv = static_cast<int>(lane) < nb && __ldg(p.blk_live + static_cast<size_t>(b) * nb + lane) != 0;
+        const bool lv = static_cast<int>(lane) < nkb && __ldg(p.blk_live + static_cast<size_t>(b) * nkb + lane) != 0;
         const uint32_t m = __ballot_sync(0xffffffffu, lv);
         if (m != 0u) live = m;
     }
-    // rows of this segment: packed layout = its kept tiles, back to back
-    const int lq = packed ? 64 * __popc(live) : p.Lq;
-    const int lk = packed ? lq : p.Lk;
-    if (qt * BQ >= lq) return;                       // (packed) this query tile does not exist
-    const int q_row0 = packed ? 64 * __ldg(p.seg_tile + static_cast<size_t>(b) * nb) : (b / p.q_div) * p.Lq;
-    const int k_row0 = packed ? q_row0 : b * p.Lk;
-    const int o_row0 = packed ? q_row0 : b * p.Lq;
-    const int nkb = (lk + BK - 1) / BK;
+    const int q_row0 = (b / p.q_div) * p.Lq;
+    const int k_row0 = b * p.Lk;
+    const int o_row0 = b * p.Lq;
 
     if (threadIdx.x == 0) {
         ab::mbar_init(&load_bar, 1);
@@ -237,7 +231,7 @@ attention_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_consta
     // mask / bias tables while the loads are in flight
     const bool has_bias = (p.bias_delta != nullptr) || (p.causal_value != 0.f);
     for (int j = threadIdx.x; j < nkb * BK; j += THREADS)
-        s_mask[j] = (j < lk) ? (p.add_mask ? p.add_mask[static_cast<size_t>(b) * p.Lk + j] * LOG2E : 0.f) : -INFINITY;
+        s_mask[j] = (j < p.Lk) ? (p.add_mask ? p.add_mask[static_cast<size_t>(b) * p.Lk + j] * LOG2E : 0.f) : -INFINITY;
     if (has_bias) {
         const int n_valid = p.Lq + p.Lk - 1;
         for (int d = threadIdx.x; d < 2 * MAX_LK + BK; d += THREADS) {   // entries past the valid offsets stay finite (0)
@@ -359,7 +353,7 @@ attention_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_consta
         l += __shfl_xor_sync(0xffffffffu, l, 1);
         l += __shfl_xor_sync(0xffffffffu, l, 2);
         const int i = i0 + 8 * hh;
-        if (i >= lq) continue;
+        if (i >= p.Lq) continue;
         const size_t orow = static_cast<size_t>(o_row0) + i;
         if (p.o_partial != nullptr) {
             const float ik = p.drop.inv_keep;
@@ -520,6 +514,277 @@ attention_long_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_c
     }
 }
 
+// ---- attention_packed_kernel: self-attention over the packed rows of the padding-compacted encoders.  Segment b keeps its
+// first n_b = popcount(keep[b, :]) 64-row tiles, stored back to back from row 64 * tile_off[b * nb] of qkv / out; its n_b query
+// tiles attend to its n_b key tiles.  Persistent: CTA c owns head h = c % H (its bias row is staged once) and the segments
+// c / H, c / H + G, ... (G = grid / H).  One producer warp loads, per (segment, head) item, the item's K and V tiles ONCE into
+// one of two item slots (the next item's slot fills while the consumers work on the current one) and the item's 64-row query
+// tiles into a ring of PK_Q_STAGES tiles.  The CTA's query tiles are numbered across its items; consumer warpgroup g takes the
+// ones with number % 2 == g.  Per key block the arithmetic is attention_kernel's (same blocks, same order, same fp32
+// operations), only the issue order differs: S_{j+1} = Q K_{j+1}^T and O += P_j V_j are in flight while the softmax of block
+// j + 1 runs.  Shared memory at L = 384: 2 slots x 12 tiles (192 KB) + 3 query tiles (24 KB) + bias row and masks (6 KB).
+constexpr int PK_MAX_TILES = 6;                // L <= 384
+constexpr int PK_Q_STAGES = 3;
+constexpr int PK_THREADS = THREADS + 32;       // two consumer warpgroups + one producer warp
+
+struct PackedParams {
+    int S, H, L, G;
+    int q_col0, k_col0, v_col0;
+    uint16_t* O;
+    int64_t ldo;
+    const float* add_mask;     // [S, L] or nullptr
+    const float* bias_delta;   // [H, 2L - 1] or nullptr
+    const uint8_t* keep;       // [S, L / 64]
+    const int32_t* tile_off;   // [S * L / 64]
+    float scale;
+};
+
+static size_t packed_smem_bytes(int L) {
+    const int nt = L / BK;
+    return 1024 + static_cast<size_t>(2 * 2 * nt + PK_Q_STAGES) * TILE_BYTES + static_cast<size_t>(2 * L + 2 * L) * 4;
+}
+
+template <bool kBF16>
+__global__ void __launch_bounds__(PK_THREADS, 1)
+attention_packed_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ CUtensorMap tmap_k,
+                        const __grid_constant__ CUtensorMap tmap_v, const PackedParams p) {
+    extern __shared__ uint8_t smem_raw[];
+    __shared__ __align__(8) uint64_t full_kv[2], empty_kv[2], full_q[PK_Q_STAGES], empty_q[PK_Q_STAGES];
+    __shared__ int2 s_item[2];                     // per slot: (tiles n, first packed row)
+
+    const uint32_t warp = threadIdx.x >> 5;
+    const uint32_t lane = threadIdx.x & 31u;
+    const uint32_t smem_base = (ab::smem_u32(smem_raw) + 1023u) & ~1023u;
+    uint8_t* smem_gen = smem_raw + (smem_base - ab::smem_u32(smem_raw));
+    const int nt = p.L / BK;
+    const uint32_t slot_bytes = 2u * nt * TILE_BYTES;  // K tiles | V tiles
+    // K/V slot 0 | K/V slot 1 | query ring | bias row (2L - 1 offsets) | key mask per slot
+    const uint32_t sKV = smem_base, sQ = sKV + 2u * slot_bytes;
+    float* s_bias = reinterpret_cast<float*>(smem_gen + 2u * slot_bytes + PK_Q_STAGES * TILE_BYTES);
+    float* s_mask = s_bias + 2 * p.L;
+
+    const int h = static_cast<int>(blockIdx.x) % p.H;
+    const int b0 = static_cast<int>(blockIdx.x) / p.H;
+    const int n_items = (p.S - b0 + p.G - 1) / p.G;
+    if (threadIdx.x == 0) {
+        for (int s = 0; s < 2; ++s) {
+            ab::mbar_init(&full_kv[s], 32);                 // every producer lane arrives after staging its part of the mask
+            ab::mbar_init(&empty_kv[s], THREADS / 32);      // one arrival per consumer warp
+        }
+        for (int s = 0; s < PK_Q_STAGES; ++s) {
+            ab::mbar_init(&full_q[s], 1);
+            ab::mbar_init(&empty_q[s], 4);                  // the 4 warps of the consuming warpgroup
+        }
+        ab::fence_barrier_init();
+    }
+    const bool has_bias = p.bias_delta != nullptr;
+    if (has_bias)
+        for (int d = threadIdx.x; d < 2 * p.L - 1; d += PK_THREADS)
+            s_bias[d] = p.bias_delta[static_cast<size_t>(h) * (2 * p.L - 1) + d] * LOG2E;
+    __syncthreads();
+
+    if (warp == THREADS / 32) {
+        // producer: item k's K / V into slot k % 2 once item k - 2 has left it; query tiles in order into the ring.  The two
+        // streams wait on different barriers, so neither blocks the other: poll both.
+        int kv_k = 0, q_k = 0, q_t = 0, qi = 0;
+        if (lane == 0) {
+            ab::tma_prefetch_desc(&tmap_q);
+            ab::tma_prefetch_desc(&tmap_k);
+            ab::tma_prefetch_desc(&tmap_v);
+        }
+        while (q_k < n_items) {
+            bool issued = false;
+            if (kv_k < n_items) {
+                const int slot = kv_k & 1;
+                int ready = kv_k < 2 || ab::mbar_test_wait(&empty_kv[slot], ((kv_k >> 1) & 1) ^ 1);
+                ready = __shfl_sync(0xffffffffu, ready, 0);
+                if (ready) {
+                    const int b = b0 + kv_k * p.G;
+                    const bool kp = static_cast<int>(lane) < nt && __ldg(p.keep + static_cast<size_t>(b) * nt + lane) != 0;
+                    const uint32_t m = __ballot_sync(0xffffffffu, kp);
+                    const int n = m != 0u ? __popc(m) : nt;
+                    const int row0 = 64 * __ldg(p.tile_off + static_cast<size_t>(b) * nt);
+                    float* mk = s_mask + slot * p.L;
+                    for (int j = lane; j < n * BK; j += 32)
+                        mk[j] = p.add_mask ? p.add_mask[static_cast<size_t>(b) * p.L + j] * LOG2E : 0.f;
+                    if (lane == 0) {
+                        s_item[slot] = make_int2(n, row0);
+                        ab::mbar_arrive_expect_tx(&full_kv[slot], static_cast<uint32_t>(2 * n * TILE_BYTES));
+                        for (int t = 0; t < n; ++t) {
+                            ab::tma_load_2d(&tmap_k, &full_kv[slot], smem_gen + slot * slot_bytes + t * TILE_BYTES,
+                                            p.k_col0 + h * D, row0 + t * BK, ab::kEvictFirst);
+                            ab::tma_load_2d(&tmap_v, &full_kv[slot], smem_gen + slot * slot_bytes + (nt + t) * TILE_BYTES,
+                                            p.v_col0 + h * D, row0 + t * BK, ab::kEvictFirst);
+                        }
+                    } else {
+                        ab::mbar_arrive(&full_kv[slot]);
+                    }
+                    __syncwarp();
+                    ++kv_k;
+                    issued = true;
+                }
+            }
+            if (q_k < kv_k) {
+                const int s = qi % PK_Q_STAGES;
+                int ready = qi < PK_Q_STAGES || ab::mbar_test_wait(&empty_q[s], ((qi / PK_Q_STAGES) & 1) ^ 1);
+                ready = __shfl_sync(0xffffffffu, ready, 0);
+                if (ready) {
+                    const int2 it = s_item[q_k & 1];
+                    if (lane == 0) {
+                        ab::mbar_arrive_expect_tx(&full_q[s], static_cast<uint32_t>(TILE_BYTES));
+                        ab::tma_load_2d(&tmap_q, &full_q[s], smem_gen + 2u * slot_bytes + s * TILE_BYTES, p.q_col0 + h * D,
+                                        it.y + q_t * BK, ab::kEvictFirst);
+                    }
+                    ++qi;
+                    if (++q_t == it.x) q_t = 0, ++q_k;
+                    issued = true;
+                }
+            }
+            if (!issued) __nanosleep(32);
+        }
+        return;
+    }
+
+    // ---- consumers: warpgroup g; this thread: rows r and r + 8 of the 64-row query tile, key pairs 8 j + 2 (lane % 4)
+    const uint32_t g = warp >> 2, wl = warp & 3u;
+    const int cq = static_cast<int>(2u * (lane & 3u));
+    const float scale2 = p.scale * LOG2E;
+    int q0 = 0;                                            // number of the item's first query tile
+    for (int k = 0; k < n_items; ++k) {
+        const int slot = k & 1;
+        ab::mbar_wait_nocall(&full_kv[slot], (k >> 1) & 1);
+        const int2 it = s_item[slot];
+        const int n = it.x;
+        const float* mk = s_mask + slot * p.L;
+        const uint32_t sK = sKV + slot * slot_bytes, sV = sK + nt * TILE_BYTES;
+        for (int qi = q0 + ((static_cast<int>(g) - q0) & 1); qi < q0 + n; qi += 2) {
+            const int s = qi % PK_Q_STAGES;
+            const uint32_t sQs = sQ + s * TILE_BYTES;
+            const int i0 = (qi - q0) * BK + static_cast<int>(wl * 16u + (lane >> 2));   // segment row of row r
+            ab::mbar_wait_nocall(&full_q[s], (qi / PK_Q_STAGES) & 1);
+
+            float o[32], sc[32];
+            uint32_t pa[16];
+            float m_run[2] = {-INFINITY, -INFINITY}, l_run[2] = {0.f, 0.f}, corr[2];
+            auto issue_s = [&](int kb) {
+#pragma unroll
+                for (int kk = 0; kk < D / 16; ++kk)
+                    ab::wgmma_m64n64k16_ss<kBF16, 0, 0>(sc, ab::wgmma_desc_sw128(sQs + kk * 32u),
+                                                        ab::wgmma_desc_sw128(sK + kb * TILE_BYTES + kk * 32u), kk);
+                ab::wgmma_commit();
+            };
+            auto issue_pv = [&](int kb) {
+#pragma unroll
+                for (int kk = 0; kk < BK / 16; ++kk)
+                    ab::wgmma_m64n64k16_rs<kBF16, 1>(o, *reinterpret_cast<const uint32_t(*)[4]>(&pa[4 * kk]),
+                                                     ab::wgmma_desc_sw128(sV + kb * TILE_BYTES + kk * 2048u, 8192), 1);
+                ab::wgmma_commit();
+            };
+            // block kb's softmax on the completed S in sc: sc <- p = 2^(t - m), (m_run, l_run) updated, corr for o
+            auto softmax = [&](int kb) {
+                ab::wgmma_reg_fence(sc);
+                // t = S * scale2 + (mask + bias) in the log2 domain; new row maxima
+                float mx[2] = {m_run[0], m_run[1]};
+#pragma unroll
+                for (int j = 0; j < 8; ++j) {
+#pragma unroll
+                    for (int c = 0; c < 2; ++c) {
+                        const int key = kb * BK + 8 * j + cq + c;
+                        const float mkv = mk[key];
+#pragma unroll
+                        for (int hh = 0; hh < 2; ++hh) {
+                            float a = mkv;
+                            if (has_bias) a += s_bias[key - (i0 + 8 * hh) + (p.L - 1)];
+                            const float t = fmaf(sc[4 * j + 2 * hh + c], scale2, a);
+                            sc[4 * j + 2 * hh + c] = t;
+                            mx[hh] = fmaxf(mx[hh], t);
+                        }
+                    }
+                }
+                float base[2];
+#pragma unroll
+                for (int hh = 0; hh < 2; ++hh) {
+                    mx[hh] = fmaxf(mx[hh], __shfl_xor_sync(0xffffffffu, mx[hh], 1));
+                    mx[hh] = fmaxf(mx[hh], __shfl_xor_sync(0xffffffffu, mx[hh], 2));
+                    base[hh] = mx[hh] == -INFINITY ? 0.f : mx[hh];
+                    corr[hh] = ex2_approx(m_run[hh] - base[hh]);     // 0 for the first block (m_run = -inf)
+                    m_run[hh] = mx[hh];
+                    l_run[hh] *= corr[hh];
+                }
+#pragma unroll
+                for (int hh = 0; hh < 2; ++hh) {
+#pragma unroll
+                    for (int j = 0; j < 8; ++j) {
+                        const float e0 = ex2_approx(sc[4 * j + 2 * hh] - base[hh]);
+                        const float e1 = ex2_approx(sc[4 * j + 2 * hh + 1] - base[hh]);
+                        l_run[hh] += e0 + e1;
+                        sc[4 * j + 2 * hh] = e0;
+                        sc[4 * j + 2 * hh + 1] = e1;
+                    }
+                }
+            };
+            // o *= corr, then P = p rounded to 16 bits as the A fragment of k16 step j / 2: a0 = (r, keys 0-7),
+            // a1 = (r + 8, keys 0-7), a2 / a3 = keys 8-15
+            auto rescale_and_pack = [&]() {
+#pragma unroll
+                for (int j = 0; j < 8; ++j) {
+                    o[4 * j] *= corr[0];
+                    o[4 * j + 1] *= corr[0];
+                    o[4 * j + 2] *= corr[1];
+                    o[4 * j + 3] *= corr[1];
+                }
+#pragma unroll
+                for (int hh = 0; hh < 2; ++hh)
+#pragma unroll
+                    for (int j = 0; j < 8; ++j)
+                        pa[4 * (j >> 1) + 2 * (j & 1) + hh] = pack2<kBF16>(sc[4 * j + 2 * hh], sc[4 * j + 2 * hh + 1]);
+            };
+
+#pragma unroll
+            for (int x = 0; x < 32; ++x) o[x] = 0.f;
+            ab::wgmma_fence();
+            issue_s(0);
+            ab::wgmma_wait<0>();
+            softmax(0);
+            rescale_and_pack();
+            for (int kb = 1; kb < n; ++kb) {
+                // S_kb and O += P_{kb-1} V_{kb-1} in flight; the softmax of block kb runs under the P V
+                ab::wgmma_fence();
+                issue_s(kb);
+                issue_pv(kb - 1);
+                ab::wgmma_wait<1>();
+                softmax(kb);
+                ab::wgmma_wait<0>();
+                ab::wgmma_reg_fence(o);
+#pragma unroll
+                for (int x = 0; x < 16; ++x) asm volatile("" : "+r"(pa[x])::"memory");   // P_{kb-1} was read until here
+                rescale_and_pack();
+            }
+            ab::wgmma_fence();
+            issue_pv(n - 1);
+            __syncwarp();
+            if (lane == 0) ab::mbar_arrive(&empty_q[s]);     // every S of the query tile is complete
+            ab::wgmma_wait<0>();
+            ab::wgmma_reg_fence(o);
+
+#pragma unroll
+            for (int hh = 0; hh < 2; ++hh) {
+                float l = l_run[hh];
+                l += __shfl_xor_sync(0xffffffffu, l, 1);
+                l += __shfl_xor_sync(0xffffffffu, l, 2);
+                const float inv = 1.0f / l;
+                uint16_t* dst = p.O + (static_cast<size_t>(it.y) + i0 + 8 * hh) * p.ldo + h * D + cq;
+#pragma unroll
+                for (int j = 0; j < 8; ++j)
+                    *reinterpret_cast<uint32_t*>(dst + 8 * j) = pack2<kBF16>(o[4 * j + 2 * hh] * inv, o[4 * j + 2 * hh + 1] * inv);
+            }
+        }
+        q0 += n;
+        __syncwarp();
+        if (lane == 0) ab::mbar_arrive(&empty_kv[slot]);     // this warp's MMAs on the slot have completed
+    }
+}
+
 template <bool kBF16>
 static int make_tmaps(CUtensorMap& tq, CUtensorMap& tk, CUtensorMap& tv, const void* q, int64_t ldq, const void* k, int64_t ldk,
                       const void* v, int64_t ldv, int q_rows, int k_rows, const Params& p) {
@@ -568,6 +833,22 @@ static int launch(const void* q, int64_t ldq, const void* k, int64_t ldk, const 
     return ATLAS_B200_OK;
 }
 
+template <bool kBF16>
+static int launch_packed(const void* qkv, int64_t ld, int rows, const Params& tp, const PackedParams& p, cudaStream_t s) {
+    CUtensorMap tq, tk, tv;
+    const int rc = make_tmaps<kBF16>(tq, tk, tv, qkv, ld, qkv, ld, qkv, ld, rows, rows, tp);
+    if (rc) return rc;
+    static bool attr_set = false;
+    if (!attr_set) {
+        AB_CUDA_CHECK(cudaFuncSetAttribute(attention_packed_kernel<kBF16>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                           static_cast<int>(packed_smem_bytes(PK_MAX_TILES * BK))));
+        attr_set = true;
+    }
+    attention_packed_kernel<kBF16><<<static_cast<unsigned>(p.G * p.H), PK_THREADS, packed_smem_bytes(p.L), s>>>(tq, tk, tv, p);
+    AB_CUDA_CHECK(cudaGetLastError());
+    return ATLAS_B200_OK;
+}
+
 static Params base_params(int B, int H, int Lq, int Lk, int q_col0, int k_col0, int v_col0, void* out, int64_t ldo,
                           const float* add_mask, const float* bias_delta, float scale, float causal_value) {
     Params p;
@@ -585,7 +866,6 @@ static Params base_params(int B, int H, int Lq, int Lk, int q_col0, int k_col0, 
     p.lse_out = nullptr;
     p.drop = abdrop::make_key(0.f, 0, 0);
     p.blk_live = nullptr;
-    p.seg_tile = nullptr;
     p.n_qt = (Lq + BQ - 1) / BQ;
     return p;
 }
@@ -651,15 +931,25 @@ int atlas_b200_attention_packed(const void* qkv, int64_t ld, int32_t q_col0, int
                "attention_packed: 0 < L <= 384, L %% 64 == 0 and the segment tables are required (got L=%d)", L);
     AB_REQUIRE(ld % 8 == 0 && ldo % 8 == 0 && q_col0 % 8 == 0 && k_col0 % 8 == 0 && v_col0 % 8 == 0,
                "attention_packed: strides and column offsets must be multiples of 8 elements");
+    AB_REQUIRE(static_cast<int64_t>(B) * L < (1ll << 31), "attention_packed: more than 2^31 rows");
     cudaStream_t ls = static_cast<cudaStream_t>(stream);
-    Params p = base_params(B, H, L, L, q_col0, k_col0, v_col0, out, ldo, add_mask, bias_delta, scale, 0.f);
-    p.blk_live = keep;
-    p.seg_tile = tile_off;
+    const Params tp = base_params(B, H, L, L, q_col0, k_col0, v_col0, out, ldo, add_mask, bias_delta, scale, 0.f);
+    PackedParams p;
+    p.S = B, p.H = H, p.L = L;
+    // CTAs per head: one CTA per SM in all, every CTA with at least one segment
+    p.G = std::max(1, std::min(B, abh::num_sms() / H));
+    p.q_col0 = q_col0, p.k_col0 = k_col0, p.v_col0 = v_col0;
+    p.O = static_cast<uint16_t*>(out);
+    p.ldo = ldo;
+    p.add_mask = add_mask;
+    p.bias_delta = bias_delta;
+    p.keep = keep;
+    p.tile_off = tile_off;
+    p.scale = scale;
     // the packed rows of all segments: at most B * L (the tensor maps only bound the TMA boxes)
     const int rows = B * L;
     abh::prof_begin(ls, abh::PROF_ATTENTION);
-    const int lrc = is_bf16 ? launch<true>(qkv, ld, qkv, ld, qkv, ld, rows, rows, p, ls)
-                            : launch<false>(qkv, ld, qkv, ld, qkv, ld, rows, rows, p, ls);
+    const int lrc = is_bf16 ? launch_packed<true>(qkv, ld, rows, tp, p, ls) : launch_packed<false>(qkv, ld, rows, tp, p, ls);
     if (lrc) return lrc;
     // dense-equivalent work, like the masked-block skipping of the padded layout
     abh::prof_end(ls, abh::PROF_ATTENTION, 4.0 * B * H * static_cast<double>(L) * L * attn::D);
