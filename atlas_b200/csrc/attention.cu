@@ -17,13 +17,13 @@
 // probabilities are exactly 0 in fp32.
 //
 // Segments of 577 to 4096 keys (the FiD encoder on long passages) run on attention_long_kernel below: the same per-block
-// arithmetic, with K and V streamed through a ring of shared-memory slots instead of held resident.  Its per-block code
-// (attend_block) is a copy of attention_kernel's loop body rather than shared with it: calling one inlined function from both
-// kernels changes how ptxas allocates attention_kernel (124 -> 122 registers, different SASS), so attention_kernel keeps
-// its own loop and stays instruction-for-instruction what it was.
+// arithmetic, with K and V streamed through a ring of shared-memory slots instead of held resident.
 //
 // The padding-compacted encoders (segment b keeps the first n_b of its 64-row tiles, stored back to back) run on
 // attention_packed_kernel below: a persistent kernel over (segment, head) items with the same per-block arithmetic.
+//
+// All three kernels run that arithmetic through the same functions (issue_s, block_softmax, rescale_and_pack, drop_probs,
+// issue_pv, write_rows), so their results agree bit for bit where their inputs do.
 #include "common.cuh"
 #include "dropout.cuh"
 #include "host_common.h"
@@ -78,48 +78,55 @@ __device__ __forceinline__ float ex2_approx(float x) {
     return y;
 }
 
-// attention_long_kernel's step over one live 64-key block kb, the loop body of attention_kernel (see the header): for this
-// thread's query rows i0 and i0 + 8 (warpgroup g of the 128-row tile at sQ; the block's K and V in slot `slot` of sK / sV),
-// S = Q K^T, t = S * scale2 + mask + bias in the log2 domain, the online-softmax update of (m_run, l_run, o) and O += P V
-// with P from registers.  s_mask is indexed by key, s_bias by key - min(i, Lq - 1) + bias_off.
-template <bool kBF16>
-__device__ __forceinline__ void attend_block(float (&o)[32], float (&m_run)[2], float (&l_run)[2], const uint32_t sQ,
-                                             const uint32_t g, const uint32_t sK, const uint32_t sV, const int slot,
-                                             const float* s_mask, const float* s_bias,
-                                             const int bias_off, const bool has_bias, const int kb, const int i0, const int cq,
-                                             const float scale2, const bool dropping, const Params& p, const int b, const int h,
-                                             const uint32_t lane) {
-    float sc[32];
-    ab::wgmma_fence();
-#pragma unroll
-    for (int k = 0; k < D / 16; ++k) {
-        const uint64_t adesc = ab::wgmma_desc_sw128(sQ + g * 8192u + k * 32u);
-        const uint64_t bdesc = ab::wgmma_desc_sw128(sK + slot * TILE_BYTES + k * 32u);
-        ab::wgmma_m64n64k16_ss<kBF16, 0, 0>(sc, adesc, bdesc, k);
-    }
-    ab::wgmma_commit();
-    ab::wgmma_wait<0>();
-    ab::wgmma_reg_fence(sc);
+// ---- The per-block arithmetic, shared by the three kernels.  A warpgroup owns 64 query rows; this thread holds rows r and
+// r + 8 of them (segment rows i0 and i0 + 8) and, of each 8-key group j of a 64-key block, the keys 8 j + cq + c, cq =
+// 2 (lane % 4), c = 0, 1: element 4 j + 2 hh + c of the fragments sc (S, then t, then p) and o is (row r + 8 hh, key c).
 
-    // t = S * scale2 + (mask + bias) in the log2 domain; new row maxima
+// S = Q K^T for one 64-key block: the warpgroup's 64-row query tile at sQ, the block's K tile at sK; one commit group
+template <bool kBF16>
+__device__ __forceinline__ void issue_s(float (&sc)[32], const uint32_t sQ, const uint32_t sK) {
+#pragma unroll
+    for (int k = 0; k < D / 16; ++k)
+        ab::wgmma_m64n64k16_ss<kBF16, 0, 0>(sc, ab::wgmma_desc_sw128(sQ + k * 32u), ab::wgmma_desc_sw128(sK + k * 32u), k);
+    ab::wgmma_commit();
+}
+
+// O += P V for one 64-key block: P from registers (rescale_and_pack), the block's V tile at sV as it lies in memory (the
+// MN-major operand); one commit group
+template <bool kBF16>
+__device__ __forceinline__ void issue_pv(float (&o)[32], const uint32_t (&pa)[16], const uint32_t sV) {
+#pragma unroll
+    for (int k = 0; k < BK / 16; ++k)
+        ab::wgmma_m64n64k16_rs<kBF16, 1>(o, *reinterpret_cast<const uint32_t(*)[4]>(&pa[4 * k]),
+                                         ab::wgmma_desc_sw128(sV + k * 2048u, 8192), 1);
+    ab::wgmma_commit();
+}
+
+// The online softmax of one block on its completed S (keys key0 + 8 j + c, key0 = 64 kb + cq): t = S * scale2 + mask[key]
+// + bias[hh][key] in the log2 domain (bias[hh] = the staged bias row of row r + 8 hh, read only if has_bias), the new row
+// maxima over the quad, sc <- p = 2^(t - base) and l_run <- l_run * corr + sum p.  corr = 2^(m_old - base) is o's rescale.
+__device__ __forceinline__ void block_softmax(float (&sc)[32], float (&m_run)[2], float (&l_run)[2], float (&corr)[2],
+                                              const float* mask, const float* const (&bias)[2], const bool has_bias,
+                                              const int key0, const float scale2) {
+    ab::wgmma_reg_fence(sc);
     float mx[2] = {m_run[0], m_run[1]};
 #pragma unroll
     for (int j = 0; j < 8; ++j) {
 #pragma unroll
         for (int c = 0; c < 2; ++c) {
-            const int key = kb * BK + 8 * j + cq + c;
-            const float mk = s_mask[key];
+            const int key = key0 + 8 * j + c;
+            const float mk = mask[key];
 #pragma unroll
             for (int hh = 0; hh < 2; ++hh) {
                 float a = mk;
-                if (has_bias) a += s_bias[key - min(i0 + 8 * hh, p.Lq - 1) + bias_off];   // rows past Lq are not stored
+                if (has_bias) a += bias[hh][key];
                 const float t = fmaf(sc[4 * j + 2 * hh + c], scale2, a);
                 sc[4 * j + 2 * hh + c] = t;
                 mx[hh] = fmaxf(mx[hh], t);
             }
         }
     }
-    float corr[2], base[2];
+    float base[2];
 #pragma unroll
     for (int hh = 0; hh < 2; ++hh) {
         mx[hh] = fmaxf(mx[hh], __shfl_xor_sync(0xffffffffu, mx[hh], 1));
@@ -127,8 +134,27 @@ __device__ __forceinline__ void attend_block(float (&o)[32], float (&m_run)[2], 
         base[hh] = mx[hh] == -INFINITY ? 0.f : mx[hh];
         corr[hh] = ex2_approx(m_run[hh] - base[hh]);     // 0 for the first block (m_run = -inf)
         m_run[hh] = mx[hh];
-        l_run[hh] *= corr[hh];
     }
+#pragma unroll
+    for (int hh = 0; hh < 2; ++hh) {
+#pragma unroll
+        for (int j = 0; j < 8; ++j) {
+            const float e0 = ex2_approx(sc[4 * j + 2 * hh] - base[hh]);
+            const float e1 = ex2_approx(sc[4 * j + 2 * hh + 1] - base[hh]);
+            // l_run * corr and the first pair's sum round once, as one fma: written out rather than left to the compiler's
+            // contraction, which code between the multiply and the add (a branch) can prevent in one kernel and not another
+            l_run[hh] = j == 0 ? fmaf(l_run[hh], corr[hh], e0 + e1) : l_run[hh] + (e0 + e1);
+            sc[4 * j + 2 * hh] = e0;
+            sc[4 * j + 2 * hh + 1] = e1;
+        }
+    }
+}
+
+// o *= corr, then P = p rounded to 16 bits as the A fragment of k16 step j / 2: a0 = (r, keys 0-7), a1 = (r + 8, keys 0-7),
+// a2 / a3 = keys 8-15
+template <bool kBF16>
+__device__ __forceinline__ void rescale_and_pack(uint32_t (&pa)[16], float (&o)[32], const float (&sc)[32],
+                                                 const float (&corr)[2]) {
 #pragma unroll
     for (int j = 0; j < 8; ++j) {
         o[4 * j] *= corr[0];
@@ -136,44 +162,90 @@ __device__ __forceinline__ void attend_block(float (&o)[32], float (&m_run)[2], 
         o[4 * j + 2] *= corr[1];
         o[4 * j + 3] *= corr[1];
     }
-    // p = 2^(t - m); the row sum takes every probability, the P operand only the kept ones (dropout)
-    uint32_t pa[16];
+#pragma unroll
+    for (int hh = 0; hh < 2; ++hh)
+#pragma unroll
+        for (int j = 0; j < 8; ++j)
+            pa[4 * (j >> 1) + 2 * (j & 1) + hh] = pack2<kBF16>(sc[4 * j + 2 * hh], sc[4 * j + 2 * hh + 1]);
+}
+
+// Dropout on P (rescale_and_pack's fragment), after the row sums took every probability: a dropped probability's 16 bits are
+// cleared, which are the bits of a packed 0.  The keep bits of rows R[hh] (row r + 8 hh in the key's row numbering), in
+// groups of 32 keys from key column col.
+__device__ __forceinline__ void drop_probs(uint32_t (&pa)[16], const abdrop::Key& drop, const uint64_t (&R)[2], const int col,
+                                           const uint32_t lane) {
 #pragma unroll
     for (int hh = 0; hh < 2; ++hh) {
         uint32_t w[2][4];
-        if (dropping) {
-            const uint64_t R = (static_cast<uint64_t>(b / p.q_div) * p.H + h) * p.Lq + min(i0 + 8 * hh, p.Lq - 1);
 #pragma unroll
-            for (int gg = 0; gg < 2; ++gg) {
-                const uint32_t G = static_cast<uint32_t>(((b % p.q_div) * p.Lk + kb * BK + gg * 32) >> 5);
-                abdrop::attn_words(p.drop, R, G, static_cast<uint32_t>(lane & 3u), w[gg]);
-            }
-        }
+        for (int gg = 0; gg < 2; ++gg)
+            abdrop::attn_words(drop, R[hh], static_cast<uint32_t>((col + gg * 32) >> 5), lane & 3u, w[gg]);
 #pragma unroll
         for (int j = 0; j < 8; ++j) {
-            const float e0 = ex2_approx(sc[4 * j + 2 * hh] - base[hh]);
-            const float e1 = ex2_approx(sc[4 * j + 2 * hh + 1] - base[hh]);
-            l_run[hh] += e0 + e1;
-            float k0 = e0, k1 = e1;
-            if (dropping) {
-                const uint32_t word = w[j >> 2][j & 3];
-                k0 = abdrop::keep_lo(p.drop, word) ? e0 : 0.f;
-                k1 = abdrop::keep_hi(p.drop, word) ? e1 : 0.f;
-            }
-            // A fragment of k16 step j / 2: a0 = (r, keys 0-7), a1 = (r + 8, keys 0-7), a2 / a3 = keys 8-15
-            pa[4 * (j >> 1) + 2 * (j & 1) + hh] = pack2<kBF16>(k0, k1);
+            const uint32_t word = w[j >> 2][j & 3];
+            pa[4 * (j >> 1) + 2 * (j & 1) + hh] &=
+                (abdrop::keep_lo(drop, word) ? 0x0000FFFFu : 0u) | (abdrop::keep_hi(drop, word) ? 0xFFFF0000u : 0u);
         }
     }
-    ab::wgmma_fence();
+}
+
+// a row's sum over the four threads of its quad
+__device__ __forceinline__ float quad_sum(float x) {
+    x += __shfl_xor_sync(0xffffffffu, x, 1);
+    return x + __shfl_xor_sync(0xffffffffu, x, 2);
+}
+
+// The finished rows i = i0 and i0 + 8 below n_rows: the log-sum-exp (natural log) at lse[i] unless lse is null, and
+// O * inv_keep / l rounded to 16 bits at out + i * ldo (out: this thread's first column in the segment's row 0).
+template <bool kBF16>
+__device__ __forceinline__ void write_rows(const float (&o)[32], const float (&m_run)[2], const float (&l_run)[2], const int i0,
+                                           const int n_rows, uint16_t* out, const int64_t ldo, float* lse,
+                                           const float inv_keep, const uint32_t lane) {
 #pragma unroll
-    for (int k = 0; k < BK / 16; ++k) {
-        const uint32_t a[4] = {pa[4 * k], pa[4 * k + 1], pa[4 * k + 2], pa[4 * k + 3]};
-        const uint64_t bdesc = ab::wgmma_desc_sw128(sV + slot * TILE_BYTES + k * 2048u, 8192);
-        ab::wgmma_m64n64k16_rs<kBF16, 1>(o, a, bdesc, 1);
+    for (int hh = 0; hh < 2; ++hh) {
+        const float l = quad_sum(l_run[hh]);
+        const int i = i0 + 8 * hh;
+        if (i >= n_rows) continue;
+        const float inv = inv_keep / l;
+        if (lse != nullptr && (lane & 3u) == 0u) lse[i] = m_run[hh] * (1.0f / LOG2E) + __logf(l);
+        uint16_t* dst = out + i * ldo;
+#pragma unroll
+        for (int j = 0; j < 8; ++j)
+            *reinterpret_cast<uint32_t*>(dst + 8 * j) = pack2<kBF16>(o[4 * j + 2 * hh] * inv, o[4 * j + 2 * hh + 1] * inv);
     }
-    ab::wgmma_commit();
-    ab::wgmma_wait<0>();
-    ab::wgmma_reg_fence(o);
+}
+
+// Shared-memory tables of attention_kernel and attention_long_kernel, both times log2e, written by nthreads threads: the key
+// mask of segment b for keys 0 .. 64 nkb - 1 (-inf past Lk) and, if has_bias, entries d0 .. d0 + n_bias - 1 of head h's row
+// of the [H, Lq + Lk - 1] bias table plus the causal value where j > i (entries past the table stay finite: 0).
+__device__ __forceinline__ void stage_tables(float* s_mask, float* s_bias, const Params& p, const int b, const int h,
+                                             const int nkb, const bool has_bias, const int d0, const int n_bias,
+                                             const int nthreads) {
+    for (int j = threadIdx.x; j < nkb * BK; j += nthreads)
+        s_mask[j] = (j < p.Lk) ? (p.add_mask ? p.add_mask[static_cast<size_t>(b) * p.Lk + j] * LOG2E : 0.f) : -INFINITY;
+    if (!has_bias) return;
+    const int n_valid = p.Lq + p.Lk - 1;
+    for (int t = threadIdx.x; t < n_bias; t += nthreads) {
+        const int d = d0 + t;
+        float v = 0.f;
+        if (d < n_valid) {
+            v = p.bias_delta ? p.bias_delta[static_cast<size_t>(h) * n_valid + d] : 0.f;
+            if (p.causal_value != 0.f && d > p.Lq - 1) v += p.causal_value;   // j > i
+        }
+        s_bias[t] = v * LOG2E;
+    }
+}
+
+// Per-row constants of attention_kernel and attention_long_kernel for rows r and r + 8: the staged bias row (s_bias holds the
+// table from the offset of row bias_off to key 0) and the dropout row.  Rows past Lq, which are not stored, take row Lq - 1.
+__device__ __forceinline__ void row_setup(const float* (&bias)[2], uint64_t (&R)[2], const float* s_bias, const int bias_off,
+                                          const Params& p, const int b, const int h, const int i0) {
+#pragma unroll
+    for (int hh = 0; hh < 2; ++hh) {
+        const int i = min(i0 + 8 * hh, p.Lq - 1);
+        bias[hh] = s_bias + bias_off - i;
+        R[hh] = (static_cast<uint64_t>(b / p.q_div) * p.H + h) * p.Lq + i;
+    }
 }
 
 // grid = (query tiles, H, B)
@@ -230,19 +302,7 @@ attention_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_consta
     }
     // mask / bias tables while the loads are in flight
     const bool has_bias = (p.bias_delta != nullptr) || (p.causal_value != 0.f);
-    for (int j = threadIdx.x; j < nkb * BK; j += THREADS)
-        s_mask[j] = (j < p.Lk) ? (p.add_mask ? p.add_mask[static_cast<size_t>(b) * p.Lk + j] * LOG2E : 0.f) : -INFINITY;
-    if (has_bias) {
-        const int n_valid = p.Lq + p.Lk - 1;
-        for (int d = threadIdx.x; d < 2 * MAX_LK + BK; d += THREADS) {   // entries past the valid offsets stay finite (0)
-            float v = 0.f;
-            if (d < n_valid) {
-                v = p.bias_delta ? p.bias_delta[static_cast<size_t>(h) * n_valid + d] : 0.f;
-                if (p.causal_value != 0.f && d > p.Lq - 1) v += p.causal_value;   // j > i
-            }
-            s_bias[d] = v * LOG2E;
-        }
-    }
+    stage_tables(s_mask, s_bias, p, b, h, nkb, has_bias, 0, 2 * MAX_LK + BK, THREADS);
     __syncthreads();
     ab::mbar_wait(&load_bar, 0, 40);
 
@@ -252,6 +312,9 @@ attention_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_consta
     const int cq = static_cast<int>(2u * (lane & 3u));
     const float scale2 = p.scale * LOG2E;
     const bool dropping = p.drop.thr16 != 0u;
+    const float* bias[2];
+    uint64_t R[2];
+    row_setup(bias, R, s_bias, p.Lq - 1, p, b, h, i0);
     float o[32];
 #pragma unroll
     for (int x = 0; x < 32; ++x) o[x] = 0.f;
@@ -259,128 +322,48 @@ attention_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_consta
 
     for (int kb = 0; kb < nkb; ++kb) {
         if (!((live >> kb) & 1u)) continue;
-        float sc[32];
-        ab::wgmma_fence();
-#pragma unroll
-        for (int k = 0; k < D / 16; ++k) {
-            const uint64_t adesc = ab::wgmma_desc_sw128(sQ + g * 8192u + k * 32u);
-            const uint64_t bdesc = ab::wgmma_desc_sw128(sK + kb * TILE_BYTES + k * 32u);
-            ab::wgmma_m64n64k16_ss<kBF16, 0, 0>(sc, adesc, bdesc, k);
-        }
-        ab::wgmma_commit();
-        ab::wgmma_wait<0>();
-        ab::wgmma_reg_fence(sc);
-
-        // t = S * scale2 + (mask + bias) in the log2 domain; new row maxima
-        float mx[2] = {m_run[0], m_run[1]};
-#pragma unroll
-        for (int j = 0; j < 8; ++j) {
-#pragma unroll
-            for (int c = 0; c < 2; ++c) {
-                const int key = kb * BK + 8 * j + cq + c;
-                const float mk = s_mask[key];
-#pragma unroll
-                for (int hh = 0; hh < 2; ++hh) {
-                    float a = mk;
-                    if (has_bias) a += s_bias[key - min(i0 + 8 * hh, p.Lq - 1) + (p.Lq - 1)];   // rows past Lq are not stored
-                    const float t = fmaf(sc[4 * j + 2 * hh + c], scale2, a);
-                    sc[4 * j + 2 * hh + c] = t;
-                    mx[hh] = fmaxf(mx[hh], t);
-                }
-            }
-        }
-        float corr[2], base[2];
-#pragma unroll
-        for (int hh = 0; hh < 2; ++hh) {
-            mx[hh] = fmaxf(mx[hh], __shfl_xor_sync(0xffffffffu, mx[hh], 1));
-            mx[hh] = fmaxf(mx[hh], __shfl_xor_sync(0xffffffffu, mx[hh], 2));
-            base[hh] = mx[hh] == -INFINITY ? 0.f : mx[hh];
-            corr[hh] = ex2_approx(m_run[hh] - base[hh]);     // 0 for the first block (m_run = -inf)
-            m_run[hh] = mx[hh];
-            l_run[hh] *= corr[hh];
-        }
-#pragma unroll
-        for (int j = 0; j < 8; ++j) {
-            o[4 * j] *= corr[0];
-            o[4 * j + 1] *= corr[0];
-            o[4 * j + 2] *= corr[1];
-            o[4 * j + 3] *= corr[1];
-        }
-        // p = 2^(t - m); the row sum takes every probability, the P operand only the kept ones (dropout)
+        float sc[32], corr[2];
         uint32_t pa[16];
-#pragma unroll
-        for (int hh = 0; hh < 2; ++hh) {
-            uint32_t w[2][4];
-            if (dropping) {
-                const uint64_t R = (static_cast<uint64_t>(b / p.q_div) * p.H + h) * p.Lq + min(i0 + 8 * hh, p.Lq - 1);
-#pragma unroll
-                for (int gg = 0; gg < 2; ++gg) {
-                    const uint32_t G = static_cast<uint32_t>(((b % p.q_div) * p.Lk + kb * BK + gg * 32) >> 5);
-                    abdrop::attn_words(p.drop, R, G, static_cast<uint32_t>(lane & 3u), w[gg]);
-                }
-            }
-#pragma unroll
-            for (int j = 0; j < 8; ++j) {
-                const float e0 = ex2_approx(sc[4 * j + 2 * hh] - base[hh]);
-                const float e1 = ex2_approx(sc[4 * j + 2 * hh + 1] - base[hh]);
-                l_run[hh] += e0 + e1;
-                float k0 = e0, k1 = e1;
-                if (dropping) {
-                    const uint32_t word = w[j >> 2][j & 3];
-                    k0 = abdrop::keep_lo(p.drop, word) ? e0 : 0.f;
-                    k1 = abdrop::keep_hi(p.drop, word) ? e1 : 0.f;
-                }
-                // A fragment of k16 step j / 2: a0 = (r, keys 0-7), a1 = (r + 8, keys 0-7), a2 / a3 = keys 8-15
-                pa[4 * (j >> 1) + 2 * (j & 1) + hh] = pack2<kBF16>(k0, k1);
-            }
-        }
         ab::wgmma_fence();
-#pragma unroll
-        for (int k = 0; k < BK / 16; ++k) {
-            const uint32_t a[4] = {pa[4 * k], pa[4 * k + 1], pa[4 * k + 2], pa[4 * k + 3]};
-            const uint64_t bdesc = ab::wgmma_desc_sw128(sV + kb * TILE_BYTES + k * 2048u, 8192);
-            ab::wgmma_m64n64k16_rs<kBF16, 1>(o, a, bdesc, 1);
-        }
-        ab::wgmma_commit();
+        issue_s<kBF16>(sc, sQ + g * 8192u, sK + kb * TILE_BYTES);
+        ab::wgmma_wait<0>();
+        block_softmax(sc, m_run, l_run, corr, s_mask, bias, has_bias, kb * BK + cq, scale2);
+        rescale_and_pack<kBF16>(pa, o, sc, corr);
+        if (dropping) drop_probs(pa, p.drop, R, (b % p.q_div) * p.Lk + kb * BK, lane);
+        ab::wgmma_fence();
+        issue_pv<kBF16>(o, pa, sV + kb * TILE_BYTES);
         ab::wgmma_wait<0>();
         ab::wgmma_reg_fence(o);
     }
 
-    // ---- output: full row sums across the quad, then normalised 16-bit rows or split-KV partials
+    // ---- output: normalised 16-bit rows, or split-KV partials (un-normalised fp32 O, row max and row sum)
+    if (p.o_partial == nullptr) {
+        write_rows<kBF16>(o, m_run, l_run, i0, p.Lq, p.O + static_cast<size_t>(o_row0) * p.ldo + h * D + cq, p.ldo,
+                          p.lse_out ? p.lse_out + (static_cast<size_t>(b) * p.H + h) * p.Lq : nullptr, p.drop.inv_keep, lane);
+        return;
+    }
 #pragma unroll
     for (int hh = 0; hh < 2; ++hh) {
-        float l = l_run[hh];
-        l += __shfl_xor_sync(0xffffffffu, l, 1);
-        l += __shfl_xor_sync(0xffffffffu, l, 2);
+        const float l = quad_sum(l_run[hh]);
         const int i = i0 + 8 * hh;
         if (i >= p.Lq) continue;
         const size_t orow = static_cast<size_t>(o_row0) + i;
-        if (p.o_partial != nullptr) {
-            const float ik = p.drop.inv_keep;
-            float* dst = p.o_partial + orow * (static_cast<size_t>(p.H) * D) + h * D + cq;
+        const float ik = p.drop.inv_keep;
+        float* dst = p.o_partial + orow * (static_cast<size_t>(p.H) * D) + h * D + cq;
 #pragma unroll
-            for (int j = 0; j < 8; ++j)
-                *reinterpret_cast<float2*>(dst + 8 * j) = make_float2(o[4 * j + 2 * hh] * ik, o[4 * j + 2 * hh + 1] * ik);
-            if ((lane & 3u) == 0u) {
-                float* ml = p.ml_partial + (orow * p.H + h) * 2;
-                ml[0] = m_run[hh] * (1.0f / LOG2E);
-                ml[1] = l;
-            }
-        } else {
-            const float inv = p.drop.inv_keep / l;
-            if (p.lse_out != nullptr && (lane & 3u) == 0u)
-                p.lse_out[(static_cast<size_t>(b) * p.H + h) * p.Lq + i] = m_run[hh] * (1.0f / LOG2E) + __logf(l);
-            uint16_t* dst = p.O + orow * p.ldo + h * D + cq;
-#pragma unroll
-            for (int j = 0; j < 8; ++j)
-                *reinterpret_cast<uint32_t*>(dst + 8 * j) = pack2<kBF16>(o[4 * j + 2 * hh] * inv, o[4 * j + 2 * hh + 1] * inv);
+        for (int j = 0; j < 8; ++j)
+            *reinterpret_cast<float2*>(dst + 8 * j) = make_float2(o[4 * j + 2 * hh] * ik, o[4 * j + 2 * hh + 1] * ik);
+        if ((lane & 3u) == 0u) {
+            float* ml = p.ml_partial + (orow * p.H + h) * 2;
+            ml[0] = m_run[hh] * (1.0f / LOG2E);
+            ml[1] = l;
         }
     }
 }
 
 // ---- attention_long_kernel: the same contract for Lk up to LONG_MAX_LK keys (no split-KV partials, no packed layout).  K and V
 // stream through a LONG_STAGES-deep ring of 64-key tiles: one producer warp issues their TMA loads (full / empty mbarriers),
-// the two consumer warpgroups of attention_kernel sweep the live blocks with attend_block.  The CTA's slice of the bias table
+// the two consumer warpgroups of attention_kernel sweep the live blocks.  The CTA's slice of the bias table
 // (offsets of its 128 query rows to every key) and the key mask are staged in shared memory once.
 constexpr int LONG_MAX_LK = 4096;              // Lq + Lk - 1 <= 8192: the bias table of the backward (attention_bwd.cu)
 constexpr int LONG_STAGES = 4;
@@ -450,24 +433,10 @@ attention_long_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_c
         produce(LONG_STAGES);
     }
     // mask and the bias slice: offsets d_lo .. d_lo + 64 nkb + 126 of the [H, Lq + Lk - 1] table, d_lo = that of the tile's
-    // last (clamped) row to key 0; entries past the valid offsets stay finite (0)
+    // last (clamped) row, bias_off, to key 0
     const bool has_bias = (p.bias_delta != nullptr) || (p.causal_value != 0.f);
-    for (int j = threadIdx.x; j < nkb * BK; j += LONG_THREADS)
-        s_mask[j] = (j < p.Lk) ? (p.add_mask ? p.add_mask[static_cast<size_t>(b) * p.Lk + j] * LOG2E : 0.f) : -INFINITY;
     const int bias_off = min(qt * BQ + BQ - 1, p.Lq - 1);
-    if (has_bias) {
-        const int n_valid = p.Lq + p.Lk - 1;
-        const int d_lo = (p.Lq - 1) - bias_off;
-        for (int t = threadIdx.x; t < nkb * BK + BQ - 1; t += LONG_THREADS) {
-            const int d = d_lo + t;
-            float v = 0.f;
-            if (d < n_valid) {
-                v = p.bias_delta ? p.bias_delta[static_cast<size_t>(h) * n_valid + d] : 0.f;
-                if (p.causal_value != 0.f && d > p.Lq - 1) v += p.causal_value;   // j > i
-            }
-            s_bias[t] = v * LOG2E;
-        }
-    }
+    stage_tables(s_mask, s_bias, p, b, h, nkb, has_bias, (p.Lq - 1) - bias_off, nkb * BK + BQ - 1, LONG_THREADS);
     __syncthreads();
     if (producer) {
         if (lane == 0) produce(nkb);
@@ -480,6 +449,9 @@ attention_long_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_c
     const int cq = static_cast<int>(2u * (lane & 3u));
     const float scale2 = p.scale * LOG2E;
     const bool dropping = p.drop.thr16 != 0u;
+    const float* bias[2];
+    uint64_t R[2];
+    row_setup(bias, R, s_bias, bias_off, p, b, h, i0);
     float o[32];
 #pragma unroll
     for (int x = 0; x < 32; ++x) o[x] = 0.f;
@@ -490,28 +462,25 @@ attention_long_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_c
         if (!all_live && !s_live[kb]) continue;
         const int s = n_used % LONG_STAGES;
         ab::mbar_wait(&full_bar[s], (n_used / LONG_STAGES) & 1, 52);
-        attend_block<kBF16>(o, m_run, l_run, sQ, g, sK, sV, s, s_mask, s_bias, bias_off, has_bias, kb, i0, cq, scale2,
-                            dropping, p, b, h, lane);
+        float sc[32], corr[2];
+        uint32_t pa[16];
+        ab::wgmma_fence();
+        issue_s<kBF16>(sc, sQ + g * 8192u, sK + s * TILE_BYTES);
+        ab::wgmma_wait<0>();
+        block_softmax(sc, m_run, l_run, corr, s_mask, bias, has_bias, kb * BK + cq, scale2);
+        rescale_and_pack<kBF16>(pa, o, sc, corr);
+        if (dropping) drop_probs(pa, p.drop, R, (b % p.q_div) * p.Lk + kb * BK, lane);
+        ab::wgmma_fence();
+        issue_pv<kBF16>(o, pa, sV + s * TILE_BYTES);
+        ab::wgmma_wait<0>();
+        ab::wgmma_reg_fence(o);
         __syncwarp();
         if (lane == 0) ab::mbar_arrive(&empty_bar[s]);     // this warp's MMAs on the slot have completed
         ++n_used;
     }
 
-#pragma unroll
-    for (int hh = 0; hh < 2; ++hh) {
-        float l = l_run[hh];
-        l += __shfl_xor_sync(0xffffffffu, l, 1);
-        l += __shfl_xor_sync(0xffffffffu, l, 2);
-        const int i = i0 + 8 * hh;
-        if (i >= p.Lq) continue;
-        const float inv = p.drop.inv_keep / l;
-        if (p.lse_out != nullptr && (lane & 3u) == 0u)
-            p.lse_out[(static_cast<size_t>(b) * p.H + h) * p.Lq + i] = m_run[hh] * (1.0f / LOG2E) + __logf(l);
-        uint16_t* dst = p.O + (static_cast<size_t>(b) * p.Lq + i) * p.ldo + h * D + cq;
-#pragma unroll
-        for (int j = 0; j < 8; ++j)
-            *reinterpret_cast<uint32_t*>(dst + 8 * j) = pack2<kBF16>(o[4 * j + 2 * hh] * inv, o[4 * j + 2 * hh + 1] * inv);
-    }
+    write_rows<kBF16>(o, m_run, l_run, i0, p.Lq, p.O + static_cast<size_t>(b) * p.Lq * p.ldo + h * D + cq, p.ldo,
+                      p.lse_out ? p.lse_out + (static_cast<size_t>(b) * p.H + h) * p.Lq : nullptr, p.drop.inv_keep, lane);
 }
 
 // ---- attention_packed_kernel: self-attention over the packed rows of the padding-compacted encoders.  Segment b keeps its
@@ -661,123 +630,40 @@ attention_packed_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid
             const int s = qi % PK_Q_STAGES;
             const uint32_t sQs = sQ + s * TILE_BYTES;
             const int i0 = (qi - q0) * BK + static_cast<int>(wl * 16u + (lane >> 2));   // segment row of row r
+            const float* const bias[2] = {s_bias + (p.L - 1) - i0, s_bias + (p.L - 1) - (i0 + 8)};
             ab::mbar_wait_nocall(&full_q[s], (qi / PK_Q_STAGES) & 1);
 
-            float o[32], sc[32];
+            float o[32], sc[32], corr[2];
             uint32_t pa[16];
-            float m_run[2] = {-INFINITY, -INFINITY}, l_run[2] = {0.f, 0.f}, corr[2];
-            auto issue_s = [&](int kb) {
-#pragma unroll
-                for (int kk = 0; kk < D / 16; ++kk)
-                    ab::wgmma_m64n64k16_ss<kBF16, 0, 0>(sc, ab::wgmma_desc_sw128(sQs + kk * 32u),
-                                                        ab::wgmma_desc_sw128(sK + kb * TILE_BYTES + kk * 32u), kk);
-                ab::wgmma_commit();
-            };
-            auto issue_pv = [&](int kb) {
-#pragma unroll
-                for (int kk = 0; kk < BK / 16; ++kk)
-                    ab::wgmma_m64n64k16_rs<kBF16, 1>(o, *reinterpret_cast<const uint32_t(*)[4]>(&pa[4 * kk]),
-                                                     ab::wgmma_desc_sw128(sV + kb * TILE_BYTES + kk * 2048u, 8192), 1);
-                ab::wgmma_commit();
-            };
-            // block kb's softmax on the completed S in sc: sc <- p = 2^(t - m), (m_run, l_run) updated, corr for o
-            auto softmax = [&](int kb) {
-                ab::wgmma_reg_fence(sc);
-                // t = S * scale2 + (mask + bias) in the log2 domain; new row maxima
-                float mx[2] = {m_run[0], m_run[1]};
-#pragma unroll
-                for (int j = 0; j < 8; ++j) {
-#pragma unroll
-                    for (int c = 0; c < 2; ++c) {
-                        const int key = kb * BK + 8 * j + cq + c;
-                        const float mkv = mk[key];
-#pragma unroll
-                        for (int hh = 0; hh < 2; ++hh) {
-                            float a = mkv;
-                            if (has_bias) a += s_bias[key - (i0 + 8 * hh) + (p.L - 1)];
-                            const float t = fmaf(sc[4 * j + 2 * hh + c], scale2, a);
-                            sc[4 * j + 2 * hh + c] = t;
-                            mx[hh] = fmaxf(mx[hh], t);
-                        }
-                    }
-                }
-                float base[2];
-#pragma unroll
-                for (int hh = 0; hh < 2; ++hh) {
-                    mx[hh] = fmaxf(mx[hh], __shfl_xor_sync(0xffffffffu, mx[hh], 1));
-                    mx[hh] = fmaxf(mx[hh], __shfl_xor_sync(0xffffffffu, mx[hh], 2));
-                    base[hh] = mx[hh] == -INFINITY ? 0.f : mx[hh];
-                    corr[hh] = ex2_approx(m_run[hh] - base[hh]);     // 0 for the first block (m_run = -inf)
-                    m_run[hh] = mx[hh];
-                    l_run[hh] *= corr[hh];
-                }
-#pragma unroll
-                for (int hh = 0; hh < 2; ++hh) {
-#pragma unroll
-                    for (int j = 0; j < 8; ++j) {
-                        const float e0 = ex2_approx(sc[4 * j + 2 * hh] - base[hh]);
-                        const float e1 = ex2_approx(sc[4 * j + 2 * hh + 1] - base[hh]);
-                        l_run[hh] += e0 + e1;
-                        sc[4 * j + 2 * hh] = e0;
-                        sc[4 * j + 2 * hh + 1] = e1;
-                    }
-                }
-            };
-            // o *= corr, then P = p rounded to 16 bits as the A fragment of k16 step j / 2: a0 = (r, keys 0-7),
-            // a1 = (r + 8, keys 0-7), a2 / a3 = keys 8-15
-            auto rescale_and_pack = [&]() {
-#pragma unroll
-                for (int j = 0; j < 8; ++j) {
-                    o[4 * j] *= corr[0];
-                    o[4 * j + 1] *= corr[0];
-                    o[4 * j + 2] *= corr[1];
-                    o[4 * j + 3] *= corr[1];
-                }
-#pragma unroll
-                for (int hh = 0; hh < 2; ++hh)
-#pragma unroll
-                    for (int j = 0; j < 8; ++j)
-                        pa[4 * (j >> 1) + 2 * (j & 1) + hh] = pack2<kBF16>(sc[4 * j + 2 * hh], sc[4 * j + 2 * hh + 1]);
-            };
-
+            float m_run[2] = {-INFINITY, -INFINITY}, l_run[2] = {0.f, 0.f};
 #pragma unroll
             for (int x = 0; x < 32; ++x) o[x] = 0.f;
             ab::wgmma_fence();
-            issue_s(0);
+            issue_s<kBF16>(sc, sQs, sK);
             ab::wgmma_wait<0>();
-            softmax(0);
-            rescale_and_pack();
+            block_softmax(sc, m_run, l_run, corr, mk, bias, has_bias, cq, scale2);
+            rescale_and_pack<kBF16>(pa, o, sc, corr);
             for (int kb = 1; kb < n; ++kb) {
                 // S_kb and O += P_{kb-1} V_{kb-1} in flight; the softmax of block kb runs under the P V
                 ab::wgmma_fence();
-                issue_s(kb);
-                issue_pv(kb - 1);
+                issue_s<kBF16>(sc, sQs, sK + kb * TILE_BYTES);
+                issue_pv<kBF16>(o, pa, sV + (kb - 1) * TILE_BYTES);
                 ab::wgmma_wait<1>();
-                softmax(kb);
+                block_softmax(sc, m_run, l_run, corr, mk, bias, has_bias, kb * BK + cq, scale2);
                 ab::wgmma_wait<0>();
                 ab::wgmma_reg_fence(o);
 #pragma unroll
                 for (int x = 0; x < 16; ++x) asm volatile("" : "+r"(pa[x])::"memory");   // P_{kb-1} was read until here
-                rescale_and_pack();
+                rescale_and_pack<kBF16>(pa, o, sc, corr);
             }
             ab::wgmma_fence();
-            issue_pv(n - 1);
+            issue_pv<kBF16>(o, pa, sV + (n - 1) * TILE_BYTES);
             __syncwarp();
             if (lane == 0) ab::mbar_arrive(&empty_q[s]);     // every S of the query tile is complete
             ab::wgmma_wait<0>();
             ab::wgmma_reg_fence(o);
-
-#pragma unroll
-            for (int hh = 0; hh < 2; ++hh) {
-                float l = l_run[hh];
-                l += __shfl_xor_sync(0xffffffffu, l, 1);
-                l += __shfl_xor_sync(0xffffffffu, l, 2);
-                const float inv = 1.0f / l;
-                uint16_t* dst = p.O + (static_cast<size_t>(it.y) + i0 + 8 * hh) * p.ldo + h * D + cq;
-#pragma unroll
-                for (int j = 0; j < 8; ++j)
-                    *reinterpret_cast<uint32_t*>(dst + 8 * j) = pack2<kBF16>(o[4 * j + 2 * hh] * inv, o[4 * j + 2 * hh + 1] * inv);
-            }
+            write_rows<kBF16>(o, m_run, l_run, i0, n * BK, p.O + static_cast<size_t>(it.y) * p.ldo + h * D + cq, p.ldo, nullptr,
+                              1.0f, lane);
         }
         q0 += n;
         __syncwarp();
@@ -785,66 +671,35 @@ attention_packed_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid
     }
 }
 
-template <bool kBF16>
-static int make_tmaps(CUtensorMap& tq, CUtensorMap& tk, CUtensorMap& tv, const void* q, int64_t ldq, const void* k, int64_t ldk,
-                      const void* v, int64_t ldv, int q_rows, int k_rows, const Params& p) {
+static int make_tmaps(CUtensorMap& tq, CUtensorMap& tk, CUtensorMap& tv, const bool bf16, const void* q, int64_t ldq,
+                      const void* k, int64_t ldk, const void* v, int64_t ldv, int q_rows, int k_rows, const Params& p) {
     int rc = abh::make_tmap_2d_16bit(&tq, q, static_cast<uint64_t>(q_rows), static_cast<uint64_t>(p.q_col0 + p.H * D),
-                                     static_cast<uint64_t>(ldq), BK, D, kBF16);
+                                     static_cast<uint64_t>(ldq), BK, D, bf16);
     if (rc) return rc;
     rc = abh::make_tmap_2d_16bit(&tk, k, static_cast<uint64_t>(k_rows), static_cast<uint64_t>(p.k_col0 + p.H * D),
-                                 static_cast<uint64_t>(ldk), BK, D, kBF16);
+                                 static_cast<uint64_t>(ldk), BK, D, bf16);
     if (rc) return rc;
     return abh::make_tmap_2d_16bit(&tv, v, static_cast<uint64_t>(k_rows), static_cast<uint64_t>(p.v_col0 + p.H * D),
-                                   static_cast<uint64_t>(ldv), BK, D, kBF16);
+                                   static_cast<uint64_t>(ldv), BK, D, bf16);
 }
 
-template <bool kBF16>
-static int launch_long(const void* q, int64_t ldq, const void* k, int64_t ldk, const void* v, int64_t ldv, const Params& p,
-                       cudaStream_t s) {
+// One launch of kernel kF16 or kBF16 (by bf16) with kernel parameters kp, on the tensor maps of Q (q_rows rows) and K / V
+// (k_rows rows) with the columns of tp's heads.  Each kernel's dynamic shared-memory limit is raised to max_smem on its
+// first launch.
+template <auto kF16, auto kBF16, typename KP>
+static int launch(const bool bf16, const dim3 grid, const int threads, const size_t smem, const int max_smem, const void* q,
+                  int64_t ldq, const void* k, int64_t ldk, const void* v, int64_t ldv, int q_rows, int k_rows,
+                  const Params& tp, const KP& kp, cudaStream_t s) {
     CUtensorMap tq, tk, tv;
-    const int rc = make_tmaps<kBF16>(tq, tk, tv, q, ldq, k, ldk, v, ldv, p.B * p.Lq, p.B * p.Lk, p);
+    const int rc = make_tmaps(tq, tk, tv, bf16, q, ldq, k, ldk, v, ldv, q_rows, k_rows, tp);
     if (rc) return rc;
-    static bool attr_set = false;
-    if (!attr_set) {
-        AB_CUDA_CHECK(cudaFuncSetAttribute(attention_long_kernel<kBF16>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                           LONG_SMEM_BYTES));
-        attr_set = true;
+    const auto kernel = bf16 ? kBF16 : kF16;
+    static bool attr_set[2] = {false, false};
+    if (!attr_set[bf16]) {
+        AB_CUDA_CHECK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, max_smem));
+        attr_set[bf16] = true;
     }
-    attention_long_kernel<kBF16><<<dim3(static_cast<unsigned>(p.n_qt), static_cast<unsigned>(p.H), static_cast<unsigned>(p.B)),
-                                   LONG_THREADS, LONG_SMEM_BYTES, s>>>(tq, tk, tv, p);
-    AB_CUDA_CHECK(cudaGetLastError());
-    return ATLAS_B200_OK;
-}
-
-template <bool kBF16>
-static int launch(const void* q, int64_t ldq, const void* k, int64_t ldk, const void* v, int64_t ldv, int q_rows, int k_rows,
-                  const Params& p, cudaStream_t s) {
-    CUtensorMap tq, tk, tv;
-    const int rc = make_tmaps<kBF16>(tq, tk, tv, q, ldq, k, ldk, v, ldv, q_rows, k_rows, p);
-    if (rc) return rc;
-    static bool attr_set = false;
-    if (!attr_set) {
-        AB_CUDA_CHECK(cudaFuncSetAttribute(attention_kernel<kBF16>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES));
-        attr_set = true;
-    }
-    attention_kernel<kBF16><<<dim3(static_cast<unsigned>(p.n_qt), static_cast<unsigned>(p.H), static_cast<unsigned>(p.B)),
-                              THREADS, SMEM_BYTES, s>>>(tq, tk, tv, p);
-    AB_CUDA_CHECK(cudaGetLastError());
-    return ATLAS_B200_OK;
-}
-
-template <bool kBF16>
-static int launch_packed(const void* qkv, int64_t ld, int rows, const Params& tp, const PackedParams& p, cudaStream_t s) {
-    CUtensorMap tq, tk, tv;
-    const int rc = make_tmaps<kBF16>(tq, tk, tv, qkv, ld, qkv, ld, qkv, ld, rows, rows, tp);
-    if (rc) return rc;
-    static bool attr_set = false;
-    if (!attr_set) {
-        AB_CUDA_CHECK(cudaFuncSetAttribute(attention_packed_kernel<kBF16>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                           static_cast<int>(packed_smem_bytes(PK_MAX_TILES * BK))));
-        attr_set = true;
-    }
-    attention_packed_kernel<kBF16><<<static_cast<unsigned>(p.G * p.H), PK_THREADS, packed_smem_bytes(p.L), s>>>(tq, tk, tv, p);
+    kernel<<<grid, threads, smem, s>>>(tq, tk, tv, kp);
     AB_CUDA_CHECK(cudaGetLastError());
     return ATLAS_B200_OK;
 }
@@ -949,7 +804,9 @@ int atlas_b200_attention_packed(const void* qkv, int64_t ld, int32_t q_col0, int
     // the packed rows of all segments: at most B * L (the tensor maps only bound the TMA boxes)
     const int rows = B * L;
     abh::prof_begin(ls, abh::PROF_ATTENTION);
-    const int lrc = is_bf16 ? launch_packed<true>(qkv, ld, rows, tp, p, ls) : launch_packed<false>(qkv, ld, rows, tp, p, ls);
+    const int lrc = launch<attention_packed_kernel<false>, attention_packed_kernel<true>>(
+        is_bf16, dim3(p.G * p.H), PK_THREADS, packed_smem_bytes(L), static_cast<int>(packed_smem_bytes(PK_MAX_TILES * BK)), qkv,
+        ld, qkv, ld, qkv, ld, rows, rows, tp, p, ls);
     if (lrc) return lrc;
     // dense-equivalent work, like the masked-block skipping of the padded layout
     abh::prof_end(ls, abh::PROF_ATTENTION, 4.0 * B * H * static_cast<double>(L) * L * attn::D);
@@ -988,8 +845,8 @@ int atlas_b200_attention_train(const void* q, int64_t ldq, int32_t q_col0, const
     p.blk_live = key_block_live;
     cudaStream_t s = static_cast<cudaStream_t>(stream);
     abh::prof_begin(s, abh::PROF_ATTENTION);
-    const int lrc = is_bf16 ? launch<true>(q, ldq, k, ldk, v, ldv, (B / q_div) * Lq, B * Lk, p, s)
-                            : launch<false>(q, ldq, k, ldk, v, ldv, (B / q_div) * Lq, B * Lk, p, s);
+    const int lrc = launch<attention_kernel<false>, attention_kernel<true>>(
+        is_bf16, dim3(p.n_qt, H, B), THREADS, SMEM_BYTES, SMEM_BYTES, q, ldq, k, ldk, v, ldv, (B / q_div) * Lq, B * Lk, p, p, s);
     if (lrc) return lrc;
     abh::prof_end(s, abh::PROF_ATTENTION, 4.0 * B * H * static_cast<double>(Lq) * Lk * D);
     abh::count_launch();
@@ -1019,7 +876,9 @@ int atlas_b200_attention_long(const void* q, int64_t ldq, int32_t q_col0, const 
     p.blk_live = key_block_live;
     cudaStream_t s = static_cast<cudaStream_t>(stream);
     abh::prof_begin(s, abh::PROF_ATTENTION);
-    const int lrc = is_bf16 ? launch_long<true>(q, ldq, k, ldk, v, ldv, p, s) : launch_long<false>(q, ldq, k, ldk, v, ldv, p, s);
+    const int lrc = launch<attention_long_kernel<false>, attention_long_kernel<true>>(
+        is_bf16, dim3(p.n_qt, H, B), LONG_THREADS, LONG_SMEM_BYTES, LONG_SMEM_BYTES, q, ldq, k, ldk, v, ldv, B * Lq, B * Lk, p, p,
+        s);
     if (lrc) return lrc;
     abh::prof_end(s, abh::PROF_ATTENTION, 4.0 * B * H * static_cast<double>(Lq) * Lk * D);
     abh::count_launch();

@@ -133,18 +133,24 @@ def test_rectangular_and_causal_long(dev, dtype, Lq, Lk):
 @pytest.mark.parametrize("dtype", DTYPES)
 @pytest.mark.parametrize("L", [64, 200, 576])
 def test_boundary_both_kernels_meet_the_bound(dev, dtype, L):
-    """At Lk <= 576 both kernels take the input: on the same inputs each meets the same fp64 bound."""
+    """At Lk <= 576 both kernels take the input: on the same inputs each meets the same fp64 bound, and since both run the
+    same per-block functions on the same blocks in the same order, their O and lse are bit-identical, with dropout too."""
     from atlas_b200 import ops
 
     S, H = 3, 4
     mask, bias = _holey_mask(S, L, seed=L + 5), _bias(H, L, L, L + 5)
-    (o_long, lse_long), (qbuf, kvbuf, k_col0, v_col0, Q, K, V, maskd, biasd) = _run_long(
-        dev, dtype, S, H, L, L, mask, bias, 1.0, 0.0, seed=L + 6, qmul=0.35, what=f"boundary L{L}")
-    O64, lse64, bo, bl = afo.forward_bound(Q, K, V, maskd, biasd, 1.0, 0.0, dtype=dtype)
-    out, lse = ops.attention(qbuf, 8, kvbuf, k_col0, kvbuf, v_col0, S, H, L, L, add_mask=maskd, bias_delta=biasd, scale=1.0,
-                             return_lse=True, block_live=ops.key_block_live(maskd))
-    _assert_within(out, O64.reshape(S * L, H * 64), bo.reshape(S * L, H * 64), f"boundary resident L{L} O", "L", dtype)
-    _assert_within(lse, lse64, bl, f"boundary resident L{L} lse", "L-lse", dtype)
+    for dropout in (None, (0.1, 4321, 64)):
+        tag = f"boundary L{L} dropout={dropout is not None}"
+        (o_long, lse_long), (qbuf, kvbuf, k_col0, v_col0, Q, K, V, maskd, biasd) = _run_long(
+            dev, dtype, S, H, L, L, mask, bias, 1.0, 0.0, seed=L + 6, qmul=0.35, what=tag, dropout=dropout)
+        out, lse = ops.attention(qbuf, 8, kvbuf, k_col0, kvbuf, v_col0, S, H, L, L, add_mask=maskd, bias_delta=biasd,
+                                 scale=1.0, return_lse=True, dropout=dropout, block_live=ops.key_block_live(maskd))
+        if dropout is None:
+            O64, lse64, bo, bl = afo.forward_bound(Q, K, V, maskd, biasd, 1.0, 0.0, dtype=dtype)
+            _assert_within(out, O64.reshape(S * L, H * 64), bo.reshape(S * L, H * 64), f"boundary resident L{L} O", "L", dtype)
+            _assert_within(lse, lse64, bl, f"boundary resident L{L} lse", "L-lse", dtype)
+        assert torch.equal(out.view(torch.int16), o_long.view(torch.int16)), f"{tag}: O differs between the kernels"
+        assert torch.equal(lse, lse_long), f"{tag}: lse differs between the kernels"
 
 
 # ------------------------------------------------------------------------------------------------------------------------
