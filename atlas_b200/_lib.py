@@ -59,14 +59,6 @@ def lib():
     ]
     L.atlas_b200_cast_f32.restype = c.c_int
     L.atlas_b200_cast_f32.argtypes = [c.c_void_p, c.c_void_p, c.c_int64, c.c_int32, c.c_void_p]
-    L.atlas_b200_linear.restype = c.c_int
-    L.atlas_b200_linear.argtypes = [c.c_void_p, c.c_int64, c.c_void_p, c.c_int64, c.c_void_p, c.c_void_p, c.c_int64,
-                                    c.c_void_p, c.c_int64, c.c_int32, c.c_int32, c.c_int32, c.c_int32, c.c_int32,
-                                    c.c_void_p]
-    L.atlas_b200_linear_ex.restype = c.c_int
-    L.atlas_b200_linear_ex.argtypes = [c.c_void_p, c.c_int64, c.c_void_p, c.c_int64, c.c_void_p, c.c_void_p, c.c_int64,
-                                       c.c_void_p, c.c_int64, c.c_int32, c.c_int32, c.c_int32, c.c_int32, c.c_int32,
-                                       c.c_void_p, c.c_void_p, c.c_float, c.c_void_p]
     L.atlas_b200_linear_schedule.restype = c.c_int
     L.atlas_b200_linear_schedule.argtypes = [c.c_int32, c.c_int32, c.c_int32, c.c_int32]
     L.atlas_b200_layernorm.restype = c.c_int
@@ -78,14 +70,6 @@ def lib():
     L.atlas_b200_masked_mean_pool.restype = c.c_int
     L.atlas_b200_masked_mean_pool.argtypes = [c.c_void_p, c.c_void_p, c.c_void_p, c.c_int64, c.c_int32, c.c_int32,
                                               c.c_int32, c.c_int32, c.c_void_p]
-    L.atlas_b200_attention.restype = c.c_int
-    L.atlas_b200_attention.argtypes = [c.c_void_p, c.c_int64, c.c_int32, c.c_void_p, c.c_int64, c.c_int32, c.c_void_p,
-                                       c.c_int64, c.c_int32, c.c_void_p, c.c_int64, c.c_void_p, c.c_void_p, c.c_int32,
-                                       c.c_int32, c.c_int32, c.c_int32, c.c_float, c.c_float, c.c_int32, c.c_void_p,
-                                       c.c_void_p, c.c_int32, c.c_void_p]
-    L.atlas_b200_attention_combine.restype = c.c_int
-    L.atlas_b200_attention_combine.argtypes = [c.c_void_p, c.c_void_p, c.c_int32, c.c_int32, c.c_int32, c.c_int32,
-                                               c.c_void_p, c.c_int64, c.c_int32, c.c_void_p]
     L.atlas_b200_profile_enable.restype = None
     L.atlas_b200_profile_enable.argtypes = [c.c_int32]
     L.atlas_b200_profile_work.restype = c.c_double
@@ -95,13 +79,6 @@ def lib():
     L.atlas_b200_profile_collect.restype = c.c_int
     L.atlas_b200_profile_collect.argtypes = [c.POINTER(c.c_double), c.POINTER(c.c_int32)]
     i32, i64, vp, f32 = c.c_int32, c.c_int64, c.c_void_p, c.c_float
-    L.atlas_b200_attention_bwd.restype = c.c_int
-    L.atlas_b200_attention_bwd.argtypes = [vp, i64, i32, vp, i64, i32, vp, i64, i32, vp, i64, vp, i64, vp, i64, i32, vp,
-                                           i64, i32, vp, i64, i32, vp, vp, vp, vp, i32, vp, vp, i32, i32, i32, i32, f32,
-                                           f32, i32, vp]
-    L.atlas_b200_attention_ex.restype = c.c_int
-    L.atlas_b200_attention_ex.argtypes = [vp, i64, i32, vp, i64, i32, vp, i64, i32, vp, i64, vp, vp, i32, i32, i32, i32,
-                                          f32, f32, i32, vp, vp, vp, i32, vp]
     L.atlas_b200_attention_combine_ex.restype = c.c_int
     L.atlas_b200_attention_combine_ex.argtypes = [vp, vp, i32, i32, i32, i32, vp, i64, vp, i32, vp]
     L.atlas_b200_cross_attention_stats.restype = c.c_int
@@ -133,8 +110,6 @@ def lib():
     L.atlas_b200_cross_entropy_fwd.argtypes = [vp, i64, vp, vp, vp, i32, i32, i32, vp]
     L.atlas_b200_cross_entropy_bwd.restype = c.c_int
     L.atlas_b200_cross_entropy_bwd.argtypes = [vp, i64, vp, vp, vp, vp, i64, i32, i32, i32, vp]
-    L.atlas_b200_decode_cross_attention.restype = c.c_int
-    L.atlas_b200_decode_cross_attention.argtypes = [vp, i64, vp, i64, i32, i32, vp, i32, i32, i32, i32, f32, vp, vp, i32, vp]
     L.atlas_b200_decode_cross_attention_live.restype = c.c_int
     L.atlas_b200_decode_cross_attention_live.argtypes = [vp, i64, vp, i64, i32, i32, vp, vp, i32, i32, i32, i32, f32, vp, vp, i32,
                                                          vp]
@@ -164,8 +139,8 @@ def lib():
                                             f32, vp, f32, u64, u64, vp, i32, vp]
     L.atlas_b200_attention_bwd_train.restype = c.c_int
     L.atlas_b200_attention_bwd_train.argtypes = [vp, i64, i32, vp, i64, i32, vp, i64, i32, vp, i64, vp, i64, vp, i64, i32,
-                                                 vp, i64, i32, vp, i64, i32, vp, vp, vp, vp, i32, vp, vp, i32, i32, i32,
-                                                 i32, f32, f32, f32, u64, u64, vp, i32, vp]
+                                                 vp, i64, i32, vp, i64, i32, vp, vp, vp, vp, vp, vp, i32, i32, i32, i32,
+                                                 f32, f32, f32, u64, u64, vp, i32, vp]
     L.atlas_b200_adamw_fp32copy.restype = c.c_int
     L.atlas_b200_adamw_fp32copy.argtypes = [vp, vp, i32, i32, f32, f32, f32, f32, f32, f32, vp]
     L.atlas_b200_grad_stats.restype = c.c_int
@@ -177,8 +152,6 @@ def lib():
                                                     vp, i32, vp]
     L.atlas_b200_compact_live_tiles.restype = c.c_int
     L.atlas_b200_compact_live_tiles.argtypes = [vp, i64, vp, i32, i32, vp, i64, vp, vp, vp]
-    L.atlas_b200_linear_dynm.restype = c.c_int
-    L.atlas_b200_linear_dynm.argtypes = [vp, i64, vp, i64, vp, i64, i32, i32, i32, vp, i32, vp]
     L.atlas_b200_cross_attention_stream_compact.restype = c.c_int
     L.atlas_b200_cross_attention_stream_compact.argtypes = [vp, i64, i32, vp, i64, i32, i32, vp, vp, vp, i32, i32, i32, i32, i32,
                                                             f32, vp, vp, i32, vp]
@@ -231,20 +204,14 @@ EXPORTED_SYMBOLS = [
     "atlas_b200_topk_merge",
     "atlas_b200_search_host",
     "atlas_b200_cast_f32",
-    "atlas_b200_linear",
-    "atlas_b200_linear_ex",
     "atlas_b200_linear_schedule",
     "atlas_b200_layernorm",
     "atlas_b200_bert_embed_ln",
     "atlas_b200_masked_mean_pool",
-    "atlas_b200_attention",
-    "atlas_b200_attention_combine",
     "atlas_b200_profile_enable",
     "atlas_b200_profile_work",
     "atlas_b200_profile_collect",
     "atlas_b200_profile_launches",
-    "atlas_b200_attention_bwd",
-    "atlas_b200_attention_ex",
     "atlas_b200_attention_combine_ex",
     "atlas_b200_cross_attention_stats",
     "atlas_b200_linear_wgrad",
@@ -261,7 +228,6 @@ EXPORTED_SYMBOLS = [
     "atlas_b200_cross_entropy_fwd",
     "atlas_b200_cross_entropy_bwd",
     "atlas_b200_splice_tokens",
-    "atlas_b200_decode_cross_attention",
     "atlas_b200_decode_self_attention",
     "atlas_b200_decode_argmax",
     "atlas_b200_decode_self_attention_beam",
@@ -279,7 +245,6 @@ EXPORTED_SYMBOLS = [
     "atlas_b200_cross_attention_stream",
     "atlas_b200_decode_cross_attention_live",
     "atlas_b200_compact_live_tiles",
-    "atlas_b200_linear_dynm",
     "atlas_b200_cross_attention_stream_compact",
     "atlas_b200_segment_tile_scan",
     "atlas_b200_embed_packed_tiles",

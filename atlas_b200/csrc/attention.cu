@@ -757,25 +757,6 @@ __global__ void combine_splits_kernel(const float* __restrict__ o_partial, const
 
 extern "C" {
 
-int atlas_b200_attention(const void* q, int64_t ldq, int32_t q_col0, const void* k, int64_t ldk, int32_t k_col0,
-                         const void* v, int64_t ldv, int32_t v_col0, void* out, int64_t ldo, const float* add_mask,
-                         const float* bias_delta, int32_t B, int32_t H, int32_t Lq, int32_t Lk, float scale,
-                         float causal_value, int32_t q_div, float* o_partial, float* ml_partial, int32_t is_bf16,
-                         void* stream) {
-    return atlas_b200_attention_ex(q, ldq, q_col0, k, ldk, k_col0, v, ldv, v_col0, out, ldo, add_mask, bias_delta, B, H, Lq,
-                                   Lk, scale, causal_value, q_div, o_partial, ml_partial, nullptr, is_bf16, stream);
-}
-
-int atlas_b200_attention_ex(const void* q, int64_t ldq, int32_t q_col0, const void* k, int64_t ldk, int32_t k_col0,
-                            const void* v, int64_t ldv, int32_t v_col0, void* out, int64_t ldo, const float* add_mask,
-                            const float* bias_delta, int32_t B, int32_t H, int32_t Lq, int32_t Lk, float scale,
-                            float causal_value, int32_t q_div, float* o_partial, float* ml_partial, float* lse_out,
-                            int32_t is_bf16, void* stream) {
-    return atlas_b200_attention_train(q, ldq, q_col0, k, ldk, k_col0, v, ldv, v_col0, out, ldo, add_mask, bias_delta, B, H, Lq,
-                                      Lk, scale, causal_value, q_div, o_partial, ml_partial, lse_out, 0.f, 0, 0, nullptr,
-                                      is_bf16, stream);
-}
-
 // Self-attention over the PACKED rows of the padding-compacted FiD encoder (atlas_b200_segment_tile_scan): segment b keeps the
 // first popcount(keep[b, :]) of its L / 64 tiles, stored back to back from row 64 * tile_off[b * (L / 64)] of qkv / out.
 int atlas_b200_attention_packed(const void* qkv, int64_t ld, int32_t q_col0, int32_t k_col0, int32_t v_col0, void* out, int64_t ldo,
@@ -883,11 +864,6 @@ int atlas_b200_attention_long(const void* q, int64_t ldq, int32_t q_col0, const 
     abh::prof_end(s, abh::PROF_ATTENTION, 4.0 * B * H * static_cast<double>(Lq) * Lk * D);
     abh::count_launch();
     return ATLAS_B200_OK;
-}
-
-int atlas_b200_attention_combine(const float* o_partial, const float* ml_partial, int32_t B, int32_t splits, int32_t Lq,
-                                 int32_t H, void* out, int64_t ldo, int32_t is_bf16, void* stream) {
-    return atlas_b200_attention_combine_ex(o_partial, ml_partial, B, splits, Lq, H, out, ldo, nullptr, is_bf16, stream);
 }
 
 int atlas_b200_attention_combine_ex(const float* o_partial, const float* ml_partial, int32_t B, int32_t splits, int32_t Lq,

@@ -11,7 +11,7 @@
 // Warp-level `mma.sync.m16n8k16` tiles (64 queries x 64 keys per CTA step, 4 warps, operands through XOR-swizzled shared
 // memory + ldmatrix), two kernels so that no output needs atomics:
 //   attn_bwd_dq2_kernel   CTA = (b, h, 64-query block [, key chunk]): reads the row log-sum-exp the forward kernel wrote
-//                         (atlas_b200_attention_ex), writes D_i = sum_d dO O to `dsum`, accumulates dQ over the key blocks
+//                         (atlas_b200_attention_train), writes D_i = sum_d dO O to `dsum`, accumulates dQ over the key blocks
 //                         (cp.async double-buffered K / V tiles); dbias through a staged dS tile + diagonal sums.  A long
 //                         few-query key range (FiD cross-attention) is split over key chunks with fp32 dQ atomics.
 //   attn_bwd_dkv2_kernel  CTA = (b, h, 64-key block): the transposed problem, loops over the query blocks, accumulates dK, dV.
@@ -522,30 +522,16 @@ attn_bwd_dkv2_kernel(const Params p) {
 
 extern "C" {
 
-int atlas_b200_attention_bwd(const void* q, int64_t ldq, int32_t q_col0, const void* k, int64_t ldk, int32_t k_col0,
-                             const void* v, int64_t ldv, int32_t v_col0, const void* out, int64_t ldo, const void* dout,
-                             int64_t lddo, void* dq, int64_t lddq, int32_t dq_col0, void* dk, int64_t lddk,
-                             int32_t dk_col0, void* dv, int64_t lddv, int32_t dv_col0, const float* add_mask,
-                             const float* bias_delta, float* dbias_delta, float* lse, int32_t lse_given, float* dsum,
-                             float* dq_accum, int32_t B, int32_t H, int32_t Lq, int32_t Lk, float scale,
-                             float causal_value, int32_t is_bf16, void* stream) {
-    return atlas_b200_attention_bwd_train(q, ldq, q_col0, k, ldk, k_col0, v, ldv, v_col0, out, ldo, dout, lddo, dq, lddq,
-                                          dq_col0, dk, lddk, dk_col0, dv, lddv, dv_col0, add_mask, bias_delta, dbias_delta,
-                                          lse, lse_given, dsum, dq_accum, B, H, Lq, Lk, scale, causal_value, 0.f, 0, 0, nullptr,
-                                          is_bf16, stream);
-}
-
 int atlas_b200_attention_bwd_train(const void* q, int64_t ldq, int32_t q_col0, const void* k, int64_t ldk, int32_t k_col0,
                                    const void* v, int64_t ldv, int32_t v_col0, const void* out, int64_t ldo,
                                    const void* dout, int64_t lddo, void* dq, int64_t lddq, int32_t dq_col0, void* dk,
                                    int64_t lddk, int32_t dk_col0, void* dv, int64_t lddv, int32_t dv_col0,
                                    const float* add_mask, const float* bias_delta, float* dbias_delta, float* lse,
-                                   int32_t lse_given, float* dsum, float* dq_accum, int32_t B, int32_t H, int32_t Lq,
-                                   int32_t Lk, float scale, float causal_value, float dropout_p, uint64_t seed,
-                                   uint64_t offset, const uint8_t* key_block_live, int32_t is_bf16, void* stream) {
+                                   float* dsum, float* dq_accum, int32_t B, int32_t H, int32_t Lq, int32_t Lk, float scale,
+                                   float causal_value, float dropout_p, uint64_t seed, uint64_t offset,
+                                   const uint8_t* key_block_live, int32_t is_bf16, void* stream) {
     using namespace attnb;
     AB_REQUIRE(dropout_p >= 0.f && dropout_p < 1.f, "attention_bwd: need 0 <= dropout_p < 1 (got %f)", dropout_p);
-    AB_REQUIRE(lse_given != 0, "attention_bwd: the forward's log-sum-exp is required in lse (lse_given != 0)");
     const abdrop::Key drop = abdrop::make_key(dropout_p, seed, offset);
     AB_REQUIRE(dq_accum == nullptr || dbias_delta == nullptr,
                "attention_bwd: dq_accum (keys split over CTAs) cannot be combined with dbias_delta");
@@ -554,7 +540,8 @@ int atlas_b200_attention_bwd_train(const void* q, int64_t ldq, int32_t q_col0, c
                    lddk % 8 == 0 && lddv % 8 == 0 && q_col0 % 8 == 0 && k_col0 % 8 == 0 && v_col0 % 8 == 0 &&
                    dq_col0 % 8 == 0 && dk_col0 % 8 == 0 && dv_col0 % 8 == 0,
                "attention_bwd: strides and column offsets must be multiples of 8 elements");
-    AB_REQUIRE(lse != nullptr && dsum != nullptr, "attention_bwd: lse and dsum ([B, H, Lq] fp32 each) are required");
+    AB_REQUIRE(lse != nullptr && dsum != nullptr,
+               "attention_bwd: lse (the forward's log-sum-exp) and dsum ([B, H, Lq] fp32 each) are required");
     AB_REQUIRE(dbias_delta == nullptr || bias_delta != nullptr, "attention_bwd: dbias_delta without bias_delta");
     const int64_t ntab = static_cast<int64_t>(Lq) + Lk - 1;
     AB_REQUIRE(bias_delta == nullptr || ntab <= 8192, "attention_bwd: Lq + Lk - 1 = %lld exceeds the bias table (8192)",

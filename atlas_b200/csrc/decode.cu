@@ -293,14 +293,6 @@ __global__ void advance_step_kernel(int32_t* t_dev) { *t_dev += 1; }
 
 extern "C" {
 
-int atlas_b200_decode_cross_attention(const void* q, int64_t ldq, const void* kv, int64_t ldkv, int32_t k_col0,
-                                      int32_t v_col0, const float* add_mask, int32_t B, int32_t H, int32_t Lk,
-                                      int32_t chunk, float scale, float* o_partial, float* ml_partial, int32_t is_bf16,
-                                      void* stream) {
-    return atlas_b200_decode_cross_attention_live(q, ldq, kv, ldkv, k_col0, v_col0, add_mask, nullptr, B, H, Lk, chunk, scale,
-                                                  o_partial, ml_partial, is_bf16, stream);
-}
-
 int atlas_b200_decode_cross_attention_live(const void* q, int64_t ldq, const void* kv, int64_t ldkv, int32_t k_col0,
                                            int32_t v_col0, const float* add_mask, const uint8_t* tile_live, int32_t B,
                                            int32_t H, int32_t Lk, int32_t chunk, float scale, float* o_partial,

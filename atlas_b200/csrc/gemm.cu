@@ -87,7 +87,7 @@ struct Params {
     // splitk_reduce_kernel sums the partials and rounds once.  splits == 1 / C32 == nullptr: the ordinary epilogues.
     int splits, kb_per_split;
     float* C32;
-    int l2_prefetch;      // producer prefetches the next work item's A rows into L2 (ATLAS_B200_GEMM_PREFETCH=0: off)
+    int l2_prefetch;      // producer prefetches the next work item's A rows into L2 (off for the weight gradients)
     const int32_t* m_dev; // optional: the number of valid rows lives in device memory (<= M): only ceil(*m_dev / tile) row blocks
                           // are computed (compacted activations under a CUDA graph: the launch shape stays static)
 };
@@ -919,47 +919,11 @@ splitk_reduce_kernel(const float* __restrict__ part, uint16_t* __restrict__ out,
 
 }  // namespace gemm
 
-// device-side row count of the NEXT atlas_b200_linear_ex call of this thread (atlas_b200_linear_dynm sets it)
-static thread_local const int32_t* g_next_m_dev = nullptr;
-
 extern "C" {
 
-int atlas_b200_linear_ex(const void* A, int64_t lda, const void* W, int64_t ldw, const void* bias, const void* residual,
-                         int64_t ldr, void* C, int64_t ldc, int32_t M, int32_t N, int32_t K, int32_t epilogue,
-                         int32_t is_bf16, const float* row_ss, float* out_ss, float rs_eps, void* stream);
-
-int atlas_b200_linear_dynm(const void* A, int64_t lda, const void* W, int64_t ldw, void* C, int64_t ldc, int32_t M_max, int32_t N,
-                           int32_t K, const int32_t* m_dev, int32_t is_bf16, void* stream) {
-    AB_REQUIRE(m_dev != nullptr, "linear_dynm: m_dev is required");
-    g_next_m_dev = m_dev;
-    const int rc = atlas_b200_linear_ex(A, lda, W, ldw, nullptr, nullptr, 0, C, ldc, M_max, N, K, gemm::EPI_NONE, is_bf16, nullptr,
-                                        nullptr, 0.f, stream);
-    g_next_m_dev = nullptr;
-    return rc;
-}
-
-// atlas_b200_linear_ex over the first *m_dev rows only (m_dev in device memory, <= M_max; nullptr = all M_max rows): the encoder
-// of the padding-compacted FiD forward (fid.py: encode_compact) runs every projection this way
 int atlas_b200_linear_rows(const void* A, int64_t lda, const void* W, int64_t ldw, const void* bias, const void* residual,
-                           int64_t ldr, void* C, int64_t ldc, int32_t M_max, int32_t N, int32_t K, int32_t epilogue,
+                           int64_t ldr, void* C, int64_t ldc, int32_t M, int32_t N, int32_t K, int32_t epilogue,
                            int32_t is_bf16, const float* row_ss, float* out_ss, float rs_eps, const int32_t* m_dev, void* stream) {
-    g_next_m_dev = m_dev;
-    const int rc = atlas_b200_linear_ex(A, lda, W, ldw, bias, residual, ldr, C, ldc, M_max, N, K, epilogue, is_bf16, row_ss, out_ss,
-                                        rs_eps, stream);
-    g_next_m_dev = nullptr;
-    return rc;
-}
-
-int atlas_b200_linear(const void* A, int64_t lda, const void* W, int64_t ldw, const void* bias, const void* residual,
-                      int64_t ldr, void* C, int64_t ldc, int32_t M, int32_t N, int32_t K, int32_t epilogue,
-                      int32_t is_bf16, void* stream) {
-    return atlas_b200_linear_ex(A, lda, W, ldw, bias, residual, ldr, C, ldc, M, N, K, epilogue, is_bf16, nullptr, nullptr,
-                                0.f, stream);
-}
-
-int atlas_b200_linear_ex(const void* A, int64_t lda, const void* W, int64_t ldw, const void* bias, const void* residual,
-                         int64_t ldr, void* C, int64_t ldc, int32_t M, int32_t N, int32_t K, int32_t epilogue,
-                         int32_t is_bf16, const float* row_ss, float* out_ss, float rs_eps, void* stream) {
     using namespace gemm;
     AB_REQUIRE(M >= 0 && N > 0 && K > 0, "bad GEMM shape M=%d N=%d K=%d", M, N, K);
     if (M == 0) return ATLAS_B200_OK;
@@ -974,10 +938,8 @@ int atlas_b200_linear_ex(const void* A, int64_t lda, const void* W, int64_t ldw,
     p.splits = 1;
     p.kb_per_split = (K + BLOCK_K - 1) / BLOCK_K;
     p.C32 = nullptr;
-    static const int pf_on = (getenv("ATLAS_B200_GEMM_PREFETCH") != nullptr && getenv("ATLAS_B200_GEMM_PREFETCH")[0] == '0') ? 0 : 1;
-    p.l2_prefetch = pf_on;
-    p.m_dev = g_next_m_dev;
-    g_next_m_dev = nullptr;
+    p.l2_prefetch = 1;
+    p.m_dev = m_dev;
     p.row_ss = row_ss;
     p.out_ss = out_ss;
     p.rs_eps = rs_eps;

@@ -11,7 +11,7 @@
 // order (<= 256 points per centroid), the first k rows are the initial centroids, `iters` Lloyd iterations, an empty
 // cluster is re-seeded by splitting the largest one with a symmetric 1/1024 perturbation.  Deterministic: assignments are
 // argmin / argmax with the lowest index on ties, centroid sums run over the members in sample order (no float atomics).
-//   coarse assignment  the wgmma GEMM atlas_b200_linear (fp16 rows x fp16 copy of the centroids) + a row argmax
+//   coarse assignment  the wgmma GEMM atlas_b200_linear_rows (fp16 rows x fp16 copy of the centroids) + a row argmax
 //   PQ assignment      ||c||^2 - 2 <r, c> in fp32 on CUDA cores (pq_subdot_kernel + pq_argmin_kernel), residuals in fp32
 //
 // Search per block of <= 256 queries: fp32 lookup tables LUT[q][m][256] (and coarse terms T[q][list] for ivfpq) from the
@@ -518,7 +518,8 @@ static int coarse_assign(const __half* x, int64_t n, const __half* coarse16, int
     const int nlp = pad8(n_list);
     for (int64_t r0 = 0; r0 < n; r0 += R) {
         const int rows = static_cast<int>(n - r0 < R ? n - r0 : R);
-        int rc = atlas_b200_linear(x + r0 * DIM, DIM, coarse16, DIM, nullptr, nullptr, 0, w.gemm, nlp, rows, nlp, DIM, 0, 0, s);
+        int rc = atlas_b200_linear_rows(x + r0 * DIM, DIM, coarse16, DIM, nullptr, nullptr, 0, w.gemm, nlp, rows, nlp, DIM, 0, 0,
+                                        nullptr, nullptr, 0.f, nullptr, s);
         if (rc) return rc;
         pq_argmax_rows_kernel<<<grid_1d(static_cast<int64_t>(rows) * 32, 256), 256, 0, s>>>(
             w.gemm, nlp, rows, n_list, assign ? assign + r0 : nullptr,

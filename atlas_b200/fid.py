@@ -453,7 +453,7 @@ class FiD(nn.Module):
         qkv = torch.empty((S * L, 3 * H * 64), dtype=dt, device=h.device)
         eps = c.layer_norm_epsilon
         if self.fuse_norm:
-            # RMSNorm fused around the GEMMs (atlas_b200_linear_ex): the residual GEMMs emit each row's sum of squares,
+            # RMSNorm fused around the GEMMs (row_ss / out_ss of ops.linear): the residual GEMMs emit each row's sum of squares,
             # the consuming projection reads the UN-normalised hidden state with the norm weight folded into its matrix
             # and scales its accumulator rows by rsqrt(ss / d + eps).  Only the very first and the final norm run as
             # kernels; 2 x num_layers normalised [tokens, d] tensors are never written or read.
@@ -539,14 +539,14 @@ class FiD(nn.Module):
             # the encoder already ran on its kept tiles (a superset of the live ones, same tile order): project those rows
             enc_live, keep, tile_off, n_live_rows = enc_packed
             cross_live = keep.view(B, Lk // 64)
-            xkv = [ops.linear_dynm(enc_live, G[f"decoder.block.{i}.layer.1.EncDecAttention.kv"], n_live_rows)
+            xkv = [ops.linear(enc_live, G[f"decoder.block.{i}.layer.1.EncDecAttention.kv"], rows=n_live_rows)
                    for i in range(c.num_decoder_layers)]
         elif compact:
             flat = enc.reshape(-1, d)
             if flat.dtype != dt:
                 flat = flat.to(dt)
             enc_live, tile_off, n_live_rows = ops.compact_live_tiles(flat, cross_live)
-            xkv = [ops.linear_dynm(enc_live, G[f"decoder.block.{i}.layer.1.EncDecAttention.kv"], n_live_rows)
+            xkv = [ops.linear(enc_live, G[f"decoder.block.{i}.layer.1.EncDecAttention.kv"], rows=n_live_rows)
                    for i in range(c.num_decoder_layers)]
         elif cross_kv is None:
             cross_kv = self.cross_kv(enc)

@@ -289,10 +289,10 @@ def linear(x, weight, bias=None, residual=None, epilogue=None, out=None, row_ss=
 
     epilogue: EPI_NONE / EPI_BIAS / EPI_GELU / EPI_RESIDUAL / EPI_GATED / EPI_RELU (see include/atlas_b200.h);
     default: EPI_RESIDUAL if `residual` is given, else EPI_BIAS if `bias` is given, else EPI_NONE.
-    Fused T5 RMSNorm (atlas_b200_linear_ex): `row_ss` fp32 [M] = sum of squares of the rows of x -> accumulator rows are
+    Fused T5 RMSNorm: `row_ss` fp32 [M] = sum of squares of the rows of x -> accumulator rows are
     scaled by rsqrt(row_ss / K + rs_eps) (x is the UN-normalised hidden state, the norm weight is folded into `weight`);
     `out_ss` fp32 [M] (pre-zeroed) receives the sum of squares of the stored output rows.
-    `rows`: int32 [1] device tensor - only the first *rows rows are computed (atlas_b200_linear_rows; static launch shape)."""
+    `rows`: int32 [1] device tensor - only the first *rows rows are computed (static launch shape)."""
     require_cuda(x, "x")
     if x.dtype not in (torch.float16, torch.bfloat16) or weight.dtype != x.dtype:
         raise AtlasB200Error(f"linear: x and weight must both be fp16 or bf16 (got {x.dtype}, {weight.dtype})")
@@ -531,21 +531,21 @@ def expand_packed_tiles(x, tile_off):
     return out
 
 
-def linear_dynm(x, weight, m_dev, out=None):
-    """y[m] = x[m] @ weight.T for m < *m_dev (device int32): row blocks past the device-side count are skipped."""
-    require_cuda(x, "x")
-    M, K = x.shape
-    N = weight.shape[0]
+def _combine(o_part, ml, B, splits, Lq, H, dtype, out=None, return_lse=False):
+    """Merge the split-KV partials o_part [B*splits*Lq, H*64] / ml [B*splits*Lq, H, 2] (atlas_b200_attention_combine_ex)
+    -> out [B*Lq, H*64] in `dtype` (and the row log-sum-exp [B, H, Lq] fp32 over all splits with return_lse)."""
     if out is None:
-        out = torch.empty((M, N), dtype=x.dtype, device=x.device)
-    check(lib().atlas_b200_linear_dynm(_ptr(x), x.stride(0), _ptr(weight), weight.stride(0), _ptr(out), out.stride(0), M, N, K,
-                                       _ptr(m_dev), _bf(x), current_stream_ptr()))
-    return out
+        out = torch.empty((B * Lq, H * 64), dtype=dtype, device=o_part.device)
+    lse = torch.empty((B, H, Lq), dtype=torch.float32, device=o_part.device) if return_lse else None
+    check(lib().atlas_b200_attention_combine_ex(_ptr(o_part), _ptr(ml), B, splits, Lq, H, _ptr(out), out.stride(0),
+                                                _ptr(lse) if lse is not None else None, 1 if dtype == torch.bfloat16 else 0,
+                                                current_stream_ptr()))
+    return (out, lse) if return_lse else out
 
 
 def cross_attention_stream_compact(q, kv_live, tile_live, tile_off, B, H, Lq, Lk_total, add_mask, scale=1.0, return_lse=False):
     """`cross_attention_split` on the stream kernel with K | V given as the compacted live tiles (`compact_live_tiles` of the
-    encoder output, projected by `linear_dynm`)."""
+    encoder output, projected by `linear(..., rows=count)`)."""
     require_cuda(q, "q")
     am = add_mask.float().contiguous()
     chunk = _XATTN_CHUNK
@@ -556,11 +556,7 @@ def cross_attention_stream_compact(q, kv_live, tile_live, tile_off, B, H, Lq, Lk
                                                           _ptr(am), _ptr(tile_live), _ptr(tile_off), B, H, Lq, Lk_total,
                                                           chunk, float(scale), _ptr(o_part), _ptr(ml), _bf(q),
                                                           current_stream_ptr()))
-    out = torch.empty((B * Lq, H * 64), dtype=q.dtype, device=q.device)
-    lse = torch.empty((B, H, Lq), dtype=torch.float32, device=q.device) if return_lse else None
-    check(lib().atlas_b200_attention_combine_ex(_ptr(o_part), _ptr(ml), B, chunks, Lq, H, _ptr(out), out.stride(0),
-                                                _ptr(lse) if lse is not None else None, _bf(q), current_stream_ptr()))
-    return (out, lse) if return_lse else out
+    return _combine(o_part, ml, B, chunks, Lq, H, q.dtype, return_lse=return_lse)
 
 
 _XATTN_STREAM = os.environ.get("ATLAS_B200_XATTN_STREAM", "1") != "0"      # A/B switch of the stream kernel
@@ -586,11 +582,7 @@ def cross_attention_split(q, q_col0, kv, k_col0, v_col0, B, H, Lq, Lk_total, add
                                                       _ptr(tile_live) if tile_live is not None else None, B, H, Lq, Lk_total,
                                                       chunk, float(scale), _ptr(o_part), _ptr(ml), _bf(q),
                                                       current_stream_ptr()))
-        out = torch.empty((B * Lq, H * 64), dtype=q.dtype, device=q.device)
-        lse = torch.empty((B, H, Lq), dtype=torch.float32, device=q.device) if return_lse else None
-        check(lib().atlas_b200_attention_combine_ex(_ptr(o_part), _ptr(ml), B, chunks, Lq, H, _ptr(out), out.stride(0),
-                                                    _ptr(lse) if lse is not None else None, _bf(q), current_stream_ptr()))
-        return (out, lse) if return_lse else out
+        return _combine(o_part, ml, B, chunks, Lq, H, q.dtype, return_lse=return_lse)
     if Lk_total % split != 0:
         raise AtlasB200Error(f"cross_attention_split: Lk_total={Lk_total} must be a multiple of {split}")
     splits = Lk_total // split
@@ -602,11 +594,7 @@ def cross_attention_split(q, q_col0, kv, k_col0, v_col0, B, H, Lq, Lk_total, add
                                            kv.stride(0), v_col0, _ptr(dummy), 8, _ptr(am) if am is not None else None, None,
                                            B * splits, H, Lq, split, float(scale), 0.0, splits, _ptr(o_part), _ptr(ml),
                                            None, float(dp), int(dseed), int(doff), None, _bf(q), current_stream_ptr()))
-    out = torch.empty((B * Lq, H * 64), dtype=q.dtype, device=q.device)
-    lse = torch.empty((B, H, Lq), dtype=torch.float32, device=q.device) if return_lse else None
-    check(lib().atlas_b200_attention_combine_ex(_ptr(o_part), _ptr(ml), B, splits, Lq, H, _ptr(out), out.stride(0),
-                                                _ptr(lse) if lse is not None else None, _bf(q), current_stream_ptr()))
-    return (out, lse) if return_lse else out
+    return _combine(o_part, ml, B, splits, Lq, H, q.dtype, return_lse=return_lse)
 
 
 # ---------------------------------------------------------------------------------------------
@@ -855,7 +843,7 @@ def attention_bwd(q, q_col0, k, k_col0, v, v_col0, out, dout, dq, dq_col0, dk, d
         _ptr(q), q.stride(0), q_col0, _ptr(k), k.stride(0), k_col0, _ptr(v), v.stride(0), v_col0, _ptr(o2), o2.stride(0),
         _ptr(do2), do2.stride(0), _ptr(dq), dq.stride(0), dq_col0, _ptr(dk), dk.stride(0), dk_col0, _ptr(dv),
         dv.stride(0), dv_col0, _ptr(am) if am is not None else None, _ptr(bd) if bd is not None else None,
-        _ptr(dbias) if dbias is not None else None, _ptr(lse), 1, _ptr(dsum),
+        _ptr(dbias) if dbias is not None else None, _ptr(lse), _ptr(dsum),
         _ptr(accum) if accum is not None else None, B, H, Lq, Lk, float(scale), float(causal_value), float(dp),
         int(dseed), int(doff), _ptr(block_live) if block_live is not None else None, _bf(q), current_stream_ptr()))
     if accum is not None:
@@ -904,11 +892,7 @@ def decode_cross_attention(q, kv, B, H, Lk, add_mask=None, scale=1.0, chunk=256,
                                                        _ptr(am) if am is not None else None,
                                                        _ptr(tile_live) if tile_live is not None else None, B, H, Lk, chunk,
                                                        float(scale), _ptr(o_part), _ptr(ml), _bf(q), current_stream_ptr()))
-    if out is None:
-        out = torch.empty((B, H * 64), dtype=q.dtype, device=q.device)
-    check(lib().atlas_b200_attention_combine_ex(_ptr(o_part), _ptr(ml), B, chunks, 1, H, _ptr(out), out.stride(0), None,
-                                                _bf(q), current_stream_ptr()))
-    return out
+    return _combine(o_part, ml, B, chunks, 1, H, q.dtype, out=out)
 
 
 def decode_argmax(logits, seq, tok_in, done, t_dev, eos_id, pad_id, min_length):
@@ -957,10 +941,7 @@ def decode_cross_attention_beams(q, kv, B, nb, H, Lk, add_mask, chunk, tile_live
                                                   _ptr(am) if am is not None else None,
                                                   _ptr(tile_live) if tile_live is not None else None, B, H, nb, Lk, chunk,
                                                   1.0, _ptr(o_part), _ptr(ml), _bf(q), current_stream_ptr()))
-    out = torch.empty((B * nb, H * 64), dtype=q.dtype, device=q.device)
-    check(lib().atlas_b200_attention_combine_ex(_ptr(o_part), _ptr(ml), B, chunks, nb, H, _ptr(out), out.stride(0), None,
-                                                _bf(q), current_stream_ptr()))
-    return out
+    return _combine(o_part, ml, B, chunks, nb, H, q.dtype)
 
 
 # ---------------------------------------------------------------------------------------------
@@ -1029,11 +1010,7 @@ def decode_cross_attention_e4m3(q, kv8, kv_scale, B, H, Lk, add_mask=None, scale
                                                        _ptr(am) if am is not None else None,
                                                        _ptr(tile_live) if tile_live is not None else None, B, H, Lk, chunk,
                                                        float(scale), _ptr(o_part), _ptr(ml), _bf(q), current_stream_ptr()))
-    if out is None:
-        out = torch.empty((B, H * 64), dtype=q.dtype, device=q.device)
-    check(lib().atlas_b200_attention_combine_ex(_ptr(o_part), _ptr(ml), B, chunks, 1, H, _ptr(out), out.stride(0), None,
-                                                _bf(q), current_stream_ptr()))
-    return out
+    return _combine(o_part, ml, B, chunks, 1, H, q.dtype, out=out)
 
 
 def decode_cross_attention_beams_e4m3(q, kv8, kv_scale, B, nb, H, Lk, add_mask, chunk, tile_live=None, scale=1.0):
@@ -1051,10 +1028,7 @@ def decode_cross_attention_beams_e4m3(q, kv8, kv_scale, B, nb, H, Lk, add_mask, 
                                                        _ptr(am) if am is not None else None,
                                                        _ptr(tile_live) if tile_live is not None else None, B, H, nb, Lk, chunk,
                                                        float(scale), _ptr(o_part), _ptr(ml), _bf(q), current_stream_ptr()))
-    out = torch.empty((B * nb, H * 64), dtype=q.dtype, device=q.device)
-    check(lib().atlas_b200_attention_combine_ex(_ptr(o_part), _ptr(ml), B, chunks, nb, H, _ptr(out), out.stride(0), None,
-                                                _bf(q), current_stream_ptr()))
-    return out
+    return _combine(o_part, ml, B, chunks, nb, H, q.dtype)
 
 
 def beam_topk(logits, beam_scores, t_dev, k, eos_id, min_length, round_lp, add_mask=None, cand_score=None, cand_tok=None,

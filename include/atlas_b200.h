@@ -168,26 +168,23 @@ int atlas_b200_pq_refine_topk(const void* rows_host, int64_t n, const void* quer
  *             | 4 gated: C[m, j] = gelu_new(acc[m, 2j]) * acc[m, 2j+1], C has N/2 columns; W rows are
  *               wi_0 / wi_1 interleaved (modeling_t5.py:281-285; GELU evaluated in fp32 as at :283)
  *             | 5 relu: C = max(acc +bias, 0) (T5 v1.0 T5DenseReluDense wi, modeling_t5.py:256-270; with
- *               atlas_b200_linear_ex's row_ss the row scale is applied first, then the bias and the ReLU)
+ *               row_ss the row scale is applied first, then the bias and the ReLU)
  * lda / ldw / ldc / ldr are row strides in elements (multiples of 8); N and K multiples of 8.
- * bias may be NULL (no bias added) for epilogues 1-3 and 5. */
-int atlas_b200_linear(const void* A, int64_t lda, const void* W, int64_t ldw, const void* bias,
-                      const void* residual, int64_t ldr, void* C, int64_t ldc,
-                      int32_t M, int32_t N, int32_t K, int32_t epilogue, int32_t is_bf16, void* stream);
-
-/* atlas_b200_linear with T5's RMSNorm (src/modeling_t5.py:244-253) fused around it, so the normalised activations never
- * exist in memory:
+ * bias may be NULL (no bias added) for epilogues 1-3 and 5.
+ * T5's RMSNorm (src/modeling_t5.py:244-253) fused around the GEMM, so the normalised activations never exist in memory:
  *   row_ss  device fp32 [M] = sum of squares of every A row, or NULL.  The accumulator row m is multiplied by
  *           rsqrt(row_ss[m] / K + rs_eps) before the epilogue: A holds the UN-normalised hidden states and the caller
  *           folds the norm weight into W (W'[n, k] = W[n, k] * ln_weight[k]).
  *   out_ss  device fp32 [M] or NULL (not with the gated epilogue): incremented by the sum of squares of the 16-bit values
- *           this launch stores in each row (zero it first) - the statistic of the NEXT norm, produced by the residual GEMM. */
-int atlas_b200_linear_ex(const void* A, int64_t lda, const void* W, int64_t ldw, const void* bias,
-                         const void* residual, int64_t ldr, void* C, int64_t ldc, int32_t M, int32_t N, int32_t K,
-                         int32_t epilogue, int32_t is_bf16, const float* row_ss, float* out_ss, float rs_eps,
-                         void* stream);
+ *           this launch stores in each row (zero it first) - the statistic of the NEXT norm, produced by the residual GEMM.
+ * m_dev     device int32 [1] or NULL (= M): only the first min(M, *m_dev) rows are computed; row blocks past it are not, rows
+ *           of the last computed block past *m_dev hold unspecified values.  The row count lives in device memory so that a
+ *           captured CUDA graph keeps one launch shape for a data-dependent number of rows (the compacted encoders below). */
+int atlas_b200_linear_rows(const void* A, int64_t lda, const void* W, int64_t ldw, const void* bias, const void* residual,
+                           int64_t ldr, void* C, int64_t ldc, int32_t M, int32_t N, int32_t K, int32_t epilogue,
+                           int32_t is_bf16, const float* row_ss, float* out_ss, float rs_eps, const int32_t* m_dev, void* stream);
 
-/* Which kernel schedule atlas_b200_linear / _ex / _rows run for an (M, N, K, epilogue) launch, with a 16-byte aligned
+/* Which kernel schedule atlas_b200_linear_rows runs for an (M, N, K, epilogue) launch, with a 16-byte aligned
  * residual (an unaligned one falls back to a cooperative schedule):
  *   0  cooperative, 128 x 128 tiles       1  cooperative, 128 x 256 tiles      (decoder-sized launches)
  *   2  ping-pong, 128 x 128 tiles         3  wide, 128 x 256 tiles, TMA-store  (encoder-sized launches)
@@ -220,22 +217,18 @@ int atlas_b200_masked_mean_pool(const void* x, const int64_t* mask, void* out, i
 
 /* Single-token decode attention of FiD.generate (csrc/decode.cu; reference: transformers 4.18 `generate` with use_cache
  * through src/atlas.py:592-619, T5Attention.forward with past_key_value src/modeling_t5.py:418-531):
- *  decode_cross_attention  q [B, H*64] (one new token per sequence) against the cross K | V rows kv [B*Lk, ldkv] projected once
- *      per generation; grid = (ceil(Lk / chunk), H, B); writes un-normalised fp32 partials o_partial [B*chunks, H*64] and
- *      (max, sum) ml_partial [B*chunks, H, 2] for atlas_b200_attention_combine(_ex) with Lq = 1, splits = chunks.
- *      HBM-bound: every K / V byte is read once per step (Lk * 2 * H*64 * 2 B per query and layer).
+ *  decode_cross_attention_live  q [B, H*64] (one new token per sequence) against the cross K | V rows kv [B*Lk, ldkv]
+ *      projected once per generation; grid = (ceil(Lk / chunk), H, B), chunk a multiple of 16; writes un-normalised fp32
+ *      partials o_partial [B*chunks, H*64] and (max, sum) ml_partial [B*chunks, H, 2] for atlas_b200_attention_combine_ex with
+ *      Lq = 1, splits = chunks.  HBM-bound: every K / V byte is read once per step (Lk * 2 * H*64 * 2 B per query and layer).
+ *      tile_live: the live-tile flags of atlas_b200_cross_attention_stream (uint8 [B, ceil(Lk / 64)], NULL = all live); 64-key
+ *      tiles of masked keys only are not read (a warp's 16-key group never straddles a tile).
  *  decode_self_attention   appends the new token's K | V (columns H*64.. of qkv [B, 3*H*64]) to cache [B, Tmax, 2*H*64] at
  *      row *t_dev and attends over keys 0..*t_dev with bias_delta [H, 2*Tmax-1] (T5 relative bias by offset, NULL = none).
  *      The step index lives in DEVICE memory so that one captured CUDA graph serves every step.
  *  decode_argmax           greedy pick as torch.argmax (a NaN beats every number; among equal values or among NaNs the lowest
  *      index wins; EOS banned while *t_dev + 1 < min_length, finished rows emit pad_id):
  *      seq[b, *t_dev + 1] = tok_in[b] = next; done[b] |= next == eos; then *t_dev += 1. */
-int atlas_b200_decode_cross_attention(const void* q, int64_t ldq, const void* kv, int64_t ldkv, int32_t k_col0,
-                                      int32_t v_col0, const float* add_mask, int32_t B, int32_t H, int32_t Lk,
-                                      int32_t chunk, float scale, float* o_partial, float* ml_partial, int32_t is_bf16,
-                                      void* stream);
-/* ... with the live-tile flags of atlas_b200_cross_attention_stream (uint8 [B, ceil(Lk / 64)], NULL = all live): 64-key tiles of
- * masked keys only are not read.  chunk is a multiple of 16 as without flags: a warp's 16-key group never straddles a tile. */
 int atlas_b200_decode_cross_attention_live(const void* q, int64_t ldq, const void* kv, int64_t ldkv, int32_t k_col0,
                                       int32_t v_col0, const float* add_mask, const uint8_t* tile_live, int32_t B, int32_t H, int32_t Lk,
                                       int32_t chunk, float scale, float* o_partial, float* ml_partial, int32_t is_bf16,
@@ -324,36 +317,54 @@ int atlas_b200_splice_tokens(const int32_t* bank_ids, const int32_t* bank_lens, 
                              int32_t batch, int32_t n_ctx, int32_t L, int32_t eos_id, int32_t pad_id, int64_t* out_ids,
                              uint8_t* out_mask, void* stream);
 
-/* Fused multi-head attention, head_dim 64, Lk <= 512 keys per segment (csrc/attention.cu):
+/* Fused multi-head attention, head_dim 64, 0 < Lk <= 576 keys per segment (K and V stay resident in shared memory;
+ * csrc/attention.cu):
  *   O[b,i,h,:] = softmax_j( scale*Q[b,i,h].K[b,j,h] + bias_delta[h, j-i+Lq-1] + add_mask[b,j] (+causal) ) V[b,j,h,:]
  * q / k / v point at row-major [B*L, ld] 16-bit buffers (e.g. the fused QKV projection output); head h
- * occupies columns [col0 + 64h, col0 + 64h + 64).  add_mask [B, Lk] fp32 additive (NULL = none),
- * bias_delta [H, Lq+Lk-1] fp32 (NULL = none; T5 relative-position bias by offset), causal_value 0 = off,
- * otherwise added where j > i (the reference adds -10000, transformers 4.18 get_extended_attention_mask).
+ * occupies columns [col0 + 64h, col0 + 64h + 64); strides and column offsets are multiples of 8 elements.
+ * add_mask [B, Lk] fp32 additive (NULL = none), bias_delta [H, Lq+Lk-1] fp32 (NULL = none; T5 relative-position bias by
+ * offset; Lq + Lk - 1 <= 1152), causal_value 0 = off, otherwise added where j > i (the reference adds -10000,
+ * transformers 4.18 get_extended_attention_mask).
+ *   lse_out         [B, H, Lq] fp32, the row log-sum-exp of the scores (natural log; NULL = not needed): all the backward
+ *                   pass needs besides the output itself.  Not with split-KV partials (atlas_b200_attention_combine_ex
+ *                   writes it then).
+ *   split KV        the FiD decoder's cross-attention over n_ctx*L (= 15 360) keys (fid.py:298-349 /
+ *                   src/modeling_t5.py:478-524): B = batch*splits key segments, q_div = splits (segment s reads the queries
+ *                   of batch s / splits), and o_partial [B*Lq, H*64] / ml_partial [B*Lq, H, 2] fp32 (un-normalised output,
+ *                   row max, row sum) are written instead of `out`; atlas_b200_attention_combine_ex merges them.  Otherwise
+ *                   q_div = 1 and both partials NULL.
+ *   dropout_p       dropout on the probabilities (training: src/modeling_t5.py:515-516, src/modeling_bert.py:354):
+ *                   O = (keep o softmax(S)) V / (1 - p), lse_out is that of the un-dropped softmax.  keep[b, h, i, j] is a
+ *                   function of (seed, offset, (b * H + h) * Lq + i, j) (csrc/dropout.cuh; j = key index over the whole key
+ *                   range when the keys are split: segment s of `q_div` covers j = s * Lk ..., Lk % 32 == 0 required then);
+ *                   atlas_b200_attention_bwd_train re-derives the same mask.  0 <= dropout_p < 1; 0 = no dropout.
+ *   key_block_live  optional, uint8 [B, ceil(Lk / 64)]: 0 marks a 64-key block whose keys are ALL masked out (additive mask
+ *                   <= -5000, softmax weight exactly 0 in fp32): it is neither loaded nor computed - identical results; every
+ *                   row keeps at least one live block (see atlas_b200_cross_attention_stream).
  * Replaces BertSelfAttention.forward (src/modeling_bert.py:328-366, scale 1/8) and T5Attention.forward
  * (src/modeling_t5.py:478-524, scale 1) incl. the materialised scores / probabilities. */
-int atlas_b200_attention(const void* q, int64_t ldq, int32_t q_col0, const void* k, int64_t ldk, int32_t k_col0,
-                         const void* v, int64_t ldv, int32_t v_col0, void* out, int64_t ldo,
-                         const float* add_mask, const float* bias_delta, int32_t B, int32_t H, int32_t Lq,
-                         int32_t Lk, float scale, float causal_value, int32_t q_div, float* o_partial,
-                         float* ml_partial, int32_t is_bf16, void* stream);
+int atlas_b200_attention_train(const void* q, int64_t ldq, int32_t q_col0, const void* k, int64_t ldk, int32_t k_col0,
+                               const void* v, int64_t ldv, int32_t v_col0, void* out, int64_t ldo, const float* add_mask,
+                               const float* bias_delta, int32_t B, int32_t H, int32_t Lq, int32_t Lk, float scale,
+                               float causal_value, int32_t q_div, float* o_partial, float* ml_partial, float* lse_out,
+                               float dropout_p, uint64_t seed, uint64_t offset, const uint8_t* key_block_live,
+                               int32_t is_bf16, void* stream);
+/* atlas_b200_attention_train for long key ranges: 0 < Lk <= 4096 keys per segment and Lq + Lk - 1 <= 8192 (the bias table
+ * of atlas_b200_attention_bwd_train), same arguments and results except that there are no split-KV partials (q_div = 1).
+ * K and V stream through shared memory in 64-key blocks instead of staying resident (csrc/attention.cu,
+ * attention_long_kernel), so the key count is not bounded by shared memory.  The FiD encoder takes it for passages longer
+ * than the 576 keys of atlas_b200_attention_train.  Strides and column offsets must be multiples of 8 elements; any violated
+ * limit returns ATLAS_B200_EINVAL before a launch. */
+int atlas_b200_attention_long(const void* q, int64_t ldq, int32_t q_col0, const void* k, int64_t ldk, int32_t k_col0,
+                              const void* v, int64_t ldv, int32_t v_col0, void* out, int64_t ldo, const float* add_mask,
+                              const float* bias_delta, int32_t B, int32_t H, int32_t Lq, int32_t Lk, float scale,
+                              float causal_value, float* lse_out, float dropout_p, uint64_t seed, uint64_t offset,
+                              const uint8_t* key_block_live, int32_t is_bf16, void* stream);
 
-/* atlas_b200_attention that also writes the row log-sum-exp of the scores, lse_out [B, H, Lq] fp32 (natural log; NULL =
- * not needed, not available together with o_partial): all the backward pass needs besides the output itself. */
-int atlas_b200_attention_ex(const void* q, int64_t ldq, int32_t q_col0, const void* k, int64_t ldk, int32_t k_col0,
-                            const void* v, int64_t ldv, int32_t v_col0, void* out, int64_t ldo, const float* add_mask,
-                            const float* bias_delta, int32_t B, int32_t H, int32_t Lq, int32_t Lk, float scale,
-                            float causal_value, int32_t q_div, float* o_partial, float* ml_partial, float* lse_out,
-                            int32_t is_bf16, void* stream);
-
-/* Split-KV support for the FiD decoder's cross-attention over n_ctx*L (= 15 360) keys
- * (fid.py:298-349 / src/modeling_t5.py:478-524): call atlas_b200_attention with B = batch*splits key
- * segments of <= 512 keys, q_div = splits (segment s reads the queries of batch s / splits) and
- * o_partial [B*Lq, H*64] / ml_partial [B*Lq, H, 2] fp32 (un-normalised output, row max, row sum);
- * then this merges the splits:  out[b,i,h,:] = sum_s e^(m_s-M) O_s / sum_s e^(m_s-M) l_s. */
-int atlas_b200_attention_combine(const float* o_partial, const float* ml_partial, int32_t B, int32_t splits,
-                                 int32_t Lq, int32_t H, void* out, int64_t ldo, int32_t is_bf16, void* stream);
-/* ... and the log-sum-exp over ALL splits, lse_out [B, H, Lq] fp32 (NULL = not needed). */
+/* Merge of the split-KV partials (atlas_b200_attention_train with q_div = splits, atlas_b200_cross_attention_stream and the
+ * decode cross-attention kernels): o_partial [B*splits*Lq, H*64] and ml_partial [B*splits*Lq, H, 2] fp32, row
+ * (b * splits + s) * Lq + i for split s:  out[b,i,h,:] = sum_s e^(m_s-M) O_s / sum_s e^(m_s-M) l_s  (16-bit, row stride ldo),
+ * and lse_out [B, H, Lq] fp32 = M + log(sum_s e^(m_s-M) l_s), the log-sum-exp over ALL splits (NULL = not needed). */
 int atlas_b200_attention_combine_ex(const float* o_partial, const float* ml_partial, int32_t B, int32_t splits,
                                     int32_t Lq, int32_t H, void* out, int64_t ldo, float* lse_out, int32_t is_bf16,
                                     void* stream);
@@ -361,28 +372,30 @@ int atlas_b200_attention_combine_ex(const float* o_partial, const float* ml_part
 /* --------------------------------------------------------------------------------------------
  * Backward pass (training): what autograd derives in the reference's train.py step
  * (`Atlas.forward` -> `loss.backward()`, src/atlas.py:399-550) for the kernels above.  Weight and
- * input gradients of the linear layers are wgmma GEMMs (dX = dY . W: atlas_b200_linear on W^T;
+ * input gradients of the linear layers are wgmma GEMMs (dX = dY . W: atlas_b200_linear_rows on W^T;
  * dW = dY^T . X: atlas_b200_linear_wgrad); the entry points below are the rest.
  * -------------------------------------------------------------------------------------------- */
 
-/* Backward of atlas_b200_attention (any Lq / Lk, head_dim 64; csrc/attention_bwd.cu).  q / k / v / out as in the
- * forward (out = the forward's result [B*Lq, H*64]); dout [B*Lq, H*64]; dq / dk / dv are written at column offsets
- * d?_col0 + 64h of [B*L, ld] buffers (so one [tokens, 3*H*64] buffer can receive dQ | dK | dV for a fused projection).
- * dbias_delta [H, Lq+Lk-1] fp32 is INCREMENTED (zero it first; NULL = not needed); lse / dsum are [B, H, Lq] fp32:
- * `lse` holds the forward's log-sum-exp (atlas_b200_attention_ex / _train / _combine_ex) and is only read; lse_given must
- * be non-zero (ATLAS_B200_EINVAL otherwise), `dsum` is scratch.  For FiD's cross-attention
- * (src/fid.py:298-349) pass the un-split key range: B = batch, Lk = n_ctx * L; with dq_accum [B*Lq, H*64] fp32 (zeroed,
- * no dbias) the keys are split over several CTAs that add their partial dQ into dq_accum instead of
- * writing `dq` - the caller converts it to 16 bits (atlas_b200_cast_f32).
+/* Backward of atlas_b200_attention_train / atlas_b200_attention_long (any Lq / Lk, head_dim 64; csrc/attention_bwd.cu).
+ * q / k / v / out as in the forward (out = the forward's result [B*Lq, H*64]); dout [B*Lq, H*64]; dq / dk / dv are written at
+ * column offsets d?_col0 + 64h of [B*L, ld] buffers (so one [tokens, 3*H*64] buffer can receive dQ | dK | dV for a fused
+ * projection).  dbias_delta [H, Lq+Lk-1] fp32 is INCREMENTED (zero it first; NULL = not needed; Lq + Lk - 1 <= 8192 with a
+ * bias); lse / dsum are [B, H, Lq] fp32, both required: `lse` holds the forward's log-sum-exp (lse_out of the forward or of
+ * atlas_b200_attention_combine_ex) and is only read - there is no path that recomputes it; `dsum` is scratch.  dropout_p /
+ * seed / offset / key_block_live as in the forward: the same keep mask is re-derived, dead blocks are skipped.  For FiD's
+ * cross-attention (src/fid.py:298-349) pass the un-split key range: B = batch, Lk = n_ctx * L; with dq_accum [B*Lq, H*64]
+ * fp32 (zeroed, no dbias) the keys are split over several CTAs that add their partial dQ into dq_accum instead of writing
+ * `dq` - the caller converts it to 16 bits (atlas_b200_cast_f32).
  * Replaces autograd through BertSelfAttention.forward (src/modeling_bert.py:328-366) and T5Attention.forward
  * (src/modeling_t5.py:478-524). */
-int atlas_b200_attention_bwd(const void* q, int64_t ldq, int32_t q_col0, const void* k, int64_t ldk, int32_t k_col0,
-                             const void* v, int64_t ldv, int32_t v_col0, const void* out, int64_t ldo, const void* dout,
-                             int64_t lddo, void* dq, int64_t lddq, int32_t dq_col0, void* dk, int64_t lddk,
-                             int32_t dk_col0, void* dv, int64_t lddv, int32_t dv_col0, const float* add_mask,
-                             const float* bias_delta, float* dbias_delta, float* lse, int32_t lse_given, float* dsum,
-                             float* dq_accum, int32_t B, int32_t H, int32_t Lq, int32_t Lk, float scale,
-                             float causal_value, int32_t is_bf16, void* stream);
+int atlas_b200_attention_bwd_train(const void* q, int64_t ldq, int32_t q_col0, const void* k, int64_t ldk, int32_t k_col0,
+                                   const void* v, int64_t ldv, int32_t v_col0, const void* out, int64_t ldo,
+                                   const void* dout, int64_t lddo, void* dq, int64_t lddq, int32_t dq_col0, void* dk,
+                                   int64_t lddk, int32_t dk_col0, void* dv, int64_t lddv, int32_t dv_col0,
+                                   const float* add_mask, const float* bias_delta, float* dbias_delta, float* lse,
+                                   float* dsum, float* dq_accum, int32_t B, int32_t H, int32_t Lq, int32_t Lk, float scale,
+                                   float causal_value, float dropout_p, uint64_t seed, uint64_t offset,
+                                   const uint8_t* key_block_live, int32_t is_bf16, void* stream);
 
 /* Cross-attention statistics for retriever distillation (`cross_attention_forward`, src/fid.py:333-343): with
  * S = scale * Q K^T + add_mask and P = softmax over the Lk = n_ctx * L keys (lse = the forward's log-sum-exp [B, H, T],
@@ -476,40 +489,6 @@ int atlas_b200_dropout_mask(uint8_t* out, int64_t M, int32_t N, float p, uint64_
 int atlas_b200_attention_dropout_mask(uint8_t* out, int64_t rows, int32_t Lk, float p, uint64_t seed, uint64_t offset,
                                       void* stream);
 
-/* atlas_b200_attention_ex with dropout on the attention probabilities (training: src/modeling_t5.py:515-516,
- * src/modeling_bert.py:354):  O = (keep o softmax(S)) V / (1 - p), the row log-sum-exp is that of the un-dropped softmax.
- * keep[b, h, i, j] is a function of (seed, offset, (b * H + h) * Lq + i, j) (csrc/dropout.cuh; j = key index over the whole
- * key range when the keys are split: segment s of `q_div` covers j = s * Lk ..., Lk % 32 == 0 required then);
- * atlas_b200_attention_bwd_train re-derives the same mask.  dropout_p == 0 is atlas_b200_attention_ex.
- * key_block_live (optional, uint8 [B, ceil(Lk / 64)]): 0 marks a 64-key block whose keys
- * are ALL masked out (additive mask <= -5000, softmax weight exactly 0 in fp32): it is neither loaded nor computed - identical
- * results; every row keeps at least one live block (see atlas_b200_cross_attention_stream). */
-int atlas_b200_attention_train(const void* q, int64_t ldq, int32_t q_col0, const void* k, int64_t ldk, int32_t k_col0,
-                               const void* v, int64_t ldv, int32_t v_col0, void* out, int64_t ldo, const float* add_mask,
-                               const float* bias_delta, int32_t B, int32_t H, int32_t Lq, int32_t Lk, float scale,
-                               float causal_value, int32_t q_div, float* o_partial, float* ml_partial, float* lse_out,
-                               float dropout_p, uint64_t seed, uint64_t offset, const uint8_t* key_block_live,
-                               int32_t is_bf16, void* stream);
-/* atlas_b200_attention_train for long key ranges: 0 < Lk <= 4096 keys per segment and Lq + Lk - 1 <= 8192 (the bias table
- * of atlas_b200_attention_bwd_train), same arguments and results except that there are no split-KV partials (q_div = 1).
- * K and V stream through shared memory in 64-key blocks instead of staying resident (csrc/attention.cu,
- * attention_long_kernel), so the key count is not bounded by shared memory.  The FiD encoder takes it for passages longer
- * than the 576 keys of atlas_b200_attention.  Strides and column offsets must be multiples of 8 elements; any violated
- * limit returns ATLAS_B200_EINVAL before a launch. */
-int atlas_b200_attention_long(const void* q, int64_t ldq, int32_t q_col0, const void* k, int64_t ldk, int32_t k_col0,
-                              const void* v, int64_t ldv, int32_t v_col0, void* out, int64_t ldo, const float* add_mask,
-                              const float* bias_delta, int32_t B, int32_t H, int32_t Lq, int32_t Lk, float scale,
-                              float causal_value, float* lse_out, float dropout_p, uint64_t seed, uint64_t offset,
-                              const uint8_t* key_block_live, int32_t is_bf16, void* stream);
-int atlas_b200_attention_bwd_train(const void* q, int64_t ldq, int32_t q_col0, const void* k, int64_t ldk, int32_t k_col0,
-                                   const void* v, int64_t ldv, int32_t v_col0, const void* out, int64_t ldo,
-                                   const void* dout, int64_t lddo, void* dq, int64_t lddq, int32_t dq_col0, void* dk,
-                                   int64_t lddk, int32_t dk_col0, void* dv, int64_t lddv, int32_t dv_col0,
-                                   const float* add_mask, const float* bias_delta, float* dbias_delta, float* lse,
-                                   int32_t lse_given, float* dsum, float* dq_accum, int32_t B, int32_t H, int32_t Lq,
-                                   int32_t Lk, float scale, float causal_value, float dropout_p, uint64_t seed,
-                                   uint64_t offset, const uint8_t* key_block_live, int32_t is_bf16, void* stream);
-
 /* Multi-tensor optimiser step and gradient statistics of the training loop.  The work list is a device
  * table of (tensor index, chunk index) int32 pairs, `chunk_elems` elements per chunk (multiple of 4).
  *   atlas_b200_adamw_fp32copy: src/AdamWFP32Copy.py:79-169 for one param group - per element, on the fp32 master copy:
@@ -566,15 +545,12 @@ int atlas_b200_cross_attention_stream(const void* q, int64_t ldq, int32_t q_col0
  * key are ever read by the cross-attention (atlas_b200_cross_attention_stream skips the others), so only they get a K | V
  * projection.  Everything keeps STATIC launch shapes (CUDA graphs): the live-row count lives in device memory.
  *   atlas_b200_compact_live_tiles: tile_off[t] = index of live 64-row tile t among the live tiles (-1 = dead), *count_rows =
- *     64 x #live; the rows of the live tiles of src [n_tiles * 64, d] are copied to dst rows [64 tile_off[t], +64).
- *   atlas_b200_linear_dynm: C[m, :] = A[m, :] . W^T for m < min(M_max, *m_dev) (plain epilogue): row blocks past *m_dev are
- *     not computed; rows of the last computed block past *m_dev hold unspecified values.
+ *     64 x #live; the rows of the live tiles of src [n_tiles * 64, d] are copied to dst rows [64 tile_off[t], +64), which
+ *     atlas_b200_linear_rows with m_dev = count_rows then projects.
  *   atlas_b200_cross_attention_stream_compact: as atlas_b200_cross_attention_stream with kv holding only the live tiles:
  *     tile t of batch b starts at row 64 * tile_row[b * (Lk / 64) + t] (tile_row = the tile_off table above). */
 int atlas_b200_compact_live_tiles(const void* src, int64_t lds, const uint8_t* tile_live, int32_t n_tiles, int32_t d, void* dst,
                                   int64_t ldd, int32_t* tile_off, int32_t* count_rows, void* stream);
-int atlas_b200_linear_dynm(const void* A, int64_t lda, const void* W, int64_t ldw, void* C, int64_t ldc, int32_t M_max, int32_t N,
-                           int32_t K, const int32_t* m_dev, int32_t is_bf16, void* stream);
 int atlas_b200_cross_attention_stream_compact(const void* q, int64_t ldq, int32_t q_col0, const void* kv, int64_t ldkv,
                                               int32_t k_col0, int32_t v_col0, const float* add_mask, const uint8_t* tile_live,
                                               const int32_t* tile_row, int32_t B, int32_t H, int32_t Lq, int32_t Lk,
@@ -591,20 +567,16 @@ int atlas_b200_cross_attention_stream_compact(const void* q, int64_t ldq, int32_
  *     tile of packed tile o, -1 past the end), *count_rows = 64 x #kept.
  *   atlas_b200_embed_packed_tiles: dst[64 o + r, :] = table[ids[64 tile_src[o] + r], :] (zeros past the end): T5Stack's
  *     embed_tokens (src/modeling_t5.py:930-934) straight into the packed layout.
- *   atlas_b200_linear_rows: atlas_b200_linear_ex over the first *m_dev rows (row blocks past it are not computed; rows of the
- *     last computed block past *m_dev hold unspecified values); m_dev == NULL = atlas_b200_linear_ex.
+ *   The projections run on atlas_b200_linear_rows with m_dev = count_rows.
  *   atlas_b200_attention_packed: T5Attention.forward (src/modeling_t5.py:478-524) of the encoder on the packed rows: segment b =
  *     rows [64 tile_off[b * nb], + 64 popcount(keep[b, :])) of qkv / out; add_mask [B, L] and bias_delta [H, 2L - 1] as in
- *     atlas_b200_attention_ex (positions are those of the padded layout: kept tiles are a prefix of the segment).
+ *     atlas_b200_attention_train (positions are those of the padded layout: kept tiles are a prefix of the segment).
  *   atlas_b200_expand_packed_tiles: back to the padded layout [S * nb * 64, d] (zeros at dropped tiles - the positions the
  *     reference fills with values nothing reads). */
 int atlas_b200_segment_tile_scan(const uint8_t* live, int32_t S, int32_t nb, uint8_t* keep, int32_t* tile_off, int32_t* tile_src,
                                  int32_t* count_rows, void* stream);
 int atlas_b200_embed_packed_tiles(const int64_t* ids, const void* table, int64_t ldt, int32_t vocab, const int32_t* tile_src,
                                   int32_t n_tiles, void* dst, int64_t ldd, int32_t d, void* stream);
-int atlas_b200_linear_rows(const void* A, int64_t lda, const void* W, int64_t ldw, const void* bias, const void* residual,
-                           int64_t ldr, void* C, int64_t ldc, int32_t M_max, int32_t N, int32_t K, int32_t epilogue,
-                           int32_t is_bf16, const float* row_ss, float* out_ss, float rs_eps, const int32_t* m_dev, void* stream);
 int atlas_b200_attention_packed(const void* qkv, int64_t ld, int32_t q_col0, int32_t k_col0, int32_t v_col0, void* out, int64_t ldo,
                                 const float* add_mask, const float* bias_delta, const uint8_t* keep, const int32_t* tile_off,
                                 int32_t B, int32_t H, int32_t L, float scale, int32_t is_bf16, void* stream);
@@ -614,9 +586,13 @@ int atlas_b200_expand_packed_tiles(const void* src, int64_t lds, const int32_t* 
 /* Measurement hook for bench.py's roofline: while enabled, every launch of ONE kind of kernel is bracketed
  * with CUDA events on its launching stream:
  *   kind 1  the bank sweep of atlas_b200_mips_topk (work = algorithmic bytes swept)
- *   kind 2  the wgmma GEMM of atlas_b200_linear   (work = 2*M*N*K FLOPs)
- *   kind 3  the attention kernel                     (work = 4*B*H*Lq*Lk*64 FLOPs)
+ *   kind 2  the wgmma GEMM of atlas_b200_linear_rows (work = 2*M*N*K FLOPs over the computed rows)
+ *   kind 3  the attention forward kernels: atlas_b200_attention_train / _long / _packed, the cross-attention stream
+ *           kernels (work = 4*B*H*Lq*Lk*64 FLOPs)
  *   kind 4  the attention backward kernels           (work = 16*B*H*Lq*Lk*64 FLOPs)
+ *   kind 5  the decode cross-attention kernels of atlas_b200_decode_cross_attention_live / _e4m3 (work = K | V bytes read:
+ *           4*B*H*Lk*64, or 2*B*H*Lk*68 for the e4m3 codes and scales)
+ *   kind 6  atlas_b200_beam_topk and atlas_b200_beam_select (work = bytes read: 2*R*V of logits, 16*B*nb*nb of candidates)
  *   kind 7  the refine kernel of atlas_b200_pq_refine_topk (work = host-row bytes read, nq * k_cand * 1536)
  *   kind 0  off (default).
  * atlas_b200_profile_work() returns the work summed over the bracketed launches so far;

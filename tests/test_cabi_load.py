@@ -46,17 +46,33 @@ def test_no_cpu_fallback():
         ops.mips_topk(bank, torch.zeros(1, 768), 4)
 
 
-def test_attention_bwd_requires_forward_lse():
-    """atlas_b200_attention_bwd_train with lse_given = 0 is rejected during argument validation, before any CUDA call:
-    the backward reads the log-sum-exp the forward wrote and has no path that recomputes it."""
+def test_argtypes_match_header_prototypes():
+    """Every prototype in include/atlas_b200.h has as many parameters as the ctypes argtypes of `_lib.lib()`: with a wrong
+    count ctypes passes the arguments shifted, which shows only on a GPU run, as garbage pointers."""
+    from atlas_b200 import _lib
+
+    L = _lib.lib()
+    text = re.sub(r"/\*.*?\*/", "", open(os.path.join(ROOT, "include", "atlas_b200.h")).read(), flags=re.S)
+    protos = re.findall(r"(atlas_b200_\w+)\s*\(([^)]*)\)\s*;", text)
+    assert {name for name, _ in protos} == set(_lib.EXPORTED_SYMBOLS)
+    for name, params in protos:
+        n = 0 if params.strip() in ("", "void") else len(params.split(","))
+        argtypes = getattr(L, name).argtypes or []
+        assert len(argtypes) == n, f"{name}: {n} parameters in the header, {len(argtypes)} argtypes"
+
+
+def test_attention_bwd_rejects_missing_lse():
+    """atlas_b200_attention_bwd_train without the forward's log-sum-exp (lse = NULL) is rejected during argument
+    validation, before any CUDA call: the backward reads the log-sum-exp the forward wrote and has no path that
+    recomputes it."""
     from atlas_b200 import _lib
 
     L = _lib.lib()
     B, H, Lq, Lk, ld = 2, 4, 64, 64, 3 * 4 * 64
     buf = (ctypes.c_float * (B * H * Lq))()
-    p = ctypes.cast(buf, ctypes.c_void_p)     # non-null stand-in for q, k, v, out, dout, dq, dk, dv, lse and dsum
+    p = ctypes.cast(buf, ctypes.c_void_p)     # non-null stand-in for q, k, v, out, dout, dq, dk, dv and dsum
     rc = L.atlas_b200_attention_bwd_train(p, ld, 0, p, ld, 64 * H, p, ld, 128 * H, p, 64 * H, p, 64 * H, p, ld, 0, p, ld,
-                                          64 * H, p, ld, 128 * H, None, None, None, p, 0, p, None, B, H, Lq, Lk,
+                                          64 * H, p, ld, 128 * H, None, None, None, None, p, None, B, H, Lq, Lk,
                                           0.125, 0.0, 0.0, 0, 0, None, 1, None)
     assert rc == 1, rc                                             # ATLAS_B200_EINVAL
     assert b"log-sum-exp" in L.atlas_b200_last_error() and b"lse" in L.atlas_b200_last_error()

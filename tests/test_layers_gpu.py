@@ -207,8 +207,8 @@ def test_masked_key_blocks_are_skipped_without_changing_the_result(dev, dtype, S
 
 
 @pytest.mark.parametrize("dtype", [torch.bfloat16, torch.float16])
-def test_compacted_cross_kv_path_is_identical(dev, dtype):
-    """Cross K | V projected only for the encoder positions inside live 64-key tiles (ops.compact_live_tiles + linear_dynm with
+def test_compacted_cross_kv_rows_path_is_identical(dev, dtype):
+    """Cross K | V projected only for the encoder positions inside live 64-key tiles (ops.compact_live_tiles + ops.linear with
     a device-side row count + the stream kernel reading the compacted rows) against the dense projection + the same kernel:
     bit-identical attention output; the compaction tables against a torch restatement."""
     from atlas_b200 import ops
@@ -230,7 +230,7 @@ def test_compacted_cross_kv_path_is_identical(dev, dtype):
     assert torch.equal(tile_off.cpu(), want_off.int()) and int(count) == 64 * int(flags.sum())
     rows = enc.view(-1, 64, d)[flags.to(dev)].reshape(-1, d)
     assert torch.equal(enc_live[: rows.shape[0]], rows)
-    kv_live = ops.linear_dynm(enc_live, wkv, count)
+    kv_live = ops.linear(enc_live, wkv, rows=count)
     kv_dense = ops.linear(enc, wkv)
     assert torch.equal(kv_live[: rows.shape[0]].view(-1, 64, 2 * H * 64), kv_dense.view(-1, 64, 2 * H * 64)[flags.to(dev)])
     a = ops.cross_attention_stream_compact(q, kv_live, live, tile_off, B, H, T, Lk, mask, scale=1.0)

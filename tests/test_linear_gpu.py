@@ -105,7 +105,7 @@ def test_strided_input_and_output_view(dev):
 @pytest.mark.parametrize("dtype", [torch.float16, torch.bfloat16])
 @pytest.mark.parametrize("M", [300, 6000])      # cooperative / ping-pong schedule
 def test_fused_rmsnorm_around_the_gemm(dev, dtype, M):
-    """atlas_b200_linear_ex: (a) `out_ss` = sum of squares of the stored residual output rows, (b) `row_ss` scales the
+    """atlas_b200_linear_rows: (a) `out_ss` = sum of squares of the stored residual output rows, (b) `row_ss` scales the
     accumulator rows by rsqrt(ss / K + eps) - together T5's RMSNorm (src/modeling_t5.py:244-253) with the norm weight
     folded into the consumer's matrix.  Reference: fp32 torch of the same folded computation, and the un-fused
     layernorm + linear path of this library (same result up to the 16-bit rounding of the normalised activations)."""

@@ -80,7 +80,7 @@ elif what == "gemm4":
               f"{fl / ms_ref / 1e9:.0f} TFLOP/s")
 elif what == "gemm_small":
     # both sides of the schedule selection (ping-pong from 2 x #SMs 128 x 128 tiles): the decoder's cross-attention K|V
-    # projection over the packed encoder rows (linear_dynm, device-side row count, ping-pong), then 256-row decoder-sized
+    # projection over the packed encoder rows (device-side row count, ping-pong), then 256-row decoder-sized
     # launches (8 queries x 32 target tokens) with each epilogue: cooperative, except the LM head (2 x 251 tiles of
     # 128 x 128: ping-pong); each next to cuBLAS plain on the same rows, all timed inside CUDA graphs
     S, L = 320, 384
@@ -88,7 +88,7 @@ elif what == "gemm_small":
     mask = (torch.arange(L, device=dev)[None, :] >= lens[:, None]).float() * -10000.0
     count = ops.segment_tile_scan(ops.key_block_live(mask))[3]
     rows = int(count)
-    shapes = [("cross K|V", S * L, 1536, 768, "dynm")]
+    shapes = [("cross K|V", S * L, 1536, 768, "rows")]
     shapes += [(f"dec {nm}", 256, N, K, epi) for nm, N, K, epi in
                (("qkv", 2304, 768, None), ("o+res", 768, 768, "res"), ("wi gated", 4096, 768, "gated"),
                 ("wo+res", 768, 2048, "res"), ("bias", 768, 768, "bias"), ("gelu", 3072, 768, "gelu"),
@@ -98,8 +98,8 @@ elif what == "gemm_small":
         w = torch.randn(N, K, device=dev).bfloat16() * 0.03
         b = torch.randn(N, device=dev).bfloat16() * 0.1
         r = torch.randn(M, N, device=dev).bfloat16() if epi == "res" else None
-        if epi == "dynm":
-            fn = lambda: ops.linear_dynm(x, w, count)
+        if epi == "rows":
+            fn = lambda: ops.linear(x, w, rows=count)
         elif epi == "gated":
             fn = lambda: ops.linear(x, w, epilogue=ops.EPI_GATED)
         elif epi == "res":
@@ -111,7 +111,7 @@ elif what == "gemm_small":
         else:
             fn = lambda: ops.linear(x, w)
         ms = graph_timed(fn, reps=reps)
-        m = rows if epi == "dynm" else M
+        m = rows if epi == "rows" else M
         xm, wt = x[:m], w.t().contiguous()
         ms_ref = graph_timed(lambda: torch.matmul(xm, wt), reps=reps)
         fl = 2 * m * N * K
@@ -139,7 +139,7 @@ elif what == "gemm_sched1":
     rows = int(count)
     for name, M, N, K, epi in (("qkv", S * L, 2304, 768, "rows"), ("o-proj+res", S * L, 768, 768, "res"),
                                ("wi gated", S * L, 4096, 768, "gated"), ("wo+res+ss", S * L, 768, 2048, "res_ss"),
-                               ("cross K|V", S * L, 1536, 768, "dynm"), ("qkv+bias", S * L, 2304, 768, "bias"),
+                               ("cross K|V", S * L, 1536, 768, "rows"), ("qkv+bias", S * L, 2304, 768, "bias"),
                                ("wi+gelu", S * L, 3072, 768, "gelu"), ("wi+relu", S * L, 3072, 768, "relu"),
                                ("mainloop", 61440, 2304, 4096, None)):
         x = torch.randn(M, K, device=dev).bfloat16() * 0.1
@@ -149,9 +149,7 @@ elif what == "gemm_sched1":
         ss = torch.zeros(M, device=dev)
         e = {"gated": ops.EPI_GATED, "res": ops.EPI_RESIDUAL, "res_ss": ops.EPI_RESIDUAL, "bias": ops.EPI_BIAS,
              "gelu": ops.EPI_GELU, "relu": ops.EPI_RELU}.get(epi, ops.EPI_NONE)
-        if epi == "dynm":
-            fn = lambda: ops.linear_dynm(x, w, count)
-        elif epi is None:
+        if epi is None:
             fn = lambda: ops.linear(x, w)
         else:
             fn = lambda: ops.linear(x, w, b if epi in ("bias", "gelu", "relu") else None, residual=r, epilogue=e,
