@@ -931,6 +931,11 @@ int atlas_b200_linear_rows(const void* A, int64_t lda, const void* W, int64_t ld
                "N, K and the leading dimensions must be multiples of 8 (16-byte rows)");
     AB_REQUIRE(epilogue >= EPI_NONE && epilogue <= EPI_RELU, "unknown epilogue %d", epilogue);
     AB_REQUIRE(epilogue != EPI_RESIDUAL || (residual != nullptr && ldr % 8 == 0), "EPI_RESIDUAL needs a residual");
+    // epilogue_pair reads the bias, and the cooperative epilogue the residual, as 32-bit pairs of 16-bit values
+    AB_REQUIRE(bias == nullptr || epilogue == EPI_NONE || epilogue == EPI_GATED || (reinterpret_cast<uintptr_t>(bias) & 3u) == 0,
+               "the bias must be 4-byte aligned");
+    AB_REQUIRE(epilogue != EPI_RESIDUAL || (reinterpret_cast<uintptr_t>(residual) & 3u) == 0,
+               "the residual must be 4-byte aligned");
     AB_REQUIRE(epilogue != EPI_GATED || N % 32 == 0, "EPI_GATED needs N %% 32 == 0");
     AB_REQUIRE((reinterpret_cast<uintptr_t>(C) & 15u) == 0, "C must be 16-byte aligned");
     AB_REQUIRE(out_ss == nullptr || epilogue != EPI_GATED, "out_ss is not available with the gated epilogue");

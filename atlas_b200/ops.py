@@ -308,23 +308,38 @@ def linear(x, weight, bias=None, residual=None, epilogue=None, out=None, row_ss=
     if epilogue is None:
         epilogue = EPI_RESIDUAL if residual is not None else (EPI_BIAS if bias is not None else EPI_NONE)
     n_out = N // 2 if epilogue == EPI_GATED else N
+    # the kernel reads these through raw pointers: a wrong dtype, length or layout would be read (or written) past its end
+    if bias is not None and (bias.dtype != x.dtype or bias.device != x.device or not bias.is_contiguous()
+                             or bias.numel() != N):
+        raise AtlasB200Error(f"linear: bias must be a contiguous {x.dtype} tensor of {N} elements on {x.device} "
+                             f"(got {bias.dtype} {tuple(bias.shape)} on {bias.device})")
     if out is None:
         out = torch.empty((M, n_out), dtype=x.dtype, device=x.device)
+    elif (out.dtype != x.dtype or out.device != x.device or out.dim() != 2 or out.stride(-1) != 1
+          or out.shape[0] < M or out.shape[1] < n_out):
+        raise AtlasB200Error(f"linear: out must be a {x.dtype} [>= {M}, >= {n_out}] tensor on {x.device} with unit column "
+                             f"stride (got {out.dtype} {tuple(out.shape)} stride {out.stride()} on {out.device})")
     r2 = None
     if residual is not None:
         r2 = residual.reshape(-1, residual.shape[-1])
+        if r2.dtype != x.dtype or r2.device != x.device or tuple(r2.shape) != (M, N):
+            raise AtlasB200Error(f"linear: residual must be a {x.dtype} [{M}, {N}] tensor on {x.device} "
+                                 f"(got {residual.dtype} {tuple(residual.shape)} on {residual.device})")
         if r2.stride(-1) != 1:
             r2 = r2.contiguous()
     for t in (row_ss, out_ss):
         if t is not None and (t.dtype != torch.float32 or t.numel() != M or not t.is_contiguous() or not t.is_cuda):
             raise AtlasB200Error("linear: row_ss / out_ss must be contiguous CUDA fp32 tensors with one element per row")
+    if rows is not None and (rows.dtype != torch.int32 or rows.numel() != 1 or rows.device != x.device):
+        raise AtlasB200Error(f"linear: rows must be an int32 tensor of one element on {x.device} "
+                             f"(got {rows.dtype} {tuple(rows.shape)} on {rows.device})")
     check(lib().atlas_b200_linear_rows(
         _ptr(x2), x2.stride(0), _ptr(w), w.stride(0), _ptr(bias) if bias is not None else None,
         _ptr(r2) if r2 is not None else None, r2.stride(0) if r2 is not None else 0, _ptr(out), out.stride(0),
         M, N, K, epilogue, 1 if x.dtype == torch.bfloat16 else 0, _ptr(row_ss) if row_ss is not None else None,
         _ptr(out_ss) if out_ss is not None else None, float(rs_eps), _ptr(rows) if rows is not None else None,
         current_stream_ptr()))
-    return out.reshape(*x.shape[:-1], n_out)
+    return out[:M, :n_out].reshape(*x.shape[:-1], n_out)
 
 
 # ---------------------------------------------------------------------------------------------

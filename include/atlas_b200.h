@@ -170,7 +170,9 @@ int atlas_b200_pq_refine_topk(const void* rows_host, int64_t n, const void* quer
  *             | 5 relu: C = max(acc +bias, 0) (T5 v1.0 T5DenseReluDense wi, modeling_t5.py:256-270; with
  *               row_ss the row scale is applied first, then the bias and the ReLU)
  * lda / ldw / ldc / ldr are row strides in elements (multiples of 8); N and K multiples of 8.
- * bias may be NULL (no bias added) for epilogues 1-3 and 5.
+ * bias may be NULL (no bias added) for epilogues 1-3 and 5.  The epilogues read the bias and the residual in pairs of
+ * 16-bit values: a bias (epilogues 1-3, 5) or residual (epilogue 3) that is not 4-byte aligned is refused; C must be
+ * 16-byte aligned.  A 4-byte but not 16-byte aligned residual runs a cooperative schedule (see below).
  * T5's RMSNorm (src/modeling_t5.py:244-253) fused around the GEMM, so the normalised activations never exist in memory:
  *   row_ss  device fp32 [M] = sum of squares of every A row, or NULL.  The accumulator row m is multiplied by
  *           rsqrt(row_ss[m] / K + rs_eps) before the epilogue: A holds the UN-normalised hidden states and the caller
