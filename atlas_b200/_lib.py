@@ -146,7 +146,7 @@ def lib():
     L.atlas_b200_grad_stats.restype = c.c_int
     L.atlas_b200_grad_stats.argtypes = [vp, i32, vp, i32, i32, vp, vp]
     L.atlas_b200_clamp_inf_fp16.restype = c.c_int
-    L.atlas_b200_clamp_inf_fp16.argtypes = [vp, i64, i64, i32, vp, vp, vp]
+    L.atlas_b200_clamp_inf_fp16.argtypes = [vp, i64, i64, i32, vp, vp, vp, vp]
     L.atlas_b200_cross_attention_stream.restype = c.c_int
     L.atlas_b200_cross_attention_stream.argtypes = [vp, i64, i32, vp, i64, i32, i32, vp, vp, i32, i32, i32, i32, i32, f32, vp,
                                                     vp, i32, vp]

@@ -571,6 +571,8 @@ int atlas_b200_bert_embed_sum(const int64_t* input_ids, const int64_t* token_typ
                               const void* type_emb, const void* pos_emb, void* y, int32_t batch, int32_t L, int32_t H,
                               int32_t is_bf16, void* stream) {
     AB_REQUIRE(batch >= 0 && L > 0 && H > 0 && H % 2 == 0, "bert_embed_sum: bad shape");
+    AB_REQUIRE(abh::aligned(word_emb, 4) && abh::aligned(type_emb, 4) && abh::aligned(pos_emb, 4) && abh::aligned(y, 4),
+               "bert_embed_sum: the tables and y must be 4-byte aligned");
     const int64_t rows = static_cast<int64_t>(batch) * L;
     if (rows == 0) return ATLAS_B200_OK;
     cudaStream_t s = static_cast<cudaStream_t>(stream);

@@ -247,10 +247,19 @@ __global__ void splice_tokens_kernel(const int32_t* __restrict__ bank_ids, const
 // i.e. three host synchronisations per block.  Here: a detect pass raises a device flag, the clamp pass reads it and leaves
 // at once when it is clear - same values, no synchronisation, capturable in a CUDA graph.  65504 - 1000 rounds to 64512
 // (0x7BE0) in fp16; NaNs stay NaNs (torch.clamp propagates them).
+// rows the clamp looks at: min(max(*m_dev, 0), M), or all M without a device count (read on the device, so a captured graph
+// follows the count of every replay).  Rows past it were never computed by the producing GEMM: neither read nor written.
+__device__ __forceinline__ int64_t rows_in(int64_t M, const int32_t* m_dev) {
+    if (m_dev == nullptr) return M;
+    const int64_t m = *m_dev;
+    return m < 0 ? 0 : (m < M ? m : M);
+}
+
 __global__ void __launch_bounds__(256)
-inf_detect_kernel(const uint16_t* __restrict__ x, int64_t ld, int64_t M, int N, int* __restrict__ flag) {
+inf_detect_kernel(const uint16_t* __restrict__ x, int64_t ld, int64_t M, const int32_t* __restrict__ m_dev, int N,
+                  int* __restrict__ flag) {
     const int vec_per_row = N / 8;
-    const int64_t nvec = M * vec_per_row;
+    const int64_t nvec = rows_in(M, m_dev) * vec_per_row;
     bool found = false;
     for (int64_t v = blockIdx.x * 256ll + threadIdx.x; v < nvec; v += gridDim.x * 256ll) {
         const uint4 w = __ldg(reinterpret_cast<const uint4*>(x + (v / vec_per_row) * ld + (v % vec_per_row) * 8));
@@ -265,9 +274,10 @@ inf_detect_kernel(const uint16_t* __restrict__ x, int64_t ld, int64_t M, int N, 
 // values, the statistic the fused RMSNorm of the next GEMM consumes (the GEMM that produced x accumulated it from the
 // un-clamped values, inf included).
 __global__ void __launch_bounds__(256)
-inf_clamp_kernel(uint16_t* __restrict__ x, int64_t ld, int64_t M, int N, const int* __restrict__ flag,
-                 float* __restrict__ row_ss) {
+inf_clamp_kernel(uint16_t* __restrict__ x, int64_t ld, int64_t M, const int32_t* __restrict__ m_dev, int N,
+                 const int* __restrict__ flag, float* __restrict__ row_ss) {
     if (*flag == 0) return;
+    M = rows_in(M, m_dev);
     const int lane = threadIdx.x & 31;
     for (int64_t row = blockIdx.x * 8ll + (threadIdx.x >> 5); row < M; row += gridDim.x * 8ll) {
         uint16_t* xr = x + row * ld;
@@ -457,6 +467,7 @@ int atlas_b200_embed_packed_tiles(const int64_t* ids, const void* table, int64_t
                                   int32_t n_tiles, void* dst, int64_t ldd, int32_t d, void* stream) {
     AB_REQUIRE(n_tiles >= 0 && vocab > 0 && d > 0 && d % 8 == 0 && ldt % 8 == 0 && ldd % 8 == 0 && ids != nullptr && tile_src != nullptr,
                "embed_packed_tiles: d and the strides must be multiples of 8");
+    AB_REQUIRE(abh::aligned(table, 16) && abh::aligned(dst, 16), "embed_packed_tiles: table and dst must be 16-byte aligned");
     if (n_tiles == 0) return ATLAS_B200_OK;
     ew::embed_packed_tiles_kernel<<<n_tiles, 256, 0, static_cast<cudaStream_t>(stream)>>>(
         ids, static_cast<const uint16_t*>(table), ldt, vocab, tile_src, static_cast<uint16_t*>(dst), ldd, d);
@@ -469,6 +480,7 @@ int atlas_b200_expand_packed_tiles(const void* src, int64_t lds, const int32_t* 
                                    int32_t d, void* stream) {
     AB_REQUIRE(n_tiles >= 0 && d > 0 && d % 8 == 0 && lds % 8 == 0 && ldd % 8 == 0 && tile_off != nullptr,
                "expand_packed_tiles: d and the strides must be multiples of 8");
+    AB_REQUIRE(abh::aligned(src, 16) && abh::aligned(dst, 16), "expand_packed_tiles: src and dst must be 16-byte aligned");
     if (n_tiles == 0) return ATLAS_B200_OK;
     ew::expand_packed_tiles_kernel<<<n_tiles, 256, 0, static_cast<cudaStream_t>(stream)>>>(
         static_cast<const uint16_t*>(src), lds, tile_off, static_cast<uint16_t*>(dst), ldd, d);
@@ -481,6 +493,7 @@ int atlas_b200_compact_live_tiles(const void* src, int64_t lds, const uint8_t* t
                                   int64_t ldd, int32_t* tile_off, int32_t* count_rows, void* stream) {
     AB_REQUIRE(n_tiles >= 0 && d > 0 && d % 8 == 0 && lds % 8 == 0 && ldd % 8 == 0 && tile_off != nullptr && count_rows != nullptr,
                "compact_live_tiles: d and the strides must be multiples of 8");
+    AB_REQUIRE(abh::aligned(src, 16) && abh::aligned(dst, 16), "compact_live_tiles: src and dst must be 16-byte aligned");
     cudaStream_t s = static_cast<cudaStream_t>(stream);
     ew::live_tile_scan_kernel<<<1, 1024, 0, s>>>(tile_live, n_tiles, tile_off, count_rows);
     if (n_tiles > 0)
@@ -491,18 +504,20 @@ int atlas_b200_compact_live_tiles(const void* src, int64_t lds, const uint8_t* t
     return ATLAS_B200_OK;
 }
 
-int atlas_b200_clamp_inf_fp16(void* x, int64_t ld, int64_t M, int32_t N, int32_t* flag, float* row_ss, void* stream) {
+int atlas_b200_clamp_inf_fp16(void* x, int64_t ld, int64_t M, int32_t N, const int32_t* m_dev, int32_t* flag, float* row_ss,
+                              void* stream) {
     AB_REQUIRE(M >= 0 && N > 0 && N % 8 == 0 && ld % 8 == 0 && flag != nullptr, "clamp_inf_fp16: N and ld must be multiples of 8");
+    AB_REQUIRE(abh::aligned(x, 16), "clamp_inf_fp16: x must be 16-byte aligned");
     if (M == 0) return ATLAS_B200_OK;
     cudaStream_t s = static_cast<cudaStream_t>(stream);
     AB_CUDA_CHECK(cudaMemsetAsync(flag, 0, sizeof(int32_t), s));
     const int64_t blocks = (M * (N / 8) + 255) / 256;
     const int64_t cap = static_cast<int64_t>(abh::num_sms()) * 16;
     ew::inf_detect_kernel<<<static_cast<unsigned>(blocks < cap ? blocks : cap), 256, 0, s>>>(
-        static_cast<const uint16_t*>(x), ld, M, N, flag);
+        static_cast<const uint16_t*>(x), ld, M, m_dev, N, flag);
     const int64_t rb = (M + 7) / 8;
-    ew::inf_clamp_kernel<<<static_cast<unsigned>(rb < cap ? rb : cap), 256, 0, s>>>(static_cast<uint16_t*>(x), ld, M, N, flag,
-                                                                                   row_ss);
+    ew::inf_clamp_kernel<<<static_cast<unsigned>(rb < cap ? rb : cap), 256, 0, s>>>(static_cast<uint16_t*>(x), ld, M, m_dev, N,
+                                                                                   flag, row_ss);
     abh::count_launch(2);
     AB_CUDA_CHECK(cudaGetLastError());
     return ATLAS_B200_OK;
@@ -515,6 +530,8 @@ int atlas_b200_layernorm(const void* x, int64_t ldx, const void* weight, const v
     AB_REQUIRE(ldx % 8 == 0 && ldy % 8 == 0, "layernorm: row strides must be multiples of 8");
     AB_REQUIRE(kind == 0 || kind == 1, "layernorm: kind must be 0 (BertLayerNorm) or 1 (T5 RMSNorm)");
     AB_REQUIRE(kind == 1 || bias != nullptr, "BertLayerNorm needs a bias");
+    AB_REQUIRE(abh::aligned(x, 16) && abh::aligned(weight, 16) && abh::aligned(bias, 16) && abh::aligned(y, 16),
+               "layernorm: x, weight, bias and y must be 16-byte aligned");
     if (rows == 0) return ATLAS_B200_OK;
     cudaStream_t s = static_cast<cudaStream_t>(stream);
     const int grid = (rows + 7) / 8;
@@ -536,7 +553,10 @@ int atlas_b200_layernorm(const void* x, int64_t ldx, const void* weight, const v
 int atlas_b200_bert_embed_ln(const int64_t* input_ids, const int64_t* token_type_ids, const void* word_emb,
                              const void* type_emb, const void* pos_emb, const void* ln_weight, const void* ln_bias,
                              void* y, int32_t batch, int32_t L, int32_t H, float eps, int32_t is_bf16, void* stream) {
-    AB_REQUIRE(batch >= 0 && L > 0 && H % 8 == 0 && H <= ew::MAXV * 256, "bert_embed_ln: bad shape");
+    AB_REQUIRE(batch >= 0 && L > 0 && H > 0 && H % 8 == 0 && H <= ew::MAXV * 256, "bert_embed_ln: bad shape");
+    AB_REQUIRE(abh::aligned(word_emb, 16) && abh::aligned(type_emb, 16) && abh::aligned(pos_emb, 16) &&
+                   abh::aligned(ln_weight, 16) && abh::aligned(ln_bias, 16) && abh::aligned(y, 16),
+               "bert_embed_ln: the tables, weight, bias and y must be 16-byte aligned");
     const int rows = batch * L;
     if (rows == 0) return ATLAS_B200_OK;
     cudaStream_t s = static_cast<cudaStream_t>(stream);

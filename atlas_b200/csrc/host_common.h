@@ -61,4 +61,7 @@ void prof_end_dyn(cudaStream_t s, int kind, double work_per_row, const int32_t* 
 
 inline size_t align_up(size_t x, size_t a) { return (x + a - 1) / a * a; }
 
+// true when p is a multiple of `a` bytes (a power of two); NULL counts as aligned (optional operands are checked by the caller)
+inline bool aligned(const void* p, uintptr_t a) { return (reinterpret_cast<uintptr_t>(p) & (a - 1)) == 0; }
+
 }  // namespace abh

@@ -400,7 +400,7 @@ class FiD(nn.Module):
         g = self._ff_in(W, G, prefix, n, rows=rows)
         # + the fp16 overflow clamp the reference applies after every sub-layer (src/modeling_t5.py:657-708; no-op in bf16)
         return ops.clamp_inf_(ops.linear(g, W[prefix + "DenseReluDense.wo.weight"], None, residual=h,
-                                         epilogue=ops.EPI_RESIDUAL, rows=rows))
+                                         epilogue=ops.EPI_RESIDUAL, rows=rows), rows=rows)
 
     @torch.no_grad()
     def encode(self, input_ids, attention_mask):
@@ -468,12 +468,12 @@ class FiD(nn.Module):
                 ctx = attn(qkv)
                 h = ops.linear(ctx, W[p + "SelfAttention.o.weight"], None, residual=h, epilogue=ops.EPI_RESIDUAL,
                                out_ss=ss[2 * i], rows=rows)
-                ops.clamp_inf_(h, row_ss=ss[2 * i])
+                ops.clamp_inf_(h, row_ss=ss[2 * i], rows=rows)
                 p = f"encoder.block.{i}.layer.1."
                 g = self._ff_in(W, G, p, h, rows=rows, row_ss=ss[2 * i], eps=eps)
                 h = ops.linear(g, W[p + "DenseReluDense.wo.weight"], None, residual=h, epilogue=ops.EPI_RESIDUAL,
                                out_ss=ss[2 * i + 1], rows=rows)
-                ops.clamp_inf_(h, row_ss=ss[2 * i + 1])
+                ops.clamp_inf_(h, row_ss=ss[2 * i + 1], rows=rows)
         else:
             for i in range(c.num_layers):
                 p = f"encoder.block.{i}.layer.0."
@@ -481,7 +481,7 @@ class FiD(nn.Module):
                 ops.linear(n, G[p + "SelfAttention.qkv"], out=qkv, rows=rows)
                 ctx = attn(qkv)
                 h = ops.clamp_inf_(ops.linear(ctx, W[p + "SelfAttention.o.weight"], None, residual=h,
-                                              epilogue=ops.EPI_RESIDUAL, rows=rows))
+                                              epilogue=ops.EPI_RESIDUAL, rows=rows), rows=rows)
                 h = self._ff(W, G, f"encoder.block.{i}.layer.1.", h, eps, rows=rows)
         h = ops.layernorm(h, W["encoder.final_layer_norm.weight"], None, c.layer_norm_epsilon, kind=1)
         return (h, keep, tile_off, rows) if packed else h

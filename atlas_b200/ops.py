@@ -752,17 +752,22 @@ def attention_dropout_mask(B, H, Lq, Lk, p, seed, offset, device):
 _inf_flags = {}
 
 
-def clamp_inf_(x, row_ss=None):
+def clamp_inf_(x, row_ss=None, rows=None):
     """The reference's per-sub-layer fp16 overflow clamp (src/modeling_t5.py:657-708), in place, decided on the device
-    (no host synchronisation).  A no-op for any other dtype, like the reference's `dtype == torch.float16` test."""
+    (no host synchronisation).  A no-op for any other dtype, like the reference's `dtype == torch.float16` test.
+    rows: int32 [1] device row count (as `linear(..., rows=)`): only the first min(max(rows, 0), M) rows are looked at,
+    the rest (never computed) is neither read nor written."""
     if x.dtype != torch.float16:
         return x
     require_cuda(x, "x")
     x2 = _rows2d(x)
+    if rows is not None and (rows.dtype != torch.int32 or rows.numel() != 1 or rows.device != x.device):
+        raise AtlasB200Error(f"clamp_inf_: rows must be an int32 tensor of one element on {x.device}")
     flag = _inf_flags.get(x.device)
     if flag is None:
         flag = _inf_flags[x.device] = torch.zeros(1, dtype=torch.int32, device=x.device)
-    check(lib().atlas_b200_clamp_inf_fp16(_ptr(x2), x2.stride(0), x2.shape[0], x2.shape[1], _ptr(flag),
+    check(lib().atlas_b200_clamp_inf_fp16(_ptr(x2), x2.stride(0), x2.shape[0], x2.shape[1],
+                                          _ptr(rows) if rows is not None else None, _ptr(flag),
                                           _ptr(row_ss) if row_ss is not None else None, current_stream_ptr()))
     return x
 

@@ -201,13 +201,16 @@ int atlas_b200_linear_schedule(int32_t M, int32_t N, int32_t K, int32_t epilogue
 /* Row-wise normalisation of 16-bit activations (csrc/elementwise.cu), one rounding point per torch op:
  *   kind 0  BertLayerNorm (src/modeling_bert.py:104-114): y = w * r16((x - mean) * rsqrt(mean(x^2) + eps)) + b
  *           — note the UNCENTRED second moment; callers pass the residual sum already rounded to 16 bits.
- *   kind 1  T5LayerNorm / RMSNorm (src/modeling_t5.py:244-253): y = w * r16(x * rsqrt(mean(x^2) + eps)) */
+ *   kind 1  T5LayerNorm / RMSNorm (src/modeling_t5.py:244-253): y = w * r16(x * rsqrt(mean(x^2) + eps))
+ * H a multiple of 8 up to 2048, ldx / ldy multiples of 8; x, weight, bias and y 16-byte aligned (16-byte vector accesses),
+ * else ATLAS_B200_EINVAL before any launch. */
 int atlas_b200_layernorm(const void* x, int64_t ldx, const void* weight, const void* bias, void* y, int64_t ldy,
                          int32_t rows, int32_t H, float eps, int32_t kind, int32_t is_bf16, void* stream);
 
 /* BertEmbeddings.forward (src/modeling_bert.py:213-247): word + token_type + position embeddings
  * (16-bit adds in that order), BertLayerNorm.  input_ids / token_type_ids [batch, L] int64
- * (token_type_ids may be NULL = zeros); y [batch*L, H]. */
+ * (token_type_ids may be NULL = zeros); y [batch*L, H].  H a multiple of 8 up to 2048; the three tables, ln_weight, ln_bias
+ * and y 16-byte aligned, else ATLAS_B200_EINVAL. */
 int atlas_b200_bert_embed_ln(const int64_t* input_ids, const int64_t* token_type_ids, const void* word_emb,
                              const void* type_emb, const void* pos_emb, const void* ln_weight, const void* ln_bias,
                              void* y, int32_t batch, int32_t L, int32_t H, float eps, int32_t is_bf16, void* stream);
@@ -452,7 +455,7 @@ int atlas_b200_relu_bwd(const void* g, int64_t ldg, const void* dg, int64_t lddg
                         int32_t is_bf16, void* stream);
 
 /* word + token_type + position embeddings WITHOUT the LayerNorm (src/modeling_bert.py:236-243): the training forward
- * keeps the sum for the LayerNorm backward. */
+ * keeps the sum for the LayerNorm backward.  H even; the three tables and y 4-byte aligned, else ATLAS_B200_EINVAL. */
 int atlas_b200_bert_embed_sum(const int64_t* input_ids, const int64_t* token_type_ids, const void* word_emb,
                               const void* type_emb, const void* pos_emb, void* y, int32_t batch, int32_t L, int32_t H,
                               int32_t is_bf16, void* stream);
@@ -526,8 +529,12 @@ int atlas_b200_grad_stats(const AtlasB200GradTensor* descs_dev, int32_t n_tensor
 /* fp16 overflow clamp of the T5 blocks (src/modeling_t5.py:657-708: `if dtype == fp16 and isinf(h).any(): h = clamp(h,
  * +-(65504 - 1000))` after every sub-layer, three host synchronisations per block in the reference): in place on x [M, N]
  * fp16, decided on the device through `flag` (one int32 of scratch), no synchronisation.  row_ss (optional, [M] fp32) is
- * rewritten with the rows' sums of squares when (and only when) the clamp fires (fused-RMSNorm statistic). */
-int atlas_b200_clamp_inf_fp16(void* x, int64_t ld, int64_t M, int32_t N, int32_t* flag, float* row_ss, void* stream);
+ * rewritten with the rows' sums of squares when (and only when) the clamp fires (fused-RMSNorm statistic).
+ * m_dev (optional, device int32): only rows [0, min(max(*m_dev, 0), M)) are scanned, clamped and get a row_ss, the row count
+ * atlas_b200_linear_rows computed (m_dev = NULL: all M).  It is read on the device, so a captured graph follows it.  x must be
+ * 16-byte aligned. */
+int atlas_b200_clamp_inf_fp16(void* x, int64_t ld, int64_t M, int32_t N, const int32_t* m_dev, int32_t* flag, float* row_ss,
+                              void* stream);
 
 /* FiD decoder cross-attention for FEW queries (Lq <= 64 target tokens) against Lk concatenated encoder keys per batch element
  * (src/fid.py:298-349 at the teacher-forced / training forward shape): an HBM-bound K / V stream.  q [B*Lq, ldq], kv [B*Lk, ldkv]
@@ -574,7 +581,9 @@ int atlas_b200_cross_attention_stream_compact(const void* q, int64_t ldq, int32_
  *     rows [64 tile_off[b * nb], + 64 popcount(keep[b, :])) of qkv / out; add_mask [B, L] and bias_delta [H, 2L - 1] as in
  *     atlas_b200_attention_train (positions are those of the padded layout: kept tiles are a prefix of the segment).
  *   atlas_b200_expand_packed_tiles: back to the padded layout [S * nb * 64, d] (zeros at dropped tiles - the positions the
- *     reference fills with values nothing reads). */
+ *     reference fills with values nothing reads).
+ * embed_packed_tiles, expand_packed_tiles and compact_live_tiles move 16-byte vectors: d and the row strides are multiples of 8
+ * and table / src / dst 16-byte aligned, else ATLAS_B200_EINVAL. */
 int atlas_b200_segment_tile_scan(const uint8_t* live, int32_t S, int32_t nb, uint8_t* keep, int32_t* tile_off, int32_t* tile_src,
                                  int32_t* count_rows, void* stream);
 int atlas_b200_embed_packed_tiles(const int64_t* ids, const void* table, int64_t ldt, int32_t vocab, const int32_t* tile_src,

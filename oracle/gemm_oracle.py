@@ -65,8 +65,20 @@ _FMT = {torch.float16: (11, -14), torch.bfloat16: (8, -126)}
 def ulp16(a, dtype):
     """Spacing of the 16-bit type in the binade of |a| (float64 tensor); the subnormal spacing below the normal range."""
     p, emin = _FMT[dtype]
-    e = torch.floor(torch.log2(a.abs().clamp_min(2.0 ** emin)))
-    return torch.pow(2.0, e - (p - 1))
+    _, e = torch.frexp(a.double().abs().clamp_min(2.0 ** emin))        # |a| = f 2^e with f in [0.5, 1): binade 2^(e - 1)
+    # 2^(e - p) built from its bits: exact on every device (pow / log2 need not be correctly rounded on the GPU)
+    return ((e.to(torch.int64) - p + 1023) << 52).view(torch.float64)
+
+
+def round16(a, dtype):
+    """float64 tensor -> the nearest value of the 16-bit type (ties to even), still as float64; overflow gives +-inf, NaN and
+    +-inf pass through.  Rounds once, directly from float64: going through fp32 would round bf16 twice."""
+    a = a.double()
+    fin = torch.isfinite(a)
+    u = ulp16(torch.where(fin, a, torch.zeros_like(a)), dtype)
+    r = torch.where(fin, torch.round(a / u) * u, a)          # torch.round: half to even; a / u and the product are exact
+    big = torch.finfo(dtype).max
+    return torch.where(fin & (r.abs() > big), torch.copysign(torch.full_like(r, math.inf), a), r)
 
 
 def gelu_erf64(v):
@@ -178,14 +190,6 @@ def reference(x, w, epi, dtype, bias=None, residual=None, scale=None, exact_acc=
     return v, e
 
 
-def round16(y64, dtype):
-    """y64 rounded once to the 16-bit type; y64 must be exact in fp32 (so fp64 -> fp32 -> 16 bits rounds once)."""
-    y32 = y64.float()
-    ok = torch.isnan(y64) | (y32.double() == y64)
-    assert bool(ok.all()), "value not exact in fp32: one rounding to 16 bits cannot be formed through fp32"
-    return y32.to(dtype)
-
-
 def compare(y, y64, E, dtype):
     """Per-element check of a 16-bit output y against (y64, E): where E == 0 the output must equal y64 rounded once
     (bit for bit; y64 is then exact in fp32), elsewhere |y - y64| <= E + ulp16(|y64| + E) / 2.  NaN must meet NaN.
@@ -195,7 +199,7 @@ def compare(y, y64, E, dtype):
     bad = nan_ref != nan_got
     exact = (E == 0) & ~nan_ref
     if bool(exact.any()):
-        want = round16(torch.where(exact, y64, torch.zeros_like(y64)), dtype)
+        want = round16(torch.where(exact, y64, torch.zeros_like(y64)), dtype).to(dtype)
         bad |= exact & ~((want == y) | (torch.isnan(want.double()) & nan_got))
     fin = ~exact & ~nan_ref & ~nan_got
     bound = E + 0.5 * ulp16(y64.abs() + E, dtype)

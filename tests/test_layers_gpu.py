@@ -17,79 +17,6 @@ def dev():
     return torch.device("cuda:0")
 
 
-def _bert_ln_ref(x16, w, b, eps):
-    """BertLayerNorm on `.float()` input then `.type_as` (src/modeling_bert.py:104-114,386)."""
-    x = x16.float()
-    mean = x.mean(-1, keepdim=True)
-    var = x.pow(2).mean(-1, keepdim=True)
-    h = ((x - mean) * torch.rsqrt(var + eps)).to(w.dtype)
-    return w * h + b
-
-
-def _rms_ref(x16, w, eps):
-    var = x16.float().pow(2).mean(-1, keepdim=True)
-    h = (x16 * torch.rsqrt(var + eps)).to(w.dtype)
-    return w * h
-
-
-@pytest.mark.parametrize("dtype", [torch.float16, torch.bfloat16])
-@pytest.mark.parametrize("H", [768, 2048, 64])
-def test_layernorm_kinds(dev, dtype, H):
-    from atlas_b200 import ops
-
-    g = torch.Generator(device="cpu").manual_seed(H)
-    x = (torch.randn(1000, H, generator=g) * 2 + 0.3).to(dtype).to(dev)
-    w = (1 + 0.1 * torch.randn(H, generator=g)).to(dtype).to(dev)
-    b = (0.1 * torch.randn(H, generator=g)).to(dtype).to(dev)
-    y0 = ops.layernorm(x, w, b, eps=1e-12, kind=0)
-    r0 = _bert_ln_ref(x, w, b, 1e-12)
-    y1 = ops.layernorm(x, w, None, eps=1e-6, kind=1)
-    r1 = _rms_ref(x, w, 1e-6)
-    for y, r, bb in ((y0, r0, b), (y1, r1, torch.zeros_like(b))):
-        # identical rounding points; the fp32 statistics may differ in reduction order, which can move the
-        # 16-bit intermediate w*h by one ulp -> tolerance in ulps of the INTERMEDIATE magnitude (|y| + |b|),
-        # and almost all outputs must be bit-identical
-        ulp = torch.finfo(dtype).eps * (r.float().abs() + bb.float().abs()) + 1e-6
-        assert torch.all((y.float() - r.float()).abs() <= 2.0 * ulp), float((y.float() - r.float()).abs().max())
-        assert float((y == r).float().mean()) > 0.97
-
-
-def test_bert_embed_ln(dev):
-    from atlas_b200 import ops
-
-    g = torch.Generator(device="cpu").manual_seed(3)
-    V, L, H, B = 1000, 37, 768, 5
-    we = (torch.randn(V, H, generator=g) * 0.02).half().to(dev)
-    te = (torch.randn(2, H, generator=g) * 0.02).half().to(dev)
-    pe = (torch.randn(512, H, generator=g) * 0.02).half().to(dev)
-    w = (1 + 0.1 * torch.randn(H, generator=g)).half().to(dev)
-    b = (0.1 * torch.randn(H, generator=g)).half().to(dev)
-    ids = torch.randint(0, V, (B, L), generator=g).to(dev)
-    y = ops.bert_embed_ln(ids, None, we, te, pe, w, b, 1e-12)
-    emb = we[ids] + te[torch.zeros_like(ids)]
-    emb += pe[torch.arange(L, device=dev)][None]
-    ref = _bert_ln_ref(emb, w, b, 1e-12)
-    tol = 2 * torch.finfo(torch.float16).eps * (ref.float().abs() + b.float().abs()) + 1e-6
-    assert torch.all((y.float() - ref.float()).abs() <= tol)
-    assert float((y == ref).float().mean()) > 0.97
-
-
-def test_masked_mean_pool_into_bank_rows(dev):
-    from atlas_b200 import ops
-
-    g = torch.Generator(device="cpu").manual_seed(4)
-    B, L, H = 9, 50, 768
-    x = torch.randn(B, L, H, generator=g).half().to(dev)
-    lens = torch.randint(1, L + 1, (B,), generator=g)
-    mask = (torch.arange(L)[None] < lens[:, None]).long().to(dev)
-    bank = torch.zeros(20, H, dtype=torch.float16, device=dev)
-    ops.masked_mean_pool(x, mask, out=bank[4:4 + B])
-    last = x.masked_fill(~mask[..., None].bool(), 0.0)
-    ref = last.sum(dim=1) / mask.sum(dim=1)[..., None]       # src/retrievers.py:50-53 on a half tensor
-    assert torch.all((bank[4:4 + B].float() - ref.float()).abs() <= torch.finfo(torch.float16).eps * ref.float().abs() + 1e-7)
-    assert float(bank[:4].abs().max()) == 0 and float(bank[4 + B:].abs().max()) == 0
-
-
 def test_fp16_inf_clamp(dev):
     """ops.clamp_inf_ = the reference's `if dtype == fp16 and isinf(h).any(): h = clamp(h, +-(65504 - 1000))`
     (src/modeling_t5.py:657-708) decided on the device: untouched without an inf, torch.clamp's values with one."""

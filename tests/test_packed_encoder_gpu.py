@@ -31,7 +31,7 @@ def _keep_tables(live):
     return torch.from_numpy(keep), torch.from_numpy(off), torch.from_numpy(src), rows
 
 
-@pytest.mark.parametrize("S,nb", [(1, 1), (7, 6), (320, 6), (2500, 3), (33, 9)])
+@pytest.mark.parametrize("S,nb", [(1, 1), (7, 6), (320, 6), (2500, 3), (33, 9), (1023, 64), (1024, 64), (1025, 64)])
 def test_segment_tile_scan(dev, S, nb):
     from atlas_b200 import ops
 
