@@ -145,6 +145,20 @@ def bias_by_delta(weight, lq, lk, bidirectional, num_buckets):
     return weight[buckets].t().float().contiguous()
 
 
+def _capture(fn):
+    """(CUDA graph of `fn()`, what the captured call returned), after one eager warm-up call on a side stream (lazy kernel
+    attributes, allocator, weight caches).  The warm-up really runs: state it writes is the caller's to reset."""
+    side = torch.cuda.Stream()
+    side.wait_stream(torch.cuda.current_stream())
+    with torch.cuda.stream(side):
+        fn()
+    torch.cuda.current_stream().wait_stream(side)
+    graph = torch.cuda.CUDAGraph()
+    with torch.cuda.graph(graph):
+        out = fn()
+    return graph, out
+
+
 class _GraphRunner:
     """One captured CUDA graph of a static-shape function of device tensors.  Every kernel of this package is
     launched through the C ABI on `torch.cuda.current_stream()`, so capturing the whole forward removes the ~150
@@ -152,14 +166,7 @@ class _GraphRunner:
 
     def __init__(self, fn, example_inputs):
         self.static_in = [t.clone() for t in example_inputs]
-        side = torch.cuda.Stream()
-        side.wait_stream(torch.cuda.current_stream())
-        with torch.cuda.stream(side):           # eager warm-up: lazy kernel attributes, allocator, weight caches
-            fn(*self.static_in)
-        torch.cuda.current_stream().wait_stream(side)
-        self.graph = torch.cuda.CUDAGraph()
-        with torch.cuda.graph(self.graph):
-            self.static_out = fn(*self.static_in)
+        self.graph, self.static_out = _capture(lambda: fn(*self.static_in))
 
     def __call__(self, *inputs):
         for dst, src in zip(self.static_in, inputs):
@@ -172,6 +179,39 @@ def _check_passage_length(L):
     if L > ops.ATTENTION_LONG_MAX_LK:
         raise AtlasB200Error(f"text_maxlength = {L} is not supported: the encoder self-attention takes passages of at most "
                              f"{ops.ATTENTION_LONG_MAX_LK} tokens")
+
+
+def _cross_split(Lk, dropout=False):
+    """Key segment of the split-KV cross-attention over Lk keys: the largest divisor of Lk up to 384 keys, else up to 512 (the
+    attention kernel keeps a whole segment's K / V in shared memory).  dropout: the training forward's dropout mask is
+    addressed in 32-key groups over the whole key range (csrc/dropout.cuh), so a multiple of 32 in [64, 512] comes first."""
+    split = None
+    if dropout:
+        split = next((s for s in range(min(512, Lk) // 32 * 32, 63, -32) if Lk % s == 0), None)
+    split = split or next((s for s in range(min(384, Lk), 63, -1) if Lk % s == 0), None) or \
+        next(s for s in range(min(512, Lk), 0, -1) if Lk % s == 0)
+    if split < 64 and Lk > 512:
+        raise AtlasB200Error(f"n_context*text_maxlength = {Lk} has no divisor in [64, 512] for the split-KV kernel")
+    if dropout and split % 32 != 0 and split != Lk:
+        raise AtlasB200Error(f"dropout on the cross-attention probabilities needs a key split that is a multiple of 32 "
+                             f"(n_context*text_maxlength = {Lk} gave {split})")
+    return split
+
+
+def _cross_mask(enc_mask, B, Lk, dt):
+    """The additive cross-attention mask [B, Lk] fp32 of `invert_attention_mask` (4.18): -1e4 for fp16, -1e9 otherwise
+    (src/modeling_t5.py:950)."""
+    neg = -1e4 if dt == torch.float16 else -1e9
+    return (1.0 - enc_mask.reshape(B, Lk).to(torch.float32)) * neg
+
+
+def _norm_sums(n_sub, M, device, fused):
+    """Row sums of squares for a stack of n_sub normed sub-layers of M rows (fused RMSNorm, see _norm_in): entry j is what
+    sub-layer j's norm reads, entry j + 1 what its residual GEMM writes.  Entry 0 (the first norm has no producing GEMM) and
+    every entry of an unfused stack are None: that norm runs as a kernel."""
+    if not fused:
+        return [None] * (n_sub + 1)
+    return [None] + list(torch.zeros((n_sub, M), dtype=torch.float32, device=device).unbind(0))
 
 
 class FiDOutput(tuple):
@@ -352,55 +392,82 @@ class FiD(nn.Module):
         return W["lm_head.weight"] if "lm_head.weight" in W else W["shared.weight"]
 
     @staticmethod
-    def _fuse(W):
-        """Weights derived once per parameter version: interleaved wi_0/wi_1, fused q|k|v and cross k|v."""
+    def _concat_weights(W):
+        """The concatenated weights the kernels read, by name: the rows of wi_0 and wi_1 interleaved (wi_0[j], wi_1[j]) for the
+        gated-GELU GEMM epilogue ("...DenseReluDense.wi_01"); one [3*H*64, d] q|k|v projection whose single GEMM writes the
+        [tokens, q|k|v] buffer the attention reads ("...SelfAttention.qkv"); the cross-attention k|v ("...EncDecAttention.kv").
+        Built from W with differentiable ops only."""
         g = {}
-        for name in list(W.keys()):
+        for name in W:
             if name.endswith("DenseReluDense.wi_0.weight"):
                 w0, w1 = W[name], W[name.replace("wi_0", "wi_1")]
-                # rows interleaved (wi_0[j], wi_1[j]) for the gated-GELU GEMM epilogue
-                g[name.replace("wi_0.weight", "wi_01")] = torch.stack([w0, w1], dim=1).reshape(-1, w0.shape[1]).contiguous()
+                g[name.replace("wi_0.weight", "wi_01")] = torch.stack([w0, w1], dim=1).reshape(-1, w0.shape[1])
             elif name.endswith("SelfAttention.q.weight"):
-                # one [3*H*64, d] projection: a single GEMM writes the [tokens, q|k|v] buffer the attention reads
                 g[name.replace("q.weight", "qkv")] = torch.cat(
                     [W[name], W[name.replace("q.weight", "k.weight")], W[name.replace("q.weight", "v.weight")]], 0)
             elif name.endswith("EncDecAttention.k.weight"):
                 g[name.replace("k.weight", "kv")] = torch.cat([W[name], W[name.replace("k.weight", "v.weight")]], 0)
-        # projections with the preceding RMSNorm weight folded in (W'[n, k] = W[n, k] * ln[k]) for the fused norm
-        for name in list(g):
-            if name.endswith("SelfAttention.qkv"):
-                ln = W[name.replace("SelfAttention.qkv", "layer_norm.weight")]
-            elif name.endswith("DenseReluDense.wi_01"):
-                ln = W[name.replace("DenseReluDense.wi_01", "layer_norm.weight")]
-            else:
-                continue
-            g[name + "_n"] = (g[name].float() * ln.float()[None, :]).to(g[name].dtype).contiguous()
-        for name in list(W):        # decoder cross-attention query projection behind layer.1's norm; T5 v1.0's wi
-            if name.endswith("EncDecAttention.q.weight"):
-                ln = W[name.replace("EncDecAttention.q.weight", "layer_norm.weight")]
-                g[name + "_n"] = (W[name].float() * ln.float()[None, :]).to(W[name].dtype).contiguous()
-            elif name.endswith("DenseReluDense.wi.weight"):
-                ln = W[name.replace("DenseReluDense.wi.weight", "layer_norm.weight")]
-                g[name.replace("wi.weight", "wi_n")] = (W[name].float() * ln.float()[None, :]).to(W[name].dtype).contiguous()
         return g
 
-    # ---- encoder ---------------------------------------------------------------------------
-    def _ff_in(self, W, G, prefix, x, rows=None, row_ss=None, eps=1e-6):
-        """The feed-forward's input GEMM with its activation in the epilogue: ReLU on wi (T5 v1.0) or the gated GELU on the
-        interleaved wi_0 | wi_1 (v1.1).  row_ss: x is the UN-normalised hidden state and the norm is fused (see encode)."""
-        p = prefix + "DenseReluDense."
-        if self.config.feed_forward_proj == "relu":
-            w, epi = (G[p + "wi_n"] if row_ss is not None else W[p + "wi.weight"]), ops.EPI_RELU
-        else:
-            w, epi = (G[p + "wi_01_n"] if row_ss is not None else G[p + "wi_01"]), ops.EPI_GATED
-        return ops.linear(x, w, epilogue=epi, row_ss=row_ss, rs_eps=eps, rows=rows)
+    # the projections that read a normalised hidden state, by the suffix of their weight's name in W or _concat_weights
+    _NORMED_INPUTS = ("SelfAttention.qkv", "EncDecAttention.q.weight", "DenseReluDense.wi_01", "DenseReluDense.wi.weight")
 
-    def _ff(self, W, G, prefix, h, eps, rows=None):
-        n = ops.layernorm(h, W[prefix + "layer_norm.weight"], None, eps, kind=1)
-        g = self._ff_in(W, G, prefix, n, rows=rows)
-        # + the fp16 overflow clamp the reference applies after every sub-layer (src/modeling_t5.py:657-708; no-op in bf16)
-        return ops.clamp_inf_(ops.linear(g, W[prefix + "DenseReluDense.wo.weight"], None, residual=h,
-                                         epilogue=ops.EPI_RESIDUAL, rows=rows), rows=rows)
+    @staticmethod
+    def _fuse(W):
+        """Weights derived once per parameter version: `_concat_weights`, and for the fused norm every projection behind an
+        RMSNorm again with the norm weight folded in (W'[n, k] = W[n, k] * ln[k]), named with a "_n" suffix."""
+        g = {name: w.contiguous() for name, w in FiD._concat_weights(W).items()}
+        for name, w in list(W.items()) + list(g.items()):
+            sub = next((s for s in FiD._NORMED_INPUTS if name.endswith(s)), None)
+            if sub is not None:
+                ln = W[name[: -len(sub)] + "layer_norm.weight"]
+                g[name + "_n"] = (w.float() * ln.float()[None, :]).to(w.dtype).contiguous()
+        return g
+
+    # ---- the sub-layers of the no-grad forward -------------------------------------------------
+    def _norm_in(self, W, G, p, name, x, ss=None, rows=None, **kw):
+        """RMSNorm of x with the norm weight of layer prefix p, then the projection p + name (a weight of G or W) on
+        ops.linear (kw: its epilogue / out).  ss None: the norm runs as a kernel.  ss given, the norm fused: x is the
+        UN-normalised hidden state and ss its rows' sums of squares; the GEMM reads the matrix with the norm weight folded in
+        (_fuse) and scales its accumulator rows by rsqrt(ss / d + eps), so the normalised rows are never written or read."""
+        eps = self.config.layer_norm_epsilon
+        if ss is not None:
+            return ops.linear(x, G[p + name + "_n"], row_ss=ss, rs_eps=eps, rows=rows, **kw)
+        n = ops.layernorm(x, W[p + "layer_norm.weight"], None, eps, kind=1)
+        return ops.linear(n, G[p + name] if p + name in G else W[p + name], rows=rows, **kw)
+
+    def _ff_in(self, W, G, p, x, ss=None, rows=None):
+        """The feed-forward's normed input GEMM with its activation in the epilogue: ReLU on wi (T5 v1.0) or the gated GELU
+        on the interleaved wi_0 | wi_1 (v1.1)."""
+        if self.config.feed_forward_proj == "relu":
+            return self._norm_in(W, G, p, "DenseReluDense.wi.weight", x, ss, rows, epilogue=ops.EPI_RELU)
+        return self._norm_in(W, G, p, "DenseReluDense.wi_01", x, ss, rows, epilogue=ops.EPI_GATED)
+
+    @staticmethod
+    def _residual(x, w, h, ss=None, rows=None):
+        """h + x @ w.T in the GEMM's epilogue, then the fp16 overflow clamp the reference applies after every sub-layer
+        (src/modeling_t5.py:657-708; no-op in bf16).  ss: receives the sums of squares of the new rows (fused norm)."""
+        h = ops.linear(x, w, None, residual=h, epilogue=ops.EPI_RESIDUAL, out_ss=ss, rows=rows)
+        return ops.clamp_inf_(h, row_ss=ss, rows=rows)
+
+    def _decoder_block(self, W, G, i, h, self_attn, cross_attn, ss, qkv=None):
+        """Decoder block i on the rows h: self_attn(qkv, i) and cross_attn(q, i) return the attention context.  ss: the
+        block's four entries of _norm_sums.  qkv: the buffer the q|k|v projection writes (None: a new one)."""
+        p = f"decoder.block.{i}.layer."
+        qkv = self._norm_in(W, G, p + "0.", "SelfAttention.qkv", h, ss[0], out=qkv)
+        h = self._residual(self_attn(qkv, i), W[p + "0.SelfAttention.o.weight"], h, ss[1])
+        q = self._norm_in(W, G, p + "1.", "EncDecAttention.q.weight", h, ss[1])
+        h = self._residual(cross_attn(q, i), W[p + "1.EncDecAttention.o.weight"], h, ss[2])
+        g = self._ff_in(W, G, p + "2.", h, ss[2])
+        return self._residual(g, W[p + "2.DenseReluDense.wo.weight"], h, ss[3])
+
+    def _lm_head(self, W, h, dt):
+        """Final norm, T5 v1.0's d_model^-0.5 rescale of a tied head (src/modeling_t5.py:1642-1645), LM head."""
+        c = self.config
+        h = ops.layernorm(h, W["decoder.final_layer_norm.weight"], None, c.layer_norm_epsilon, kind=1)
+        if getattr(c, "tie_word_embeddings", False):
+            h = (h.float() * (c.d_model ** -0.5)).to(dt)
+        return ops.linear(h, self._head(W))
 
     @torch.no_grad()
     def encode(self, input_ids, attention_mask):
@@ -434,7 +501,7 @@ class FiD(nn.Module):
         live = ops.key_block_live(add_mask)
         bias = bias_by_delta(W["encoder.block.0.layer.0.SelfAttention.relative_attention_bias.weight"], L, L, True,
                              c.relative_attention_num_buckets)
-        packed = packed and live is not None and L % 64 == 0 and 64 <= L <= 384
+        packed = packed and ops.encoder_packs(live, L)
         rows = None
         if packed:
             keep, tile_off, tile_src, rows = ops.segment_tile_scan(live)
@@ -451,38 +518,15 @@ class FiD(nn.Module):
                 return fwd(qkv, 0, qkv, H * 64, qkv, 2 * H * 64, S, H, L, L, add_mask=add_mask, bias_delta=bias, scale=1.0,
                            block_live=live)
         qkv = torch.empty((S * L, 3 * H * 64), dtype=dt, device=h.device)
-        eps = c.layer_norm_epsilon
-        if self.fuse_norm:
-            # RMSNorm fused around the GEMMs (row_ss / out_ss of ops.linear): the residual GEMMs emit each row's sum of squares,
-            # the consuming projection reads the UN-normalised hidden state with the norm weight folded into its matrix
-            # and scales its accumulator rows by rsqrt(ss / d + eps).  Only the very first and the final norm run as
-            # kernels; 2 x num_layers normalised [tokens, d] tensors are never written or read.
-            ss = torch.zeros((2 * c.num_layers, S * L), dtype=torch.float32, device=h.device)
-            for i in range(c.num_layers):
-                p = f"encoder.block.{i}.layer.0."
-                if i == 0:
-                    n = ops.layernorm(h, W[p + "layer_norm.weight"], None, eps, kind=1)
-                    ops.linear(n, G[p + "SelfAttention.qkv"], out=qkv, rows=rows)
-                else:
-                    ops.linear(h, G[p + "SelfAttention.qkv_n"], out=qkv, row_ss=ss[2 * i - 1], rs_eps=eps, rows=rows)
-                ctx = attn(qkv)
-                h = ops.linear(ctx, W[p + "SelfAttention.o.weight"], None, residual=h, epilogue=ops.EPI_RESIDUAL,
-                               out_ss=ss[2 * i], rows=rows)
-                ops.clamp_inf_(h, row_ss=ss[2 * i], rows=rows)
-                p = f"encoder.block.{i}.layer.1."
-                g = self._ff_in(W, G, p, h, rows=rows, row_ss=ss[2 * i], eps=eps)
-                h = ops.linear(g, W[p + "DenseReluDense.wo.weight"], None, residual=h, epilogue=ops.EPI_RESIDUAL,
-                               out_ss=ss[2 * i + 1], rows=rows)
-                ops.clamp_inf_(h, row_ss=ss[2 * i + 1], rows=rows)
-        else:
-            for i in range(c.num_layers):
-                p = f"encoder.block.{i}.layer.0."
-                n = ops.layernorm(h, W[p + "layer_norm.weight"], None, eps, kind=1)
-                ops.linear(n, G[p + "SelfAttention.qkv"], out=qkv, rows=rows)
-                ctx = attn(qkv)
-                h = ops.clamp_inf_(ops.linear(ctx, W[p + "SelfAttention.o.weight"], None, residual=h,
-                                              epilogue=ops.EPI_RESIDUAL, rows=rows), rows=rows)
-                h = self._ff(W, G, f"encoder.block.{i}.layer.1.", h, eps, rows=rows)
+        # fuse_norm: the RMSNorms fused around the GEMMs (_norm_in); only the very first and the final norm run as kernels,
+        # 2 x num_layers normalised [tokens, d] tensors are never written or read
+        ss = _norm_sums(2 * c.num_layers, S * L, h.device, self.fuse_norm)
+        for i in range(c.num_layers):
+            p = f"encoder.block.{i}.layer."
+            self._norm_in(W, G, p + "0.", "SelfAttention.qkv", h, ss[2 * i], rows, out=qkv)
+            h = self._residual(attn(qkv), W[p + "0.SelfAttention.o.weight"], h, ss[2 * i + 1], rows)
+            g = self._ff_in(W, G, p + "1.", h, ss[2 * i + 1], rows)
+            h = self._residual(g, W[p + "1.DenseReluDense.wo.weight"], h, ss[2 * i + 2], rows)
         h = ops.layernorm(h, W["encoder.final_layer_norm.weight"], None, c.layer_norm_epsilon, kind=1)
         return (h, keep, tile_off, rows) if packed else h
 
@@ -518,15 +562,8 @@ class FiD(nn.Module):
         B, T = decoder_input_ids.shape
         d, H = c.d_model, c.num_heads
         Lk = enc.shape[1]
-        # key segments of the split-KV cross-attention: the largest divisor of Lk up to 384 keys, else up to 512 (the
-        # attention kernel keeps a whole segment's K / V in shared memory)
-        split = next((s for s in range(min(384, Lk), 63, -1) if Lk % s == 0), None) or \
-            next(s for s in range(min(512, Lk), 0, -1) if Lk % s == 0)
-        if split < 64 and Lk > 512:
-            raise AtlasB200Error(f"n_context*text_maxlength = {Lk} has no divisor in [64, 512] for the split-KV kernel")
-        # invert_attention_mask (4.18): -1e4 for fp16, -1e9 otherwise (src/modeling_t5.py:950)
-        neg = -1e4 if dt == torch.float16 else -1e9
-        cross_mask = (1.0 - enc_mask.reshape(B, Lk).to(torch.float32)) * neg
+        split = _cross_split(Lk)
+        cross_mask = _cross_mask(enc_mask, B, Lk, dt)
         cross_live = ops.key_block_live(cross_mask)           # padded 64-key tiles of the encoder output: skipped, once
         capture = getattr(self, "_capture", False)
         # Only the encoder positions inside a live 64-key tile are ever read by the cross-attention: project K | V for those
@@ -535,17 +572,16 @@ class FiD(nn.Module):
         compact = (cross_kv is None and cross_live is not None and not capture and ops._XKV_COMPACT and ops._XATTN_STREAM
                    and T <= 64 and Lk % 64 == 0 and Lk >= 1024)
         xkv = None
-        if compact and enc_packed is not None:
-            # the encoder already ran on its kept tiles (a superset of the live ones, same tile order): project those rows
-            enc_live, keep, tile_off, n_live_rows = enc_packed
-            cross_live = keep.view(B, Lk // 64)
-            xkv = [ops.linear(enc_live, G[f"decoder.block.{i}.layer.1.EncDecAttention.kv"], rows=n_live_rows)
-                   for i in range(c.num_decoder_layers)]
-        elif compact:
-            flat = enc.reshape(-1, d)
-            if flat.dtype != dt:
-                flat = flat.to(dt)
-            enc_live, tile_off, n_live_rows = ops.compact_live_tiles(flat, cross_live)
+        if compact:
+            if enc_packed is not None:
+                # the encoder already ran on its kept tiles (a superset of the live ones, same tile order): project those rows
+                enc_live, keep, tile_off, n_live_rows = enc_packed
+                cross_live = keep.view(B, Lk // 64)
+            else:
+                flat = enc.reshape(-1, d)
+                if flat.dtype != dt:
+                    flat = flat.to(dt)
+                enc_live, tile_off, n_live_rows = ops.compact_live_tiles(flat, cross_live)
             xkv = [ops.linear(enc_live, G[f"decoder.block.{i}.layer.1.EncDecAttention.kv"], rows=n_live_rows)
                    for i in range(c.num_decoder_layers)]
         elif cross_kv is None:
@@ -555,70 +591,26 @@ class FiD(nn.Module):
                              c.relative_attention_num_buckets)
         qkv = torch.empty((B * T, 3 * H * 64), dtype=dt, device=h.device)
 
+        def self_attn(qkv, i):
+            return ops.attention(qkv, 0, qkv, H * 64, qkv, 2 * H * 64, B, H, T, T, bias_delta=bias, scale=1.0,
+                                 causal_value=-10000.0)
+
         def cross(q, i):
             if xkv is not None:
                 return ops.cross_attention_stream_compact(q, xkv[i], cross_live, tile_off, B, H, T, Lk, cross_mask, scale=1.0)
-            return ops.cross_attention_split(q, 0, cross_kv[i], 0, H * 64, B, H, T, Lk, add_mask=cross_mask, scale=1.0,
-                                             split=split, tile_live=cross_live)
+            r = ops.cross_attention_split(q, 0, cross_kv[i], 0, H * 64, B, H, T, Lk, add_mask=cross_mask, scale=1.0,
+                                          split=split, return_lse=capture, tile_live=cross_live)
+            if not capture:
+                return r
+            self._record_xattn(q, cross_kv[i], B, H, T, Lk, r[1], cross_mask, layer=i)
+            return r[0]
 
-        if self.fuse_norm and not capture:
-            # RMSNorm fused around the decoder GEMMs exactly like the encoder's (see encode): the three residual GEMMs of a
-            # block emit each row's sum of squares, the consuming projections read the un-normalised rows with the norm weight
-            # folded into their matrices.  3 x num_decoder_layers - 1 launches of a ~150-launch dependent chain disappear.
-            eps = c.layer_norm_epsilon
-            nl = c.num_decoder_layers
-            ss = torch.zeros((3 * nl, B * T), dtype=torch.float32, device=h.device)
-            for i in range(nl):
-                p = f"decoder.block.{i}.layer.0."
-                if i == 0:
-                    n = ops.layernorm(h, W[p + "layer_norm.weight"], None, eps, kind=1)
-                    ops.linear(n, G[p + "SelfAttention.qkv"], out=qkv)
-                else:
-                    ops.linear(h, G[p + "SelfAttention.qkv_n"], out=qkv, row_ss=ss[3 * i - 1], rs_eps=eps)
-                ctx = ops.attention(qkv, 0, qkv, H * 64, qkv, 2 * H * 64, B, H, T, T, bias_delta=bias, scale=1.0,
-                                    causal_value=-10000.0)
-                h = ops.linear(ctx, W[p + "SelfAttention.o.weight"], None, residual=h, epilogue=ops.EPI_RESIDUAL,
-                               out_ss=ss[3 * i])
-                ops.clamp_inf_(h, row_ss=ss[3 * i])
-                p = f"decoder.block.{i}.layer.1."
-                q = ops.linear(h, G[p + "EncDecAttention.q.weight_n"], row_ss=ss[3 * i], rs_eps=eps)
-                ctx = cross(q, i)
-                h = ops.linear(ctx, W[p + "EncDecAttention.o.weight"], None, residual=h, epilogue=ops.EPI_RESIDUAL,
-                               out_ss=ss[3 * i + 1])
-                ops.clamp_inf_(h, row_ss=ss[3 * i + 1])
-                p = f"decoder.block.{i}.layer.2."
-                g = self._ff_in(W, G, p, h, row_ss=ss[3 * i + 1], eps=eps)
-                h = ops.linear(g, W[p + "DenseReluDense.wo.weight"], None, residual=h, epilogue=ops.EPI_RESIDUAL,
-                               out_ss=ss[3 * i + 2])
-                ops.clamp_inf_(h, row_ss=ss[3 * i + 2])
-            h = ops.layernorm(h, W["decoder.final_layer_norm.weight"], None, eps, kind=1)
-            if getattr(c, "tie_word_embeddings", False):
-                h = (h.float() * (d ** -0.5)).to(dt)                              # src/modeling_t5.py:1642-1645
-            return ops.linear(h, self._head(W)).view(B, T, -1)
+        # fuse_norm: the RMSNorms fused around the GEMMs like the encoder's; 3 x num_decoder_layers - 1 launches of a
+        # ~150-launch dependent chain disappear.  The recording forward keeps the norm kernels.
+        ss = _norm_sums(3 * c.num_decoder_layers, B * T, h.device, self.fuse_norm and not capture)
         for i in range(c.num_decoder_layers):
-            p = f"decoder.block.{i}.layer.0."
-            n = ops.layernorm(h, W[p + "layer_norm.weight"], None, c.layer_norm_epsilon, kind=1)
-            ops.linear(n, G[p + "SelfAttention.qkv"], out=qkv)
-            ctx = ops.attention(qkv, 0, qkv, H * 64, qkv, 2 * H * 64, B, H, T, T, bias_delta=bias, scale=1.0,
-                                causal_value=-10000.0)
-            h = ops.clamp_inf_(ops.linear(ctx, W[p + "SelfAttention.o.weight"], None, residual=h, epilogue=ops.EPI_RESIDUAL))
-            p = f"decoder.block.{i}.layer.1."
-            n = ops.layernorm(h, W[p + "layer_norm.weight"], None, c.layer_norm_epsilon, kind=1)
-            q = ops.linear(n, W[p + "EncDecAttention.q.weight"])
-            if capture:
-                ctx, lse = ops.cross_attention_split(q, 0, cross_kv[i], 0, H * 64, B, H, T, Lk, add_mask=cross_mask,
-                                                     scale=1.0, split=split, return_lse=True, tile_live=cross_live)
-                self._record_xattn(q, cross_kv[i], B, H, T, Lk, lse, cross_mask, layer=i)
-            else:
-                ctx = cross(q, i)
-            h = ops.clamp_inf_(ops.linear(ctx, W[p + "EncDecAttention.o.weight"], None, residual=h,
-                                          epilogue=ops.EPI_RESIDUAL))
-            h = self._ff(W, G, f"decoder.block.{i}.layer.2.", h, c.layer_norm_epsilon)
-        h = ops.layernorm(h, W["decoder.final_layer_norm.weight"], None, c.layer_norm_epsilon, kind=1)
-        if getattr(c, "tie_word_embeddings", False):
-            h = (h.float() * (d ** -0.5)).to(dt)                                  # src/modeling_t5.py:1642-1645
-        logits = ops.linear(h, self._head(W))
-        return logits.view(B, T, -1)
+            h = self._decoder_block(W, G, i, h, self_attn, cross, ss[3 * i: 3 * i + 4], qkv)
+        return self._lm_head(W, h, dt).view(B, T, -1)
 
     # ---- training path (autograd through the kernels, grad_ops.py) ---------------------------------------
     def _train_weights(self):
@@ -626,17 +618,7 @@ class FiD(nn.Module):
         the kernels' weight gradients back to the reference-named parameters (q / k / v, wi_0 / wi_1 ...)."""
         dt = self._dtype()
         W = {n: (p if p.dtype == dt else p.to(dt)) for n, p in self.named_parameters()}
-        G = {}
-        for name in list(W.keys()):
-            if name.endswith("DenseReluDense.wi_0.weight"):
-                w0, w1 = W[name], W[name.replace("wi_0", "wi_1")]
-                G[name.replace("wi_0.weight", "wi_01")] = torch.stack([w0, w1], dim=1).reshape(-1, w0.shape[1])
-            elif name.endswith("SelfAttention.q.weight"):
-                G[name.replace("q.weight", "qkv")] = torch.cat(
-                    [W[name], W[name.replace("q.weight", "k.weight")], W[name.replace("q.weight", "v.weight")]], 0)
-            elif name.endswith("EncDecAttention.k.weight"):
-                G[name.replace("k.weight", "kv")] = torch.cat([W[name], W[name.replace("k.weight", "v.weight")]], 0)
-        return W, G, dt
+        return W, self._concat_weights(W), dt
 
     def _check_trainable(self):
         return None
@@ -720,19 +702,10 @@ class FiD(nn.Module):
         Lk = enc.shape[1]
         eps = c.layer_norm_epsilon
         pdrop = self._dropout_p()
-        split = None
-        if pdrop:    # the dropout mask is addressed in 32-key groups over the whole key range (csrc/dropout.cuh)
-            split = next((s for s in range(min(512, Lk) // 32 * 32, 63, -32) if Lk % s == 0), None)
-        split = split or next((s for s in range(min(384, Lk), 63, -1) if Lk % s == 0), None) or \
-            next(s for s in range(min(512, Lk), 0, -1) if Lk % s == 0)
-        if split < 64 and Lk > 512:
-            raise AtlasB200Error(f"n_context*text_maxlength = {Lk} has no divisor in [64, 512] for the split-KV kernel")
+        split = _cross_split(Lk, dropout=pdrop > 0)
         flat = enc.reshape(-1, d)
         if flat.dtype != dt:
             flat = flat.to(dt)
-        if pdrop and split % 32 != 0 and split != Lk:
-            raise AtlasB200Error(f"dropout on the cross-attention probabilities needs a key split that is a multiple of 32 "
-                                 f"(n_context*text_maxlength = {Lk} gave {split})")
         h = g.dropout(self._embed_train(W, dt, decoder_input_ids), pdrop)
 
         def lin_res(x, w, res):
@@ -742,8 +715,7 @@ class FiD(nn.Module):
 
         bias = bias_by_delta(W["decoder.block.0.layer.0.SelfAttention.relative_attention_bias.weight"], T, T, False,
                              c.relative_attention_num_buckets)
-        neg = -1e4 if dt == torch.float16 else -1e9
-        cross_mask = (1.0 - enc_mask.reshape(B, Lk).to(torch.float32)) * neg
+        cross_mask = _cross_mask(enc_mask, B, Lk, dt)
         cross_mask._atlas_block_live = ops.key_block_live(cross_mask)     # padded 64-key tiles: skipped forward and backward
 
         def block(i, h, bias, flat):
@@ -865,6 +837,14 @@ class FiD(nn.Module):
             self.graph = None
             self.cross_live = None
 
+        def reset(self, start, pad):
+            """greedy_search's start: every sequence holds the decoder start token, none is done."""
+            self.seq.fill_(pad)
+            self.seq[:, 0] = start
+            self.tok_in.fill_(start)
+            self.done.zero_()
+            self.t_dev.zero_()
+
     @staticmethod
     def _cross_kv_buffers(rows, H, nl, dt, dev, xkv):
         """The cross K|V cache of a decode state: per layer [rows, 2*H*64] in the run's 16-bit dtype (xkv None), or for
@@ -881,42 +861,31 @@ class FiD(nn.Module):
         c = self.config
         W, G, dt = self._weights()
         H = c.num_heads
-        eps = c.layer_norm_epsilon
         B, Lk = st.B, st.Lk
         nb = getattr(st, "nb", 1)           # beam search: B * nb rows, the nb beams of a batch element consecutive
         h = W["shared.weight"][st.tok_in]                                          # [B * nb, d]
-        for i in range(c.num_decoder_layers):
-            p = f"decoder.block.{i}.layer.0."
-            n = ops.layernorm(h, W[p + "layer_norm.weight"], None, eps, kind=1)
-            qkv = ops.linear(n, G[p + "SelfAttention.qkv"])
+
+        def self_attn(qkv, i):
             if nb > 1:      # history gathered through the beams' ancestry table: the cache is never reordered
-                ctx = ops.decode_self_attention_beam(qkv, st.self_kv[i], st.t_dev, st.anc, H, bias_delta=st.bias, scale=1.0)
-            else:
-                ctx = ops.decode_self_attention(qkv, st.self_kv[i], st.t_dev, H, bias_delta=st.bias, scale=1.0)
-            h = ops.clamp_inf_(ops.linear(ctx, W[p + "SelfAttention.o.weight"], None, residual=h, epilogue=ops.EPI_RESIDUAL))
-            p = f"decoder.block.{i}.layer.1."
-            n = ops.layernorm(h, W[p + "layer_norm.weight"], None, eps, kind=1)
-            q = ops.linear(n, W[p + "EncDecAttention.q.weight"])
+                return ops.decode_self_attention_beam(qkv, st.self_kv[i], st.t_dev, st.anc, H, bias_delta=st.bias, scale=1.0)
+            return ops.decode_self_attention(qkv, st.self_kv[i], st.t_dev, H, bias_delta=st.bias, scale=1.0)
+
+        def cross(q, i):
             if st.cross_scale is not None:      # opt-in e4m3 cross K|V cache (cross_kv_dtype="fp8")
                 if nb > 1:
-                    ctx = ops.decode_cross_attention_beams_e4m3(q, st.cross_kv[i], st.cross_scale[i], B, nb, H, Lk, st.cross_mask,
-                                                                st.chunk, tile_live=st.cross_live)
-                else:
-                    ctx = ops.decode_cross_attention_e4m3(q, st.cross_kv[i], st.cross_scale[i], B, H, Lk, add_mask=st.cross_mask,
-                                                          scale=1.0, chunk=st.chunk, tile_live=st.cross_live)
-            elif nb > 1:    # the nb beams share their batch element's cross K | V, streamed once per step
-                ctx = ops.decode_cross_attention_beams(q, st.cross_kv[i], B, nb, H, Lk, st.cross_mask, st.chunk,
-                                                       tile_live=st.cross_live)
-            else:
-                ctx = ops.decode_cross_attention(q, st.cross_kv[i], B, H, Lk, add_mask=st.cross_mask, scale=1.0,
-                                                 chunk=st.chunk, tile_live=st.cross_live)
-            h = ops.clamp_inf_(ops.linear(ctx, W[p + "EncDecAttention.o.weight"], None, residual=h,
-                                          epilogue=ops.EPI_RESIDUAL))
-            h = self._ff(W, G, f"decoder.block.{i}.layer.2.", h, eps)
-        h = ops.layernorm(h, W["decoder.final_layer_norm.weight"], None, eps, kind=1)
-        if getattr(c, "tie_word_embeddings", False):
-            h = (h.float() * (c.d_model ** -0.5)).to(dt)
-        return ops.linear(h, self._head(W))
+                    return ops.decode_cross_attention_beams_e4m3(q, st.cross_kv[i], st.cross_scale[i], B, nb, H, Lk,
+                                                                 st.cross_mask, st.chunk, tile_live=st.cross_live)
+                return ops.decode_cross_attention_e4m3(q, st.cross_kv[i], st.cross_scale[i], B, H, Lk, add_mask=st.cross_mask,
+                                                       scale=1.0, chunk=st.chunk, tile_live=st.cross_live)
+            if nb > 1:      # the nb beams share their batch element's cross K | V, streamed once per step
+                return ops.decode_cross_attention_beams(q, st.cross_kv[i], B, nb, H, Lk, st.cross_mask, st.chunk,
+                                                        tile_live=st.cross_live)
+            return ops.decode_cross_attention(q, st.cross_kv[i], B, H, Lk, add_mask=st.cross_mask, scale=1.0,
+                                              chunk=st.chunk, tile_live=st.cross_live)
+
+        for i in range(c.num_decoder_layers):       # the step keeps the norm kernels
+            h = self._decoder_block(W, G, i, h, self_attn, cross, (None,) * 4)
+        return self._lm_head(W, h, dt)
 
     class _BeamState:
         """Static buffers of one (batch, beams, keys, max_length, dtype) beam-search shape (csrc/beam.cu): the per-layer
@@ -1000,8 +969,7 @@ class FiD(nn.Module):
             # e4m3 cache: each layer's 16-bit projection (one reused scratch buffer) is quantized into the state's fixed
             # buffers (the captured step graph reads them)
             self.cross_kv(enc, sink=lambda i, kv: ops.quantize_kv_e4m3(kv, out=st.cross_kv[i], scale_out=st.cross_scale[i]))
-        neg = -1e4 if dt == torch.float16 else -1e9                                 # invert_attention_mask (4.18)
-        st.cross_mask.copy_((1.0 - attention_mask.reshape(B, Lk).to(torch.float32)) * neg)
+        st.cross_mask.copy_(_cross_mask(attention_mask, B, Lk, dt))
         live = ops.key_block_live(st.cross_mask)              # padded 64-key tiles: not read by the decode steps
         if live is not None:
             if st.cross_live is None:
@@ -1055,11 +1023,7 @@ class FiD(nn.Module):
         W, G, dt = self._weights()
         st = self._decode_state(B, Lk, int(max_length), dt, enc.device, xkv=cross_kv_dtype)
         self._prepare_decode(st, enc, attention_mask, W, dt)
-        st.seq.fill_(c.pad_token_id)
-        st.seq[:, 0] = c.decoder_start_token_id
-        st.tok_in.fill_(c.decoder_start_token_id)
-        st.done.zero_()
-        st.t_dev.zero_()
+        st.reset(c.decoder_start_token_id, c.pad_token_id)
         n_steps = int(max_length) - 1
 
         def step():
@@ -1068,20 +1032,9 @@ class FiD(nn.Module):
 
         use_graph = self.cuda_graphs and prefix_allowed_tokens_fn is None and n_steps > 0
         if use_graph and (st.graph is None or getattr(st, "min_length", None) != int(min_length)):
-            side = torch.cuda.Stream()
-            side.wait_stream(torch.cuda.current_stream())
-            with torch.cuda.stream(side):                    # eager warm-up step on scratch state (then reset below)
-                step()
-            torch.cuda.current_stream().wait_stream(side)
-            st.graph = torch.cuda.CUDAGraph()
-            with torch.cuda.graph(st.graph):
-                step()
+            st.graph = _capture(step)[0]
             st.min_length = int(min_length)
-            st.seq.fill_(c.pad_token_id)
-            st.seq[:, 0] = c.decoder_start_token_id
-            st.tok_in.fill_(c.decoder_start_token_id)
-            st.done.zero_()
-            st.t_dev.zero_()
+            st.reset(c.decoder_start_token_id, c.pad_token_id)
         ran = 0
         for s_i in range(n_steps):
             if use_graph:
@@ -1150,14 +1103,7 @@ class FiD(nn.Module):
         use_graph = self.cuda_graphs and prefix_allowed_tokens_fn is None and n_steps > 0
         gkey = (min_length, length_penalty, round_lp)
         if use_graph and (st.graph is None or getattr(st, "gkey", None) != gkey):
-            side = torch.cuda.Stream()
-            side.wait_stream(torch.cuda.current_stream())
-            with torch.cuda.stream(side):                    # eager warm-up step on scratch state (then reset below)
-                step()
-            torch.cuda.current_stream().wait_stream(side)
-            st.graph = torch.cuda.CUDAGraph()
-            with torch.cuda.graph(st.graph):
-                step()
+            st.graph = _capture(step)[0]
             st.gkey = gkey
             st.reset(c.decoder_start_token_id, pad)
         for s_i in range(n_steps):

@@ -490,6 +490,12 @@ _ENC_PACKED = os.environ.get("ATLAS_B200_ENC_PACKED", "1") != "0"          # A/B
 _BERT_PACKED = os.environ.get("ATLAS_B200_BERT_PACKED", "1") != "0"        # ... of the Contriever encoder (needs _ENC_PACKED too)
 
 
+def encoder_packs(live, L):
+    """Whether the padding-compacted encoder takes segments of L tokens with the live 64-key blocks `live`
+    (key_block_live): there is a mask, the segments are whole 64-row tiles, and at most 384 tokens long."""
+    return live is not None and L % 64 == 0 and 64 <= L <= 384
+
+
 def segment_tile_scan(live):
     """live uint8 [S, nb] (key_block_live) -> (keep uint8 [S, nb], tile_off int32 [S * nb], tile_src int32 [S * nb], count_rows
     int32 [1]): the packed layout of the padding-compacted encoder (include/atlas_b200.h).  No host synchronisation."""

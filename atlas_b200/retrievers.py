@@ -252,7 +252,7 @@ class Contriever(nn.Module):
         # to its last live key, packed back to back; projections run over the device-side row count, the attention on the
         # packed rows.  Padded positions never influence live ones and every consumer of the result masks them (mean pooling)
         # or reads position 0 (cls pooling): the returned rows of dropped tiles are 0.
-        packed = ops._ENC_PACKED and ops._BERT_PACKED and live is not None and L % 64 == 0 and 64 <= L <= 384
+        packed = ops._ENC_PACKED and ops._BERT_PACKED and ops.encoder_packs(live, L)
         rows = None
         if packed:
             keep, tile_off, _, rows = ops.segment_tile_scan(live)

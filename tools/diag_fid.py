@@ -77,7 +77,7 @@ with torch.no_grad():
         n = rms(h, W[p + "layer_norm.weight"])
         ff = torch.nn.functional.gelu(n @ W[p + "DenseReluDense.wi_0.weight"].T, approximate="tanh") * (n @ W[p + "DenseReluDense.wi_1.weight"].T)
         h = h + ff @ W[p + "DenseReluDense.wo.weight"].T
-        hh = model._ff(Wh, G, p, hh, 1e-6)
+        hh = model._residual(model._ff_in(Wh, G, p, hh), Wh[p + "DenseReluDense.wo.weight"], hh)
         print(f"layer {L_} after FF err", float((hh.float().view(B, T, d) - h).abs().max()))
     h = rms(h, W["decoder.final_layer_norm.weight"])
     logits_ref = h @ W["lm_head.weight"].T
