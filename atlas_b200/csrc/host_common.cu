@@ -60,6 +60,29 @@ int make_tmap_2d_16bit(CUtensorMap* out, const void* base, uint64_t rows, uint64
     return ATLAS_B200_OK;
 }
 
+int make_tmap_2d_bytes(CUtensorMap* out, const void* base, uint64_t rows, uint64_t cols, uint64_t ld, uint32_t box_rows,
+                       uint32_t box_cols) {
+    EncodeTiledFn fn = get_encode();
+    if (!fn) return ATLAS_B200_ECUDA;
+    if ((reinterpret_cast<uintptr_t>(base) & 15u) != 0 || ld % 16 != 0) {
+        set_error("tensor map: base must be 16-byte aligned and the row stride a multiple of 16 bytes");
+        return ATLAS_B200_EINVAL;
+    }
+    cuuint64_t gdim[2] = {cols, rows};
+    cuuint64_t gstride[1] = {ld};
+    cuuint32_t box[2] = {box_cols, box_rows};
+    cuuint32_t estr[2] = {1, 1};
+    CUresult r = fn(out, CU_TENSOR_MAP_DATA_TYPE_UINT8, 2, const_cast<void*>(base), gdim, gstride, box, estr,
+                    CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                    CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+    if (r != CUDA_SUCCESS) {
+        set_error("cuTensorMapEncodeTiled failed with CUresult %d (rows=%llu cols=%llu ld=%llu box=%ux%u)", (int)r,
+                  (unsigned long long)rows, (unsigned long long)cols, (unsigned long long)ld, box_rows, box_cols);
+        return ATLAS_B200_ECUDA;
+    }
+    return ATLAS_B200_OK;
+}
+
 int num_sms() {
     static int n = 0;
     if (n == 0) {

@@ -41,6 +41,10 @@ inline void count_launch(int n = 1) { g_launches.fetch_add(static_cast<uint64_t>
 int make_tmap_2d_16bit(CUtensorMap* out, const void* base, uint64_t rows, uint64_t cols, uint64_t ld,
                        uint32_t box_rows, uint32_t box_cols, bool bf16);
 
+// 2-D row-major tensor map of bytes: `rows` x `cols`, row stride `ld` bytes, box = {box_cols, box_rows}, no swizzle.
+int make_tmap_2d_bytes(CUtensorMap* out, const void* base, uint64_t rows, uint64_t cols, uint64_t ld, uint32_t box_rows,
+                       uint32_t box_cols);
+
 int num_sms();
 
 // Optional CUDA-event bracketing of the dominant kernel (bench.py's roofline measurement): when

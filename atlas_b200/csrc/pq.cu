@@ -20,6 +20,10 @@
 //   and the chunked exhaustive variant.  Scores accumulate in fp32 over m = 0..M-1, then + T, and are rounded ONCE to fp16.
 // Scan kernel: one row per thread, QPC queries per CTA whose LUTs (and coarse terms) sit in shared memory for the whole
 // sweep; a row's codes are read once per query group.
+//
+// The IVF-SQ index (type ivfsq) shares the coarse k-means, the coarse assignment and the top-k driver: its training,
+// encoding and search host code are at the end of this file, its scan kernel in ivfsq.cu.
+#include "ivfsq.cuh"
 #include "mips_select.cuh"
 
 #include <math.h>
@@ -553,6 +557,27 @@ static int codebook_norms(const float* codebooks, int M, float* norms, cudaStrea
     return ATLAS_B200_OK;
 }
 
+// Coarse quantizer (ivfpq, ivfsq): inner-product k-means on the first min(S, 256 n_list) sample rows (n_list >= 1,
+// S >= n_list); the first n_list rows are the initial centroids.  Leaves the fp16 copy of the result in w.coarse16.
+static int coarse_kmeans(const __half* sample, int64_t S, int n_list, int iters, float* coarse, const ChunkWs& w, int64_t R,
+                         int32_t* assign, int32_t* counts, cudaStream_t s) {
+    int rc;
+    const int64_t sc = S < static_cast<int64_t>(n_list) * KSUB ? S : static_cast<int64_t>(n_list) * KSUB;
+    pq_half_to_float_kernel<<<grid_1d(static_cast<int64_t>(n_list) * DIM, 256), 256, 0, s>>>(
+        sample, static_cast<int64_t>(n_list) * DIM, coarse);
+    abh::count_launch();
+    for (int it = 0; it < iters; ++it) {
+        if ((rc = coarse_to_half(coarse, n_list, w.coarse16, s))) return rc;
+        if ((rc = coarse_assign(sample, sc, w.coarse16, n_list, w, R, assign, nullptr, 0, s))) return rc;
+        pq_update_kernel<__half, int32_t><<<dim3(n_list, 1), 256, 0, s>>>(sample, DIM, assign, 1, static_cast<int>(sc),
+                                                                        n_list, DIM, coarse, counts);
+        pq_split_kernel<<<1, 256, 0, s>>>(coarse, counts, n_list, DIM);
+        abh::count_launch(2);
+        AB_CUDA_CHECK(cudaGetLastError());
+    }
+    return coarse_to_half(coarse, n_list, w.coarse16, s);
+}
+
 static int check_shape(int M, int n_list) {
     AB_REQUIRE(valid_m(M), "code_size M=%d is not supported: M must divide 768 with 768 / M >= 8 "
                "(1, 2, 3, 4, 6, 8, 12, 16, 24, 32, 48, 64, 96)", M);
@@ -582,22 +607,7 @@ static int train(const __half* sample, int64_t S, int M, int n_list, int iters, 
     const int dsub = DIM / M;
 
     // ---- coarse quantizer: inner-product k-means on the first min(S, 256 n_list) rows
-    if (n_list > 0) {
-        const int64_t sc = S < static_cast<int64_t>(n_list) * KSUB ? S : static_cast<int64_t>(n_list) * KSUB;
-        pq_half_to_float_kernel<<<grid_1d(static_cast<int64_t>(n_list) * DIM, 256), 256, 0, s>>>(
-            sample, static_cast<int64_t>(n_list) * DIM, coarse);
-        abh::count_launch();
-        for (int it = 0; it < iters; ++it) {
-            if ((rc = coarse_to_half(coarse, n_list, w.coarse16, s))) return rc;
-            if ((rc = coarse_assign(sample, sc, w.coarse16, n_list, w, R, assign, nullptr, 0, s))) return rc;
-            pq_update_kernel<__half, int32_t><<<dim3(n_list, 1), 256, 0, s>>>(sample, DIM, assign, 1, static_cast<int>(sc),
-                                                                            n_list, DIM, coarse, counts);
-            pq_split_kernel<<<1, 256, 0, s>>>(coarse, counts, n_list, DIM);
-            abh::count_launch(2);
-            AB_CUDA_CHECK(cudaGetLastError());
-        }
-        if ((rc = coarse_to_half(coarse, n_list, w.coarse16, s))) return rc;
-    }
+    if (n_list > 0 && (rc = coarse_kmeans(sample, S, n_list, iters, coarse, w, R, assign, counts, s))) return rc;
 
     // ---- product quantizer: L2 k-means per sub-space on the residuals of the first min(S, 65536) rows
     const int64_t sp = S < PQ_TRAIN_MAX ? S : PQ_TRAIN_MAX;
@@ -697,6 +707,52 @@ static int launch_scan(int qpc, const ScanParams& p, size_t smem, cudaStream_t s
     }
 }
 
+// The exact top-k pipeline of one block of nqb queries over the scores of a code sweep (mips.cu's one-stage sample):
+//   bound from a strided sample of ~2 sqrt(k n) rows (every score kept) -> full sweep with the bound -> select + emit,
+//   `status` on overflow; or the chunked exhaustive variant (every score of a chunk is a candidate, winners carried).
+// scan(tile_begin, tile_step, num_tiles) launches the scan kernel over tiles of `tile_rows` rows (n rows or slots in all);
+// it appends only real rows, so the sampled bound is the k-th best among real rows.  The sweep is profiled as kind 1.
+template <class Scan>
+static int sweep_select(const Scan& scan, int64_t n, int total_tiles, int tile_rows, int nqb, int k, uint64_t* cand,
+                        uint32_t* count, float* bound, uint32_t capq, uint16_t* os16, int64_t* oi_b, int64_t id_base,
+                        int64_t id_stride, int32_t* status, bool exhaustive, double sweep_work, cudaStream_t s) {
+    int rc;
+    if (!exhaustive) {
+        if (n > static_cast<int64_t>(capq)) {
+            double m = 2.0 * sqrt(static_cast<double>(k) * static_cast<double>(n));
+            if (m < 4096) m = 4096;
+            if (m > capq / 2) m = capq / 2;
+            int sample_tiles = static_cast<int>(m / tile_rows);
+            if (sample_tiles < 1) sample_tiles = 1;
+            if (sample_tiles > total_tiles) sample_tiles = total_tiles;
+            if ((rc = scan(0, total_tiles / sample_tiles, sample_tiles))) return rc;
+            mips::mips_select_kernel<false><<<nqb, mips::SEL_THREADS, 0, s>>>(
+                cand, count, capq, k, mips::SEL_WRITE_BOUND, bound, nullptr, nullptr, 0, 0, nullptr);
+            abh::count_launch();
+        }
+        abh::prof_begin(s, abh::PROF_SCAN);
+        rc = scan(0, 1, total_tiles);
+        abh::prof_end(s, abh::PROF_SCAN, sweep_work);
+        if (rc) return rc;
+        mips::mips_select_kernel<false><<<nqb, mips::SEL_THREADS, 0, s>>>(
+            cand, count, capq, k, mips::SEL_EMIT, bound, os16, oi_b, id_base, id_stride, status);
+        abh::count_launch();
+    } else {
+        int chunk_tiles = static_cast<int>((capq - static_cast<uint32_t>(k)) / tile_rows);
+        if (chunk_tiles < 1) chunk_tiles = 1;
+        for (int t0 = 0; t0 < total_tiles; t0 += chunk_tiles) {
+            const bool last = t0 + chunk_tiles >= total_tiles;
+            if ((rc = scan(t0, 1, last ? total_tiles - t0 : chunk_tiles))) return rc;
+            mips::mips_select_kernel<false><<<nqb, mips::SEL_THREADS, 0, s>>>(
+                cand, count, capq, k, last ? mips::SEL_EMIT : mips::SEL_CARRY, bound, os16, oi_b, id_base, id_stride,
+                nullptr);
+            abh::count_launch();
+        }
+    }
+    AB_CUDA_CHECK(cudaGetLastError());
+    return ATLAS_B200_OK;
+}
+
 static int topk(const uint8_t* codes, const void* lists, int64_t n, int M, const float* codebooks, const float* coarse,
                 int n_list, const __half* queries, int nq, int k, __half* out_scores, int64_t* out_ids, int64_t id_base,
                 int64_t id_stride, int32_t* status, void* ws, size_t ws_bytes, cudaStream_t s, bool exhaustive) {
@@ -745,52 +801,342 @@ static int topk(const uint8_t* codes, const void* lists, int64_t n, int M, const
         p.count = w.count;
         p.cand = w.cand;
         p.capq = w.capq;
-        __half* os_b = out_scores + static_cast<size_t>(q0) * k;
         int64_t* oi_b = out_ids + static_cast<size_t>(q0) * k;
-        uint16_t* os16 = reinterpret_cast<uint16_t*>(os_b);
-        if (!exhaustive) {
-            if (n > static_cast<int64_t>(w.capq)) {
-                // bound from a strided sample of ~2 sqrt(k n) rows (every score kept), as in mips.cu's one-stage sample
-                double m = 2.0 * sqrt(static_cast<double>(k) * static_cast<double>(n));
-                if (m < 4096) m = 4096;
-                if (m > w.capq / 2) m = w.capq / 2;
-                int sample_tiles = static_cast<int>(m / SCAN_THREADS);
-                if (sample_tiles < 1) sample_tiles = 1;
-                if (sample_tiles > total_tiles) sample_tiles = total_tiles;
-                p.tile_begin = 0;
-                p.tile_step = total_tiles / sample_tiles;
-                p.num_tiles = sample_tiles;
-                if ((rc = launch_scan(qpc, p, smem, s))) return rc;
-                mips::mips_select_kernel<false><<<nqb, mips::SEL_THREADS, 0, s>>>(
-                    w.cand, w.count, w.capq, k, mips::SEL_WRITE_BOUND, w.bound, nullptr, nullptr, 0, 0, nullptr);
-                abh::count_launch();
-            }
-            p.tile_begin = 0;
-            p.tile_step = 1;
-            p.num_tiles = total_tiles;
-            abh::prof_begin(s, abh::PROF_SCAN);
-            rc = launch_scan(qpc, p, smem, s);
-            abh::prof_end(s, abh::PROF_SCAN, static_cast<double>(n) * M * ((nqb + qpc - 1) / qpc));
-            if (rc) return rc;
-            mips::mips_select_kernel<false><<<nqb, mips::SEL_THREADS, 0, s>>>(
-                w.cand, w.count, w.capq, k, mips::SEL_EMIT, w.bound, os16, oi_b, id_base, id_stride, status);
-            abh::count_launch();
-        } else {
-            // chunked exact scan: every score of a chunk is a candidate, winners are carried forward
-            int chunk_tiles = static_cast<int>((w.capq - static_cast<uint32_t>(k)) / SCAN_THREADS);
-            if (chunk_tiles < 1) chunk_tiles = 1;
-            for (int t0 = 0; t0 < total_tiles; t0 += chunk_tiles) {
-                const bool last = t0 + chunk_tiles >= total_tiles;
-                p.tile_begin = t0;
-                p.tile_step = 1;
-                p.num_tiles = last ? total_tiles - t0 : chunk_tiles;
-                if ((rc = launch_scan(qpc, p, smem, s))) return rc;
-                mips::mips_select_kernel<false><<<nqb, mips::SEL_THREADS, 0, s>>>(
-                    w.cand, w.count, w.capq, k, last ? mips::SEL_EMIT : mips::SEL_CARRY, w.bound, os16, oi_b, id_base,
-                    id_stride, nullptr);
-                abh::count_launch();
-            }
+        uint16_t* os16 = reinterpret_cast<uint16_t*>(out_scores + static_cast<size_t>(q0) * k);
+        auto scan = [&](int tile_begin, int tile_step, int num_tiles) {
+            p.tile_begin = tile_begin;
+            p.tile_step = tile_step;
+            p.num_tiles = num_tiles;
+            return launch_scan(qpc, p, smem, s);
+        };
+        if ((rc = sweep_select(scan, n, total_tiles, SCAN_THREADS, nqb, k, w.cand, w.count, w.bound, w.capq, os16, oi_b, id_base,
+                               id_stride, status, exhaustive, static_cast<double>(n) * M * ((nqb + qpc - 1) / qpc), s)))
+            return rc;
+    }
+    AB_CUDA_CHECK(cudaGetLastError());
+    return ATLAS_B200_OK;
+}
+
+// ---------------------------------------------------------------------------------------------
+// IVF-SQ (faiss IndexIVFScalarQuantizer, QT_4bit, residuals, inner product; layout: ivfsq.cuh, scan: ivfsq.cu)
+//   range    per dim: vmin = min r_d, vdiff = max r_d - vmin over the residuals r = fp32(x) - coarse[list(x)] of the
+//            first min(S, 100000) sample rows (faiss RS_minmax, non-uniform)
+//   encode   xi = (r_d - vmin_d) / vdiff_d (0 when vdiff_d == 0), clamped to [0, 1]; code = (int)(xi * 15.0) in double
+//   search   w^[q][d] = fp16(2^e_q * q_d * (vdiff_d / 15)), e_q putting max_d |w^| in [2^14, 2^15);
+//            C[q] = sum_d q_d (vmin_d + 0.5 vdiff_d / 15) + 2^-e_q * 8 sum_d w^[q][d], T[l][q] = <q, c_l> (fp32);
+//            s = fp16(T[list][q] + C[q] + 2^-e_q * sum_d w^[q][d] (code_d - 8))
+// ---------------------------------------------------------------------------------------------
+constexpr int64_t SQ_RANGE_MAX = 100000;   // faiss ScalarQuantizer::train_residual's subsample
+constexpr int SQ_RANGE_ROWS = 512;         // rows per partial min / max block
+
+// partial per-dim min / max of the residuals of rows [c * SQ_RANGE_ROWS, ...) of the first ns rows, c = blockIdx.x
+__global__ void __launch_bounds__(256) sq_range_partial_kernel(const __half* __restrict__ x, int64_t ns,
+                                                               const float* __restrict__ coarse,
+                                                               const int32_t* __restrict__ assign, float* __restrict__ pmin,
+                                                               float* __restrict__ pmax) {
+    const int64_t r0 = static_cast<int64_t>(blockIdx.x) * SQ_RANGE_ROWS;
+    const int64_t r1 = r0 + SQ_RANGE_ROWS < ns ? r0 + SQ_RANGE_ROWS : ns;
+    for (int d = threadIdx.x; d < DIM; d += 256) {
+        float lo = INFINITY, hi = -INFINITY;
+        for (int64_t i = r0; i < r1; ++i) {
+            const float r = __fsub_rn(__half2float(x[i * DIM + d]), coarse[static_cast<int64_t>(assign[i]) * DIM + d]);
+            lo = fminf(lo, r);
+            hi = fmaxf(hi, r);
         }
+        pmin[static_cast<int64_t>(blockIdx.x) * DIM + d] = lo;
+        pmax[static_cast<int64_t>(blockIdx.x) * DIM + d] = hi;
+    }
+}
+
+__global__ void sq_range_final_kernel(const float* __restrict__ pmin, const float* __restrict__ pmax, int parts,
+                                      float* __restrict__ vmin, float* __restrict__ vdiff) {
+    const int d = blockIdx.x * blockDim.x + threadIdx.x;
+    if (d >= DIM) return;
+    float lo = INFINITY, hi = -INFINITY;
+    for (int c = 0; c < parts; ++c) {
+        lo = fminf(lo, pmin[static_cast<int64_t>(c) * DIM + d]);
+        hi = fmaxf(hi, pmax[static_cast<int64_t>(c) * DIM + d]);
+    }
+    vmin[d] = lo;
+    vdiff[d] = __fsub_rn(hi, lo);
+}
+
+// 4-bit codes of rows [n] (list assign[i]) into slot row_slot[i] of `codes`, in the slot's nibble order; one thread per
+// 32-bit output word
+__global__ void sq_encode_kernel(const __half* __restrict__ x, int64_t n, const float* __restrict__ coarse,
+                                 const int32_t* __restrict__ assign, const float* __restrict__ vmin,
+                                 const float* __restrict__ vdiff, const int32_t* __restrict__ row_slot,
+                                 uint8_t* __restrict__ codes) {
+    constexpr int WORDS = ivfsq::SQ_CODE_BYTES / 4;
+    const int64_t total = n * WORDS;
+    for (int64_t e = blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x; e < total;
+         e += static_cast<int64_t>(gridDim.x) * blockDim.x) {
+        const int64_t i = e / WORDS;
+        const int wd = static_cast<int>(e - i * WORDS);
+        const float* c = coarse + static_cast<int64_t>(assign[i]) * DIM;
+        uint32_t word = 0;
+#pragma unroll
+        for (int b = 0; b < 8; ++b) {
+            const int d = ivfsq::sq_dim_of_nibble(8 * wd + b);
+            const float r = __fsub_rn(__half2float(x[i * DIM + d]), c[d]);
+            float xi = 0.f;
+            if (vdiff[d] != 0.f) {
+                xi = __fdiv_rn(__fsub_rn(r, vmin[d]), vdiff[d]);
+                xi = xi < 0.f ? 0.f : (xi > 1.f ? 1.f : xi);
+            }
+            const uint32_t code = static_cast<uint32_t>(static_cast<int>(static_cast<double>(xi) * 15.0));
+            word |= code << (4 * b);
+        }
+        reinterpret_cast<uint32_t*>(codes + static_cast<int64_t>(row_slot[i]) * ivfsq::SQ_CODE_BYTES)[wd] = word;
+    }
+}
+
+// Per query row q of a block (one CTA each, rows past nq are zero): the fp16 operand w^, the fp32 row, C[q], 2^-e_q;
+// resets the block's candidate counters and bounds.
+__global__ void __launch_bounds__(256) sq_query_kernel(const __half* __restrict__ q16, int nq, const float* __restrict__ vmin,
+                                                       const float* __restrict__ vdiff, __half* __restrict__ what,
+                                                       float* __restrict__ qf32, float* __restrict__ cterm,
+                                                       float* __restrict__ scale, uint32_t* __restrict__ count,
+                                                       float* __restrict__ bound) {
+    __shared__ float s_max[256], s_sum[256], s_wsum[256];
+    const int q = blockIdx.x, t = threadIdx.x;
+    float pv[DIM / 256];
+    float mx = 0.f, cs = 0.f;
+#pragma unroll
+    for (int r = 0; r < DIM / 256; ++r) {
+        const int d = t + 256 * r;
+        const float qf = q < nq ? __half2float(q16[static_cast<int64_t>(q) * DIM + d]) : 0.f;
+        qf32[static_cast<int64_t>(q) * DIM + d] = qf;
+        pv[r] = __fmul_rn(qf, __fdiv_rn(vdiff[d], 15.f));
+        mx = fmaxf(mx, fabsf(pv[r]));
+        cs = __fadd_rn(cs, __fmul_rn(qf, __fadd_rn(vmin[d], __fdiv_rn(__fmul_rn(0.5f, vdiff[d]), 15.f))));
+    }
+    s_max[t] = mx;
+    s_sum[t] = cs;
+    __syncthreads();
+    for (int o = 128; o > 0; o >>= 1) {
+        if (t < o) {
+            s_max[t] = fmaxf(s_max[t], s_max[t + o]);
+            s_sum[t] = __fadd_rn(s_sum[t], s_sum[t + o]);
+        }
+        __syncthreads();
+    }
+    int e = 0;
+    if (s_max[0] > 0.f && s_max[0] < INFINITY) {
+        int x;
+        frexpf(s_max[0], &x);     // max in [2^(x-1), 2^x)  ->  max * 2^(15 - x) in [2^14, 2^15)
+        e = 15 - x;
+    }
+    float ws = 0.f;
+#pragma unroll
+    for (int r = 0; r < DIM / 256; ++r) {
+        const __half w = __float2half_rn(ldexpf(pv[r], e));
+        what[static_cast<int64_t>(q) * DIM + t + 256 * r] = w;
+        ws = __fadd_rn(ws, __half2float(w));
+    }
+    s_wsum[t] = ws;
+    __syncthreads();
+    for (int o = 128; o > 0; o >>= 1) {
+        if (t < o) s_wsum[t] = __fadd_rn(s_wsum[t], s_wsum[t + o]);
+        __syncthreads();
+    }
+    if (t == 0) {
+        // the MMA sums w^ (code - 8): C carries the offset 8 sum_d w^
+        cterm[q] = __fadd_rn(s_sum[0], ldexpf(8.f * s_wsum[0], -e));
+        scale[q] = ldexpf(1.f, -e);
+        count[q] = 0;
+        bound[q] = -INFINITY;
+    }
+}
+
+static int64_t sq_chunk_rows(int n_list) {
+    int64_t r = static_cast<int64_t>(CHUNK_BUDGET / (static_cast<size_t>(pad8(n_list)) * 2 + 4));
+    if (r > 65536) r = 65536;
+    r = r / 64 * 64;
+    return r < 64 ? 64 : r;
+}
+
+static size_t sq_train_bytes(int64_t S, int n_list, ChunkWs* w, int32_t** assign, int32_t** counts, float** pmin,
+                             float** pmax, void* base) {
+    Carver cv{static_cast<uint8_t*>(base)};
+    const int64_t R = sq_chunk_rows(n_list);
+    const int64_t ns = S < SQ_RANGE_MAX ? S : SQ_RANGE_MAX;
+    const int parts = static_cast<int>((ns + SQ_RANGE_ROWS - 1) / SQ_RANGE_ROWS);
+    ChunkWs tmp{};
+    ChunkWs& c = w ? *w : tmp;
+    c.gemm = cv.take<__half>(static_cast<size_t>(R) * pad8(n_list));
+    c.coarse16 = cv.take<__half>(static_cast<size_t>(pad8(n_list)) * DIM);
+    int32_t* a = cv.take<int32_t>(static_cast<size_t>(S));
+    int32_t* n = cv.take<int32_t>(static_cast<size_t>(n_list));
+    float* lo = cv.take<float>(static_cast<size_t>(parts) * DIM);
+    float* hi = cv.take<float>(static_cast<size_t>(parts) * DIM);
+    if (assign) *assign = a;
+    if (counts) *counts = n;
+    if (pmin) *pmin = lo;
+    if (pmax) *pmax = hi;
+    return cv.off;
+}
+
+static size_t sq_encode_bytes(int n_list, ChunkWs* w, void* base) {
+    Carver cv{static_cast<uint8_t*>(base)};
+    const int64_t R = sq_chunk_rows(n_list);
+    ChunkWs tmp{};
+    ChunkWs& c = w ? *w : tmp;
+    c.gemm = cv.take<__half>(static_cast<size_t>(R) * pad8(n_list));
+    c.coarse16 = cv.take<__half>(static_cast<size_t>(pad8(n_list)) * DIM);
+    c.assign = cv.take<int32_t>(static_cast<size_t>(R));
+    return cv.off;
+}
+
+struct SqSearchWs {
+    uint32_t* count;
+    float* bound;
+    uint64_t* cand;
+    uint32_t capq;
+    __half* what;   // [QBLOCK][768]
+    float* qf32;    // [QBLOCK][768]
+    float* tterm;   // [n_list][nqb]
+    float* cterm;   // [QBLOCK]
+    float* scale;   // [QBLOCK]
+};
+
+static size_t sq_search_bytes(int64_t n_slots, int n_list, int k, SqSearchWs* w, void* base) {
+    Carver cv{static_cast<uint8_t*>(base)};
+    const uint32_t capq = mips::capq_for(n_slots, k);
+    SqSearchWs x;
+    x.count = cv.take<uint32_t>(QBLOCK);
+    x.bound = cv.take<float>(QBLOCK);
+    x.cand = cv.take<uint64_t>(static_cast<size_t>(QBLOCK) * capq);
+    x.capq = capq;
+    x.what = cv.take<__half>(static_cast<size_t>(QBLOCK) * DIM);
+    x.qf32 = cv.take<float>(static_cast<size_t>(QBLOCK) * DIM);
+    x.tterm = cv.take<float>(static_cast<size_t>(n_list) * QBLOCK);
+    x.cterm = cv.take<float>(QBLOCK);
+    x.scale = cv.take<float>(QBLOCK);
+    if (w) *w = x;
+    return cv.off;
+}
+
+static int sq_train(const __half* sample, int64_t S, int n_list, int iters, float* coarse, float* vmin, float* vdiff, void* ws,
+                    size_t ws_bytes, cudaStream_t s) {
+    AB_REQUIRE(sample != nullptr && coarse != nullptr && vmin != nullptr && vdiff != nullptr, "null pointer argument");
+    AB_REQUIRE(n_list >= 1, "n_list=%d must be >= 1", n_list);
+    AB_REQUIRE(S >= n_list && S < (1ll << 31), "training needs at least n_list=%d rows (got %lld)", n_list, (long long)S);
+    AB_REQUIRE(iters >= 0, "iters=%d must be >= 0", iters);
+    ChunkWs w{};
+    int32_t *assign, *counts;
+    float *pmin, *pmax;
+    const size_t need = sq_train_bytes(S, n_list, &w, &assign, &counts, &pmin, &pmax, ws);
+    if (ws == nullptr || ws_bytes < need) {
+        abh::set_error("workspace too small: have %zu need %zu", ws_bytes, need);
+        return ATLAS_B200_EWORKSPACE;
+    }
+    const int64_t R = sq_chunk_rows(n_list);
+    int rc = coarse_kmeans(sample, S, n_list, iters, coarse, w, R, assign, counts, s);
+    if (rc) return rc;
+    const int64_t ns = S < SQ_RANGE_MAX ? S : SQ_RANGE_MAX;
+    if ((rc = coarse_assign(sample, ns, w.coarse16, n_list, w, R, assign, nullptr, 0, s))) return rc;
+    const int parts = static_cast<int>((ns + SQ_RANGE_ROWS - 1) / SQ_RANGE_ROWS);
+    sq_range_partial_kernel<<<parts, 256, 0, s>>>(sample, ns, coarse, assign, pmin, pmax);
+    sq_range_final_kernel<<<(DIM + 255) / 256, 256, 0, s>>>(pmin, pmax, parts, vmin, vdiff);
+    abh::count_launch(2);
+    AB_CUDA_CHECK(cudaGetLastError());
+    return ATLAS_B200_OK;
+}
+
+static int sq_encode(const __half* rows, int64_t n, const float* coarse, int n_list, const float* vmin, const float* vdiff,
+                     int32_t* lists, const int32_t* row_slot, uint8_t* codes, void* ws, size_t ws_bytes, cudaStream_t s) {
+    AB_REQUIRE(n >= 0, "n=%lld must be >= 0", (long long)n);
+    AB_REQUIRE(n_list >= 1, "n_list=%d must be >= 1", n_list);
+    if (n == 0) return ATLAS_B200_OK;
+    AB_REQUIRE(rows != nullptr && coarse != nullptr, "null pointer argument");
+    AB_REQUIRE(lists != nullptr || codes != nullptr, "nothing to write: list_ids and codes are both NULL");
+    AB_REQUIRE(codes == nullptr || (row_slot != nullptr && vmin != nullptr && vdiff != nullptr &&
+                                    abh::aligned(codes, 4)),
+               "codes need row_slot, vmin and vdiff, and must be 4-byte aligned");
+    ChunkWs w{};
+    const size_t need = sq_encode_bytes(n_list, &w, ws);
+    if (ws == nullptr || ws_bytes < need) {
+        abh::set_error("workspace too small: have %zu need %zu", ws_bytes, need);
+        return ATLAS_B200_EWORKSPACE;
+    }
+    const int64_t R = sq_chunk_rows(n_list);
+    int rc = coarse_to_half(coarse, n_list, w.coarse16, s);
+    if (rc) return rc;
+    for (int64_t r0 = 0; r0 < n; r0 += R) {
+        const int64_t cn = n - r0 < R ? n - r0 : R;
+        const __half* x = rows + r0 * DIM;
+        if ((rc = coarse_assign(x, cn, w.coarse16, n_list, w, R, w.assign, lists ? lists + r0 : nullptr, 0, s))) return rc;
+        if (codes) {
+            sq_encode_kernel<<<grid_1d(cn * (ivfsq::SQ_CODE_BYTES / 4), 256), 256, 0, s>>>(x, cn, coarse, w.assign, vmin, vdiff,
+                                                                                        row_slot + r0, codes);
+            abh::count_launch();
+            AB_CUDA_CHECK(cudaGetLastError());
+        }
+    }
+    return ATLAS_B200_OK;
+}
+
+static int sq_topk(const uint8_t* codes, const int32_t* slot_rows, const int32_t* tile_lists, int64_t n_tiles, int64_t n_rows,
+                   const float* coarse, int n_list, const float* vmin, const float* vdiff, const __half* queries, int nq, int k,
+                   __half* out_scores, int64_t* out_ids, int64_t id_base, int64_t id_stride, int32_t* status, void* ws,
+                   size_t ws_bytes, cudaStream_t s, bool exhaustive) {
+    AB_REQUIRE(nq >= 0 && k >= 1, "nq must be >= 0 and k >= 1 (nq=%d k=%d)", nq, k);
+    AB_REQUIRE(k <= ATLAS_B200_MAX_TOPK, "k=%d exceeds ATLAS_B200_MAX_TOPK=%d", k, ATLAS_B200_MAX_TOPK);
+    AB_REQUIRE(n_list >= 1, "n_list=%d must be >= 1", n_list);
+    AB_REQUIRE(n_rows >= 1 && n_tiles >= 1 && n_rows <= n_tiles * ivfsq::SQ_TILE &&
+                   n_tiles * ivfsq::SQ_TILE < (1ll << 31) - ivfsq::SQ_TILE,
+               "rows n=%lld / tiles %lld out of range", (long long)n_rows, (long long)n_tiles);
+    AB_REQUIRE(k <= n_rows, "selected index k out of range: k=%d > n=%lld", k, (long long)n_rows);
+    AB_REQUIRE(codes != nullptr && slot_rows != nullptr && tile_lists != nullptr && coarse != nullptr && vmin != nullptr &&
+                   vdiff != nullptr, "null pointer argument");
+    AB_REQUIRE(abh::aligned(codes, 16), "codes must be 16-byte aligned");
+    AB_REQUIRE(nq == 0 || queries != nullptr, "queries is null");
+    if (status) AB_CUDA_CHECK(cudaMemsetAsync(status, 0, sizeof(int32_t), s));
+    if (nq == 0) return ATLAS_B200_OK;
+    SqSearchWs w;
+    const int64_t n_slots = n_tiles * ivfsq::SQ_TILE;
+    const size_t need = sq_search_bytes(n_slots, n_list, k, &w, ws);
+    if (ws == nullptr || ws_bytes < need) {
+        abh::set_error("workspace too small: have %zu need %zu", ws_bytes, need);
+        return ATLAS_B200_EWORKSPACE;
+    }
+    int rc;
+    for (int q0 = 0; q0 < nq; q0 += QBLOCK) {
+        const int nqb = nq - q0 < QBLOCK ? nq - q0 : QBLOCK;
+        sq_query_kernel<<<QBLOCK, 256, 0, s>>>(queries + static_cast<int64_t>(q0) * DIM, nqb, vmin, vdiff, w.what, w.qf32,
+                                               w.cterm, w.scale, w.count, w.bound);
+        abh::count_launch();
+        // T[l][q] = <c_l, q>: the coarse centroids against the block's queries
+        if ((rc = subdot(coarse, DIM, n_list, w.qf32, nqb, DIM, 1, w.tterm, s))) return rc;
+        ivfsq::ScanParams p;
+        p.codes = codes;
+        p.slot_rows = slot_rows;
+        p.tile_lists = tile_lists;
+        p.n_tiles = static_cast<int>(n_tiles);
+        p.what = w.what;
+        p.tterm = w.tterm;
+        p.ldt = nqb;
+        p.cterm = w.cterm;
+        p.scale = w.scale;
+        p.nq = nqb;
+        p.bound = w.bound;
+        p.count = w.count;
+        p.cand = w.cand;
+        p.capq = w.capq;
+        int64_t* oi_b = out_ids + static_cast<size_t>(q0) * k;
+        uint16_t* os16 = reinterpret_cast<uint16_t*>(out_scores + static_cast<size_t>(q0) * k);
+        auto scan = [&](int tile_begin, int tile_step, int num_tiles) {
+            p.tile_begin = tile_begin;
+            p.tile_step = tile_step;
+            p.num_tiles = num_tiles;
+            return ivfsq::launch_scan(p, s);
+        };
+        // work = code bytes swept (once per 128 queries of the block)
+        const double sweep_bytes = static_cast<double>(n_slots) * ivfsq::SQ_CODE_BYTES * ((nqb + 127) / 128);
+        if ((rc = sweep_select(scan, n_slots, static_cast<int>(n_tiles), ivfsq::SQ_TILE, nqb, k, w.cand, w.count, w.bound,
+                               w.capq, os16, oi_b, id_base, id_stride, status, exhaustive, sweep_bytes, s)))
+            return rc;
     }
     AB_CUDA_CHECK(cudaGetLastError());
     return ATLAS_B200_OK;
@@ -840,6 +1186,50 @@ int atlas_b200_pq_topk_exhaustive(const uint8_t* codes, const void* list_ids, in
     return pq::topk(codes, list_ids, n, M, codebooks, coarse, n_list, static_cast<const __half*>(queries), nq, k,
                     static_cast<__half*>(out_scores), out_ids, id_base, id_stride, nullptr, workspace, workspace_bytes,
                     static_cast<cudaStream_t>(stream), true);
+}
+
+size_t atlas_b200_ivfsq_workspace_bytes(int32_t op, int64_t n, int32_t n_list, int32_t k) {
+    if (n_list < 1) return 0;
+    if (n < 1) n = 1;
+    if (k < 1) k = 1;
+    switch (op) {
+        case ATLAS_B200_PQ_OP_TRAIN: return pq::sq_train_bytes(n, n_list, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr);
+        case ATLAS_B200_PQ_OP_ENCODE: return pq::sq_encode_bytes(n_list, nullptr, nullptr);
+        case ATLAS_B200_PQ_OP_SEARCH: return pq::sq_search_bytes(n, n_list, k, nullptr, nullptr);
+        default: return 0;
+    }
+}
+
+int atlas_b200_ivfsq_train(const void* sample, int64_t n_sample, int32_t n_list, int32_t iters, float* coarse, float* vmin,
+                           float* vdiff, void* workspace, size_t workspace_bytes, void* stream) {
+    return pq::sq_train(static_cast<const __half*>(sample), n_sample, n_list, iters, coarse, vmin, vdiff, workspace,
+                        workspace_bytes, static_cast<cudaStream_t>(stream));
+}
+
+int atlas_b200_ivfsq_encode(const void* rows, int64_t n, const float* coarse, int32_t n_list, const float* vmin,
+                            const float* vdiff, int32_t* list_ids, const int32_t* row_slot, uint8_t* codes, void* workspace,
+                            size_t workspace_bytes, void* stream) {
+    return pq::sq_encode(static_cast<const __half*>(rows), n, coarse, n_list, vmin, vdiff, list_ids, row_slot, codes,
+                         workspace, workspace_bytes, static_cast<cudaStream_t>(stream));
+}
+
+int atlas_b200_ivfsq_topk(const uint8_t* codes, const int32_t* slot_rows, const int32_t* tile_lists, int64_t n_tiles,
+                          int64_t n_rows, const float* coarse, int32_t n_list, const float* vmin, const float* vdiff,
+                          const void* queries, int32_t nq, int32_t k, void* out_scores, int64_t* out_ids, int64_t id_base,
+                          int64_t id_stride, int32_t* status, void* workspace, size_t workspace_bytes, void* stream) {
+    return pq::sq_topk(codes, slot_rows, tile_lists, n_tiles, n_rows, coarse, n_list, vmin, vdiff,
+                       static_cast<const __half*>(queries), nq, k, static_cast<__half*>(out_scores), out_ids, id_base,
+                       id_stride, status, workspace, workspace_bytes, static_cast<cudaStream_t>(stream), false);
+}
+
+int atlas_b200_ivfsq_topk_exhaustive(const uint8_t* codes, const int32_t* slot_rows, const int32_t* tile_lists,
+                                     int64_t n_tiles, int64_t n_rows, const float* coarse, int32_t n_list, const float* vmin,
+                                     const float* vdiff, const void* queries, int32_t nq, int32_t k, void* out_scores,
+                                     int64_t* out_ids, int64_t id_base, int64_t id_stride, void* workspace,
+                                     size_t workspace_bytes, void* stream) {
+    return pq::sq_topk(codes, slot_rows, tile_lists, n_tiles, n_rows, coarse, n_list, vmin, vdiff,
+                       static_cast<const __half*>(queries), nq, k, static_cast<__half*>(out_scores), out_ids, id_base,
+                       id_stride, nullptr, workspace, workspace_bytes, static_cast<cudaStream_t>(stream), true);
 }
 
 }  // extern "C"

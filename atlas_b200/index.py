@@ -15,7 +15,8 @@ Same public surface: `embeddings` ([768, N] fp16 CUDA, slice-assignable on dim 1
   * ties are ordered canonically: score descending, then global passage id ascending.
 
 There is no CPU path: `is_in_gpu = False` raises here.  `DistributedFAISSIndex` (below) is the reference's
-`--index_mode faiss` with host-resident rows and a product-quantized device index (csrc/pq.cu).
+`--index_mode faiss` with host-resident rows and a product-quantized (csrc/pq.cu) or 4-bit scalar-quantized
+(csrc/ivfsq.cu) device index.
 """
 import ctypes
 import logging
@@ -347,9 +348,16 @@ class DistributedFAISSIndex(DistributedIndex):
     before, which gives the exact top k of the union of the candidates.  The scores returned are then the exact inner
     products rounded once to fp16 (the flat index's scores up to the fp32 summation order), not PQ scores.  k' must
     not exceed MAX_TOPK.  No per-passage device memory is added; nothing is added to the index files.  `status` and the
-    exhaustive retry refer to the candidate search; the retry refines too.  R = 1 (default) runs the PQ search alone."""
+    exhaustive retry refer to the candidate search; the retry refines too.  R = 1 (default) runs the PQ search alone.
 
-    SUPPORTED_TYPES = ("pq", "ivfpq")
+    index_type "ivfsq" (faiss IndexIVFScalarQuantizer, QT_4bit, residual encoding): the ivfpq coarse quantizer, then each
+    residual dim in 4 bits between the per-dim min and max of the training residuals, scored by faiss's decode rule and
+    rounded once to fp16 (csrc/ivfsq.cu, include/atlas_b200.h).  `code_size` is bits per dimension (faiss's SQ4 naming):
+    None or 4.  The device holds 384 bytes of codes and a 4-byte row id per slot, in inverted-list order with every list
+    padded to a multiple of 64 slots; the index file holds the codes in row order and faiss's packing, with the list
+    ids, and `load_index` rebuilds the slot layout from them.  Training needs one row."""
+
+    SUPPORTED_TYPES = ("pq", "ivfpq", "ivfsq")
     FILE_FORMAT = 1
     TRAIN_SEED = 1234
     STAGE_ROWS = 65536
@@ -360,15 +368,24 @@ class DistributedFAISSIndex(DistributedIndex):
                 f"DistributedFAISSIndex: index_type={index_type!r} is not provided by atlas_b200; supported types are "
                 f"{', '.join(self.SUPPORTED_TYPES)}.  For exact search use --index_mode flat "
                 "(atlas_b200.index.DistributedIndex): flat and ivfflat with nprobe = n_list are exact anyway")
-        if code_size is None:
+        if index_type == "ivfsq":
+            # faiss's SQ4 naming: code_size is bits per dimension; the reference builds QT_4bit whatever its value
+            if code_size is not None and (isinstance(code_size, bool) or code_size != ops.SQ_BITS):
+                raise AtlasB200Error(f"DistributedFAISSIndex('ivfsq'): code_size={code_size!r} is bits per dimension and "
+                                     f"the scalar quantizer is {ops.SQ_BITS}-bit: pass None or {ops.SQ_BITS}.  For exact "
+                                     "search use --index_mode flat (atlas_b200.index.DistributedIndex)")
+        elif code_size is None:
             raise AtlasB200Error(f"DistributedFAISSIndex({index_type!r}) needs a code_size (--faiss_code_size)")
-        ops.pq_check_code_size(code_size)
+        else:
+            ops.pq_check_code_size(code_size)
         super().__init__()
         self._device()                 # no CUDA device: raise here, like the flat index (no CPU path)
         self.index_type = index_type
-        self.code_size = int(code_size)
+        self.code_size = None if code_size is None else int(code_size)
         self.is_in_gpu = False
-        self._pq = None                # dict(codebooks, coarse, codes, list_ids, n_list) of the trained index
+        # the trained index: dict(codebooks, coarse, codes, list_ids, n_list) for pq / ivfpq;
+        # dict(coarse, vmin, vdiff, codes, slot_rows, tile_lists, n_list) in the device slot layout for ivfsq
+        self._pq = None
         self.refine_factor = refine_factor
         self._refine_factor()
 
@@ -421,39 +438,74 @@ class DistributedFAISSIndex(DistributedIndex):
 
     def n_list(self, n_rows=None):
         n = self._bank.shape[0] if n_rows is None else n_rows
-        return int(math.floor(math.sqrt(n))) if self.index_type == "ivfpq" else 0
+        return int(math.floor(math.sqrt(n))) if self.index_type in ("ivfpq", "ivfsq") else 0
+
+    def _min_train_rows(self):
+        """faiss's k-means needs 256 points per PQ centroid; IVF-SQ needs one row per list, i.e. one row."""
+        return 1 if self.index_type == "ivfsq" else ops.PQ_KSUB
 
     def train_index(self):
         """Train the quantizers on the current rows and encode every row (src/index.py:352-381 trains + adds)."""
         if self._bank is None:
             raise AtlasB200Error("train_index before init_embeddings/load_index")
         n = self._bank.shape[0]
-        if n < ops.PQ_KSUB:
-            raise AtlasB200Error(f"train_index: {n} rows on this rank; product quantization needs at least "
-                                 f"{ops.PQ_KSUB} training points (faiss raises the same way)")
+        if n < self._min_train_rows():
+            raise AtlasB200Error(f"train_index: {n} rows on this rank; index type {self.index_type} needs at least "
+                                 f"{self._min_train_rows()} training points (faiss raises the same way)")
         self._pq = None
-        self._pq = self._train_and_encode(self._bank, n)
+        if self.index_type == "ivfsq":
+            self._pq = self._train_and_encode_sq(self._bank, n)
+        else:
+            self._pq = self._train_and_encode(self._bank, n)
 
-    def _train_and_encode(self, rows, n):
-        device = self._device()
-        n_list = self.n_list(n)
-        n_sample = min(n, max(ops.PQ_KSUB * ops.PQ_KSUB, ops.PQ_KSUB * n_list))
+    def _sample(self, rows, n, n_sample, device):
+        """The first n_sample rows of the seeded permutation, on the device."""
         perm = np.random.default_rng(self.TRAIN_SEED).permutation(n)[:n_sample]
-        sample = rows[torch.from_numpy(perm)].to(device)
-        codebooks, coarse = ops.pq_train(sample, self.code_size, n_list)
-        del sample
-        codes = torch.empty((n, self.code_size), dtype=torch.uint8, device=device)
-        list_ids = torch.empty(n, dtype=ops.pq_list_dtype(n_list), device=device) if n_list else None
-        ws = ops.Workspace()
+        return rows[torch.from_numpy(perm)].to(device)
+
+    def _stream_rows(self, rows, n, device, fn):
+        """fn(chunk, a, b) for the pinned host rows [a, b), staged through two device buffers of STAGE_ROWS rows."""
         width = min(self.STAGE_ROWS, n)
         stage = [torch.empty((width, EMBEDDINGS_DIM), dtype=torch.float16, device=device) for _ in range(2)]
         for it, a in enumerate(range(0, n, width)):
             b = min(n, a + width)
             st = stage[it & 1][: b - a]
             st.copy_(rows[a:b], non_blocking=True)       # pinned source; the stream orders the reuse of `st`
-            ops.pq_encode(st, codebooks, coarse, codes[a:b], list_ids[a:b] if n_list else None, ws)
+            fn(st, a, b)
         torch.cuda.current_stream(device).synchronize()
+
+    def _train_and_encode(self, rows, n):
+        device = self._device()
+        n_list = self.n_list(n)
+        sample = self._sample(rows, n, min(n, max(ops.PQ_KSUB * ops.PQ_KSUB, ops.PQ_KSUB * n_list)), device)
+        codebooks, coarse = ops.pq_train(sample, self.code_size, n_list)
+        del sample
+        codes = torch.empty((n, self.code_size), dtype=torch.uint8, device=device)
+        list_ids = torch.empty(n, dtype=ops.pq_list_dtype(n_list), device=device) if n_list else None
+        ws = ops.Workspace()
+        self._stream_rows(rows, n, device, lambda st, a, b: ops.pq_encode(st, codebooks, coarse, codes[a:b],
+                                                                          list_ids[a:b] if n_list else None, ws))
         return dict(codebooks=codebooks, coarse=coarse, codes=codes, list_ids=list_ids, n_list=n_list)
+
+    def _train_and_encode_sq(self, rows, n):
+        """IVF-SQ: coarse k-means and ranges on the seeded sample, then two passes over the rows: their lists (which
+        fix the slot layout), then their codes straight into their slots."""
+        device = self._device()
+        n_list = self.n_list(n)
+        sample = self._sample(rows, n, min(n, max(ops.SQ_RANGE_MAX, ops.PQ_KSUB * n_list)), device)
+        coarse, vmin, vdiff = ops.ivfsq_train(sample, n_list)
+        del sample
+        ws = ops.Workspace()
+        lists = torch.empty(n, dtype=torch.int32, device=device)
+        self._stream_rows(rows, n, device,
+                          lambda st, a, b: ops.ivfsq_encode(st, coarse, vmin, vdiff, list_ids=lists[a:b], workspace=ws))
+        slot_rows, tile_lists, row_slot = ops.ivfsq_layout(lists, n_list)
+        del lists
+        codes = torch.zeros((slot_rows.numel(), ops.SQ_CODE_BYTES), dtype=torch.uint8, device=device)
+        self._stream_rows(rows, n, device, lambda st, a, b: ops.ivfsq_encode(st, coarse, vmin, vdiff, row_slot=row_slot[a:b],
+                                                                             codes=codes, workspace=ws))
+        return dict(coarse=coarse, vmin=vmin, vdiff=vdiff, codes=codes, slot_rows=slot_rows, tile_lists=tile_lists,
+                    n_list=n_list)
 
     # ------------------------------------------------------------------ search
     def _trained(self):
@@ -482,6 +534,10 @@ class DistributedFAISSIndex(DistributedIndex):
     def _candidate_search(self, allqueries, k, id_base, id_stride, exhaustive):
         """Top k by PQ score: (scores, ids = id_base + id_stride * row, device status word)."""
         p = self._trained()
+        if self.index_type == "ivfsq":
+            return ops.ivfsq_topk(p["codes"], p["slot_rows"], p["tile_lists"], int(self._bank.shape[0]), p["coarse"],
+                                  p["vmin"], p["vdiff"], allqueries, k, id_base, id_stride, self._workspace,
+                                  exhaustive=exhaustive)
         return ops.pq_topk(p["codes"], p["list_ids"], p["codebooks"], p["coarse"], allqueries, k, id_base, id_stride,
                            self._workspace, exhaustive=exhaustive)
 
@@ -491,12 +547,17 @@ class DistributedFAISSIndex(DistributedIndex):
                                   self._workspace)
 
     # ------------------------------------------------------------------ persistence
+    def _index_file_stem(self) -> str:
+        """src/index.py:175-182: `index{type}_{code_size}_rank_{r}`, without the code size when it is None."""
+        size = f"_{self.code_size}" if self.code_size else ""
+        return f"index{self.index_type}{size}_rank_{dist_utils.get_rank()}"
+
     def _get_index_filename(self, path: str) -> str:
-        """src/index.py:175-183 names `index{type}_{code_size}_rank_{r}.faiss`; this format gets its own suffix."""
-        return os.path.join(path, f"index{self.index_type}_{self.code_size}_rank_{dist_utils.get_rank()}.atlas_b200.pt")
+        """The reference's `.faiss` name with this format's own suffix."""
+        return os.path.join(path, f"{self._index_file_stem()}.atlas_b200.pt")
 
     def _get_faiss_index_filename(self, path: str) -> str:
-        return os.path.join(path, f"index{self.index_type}_{self.code_size}_rank_{dist_utils.get_rank()}.faiss")
+        return os.path.join(path, f"{self._index_file_stem()}.faiss")
 
     def save_index(self, path: str, total_saved_shards: int, overwrite_saved_passages: bool = False) -> None:
         super().save_index(path, total_saved_shards, overwrite_saved_passages)
@@ -504,6 +565,13 @@ class DistributedFAISSIndex(DistributedIndex):
             return
         p = self._pq
         cpu = lambda t: None if t is None else t.cpu()
+        if self.index_type == "ivfsq":
+            codes, lists = ops.ivfsq_export(p["codes"], p["slot_rows"], p["tile_lists"], int(self._bank.shape[0]))
+            torch.save(dict(format=self.FILE_FORMAT, index_type=self.index_type, code_size=self.code_size,
+                            n_list=p["n_list"], n_rows=int(self._bank.shape[0]), coarse=cpu(p["coarse"]),
+                            vmin=cpu(p["vmin"]), vdiff=cpu(p["vdiff"]), codes=cpu(codes), list_ids=cpu(lists)),
+                       self._get_index_filename(path))
+            return
         torch.save(dict(format=self.FILE_FORMAT, index_type=self.index_type, code_size=self.code_size, n_list=p["n_list"],
                         n_rows=int(self._bank.shape[0]), codebooks=cpu(p["codebooks"]), coarse=cpu(p["coarse"]),
                         codes=cpu(p["codes"]), list_ids=cpu(p["list_ids"])),
@@ -522,6 +590,11 @@ class DistributedFAISSIndex(DistributedIndex):
                     and d.get("n_list") == self.n_list(n)):
                 dev = self._device()
                 to = lambda t: None if t is None else t.to(dev)
+                if self.index_type == "ivfsq":
+                    codes, slot_rows, tile_lists = ops.ivfsq_import(to(d["codes"]), to(d["list_ids"]), int(d["n_list"]))
+                    self._pq = dict(coarse=to(d["coarse"]), vmin=to(d["vmin"]), vdiff=to(d["vdiff"]), codes=codes,
+                                    slot_rows=slot_rows, tile_lists=tile_lists, n_list=int(d["n_list"]))
+                    return
                 self._pq = dict(codebooks=to(d["codebooks"]), coarse=to(d["coarse"]), codes=to(d["codes"]),
                                 list_ids=to(d["list_ids"]), n_list=int(d["n_list"]))
                 return
@@ -529,5 +602,5 @@ class DistributedFAISSIndex(DistributedIndex):
                         "retraining")
         elif os.path.exists(self._get_faiss_index_filename(path)):
             logger.info(f"{self._get_faiss_index_filename(path)} is a faiss file, which atlas_b200 does not read: retraining")
-        if n >= ops.PQ_KSUB:
+        if n >= self._min_train_rows():
             self.train_index()

@@ -279,6 +279,170 @@ def pq_refine_topk(rows_host, queries, cand_local, k, id_base=0, id_stride=1, wo
 
 
 # ---------------------------------------------------------------------------------------------
+# IVF-SQ index (csrc/pq.cu, csrc/ivfsq.cu)
+# ---------------------------------------------------------------------------------------------
+SQ_BITS = 4
+SQ_CODE_BYTES = DIM * SQ_BITS // 8
+SQ_TILE = 64                # slots per tile: every tile belongs to one inverted list
+SQ_RANGE_MAX = 100000       # faiss ScalarQuantizer::train_residual's subsample
+_SQ_CHUNK = 65536           # rows per step of the layout conversions
+
+
+def sq_nibble_of_dim():
+    """Nibble position (2 * byte + high) of every dim inside a device slot (csrc/ivfsq.cuh's permutation), int64 [768]."""
+    d = torch.arange(DIM)
+    kb, s, c = d // 64, (d % 64) // 16, d % 16
+    j, e, hi = (c % 8) // 2, c % 2, c // 8
+    byte = kb * 32 + j * 8 + (s // 2) * 4 + (s % 2) + 2 * e
+    return 2 * byte + hi
+
+
+def _sq_check_state(coarse, vmin, vdiff):
+    for name, t in (("coarse", coarse), ("vmin", vmin), ("vdiff", vdiff)):
+        require_cuda(t, name)
+        if t.dtype != torch.float32 or not t.is_contiguous():
+            raise AtlasB200Error(f"ivfsq: {name} must be contiguous fp32")
+    if coarse.dim() != 2 or coarse.shape[1] != DIM or coarse.shape[0] < 1 or vmin.shape != (DIM,) or vdiff.shape != (DIM,):
+        raise AtlasB200Error(f"ivfsq: coarse must be [n_list >= 1, {DIM}] and vmin / vdiff [{DIM}], got "
+                             f"{tuple(coarse.shape)}, {tuple(vmin.shape)}, {tuple(vdiff.shape)}")
+    return coarse.shape[0]
+
+
+def ivfsq_train(sample, n_list, iters=PQ_ITERS):
+    """Coarse k-means + per-dim residual ranges on the device (atlas_b200_ivfsq_train).  sample: CUDA fp16 [S, 768] in a
+    seeded random order, S >= n_list.  Returns (coarse fp32 [n_list, 768], vmin fp32 [768], vdiff fp32 [768])."""
+    require_cuda(sample, "sample")
+    s = sample.reshape(-1, DIM).to(torch.float16).contiguous()
+    if n_list < 1 or s.shape[0] < n_list:
+        raise AtlasB200Error(f"ivfsq_train: need 1 <= n_list <= sample rows (n_list={n_list}, rows={s.shape[0]})")
+    dev = s.device
+    coarse = torch.empty((n_list, DIM), dtype=torch.float32, device=dev)
+    vmin = torch.empty(DIM, dtype=torch.float32, device=dev)
+    vdiff = torch.empty(DIM, dtype=torch.float32, device=dev)
+    ws = torch.empty(int(lib().atlas_b200_ivfsq_workspace_bytes(PQ_OP_TRAIN, s.shape[0], n_list, 1)), dtype=torch.uint8,
+                     device=dev)
+    check(lib().atlas_b200_ivfsq_train(_ptr(s), s.shape[0], n_list, iters, _ptr(coarse), _ptr(vmin), _ptr(vdiff), _ptr(ws),
+                                       ws.numel(), current_stream_ptr()))
+    return coarse, vmin, vdiff
+
+
+def ivfsq_encode(rows, coarse, vmin, vdiff, list_ids=None, row_slot=None, codes=None, workspace=None):
+    """For CUDA fp16 rows [n, 768]: the coarse list of each row into `list_ids` (int32 [n]) and/or its 384 code bytes
+    into slot `row_slot[i]` (int32 [n]) of `codes` (uint8 [slots, 384], the device layout)."""
+    require_cuda(rows, "rows")
+    r = rows.reshape(-1, DIM)
+    if r.dtype != torch.float16 or not r.is_contiguous():
+        raise AtlasB200Error("ivfsq_encode: rows must be contiguous fp16 [n, 768]")
+    n_list = _sq_check_state(coarse, vmin, vdiff)
+    n = r.shape[0]
+    if list_ids is None and codes is None:
+        raise AtlasB200Error("ivfsq_encode: pass list_ids and/or codes")
+    if list_ids is not None and (list_ids.dtype != torch.int32 or list_ids.shape != (n,) or not list_ids.is_contiguous()):
+        raise AtlasB200Error(f"ivfsq_encode: list_ids must be contiguous int32 [{n}]")
+    if codes is not None:
+        if codes.dtype != torch.uint8 or codes.dim() != 2 or codes.shape[1] != SQ_CODE_BYTES or not codes.is_contiguous():
+            raise AtlasB200Error(f"ivfsq_encode: codes must be contiguous uint8 [slots, {SQ_CODE_BYTES}]")
+        if row_slot is None or row_slot.dtype != torch.int32 or row_slot.shape != (n,) or not row_slot.is_contiguous():
+            raise AtlasB200Error(f"ivfsq_encode: codes need row_slot, contiguous int32 [{n}]")
+    buf = (workspace or _default_ws).get(lib().atlas_b200_ivfsq_workspace_bytes(PQ_OP_ENCODE, n, n_list, 1), r.device)
+    check(lib().atlas_b200_ivfsq_encode(_ptr(r), n, _ptr(coarse), n_list, _ptr(vmin), _ptr(vdiff),
+                                        None if list_ids is None else _ptr(list_ids),
+                                        None if codes is None else _ptr(row_slot), None if codes is None else _ptr(codes),
+                                        _ptr(buf), buf.numel(), current_stream_ptr()))
+
+
+def ivfsq_layout(list_ids, n_list):
+    """The inverted-list slot layout of rows with list ids `list_ids` [n]: rows stable-sorted by list, each list padded
+    to a multiple of SQ_TILE slots.  Returns (slot_rows int32 [slots] (-1 = padding), tile_lists int32 [slots / 64],
+    row_slot int32 [n])."""
+    lists = list_ids.to(torch.int64)
+    dev, n = lists.device, lists.numel()
+    if n and (int(lists.min()) < 0 or int(lists.max()) >= n_list):
+        raise AtlasB200Error(f"ivfsq_layout: list ids must lie in [0, {n_list})")
+    counts = torch.bincount(lists, minlength=n_list)
+    padded = (counts + SQ_TILE - 1) // SQ_TILE * SQ_TILE
+    start = torch.cumsum(padded, 0) - padded
+    first = torch.cumsum(counts, 0) - counts
+    order = torch.sort(lists, stable=True).indices
+    ls = lists[order]
+    slot = start[ls] + torch.arange(n, device=dev) - first[ls]
+    n_slots = int(padded.sum())
+    slot_rows = torch.full((n_slots,), -1, dtype=torch.int32, device=dev)
+    slot_rows[slot] = order.to(torch.int32)
+    row_slot = torch.empty(n, dtype=torch.int32, device=dev)
+    row_slot[order] = slot.to(torch.int32)
+    tile_lists = torch.repeat_interleave(torch.arange(n_list, dtype=torch.int32, device=dev), padded // SQ_TILE)
+    return slot_rows, tile_lists, row_slot
+
+
+def ivfsq_export(codes, slot_rows, tile_lists, n_rows):
+    """Device layout -> row order: (codes uint8 [n_rows, 384] in faiss's packing - dim 2j in the low nibble of byte j,
+    dim 2j + 1 in the high one - and list ids int32 [n_rows])."""
+    dev = codes.device
+    perm = sq_nibble_of_dim().to(dev)
+    out = torch.empty((n_rows, SQ_CODE_BYTES), dtype=torch.uint8, device=dev)
+    lists = torch.empty(n_rows, dtype=torch.int32, device=dev)
+    slots = torch.nonzero(slot_rows >= 0).flatten()
+    if slots.numel() != n_rows:
+        raise AtlasB200Error(f"ivfsq_export: {slots.numel()} real slots for {n_rows} rows")
+    for a in range(0, n_rows, _SQ_CHUNK):
+        sl = slots[a:a + _SQ_CHUNK]
+        c = codes[sl]
+        nib = torch.stack([c & 15, c >> 4], dim=2).reshape(-1, 2 * SQ_CODE_BYTES)[:, perm]     # [rows, 768] by dim
+        rows = slot_rows[sl].to(torch.int64)
+        out[rows] = nib[:, 0::2] | (nib[:, 1::2] << 4)
+        lists[rows] = tile_lists[sl // SQ_TILE]
+    return out, lists
+
+
+def ivfsq_import(codes_rows, list_ids, n_list):
+    """Row order (ivfsq_export's format) -> device layout: (codes, slot_rows, tile_lists)."""
+    dev = codes_rows.device
+    n = codes_rows.shape[0]
+    if codes_rows.dtype != torch.uint8 or codes_rows.shape != (n, SQ_CODE_BYTES) or list_ids.shape != (n,):
+        raise AtlasB200Error(f"ivfsq_import: codes must be uint8 [n, {SQ_CODE_BYTES}] and list ids [n]")
+    slot_rows, tile_lists, row_slot = ivfsq_layout(list_ids, n_list)
+    perm = sq_nibble_of_dim().to(dev)
+    codes = torch.zeros((slot_rows.numel(), SQ_CODE_BYTES), dtype=torch.uint8, device=dev)
+    for a in range(0, n, _SQ_CHUNK):
+        c = codes_rows[a:a + _SQ_CHUNK]
+        by_dim = torch.stack([c & 15, c >> 4], dim=2).reshape(-1, DIM)
+        nib = torch.empty_like(by_dim)
+        nib[:, perm] = by_dim
+        codes[row_slot[a:a + _SQ_CHUNK].to(torch.int64)] = nib[:, 0::2] | (nib[:, 1::2] << 4)
+    return codes, slot_rows, tile_lists
+
+
+def ivfsq_topk(codes, slot_rows, tile_lists, n_rows, coarse, vmin, vdiff, queries, k, id_base=0, id_stride=1,
+               workspace=None, exhaustive=False):
+    """Top-k of the IVF-SQ scores of `queries` [nq, 768] over one shard's rows in the device layout
+    (atlas_b200_ivfsq_topk).  Returns (scores [nq, k] fp16 desc, ids [nq, k] int64, status int32[1]) like `mips_topk`."""
+    require_cuda(codes, "codes")
+    n_list = _sq_check_state(coarse, vmin, vdiff)
+    if codes.dtype != torch.uint8 or codes.dim() != 2 or codes.shape[1] != SQ_CODE_BYTES or not codes.is_contiguous() \
+            or codes.shape[0] % SQ_TILE or codes.data_ptr() % 16:
+        raise AtlasB200Error(f"ivfsq_topk: codes must be contiguous, 16-byte aligned uint8 [64 * tiles, {SQ_CODE_BYTES}]")
+    n_tiles = codes.shape[0] // SQ_TILE
+    if slot_rows.dtype != torch.int32 or slot_rows.shape != (codes.shape[0],) or tile_lists.dtype != torch.int32 \
+            or tile_lists.shape != (n_tiles,):
+        raise AtlasB200Error("ivfsq_topk: slot_rows must be int32 [slots] and tile_lists int32 [tiles]")
+    q = cast_queries(queries.reshape(-1, DIM).to(codes.device), torch.float16)
+    nq = q.shape[0]
+    buf = (workspace or _default_ws).get(lib().atlas_b200_ivfsq_workspace_bytes(PQ_OP_SEARCH, codes.shape[0], n_list, k),
+                                         codes.device)
+    out_s = torch.empty((nq, k), dtype=torch.float16, device=codes.device)
+    out_i = torch.empty((nq, k), dtype=torch.int64, device=codes.device)
+    status = torch.zeros(1, dtype=torch.int32, device=codes.device)
+    args = (_ptr(codes), _ptr(slot_rows.contiguous()), _ptr(tile_lists.contiguous()), n_tiles, n_rows, _ptr(coarse),
+            n_list, _ptr(vmin), _ptr(vdiff), _ptr(q), nq, k, _ptr(out_s), _ptr(out_i), id_base, id_stride)
+    if exhaustive:
+        check(lib().atlas_b200_ivfsq_topk_exhaustive(*args, _ptr(buf), buf.numel(), current_stream_ptr()))
+    else:
+        check(lib().atlas_b200_ivfsq_topk(*args, _ptr(status), _ptr(buf), buf.numel(), current_stream_ptr()))
+    return out_s, out_i, status
+
+
+# ---------------------------------------------------------------------------------------------
 # dense layers (csrc/gemm.cu)
 # ---------------------------------------------------------------------------------------------
 EPI_NONE, EPI_BIAS, EPI_GELU, EPI_RESIDUAL, EPI_GATED, EPI_RELU = 0, 1, 2, 3, 4, 5

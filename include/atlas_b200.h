@@ -139,6 +139,53 @@ int atlas_b200_pq_topk_exhaustive(const uint8_t* codes, const void* list_ids, in
                                   int32_t nq, int32_t k, void* out_scores, int64_t* out_ids, int64_t id_base,
                                   int64_t id_stride, void* workspace, size_t workspace_bytes, void* stream);
 
+/* --------------------------------------------------------------------------------------------
+ * IVF-SQ passage index (csrc/pq.cu, csrc/ivfsq.cu): `DistributedFAISSIndex` with index_type ivfsq (faiss
+ * IndexIVFScalarQuantizer with QT_4bit, residual encoding, inner product, nprobe = n_list).
+ *
+ *   n_list      coarse centroids (>= 1), coarse: device fp32 [n_list][768], trained as for ivfpq.
+ *   vmin/vdiff  device fp32 [768]: per-dim min and max - min of the residuals r = fp32(x) - coarse[list(x)].
+ *   layout      rows in inverted-list order: stable-sorted by list, every list padded to a multiple of 64 slots, so
+ *               each 64-slot tile belongs to one list.  codes: device uint8 [n_tiles * 64][384], 16-byte aligned,
+ *               nibbles permuted inside a slot (csrc/ivfsq.cuh); slot_rows: device int32 [n_tiles * 64], the local
+ *               row of each slot or -1 for padding; tile_lists: device int32 [n_tiles].
+ *   code        xi = (r_d - vmin_d) / vdiff_d (0 when vdiff_d == 0) clamped to [0, 1]; code_d = (int)(xi * 15.0) in
+ *               double, as faiss does.
+ *   score       w^[q][d] = fp16(2^e_q * q_d * (vdiff_d / 15)) with e_q putting max_d |w^| in [2^14, 2^15);
+ *               C[q] = sum_d q_d (vmin_d + 0.5 vdiff_d / 15) + 2^-e_q * 8 sum_d w^[q][d] and T[q][l] = <q, c_l>
+ *               in fp32;  s = fp16(T[q][list] + C[q] + 2^-e_q * sum_d w^[q][d] (code_d - 8)), the last sum accumulated
+ *               in fp32 on the tensor cores.
+ *               This is faiss's decode rule sum_d q_d (vmin_d + (code_d + 0.5) / 15 vdiff_d) + <q, c_l> to about one
+ *               fp16 ulp of the largest score.
+ *
+ * atlas_b200_ivfsq_train: `sample` [n_sample, 768] fp16 in a seeded random order, n_sample >= n_list: the coarse
+ *   k-means of atlas_b200_pq_train on the first min(n_sample, 256 n_list) rows, then vmin / vdiff over the residuals
+ *   of the first min(n_sample, 100000).  Bitwise deterministic.
+ * atlas_b200_ivfsq_encode: for n fp16 rows [n, 768] (call it chunk by chunk), the coarse assignment (inner product,
+ *   lowest list on ties) into list_ids (int32 [n], may be NULL) and, when `codes` is not NULL, each row's 384 code
+ *   bytes into slot row_slot[i] of `codes` (row_slot: int32 [n]).
+ * atlas_b200_ivfsq_topk / _exhaustive: atlas_b200_mips_topk's contract (fp16 scores desc, ids = id_base + id_stride *
+ *   row, canonical tie order, `status` overflow flag and the exhaustive retry) over the n_rows real rows; padding
+ *   slots are never returned.  k <= n_rows.
+ * Workspace: atlas_b200_ivfsq_workspace_bytes(op, n, n_list, k) with op ATLAS_B200_PQ_OP_TRAIN (n = n_sample),
+ *   _ENCODE (n unused) or _SEARCH (n = n_tiles * 64); 0 when n_list < 1.
+ * -------------------------------------------------------------------------------------------- */
+size_t atlas_b200_ivfsq_workspace_bytes(int32_t op, int64_t n, int32_t n_list, int32_t k);
+int atlas_b200_ivfsq_train(const void* sample, int64_t n_sample, int32_t n_list, int32_t iters, float* coarse, float* vmin,
+                           float* vdiff, void* workspace, size_t workspace_bytes, void* stream);
+int atlas_b200_ivfsq_encode(const void* rows, int64_t n, const float* coarse, int32_t n_list, const float* vmin,
+                            const float* vdiff, int32_t* list_ids, const int32_t* row_slot, uint8_t* codes, void* workspace,
+                            size_t workspace_bytes, void* stream);
+int atlas_b200_ivfsq_topk(const uint8_t* codes, const int32_t* slot_rows, const int32_t* tile_lists, int64_t n_tiles,
+                          int64_t n_rows, const float* coarse, int32_t n_list, const float* vmin, const float* vdiff,
+                          const void* queries, int32_t nq, int32_t k, void* out_scores, int64_t* out_ids, int64_t id_base,
+                          int64_t id_stride, int32_t* status, void* workspace, size_t workspace_bytes, void* stream);
+int atlas_b200_ivfsq_topk_exhaustive(const uint8_t* codes, const int32_t* slot_rows, const int32_t* tile_lists,
+                                     int64_t n_tiles, int64_t n_rows, const float* coarse, int32_t n_list, const float* vmin,
+                                     const float* vdiff, const void* queries, int32_t nq, int32_t k, void* out_scores,
+                                     int64_t* out_ids, int64_t id_base, int64_t id_stride, void* workspace,
+                                     size_t workspace_bytes, void* stream);
+
 /* Exact re-ranking of PQ search candidates (csrc/pq_refine.cu; faiss IndexRefineFlat, `k_factor`): for every query,
  * the k_cand candidate rows are re-scored against their full-precision rows and the top k are returned.
  *   rows_host   PINNED host memory, [n, 768] fp16 row-major, 16-byte aligned.  Read zero-copy by the kernel through
@@ -596,7 +643,8 @@ int atlas_b200_expand_packed_tiles(const void* src, int64_t lds, const int32_t* 
 
 /* Measurement hook for bench.py's roofline: while enabled, every launch of ONE kind of kernel is bracketed
  * with CUDA events on its launching stream:
- *   kind 1  the bank sweep of atlas_b200_mips_topk (work = algorithmic bytes swept)
+ *   kind 1  the bank sweep of atlas_b200_mips_topk (work = algorithmic bytes swept); also the code sweep of
+ *           atlas_b200_ivfsq_topk (work = code bytes swept, once per 128 queries of a block)
  *   kind 2  the wgmma GEMM of atlas_b200_linear_rows (work = 2*M*N*K FLOPs over the computed rows)
  *   kind 3  the attention forward kernels: atlas_b200_attention_train / _long / _packed, the cross-attention stream
  *           kernels (work = 4*B*H*Lq*Lk*64 FLOPs)

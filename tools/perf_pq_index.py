@@ -5,12 +5,17 @@ of bench.py (4 Mi passages of 768-d fp16 per GPU, BASELINE configs[1]).  Prints 
   flat                        the exact flat scan (ops.mips_topk) on the same bank, same timing
   sweep                       code bytes per search (computed from shapes) over the main code-sweep kernel time, against the
                               HBM peak
-  device_bytes_per_passage    codes + list ids + codebooks + coarse centroids, over the rows
+  device_bytes_per_passage    every device tensor of the trained index (codes, list ids or slot rows, codebooks or
+                              ranges, coarse centroids), over the rows
   recall_at_40                against the exact flat search, on a synthetic Gaussian bank: says little about real embeddings
   refine                      with --refine-factor R > 1 only: the same search re-ranked by exact score over the top
                               k' = 40 R PQ candidates (refine_factor = R): queries/s, recall_at_40 refined vs unrefined, the
                               refine kernel's time and the host-row bytes it reads per search (nq k' 1536, from shapes) over
                               that time
+  at_8_queries                the same search, and the flat scan, at 8 queries per search (bench.py's per-rank batch)
+  ivfsq                       with --index-type ivfsq only: each sweep's kernel time (256 and 8 queries) against the larger of its two bounds from shapes: the
+                              code bytes over the HBM peak, and 2 x 768 x slots x queries FLOPs over the dense fp16
+                              tensor peak (the tensor bound binds at 256 queries, HBM at 8)
     python tools/perf_pq_index.py [--index-type ivfpq] [--code-size 16] [--rows N] [--steps 20] [--warmup 3]
                                   [--refine-factor 1]
 Writes nothing."""
@@ -38,7 +43,8 @@ def measure(args):
     dev = torch.device("cuda", 0)
     torch.cuda.set_device(dev)
     L = lib()
-    rows, M = args.rows, args.code_size
+    rows = args.rows
+    M = None if args.index_type == "ivfsq" else args.code_size
     steps, warmup = args.steps, args.warmup
     bank = make_bank(rows, dev, seed=1)
     q = make_queries().to(dev)
@@ -55,6 +61,7 @@ def measure(args):
         return e0.elapsed_time(e1) / steps, out
 
     flat_ms, (_, exact, st) = timed(lambda: ops.mips_topk(bank, q, TOPK))
+    flat8_ms, _ = timed(lambda: ops.mips_topk(bank, q[:8], TOPK))
     assert int(st.item()) == 0
     exact = exact.cpu().numpy()
     index = DistributedFAISSIndex(args.index_type, M)
@@ -68,23 +75,48 @@ def measure(args):
     torch.cuda.synchronize()
     train_s = time.perf_counter() - t0
     p = index._pq
-    dev_bytes = sum(t.numel() * t.element_size() for t in (p["codes"], p["list_ids"], p["codebooks"], p["coarse"])
-                    if t is not None)
-    L.atlas_b200_profile_enable(1)
-    ms, (_, ids, st) = timed(lambda: index.search_device(q, TOPK, return_status=True))
-    kms, kn = ctypes.c_double(0), ctypes.c_int32(0)
-    L.atlas_b200_profile_collect(ctypes.byref(kms), ctypes.byref(kn))
-    L.atlas_b200_profile_enable(0)
+    dev_bytes = sum(t.numel() * t.element_size() for t in p.values() if torch.is_tensor(t))
+
+    def profiled(queries):
+        L.atlas_b200_profile_enable(1)
+        ms, out = timed(lambda: index.search_device(queries, TOPK, return_status=True))
+        kms, kn = ctypes.c_double(0), ctypes.c_int32(0)
+        L.atlas_b200_profile_collect(ctypes.byref(kms), ctypes.byref(kn))
+        L.atlas_b200_profile_enable(0)
+        return ms, out, kms, kn
+
+    ms, (_, ids, st), kms, kn = profiled(q)
     assert int(st.item()) == 0, "fast search path overflowed"
     ids = ids.cpu().numpy()
-    recall_of = lambda ids: float(sum(len(set(a) & set(b)) for a, b in zip(ids.tolist(), exact.tolist())) / (NQ * TOPK))
+    recall_of = lambda ids, nq=NQ: float(sum(len(set(a) & set(b)) for a, b in zip(ids.tolist(), exact[:nq].tolist()))
+                                         / (nq * TOPK))
     recall = recall_of(ids)
-    list_bytes = 0 if p["list_ids"] is None else p["list_ids"].element_size()
+    list_bytes = 0 if p.get("list_ids") is None else p["list_ids"].element_size()
     groups = kn.value // (steps + warmup) if kn.value else 0
     kernel_ms = kms.value / (steps + warmup)
-    sweep_bytes = rows * (M + list_bytes)
+    sweep_bytes = rows * (M + list_bytes) if M else p["codes"].numel()
     peak, peak_src = peaks("hbm")
     achieved = sweep_bytes / (kernel_ms * 1e-3) / 1e9 if kernel_ms > 0 else 0.0
+    ms8, (_, ids8, st8), kms8, _ = profiled(q[:8])
+    assert int(st8.item()) == 0, "fast search path overflowed"
+    recall8 = recall_of(ids8.cpu().numpy(), 8)
+    ivfsq = None
+    if args.index_type == "ivfsq":
+        slots = p["codes"].shape[0]
+        tflops, tensor_src = 989.0, "H100 SXM data sheet, dense fp16"
+
+        def bounds(nq, kernel_ms):
+            hbm_ms = slots * ops.SQ_CODE_BYTES / (peak * 1e9) * 1e3
+            tensor_ms = 2.0 * DIM * slots * nq / (tflops * 1e12) * 1e3
+            bound_ms = max(hbm_ms, tensor_ms)
+            return {"queries": nq, "kernel_ms_per_search": kernel_ms, "hbm_bound_ms": hbm_ms, "tensor_bound_ms": tensor_ms,
+                    "binding": "hbm" if hbm_ms >= tensor_ms else "tensor",
+                    "frac_of_binding_bound": bound_ms / kernel_ms if kernel_ms > 0 else None}
+
+        ivfsq = {"slots": slots, "padding_frac": slots / rows - 1.0, "tensor_peak_tflops": tflops,
+                 "tensor_peak_source": tensor_src,
+                 "at_256": {"value": NQ / (ms * 1e-3), "unit": "queries/s", "ms_per_search": ms} | bounds(NQ, kernel_ms),
+                 "at_8": bounds(8, kms8.value / (steps + warmup))}
     refine = None
     if args.refine_factor > 1:
         index.refine_factor = args.refine_factor
@@ -112,24 +144,27 @@ def measure(args):
         "metric": f"{args.index_type} index search queries/sec (top-{TOPK}, {NQ}-query batches, code_size {M})",
         "value": NQ / (ms * 1e-3), "unit": "queries/s", "ms_per_search": ms, "steps": steps, "rows": rows,
         "index_type": args.index_type, "code_size": M, "n_list": p["n_list"], "train_index_s": train_s,
+        "at_8_queries": {"value": 8 / (ms8 * 1e-3), "unit": "queries/s", "ms_per_search": ms8, "recall_at_40": recall8,
+                         "flat_value": 8 / (flat8_ms * 1e-3), "flat_ms_per_search": flat8_ms},
         "flat": {"value": NQ / (flat_ms * 1e-3), "unit": "queries/s", "ms_per_search": flat_ms,
                  "call": "ops.mips_topk (exact fp16 bank scan, device-resident bank)"},
         "sweep": {"bound": "hbm", "achieved": achieved, "peak": peak, "unit": "GB/s",
                   "frac": achieved / peak if peak else None, "peak_source": peak_src,
-                  "kernel": "pq_scan_kernel (main sweep; codes re-read once per query group, so real traffic is higher)",
+                  "kernel": "ivfsq_scan_kernel (main sweep; codes read once per 128 queries)" if M is None else
+                            "pq_scan_kernel (main sweep; codes re-read once per query group, so real traffic is higher)",
                   "kernel_ms_per_search": kernel_ms, "kernel_launches_per_search": groups,
                   "code_bytes_per_search": sweep_bytes},
         "device_bytes_per_passage": dev_bytes / rows, "flat_device_bytes_per_passage": DIM * 2,
         "recall_at_40": recall, "recall_note": "against the exact flat search on a synthetic Gaussian bank; not "
                                                "representative of real embeddings",
         "gpu": smi,
-    } | ({"refine": refine} if refine else {})
+    } | ({"refine": refine} if refine else {}) | ({"ivfsq": ivfsq} if ivfsq else {})
 
 
 def main():
     ap = argparse.ArgumentParser()
-    ap.add_argument("--index-type", choices=["pq", "ivfpq"], default="ivfpq")
-    ap.add_argument("--code-size", type=int, default=16, help="bytes of PQ code per passage")
+    ap.add_argument("--index-type", choices=["pq", "ivfpq", "ivfsq"], default="ivfpq")
+    ap.add_argument("--code-size", type=int, default=16, help="bytes of PQ code per passage (ivfsq: always 4 bits per dim)")
     ap.add_argument("--rows", type=int, default=N_LOCAL)
     ap.add_argument("--steps", type=int, default=20)
     ap.add_argument("--warmup", type=int, default=3)
