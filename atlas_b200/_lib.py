@@ -186,6 +186,12 @@ def lib():
     L.atlas_b200_pq_topk_exhaustive.restype = c.c_int
     L.atlas_b200_pq_topk_exhaustive.argtypes = [vp, vp, i64, i32, vp, vp, i32, vp, i32, i32, vp, vp, i64, i64, vp, c.c_size_t,
                                                 vp]
+    L.atlas_b200_pq_topk_probed.restype = c.c_int
+    L.atlas_b200_pq_topk_probed.argtypes = [vp, vp, i64, i32, vp, vp, i32, vp, vp, i32, vp, i32, i32, vp, vp, i64, i64, vp, vp,
+                                            c.c_size_t, vp]
+    L.atlas_b200_pq_topk_probed_exhaustive.restype = c.c_int
+    L.atlas_b200_pq_topk_probed_exhaustive.argtypes = [vp, vp, i64, i32, vp, vp, i32, vp, vp, i32, vp, i32, i32, vp, vp, i64,
+                                                       i64, vp, c.c_size_t, vp]
     L.atlas_b200_ivfsq_workspace_bytes.restype = c.c_size_t
     L.atlas_b200_ivfsq_workspace_bytes.argtypes = [i32, i64, i32, i32]
     L.atlas_b200_ivfsq_train.restype = c.c_int
@@ -198,6 +204,12 @@ def lib():
     L.atlas_b200_ivfsq_topk_exhaustive.restype = c.c_int
     L.atlas_b200_ivfsq_topk_exhaustive.argtypes = [vp, vp, vp, i64, i64, vp, i32, vp, vp, vp, i32, i32, vp, vp, i64, i64, vp,
                                                    c.c_size_t, vp]
+    L.atlas_b200_ivfsq_topk_probed.restype = c.c_int
+    L.atlas_b200_ivfsq_topk_probed.argtypes = [vp, vp, vp, i64, i64, vp, vp, vp, i32, vp, vp, i32, vp, i32, i32, vp, vp, i64,
+                                               i64, vp, vp, c.c_size_t, vp]
+    L.atlas_b200_ivfsq_topk_probed_exhaustive.restype = c.c_int
+    L.atlas_b200_ivfsq_topk_probed_exhaustive.argtypes = [vp, vp, vp, i64, i64, vp, vp, vp, i32, vp, vp, i32, vp, i32, i32,
+                                                          vp, vp, i64, i64, vp, c.c_size_t, vp]
     L.atlas_b200_pq_refine_workspace_bytes.restype = c.c_size_t
     L.atlas_b200_pq_refine_workspace_bytes.argtypes = [i32, i32]
     L.atlas_b200_pq_refine_topk.restype = c.c_int
@@ -268,11 +280,15 @@ EXPORTED_SYMBOLS = [
     "atlas_b200_pq_encode",
     "atlas_b200_pq_topk",
     "atlas_b200_pq_topk_exhaustive",
+    "atlas_b200_pq_topk_probed",
+    "atlas_b200_pq_topk_probed_exhaustive",
     "atlas_b200_ivfsq_workspace_bytes",
     "atlas_b200_ivfsq_train",
     "atlas_b200_ivfsq_encode",
     "atlas_b200_ivfsq_topk",
     "atlas_b200_ivfsq_topk_exhaustive",
+    "atlas_b200_ivfsq_topk_probed",
+    "atlas_b200_ivfsq_topk_probed_exhaustive",
     "atlas_b200_pq_refine_workspace_bytes",
     "atlas_b200_pq_refine_topk",
     "atlas_b200_quantize_kv_e4m3",

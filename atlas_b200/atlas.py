@@ -27,6 +27,7 @@ from torch import nn
 
 from . import dist_utils, token_cache
 from ._lib import AtlasB200Error
+from .index import DistributedFAISSIndex
 from .retrievers import EMBEDDINGS_DIM
 
 IGNORE_INDEX: int = -100
@@ -198,6 +199,9 @@ class Atlas(nn.Module):
         if refine is not None and hasattr(index, "refine_factor"):
             # --index_mode faiss: re-rank refine * topk PQ candidates per rank by exact score (the flat index is exact)
             index.refine_factor = int(refine)
+        if isinstance(index, DistributedFAISSIndex):
+            # --index_mode faiss: score each query against its best faiss_nprobe inverted lists only (None: every list)
+            index.nprobe = getattr(self.opt, "faiss_nprobe", None)
         if filtering_fun is not None:
             passages, scores = index.search_knn(query_emb, topk * self.opt.filtering_overretrieve_ratio)
             passages, scores = filtering_fun(batch_metadata, passages, scores, topk, training=self.training)

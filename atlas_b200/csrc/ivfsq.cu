@@ -19,6 +19,7 @@
 // codes are then read once per 128 queries.
 #include "common.cuh"
 #include "host_common.h"
+#include "ivf_probe.cuh"
 #include "ivfsq.cuh"
 #include "mips_select.cuh"
 #include "wgmma.cuh"
@@ -68,9 +69,13 @@ __device__ __forceinline__ void mma_step(float (&acc)[NQ / 2], const uint32_t (&
     else ab::wgmma_m64n128k16_rs_f16<0>(acc, a, bdesc, scale_d);
 }
 
-template <int NQ>
+// PROBED: the tiles come from the compacted items (ivf_probe.cuh); a step whose two items no query of this CTA's group
+// probes is skipped.  The producer and both consumers derive the same item sequence from the same count (read once,
+// before the loop) and the same probe bits, so the mbarrier ring stays in step.
+template <int NQ, bool PROBED>
 __global__ void __launch_bounds__(NUM_THREADS, 1)
-ivfsq_scan_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ CUtensorMap tmap_c, const ScanParams p) {
+ivfsq_scan_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ CUtensorMap tmap_c, const ScanParams p,
+                  const ProbeScan pr) {
     constexpr int STAGES = stages<NQ>();
     static_assert(STAGES >= 4, "");
     extern __shared__ uint8_t smem_raw[];
@@ -87,7 +92,17 @@ ivfsq_scan_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_const
 
     const int q0 = blockIdx.y * NQ;
     const int nqg = min(NQ, p.nq - q0);
-    const int steps = (p.num_tiles + CONSUMERS - 1) / CONSUMERS;
+    int pbegin = 0, pstep = 1, pnum = 0;
+    if constexpr (PROBED) ivfp::resolve_items(*pr.item_count, p.tile_begin, p.tile_step, p.num_tiles, pbegin, pstep, pnum);
+    const int steps = ((PROBED ? pnum : p.num_tiles) + CONSUMERS - 1) / CONSUMERS;
+    // PROBED: item i of this launch, its tile and list, and whether this CTA's queries need it
+    auto probed_item = [&](int i, int& tile, int& list) -> bool {
+        if (i >= pnum) return false;
+        const int2 it = pr.items[pbegin + i * pstep];
+        list = it.x;
+        tile = it.y;
+        return ivfp::group_probes(pr.probed, list, q0, nqg);
+    };
 
     if (threadIdx.x == 0) {
         ab::tma_prefetch_desc(&tmap_q);
@@ -115,6 +130,28 @@ ivfsq_scan_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_const
                 ab::tma_load_2d(&tmap_q, &q_bar, smem_gen + kb * Q_KB_BYTES, kb * 64, q0, ab::kEvictLast);
             uint32_t stage = 0, phase = 0;
             for (int g = blockIdx.x; g < steps; g += gridDim.x) {
+                if constexpr (PROBED) {
+                    int tile[CONSUMERS], list[CONSUMERS], ntile = 0;
+                    bool has[CONSUMERS];
+                    for (int c = 0; c < CONSUMERS; ++c)
+                        ntile += (has[c] = probed_item(g * CONSUMERS + c, tile[c], list[c])) ? 1 : 0;
+                    if (ntile == 0) continue;
+                    for (int kb = 0; kb < K_BLOCKS; ++kb) {
+                        ab::mbar_wait_nocall(&empty_bar[stage], phase ^ 1u);
+                        ab::mbar_arrive_expect_tx(&full_bar[stage], static_cast<uint32_t>(ntile * TILE_KB_BYTES));
+                        for (int c = 0; c < CONSUMERS; ++c) {
+                            if (!has[c]) continue;
+                            ab::tma_load_2d(&tmap_c, &full_bar[stage], smem_gen + K_BLOCKS * Q_KB_BYTES +
+                                            stage * STAGE_BYTES + c * TILE_KB_BYTES, kb * SQ_KBLOCK_BYTES, tile[c] * SQ_TILE,
+                                            ab::kEvictFirst);
+                        }
+                        if (++stage == STAGES) {
+                            stage = 0;
+                            phase ^= 1u;
+                        }
+                    }
+                    continue;
+                }
                 const int ntile = min(CONSUMERS, p.num_tiles - g * CONSUMERS);
                 for (int kb = 0; kb < K_BLOCKS; ++kb) {
                     ab::mbar_wait_nocall(&empty_bar[stage], phase ^ 1u);
@@ -142,9 +179,17 @@ ivfsq_scan_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_const
     ab::mbar_wait_nocall(&q_bar, 0);
     uint32_t stage = 0, phase = 0;
     for (int g = blockIdx.x; g < steps; g += gridDim.x) {
-        const int item = g * CONSUMERS + cw;
-        const bool has = item < p.num_tiles;
-        const int tile = p.tile_begin + item * p.tile_step;
+        int tile, my_list = 0;
+        bool has;
+        if constexpr (PROBED) {
+            has = probed_item(g * CONSUMERS + cw, tile, my_list);
+            int other_tile, other_list;
+            if (!has && !probed_item(g * CONSUMERS + (1 - cw), other_tile, other_list)) continue;   // the producer skips it too
+        } else {
+            const int item = g * CONSUMERS + cw;
+            has = item < p.num_tiles;
+            tile = p.tile_begin + item * p.tile_step;
+        }
         float acc[NQ / 2];
 #pragma unroll 1
         for (int kb = 0; kb < K_BLOCKS; ++kb) {
@@ -189,7 +234,7 @@ ivfsq_scan_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_const
         if (!has) continue;
 
         // epilogue: acc[4 j + 2 e + c] = (slot frag_row + 8 e, query 8 j + 2 quad + c)
-        const int list = p.tile_lists[tile];
+        const int list = PROBED ? my_list : p.tile_lists[tile];
         const float* trow = p.tterm + static_cast<int64_t>(list) * p.ldt + q0;
         int row[2];
 #pragma unroll
@@ -203,10 +248,11 @@ ivfsq_scan_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_const
                 float v[2] = {0.f, 0.f};
                 if (q < nqg) {
                     const float base = trow[q] + s_c[q];
+                    const bool probed = !PROBED || ivfp::probes(pr.probed, list, q0 + q);
 #pragma unroll
                     for (int e = 0; e < 2; ++e) {
                         v[e] = fmaf(acc[4 * j + 2 * e + c], s_scale[q], base);
-                        pass[e] = row[e] >= 0 && v[e] >= s_bnd[q];
+                        pass[e] = row[e] >= 0 && probed && v[e] >= s_bnd[q];
                     }
                 }
                 const uint32_t np = (pass[0] ? 1u : 0u) + (pass[1] ? 1u : 0u);
@@ -237,11 +283,11 @@ ivfsq_scan_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_const
     }
 }
 
-template <int NQ>
-static int launch_nq(const CUtensorMap& tq, const CUtensorMap& tc, const ScanParams& p, cudaStream_t s) {
+template <int NQ, bool PROBED>
+static int launch_nq(const CUtensorMap& tq, const CUtensorMap& tc, const ScanParams& p, const ProbeScan& pr, cudaStream_t s) {
     static bool attr_set = false;
     if (!attr_set) {
-        AB_CUDA_CHECK(cudaFuncSetAttribute(ivfsq_scan_kernel<NQ>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+        AB_CUDA_CHECK(cudaFuncSetAttribute(ivfsq_scan_kernel<NQ, PROBED>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                            smem_bytes<NQ>()));
         attr_set = true;
     }
@@ -250,13 +296,25 @@ static int launch_nq(const CUtensorMap& tq, const CUtensorMap& tc, const ScanPar
     int gx = abh::num_sms() / groups;
     if (gx > steps) gx = steps;
     if (gx < 1) gx = 1;
-    ivfsq_scan_kernel<NQ><<<dim3(gx, groups), NUM_THREADS, smem_bytes<NQ>(), s>>>(tq, tc, p);
+    ivfsq_scan_kernel<NQ, PROBED><<<dim3(gx, groups), NUM_THREADS, smem_bytes<NQ>(), s>>>(tq, tc, p, pr);
     abh::count_launch();
     AB_CUDA_CHECK(cudaGetLastError());
     return ATLAS_B200_OK;
 }
 
-int launch_scan(const ScanParams& p, cudaStream_t s) {
+template <bool PROBED>
+static int launch_cols(int nq_cols, const CUtensorMap& tq, const CUtensorMap& tc, const ScanParams& p, const ProbeScan& pr,
+                       cudaStream_t s) {
+    switch (nq_cols) {
+        case 8: return launch_nq<8, PROBED>(tq, tc, p, pr, s);
+        case 16: return launch_nq<16, PROBED>(tq, tc, p, pr, s);
+        case 32: return launch_nq<32, PROBED>(tq, tc, p, pr, s);
+        case 64: return launch_nq<64, PROBED>(tq, tc, p, pr, s);
+        default: return launch_nq<128, PROBED>(tq, tc, p, pr, s);
+    }
+}
+
+int launch_scan(const ScanParams& p, const ProbeScan* probe, cudaStream_t s) {
     if (p.num_tiles <= 0 || p.nq <= 0) return ATLAS_B200_OK;
     // query columns per CTA: the block's query count rounded up to a power of two >= 8, at most 128
     int nq_cols = 8;
@@ -267,13 +325,7 @@ int launch_scan(const ScanParams& p, cudaStream_t s) {
     rc = abh::make_tmap_2d_bytes(&tc, p.codes, static_cast<uint64_t>(p.n_tiles) * SQ_TILE, SQ_CODE_BYTES, SQ_CODE_BYTES,
                                  SQ_TILE, SQ_KBLOCK_BYTES);
     if (rc) return rc;
-    switch (nq_cols) {
-        case 8: return launch_nq<8>(tq, tc, p, s);
-        case 16: return launch_nq<16>(tq, tc, p, s);
-        case 32: return launch_nq<32>(tq, tc, p, s);
-        case 64: return launch_nq<64>(tq, tc, p, s);
-        default: return launch_nq<128>(tq, tc, p, s);
-    }
+    return probe ? launch_cols<true>(nq_cols, tq, tc, p, *probe, s) : launch_cols<false>(nq_cols, tq, tc, p, ProbeScan{}, s);
 }
 
 }  // namespace ivfsq

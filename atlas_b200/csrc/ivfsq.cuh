@@ -60,8 +60,17 @@ struct ScanParams {
     uint32_t capq;
 };
 
+// A probed scan's state (a separate kernel argument: the full scan's parameters stay as they are)
+struct ProbeScan {
+    const int2* items;           // the block's compacted (list, tile) items and their count in device memory
+    const int32_t* item_count;
+    const uint32_t* probed;      // [n_list][PROBE_WORDS] probe bits of the block's queries
+};
+
 // Scans tiles tile_begin + i * tile_step, i < num_tiles, for every query of the block; appends (fp16 key, row) of every
 // real slot whose score is >= bound[q] to the query's candidate list.
-int launch_scan(const ScanParams& p, cudaStream_t s);
+// probe != NULL: the tiles are those of probe->items (ivf_probe.cuh's resolve_items over *item_count), and a slot is
+// appended for query q only when q probes the tile's list; num_tiles is then the host's upper bound of the item count.
+int launch_scan(const ScanParams& p, const ProbeScan* probe, cudaStream_t s);
 
 }  // namespace ivfsq

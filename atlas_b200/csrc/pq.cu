@@ -23,6 +23,7 @@
 //
 // The IVF-SQ index (type ivfsq) shares the coarse k-means, the coarse assignment and the top-k driver: its training,
 // encoding and search host code are at the end of this file, its scan kernel in ivfsq.cu.
+#include "ivf_probe.cuh"
 #include "ivfsq.cuh"
 #include "mips_select.cuh"
 
@@ -314,8 +315,22 @@ struct ScanParams {
     uint32_t capq;
 };
 
-template <int QPC>
-__global__ void __launch_bounds__(SCAN_THREADS) pq_scan_kernel(const ScanParams p) {
+// A probed scan's state (a separate kernel argument: the full scan's parameters stay as they are)
+struct ProbeScan {
+    const int2* items;             // (list, first list position) chunks of PROBE_CHUNK positions, and their count
+    const int32_t* item_count;
+    const int32_t* list_order;     // rows in list order (stable) and each list's first position [n_list + 1]
+    const int32_t* list_offsets;
+    const uint32_t* probed;        // [n_list][PROBE_WORDS] probe bits of the block's queries
+};
+
+constexpr int PROBE_CHUNK = SCAN_THREADS;   // list positions per work item of a probed scan: one per thread
+
+// PROBED: a work item is one chunk of one list (ivf_probe.cuh), so the list, its coarse terms and the probe bits of the
+// CTA's queries are known once per item; an item none of them probes is skipped, and a row is appended for query q only
+// when q probes its list.
+template <int QPC, bool PROBED>
+__global__ void __launch_bounds__(SCAN_THREADS) pq_scan_kernel(const ScanParams p, const ProbeScan pr) {
     extern __shared__ float s_tab[];
     __shared__ float s_bnd[QPC];
     const int t = threadIdx.x, lane = t & 31;
@@ -329,11 +344,23 @@ __global__ void __launch_bounds__(SCAN_THREADS) pq_scan_kernel(const ScanParams 
         for (int e = t; e < nqg * p.n_list; e += SCAN_THREADS) s_ct[e] = p.cterm[static_cast<int64_t>(q0) * p.n_list + e];
     if (t < QPC) s_bnd[t] = t < nqg ? p.bound[q0 + t] : INFINITY;
     __syncthreads();
+    int begin = p.tile_begin, step = p.tile_step, num = p.num_tiles;
+    if constexpr (PROBED) ivfp::resolve_items(*pr.item_count, p.tile_begin, p.tile_step, p.num_tiles, begin, step, num);
 
-    for (int it = blockIdx.x; it < p.num_tiles; it += gridDim.x) {
-        const int tile = p.tile_begin + it * p.tile_step;
-        const int row = tile * SCAN_THREADS + t;
-        const bool live = row < p.n_rows;
+    for (int it = blockIdx.x; it < num; it += gridDim.x) {
+        int row, l = 0;
+        bool live;
+        if constexpr (PROBED) {
+            const int2 item = pr.items[begin + it * step];
+            l = item.x;
+            if (!ivfp::group_probes(pr.probed, l, q0, nqg)) continue;
+            const int pos = item.y + t;
+            live = pos < __ldg(pr.list_offsets + l + 1);
+            row = live ? __ldg(pr.list_order + pos) : 0;
+        } else {
+            row = (begin + it * step) * SCAN_THREADS + t;
+            live = row < p.n_rows;
+        }
         float acc[QPC];
 #pragma unroll
         for (int q = 0; q < QPC; ++q) acc[q] = 0.f;
@@ -358,8 +385,9 @@ __global__ void __launch_bounds__(SCAN_THREADS) pq_scan_kernel(const ScanParams 
                 }
             }
             if (p.cterm) {
-                const int l = p.list_u16 ? static_cast<int>(static_cast<const uint16_t*>(p.lists)[row])
-                                         : static_cast<const int32_t*>(p.lists)[row];
+                if constexpr (!PROBED)
+                    l = p.list_u16 ? static_cast<int>(static_cast<const uint16_t*>(p.lists)[row])
+                                   : static_cast<const int32_t*>(p.lists)[row];
 #pragma unroll
                 for (int q = 0; q < QPC; ++q)
                     if (q < nqg)
@@ -370,7 +398,7 @@ __global__ void __launch_bounds__(SCAN_THREADS) pq_scan_kernel(const ScanParams 
 #pragma unroll
         for (int q = 0; q < QPC; ++q) {
             if (q >= nqg) break;
-            const bool pass = live && acc[q] >= s_bnd[q];
+            const bool pass = live && (!PROBED || ivfp::probes(pr.probed, l, q0 + q)) && acc[q] >= s_bnd[q];
             const uint32_t bal = __ballot_sync(0xffffffffu, pass);
             if (bal == 0) continue;
             const int leader = __ffs(bal) - 1;
@@ -477,6 +505,43 @@ struct SearchWs {
     float* lut;    // [QBLOCK][M][256]
     float* cterm;  // [QBLOCK][n_list]
 };
+
+// A probed search (nprobe < n_list) takes the tables of its lists and carves its probe state after the search scratch.
+struct ProbeArgs {
+    int nprobe;
+    const int32_t* list_order;     // ivfpq: rows in list order (stable), [n]
+    const int32_t* list_offsets;   // ivfpq: first list position of every list, [n_list + 1]; ivfsq: first tile
+    const int32_t* list_rows;      // ivfsq: real rows of every list, [n_list]
+};
+
+struct ProbeWs {
+    uint32_t* probed;         // [n_list][PROBE_WORDS]
+    uint32_t* sample_lists;   // [n_list]
+    int2* items;              // [max_items]
+    int2* sample;             // [max_sample]
+    int32_t* count;           // [2]: items, sample items
+    int sample_units;         // sampled items at the front of a sample list
+    int64_t max_sample;
+};
+
+// Each sample list contributes its first max(PROBE_CHUNK, k) positions (ivf_probe.cuh), in whole units.
+static int sample_units(int k, int unit) { return ((k > PROBE_CHUNK ? k : PROBE_CHUNK) + unit - 1) / unit; }
+
+static size_t probe_bytes(size_t off, int n_list, int64_t max_items, int k, int unit, ProbeWs* w, void* base) {
+    Carver cv{static_cast<uint8_t*>(base), off};
+    const int su = sample_units(k, unit);
+    const int64_t max_sample = static_cast<int64_t>(n_list) * su < max_items ? static_cast<int64_t>(n_list) * su : max_items;
+    uint32_t* probed = cv.take<uint32_t>(static_cast<size_t>(n_list) * ivfp::PROBE_WORDS);
+    uint32_t* sample_lists = cv.take<uint32_t>(static_cast<size_t>(n_list));
+    int2* items = cv.take<int2>(static_cast<size_t>(max_items));
+    int2* sample = cv.take<int2>(static_cast<size_t>(max_sample));
+    int32_t* count = cv.take<int32_t>(2);
+    if (w) *w = ProbeWs{probed, sample_lists, items, sample, count, su, max_sample};
+    return cv.off;
+}
+
+// ivfpq: chunks of PROBE_CHUNK positions, at most one partial chunk per list
+static int64_t pq_max_items(int64_t n, int n_list) { return (n + PROBE_CHUNK - 1) / PROBE_CHUNK + n_list; }
 
 static size_t search_bytes(int64_t n, int M, int n_list, int k, SearchWs* w, void* base) {
     Carver cv{static_cast<uint8_t*>(base)};
@@ -677,11 +742,12 @@ static int choose_qpc(int M, int n_list, int nq, bool* cterm_smem) {
     return 1;
 }
 
-template <int QPC>
-static int launch_scan_q(const ScanParams& p, size_t smem, cudaStream_t s) {
+template <int QPC, bool PROBED>
+static int launch_scan_q(const ScanParams& p, const ProbeScan& pr, size_t smem, cudaStream_t s) {
     static bool attr_set = false;
     if (!attr_set) {
-        AB_CUDA_CHECK(cudaFuncSetAttribute(pq_scan_kernel<QPC>, cudaFuncAttributeMaxDynamicSharedMemorySize, SCAN_SMEM_MAX));
+        AB_CUDA_CHECK(cudaFuncSetAttribute(pq_scan_kernel<QPC, PROBED>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                           SCAN_SMEM_MAX));
         attr_set = true;
     }
     const int groups = (p.nq + QPC - 1) / QPC;
@@ -690,28 +756,32 @@ static int launch_scan_q(const ScanParams& p, size_t smem, cudaStream_t s) {
     int gx = (resident + groups - 1) / groups;
     if (gx > p.num_tiles) gx = p.num_tiles;
     if (gx < 1) gx = 1;
-    pq_scan_kernel<QPC><<<dim3(gx, groups), SCAN_THREADS, smem, s>>>(p);
+    pq_scan_kernel<QPC, PROBED><<<dim3(gx, groups), SCAN_THREADS, smem, s>>>(p, pr);
     abh::count_launch();
     AB_CUDA_CHECK(cudaGetLastError());
     return ATLAS_B200_OK;
 }
 
-static int launch_scan(int qpc, const ScanParams& p, size_t smem, cudaStream_t s) {
+template <bool PROBED>
+static int launch_scan(int qpc, const ScanParams& p, const ProbeScan& pr, size_t smem, cudaStream_t s) {
     if (p.num_tiles <= 0) return ATLAS_B200_OK;
     switch (qpc) {
-        case 16: return launch_scan_q<16>(p, smem, s);
-        case 8: return launch_scan_q<8>(p, smem, s);
-        case 4: return launch_scan_q<4>(p, smem, s);
-        case 2: return launch_scan_q<2>(p, smem, s);
-        default: return launch_scan_q<1>(p, smem, s);
+        case 16: return launch_scan_q<16, PROBED>(p, pr, smem, s);
+        case 8: return launch_scan_q<8, PROBED>(p, pr, smem, s);
+        case 4: return launch_scan_q<4, PROBED>(p, pr, smem, s);
+        case 2: return launch_scan_q<2, PROBED>(p, pr, smem, s);
+        default: return launch_scan_q<1, PROBED>(p, pr, smem, s);
     }
 }
 
 // The exact top-k pipeline of one block of nqb queries over the scores of a code sweep (mips.cu's one-stage sample):
 //   bound from a strided sample of ~2 sqrt(k n) rows (every score kept) -> full sweep with the bound -> select + emit,
 //   `status` on overflow; or the chunked exhaustive variant (every score of a chunk is a candidate, winners carried).
-// scan(tile_begin, tile_step, num_tiles) launches the scan kernel over tiles of `tile_rows` rows (n rows or slots in all);
-// it appends only real rows, so the sampled bound is the k-th best among real rows.  The sweep is profiled as kind 1.
+// scan(tile_begin, tile_step, num_tiles, sample) launches the scan kernel over tiles of `tile_rows` rows (n rows or slots in
+// all; sample marks the bound's sampling launch); it appends only real rows, so the sampled bound is the k-th best among
+// real rows.  A probed scan takes these tile counts as upper bounds of its compacted items and resolves them against the
+// item count in device memory (ivf_probe.cuh); its sampling launch scans the sample items instead, which reach every
+// query's own probe set.  The sweep is profiled as kind 1.
 template <class Scan>
 static int sweep_select(const Scan& scan, int64_t n, int total_tiles, int tile_rows, int nqb, int k, uint64_t* cand,
                         uint32_t* count, float* bound, uint32_t capq, uint16_t* os16, int64_t* oi_b, int64_t id_base,
@@ -725,13 +795,13 @@ static int sweep_select(const Scan& scan, int64_t n, int total_tiles, int tile_r
             int sample_tiles = static_cast<int>(m / tile_rows);
             if (sample_tiles < 1) sample_tiles = 1;
             if (sample_tiles > total_tiles) sample_tiles = total_tiles;
-            if ((rc = scan(0, total_tiles / sample_tiles, sample_tiles))) return rc;
+            if ((rc = scan(0, total_tiles / sample_tiles, sample_tiles, true))) return rc;
             mips::mips_select_kernel<false><<<nqb, mips::SEL_THREADS, 0, s>>>(
                 cand, count, capq, k, mips::SEL_WRITE_BOUND, bound, nullptr, nullptr, 0, 0, nullptr);
             abh::count_launch();
         }
         abh::prof_begin(s, abh::PROF_SCAN);
-        rc = scan(0, 1, total_tiles);
+        rc = scan(0, 1, total_tiles, false);
         abh::prof_end(s, abh::PROF_SCAN, sweep_work);
         if (rc) return rc;
         mips::mips_select_kernel<false><<<nqb, mips::SEL_THREADS, 0, s>>>(
@@ -742,7 +812,7 @@ static int sweep_select(const Scan& scan, int64_t n, int total_tiles, int tile_r
         if (chunk_tiles < 1) chunk_tiles = 1;
         for (int t0 = 0; t0 < total_tiles; t0 += chunk_tiles) {
             const bool last = t0 + chunk_tiles >= total_tiles;
-            if ((rc = scan(t0, 1, last ? total_tiles - t0 : chunk_tiles))) return rc;
+            if ((rc = scan(t0, 1, last ? total_tiles - t0 : chunk_tiles, false))) return rc;
             mips::mips_select_kernel<false><<<nqb, mips::SEL_THREADS, 0, s>>>(
                 cand, count, capq, k, last ? mips::SEL_EMIT : mips::SEL_CARRY, bound, os16, oi_b, id_base, id_stride,
                 nullptr);
@@ -755,9 +825,16 @@ static int sweep_select(const Scan& scan, int64_t n, int total_tiles, int tile_r
 
 static int topk(const uint8_t* codes, const void* lists, int64_t n, int M, const float* codebooks, const float* coarse,
                 int n_list, const __half* queries, int nq, int k, __half* out_scores, int64_t* out_ids, int64_t id_base,
-                int64_t id_stride, int32_t* status, void* ws, size_t ws_bytes, cudaStream_t s, bool exhaustive) {
+                int64_t id_stride, int32_t* status, void* ws, size_t ws_bytes, cudaStream_t s, bool exhaustive,
+                const ProbeArgs* probe = nullptr) {
     int rc = check_shape(M, n_list);
     if (rc) return rc;
+    if (probe) {
+        AB_REQUIRE(n_list >= 1, "a probed search needs inverted lists (n_list=%d)", n_list);
+        AB_REQUIRE(probe->nprobe >= 1, "nprobe=%d must be >= 1", probe->nprobe);
+        AB_REQUIRE(probe->list_order != nullptr && probe->list_offsets != nullptr, "null list table");
+        if (probe->nprobe >= n_list) probe = nullptr;     // every list: the full scan
+    }
     AB_REQUIRE(nq >= 0 && k >= 1, "nq must be >= 0 and k >= 1 (nq=%d k=%d)", nq, k);
     AB_REQUIRE(k <= ATLAS_B200_MAX_TOPK, "k=%d exceeds ATLAS_B200_MAX_TOPK=%d", k, ATLAS_B200_MAX_TOPK);
     AB_REQUIRE(n >= 1 && n < (1ll << 31) - SCAN_THREADS, "rows n=%lld out of range", (long long)n);
@@ -769,7 +846,10 @@ static int topk(const uint8_t* codes, const void* lists, int64_t n, int M, const
     if (status) AB_CUDA_CHECK(cudaMemsetAsync(status, 0, sizeof(int32_t), s));
     if (nq == 0) return ATLAS_B200_OK;
     SearchWs w;
-    const size_t need = search_bytes(n, M, n_list, k, &w, ws);
+    ProbeWs pw{};
+    const int64_t max_items = pq_max_items(n, n_list);
+    size_t need = search_bytes(n, M, n_list, k, &w, ws);
+    if (probe) need = probe_bytes(need, n_list, max_items, k, PROBE_CHUNK, &pw, ws);
     if (ws == nullptr || ws_bytes < need) {
         abh::set_error("workspace too small: have %zu need %zu", ws_bytes, need);
         return ATLAS_B200_EWORKSPACE;
@@ -803,13 +883,34 @@ static int topk(const uint8_t* codes, const void* lists, int64_t n, int M, const
         p.capq = w.capq;
         int64_t* oi_b = out_ids + static_cast<size_t>(q0) * k;
         uint16_t* os16 = reinterpret_cast<uint16_t*>(out_scores + static_cast<size_t>(q0) * k);
-        auto scan = [&](int tile_begin, int tile_step, int num_tiles) {
+        if (probe) {
+            // P(q) and its sample lists from the coarse terms the scan adds, then the chunks of every list some query
+            // probes and the sample chunks
+            if ((rc = ivfp::select_probes(w.cterm, n_list, 1, nqb, n_list, probe->list_offsets, nullptr, probe->nprobe, k,
+                                          w.capq, pw.sample_units * PROBE_CHUNK, pw.probed, pw.sample_lists, s)))
+                return rc;
+            if ((rc = ivfp::compact_items(pw.probed, pw.sample_lists, probe->list_offsets, n_list, PROBE_CHUNK,
+                                          pw.sample_units, pw.items, pw.sample, pw.count, s)))
+                return rc;
+        }
+        ProbeScan pr{pw.items, pw.count, probe ? probe->list_order : nullptr, probe ? probe->list_offsets : nullptr,
+                     pw.probed};
+        auto scan = [&](int tile_begin, int tile_step, int num_tiles, bool sample) {
             p.tile_begin = tile_begin;
             p.tile_step = tile_step;
             p.num_tiles = num_tiles;
-            return launch_scan(qpc, p, smem, s);
+            if (!probe) return launch_scan<false>(qpc, p, pr, smem, s);
+            ProbeScan ps = pr;
+            if (sample) {     // the bound's scan: every sample chunk (ivf_probe.cuh), not a stride over the sweep
+                ps.items = pw.sample;
+                ps.item_count = pw.count + 1;
+                p.tile_begin = 0;
+                p.tile_step = 1;
+                p.num_tiles = static_cast<int>(pw.max_sample);
+            }
+            return launch_scan<true>(qpc, p, ps, smem, s);
         };
-        if ((rc = sweep_select(scan, n, total_tiles, SCAN_THREADS, nqb, k, w.cand, w.count, w.bound, w.capq, os16, oi_b, id_base,
+        if ((rc = sweep_select(scan, n, probe ? static_cast<int>(max_items) : total_tiles, SCAN_THREADS, nqb, k, w.cand, w.count, w.bound, w.capq, os16, oi_b, id_base,
                                id_stride, status, exhaustive, static_cast<double>(n) * M * ((nqb + qpc - 1) / qpc), s)))
             return rc;
     }
@@ -1080,8 +1181,13 @@ static int sq_encode(const __half* rows, int64_t n, const float* coarse, int n_l
 static int sq_topk(const uint8_t* codes, const int32_t* slot_rows, const int32_t* tile_lists, int64_t n_tiles, int64_t n_rows,
                    const float* coarse, int n_list, const float* vmin, const float* vdiff, const __half* queries, int nq, int k,
                    __half* out_scores, int64_t* out_ids, int64_t id_base, int64_t id_stride, int32_t* status, void* ws,
-                   size_t ws_bytes, cudaStream_t s, bool exhaustive) {
+                   size_t ws_bytes, cudaStream_t s, bool exhaustive, const ProbeArgs* probe = nullptr) {
     AB_REQUIRE(nq >= 0 && k >= 1, "nq must be >= 0 and k >= 1 (nq=%d k=%d)", nq, k);
+    if (probe) {
+        AB_REQUIRE(probe->nprobe >= 1, "nprobe=%d must be >= 1", probe->nprobe);
+        AB_REQUIRE(probe->list_offsets != nullptr && probe->list_rows != nullptr, "null list table");
+        if (probe->nprobe >= n_list) probe = nullptr;     // every list: the full scan
+    }
     AB_REQUIRE(k <= ATLAS_B200_MAX_TOPK, "k=%d exceeds ATLAS_B200_MAX_TOPK=%d", k, ATLAS_B200_MAX_TOPK);
     AB_REQUIRE(n_list >= 1, "n_list=%d must be >= 1", n_list);
     AB_REQUIRE(n_rows >= 1 && n_tiles >= 1 && n_rows <= n_tiles * ivfsq::SQ_TILE &&
@@ -1095,8 +1201,10 @@ static int sq_topk(const uint8_t* codes, const int32_t* slot_rows, const int32_t
     if (status) AB_CUDA_CHECK(cudaMemsetAsync(status, 0, sizeof(int32_t), s));
     if (nq == 0) return ATLAS_B200_OK;
     SqSearchWs w;
+    ProbeWs pw{};
     const int64_t n_slots = n_tiles * ivfsq::SQ_TILE;
-    const size_t need = sq_search_bytes(n_slots, n_list, k, &w, ws);
+    size_t need = sq_search_bytes(n_slots, n_list, k, &w, ws);
+    if (probe) need = probe_bytes(need, n_list, n_tiles, k, ivfsq::SQ_TILE, &pw, ws);
     if (ws == nullptr || ws_bytes < need) {
         abh::set_error("workspace too small: have %zu need %zu", ws_bytes, need);
         return ATLAS_B200_EWORKSPACE;
@@ -1126,11 +1234,30 @@ static int sq_topk(const uint8_t* codes, const int32_t* slot_rows, const int32_t
         p.capq = w.capq;
         int64_t* oi_b = out_ids + static_cast<size_t>(q0) * k;
         uint16_t* os16 = reinterpret_cast<uint16_t*>(out_scores + static_cast<size_t>(q0) * k);
-        auto scan = [&](int tile_begin, int tile_step, int num_tiles) {
+        if (probe) {
+            // P(q) and its sample lists from T[l][q] (strided by list), then the tiles of every list some query probes
+            // and the sample tiles
+            if ((rc = ivfp::select_probes(w.tterm, 1, nqb, nqb, n_list, nullptr, probe->list_rows, probe->nprobe, k, w.capq,
+                                          pw.sample_units * ivfsq::SQ_TILE, pw.probed, pw.sample_lists, s)))
+                return rc;
+            if ((rc = ivfp::compact_items(pw.probed, pw.sample_lists, probe->list_offsets, n_list, 1, pw.sample_units,
+                                          pw.items, pw.sample, pw.count, s)))
+                return rc;
+        }
+        const ivfsq::ProbeScan pr{pw.items, pw.count, pw.probed};
+        const ivfsq::ProbeScan ps{pw.sample, pw.count + 1, pw.probed};
+        auto scan = [&](int tile_begin, int tile_step, int num_tiles, bool sample) {
             p.tile_begin = tile_begin;
             p.tile_step = tile_step;
             p.num_tiles = num_tiles;
-            return ivfsq::launch_scan(p, s);
+            if (!probe) return ivfsq::launch_scan(p, nullptr, s);
+            if (sample) {     // the bound's scan: every sample tile (ivf_probe.cuh), not a stride over the sweep
+                p.tile_begin = 0;
+                p.tile_step = 1;
+                p.num_tiles = static_cast<int>(pw.max_sample);
+                return ivfsq::launch_scan(p, &ps, s);
+            }
+            return ivfsq::launch_scan(p, &pr, s);
         };
         // work = code bytes swept (once per 128 queries of the block)
         const double sweep_bytes = static_cast<double>(n_slots) * ivfsq::SQ_CODE_BYTES * ((nqb + 127) / 128);
@@ -1154,6 +1281,10 @@ size_t atlas_b200_pq_workspace_bytes(int32_t op, int64_t n, int32_t M, int32_t n
         case ATLAS_B200_PQ_OP_TRAIN: return pq::train_bytes(n, M, n_list, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr);
         case ATLAS_B200_PQ_OP_ENCODE: return pq::encode_bytes(M, n_list, nullptr, nullptr);
         case ATLAS_B200_PQ_OP_SEARCH: return pq::search_bytes(n, M, n_list, k, nullptr, nullptr);
+        case ATLAS_B200_PQ_OP_SEARCH_PROBED:
+            if (n_list < 1) return 0;
+            return pq::probe_bytes(pq::search_bytes(n, M, n_list, k, nullptr, nullptr), n_list, pq::pq_max_items(n, n_list),
+                                   k, pq::PROBE_CHUNK, nullptr, nullptr);
         default: return 0;
     }
 }
@@ -1188,6 +1319,29 @@ int atlas_b200_pq_topk_exhaustive(const uint8_t* codes, const void* list_ids, in
                     static_cast<cudaStream_t>(stream), true);
 }
 
+int atlas_b200_pq_topk_probed(const uint8_t* codes, const void* list_ids, int64_t n, int32_t M, const float* codebooks,
+                              const float* coarse, int32_t n_list, const int32_t* list_order, const int32_t* list_offsets,
+                              int32_t nprobe, const void* queries, int32_t nq, int32_t k, void* out_scores,
+                              int64_t* out_ids, int64_t id_base, int64_t id_stride, int32_t* status, void* workspace,
+                              size_t workspace_bytes, void* stream) {
+    const pq::ProbeArgs probe{nprobe, list_order, list_offsets, nullptr};
+    return pq::topk(codes, list_ids, n, M, codebooks, coarse, n_list, static_cast<const __half*>(queries), nq, k,
+                    static_cast<__half*>(out_scores), out_ids, id_base, id_stride, status, workspace, workspace_bytes,
+                    static_cast<cudaStream_t>(stream), false, &probe);
+}
+
+int atlas_b200_pq_topk_probed_exhaustive(const uint8_t* codes, const void* list_ids, int64_t n, int32_t M,
+                                         const float* codebooks, const float* coarse, int32_t n_list,
+                                         const int32_t* list_order, const int32_t* list_offsets, int32_t nprobe,
+                                         const void* queries, int32_t nq, int32_t k, void* out_scores, int64_t* out_ids,
+                                         int64_t id_base, int64_t id_stride, void* workspace, size_t workspace_bytes,
+                                         void* stream) {
+    const pq::ProbeArgs probe{nprobe, list_order, list_offsets, nullptr};
+    return pq::topk(codes, list_ids, n, M, codebooks, coarse, n_list, static_cast<const __half*>(queries), nq, k,
+                    static_cast<__half*>(out_scores), out_ids, id_base, id_stride, nullptr, workspace, workspace_bytes,
+                    static_cast<cudaStream_t>(stream), true, &probe);
+}
+
 size_t atlas_b200_ivfsq_workspace_bytes(int32_t op, int64_t n, int32_t n_list, int32_t k) {
     if (n_list < 1) return 0;
     if (n < 1) n = 1;
@@ -1196,6 +1350,9 @@ size_t atlas_b200_ivfsq_workspace_bytes(int32_t op, int64_t n, int32_t n_list, i
         case ATLAS_B200_PQ_OP_TRAIN: return pq::sq_train_bytes(n, n_list, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr);
         case ATLAS_B200_PQ_OP_ENCODE: return pq::sq_encode_bytes(n_list, nullptr, nullptr);
         case ATLAS_B200_PQ_OP_SEARCH: return pq::sq_search_bytes(n, n_list, k, nullptr, nullptr);
+        case ATLAS_B200_PQ_OP_SEARCH_PROBED:
+            return pq::probe_bytes(pq::sq_search_bytes(n, n_list, k, nullptr, nullptr), n_list,
+                                   (n + ivfsq::SQ_TILE - 1) / ivfsq::SQ_TILE, k, ivfsq::SQ_TILE, nullptr, nullptr);
         default: return 0;
     }
 }
@@ -1230,6 +1387,29 @@ int atlas_b200_ivfsq_topk_exhaustive(const uint8_t* codes, const int32_t* slot_r
     return pq::sq_topk(codes, slot_rows, tile_lists, n_tiles, n_rows, coarse, n_list, vmin, vdiff,
                        static_cast<const __half*>(queries), nq, k, static_cast<__half*>(out_scores), out_ids, id_base,
                        id_stride, nullptr, workspace, workspace_bytes, static_cast<cudaStream_t>(stream), true);
+}
+
+int atlas_b200_ivfsq_topk_probed(const uint8_t* codes, const int32_t* slot_rows, const int32_t* tile_lists, int64_t n_tiles,
+                                 int64_t n_rows, const int32_t* list_tile_off, const int32_t* list_rows, const float* coarse,
+                                 int32_t n_list, const float* vmin, const float* vdiff, int32_t nprobe, const void* queries,
+                                 int32_t nq, int32_t k, void* out_scores, int64_t* out_ids, int64_t id_base,
+                                 int64_t id_stride, int32_t* status, void* workspace, size_t workspace_bytes, void* stream) {
+    const pq::ProbeArgs probe{nprobe, nullptr, list_tile_off, list_rows};
+    return pq::sq_topk(codes, slot_rows, tile_lists, n_tiles, n_rows, coarse, n_list, vmin, vdiff,
+                       static_cast<const __half*>(queries), nq, k, static_cast<__half*>(out_scores), out_ids, id_base,
+                       id_stride, status, workspace, workspace_bytes, static_cast<cudaStream_t>(stream), false, &probe);
+}
+
+int atlas_b200_ivfsq_topk_probed_exhaustive(const uint8_t* codes, const int32_t* slot_rows, const int32_t* tile_lists,
+                                            int64_t n_tiles, int64_t n_rows, const int32_t* list_tile_off,
+                                            const int32_t* list_rows, const float* coarse, int32_t n_list, const float* vmin,
+                                            const float* vdiff, int32_t nprobe, const void* queries, int32_t nq, int32_t k,
+                                            void* out_scores, int64_t* out_ids, int64_t id_base, int64_t id_stride,
+                                            void* workspace, size_t workspace_bytes, void* stream) {
+    const pq::ProbeArgs probe{nprobe, nullptr, list_tile_off, list_rows};
+    return pq::sq_topk(codes, slot_rows, tile_lists, n_tiles, n_rows, coarse, n_list, vmin, vdiff,
+                       static_cast<const __half*>(queries), nq, k, static_cast<__half*>(out_scores), out_ids, id_base,
+                       id_stride, nullptr, workspace, workspace_bytes, static_cast<cudaStream_t>(stream), true, &probe);
 }
 
 }  // extern "C"

@@ -318,6 +318,16 @@ class DistributedIndex(object):
         return None
 
 
+def _check_nprobe(index_type, nprobe):
+    """nprobe: None (every list) or an int >= 1 (not a bool), and None for type pq, which has no lists."""
+    if nprobe is not None and (isinstance(nprobe, bool) or not isinstance(nprobe, int) or nprobe < 1):
+        raise AtlasB200Error(f"DistributedFAISSIndex: nprobe={nprobe!r} must be None (every list) or an integer >= 1")
+    if nprobe is not None and index_type == "pq":
+        raise AtlasB200Error(f"DistributedFAISSIndex('pq'): nprobe={nprobe!r} needs inverted lists; index type pq has none "
+                             "(use ivfpq or ivfsq, or nprobe=None)")
+    return nprobe
+
+
 class DistributedFAISSIndex(DistributedIndex):
     """`--index_mode faiss` (src/index.py:163-381) with a product-quantized index on the device (csrc/pq.cu).
 
@@ -355,14 +365,26 @@ class DistributedFAISSIndex(DistributedIndex):
     rounded once to fp16 (csrc/ivfsq.cu, include/atlas_b200.h).  `code_size` is bits per dimension (faiss's SQ4 naming):
     None or 4.  The device holds 384 bytes of codes and a 4-byte row id per slot, in inverted-list order with every list
     padded to a multiple of 64 slots; the index file holds the codes in row order and faiss's packing, with the list
-    ids, and `load_index` rebuilds the slot layout from them.  Training needs one row."""
+    ids, and `load_index` rebuilds the slot layout from them.  Training needs one row.
+
+    Probing (faiss's `nprobe`, opt-in, ivfpq and ivfsq): with `nprobe` an int >= 1 (a constructor keyword and a plain
+    attribute that may be set at any time; Atlas sets it from `--faiss_nprobe`) each query is scored only against the
+    rows of its best lists: the shortest prefix of the lists ordered by the coarse term <q, c_l> (descending, then list
+    id) that has at least `nprobe` lists and holds at least k rows (faiss would return id -1 when the probed lists hold
+    fewer than k rows instead; see include/atlas_b200.h).  The result is the exact top-k over those rows, and the sweep
+    reads only the codes of lists some query of the block probes.  None (default) or nprobe >= n_list scans every row,
+    as before.  Type pq has no lists: a non-None value raises.  Refinement composes (the probed search supplies the k'
+    candidates).  ivfpq keeps its codes in row order and reads them through a list-order permutation built on the first
+    probed search: +4 bytes per row of device memory from then on, dropped with the index on retraining or
+    `mark_stale()`.  `nprobe` is not written to the index file."""
 
     SUPPORTED_TYPES = ("pq", "ivfpq", "ivfsq")
     FILE_FORMAT = 1
     TRAIN_SEED = 1234
     STAGE_ROWS = 65536
 
-    def __init__(self, index_type: str = "flat", code_size: Optional[int] = None, refine_factor: int = 1):
+    def __init__(self, index_type: str = "flat", code_size: Optional[int] = None, refine_factor: int = 1,
+                 nprobe: Optional[int] = None):
         if index_type not in self.SUPPORTED_TYPES:
             raise AtlasB200Error(
                 f"DistributedFAISSIndex: index_type={index_type!r} is not provided by atlas_b200; supported types are "
@@ -378,6 +400,7 @@ class DistributedFAISSIndex(DistributedIndex):
             raise AtlasB200Error(f"DistributedFAISSIndex({index_type!r}) needs a code_size (--faiss_code_size)")
         else:
             ops.pq_check_code_size(code_size)
+        _check_nprobe(index_type, nprobe)
         super().__init__()
         self._device()                 # no CUDA device: raise here, like the flat index (no CPU path)
         self.index_type = index_type
@@ -388,6 +411,8 @@ class DistributedFAISSIndex(DistributedIndex):
         self._pq = None
         self.refine_factor = refine_factor
         self._refine_factor()
+        self.nprobe = nprobe
+        self._nprobe()
 
     # ------------------------------------------------------------------ host rows
     @property
@@ -519,7 +544,23 @@ class DistributedFAISSIndex(DistributedIndex):
             raise AtlasB200Error(f"DistributedFAISSIndex: refine_factor={r!r} must be an integer >= 1 (1 = no refinement)")
         return r
 
+    def _nprobe(self):
+        return _check_nprobe(self.index_type, self.nprobe)
+
+    def _probe_tables(self, p, nprobe):
+        """The list tables of a probed search, built on the first one and kept in the trained index (dropped with it)."""
+        if nprobe is None or nprobe >= p["n_list"]:
+            return {}
+        if self.index_type == "ivfsq":
+            if "list_tile_off" not in p:
+                p["list_tile_off"], p["list_rows"] = ops.ivfsq_list_tables(p["slot_rows"], p["tile_lists"], p["n_list"])
+            return dict(list_tile_off=p["list_tile_off"], list_rows=p["list_rows"])
+        if "list_order" not in p:
+            p["list_order"], p["list_offsets"] = ops.ivfpq_list_tables(p["list_ids"], p["n_list"])
+        return dict(list_order=p["list_order"], list_offsets=p["list_offsets"])
+
     def _local_search(self, allqueries, topk, exhaustive=False):
+        self._nprobe()
         r = self._refine_factor()
         if r == 1:
             return self._candidate_search(allqueries, topk, self._id_base, self._id_stride, exhaustive)
@@ -534,12 +575,14 @@ class DistributedFAISSIndex(DistributedIndex):
     def _candidate_search(self, allqueries, k, id_base, id_stride, exhaustive):
         """Top k by PQ score: (scores, ids = id_base + id_stride * row, device status word)."""
         p = self._trained()
+        nprobe = self._nprobe()
+        tables = self._probe_tables(p, nprobe)
         if self.index_type == "ivfsq":
             return ops.ivfsq_topk(p["codes"], p["slot_rows"], p["tile_lists"], int(self._bank.shape[0]), p["coarse"],
                                   p["vmin"], p["vdiff"], allqueries, k, id_base, id_stride, self._workspace,
-                                  exhaustive=exhaustive)
+                                  exhaustive=exhaustive, nprobe=nprobe, **tables)
         return ops.pq_topk(p["codes"], p["list_ids"], p["codebooks"], p["coarse"], allqueries, k, id_base, id_stride,
-                           self._workspace, exhaustive=exhaustive)
+                           self._workspace, exhaustive=exhaustive, nprobe=nprobe, **tables)
 
     def _refine(self, allqueries, cand_local, topk):
         """Top `topk` of the candidate rows `cand_local` [nq, k'] by exact score: (scores, global ids)."""

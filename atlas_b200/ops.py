@@ -160,7 +160,7 @@ def topk_merge_blob(blob_all, ids_off, world, nq_total, k, q_begin, nq_out, dtyp
 # ---------------------------------------------------------------------------------------------
 # product-quantized index (csrc/pq.cu)
 # ---------------------------------------------------------------------------------------------
-PQ_OP_TRAIN, PQ_OP_ENCODE, PQ_OP_SEARCH = 0, 1, 2
+PQ_OP_TRAIN, PQ_OP_ENCODE, PQ_OP_SEARCH, PQ_OP_SEARCH_PROBED = 0, 1, 2, 3
 PQ_KSUB = 256
 PQ_ITERS = 25   # faiss's k-means default
 
@@ -213,21 +213,70 @@ def pq_encode(rows, codebooks, coarse, codes, list_ids=None, workspace=None):
     return codes, list_ids
 
 
-def pq_topk(codes, list_ids, codebooks, coarse, queries, k, id_base=0, id_stride=1, workspace=None, exhaustive=False):
+def check_nprobe(nprobe):
+    """nprobe: None (every list) or an int >= 1 (not a bool)."""
+    if nprobe is not None and (isinstance(nprobe, bool) or not isinstance(nprobe, int) or nprobe < 1):
+        raise AtlasB200Error(f"nprobe={nprobe!r} must be None (every list) or an integer >= 1")
+    return nprobe
+
+
+def _probed(nprobe, n_list, what):
+    """True when a search with `nprobe` scans only some lists (nprobe < n_list); None / >= n_list is the full scan."""
+    check_nprobe(nprobe)
+    if nprobe is not None and n_list == 0:
+        raise AtlasB200Error(f"{what}: nprobe={nprobe} needs inverted lists (index type pq has none)")
+    return nprobe is not None and nprobe < n_list
+
+
+def _check_table(t, name, shape):
+    require_cuda(t, name)
+    if t.dtype != torch.int32 or tuple(t.shape) != shape or not t.is_contiguous():
+        raise AtlasB200Error(f"{name} must be contiguous int32 {list(shape)}, got {t.dtype} {tuple(t.shape)}")
+
+
+def ivfpq_list_tables(list_ids, n_list):
+    """The list tables of a probed ivfpq search: (list_order int32 [n], the rows sorted by list id, stable;
+    list_offsets int32 [n_list + 1], list l holding list_order[list_offsets[l]:list_offsets[l + 1]])."""
+    lists = list_ids.to(torch.int64)
+    order = torch.sort(lists, stable=True).indices.to(torch.int32)
+    offsets = torch.zeros(n_list + 1, dtype=torch.int64, device=lists.device)
+    offsets[1:] = torch.cumsum(torch.bincount(lists, minlength=n_list), 0)
+    return order, offsets.to(torch.int32)
+
+
+def pq_topk(codes, list_ids, codebooks, coarse, queries, k, id_base=0, id_stride=1, workspace=None, exhaustive=False,
+            nprobe=None, list_order=None, list_offsets=None):
     """Top-k of the PQ / IVF-PQ scores of `queries` [nq, 768] over one shard's codes (atlas_b200_pq_topk).
 
-    Returns (scores [nq, k] fp16 desc, ids [nq, k] int64, status int32[1] device tensor) like `mips_topk`."""
+    Returns (scores [nq, k] fp16 desc, ids [nq, k] int64, status int32[1] device tensor) like `mips_topk`.
+    nprobe < n_list (ivfpq): only the rows of each query's best lists (atlas_b200_pq_topk_probed), with the tables of
+    `ivfpq_list_tables`; None or >= n_list scans every row.  The probed search does not synchronise with the host when
+    the tables are passed; built here (when not given) they cost a host synchronisation (torch.bincount) per call."""
     require_cuda(codes, "codes")
     n, M = codes.shape
     n_list = 0 if coarse is None else coarse.shape[0]
+    probed = _probed(nprobe, n_list, "pq_topk")
     q = cast_queries(queries.reshape(-1, DIM).to(codes.device), torch.float16)
     nq = q.shape[0]
-    buf = (workspace or _default_ws).get(lib().atlas_b200_pq_workspace_bytes(PQ_OP_SEARCH, n, M, n_list, k), codes.device)
+    op = PQ_OP_SEARCH_PROBED if probed else PQ_OP_SEARCH
+    buf = (workspace or _default_ws).get(lib().atlas_b200_pq_workspace_bytes(op, n, M, n_list, k), codes.device)
     out_s = torch.empty((nq, k), dtype=torch.float16, device=codes.device)
     out_i = torch.empty((nq, k), dtype=torch.int64, device=codes.device)
     status = torch.zeros(1, dtype=torch.int32, device=codes.device)
     lp = _ptr(list_ids) if n_list else None
     cp = _ptr(coarse) if n_list else None
+    if probed:
+        if list_order is None or list_offsets is None:
+            list_order, list_offsets = ivfpq_list_tables(list_ids, n_list)
+        _check_table(list_order, "list_order", (n,))
+        _check_table(list_offsets, "list_offsets", (n_list + 1,))
+        args = (_ptr(codes), lp, n, M, _ptr(codebooks), cp, n_list, _ptr(list_order), _ptr(list_offsets), nprobe, _ptr(q),
+                nq, k, _ptr(out_s), _ptr(out_i), id_base, id_stride)
+        if exhaustive:
+            check(lib().atlas_b200_pq_topk_probed_exhaustive(*args, _ptr(buf), buf.numel(), current_stream_ptr()))
+        else:
+            check(lib().atlas_b200_pq_topk_probed(*args, _ptr(status), _ptr(buf), buf.numel(), current_stream_ptr()))
+        return out_s, out_i, status
     if exhaustive:
         check(lib().atlas_b200_pq_topk_exhaustive(_ptr(codes), lp, n, M, _ptr(codebooks), cp, n_list, _ptr(q), nq, k,
                                                   _ptr(out_s), _ptr(out_i), id_base, id_stride, _ptr(buf), buf.numel(),
@@ -413,12 +462,27 @@ def ivfsq_import(codes_rows, list_ids, n_list):
     return codes, slot_rows, tile_lists
 
 
+def ivfsq_list_tables(slot_rows, tile_lists, n_list):
+    """The list tables of a probed ivfsq search: (list_tile_off int32 [n_list + 1], list l owning tiles
+    list_tile_off[l]:list_tile_off[l + 1]; list_rows int32 [n_list], its real rows)."""
+    tl = tile_lists.to(torch.int64)
+    off = torch.zeros(n_list + 1, dtype=torch.int64, device=tl.device)
+    off[1:] = torch.cumsum(torch.bincount(tl, minlength=n_list), 0)
+    real = (slot_rows.reshape(-1, SQ_TILE) >= 0).sum(1)
+    rows = torch.zeros(n_list, dtype=torch.int64, device=tl.device).index_add_(0, tl, real)
+    return off.to(torch.int32), rows.to(torch.int32)
+
+
 def ivfsq_topk(codes, slot_rows, tile_lists, n_rows, coarse, vmin, vdiff, queries, k, id_base=0, id_stride=1,
-               workspace=None, exhaustive=False):
+               workspace=None, exhaustive=False, nprobe=None, list_tile_off=None, list_rows=None):
     """Top-k of the IVF-SQ scores of `queries` [nq, 768] over one shard's rows in the device layout
-    (atlas_b200_ivfsq_topk).  Returns (scores [nq, k] fp16 desc, ids [nq, k] int64, status int32[1]) like `mips_topk`."""
+    (atlas_b200_ivfsq_topk).  Returns (scores [nq, k] fp16 desc, ids [nq, k] int64, status int32[1]) like `mips_topk`.
+    nprobe < n_list: only the rows of each query's best lists (atlas_b200_ivfsq_topk_probed), with the tables of
+    `ivfsq_list_tables`; None or >= n_list scans every slot.  The probed search does not synchronise with the host when
+    the tables are passed; built here (when not given) they cost a host synchronisation (torch.bincount) per call."""
     require_cuda(codes, "codes")
     n_list = _sq_check_state(coarse, vmin, vdiff)
+    probed = _probed(nprobe, n_list, "ivfsq_topk")
     if codes.dtype != torch.uint8 or codes.dim() != 2 or codes.shape[1] != SQ_CODE_BYTES or not codes.is_contiguous() \
             or codes.shape[0] % SQ_TILE or codes.data_ptr() % 16:
         raise AtlasB200Error(f"ivfsq_topk: codes must be contiguous, 16-byte aligned uint8 [64 * tiles, {SQ_CODE_BYTES}]")
@@ -428,11 +492,24 @@ def ivfsq_topk(codes, slot_rows, tile_lists, n_rows, coarse, vmin, vdiff, querie
         raise AtlasB200Error("ivfsq_topk: slot_rows must be int32 [slots] and tile_lists int32 [tiles]")
     q = cast_queries(queries.reshape(-1, DIM).to(codes.device), torch.float16)
     nq = q.shape[0]
-    buf = (workspace or _default_ws).get(lib().atlas_b200_ivfsq_workspace_bytes(PQ_OP_SEARCH, codes.shape[0], n_list, k),
-                                         codes.device)
+    op = PQ_OP_SEARCH_PROBED if probed else PQ_OP_SEARCH
+    buf = (workspace or _default_ws).get(lib().atlas_b200_ivfsq_workspace_bytes(op, codes.shape[0], n_list, k), codes.device)
     out_s = torch.empty((nq, k), dtype=torch.float16, device=codes.device)
     out_i = torch.empty((nq, k), dtype=torch.int64, device=codes.device)
     status = torch.zeros(1, dtype=torch.int32, device=codes.device)
+    if probed:
+        if list_tile_off is None or list_rows is None:
+            list_tile_off, list_rows = ivfsq_list_tables(slot_rows, tile_lists, n_list)
+        _check_table(list_tile_off, "list_tile_off", (n_list + 1,))
+        _check_table(list_rows, "list_rows", (n_list,))
+        args = (_ptr(codes), _ptr(slot_rows.contiguous()), _ptr(tile_lists.contiguous()), n_tiles, n_rows,
+                _ptr(list_tile_off), _ptr(list_rows), _ptr(coarse), n_list, _ptr(vmin), _ptr(vdiff), nprobe, _ptr(q), nq, k,
+                _ptr(out_s), _ptr(out_i), id_base, id_stride)
+        if exhaustive:
+            check(lib().atlas_b200_ivfsq_topk_probed_exhaustive(*args, _ptr(buf), buf.numel(), current_stream_ptr()))
+        else:
+            check(lib().atlas_b200_ivfsq_topk_probed(*args, _ptr(status), _ptr(buf), buf.numel(), current_stream_ptr()))
+        return out_s, out_i, status
     args = (_ptr(codes), _ptr(slot_rows.contiguous()), _ptr(tile_lists.contiguous()), n_tiles, n_rows, _ptr(coarse),
             n_list, _ptr(vmin), _ptr(vdiff), _ptr(q), nq, k, _ptr(out_s), _ptr(out_i), id_base, id_stride)
     if exhaustive:

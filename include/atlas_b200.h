@@ -124,6 +124,7 @@ int atlas_b200_search_host(const void* bank, int64_t n, int64_t ld, int32_t is_b
 #define ATLAS_B200_PQ_OP_TRAIN 0
 #define ATLAS_B200_PQ_OP_ENCODE 1
 #define ATLAS_B200_PQ_OP_SEARCH 2
+#define ATLAS_B200_PQ_OP_SEARCH_PROBED 3
 size_t atlas_b200_pq_workspace_bytes(int32_t op, int64_t n, int32_t M, int32_t n_list, int32_t k);
 int atlas_b200_pq_train(const void* sample, int64_t n_sample, int32_t M, int32_t n_list, int32_t iters,
                         float* codebooks, float* coarse, void* workspace, size_t workspace_bytes, void* stream);
@@ -138,6 +139,46 @@ int atlas_b200_pq_topk_exhaustive(const uint8_t* codes, const void* list_ids, in
                                   const float* codebooks, const float* coarse, int32_t n_list, const void* queries,
                                   int32_t nq, int32_t k, void* out_scores, int64_t* out_ids, int64_t id_base,
                                   int64_t id_stride, void* workspace, size_t workspace_bytes, void* stream);
+
+/* --------------------------------------------------------------------------------------------
+ * Probed IVF search (`nprobe`, csrc/ivf_probe.cu) for ivfpq and ivfsq (the ivfsq tables are below).
+ *
+ *   T[q][l]    the fp32 coarse term the scan adds to every row of list l: <q, c_l> from the fp16-rounded query.
+ *   order(q)   the lists sorted by T[q][l] descending, then by list id ascending.
+ *   P(q)       the shortest prefix of order(q) with at least nprobe lists (empty lists count) that holds at least k
+ *              real rows.  Unlike faiss, which returns id -1 when the probed lists hold fewer than k rows, the prefix
+ *              is extended; as k <= n, it always exists.
+ *   result     the exact top-k of the full search's contract (scores, canonical tie order) over the rows whose list
+ *              is in P(q).  It does not depend on the other queries of the call.  Probe sets grow by prefix with
+ *              nprobe, so each position of a query's sorted top-k scores is non-decreasing in nprobe.
+ *   nprobe     >= 1; nprobe >= n_list runs the full search (atlas_b200_pq_topk / atlas_b200_ivfsq_topk) unchanged.
+ *
+ * Per block of <= 256 queries: one CTA per query selects P(q) (a radix select on (T, list id), then the extension),
+ * the lists some query probes are compacted into the sweep's work items, and their count stays in device memory: the
+ * scan and select grids are sized from an upper bound, so nothing synchronises with the host (graph-capturable).
+ * The candidate bound of the sampled path comes from each query's own best probed lists (their first max(512, k)
+ * positions, until they hold max(k, 4 k |P(q)| / capq) of its rows), so large probe sets do not overflow it.
+ * The list tables are trusted: they must describe the same layout as the codes (offsets non-decreasing from 0 to n,
+ * or to n_tiles for ivfsq; list_order a permutation of the rows).  Other tables can make the compaction write past
+ * its workspace.
+ *
+ * atlas_b200_pq_topk_probed / _exhaustive: the arguments of atlas_b200_pq_topk plus
+ *   list_order    device int32 [n]: the rows sorted by list id, stable (rows of a list ascending);
+ *   list_offsets  device int32 [n_list + 1]: list l holds list_order[list_offsets[l] .. list_offsets[l + 1]);
+ *   nprobe.       n_list must be >= 1.  A work item is 512 consecutive positions of one list.
+ * Workspace: atlas_b200_pq_workspace_bytes(ATLAS_B200_PQ_OP_SEARCH_PROBED, n, M, n_list, k) (0 when n_list < 1).
+ * -------------------------------------------------------------------------------------------- */
+int atlas_b200_pq_topk_probed(const uint8_t* codes, const void* list_ids, int64_t n, int32_t M, const float* codebooks,
+                              const float* coarse, int32_t n_list, const int32_t* list_order, const int32_t* list_offsets,
+                              int32_t nprobe, const void* queries, int32_t nq, int32_t k, void* out_scores,
+                              int64_t* out_ids, int64_t id_base, int64_t id_stride, int32_t* status, void* workspace,
+                              size_t workspace_bytes, void* stream);
+int atlas_b200_pq_topk_probed_exhaustive(const uint8_t* codes, const void* list_ids, int64_t n, int32_t M,
+                                         const float* codebooks, const float* coarse, int32_t n_list,
+                                         const int32_t* list_order, const int32_t* list_offsets, int32_t nprobe,
+                                         const void* queries, int32_t nq, int32_t k, void* out_scores, int64_t* out_ids,
+                                         int64_t id_base, int64_t id_stride, void* workspace, size_t workspace_bytes,
+                                         void* stream);
 
 /* --------------------------------------------------------------------------------------------
  * IVF-SQ passage index (csrc/pq.cu, csrc/ivfsq.cu): `DistributedFAISSIndex` with index_type ivfsq (faiss
@@ -185,6 +226,23 @@ int atlas_b200_ivfsq_topk_exhaustive(const uint8_t* codes, const int32_t* slot_r
                                      const float* vdiff, const void* queries, int32_t nq, int32_t k, void* out_scores,
                                      int64_t* out_ids, int64_t id_base, int64_t id_stride, void* workspace,
                                      size_t workspace_bytes, void* stream);
+/* atlas_b200_ivfsq_topk_probed / _exhaustive: the probed IVF search above over the ivfsq layout; the arguments of
+ * atlas_b200_ivfsq_topk plus
+ *   list_tile_off  device int32 [n_list + 1]: list l owns tiles list_tile_off[l] .. list_tile_off[l + 1];
+ *   list_rows      device int32 [n_list]: the real rows of list l;
+ *   nprobe.        A work item is one 64-slot tile; a 128-query group of the scan skips tiles none of its queries probes.
+ * Workspace: atlas_b200_ivfsq_workspace_bytes(ATLAS_B200_PQ_OP_SEARCH_PROBED, n_tiles * 64, n_list, k). */
+int atlas_b200_ivfsq_topk_probed(const uint8_t* codes, const int32_t* slot_rows, const int32_t* tile_lists, int64_t n_tiles,
+                                 int64_t n_rows, const int32_t* list_tile_off, const int32_t* list_rows, const float* coarse,
+                                 int32_t n_list, const float* vmin, const float* vdiff, int32_t nprobe, const void* queries,
+                                 int32_t nq, int32_t k, void* out_scores, int64_t* out_ids, int64_t id_base,
+                                 int64_t id_stride, int32_t* status, void* workspace, size_t workspace_bytes, void* stream);
+int atlas_b200_ivfsq_topk_probed_exhaustive(const uint8_t* codes, const int32_t* slot_rows, const int32_t* tile_lists,
+                                            int64_t n_tiles, int64_t n_rows, const int32_t* list_tile_off,
+                                            const int32_t* list_rows, const float* coarse, int32_t n_list, const float* vmin,
+                                            const float* vdiff, int32_t nprobe, const void* queries, int32_t nq, int32_t k,
+                                            void* out_scores, int64_t* out_ids, int64_t id_base, int64_t id_stride,
+                                            void* workspace, size_t workspace_bytes, void* stream);
 
 /* Exact re-ranking of PQ search candidates (csrc/pq_refine.cu; faiss IndexRefineFlat, `k_factor`): for every query,
  * the k_cand candidate rows are re-scored against their full-precision rows and the top k are returned.

@@ -18,6 +18,14 @@ of bench.py (4 Mi passages of 768-d fp16 per GPU, BASELINE configs[1]).  Prints 
                               tensor peak (the tensor bound binds at 256 queries, HBM at 8)
     python tools/perf_pq_index.py [--index-type ivfpq] [--code-size 16] [--rows N] [--steps 20] [--warmup 3]
                                   [--refine-factor 1]
+With --nprobe 8,32,128 it measures the probed search instead, for ivfpq (--code-size) and ivfsq on a seeded CLUSTERED
+bank (a Gaussian mixture: on an isotropic bank IVF recall means nothing; this is still not real embeddings): per index
+type, nprobe (and "all", the full scan) and batch of 8 and 256 queries, queries/s, recall@40 against the exact flat
+search, the fast path's overflow flag (`fast_path_status`; the timed search includes the exhaustive retry when it is
+set), and the sweep's kernel time against the HBM bound of the code bytes of the lists it had to read (the union of
+the block's probe sets, computed on the host from the coarse terms; the probe-set extension for small lists is ignored,
+it does not trigger at this shard size; a probed ivfpq row costs its 4-byte list position and a 32-byte sector per
+scattered code read).
 Writes nothing."""
 import argparse
 import json
@@ -161,6 +169,115 @@ def measure(args):
     } | ({"refine": refine} if refine else {}) | ({"ivfsq": ivfsq} if ivfsq else {})
 
 
+def clustered_bank(rows, dev, centers=4096, spread=0.35, seed=3):
+    """Seeded Gaussian mixture, rows and queries drawn alike, scaled like bench.make_bank's rows."""
+    import torch
+
+    g = torch.Generator(device=dev).manual_seed(seed)
+    c = torch.randn((centers, DIM), generator=g, device=dev)
+    bank = torch.empty((rows, DIM), dtype=torch.float16, device=dev)
+    for a in range(0, rows, 1 << 20):
+        b = min(rows, a + (1 << 20))
+        pick = torch.randint(0, centers, (b - a,), generator=g, device=dev)
+        bank[a:b] = ((c[pick] + spread * torch.randn((b - a, DIM), generator=g, device=dev)) / DIM ** 0.5).half()
+    pick = torch.randint(0, centers, (NQ,), generator=g, device=dev)
+    q = ((c[pick] + spread * torch.randn((NQ, DIM), generator=g, device=dev)) / DIM ** 0.5).half()
+    return bank, q
+
+
+def measure_nprobe(args):
+    import ctypes
+
+    import torch
+
+    from atlas_b200 import ops
+    from atlas_b200._lib import lib
+    from atlas_b200.index import DistributedFAISSIndex
+
+    dev = torch.device("cuda", 0)
+    torch.cuda.set_device(dev)
+    L = lib()
+    rows, steps, warmup = args.rows, args.steps, args.warmup
+    nprobes = [int(v) for v in args.nprobe.split(",")]
+    bank, q = clustered_bank(rows, dev)
+    _, exact, st = ops.mips_topk(bank, q, TOPK)
+    assert int(st.item()) == 0
+    exact = exact.cpu().numpy()
+    host = None
+    peak, peak_src = peaks("hbm")
+    out = {"metric": "probed IVF search (nprobe), top-40", "rows": rows, "steps": steps,
+           "bank": "seeded Gaussian mixture (4096 centres, spread 0.35): clustered, still not real embeddings",
+           "hbm_peak_GBps": peak, "peak_source": peak_src, "results": []}
+    for kind in ("ivfpq", "ivfsq"):
+        index = DistributedFAISSIndex(kind, args.code_size if kind == "ivfpq" else None)
+        if host is None:
+            host = index._host_rows(rows)
+            host.copy_(bank)
+            del bank
+            torch.cuda.empty_cache()
+        index._bank = host
+        index.train_index()
+        p = index._pq
+        n_list = p["n_list"]
+        if kind == "ivfsq":
+            tl = p["tile_lists"].to(torch.int64)
+            list_bytes = torch.bincount(tl, minlength=n_list).double() * ops.SQ_TILE * ops.SQ_CODE_BYTES
+        else:
+            # a probed ivfpq sweep reads each probed row's list position (4 B, in order) and then its codes through that
+            # permutation: scattered reads that each move whole 32-byte sectors
+            sector_bytes = (args.code_size + 31) // 32 * 32
+            list_bytes = torch.bincount(p["list_ids"].to(torch.int64), minlength=n_list).double() * (sector_bytes + 4)
+        T = q.float() @ p["coarse"].t()          # the coarse terms, up to the fp32 summation order
+        for nq in (8, NQ):
+            for nprobe in nprobes + [None]:
+                index.nprobe = nprobe
+                # the fast path's overflow flag, then the timed search: the final result, i.e. with the exhaustive retry
+                # (and the host synchronisation that reads the flag) whenever the flag is set, as search_knn runs it
+                status = int(index.search_device(q[:nq], TOPK, return_status=True)[2].item())
+                fn = lambda: index.search_device(q[:nq], TOPK)
+                for _ in range(warmup):
+                    fn()
+                e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+                L.atlas_b200_profile_enable(1)
+                e0.record()
+                for _ in range(steps):
+                    _, ids = fn()
+                e1.record()
+                torch.cuda.synchronize()
+                kms, kn = ctypes.c_double(0), ctypes.c_int32(0)
+                L.atlas_b200_profile_collect(ctypes.byref(kms), ctypes.byref(kn))
+                L.atlas_b200_profile_enable(0)
+                ms = e0.elapsed_time(e1) / steps
+                kernel_ms = kms.value / steps
+                if nprobe is None or nprobe >= n_list:
+                    read = float(list_bytes.sum()) if kind == "ivfsq" else float(rows * (args.code_size + 2))
+                else:
+                    union = torch.zeros(n_list, dtype=torch.bool, device=dev)
+                    union[torch.topk(T[:nq], nprobe, dim=1).indices.flatten()] = True
+                    read = float(list_bytes[union].sum())
+                    if kind == "ivfsq" and nq > 128:     # each 128-query group reads the lists its queries probe
+                        read = sum(float(list_bytes[torch.unique(torch.topk(T[g:g + 128], nprobe, dim=1).indices)].sum())
+                                   for g in range(0, nq, 128))
+                hbm_ms = read / (peak * 1e9) * 1e3
+                rec = float(sum(len(set(a) & set(b)) for a, b in zip(ids.cpu().numpy().tolist(), exact[:nq].tolist()))
+                            / (nq * TOPK))
+                out["results"].append({
+                    "index_type": kind, "n_list": n_list, "nprobe": nprobe if nprobe is not None else "all",
+                    "queries": nq, "value": nq / (ms * 1e-3), "unit": "queries/s", "ms_per_search": ms,
+                    "recall_at_40": rec, "fast_path_status": status, "sweep_kernel_ms": kernel_ms,
+                    "code_bytes_read": read, "hbm_bound_ms": hbm_ms,
+                    "frac_of_hbm_bound": hbm_ms / kernel_ms if kernel_ms > 0 else None})
+        index.nprobe = None
+        del index, p
+        torch.cuda.empty_cache()
+    try:
+        out["gpu"] = subprocess.run(["nvidia-smi", "--id=0", "--query-gpu=name,power.limit", "--format=csv,noheader"],
+                                    capture_output=True, text=True, timeout=30).stdout.strip()
+    except Exception:
+        out["gpu"] = None
+    return out
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--index-type", choices=["pq", "ivfpq", "ivfsq"], default="ivfpq")
@@ -170,7 +287,10 @@ def main():
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--refine-factor", type=int, default=1,
                     help="also time the search re-ranked over refine-factor x 40 PQ candidates (1 = off)")
-    print(json.dumps(measure(ap.parse_args())))
+    ap.add_argument("--nprobe", default=None,
+                    help="comma-separated nprobe values: measure the probed search of ivfpq and ivfsq instead")
+    args = ap.parse_args()
+    print(json.dumps(measure_nprobe(args) if args.nprobe else measure(args)))
 
 
 if __name__ == "__main__":
