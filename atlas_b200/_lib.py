@@ -210,6 +210,14 @@ def lib():
     L.atlas_b200_ivfsq_topk_probed_exhaustive.restype = c.c_int
     L.atlas_b200_ivfsq_topk_probed_exhaustive.argtypes = [vp, vp, vp, i64, i64, vp, vp, vp, i32, vp, vp, i32, vp, i32, i32,
                                                           vp, vp, i64, i64, vp, c.c_size_t, vp]
+    L.atlas_b200_ivfflat_workspace_bytes.restype = c.c_size_t
+    L.atlas_b200_ivfflat_workspace_bytes.argtypes = [i32, i64, i32, i32]
+    L.atlas_b200_ivfflat_topk.restype = c.c_int
+    L.atlas_b200_ivfflat_topk.argtypes = [vp, vp, i64, i64, vp, vp, vp, i32, i32, vp, i32, i32, vp, vp, i64, i64, vp, vp,
+                                          c.c_size_t, vp]
+    L.atlas_b200_ivfflat_topk_exhaustive.restype = c.c_int
+    L.atlas_b200_ivfflat_topk_exhaustive.argtypes = [vp, vp, i64, i64, vp, vp, vp, i32, i32, vp, i32, i32, vp, vp, i64, i64,
+                                                     vp, c.c_size_t, vp]
     L.atlas_b200_pq_refine_workspace_bytes.restype = c.c_size_t
     L.atlas_b200_pq_refine_workspace_bytes.argtypes = [i32, i32]
     L.atlas_b200_pq_refine_topk.restype = c.c_int
@@ -289,6 +297,9 @@ EXPORTED_SYMBOLS = [
     "atlas_b200_ivfsq_topk_exhaustive",
     "atlas_b200_ivfsq_topk_probed",
     "atlas_b200_ivfsq_topk_probed_exhaustive",
+    "atlas_b200_ivfflat_workspace_bytes",
+    "atlas_b200_ivfflat_topk",
+    "atlas_b200_ivfflat_topk_exhaustive",
     "atlas_b200_pq_refine_workspace_bytes",
     "atlas_b200_pq_refine_topk",
     "atlas_b200_quantize_kv_e4m3",

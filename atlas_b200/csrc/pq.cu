@@ -22,8 +22,11 @@
 // sweep; a row's codes are read once per query group.
 //
 // The IVF-SQ index (type ivfsq) shares the coarse k-means, the coarse assignment and the top-k driver: its training,
-// encoding and search host code are at the end of this file, its scan kernel in ivfsq.cu.
+// encoding and search host code are at the end of this file, its scan kernel in ivfsq.cu.  The IVF-Flat index (types
+// ivfflat and flat) trains with ivfsq's entry point (coarse quantizer only) and shares the driver and the probe
+// selection; its search host code follows ivfsq's, its scan kernel is in ivfflat.cu.
 #include "ivf_probe.cuh"
+#include "ivfflat.cuh"
 #include "ivfsq.cuh"
 #include "mips_select.cuh"
 
@@ -1120,7 +1123,7 @@ static size_t sq_search_bytes(int64_t n_slots, int n_list, int k, SqSearchWs* w,
 
 static int sq_train(const __half* sample, int64_t S, int n_list, int iters, float* coarse, float* vmin, float* vdiff, void* ws,
                     size_t ws_bytes, cudaStream_t s) {
-    AB_REQUIRE(sample != nullptr && coarse != nullptr && vmin != nullptr && vdiff != nullptr, "null pointer argument");
+    AB_REQUIRE(sample != nullptr && coarse != nullptr && (vmin == nullptr) == (vdiff == nullptr), "null pointer argument");
     AB_REQUIRE(n_list >= 1, "n_list=%d must be >= 1", n_list);
     AB_REQUIRE(S >= n_list && S < (1ll << 31), "training needs at least n_list=%d rows (got %lld)", n_list, (long long)S);
     AB_REQUIRE(iters >= 0, "iters=%d must be >= 0", iters);
@@ -1135,6 +1138,7 @@ static int sq_train(const __half* sample, int64_t S, int n_list, int iters, floa
     const int64_t R = sq_chunk_rows(n_list);
     int rc = coarse_kmeans(sample, S, n_list, iters, coarse, w, R, assign, counts, s);
     if (rc) return rc;
+    if (vmin == nullptr) return ATLAS_B200_OK;      // the coarse quantizer alone (ivfflat)
     const int64_t ns = S < SQ_RANGE_MAX ? S : SQ_RANGE_MAX;
     if ((rc = coarse_assign(sample, ns, w.coarse16, n_list, w, R, assign, nullptr, 0, s))) return rc;
     const int parts = static_cast<int>((ns + SQ_RANGE_ROWS - 1) / SQ_RANGE_ROWS);
@@ -1262,6 +1266,135 @@ static int sq_topk(const uint8_t* codes, const int32_t* slot_rows, const int32_t
         // work = code bytes swept (once per 128 queries of the block)
         const double sweep_bytes = static_cast<double>(n_slots) * ivfsq::SQ_CODE_BYTES * ((nqb + 127) / 128);
         if ((rc = sweep_select(scan, n_slots, static_cast<int>(n_tiles), ivfsq::SQ_TILE, nqb, k, w.cand, w.count, w.bound,
+                               w.capq, os16, oi_b, id_base, id_stride, status, exhaustive, sweep_bytes, s)))
+            return rc;
+    }
+    AB_CUDA_CHECK(cudaGetLastError());
+    return ATLAS_B200_OK;
+}
+
+// ---------------------------------------------------------------------------------------------
+// IVF-Flat search (types ivfflat and flat): the scan kernel is in ivfflat.cu
+// ---------------------------------------------------------------------------------------------
+// Per query row q of a block (one CTA each, rows past nq are zero): the fp16 row for the scan's TMA, its fp32 copy for
+// the coarse terms; resets the block's candidate counters and bounds.
+__global__ void __launch_bounds__(256) flat_query_kernel(const __half* __restrict__ q16, int nq, __half* __restrict__ qstage,
+                                                         float* __restrict__ qf32, uint32_t* __restrict__ count,
+                                                         float* __restrict__ bound) {
+    const int q = blockIdx.x;
+    for (int d = threadIdx.x; d < DIM; d += blockDim.x) {
+        const __half h = q < nq ? q16[static_cast<int64_t>(q) * DIM + d] : __float2half_rn(0.f);
+        qstage[static_cast<int64_t>(q) * DIM + d] = h;
+        qf32[static_cast<int64_t>(q) * DIM + d] = __half2float(h);
+    }
+    if (threadIdx.x == 0) {
+        count[q] = 0;
+        bound[q] = -INFINITY;
+    }
+}
+
+struct FlatSearchWs {
+    uint32_t* count;
+    float* bound;
+    uint64_t* cand;
+    uint32_t capq;
+    __half* qstage;  // [QBLOCK][768]
+    float* qf32;     // [QBLOCK][768]
+    float* tterm;    // [n_list][nqb] (probed search only)
+};
+
+static size_t flat_search_bytes(int64_t n_slots, int n_list, int k, bool probed, FlatSearchWs* w, void* base) {
+    Carver cv{static_cast<uint8_t*>(base)};
+    const uint32_t capq = mips::capq_for(n_slots, k);
+    FlatSearchWs x;
+    x.count = cv.take<uint32_t>(QBLOCK);
+    x.bound = cv.take<float>(QBLOCK);
+    x.cand = cv.take<uint64_t>(static_cast<size_t>(QBLOCK) * capq);
+    x.capq = capq;
+    x.qstage = cv.take<__half>(static_cast<size_t>(QBLOCK) * DIM);
+    x.qf32 = cv.take<float>(static_cast<size_t>(QBLOCK) * DIM);
+    x.tterm = cv.take<float>(probed ? static_cast<size_t>(n_list) * QBLOCK : 0);
+    if (w) *w = x;
+    return cv.off;
+}
+
+// nprobe = 0 or >= n_list: every tile (list tables and coarse unused, may be NULL); else the probed search.
+static int flat_topk(const __half* rows, const int32_t* slot_rows, int64_t n_tiles, int64_t n_rows, const int32_t* list_tile_off,
+                     const int32_t* list_rows, const float* coarse, int n_list, int nprobe, const __half* queries, int nq, int k,
+                     __half* out_scores, int64_t* out_ids, int64_t id_base, int64_t id_stride, int32_t* status, void* ws,
+                     size_t ws_bytes, cudaStream_t s, bool exhaustive) {
+    AB_REQUIRE(nq >= 0 && k >= 1, "nq must be >= 0 and k >= 1 (nq=%d k=%d)", nq, k);
+    AB_REQUIRE(k <= ATLAS_B200_MAX_TOPK, "k=%d exceeds ATLAS_B200_MAX_TOPK=%d", k, ATLAS_B200_MAX_TOPK);
+    AB_REQUIRE(n_list >= 1, "n_list=%d must be >= 1", n_list);
+    AB_REQUIRE(nprobe >= 0, "nprobe=%d must be >= 1 (or 0 for every list)", nprobe);
+    AB_REQUIRE(n_rows >= 1 && n_tiles >= 1 && n_rows <= n_tiles * ivfflat::FLAT_TILE &&
+                   n_tiles * ivfflat::FLAT_TILE < (1ll << 31) - ivfflat::FLAT_TILE,
+               "rows n=%lld / tiles %lld out of range", (long long)n_rows, (long long)n_tiles);
+    AB_REQUIRE(k <= n_rows, "selected index k out of range: k=%d > n=%lld", k, (long long)n_rows);
+    AB_REQUIRE(rows != nullptr && slot_rows != nullptr, "null pointer argument");
+    AB_REQUIRE(abh::aligned(rows, 16), "rows must be 16-byte aligned");
+    const bool probed = nprobe > 0 && nprobe < n_list;
+    AB_REQUIRE(!probed || (coarse != nullptr && list_tile_off != nullptr && list_rows != nullptr),
+               "a probed search needs coarse, list_tile_off and list_rows");
+    AB_REQUIRE(nq == 0 || queries != nullptr, "queries is null");
+    if (status) AB_CUDA_CHECK(cudaMemsetAsync(status, 0, sizeof(int32_t), s));
+    if (nq == 0) return ATLAS_B200_OK;
+    FlatSearchWs w;
+    ProbeWs pw{};
+    const int64_t n_slots = n_tiles * ivfflat::FLAT_TILE;
+    size_t need = flat_search_bytes(n_slots, n_list, k, probed, &w, ws);
+    if (probed) need = probe_bytes(need, n_list, n_tiles, k, ivfflat::FLAT_TILE, &pw, ws);
+    if (ws == nullptr || ws_bytes < need) {
+        abh::set_error("workspace too small: have %zu need %zu", ws_bytes, need);
+        return ATLAS_B200_EWORKSPACE;
+    }
+    int rc;
+    for (int q0 = 0; q0 < nq; q0 += QBLOCK) {
+        const int nqb = nq - q0 < QBLOCK ? nq - q0 : QBLOCK;
+        flat_query_kernel<<<QBLOCK, 256, 0, s>>>(queries + static_cast<int64_t>(q0) * DIM, nqb, w.qstage, w.qf32, w.count,
+                                                 w.bound);
+        abh::count_launch();
+        ivfflat::ScanParams p;
+        p.rows = rows;
+        p.slot_rows = slot_rows;
+        p.n_tiles = static_cast<int>(n_tiles);
+        p.qstage = w.qstage;
+        p.nq = nqb;
+        p.bound = w.bound;
+        p.count = w.count;
+        p.cand = w.cand;
+        p.capq = w.capq;
+        int64_t* oi_b = out_ids + static_cast<size_t>(q0) * k;
+        uint16_t* os16 = reinterpret_cast<uint16_t*>(out_scores + static_cast<size_t>(q0) * k);
+        if (probed) {
+            // T[l][q] = <c_l, q> (ivfsq's coarse terms), P(q) and its sample lists, then the tiles of every list some
+            // query probes and the sample tiles
+            if ((rc = subdot(coarse, DIM, n_list, w.qf32, nqb, DIM, 1, w.tterm, s))) return rc;
+            if ((rc = ivfp::select_probes(w.tterm, 1, nqb, nqb, n_list, nullptr, list_rows, nprobe, k, w.capq,
+                                          pw.sample_units * ivfflat::FLAT_TILE, pw.probed, pw.sample_lists, s)))
+                return rc;
+            if ((rc = ivfp::compact_items(pw.probed, pw.sample_lists, list_tile_off, n_list, 1, pw.sample_units, pw.items,
+                                          pw.sample, pw.count, s)))
+                return rc;
+        }
+        const ivfsq::ProbeScan pr{pw.items, pw.count, pw.probed};
+        const ivfsq::ProbeScan ps{pw.sample, pw.count + 1, pw.probed};
+        auto scan = [&](int tile_begin, int tile_step, int num_tiles, bool sample) {
+            p.tile_begin = tile_begin;
+            p.tile_step = tile_step;
+            p.num_tiles = num_tiles;
+            if (!probed) return ivfflat::launch_scan(p, nullptr, s);
+            if (sample) {     // the bound's scan: every sample tile (ivf_probe.cuh), not a stride over the sweep
+                p.tile_begin = 0;
+                p.tile_step = 1;
+                p.num_tiles = static_cast<int>(pw.max_sample);
+                return ivfflat::launch_scan(p, &ps, s);
+            }
+            return ivfflat::launch_scan(p, &pr, s);
+        };
+        // work = row bytes swept (once per block)
+        const double sweep_bytes = static_cast<double>(n_slots) * DIM * 2;
+        if ((rc = sweep_select(scan, n_slots, static_cast<int>(n_tiles), ivfflat::FLAT_TILE, nqb, k, w.cand, w.count, w.bound,
                                w.capq, os16, oi_b, id_base, id_stride, status, exhaustive, sweep_bytes, s)))
             return rc;
     }
@@ -1410,6 +1543,40 @@ int atlas_b200_ivfsq_topk_probed_exhaustive(const uint8_t* codes, const int32_t*
     return pq::sq_topk(codes, slot_rows, tile_lists, n_tiles, n_rows, coarse, n_list, vmin, vdiff,
                        static_cast<const __half*>(queries), nq, k, static_cast<__half*>(out_scores), out_ids, id_base,
                        id_stride, nullptr, workspace, workspace_bytes, static_cast<cudaStream_t>(stream), true, &probe);
+}
+
+size_t atlas_b200_ivfflat_workspace_bytes(int32_t op, int64_t n_slots, int32_t n_list, int32_t k) {
+    if (n_list < 1) return 0;
+    if (n_slots < 1) n_slots = 1;
+    if (k < 1) k = 1;
+    switch (op) {
+        case ATLAS_B200_PQ_OP_SEARCH: return pq::flat_search_bytes(n_slots, n_list, k, false, nullptr, nullptr);
+        case ATLAS_B200_PQ_OP_SEARCH_PROBED:
+            return pq::probe_bytes(pq::flat_search_bytes(n_slots, n_list, k, true, nullptr, nullptr), n_list,
+                                   (n_slots + ivfflat::FLAT_TILE - 1) / ivfflat::FLAT_TILE, k, ivfflat::FLAT_TILE, nullptr,
+                                   nullptr);
+        default: return 0;
+    }
+}
+
+int atlas_b200_ivfflat_topk(const void* rows, const int32_t* slot_rows, int64_t n_tiles, int64_t n_rows,
+                            const int32_t* list_tile_off, const int32_t* list_rows, const float* coarse, int32_t n_list,
+                            int32_t nprobe, const void* queries, int32_t nq, int32_t k, void* out_scores, int64_t* out_ids,
+                            int64_t id_base, int64_t id_stride, int32_t* status, void* workspace, size_t workspace_bytes,
+                            void* stream) {
+    return pq::flat_topk(static_cast<const __half*>(rows), slot_rows, n_tiles, n_rows, list_tile_off, list_rows, coarse, n_list,
+                         nprobe, static_cast<const __half*>(queries), nq, k, static_cast<__half*>(out_scores), out_ids, id_base,
+                         id_stride, status, workspace, workspace_bytes, static_cast<cudaStream_t>(stream), false);
+}
+
+int atlas_b200_ivfflat_topk_exhaustive(const void* rows, const int32_t* slot_rows, int64_t n_tiles, int64_t n_rows,
+                                       const int32_t* list_tile_off, const int32_t* list_rows, const float* coarse,
+                                       int32_t n_list, int32_t nprobe, const void* queries, int32_t nq, int32_t k,
+                                       void* out_scores, int64_t* out_ids, int64_t id_base, int64_t id_stride, void* workspace,
+                                       size_t workspace_bytes, void* stream) {
+    return pq::flat_topk(static_cast<const __half*>(rows), slot_rows, n_tiles, n_rows, list_tile_off, list_rows, coarse, n_list,
+                         nprobe, static_cast<const __half*>(queries), nq, k, static_cast<__half*>(out_scores), out_ids, id_base,
+                         id_stride, nullptr, workspace, workspace_bytes, static_cast<cudaStream_t>(stream), true);
 }
 
 }  // extern "C"

@@ -15,8 +15,8 @@ Same public surface: `embeddings` ([768, N] fp16 CUDA, slice-assignable on dim 1
   * ties are ordered canonically: score descending, then global passage id ascending.
 
 There is no CPU path: `is_in_gpu = False` raises here.  `DistributedFAISSIndex` (below) is the reference's
-`--index_mode faiss` with host-resident rows and a product-quantized (csrc/pq.cu) or 4-bit scalar-quantized
-(csrc/ivfsq.cu) device index.
+`--index_mode faiss` with host-resident rows and a product-quantized (csrc/pq.cu), 4-bit scalar-quantized
+(csrc/ivfsq.cu) or full-precision inverted-list (csrc/ivfflat.cu) device index.
 """
 import ctypes
 import logging
@@ -319,12 +319,12 @@ class DistributedIndex(object):
 
 
 def _check_nprobe(index_type, nprobe):
-    """nprobe: None (every list) or an int >= 1 (not a bool), and None for type pq, which has no lists."""
+    """nprobe: None (every list) or an int >= 1 (not a bool), and None for types pq and flat, which have no lists."""
     if nprobe is not None and (isinstance(nprobe, bool) or not isinstance(nprobe, int) or nprobe < 1):
         raise AtlasB200Error(f"DistributedFAISSIndex: nprobe={nprobe!r} must be None (every list) or an integer >= 1")
-    if nprobe is not None and index_type == "pq":
-        raise AtlasB200Error(f"DistributedFAISSIndex('pq'): nprobe={nprobe!r} needs inverted lists; index type pq has none "
-                             "(use ivfpq or ivfsq, or nprobe=None)")
+    if nprobe is not None and index_type in ("pq", "flat"):
+        raise AtlasB200Error(f"DistributedFAISSIndex({index_type!r}): nprobe={nprobe!r} needs inverted lists; index type "
+                             f"{index_type} has none (use ivfpq, ivfsq or ivfflat, or nprobe=None)")
     return nprobe
 
 
@@ -367,18 +367,31 @@ class DistributedFAISSIndex(DistributedIndex):
     padded to a multiple of 64 slots; the index file holds the codes in row order and faiss's packing, with the list
     ids, and `load_index` rebuilds the slot layout from them.  Training needs one row.
 
-    Probing (faiss's `nprobe`, opt-in, ivfpq and ivfsq): with `nprobe` an int >= 1 (a constructor keyword and a plain
-    attribute that may be set at any time; Atlas sets it from `--faiss_nprobe`) each query is scored only against the
+    index_type "ivfflat" (faiss IndexIVFFlat, inner product): the ivfpq coarse quantizer and the full-precision rows on
+    the device in ivfsq's inverted-list slot layout (fp16 rows in place of codes, csrc/ivfflat.cu): 1536 bytes of row and
+    a 4-byte row id per slot, every list padded to a multiple of 64 slots.  Its scores are the flat index's, bit for bit:
+    the inner product of the fp16 query and row, accumulated in fp32 and rounded once to fp16, with no coarse term; with
+    `nprobe` it scores only the rows of each query's best lists, so it loses recall on the lists it skips and no precision
+    on the lists it scans.  An IVF-Flat index has no code: `code_size` must be None.  `refine_factor` is accepted and
+    ignored (the scores are already exact), as the flat index ignores `--faiss_refine_factor`.  The index file holds the
+    coarse centroids and the row-order list ids, and `load_index` rebuilds the slot layout from the shards' rows.
+    Training needs one row.
+    index_type "flat" (faiss IndexFlatIP, the reference's default `--faiss_index_type`): ivfflat with one list and no
+    k-means - the rows in row order, padded to a multiple of 64 - always fully scanned; a non-None `nprobe` raises.  Its
+    results are `DistributedIndex.search_knn`'s, with the rows kept in host memory between trainings.
+
+    Probing (faiss's `nprobe`, opt-in, ivfpq, ivfsq and ivfflat): with `nprobe` an int >= 1 (a constructor keyword and a
+    plain attribute that may be set at any time; Atlas sets it from `--faiss_nprobe`) each query is scored only against the
     rows of its best lists: the shortest prefix of the lists ordered by the coarse term <q, c_l> (descending, then list
     id) that has at least `nprobe` lists and holds at least k rows (faiss would return id -1 when the probed lists hold
     fewer than k rows instead; see include/atlas_b200.h).  The result is the exact top-k over those rows, and the sweep
     reads only the codes of lists some query of the block probes.  None (default) or nprobe >= n_list scans every row,
-    as before.  Type pq has no lists: a non-None value raises.  Refinement composes (the probed search supplies the k'
-    candidates).  ivfpq keeps its codes in row order and reads them through a list-order permutation built on the first
+    as before.  Types pq and flat have no lists: a non-None value raises.  Refinement composes (the probed search supplies
+    the k' candidates).  ivfpq keeps its codes in row order and reads them through a list-order permutation built on the first
     probed search: +4 bytes per row of device memory from then on, dropped with the index on retraining or
     `mark_stale()`.  `nprobe` is not written to the index file."""
 
-    SUPPORTED_TYPES = ("pq", "ivfpq", "ivfsq")
+    SUPPORTED_TYPES = ("pq", "ivfpq", "ivfsq", "ivfflat", "flat")
     FILE_FORMAT = 1
     TRAIN_SEED = 1234
     STAGE_ROWS = 65536
@@ -389,8 +402,15 @@ class DistributedFAISSIndex(DistributedIndex):
             raise AtlasB200Error(
                 f"DistributedFAISSIndex: index_type={index_type!r} is not provided by atlas_b200; supported types are "
                 f"{', '.join(self.SUPPORTED_TYPES)}.  For exact search use --index_mode flat "
-                "(atlas_b200.index.DistributedIndex): flat and ivfflat with nprobe = n_list are exact anyway")
-        if index_type == "ivfsq":
+                "(atlas_b200.index.DistributedIndex)")
+        if index_type in ("ivfflat", "flat"):
+            # checked before the device, so that the error does not depend on the machine
+            if code_size is not None:
+                raise AtlasB200Error(f"DistributedFAISSIndex({index_type!r}): code_size={code_size!r}, but an {index_type} "
+                                     "index stores full-precision rows and has no code: pass None (--faiss_code_size "
+                                     "unset).  For the exact search with the rows on the device use --index_mode flat "
+                                     "(atlas_b200.index.DistributedIndex)")
+        elif index_type == "ivfsq":
             # faiss's SQ4 naming: code_size is bits per dimension; the reference builds QT_4bit whatever its value
             if code_size is not None and (isinstance(code_size, bool) or code_size != ops.SQ_BITS):
                 raise AtlasB200Error(f"DistributedFAISSIndex('ivfsq'): code_size={code_size!r} is bits per dimension and "
@@ -407,7 +427,8 @@ class DistributedFAISSIndex(DistributedIndex):
         self.code_size = None if code_size is None else int(code_size)
         self.is_in_gpu = False
         # the trained index: dict(codebooks, coarse, codes, list_ids, n_list) for pq / ivfpq;
-        # dict(coarse, vmin, vdiff, codes, slot_rows, tile_lists, n_list) in the device slot layout for ivfsq
+        # dict(coarse, vmin, vdiff, codes, slot_rows, tile_lists, n_list) in the device slot layout for ivfsq;
+        # dict(coarse (None for flat), rows, slot_rows, tile_lists, n_list) in the same layout for ivfflat / flat
         self._pq = None
         self.refine_factor = refine_factor
         self._refine_factor()
@@ -463,11 +484,13 @@ class DistributedFAISSIndex(DistributedIndex):
 
     def n_list(self, n_rows=None):
         n = self._bank.shape[0] if n_rows is None else n_rows
-        return int(math.floor(math.sqrt(n))) if self.index_type in ("ivfpq", "ivfsq") else 0
+        if self.index_type == "flat":
+            return 1
+        return int(math.floor(math.sqrt(n))) if self.index_type in ("ivfpq", "ivfsq", "ivfflat") else 0
 
     def _min_train_rows(self):
-        """faiss's k-means needs 256 points per PQ centroid; IVF-SQ needs one row per list, i.e. one row."""
-        return 1 if self.index_type == "ivfsq" else ops.PQ_KSUB
+        """faiss's k-means needs 256 points per PQ centroid; IVF-SQ and IVF-Flat need one row per list, i.e. one row."""
+        return ops.PQ_KSUB if self.index_type in ("pq", "ivfpq") else 1
 
     def train_index(self):
         """Train the quantizers on the current rows and encode every row (src/index.py:352-381 trains + adds)."""
@@ -480,6 +503,8 @@ class DistributedFAISSIndex(DistributedIndex):
         self._pq = None
         if self.index_type == "ivfsq":
             self._pq = self._train_and_encode_sq(self._bank, n)
+        elif self.index_type in ("ivfflat", "flat"):
+            self._pq = self._train_flat(self._bank, n)
         else:
             self._pq = self._train_and_encode(self._bank, n)
 
@@ -532,6 +557,38 @@ class DistributedFAISSIndex(DistributedIndex):
         return dict(coarse=coarse, vmin=vmin, vdiff=vdiff, codes=codes, slot_rows=slot_rows, tile_lists=tile_lists,
                     n_list=n_list)
 
+    def _train_flat(self, rows, n):
+        """IVF-Flat: the coarse k-means of ivfpq / ivfsq on the same seeded sample rows, the rows' lists; type flat puts
+        every row in list 0 without k-means."""
+        device = self._device()
+        n_list = self.n_list(n)
+        lists = torch.zeros(n, dtype=torch.int32, device=device)
+        coarse = None
+        if self.index_type == "ivfflat":
+            sample = self._sample(rows, n, min(n, ops.PQ_KSUB * n_list), device)
+            coarse = ops.ivfflat_train(sample, n_list)
+            del sample
+            ws = ops.Workspace()
+            self._stream_rows(rows, n, device, lambda st, a, b: ops.ivf_list_ids(st, coarse, lists[a:b], ws))
+        return self._flat_layout(rows, n, coarse, lists, n_list)
+
+    def _flat_layout(self, rows, n, coarse, lists, n_list):
+        """The slot layout of the list ids `lists` (ivfsq's), then the pinned host rows scattered into their slots."""
+        device = self._device()
+        slot_rows, tile_lists, row_slot = ops.ivfsq_layout(lists, n_list)
+        del lists
+        dev_rows = torch.zeros((slot_rows.numel(), EMBEDDINGS_DIM), dtype=torch.float16, device=device)
+        self._stream_rows(rows, n, device,
+                          lambda st, a, b: dev_rows.index_copy_(0, row_slot[a:b].to(torch.int64), st))
+        return dict(coarse=coarse, rows=dev_rows, slot_rows=slot_rows, tile_lists=tile_lists, n_list=n_list)
+
+    def _flat_list_ids(self, p, n):
+        """Row-order list ids of the IVF-Flat layout."""
+        slots = torch.nonzero(p["slot_rows"] >= 0).flatten()
+        lists = torch.empty(n, dtype=torch.int32, device=slots.device)
+        lists[p["slot_rows"][slots].to(torch.int64)] = p["tile_lists"][slots // ops.SQ_TILE]
+        return lists
+
     # ------------------------------------------------------------------ search
     def _trained(self):
         if self._pq is None:
@@ -551,7 +608,7 @@ class DistributedFAISSIndex(DistributedIndex):
         """The list tables of a probed search, built on the first one and kept in the trained index (dropped with it)."""
         if nprobe is None or nprobe >= p["n_list"]:
             return {}
-        if self.index_type == "ivfsq":
+        if self.index_type in ("ivfsq", "ivfflat"):
             if "list_tile_off" not in p:
                 p["list_tile_off"], p["list_rows"] = ops.ivfsq_list_tables(p["slot_rows"], p["tile_lists"], p["n_list"])
             return dict(list_tile_off=p["list_tile_off"], list_rows=p["list_rows"])
@@ -562,7 +619,7 @@ class DistributedFAISSIndex(DistributedIndex):
     def _local_search(self, allqueries, topk, exhaustive=False):
         self._nprobe()
         r = self._refine_factor()
-        if r == 1:
+        if r == 1 or self.index_type in ("ivfflat", "flat"):     # the scores are exact already: nothing to refine
             return self._candidate_search(allqueries, topk, self._id_base, self._id_stride, exhaustive)
         k_cand = min(topk * r, int(self._bank.shape[0]))
         if k_cand > MAX_TOPK:
@@ -573,10 +630,14 @@ class DistributedFAISSIndex(DistributedIndex):
         return s, i, status
 
     def _candidate_search(self, allqueries, k, id_base, id_stride, exhaustive):
-        """Top k by PQ score: (scores, ids = id_base + id_stride * row, device status word)."""
+        """Top k by the index's score: (scores, ids = id_base + id_stride * row, device status word)."""
         p = self._trained()
         nprobe = self._nprobe()
         tables = self._probe_tables(p, nprobe)
+        if self.index_type in ("ivfflat", "flat"):
+            return ops.ivfflat_topk(p["rows"], p["slot_rows"], p["tile_lists"], int(self._bank.shape[0]), p["coarse"],
+                                    allqueries, k, id_base, id_stride, self._workspace, exhaustive=exhaustive, nprobe=nprobe,
+                                    **tables)
         if self.index_type == "ivfsq":
             return ops.ivfsq_topk(p["codes"], p["slot_rows"], p["tile_lists"], int(self._bank.shape[0]), p["coarse"],
                                   p["vmin"], p["vdiff"], allqueries, k, id_base, id_stride, self._workspace,
@@ -608,6 +669,12 @@ class DistributedFAISSIndex(DistributedIndex):
             return
         p = self._pq
         cpu = lambda t: None if t is None else t.cpu()
+        if self.index_type in ("ivfflat", "flat"):
+            n = int(self._bank.shape[0])
+            torch.save(dict(format=self.FILE_FORMAT, index_type=self.index_type, code_size=self.code_size,
+                            n_list=p["n_list"], n_rows=n, coarse=cpu(p["coarse"]), list_ids=cpu(self._flat_list_ids(p, n))),
+                       self._get_index_filename(path))
+            return
         if self.index_type == "ivfsq":
             codes, lists = ops.ivfsq_export(p["codes"], p["slot_rows"], p["tile_lists"], int(self._bank.shape[0]))
             torch.save(dict(format=self.FILE_FORMAT, index_type=self.index_type, code_size=self.code_size,
@@ -633,6 +700,12 @@ class DistributedFAISSIndex(DistributedIndex):
                     and d.get("n_list") == self.n_list(n)):
                 dev = self._device()
                 to = lambda t: None if t is None else t.to(dev)
+                if self.index_type in ("ivfflat", "flat"):
+                    lists = to(d["list_ids"]).to(torch.int32).contiguous()
+                    if tuple(lists.shape) != (n,):
+                        raise AtlasB200Error(f"{f}: list_ids must hold {n} entries, got {tuple(lists.shape)}")
+                    self._pq = self._flat_layout(self._bank, n, to(d["coarse"]), lists, int(d["n_list"]))
+                    return
                 if self.index_type == "ivfsq":
                     codes, slot_rows, tile_lists = ops.ivfsq_import(to(d["codes"]), to(d["list_ids"]), int(d["n_list"]))
                     self._pq = dict(coarse=to(d["coarse"]), vmin=to(d["vmin"]), vdiff=to(d["vdiff"]), codes=codes,

@@ -520,6 +520,97 @@ def ivfsq_topk(codes, slot_rows, tile_lists, n_rows, coarse, vmin, vdiff, querie
 
 
 # ---------------------------------------------------------------------------------------------
+# IVF-Flat index (csrc/pq.cu, csrc/ivfflat.cu): ivfsq's slot layout with fp16 rows in place of codes
+# ---------------------------------------------------------------------------------------------
+def ivfflat_train(sample, n_list, iters=PQ_ITERS):
+    """The coarse quantizer alone (atlas_b200_ivfsq_train with vmin = vdiff = NULL): bit-identical to the ivfpq / ivfsq
+    one on the same sample.  sample: CUDA fp16 [S, 768] in a seeded random order, S >= n_list.  Returns fp32 [n_list, 768]."""
+    require_cuda(sample, "sample")
+    s = sample.reshape(-1, DIM).to(torch.float16).contiguous()
+    if n_list < 1 or s.shape[0] < n_list:
+        raise AtlasB200Error(f"ivfflat_train: need 1 <= n_list <= sample rows (n_list={n_list}, rows={s.shape[0]})")
+    coarse = torch.empty((n_list, DIM), dtype=torch.float32, device=s.device)
+    ws = torch.empty(int(lib().atlas_b200_ivfsq_workspace_bytes(PQ_OP_TRAIN, s.shape[0], n_list, 1)), dtype=torch.uint8,
+                     device=s.device)
+    check(lib().atlas_b200_ivfsq_train(_ptr(s), s.shape[0], n_list, iters, _ptr(coarse), None, None, _ptr(ws), ws.numel(),
+                                       current_stream_ptr()))
+    return coarse
+
+
+def ivf_list_ids(rows, coarse, list_ids, workspace=None):
+    """The coarse list (inner product, lowest list on ties) of every CUDA fp16 row [n, 768] into `list_ids` int32 [n]
+    (atlas_b200_ivfsq_encode without codes)."""
+    require_cuda(rows, "rows")
+    require_cuda(coarse, "coarse")
+    r = rows.reshape(-1, DIM)
+    n = r.shape[0]
+    if r.dtype != torch.float16 or not r.is_contiguous():
+        raise AtlasB200Error("ivf_list_ids: rows must be contiguous fp16 [n, 768]")
+    if coarse.dtype != torch.float32 or coarse.dim() != 2 or coarse.shape[1] != DIM or not coarse.is_contiguous():
+        raise AtlasB200Error(f"ivf_list_ids: coarse must be contiguous fp32 [n_list, {DIM}]")
+    if list_ids.dtype != torch.int32 or list_ids.shape != (n,) or not list_ids.is_contiguous():
+        raise AtlasB200Error(f"ivf_list_ids: list_ids must be contiguous int32 [{n}]")
+    n_list = coarse.shape[0]
+    buf = (workspace or _default_ws).get(lib().atlas_b200_ivfsq_workspace_bytes(PQ_OP_ENCODE, n, n_list, 1), r.device)
+    check(lib().atlas_b200_ivfsq_encode(_ptr(r), n, _ptr(coarse), n_list, None, None, _ptr(list_ids), None, None, _ptr(buf),
+                                        buf.numel(), current_stream_ptr()))
+    return list_ids
+
+
+def ivfflat_topk(rows, slot_rows, tile_lists, n_rows, coarse, queries, k, id_base=0, id_stride=1, workspace=None,
+                 exhaustive=False, nprobe=None, list_tile_off=None, list_rows=None):
+    """Top-k of the exact inner products (the flat index's fp16 scores) of `queries` [nq, 768] over one shard's rows in
+    the IVF-Flat slot layout (atlas_b200_ivfflat_topk): rows CUDA fp16 [64 * tiles, 768] (padding slots zero),
+    slot_rows int32 [slots], tile_lists int32 [tiles] (`ivfsq_layout`).  Returns (scores [nq, k] fp16 desc, ids [nq, k]
+    int64, status int32[1]) like `mips_topk`.
+    coarse None is type flat: one list, always the full scan, and nprobe must be None.  nprobe < n_list: only the rows of
+    each query's best lists, with the tables of `ivfsq_list_tables`; None or >= n_list scans every slot.  The probed
+    search does not synchronise with the host when the tables are passed; built here (when not given) they cost a host
+    synchronisation (torch.bincount) per call."""
+    require_cuda(rows, "rows")
+    check_nprobe(nprobe)
+    if coarse is None:
+        if nprobe is not None:
+            raise AtlasB200Error(f"ivfflat_topk: nprobe={nprobe} needs inverted lists (index type flat has none)")
+        n_list = 1
+    else:
+        require_cuda(coarse, "coarse")
+        if coarse.dtype != torch.float32 or coarse.dim() != 2 or coarse.shape[1] != DIM or coarse.shape[0] < 1 \
+                or not coarse.is_contiguous():
+            raise AtlasB200Error(f"ivfflat_topk: coarse must be contiguous fp32 [n_list >= 1, {DIM}]")
+        n_list = coarse.shape[0]
+    probed = nprobe is not None and nprobe < n_list
+    if rows.dtype != torch.float16 or rows.dim() != 2 or rows.shape[1] != DIM or not rows.is_contiguous() \
+            or rows.shape[0] % SQ_TILE or rows.shape[0] == 0 or rows.data_ptr() % 16:
+        raise AtlasB200Error(f"ivfflat_topk: rows must be contiguous, 16-byte aligned fp16 [64 * tiles, {DIM}]")
+    n_tiles = rows.shape[0] // SQ_TILE
+    if slot_rows.dtype != torch.int32 or slot_rows.shape != (rows.shape[0],) or tile_lists.dtype != torch.int32 \
+            or tile_lists.shape != (n_tiles,):
+        raise AtlasB200Error("ivfflat_topk: slot_rows must be int32 [slots] and tile_lists int32 [tiles]")
+    q = cast_queries(queries.reshape(-1, DIM).to(rows.device), torch.float16)
+    nq = q.shape[0]
+    op = PQ_OP_SEARCH_PROBED if probed else PQ_OP_SEARCH
+    buf = (workspace or _default_ws).get(lib().atlas_b200_ivfflat_workspace_bytes(op, rows.shape[0], n_list, k), rows.device)
+    out_s = torch.empty((nq, k), dtype=torch.float16, device=rows.device)
+    out_i = torch.empty((nq, k), dtype=torch.int64, device=rows.device)
+    status = torch.zeros(1, dtype=torch.int32, device=rows.device)
+    lt = lr = None
+    if probed:
+        if list_tile_off is None or list_rows is None:
+            list_tile_off, list_rows = ivfsq_list_tables(slot_rows, tile_lists, n_list)
+        _check_table(list_tile_off, "list_tile_off", (n_list + 1,))
+        _check_table(list_rows, "list_rows", (n_list,))
+        lt, lr = _ptr(list_tile_off), _ptr(list_rows)
+    args = (_ptr(rows), _ptr(slot_rows.contiguous()), n_tiles, n_rows, lt, lr, _ptr(coarse) if probed else None, n_list,
+            nprobe if probed else 0, _ptr(q), nq, k, _ptr(out_s), _ptr(out_i), id_base, id_stride)
+    if exhaustive:
+        check(lib().atlas_b200_ivfflat_topk_exhaustive(*args, _ptr(buf), buf.numel(), current_stream_ptr()))
+    else:
+        check(lib().atlas_b200_ivfflat_topk(*args, _ptr(status), _ptr(buf), buf.numel(), current_stream_ptr()))
+    return out_s, out_i, status
+
+
+# ---------------------------------------------------------------------------------------------
 # dense layers (csrc/gemm.cu)
 # ---------------------------------------------------------------------------------------------
 EPI_NONE, EPI_BIAS, EPI_GELU, EPI_RESIDUAL, EPI_GATED, EPI_RELU = 0, 1, 2, 3, 4, 5

@@ -201,7 +201,8 @@ int atlas_b200_pq_topk_probed_exhaustive(const uint8_t* codes, const void* list_
  *
  * atlas_b200_ivfsq_train: `sample` [n_sample, 768] fp16 in a seeded random order, n_sample >= n_list: the coarse
  *   k-means of atlas_b200_pq_train on the first min(n_sample, 256 n_list) rows, then vmin / vdiff over the residuals
- *   of the first min(n_sample, 100000).  Bitwise deterministic.
+ *   of the first min(n_sample, 100000).  Bitwise deterministic.  vmin = vdiff = NULL: the coarse k-means alone (the
+ *   IVF-Flat index below).
  * atlas_b200_ivfsq_encode: for n fp16 rows [n, 768] (call it chunk by chunk), the coarse assignment (inner product,
  *   lowest list on ties) into list_ids (int32 [n], may be NULL) and, when `codes` is not NULL, each row's 384 code
  *   bytes into slot row_slot[i] of `codes` (row_slot: int32 [n]).
@@ -243,6 +244,46 @@ int atlas_b200_ivfsq_topk_probed_exhaustive(const uint8_t* codes, const int32_t*
                                             const float* vdiff, int32_t nprobe, const void* queries, int32_t nq, int32_t k,
                                             void* out_scores, int64_t* out_ids, int64_t id_base, int64_t id_stride,
                                             void* workspace, size_t workspace_bytes, void* stream);
+
+/* --------------------------------------------------------------------------------------------
+ * IVF-Flat passage index (csrc/pq.cu, csrc/ivfflat.cu): `DistributedFAISSIndex` with index_type ivfflat (faiss
+ * IndexIVFFlat, inner product) and flat (faiss IndexFlatIP: the same layout with one list, always fully scanned).
+ *
+ *   n_list      coarse centroids (>= 1), coarse: device fp32 [n_list][768], trained by atlas_b200_ivfsq_train with
+ *               vmin = vdiff = NULL (the coarse quantizer of ivfpq / ivfsq); list ids by atlas_b200_ivfsq_encode with
+ *               codes = NULL.
+ *   layout      ivfsq's with fp16 rows in place of codes: rows stable-sorted by list, every list padded to a multiple of
+ *               64 slots, so each 64-slot tile belongs to one list.  rows: device fp16 [n_tiles * 64][768], 16-byte
+ *               aligned, padding slots zero; slot_rows: device int32 [n_tiles * 64], the local row of each slot or -1
+ *               for padding.  (tile_lists, int32 [n_tiles], is not an argument of the search: the probed search takes
+ *               its lists from list_tile_off.)
+ *   score       s = fp16(<q, x>) of the fp16 query and the fp16 row, accumulated in fp32 on the tensor cores: the flat
+ *               index's score (atlas_b200_mips_topk), bit for bit with the same operands.  No coarse term is added.
+ *   probe       the probed IVF search above, with T[q][l] = <q, c_l> in fp32 from the fp16-rounded query - ivfsq's T,
+ *               which here only chooses P(q): for the same coarse quantizer and lists, ivfflat and ivfsq probe the same
+ *               lists.  The result is the exact top-k by s over the rows whose list is in P(q).
+ *
+ * atlas_b200_ivfflat_topk / _exhaustive: atlas_b200_mips_topk's contract (fp16 scores desc, ids = id_base + id_stride *
+ *   row, canonical tie order, `status` overflow flag and the exhaustive retry) over the n_rows real rows; padding slots
+ *   are never returned.  k <= n_rows.
+ *   nprobe         0 or >= n_list: every row (the full scan; coarse, list_tile_off and list_rows are unused and may be
+ *                  NULL); 1 <= nprobe < n_list: the probed search, with
+ *   list_tile_off  device int32 [n_list + 1]: list l owns tiles list_tile_off[l] .. list_tile_off[l + 1];
+ *   list_rows      device int32 [n_list]: the real rows of list l.  A work item is one 64-slot tile.
+ * Workspace: atlas_b200_ivfflat_workspace_bytes(op, n_tiles * 64, n_list, k) with op ATLAS_B200_PQ_OP_SEARCH (full
+ *   scan) or ATLAS_B200_PQ_OP_SEARCH_PROBED; 0 when n_list < 1.
+ * -------------------------------------------------------------------------------------------- */
+size_t atlas_b200_ivfflat_workspace_bytes(int32_t op, int64_t n_slots, int32_t n_list, int32_t k);
+int atlas_b200_ivfflat_topk(const void* rows, const int32_t* slot_rows, int64_t n_tiles, int64_t n_rows,
+                            const int32_t* list_tile_off, const int32_t* list_rows, const float* coarse, int32_t n_list,
+                            int32_t nprobe, const void* queries, int32_t nq, int32_t k, void* out_scores, int64_t* out_ids,
+                            int64_t id_base, int64_t id_stride, int32_t* status, void* workspace, size_t workspace_bytes,
+                            void* stream);
+int atlas_b200_ivfflat_topk_exhaustive(const void* rows, const int32_t* slot_rows, int64_t n_tiles, int64_t n_rows,
+                                       const int32_t* list_tile_off, const int32_t* list_rows, const float* coarse,
+                                       int32_t n_list, int32_t nprobe, const void* queries, int32_t nq, int32_t k,
+                                       void* out_scores, int64_t* out_ids, int64_t id_base, int64_t id_stride, void* workspace,
+                                       size_t workspace_bytes, void* stream);
 
 /* Exact re-ranking of PQ search candidates (csrc/pq_refine.cu; faiss IndexRefineFlat, `k_factor`): for every query,
  * the k_cand candidate rows are re-scored against their full-precision rows and the top k are returned.

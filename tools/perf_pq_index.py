@@ -13,12 +13,13 @@ of bench.py (4 Mi passages of 768-d fp16 per GPU, BASELINE configs[1]).  Prints 
                               refine kernel's time and the host-row bytes it reads per search (nq k' 1536, from shapes) over
                               that time
   at_8_queries                the same search, and the flat scan, at 8 queries per search (bench.py's per-rank batch)
-  ivfsq                       with --index-type ivfsq only: each sweep's kernel time (256 and 8 queries) against the larger of its two bounds from shapes: the
-                              code bytes over the HBM peak, and 2 x 768 x slots x queries FLOPs over the dense fp16
-                              tensor peak (the tensor bound binds at 256 queries, HBM at 8)
+  ivfsq / ivfflat             with --index-type ivfsq or ivfflat only: each sweep's kernel time (256 and 8 queries) against
+                              the larger of its two bounds from shapes: the code (ivfflat: fp16 row) bytes over the HBM
+                              peak, and 2 x 768 x slots x queries FLOPs over the dense fp16 tensor peak
     python tools/perf_pq_index.py [--index-type ivfpq] [--code-size 16] [--rows N] [--steps 20] [--warmup 3]
                                   [--refine-factor 1]
-With --nprobe 8,32,128 it measures the probed search instead, for ivfpq (--code-size) and ivfsq on a seeded CLUSTERED
+With --nprobe 8,32,128 it measures the probed search instead, for ivfpq (--code-size) and ivfsq (or, with --index-type
+ivfflat, for ivfflat alone, and the flat scan beside it at both batch sizes) on a seeded CLUSTERED
 bank (a Gaussian mixture: on an isotropic bank IVF recall means nothing; this is still not real embeddings): per index
 type, nprobe (and "all", the full scan) and batch of 8 and 256 queries, queries/s, recall@40 against the exact flat
 search, the fast path's overflow flag (`fast_path_status`; the timed search includes the exhaustive retry when it is
@@ -52,7 +53,7 @@ def measure(args):
     torch.cuda.set_device(dev)
     L = lib()
     rows = args.rows
-    M = None if args.index_type == "ivfsq" else args.code_size
+    M = None if args.index_type in ("ivfsq", "ivfflat") else args.code_size
     steps, warmup = args.steps, args.warmup
     bank = make_bank(rows, dev, seed=1)
     q = make_queries().to(dev)
@@ -102,19 +103,20 @@ def measure(args):
     list_bytes = 0 if p.get("list_ids") is None else p["list_ids"].element_size()
     groups = kn.value // (steps + warmup) if kn.value else 0
     kernel_ms = kms.value / (steps + warmup)
-    sweep_bytes = rows * (M + list_bytes) if M else p["codes"].numel()
+    slot_bytes = DIM * 2 if args.index_type == "ivfflat" else ops.SQ_CODE_BYTES
+    sweep_bytes = rows * (M + list_bytes) if M else p["slot_rows"].numel() * slot_bytes
     peak, peak_src = peaks("hbm")
     achieved = sweep_bytes / (kernel_ms * 1e-3) / 1e9 if kernel_ms > 0 else 0.0
     ms8, (_, ids8, st8), kms8, _ = profiled(q[:8])
     assert int(st8.item()) == 0, "fast search path overflowed"
     recall8 = recall_of(ids8.cpu().numpy(), 8)
     ivfsq = None
-    if args.index_type == "ivfsq":
-        slots = p["codes"].shape[0]
+    if args.index_type in ("ivfsq", "ivfflat"):
+        slots = p["slot_rows"].shape[0]
         tflops, tensor_src = 989.0, "H100 SXM data sheet, dense fp16"
 
         def bounds(nq, kernel_ms):
-            hbm_ms = slots * ops.SQ_CODE_BYTES / (peak * 1e9) * 1e3
+            hbm_ms = slots * slot_bytes / (peak * 1e9) * 1e3
             tensor_ms = 2.0 * DIM * slots * nq / (tflops * 1e12) * 1e3
             bound_ms = max(hbm_ms, tensor_ms)
             return {"queries": nq, "kernel_ms_per_search": kernel_ms, "hbm_bound_ms": hbm_ms, "tensor_bound_ms": tensor_ms,
@@ -158,15 +160,17 @@ def measure(args):
                  "call": "ops.mips_topk (exact fp16 bank scan, device-resident bank)"},
         "sweep": {"bound": "hbm", "achieved": achieved, "peak": peak, "unit": "GB/s",
                   "frac": achieved / peak if peak else None, "peak_source": peak_src,
-                  "kernel": "ivfsq_scan_kernel (main sweep; codes read once per 128 queries)" if M is None else
-                            "pq_scan_kernel (main sweep; codes re-read once per query group, so real traffic is higher)",
+                  "kernel": {"ivfsq": "ivfsq_scan_kernel (main sweep; codes read once per 128 queries)",
+                             "ivfflat": "ivfflat_scan_kernel (main sweep; rows read once per 256 queries)"}.get(
+                                 args.index_type,
+                                 "pq_scan_kernel (main sweep; codes re-read once per query group, so real traffic is higher)"),
                   "kernel_ms_per_search": kernel_ms, "kernel_launches_per_search": groups,
                   "code_bytes_per_search": sweep_bytes},
         "device_bytes_per_passage": dev_bytes / rows, "flat_device_bytes_per_passage": DIM * 2,
         "recall_at_40": recall, "recall_note": "against the exact flat search on a synthetic Gaussian bank; not "
                                                "representative of real embeddings",
         "gpu": smi,
-    } | ({"refine": refine} if refine else {}) | ({"ivfsq": ivfsq} if ivfsq else {})
+    } | ({"refine": refine} if refine else {}) | ({args.index_type: ivfsq} if ivfsq else {})
 
 
 def clustered_bank(rows, dev, centers=4096, spread=0.35, seed=3):
@@ -208,7 +212,24 @@ def measure_nprobe(args):
     out = {"metric": "probed IVF search (nprobe), top-40", "rows": rows, "steps": steps,
            "bank": "seeded Gaussian mixture (4096 centres, spread 0.35): clustered, still not real embeddings",
            "hbm_peak_GBps": peak, "peak_source": peak_src, "results": []}
-    for kind in ("ivfpq", "ivfsq"):
+    kinds = ("ivfflat",) if args.index_type == "ivfflat" else ("ivfpq", "ivfsq")
+    if args.index_type == "ivfflat":
+        # the exact flat scan of the same bank (ops.mips_topk, device-resident), for comparison
+        out["flat"] = []
+        for nq in (8, NQ):
+            fn = lambda: ops.mips_topk(bank, q[:nq], TOPK)
+            for _ in range(warmup):
+                fn()
+            e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+            e0.record()
+            for _ in range(steps):
+                fn()
+            e1.record()
+            torch.cuda.synchronize()
+            ms = e0.elapsed_time(e1) / steps
+            out["flat"].append({"queries": nq, "value": nq / (ms * 1e-3), "unit": "queries/s", "ms_per_search": ms,
+                                "hbm_bound_ms": rows * DIM * 2 / (peak * 1e9) * 1e3})
+    for kind in kinds:
         index = DistributedFAISSIndex(kind, args.code_size if kind == "ivfpq" else None)
         if host is None:
             host = index._host_rows(rows)
@@ -219,9 +240,10 @@ def measure_nprobe(args):
         index.train_index()
         p = index._pq
         n_list = p["n_list"]
-        if kind == "ivfsq":
+        if kind in ("ivfsq", "ivfflat"):
             tl = p["tile_lists"].to(torch.int64)
-            list_bytes = torch.bincount(tl, minlength=n_list).double() * ops.SQ_TILE * ops.SQ_CODE_BYTES
+            slot_bytes = ops.SQ_CODE_BYTES if kind == "ivfsq" else DIM * 2
+            list_bytes = torch.bincount(tl, minlength=n_list).double() * ops.SQ_TILE * slot_bytes
         else:
             # a probed ivfpq sweep reads each probed row's list position (4 B, in order) and then its codes through that
             # permutation: scattered reads that each move whole 32-byte sectors
@@ -250,7 +272,7 @@ def measure_nprobe(args):
                 ms = e0.elapsed_time(e1) / steps
                 kernel_ms = kms.value / steps
                 if nprobe is None or nprobe >= n_list:
-                    read = float(list_bytes.sum()) if kind == "ivfsq" else float(rows * (args.code_size + 2))
+                    read = float(list_bytes.sum()) if kind != "ivfpq" else float(rows * (args.code_size + 2))
                 else:
                     union = torch.zeros(n_list, dtype=torch.bool, device=dev)
                     union[torch.topk(T[:nq], nprobe, dim=1).indices.flatten()] = True
@@ -280,7 +302,7 @@ def measure_nprobe(args):
 
 def main():
     ap = argparse.ArgumentParser()
-    ap.add_argument("--index-type", choices=["pq", "ivfpq", "ivfsq"], default="ivfpq")
+    ap.add_argument("--index-type", choices=["pq", "ivfpq", "ivfsq", "ivfflat"], default="ivfpq")
     ap.add_argument("--code-size", type=int, default=16, help="bytes of PQ code per passage (ivfsq: always 4 bits per dim)")
     ap.add_argument("--rows", type=int, default=N_LOCAL)
     ap.add_argument("--steps", type=int, default=20)
@@ -288,7 +310,8 @@ def main():
     ap.add_argument("--refine-factor", type=int, default=1,
                     help="also time the search re-ranked over refine-factor x 40 PQ candidates (1 = off)")
     ap.add_argument("--nprobe", default=None,
-                    help="comma-separated nprobe values: measure the probed search of ivfpq and ivfsq instead")
+                    help="comma-separated nprobe values: measure the probed search of ivfpq and ivfsq (of ivfflat with "
+                         "--index-type ivfflat) instead")
     args = ap.parse_args()
     print(json.dumps(measure_nprobe(args) if args.nprobe else measure(args)))
 
