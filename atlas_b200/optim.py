@@ -48,6 +48,31 @@ def _to_device(arr, device):
     return host.to(device, non_blocking=True), host
 
 
+def bias_corrections(group, t):
+    """(lr / (1 - beta1^t), sqrt(1 - beta2^t)): derived in double precision like torch, rounded once to fp32 by the
+    descriptor table."""
+    beta1, beta2 = group["betas"]
+    return group["lr"] / (1.0 - beta1 ** t), math.sqrt(1.0 - beta2 ** t)
+
+
+def adamw_launch(rows, group, scale, device):
+    """One `atlas_b200_adamw_fp32copy` launch over `_ADAM_DESC` rows of one param group.  A row is a whole parameter
+    (`AdamWFP32Copy`) or a segment of one (`sharded.OSS`: every pointer offset to the segment's first element).  Returns
+    the device tables and their pinned staging copies, which must stay alive until the kernel has run."""
+    beta1, beta2 = group["betas"]
+    descs = np.array(rows, dtype=_ADAM_DESC)
+    chunks = _chunk_table([r[5] for r in rows])
+    d_dev, h1 = _to_device(descs, device)
+    c_dev, h2 = _to_device(chunks, device)
+    with torch.cuda.device(device):
+        # torch derives these scalars in double precision and rounds them once: do the same
+        check(lib().atlas_b200_adamw_fp32copy(d_dev.data_ptr(), c_dev.data_ptr(), int(chunks.shape[0]), CHUNK,
+                                              1.0 - float(group["lr"]) * float(group["weight_decay"]), float(beta2),
+                                              1.0 - float(beta1), 1.0 - float(beta2), float(group["eps"]),
+                                              1.0 / float(scale), current_stream_ptr()))
+    return d_dev, c_dev, h1, h2
+
+
 class AdamWFP32Copy(torch.optim.AdamW):
     """`src/AdamWFP32Copy.py:14-169`: AdamW whose moments and update live on an fp32 copy of every parameter; the
     (bf16) parameter receives the rounded copy after each step."""
@@ -61,7 +86,6 @@ class AdamWFP32Copy(torch.optim.AdamW):
         for group in self.param_groups:
             if group.get("amsgrad", False) or group.get("maximize", False):
                 raise AtlasB200Error("AdamWFP32Copy (B200): amsgrad / maximize are not implemented")
-            beta1, beta2 = group["betas"]
             rows = []
             keep = []          # tensors that must stay alive until the launch has been enqueued
             device = None
@@ -91,21 +115,11 @@ class AdamWFP32Copy(torch.optim.AdamW):
                 keep.append(g)
                 rows.append((p.data_ptr(), state["float32copy"].data_ptr(), state["exp_avg"].data_ptr(),
                              state["exp_avg_sq"].data_ptr(), g.data_ptr(), p.numel(), _kind(p, "parameter"),
-                             _kind(g, "gradient"), group["lr"] / (1.0 - beta1 ** t), math.sqrt(1.0 - beta2 ** t)))
+                             _kind(g, "gradient")) + bias_corrections(group, t))
             if not rows:
                 continue
-            descs = np.array(rows, dtype=_ADAM_DESC)
-            chunks = _chunk_table([r[5] for r in rows])
-            d_dev, h1 = _to_device(descs, device)
-            c_dev, h2 = _to_device(chunks, device)
-            with torch.cuda.device(device):
-                # torch derives these scalars in double precision and rounds them once: do the same
-                check(lib().atlas_b200_adamw_fp32copy(d_dev.data_ptr(), c_dev.data_ptr(), int(chunks.shape[0]), CHUNK,
-                                                      1.0 - float(group["lr"]) * float(group["weight_decay"]), float(beta2),
-                                                      1.0 - float(beta1), 1.0 - float(beta2), float(group["eps"]),
-                                                      1.0 / float(scale), current_stream_ptr()))
             # the tables are read by the kernel asynchronously: keep them (and the pinned staging copies) until the next step
-            self._live = (d_dev, c_dev, h1, h2, keep)
+            self._live = (adamw_launch(rows, group, scale, device), keep)
         from .retrievers import _bump_weights_epoch
 
         _bump_weights_epoch()          # the kernel wrote the parameters behind autograd's version counters
@@ -131,21 +145,35 @@ def grad_stats_tensor(params):
         g = g if g.is_contiguous() else g.contiguous()
         keep.append(g)
         rows.append((g.data_ptr(), g.numel(), _kind(g, "gradient"), 0))
+    out = grad_stats_launch(rows, device)
+    out._atlas_keep = (out._atlas_keep, keep)
+    return out
+
+
+def grad_stats_launch(rows, device):
+    """[len(rows), 4] fp32 device tensor of (min |g|, max |g|, mean |g|, ||g||_2) for `_GRAD_DESC` rows (grad pointer,
+    numel, kind, 0): whole gradients or segments of them (a null pointer or numel 0 gives zeros).  No synchronisation;
+    the result keeps the uploaded tables alive."""
     descs = np.array(rows, dtype=_GRAD_DESC)
     chunks = _chunk_table([r[1] for r in rows])
     d_dev, h1 = _to_device(descs, device)
     c_dev, h2 = _to_device(chunks, device)
-    out = torch.empty((len(params), 4), dtype=torch.float32, device=device)
+    out = torch.empty((len(rows), 4), dtype=torch.float32, device=device)
     with torch.cuda.device(device):
-        check(lib().atlas_b200_grad_stats(d_dev.data_ptr(), len(params), c_dev.data_ptr(), int(chunks.shape[0]), CHUNK,
+        check(lib().atlas_b200_grad_stats(d_dev.data_ptr(), len(rows), c_dev.data_ptr(), int(chunks.shape[0]), CHUNK,
                                           out.data_ptr(), current_stream_ptr()))
-    out._atlas_keep = (d_dev, c_dev, h1, h2, keep)
+    out._atlas_keep = (d_dev, c_dev, h1, h2)
     return out
 
 
 def compute_grad_stats(model):
     """`src/util.py:200-222`: {"skip_example", "min", "max", "mean"} over the reader's parameters (summed over ranks like the
-    reference's all_reduce).  ONE host synchronisation (the final read-back) instead of four per parameter."""
+    reference's all_reduce).  ONE host synchronisation (the final read-back) instead of four per parameter.
+
+    With the reader wrapped in `sharded.ShardedDataParallel` each parameter's `.grad` is its view of the flat gradient
+    buffer, which holds the rank's LOCAL gradient until the reduce-scatter of the next `clip_grad_norm` / `step`: the
+    statistics are those of the W local gradients, summed.  Under DDP every rank holds the averaged gradient, so the
+    sum is W copies of the averaged gradient's statistics instead.  The two agree when the local gradients are equal."""
     with torch.no_grad():
         inner = model.module if hasattr(model, "module") else model
         stats = grad_stats_tensor(p for _, p in inner.reader.named_parameters())
