@@ -181,28 +181,46 @@ def _check_passage_length(L):
                              f"{ops.ATTENTION_LONG_MAX_LK} tokens")
 
 
-def _cross_split(Lk, dropout=False):
-    """Key segment of the split-KV cross-attention over Lk keys: the largest divisor of Lk up to 384 keys, else up to 512 (the
-    attention kernel keeps a whole segment's K / V in shared memory).  dropout: the training forward's dropout mask is
-    addressed in 32-key groups over the whole key range (csrc/dropout.cuh), so a multiple of 32 in [64, 512] comes first."""
-    split = None
-    if dropout:
-        split = next((s for s in range(min(512, Lk) // 32 * 32, 63, -32) if Lk % s == 0), None)
-    split = split or next((s for s in range(min(384, Lk), 63, -1) if Lk % s == 0), None) or \
-        next(s for s in range(min(512, Lk), 0, -1) if Lk % s == 0)
-    if split < 64 and Lk > 512:
-        raise AtlasB200Error(f"n_context*text_maxlength = {Lk} has no divisor in [64, 512] for the split-KV kernel")
-    if dropout and split % 32 != 0 and split != Lk:
-        raise AtlasB200Error(f"dropout on the cross-attention probabilities needs a key split that is a multiple of 32 "
-                             f"(n_context*text_maxlength = {Lk} gave {split})")
-    return split
+def _cross_split(Lk, dropout=False, force_pad=False):
+    """(split, Lk_pad): key segment and padded key range of the split-KV cross-attention over Lk keys.
+
+    Segments: the largest divisor of Lk up to 384 keys, else up to 512 (the attention kernel keeps a whole segment's K / V
+    in shared memory).  dropout: the training forward's dropout mask is addressed in 32-key groups (csrc/dropout.cuh), so a
+    multiple of 32 in [64, 512] comes first.  Lk_pad = Lk then.
+    A key range without such a divisor (Lk > 512 with none in [64, 512]; with dropout, none that is a multiple of 32) is
+    padded instead: ceil(Lk / 384) segments (one up to 512 keys) of equal length rounded up to a multiple of 64, so
+    Lk_pad - Lk < 384 dead keys (< 64 up to 512 keys), which _pad_keys / _cross_mask add and mask.
+    force_pad: the padded plan even where a divisor exists (tests)."""
+    if not force_pad:
+        split = None
+        if dropout:
+            split = next((s for s in range(min(512, Lk) // 32 * 32, 63, -32) if Lk % s == 0), None)
+        split = split or next((s for s in range(min(384, Lk), 63, -1) if Lk % s == 0), None) or \
+            next(s for s in range(min(512, Lk), 0, -1) if Lk % s == 0)
+        if (split >= 64 or Lk <= 512) and (not dropout or split % 32 == 0 or split == Lk):
+            return split, Lk
+    n = 1 if Lk <= 512 else -(-Lk // 384)
+    split = (-(-Lk // n) + 63) // 64 * 64
+    return split, n * split
 
 
-def _cross_mask(enc_mask, B, Lk, dt):
+def _pad_keys(x, B, Lk, Lk_pad):
+    """[B * Lk, C] rows -> [B * Lk_pad, C]: each batch element's Lk rows followed by Lk_pad - Lk zero rows (x itself when
+    Lk_pad == Lk).  Differentiable: the backward is the slice of the real rows."""
+    if Lk_pad == Lk:
+        return x
+    return torch.nn.functional.pad(x.reshape(B, Lk, -1), (0, 0, 0, Lk_pad - Lk)).reshape(B * Lk_pad, -1)
+
+
+def _cross_mask(enc_mask, B, Lk, dt, Lk_pad=None):
     """The additive cross-attention mask [B, Lk] fp32 of `invert_attention_mask` (4.18): -1e4 for fp16, -1e9 otherwise
-    (src/modeling_t5.py:950)."""
+    (src/modeling_t5.py:950).  Lk_pad: extended to [B, Lk_pad] with twice that value on the pad keys, so that they weigh
+    exactly 0 even next to a batch element whose real keys are all masked."""
     neg = -1e4 if dt == torch.float16 else -1e9
-    return (1.0 - enc_mask.reshape(B, Lk).to(torch.float32)) * neg
+    m = (1.0 - enc_mask.reshape(B, Lk).to(torch.float32)) * neg
+    if Lk_pad is not None and Lk_pad != Lk:
+        m = torch.nn.functional.pad(m, (0, Lk_pad - Lk), value=2.0 * neg)
+    return m
 
 
 def _norm_sums(n_sub, M, device, fused):
@@ -292,14 +310,26 @@ class FiD(nn.Module):
     def create_crossattention_storage(self):
         self._xattn = []
 
-    def _record_xattn(self, q, kv, B, H, T, Lk, lse, mask, layer=None):
+    def _record_xattn(self, q, kv, B, H, T, Lk, lse, mask, layer=None, keys=None):
         """Keep ONE record per decoder layer, overwritten by every forward (the reference keeps one buffer per attention
-        module, src/fid.py:333-343): constant memory however many forwards run between two `reset_score_storage()` calls."""
+        module, src/fid.py:333-343): constant memory however many forwards run between two `reset_score_storage()` calls.
+        The statistics kernel takes at most 128 target tokens: longer targets run as 128-token slices of q and lse
+        (every row's statistics depend on its own query only).  keys: the real keys of a padded range of Lk (_cross_split),
+        the records keep those."""
         if getattr(self, "_capture", False):
             n = self.config.num_decoder_layers
             if not isinstance(getattr(self, "_xattn", None), list):
                 self._xattn = []
-            rec = ops.cross_attention_stats(q.detach(), 0, kv.detach(), 0, H * 64, B, H, T, Lk, lse, add_mask=mask, scale=1.0)
+            q, kv = q.detach(), kv.detach()
+            parts = []
+            for t0 in range(0, T, 128):
+                t = min(128, T - t0)
+                qs = q if t == T else q.view(B, T, -1)[:, t0:t0 + t].reshape(B * t, -1)
+                parts.append(ops.cross_attention_stats(qs, 0, kv, 0, H * 64, B, H, t, Lk, lse[:, :, t0:t0 + t],
+                                                       add_mask=mask, scale=1.0))
+            rec = parts[0] if len(parts) == 1 else tuple(torch.cat(r, 1) for r in zip(*parts))
+            if keys is not None and keys != Lk:
+                rec = tuple(r[..., :keys] for r in rec)
             if layer is None:                       # sequential recording: a new forward starts after n records
                 if len(self._xattn) >= n:
                     self._xattn = []
@@ -556,14 +586,24 @@ class FiD(nn.Module):
     def decode(self, decoder_input_ids, enc, enc_mask, cross_kv=None, enc_packed=None):
         """Decoder stack + LM head: [B, T] -> logits [B, T, vocab] (src/modeling_t5.py:875-1083,1619-1647).
         enc_packed: the tuple of `_encode_rows(packed=True)` that `enc` was expanded from - the cross K | V projections then
-        read the packed rows directly."""
+        read the packed rows directly.
+        cross_kv: the per-layer `cross_kv` projections of the encoder rows padded (_pad_keys) to _cross_split's key range."""
         c = self.config
         W, G, dt = self._weights()
         B, T = decoder_input_ids.shape
         d, H = c.d_model, c.num_heads
-        Lk = enc.shape[1]
-        split = _cross_split(Lk)
-        cross_mask = _cross_mask(enc_mask, B, Lk, dt)
+        keys = enc.shape[1]
+        split, Lk = _cross_split(keys)
+        if cross_kv is None and Lk != keys and ops.cross_attention_streams(T, keys):
+            Lk = keys                                         # the stream kernel takes the unpadded range
+        if cross_kv is not None and cross_kv[0].shape[0] != B * Lk:
+            raise AtlasB200Error(f"decode: cross_kv has {cross_kv[0].shape[0]} rows, the padded key range needs {B * Lk}")
+        cross_mask = _cross_mask(enc_mask, B, keys, dt, Lk)
+        if Lk != keys and cross_kv is None:
+            # no usable split of the key range: every batch element's encoder rows are padded with masked zero rows once,
+            # before the K | V projections
+            enc = _pad_keys(enc.reshape(B * keys, d), B, keys, Lk).view(B, Lk, d)
+            enc_packed = None
         cross_live = ops.key_block_live(cross_mask)           # padded 64-key tiles of the encoder output: skipped, once
         capture = getattr(self, "_capture", False)
         # Only the encoder positions inside a live 64-key tile are ever read by the cross-attention: project K | V for those
@@ -602,7 +642,7 @@ class FiD(nn.Module):
                                           split=split, return_lse=capture, tile_live=cross_live)
             if not capture:
                 return r
-            self._record_xattn(q, cross_kv[i], B, H, T, Lk, r[1], cross_mask, layer=i)
+            self._record_xattn(q, cross_kv[i], B, H, T, Lk, r[1], cross_mask, layer=i, keys=keys)
             return r[0]
 
         # fuse_norm: the RMSNorms fused around the GEMMs like the encoder's; 3 x num_decoder_layers - 1 launches of a
@@ -699,13 +739,16 @@ class FiD(nn.Module):
         W, G, dt = WG
         B, T = decoder_input_ids.shape
         d, H = c.d_model, c.num_heads
-        Lk = enc.shape[1]
+        keys = enc.shape[1]
         eps = c.layer_norm_epsilon
         pdrop = self._dropout_p()
-        split = _cross_split(Lk, dropout=pdrop > 0)
+        split, Lk = _cross_split(keys, dropout=pdrop > 0)
         flat = enc.reshape(-1, d)
         if flat.dtype != dt:
             flat = flat.to(dt)
+        # padded key range (_cross_split): masked zero rows once per forward; the dropout mask of a key depends on its
+        # index only, so the real keys keep theirs
+        flat = _pad_keys(flat, B, keys, Lk)
         h = g.dropout(self._embed_train(W, dt, decoder_input_ids), pdrop)
 
         def lin_res(x, w, res):
@@ -715,7 +758,7 @@ class FiD(nn.Module):
 
         bias = bias_by_delta(W["decoder.block.0.layer.0.SelfAttention.relative_attention_bias.weight"], T, T, False,
                              c.relative_attention_num_buckets)
-        cross_mask = _cross_mask(enc_mask, B, Lk, dt)
+        cross_mask = _cross_mask(enc_mask, B, keys, dt, Lk)
         cross_mask._atlas_block_live = ops.key_block_live(cross_mask)     # padded 64-key tiles: skipped forward and backward
 
         def block(i, h, bias, flat):
@@ -730,7 +773,7 @@ class FiD(nn.Module):
             kv = g.linear(flat, G[p + "EncDecAttention.kv"])
             ctx, lse = g.cross_attention(q, kv, B, H, T, Lk, add_mask=cross_mask, scale=1.0, split=split, return_lse=True,
                                          dropout_p=pdrop)
-            self._record_xattn(q, kv, B, H, T, Lk, lse, cross_mask, layer=i)
+            self._record_xattn(q, kv, B, H, T, Lk, lse, cross_mask, layer=i, keys=keys)
             h = lin_res(ctx, W[p + "EncDecAttention.o.weight"], h)
             p = f"decoder.block.{i}.layer.2."
             n = g.layernorm(h, W[p + "layer_norm.weight"], None, eps, kind=1)
@@ -1165,8 +1208,8 @@ class FiD(nn.Module):
         re-runs the whole decoder prefix (no self-attention cache).  Parity reference for the cached path."""
         c = self.config
         enc = self.encode(input_ids, attention_mask)
-        B = enc.shape[0]
-        kv = self.cross_kv(enc)
+        B, keys = enc.shape[0], enc.shape[1]
+        kv = self.cross_kv(_pad_keys(enc.reshape(B * keys, -1), B, keys, _cross_split(keys)[1]))   # decode's key range
         mask = attention_mask.reshape(B, -1)
         seq = torch.full((B, 1), c.decoder_start_token_id, dtype=torch.long, device=enc.device)
         done = torch.zeros(B, dtype=torch.bool, device=enc.device)

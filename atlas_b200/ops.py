@@ -916,13 +916,19 @@ _XATTN_STREAM = os.environ.get("ATLAS_B200_XATTN_STREAM", "1") != "0"      # A/B
 _XATTN_CHUNK = int(os.environ.get("ATLAS_B200_XATTN_CHUNK", "1024"))        # keys per CTA (multiple of 64)
 
 
+def cross_attention_streams(Lq, Lk_total, dropout=None):
+    """Whether `cross_attention_split` runs the K / V stream kernel, which takes any Lk_total, instead of `split`-key
+    segments."""
+    return Lq <= 64 and dropout is None and Lk_total >= 1024 and _XATTN_STREAM
+
+
 def cross_attention_split(q, q_col0, kv, k_col0, v_col0, B, H, Lq, Lk_total, add_mask=None, scale=1.0, split=512,
                           return_lse=False, dropout=None, tile_live=None):
     """Attention of Lq (<= 128) queries per batch element over Lk_total keys (FiD decoder cross-attention,
     Lk_total = n_ctx * L): split-KV over segments of `split` keys + combine.  q [B*Lq, ld], kv [B*Lk_total, ld]."""
     require_cuda(q, "q")
     am = add_mask.float().contiguous() if add_mask is not None else None
-    if Lq <= 64 and dropout is None and Lk_total >= 1024 and _XATTN_STREAM:
+    if cross_attention_streams(Lq, Lk_total, dropout):
         # few target tokens against the concatenated encoder keys: the K / V stream kernel (csrc/attention_stream.cu)
         chunk = _XATTN_CHUNK
         chunks = (Lk_total + chunk - 1) // chunk
