@@ -128,7 +128,7 @@ def lib():
     L.atlas_b200_splice_tokens.argtypes = [vp, vp, i64, i64, vp, vp, vp, i64, i32, i32, i32, i32, i32, vp, vp, vp]
     u64 = c.c_uint64
     L.atlas_b200_dropout.restype = c.c_int
-    L.atlas_b200_dropout.argtypes = [vp, i64, vp, i64, vp, i64, i64, i32, f32, u64, u64, i32, vp]
+    L.atlas_b200_dropout.argtypes = [vp, i64, vp, i64, vp, i64, i64, i32, f32, u64, u64, vp, i32, vp]
     L.atlas_b200_dropout_mask.restype = c.c_int
     L.atlas_b200_dropout_mask.argtypes = [vp, i64, i32, f32, u64, u64, vp]
     L.atlas_b200_attention_train.restype = c.c_int
@@ -164,7 +164,11 @@ def lib():
     L.atlas_b200_linear_rows.restype = c.c_int
     L.atlas_b200_linear_rows.argtypes = [vp, i64, vp, i64, vp, vp, i64, vp, i64, i32, i32, i32, i32, i32, vp, vp, f32, vp, vp]
     L.atlas_b200_attention_packed.restype = c.c_int
-    L.atlas_b200_attention_packed.argtypes = [vp, i64, i32, i32, i32, vp, i64, vp, vp, vp, vp, i32, i32, i32, f32, i32, vp]
+    L.atlas_b200_attention_packed.argtypes = [vp, i64, i32, i32, i32, vp, i64, vp, vp, vp, vp, i32, i32, i32, f32, vp, f32, u64,
+                                              u64, i32, vp]
+    L.atlas_b200_attention_packed_bwd.restype = c.c_int
+    L.atlas_b200_attention_packed_bwd.argtypes = [vp, i64, vp, i64, vp, i64, vp, i64, vp, vp, vp, vp, vp, vp, vp, i32, i32, i32,
+                                                  f32, f32, u64, u64, i32, vp]
     L.atlas_b200_expand_packed_tiles.restype = c.c_int
     L.atlas_b200_expand_packed_tiles.argtypes = [vp, i64, vp, i32, vp, i64, i32, vp]
     L.atlas_b200_quantize_kv_e4m3.restype = c.c_int
@@ -282,6 +286,7 @@ EXPORTED_SYMBOLS = [
     "atlas_b200_embed_packed_tiles",
     "atlas_b200_linear_rows",
     "atlas_b200_attention_packed",
+    "atlas_b200_attention_packed_bwd",
     "atlas_b200_expand_packed_tiles",
     "atlas_b200_pq_workspace_bytes",
     "atlas_b200_pq_train",

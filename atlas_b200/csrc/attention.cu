@@ -19,8 +19,10 @@
 // Segments of 577 to 4096 keys (the FiD encoder on long passages) run on attention_long_kernel below: the same per-block
 // arithmetic, with K and V streamed through a ring of shared-memory slots instead of held resident.
 //
-// The padding-compacted encoders (segment b keeps the first n_b of its 64-row tiles, stored back to back) run on
-// attention_packed_kernel below: a persistent kernel over (segment, head) items with the same per-block arithmetic.
+// The padding-compacted encoders (segment b keeps the first n_b of its 64-row tiles, stored back to back, L <= 576): the
+// no-grad attention up to 384 tokens runs on attention_packed_kernel below, a persistent kernel over (segment, head) items with
+// the same per-block arithmetic; with lse or dropout (the training forward) and at 448 to 576 tokens attention_kernel runs
+// with packed-row addressing (Params::tile_off), its positions, mask, bias, dropout rows and lse those of the padded layout.
 //
 // All three kernels run that arithmetic through the same functions (issue_s, block_softmax, rescale_and_pack, drop_probs,
 // issue_pv, write_rows), so their results agree bit for bit where their inputs do.
@@ -65,6 +67,10 @@ struct Params {
     abdrop::Key drop;         // attention-probability dropout (training path); thr16 == 0: off
     const uint8_t* blk_live;  // [B, ceil(Lk / 64)] or nullptr: 0 = every key of the block is masked out
     int n_qt;                 // query tiles per segment (grid.x)
+    // packed rows (atlas_b200_attention_packed, self-attention with Lq = Lk): segment b is its kept 64-row tiles, blk_live =
+    // keep (a prefix of the segment), stored back to back from row 64 * tile_off[b * nkb] of q / k / v / out; nullptr: the
+    // padded layout.  Positions, mask, bias, dropout rows and lse stay those of the padded layout.
+    const int32_t* tile_off;
 };
 
 template <bool kBF16>
@@ -274,9 +280,19 @@ attention_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_consta
         const uint32_t m = __ballot_sync(0xffffffffu, lv);
         if (m != 0u) live = m;
     }
-    const int q_row0 = (b / p.q_div) * p.Lq;
-    const int k_row0 = b * p.Lk;
-    const int o_row0 = b * p.Lq;
+    int q_row0 = (b / p.q_div) * p.Lq;
+    int k_row0 = b * p.Lk;
+    int o_row0 = b * p.Lq;
+    int n_rows = p.Lq;            // rows of the segment that are stored
+    int n_qload = 2;              // 64-row halves of the query tile loaded
+    if (p.tile_off != nullptr) {
+        q_row0 = k_row0 = o_row0 = BK * __ldg(p.tile_off + static_cast<size_t>(b) * nkb);
+        n_rows = BK * __popc(live);
+        if (qt * BQ >= n_rows) return;
+        // a half past the segment's last kept tile is not loaded: its rows are neither stored nor allocated past the last
+        // segment; the MMAs keep the rows of a tile apart
+        n_qload = min(2, (n_rows - qt * BQ) / BK);
+    }
 
     if (threadIdx.x == 0) {
         ab::mbar_init(&load_bar, 1);
@@ -288,8 +304,8 @@ attention_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_consta
         ab::tma_prefetch_desc(&tmap_q);
         int nload = 0;
         for (int kb = 0; kb < nkb; ++kb) nload += (live >> kb) & 1u;
-        ab::mbar_arrive_expect_tx(&load_bar, static_cast<uint32_t>(2 * TILE_BYTES + 2 * nload * TILE_BYTES));
-        for (int t = 0; t < 2; ++t)
+        ab::mbar_arrive_expect_tx(&load_bar, static_cast<uint32_t>(n_qload * TILE_BYTES + 2 * nload * TILE_BYTES));
+        for (int t = 0; t < n_qload; ++t)
             ab::tma_load_2d(&tmap_q, &load_bar, smem_gen + t * TILE_BYTES, p.q_col0 + h * D, q_row0 + qt * BQ + t * BK,
                             ab::kEvictFirst);
         for (int kb = 0; kb < nkb; ++kb) {
@@ -338,7 +354,7 @@ attention_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_consta
 
     // ---- output: normalised 16-bit rows, or split-KV partials (un-normalised fp32 O, row max and row sum)
     if (p.o_partial == nullptr) {
-        write_rows<kBF16>(o, m_run, l_run, i0, p.Lq, p.O + static_cast<size_t>(o_row0) * p.ldo + h * D + cq, p.ldo,
+        write_rows<kBF16>(o, m_run, l_run, i0, n_rows, p.O + static_cast<size_t>(o_row0) * p.ldo + h * D + cq, p.ldo,
                           p.lse_out ? p.lse_out + (static_cast<size_t>(b) * p.H + h) * p.Lq : nullptr, p.drop.inv_keep, lane);
         return;
     }
@@ -722,6 +738,7 @@ static Params base_params(int B, int H, int Lq, int Lk, int q_col0, int k_col0, 
     p.drop = abdrop::make_key(0.f, 0, 0);
     p.blk_live = nullptr;
     p.n_qt = (Lq + BQ - 1) / BQ;
+    p.tile_off = nullptr;
     return p;
 }
 
@@ -759,17 +776,40 @@ extern "C" {
 
 // Self-attention over the PACKED rows of the padding-compacted FiD encoder (atlas_b200_segment_tile_scan): segment b keeps the
 // first popcount(keep[b, :]) of its L / 64 tiles, stored back to back from row 64 * tile_off[b * (L / 64)] of qkv / out.
+// Without lse_out and dropout, L <= 384 runs on the persistent attention_packed_kernel; everything else (the training forward,
+// 384 < L <= 576) on attention_kernel with packed-row addressing.
 int atlas_b200_attention_packed(const void* qkv, int64_t ld, int32_t q_col0, int32_t k_col0, int32_t v_col0, void* out, int64_t ldo,
                                 const float* add_mask, const float* bias_delta, const uint8_t* keep, const int32_t* tile_off,
-                                int32_t B, int32_t H, int32_t L, float scale, int32_t is_bf16, void* stream) {
+                                int32_t B, int32_t H, int32_t L, float scale, float* lse_out, float dropout_p, uint64_t seed,
+                                uint64_t offset, int32_t is_bf16, void* stream) {
     using namespace attn;
-    AB_REQUIRE(B > 0 && H > 0 && L > 0 && L % 64 == 0 && L <= 384 && keep != nullptr && tile_off != nullptr,
-               "attention_packed: 0 < L <= 384, L %% 64 == 0 and the segment tables are required (got L=%d)", L);
+    AB_REQUIRE(B > 0 && H > 0 && L > 0 && L % 64 == 0 && L <= MAX_LK && keep != nullptr && tile_off != nullptr,
+               "attention_packed: 0 < L <= %d, L %% 64 == 0 and the segment tables are required (got L=%d)", MAX_LK, L);
+    AB_REQUIRE(dropout_p >= 0.f && dropout_p < 1.f, "attention_packed: need 0 <= dropout_p < 1 (got %f)", dropout_p);
     AB_REQUIRE(ld % 8 == 0 && ldo % 8 == 0 && q_col0 % 8 == 0 && k_col0 % 8 == 0 && v_col0 % 8 == 0,
                "attention_packed: strides and column offsets must be multiples of 8 elements");
     AB_REQUIRE(static_cast<int64_t>(B) * L < (1ll << 31), "attention_packed: more than 2^31 rows");
     cudaStream_t ls = static_cast<cudaStream_t>(stream);
-    const Params tp = base_params(B, H, L, L, q_col0, k_col0, v_col0, out, ldo, add_mask, bias_delta, scale, 0.f);
+    Params tp = base_params(B, H, L, L, q_col0, k_col0, v_col0, out, ldo, add_mask, bias_delta, scale, 0.f);
+    tp.drop = abdrop::make_key(dropout_p, seed, offset);
+    // the packed rows of all segments: at most B * L (the tensor maps only bound the TMA boxes; no box reaches past the last
+    // kept tile)
+    const int rows = B * L;
+    const int nb = L / BK;
+    // the kernels' work: 4 * 64 FLOPs per (query, key) pair of the kept tiles, 64 x 64 pairs per (query tile, key tile)
+    const double work_per_tile_pair = 4.0 * H * BK * BK * D;
+    if (L > PK_MAX_TILES * BK || lse_out != nullptr || tp.drop.thr16 != 0u) {
+        tp.lse_out = lse_out;
+        tp.blk_live = keep;
+        tp.tile_off = tile_off;
+        abh::prof_begin(ls, abh::PROF_ATTENTION);
+        const int lrc = launch<attention_kernel<false>, attention_kernel<true>>(
+            is_bf16, dim3(tp.n_qt, H, B), THREADS, SMEM_BYTES, SMEM_BYTES, qkv, ld, qkv, ld, qkv, ld, rows, rows, tp, tp, ls);
+        if (lrc) return lrc;
+        abh::prof_end_tile_pairs(ls, abh::PROF_ATTENTION, work_per_tile_pair, keep, B, nb);
+        abh::count_launch();
+        return ATLAS_B200_OK;
+    }
     PackedParams p;
     p.S = B, p.H = H, p.L = L;
     // CTAs per head: one CTA per SM in all, every CTA with at least one segment
@@ -782,15 +822,12 @@ int atlas_b200_attention_packed(const void* qkv, int64_t ld, int32_t q_col0, int
     p.keep = keep;
     p.tile_off = tile_off;
     p.scale = scale;
-    // the packed rows of all segments: at most B * L (the tensor maps only bound the TMA boxes)
-    const int rows = B * L;
     abh::prof_begin(ls, abh::PROF_ATTENTION);
     const int lrc = launch<attention_packed_kernel<false>, attention_packed_kernel<true>>(
         is_bf16, dim3(p.G * p.H), PK_THREADS, packed_smem_bytes(L), static_cast<int>(packed_smem_bytes(PK_MAX_TILES * BK)), qkv,
         ld, qkv, ld, qkv, ld, rows, rows, tp, p, ls);
     if (lrc) return lrc;
-    // dense-equivalent work, like the masked-block skipping of the padded layout
-    abh::prof_end(ls, abh::PROF_ATTENTION, 4.0 * B * H * static_cast<double>(L) * L * attn::D);
+    abh::prof_end_tile_pairs(ls, abh::PROF_ATTENTION, work_per_tile_pair, keep, B, nb);
     abh::count_launch();
     return ATLAS_B200_OK;
 }

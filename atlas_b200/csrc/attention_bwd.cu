@@ -15,6 +15,8 @@
 //                         (cp.async double-buffered K / V tiles); dbias through a staged dS tile + diagonal sums.  A long
 //                         few-query key range (FiD cross-attention) is split over key chunks with fp32 dQ atomics.
 //   attn_bwd_dkv2_kernel  CTA = (b, h, 64-key block): the transposed problem, loops over the query blocks, accumulates dK, dV.
+// atlas_b200_attention_packed_bwd runs the same two kernels on the packed rows of the padding-compacted encoder
+// (Params::tile_off); the CTAs of a segment's dropped tiles return at once.
 // Bound: tensor (warp-level mma.sync m16n8k16 fragments).
 // FLOPs per call = 2 * B*H*Lq*Lk*64 * 7 (S + dP + dQ in the first kernel, S + dP + dV + dK in the second).
 #include "common.cuh"
@@ -51,7 +53,25 @@ struct Params {
     abdrop::Key drop;         // attention-probability dropout of the forward; thr16 == 0: off
     const uint8_t* blk_live;  // [B, ceil(Lk / 64)] or nullptr: 64-key blocks whose keys are all masked out (softmax weight exactly
                               // 0 in fp32, so dS = 0, dK = dV = 0 there): skipped
+    // packed rows (atlas_b200_attention_packed_bwd, self-attention with Lq = Lk): segment b is its kept 64-row tiles, blk_live =
+    // keep (a prefix of the segment), stored back to back from row 64 * tile_off[b * nkb] of every row operand; nullptr: the
+    // padded layout.  Positions, mask, bias, dropout rows, lse and dsum stay those of the padded layout.
+    const int32_t* tile_off;
 };
+
+// The rows of segment b: first row and number of rows of its queries and of its keys
+struct SegRows {
+    int64_t q0, k0;
+    int nq, nk;
+};
+__device__ __forceinline__ SegRows segment_rows(const Params& p, const int b, const int nkb) {
+    if (p.tile_off == nullptr)
+        return {static_cast<int64_t>(b) * p.Lq, static_cast<int64_t>(b) * p.Lk, p.Lq, p.Lk};
+    const int64_t row0 = 64ll * __ldg(p.tile_off + static_cast<int64_t>(b) * nkb);
+    int n = 0;
+    for (int t = 0; t < nkb; ++t) n += __ldg(p.blk_live + static_cast<int64_t>(b) * nkb + t) != 0;
+    return {row0, row0, 64 * n, 64 * n};
+}
 
 // ---- shared-memory tiles: 64 rows x 128 bytes, 16-byte chunks XOR-swizzled by the row ------------------------------
 __device__ __forceinline__ uint32_t tile_off(int row, int chunk) {
@@ -202,7 +222,10 @@ attn_bwd_dq2_kernel(const Params p) {
     const int b = item / (nqb * p.H);
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, g = lane >> 2, t = lane & 3;
     const int q0 = qb * BM;
-    const int64_t qrow_base = static_cast<int64_t>(b) * p.Lq, krow_base = static_cast<int64_t>(b) * p.Lk;
+    const int nkb = (p.Lk + BN - 1) / BN;
+    const SegRows seg = segment_rows(p, b, nkb);
+    if (q0 >= seg.nq) return;                  // a dropped query tile of a packed segment
+    const int64_t qrow_base = seg.q0, krow_base = seg.k0;
     const float* mask_row = p.add_mask ? p.add_mask + static_cast<int64_t>(b) * p.Lk : nullptr;
 
     if (bias_s)
@@ -214,14 +237,14 @@ attn_bwd_dq2_kernel(const Params p) {
         for (int x = threadIdx.x; x < ntab; x += THREADS) dbias_s[x] = 0.f;
     const uint32_t smem_a = ab::smem_u32(smem);
     const uint32_t sQ_a = smem_a, sdO_a = smem_a + TILE_BYTES;
-    load_tile(smem, p.q, p.ldq, p.q_col0 + h * D, qrow_base, q0, p.Lq);
-    load_tile(smem + TILE_BYTES, p.dout, p.lddo, h * D, qrow_base, q0, p.Lq);
+    load_tile(smem, p.q, p.ldq, p.q_col0 + h * D, qrow_base, q0, seg.nq);
+    load_tile(smem + TILE_BYTES, p.dout, p.lddo, h * D, qrow_base, q0, seg.nq);
 
     float drow[2];
     {
         const int r = q0 + warp * 16 + (lane >> 1);
         float acc = 0.f;
-        if (r < p.Lq) {
+        if (r < seg.nq) {
             const uint16_t* po = p.o + (qrow_base + r) * p.ldo + h * D + (lane & 1) * 32;
             const uint16_t* pd = p.dout + (qrow_base + r) * p.lddo + h * D + (lane & 1) * 32;
 #pragma unroll
@@ -239,23 +262,22 @@ attn_bwd_dq2_kernel(const Params p) {
         acc += __shfl_xor_sync(0xffffffffu, acc, 1);
         drow[0] = __shfl_sync(0xffffffffu, acc, 2 * g);
         drow[1] = __shfl_sync(0xffffffffu, acc, 2 * (g + 8));
-        if ((lane & 1) == 0 && r < p.Lq) p.dsum[(static_cast<int64_t>(b) * p.H + h) * p.Lq + r] = acc;
+        if ((lane & 1) == 0 && r < seg.nq) p.dsum[(static_cast<int64_t>(b) * p.H + h) * p.Lq + r] = acc;
     }
     const int i_lo = q0 + warp * 16 + g;
     float lse[2];
 #pragma unroll
     for (int r = 0; r < 2; ++r) {
         const int i = i_lo + r * 8;
-        lse[r] = i < p.Lq ? __ldg(p.lse + (static_cast<int64_t>(b) * p.H + h) * p.Lq + i) : INFINITY;
+        lse[r] = i < seg.nq ? __ldg(p.lse + (static_cast<int64_t>(b) * p.H + h) * p.Lq + i) : INFINITY;
     }
-    const int nkb = (p.Lk + BN - 1) / BN;
     const int per_chunk = (nkb + p.key_chunks - 1) / p.key_chunks;
     const int kb_begin = chunk * per_chunk;
     const int kb_end = min(nkb, kb_begin + per_chunk);
 
     auto prefetch = [&](int kb, int buf) {
-        load_tile_async(smem_a + (2 + buf) * TILE_BYTES, p.k, p.ldk, p.k_col0 + h * D, krow_base, kb * BN, p.Lk);
-        load_tile_async(smem_a + (4 + buf) * TILE_BYTES, p.v, p.ldv, p.v_col0 + h * D, krow_base, kb * BN, p.Lk);
+        load_tile_async(smem_a + (2 + buf) * TILE_BYTES, p.k, p.ldk, p.k_col0 + h * D, krow_base, kb * BN, seg.nk);
+        load_tile_async(smem_a + (4 + buf) * TILE_BYTES, p.v, p.ldv, p.v_col0 + h * D, krow_base, kb * BN, seg.nk);
         if (threadIdx.x < BN) {
             const int j = kb * BN + static_cast<int>(threadIdx.x);
             mask_s[buf * BN + threadIdx.x] = (mask_row != nullptr && j < p.Lk) ? __ldg(mask_row + j) : 0.f;
@@ -374,7 +396,7 @@ attn_bwd_dq2_kernel(const Params p) {
             }
         }
     } else {
-        store_acc<kBF16>(dqacc, p.scale, p.dq, p.lddq, p.dq_col0 + h * D, qrow_base, q0 + warp * 16, p.Lq, lane);
+        store_acc<kBF16>(dqacc, p.scale, p.dq, p.lddq, p.dq_col0 + h * D, qrow_base, q0 + warp * 16, seg.nq, lane);
     }
     if (dbias_s != nullptr) {
         __syncthreads();
@@ -401,7 +423,9 @@ attn_bwd_dkv2_kernel(const Params p) {
     const int b = static_cast<int>(blockIdx.x) / (nkb * p.H);
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, g = lane >> 2, t = lane & 3;
     const int k0 = kb * BM;
-    const int64_t qrow_base = static_cast<int64_t>(b) * p.Lq, krow_base = static_cast<int64_t>(b) * p.Lk;
+    const SegRows seg = segment_rows(p, b, nkb);
+    if (k0 >= seg.nk) return;                  // a dropped key tile of a packed segment
+    const int64_t qrow_base = seg.q0, krow_base = seg.k0;
     const float* lse_g = p.lse + (static_cast<int64_t>(b) * p.H + h) * p.Lq;
     const float* d_g = p.dsum + (static_cast<int64_t>(b) * p.H + h) * p.Lq;
 
@@ -427,8 +451,8 @@ attn_bwd_dkv2_kernel(const Params p) {
         }
     const uint32_t smem_a = ab::smem_u32(smem);
     const uint32_t sK_a = smem_a, sV_a = smem_a + TILE_BYTES;
-    load_tile(smem, p.k, p.ldk, p.k_col0 + h * D, krow_base, k0, p.Lk);
-    load_tile(smem + TILE_BYTES, p.v, p.ldv, p.v_col0 + h * D, krow_base, k0, p.Lk);
+    load_tile(smem, p.k, p.ldk, p.k_col0 + h * D, krow_base, k0, seg.nk);
+    load_tile(smem + TILE_BYTES, p.v, p.ldv, p.v_col0 + h * D, krow_base, k0, seg.nk);
 
     const int j_lo = k0 + warp * 16 + g;
     float mk[2];
@@ -437,14 +461,14 @@ attn_bwd_dkv2_kernel(const Params p) {
         const int j = j_lo + r * 8;
         mk[r] = (p.add_mask != nullptr && j < p.Lk) ? __ldg(p.add_mask + static_cast<int64_t>(b) * p.Lk + j) : 0.f;
     }
-    const int nqb = (p.Lq + BN - 1) / BN;
+    const int nqb = (seg.nq + BN - 1) / BN;
     auto prefetch = [&](int qb, int buf) {
-        load_tile_async(smem_a + (2 + buf) * TILE_BYTES, p.q, p.ldq, p.q_col0 + h * D, qrow_base, qb * BN, p.Lq);
-        load_tile_async(smem_a + (4 + buf) * TILE_BYTES, p.dout, p.lddo, h * D, qrow_base, qb * BN, p.Lq);
+        load_tile_async(smem_a + (2 + buf) * TILE_BYTES, p.q, p.ldq, p.q_col0 + h * D, qrow_base, qb * BN, seg.nq);
+        load_tile_async(smem_a + (4 + buf) * TILE_BYTES, p.dout, p.lddo, h * D, qrow_base, qb * BN, seg.nq);
         if (threadIdx.x < BN) {
             const int i = qb * BN + static_cast<int>(threadIdx.x);
-            lse_s[buf * BN + threadIdx.x] = i < p.Lq ? __ldg(lse_g + i) : INFINITY;
-            d_s[buf * BN + threadIdx.x] = i < p.Lq ? __ldg(d_g + i) : 0.f;
+            lse_s[buf * BN + threadIdx.x] = i < seg.nq ? __ldg(lse_g + i) : INFINITY;
+            d_s[buf * BN + threadIdx.x] = i < seg.nq ? __ldg(d_g + i) : 0.f;
         }
         cp_async_commit();
     };
@@ -513,8 +537,33 @@ attn_bwd_dkv2_kernel(const Params p) {
         mma_p_tile<kBF16>(dvacc, acc, sdO_a, lane);   // dV += P^T dO
         mma_p_tile<kBF16>(dkacc, dp, sQ_a, lane);     // dK += dS^T Q
     }
-    store_acc<kBF16>(dkacc, p.scale, p.dk, p.lddk, p.dk_col0 + h * D, krow_base, k0 + warp * 16, p.Lk, lane);
-    store_acc<kBF16>(dvacc, 1.0f, p.dv, p.lddv, p.dv_col0 + h * D, krow_base, k0 + warp * 16, p.Lk, lane);
+    store_acc<kBF16>(dkacc, p.scale, p.dk, p.lddk, p.dk_col0 + h * D, krow_base, k0 + warp * 16, seg.nk, lane);
+    store_acc<kBF16>(dvacc, 1.0f, p.dv, p.lddv, p.dv_col0 + h * D, krow_base, k0 + warp * 16, seg.nk, lane);
+}
+
+// The two kernels of one backward on p (nq_ctas / nk_ctas CTAs), with their shared memory for its bias tables
+static int launch_bwd(const Params& p, const int64_t nq_ctas, const int64_t nk_ctas, const int32_t is_bf16, cudaStream_t s) {
+    const int64_t ntab = static_cast<int64_t>(p.Lq) + p.Lk - 1;
+    const int smem_dq = 7 * TILE_BYTES + 2 * BN * 4 +
+                        static_cast<int>(((p.bias_delta ? ntab + 2 * BIAS_PAD : 0) + (p.dbias ? ntab : 0)) * 4);
+    const int smem_dkv = 6 * TILE_BYTES + 4 * BN * 4 + static_cast<int>((p.bias_delta ? ntab + 2 * BIAS_PAD : 0) * 4);
+    constexpr int SMEM_MAX = 7 * TILE_BYTES + 4 * BN * 4 + 2 * (8192 + 2 * BIAS_PAD) * 4;
+    static bool attr_set = false;
+    if (!attr_set) {
+        AB_CUDA_CHECK(cudaFuncSetAttribute(attn_bwd_dq2_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_MAX));
+        AB_CUDA_CHECK(cudaFuncSetAttribute(attn_bwd_dq2_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_MAX));
+        AB_CUDA_CHECK(cudaFuncSetAttribute(attn_bwd_dkv2_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_MAX));
+        AB_CUDA_CHECK(cudaFuncSetAttribute(attn_bwd_dkv2_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_MAX));
+        attr_set = true;
+    }
+    if (is_bf16) {
+        attn_bwd_dq2_kernel<true><<<static_cast<unsigned>(nq_ctas), THREADS, smem_dq, s>>>(p);
+        attn_bwd_dkv2_kernel<true><<<static_cast<unsigned>(nk_ctas), THREADS, smem_dkv, s>>>(p);
+    } else {
+        attn_bwd_dq2_kernel<false><<<static_cast<unsigned>(nq_ctas), THREADS, smem_dq, s>>>(p);
+        attn_bwd_dkv2_kernel<false><<<static_cast<unsigned>(nk_ctas), THREADS, smem_dkv, s>>>(p);
+    }
+    return ATLAS_B200_OK;
 }
 
 }  // namespace attnb
@@ -585,28 +634,67 @@ int atlas_b200_attention_bwd_train(const void* q, int64_t ldq, int32_t q_col0, c
     p.causal_value = causal_value;
     p.drop = drop;
     p.blk_live = key_block_live;
+    p.tile_off = nullptr;
     cudaStream_t s = static_cast<cudaStream_t>(stream);
-    const int smem_dq = 7 * TILE_BYTES + 2 * BN * 4 +
-                        static_cast<int>(((bias_delta ? ntab + 2 * BIAS_PAD : 0) + (dbias_delta ? ntab : 0)) * 4);
-    const int smem_dkv = 6 * TILE_BYTES + 4 * BN * 4 + static_cast<int>((bias_delta ? ntab + 2 * BIAS_PAD : 0) * 4);
-    constexpr int SMEM_MAX = 7 * TILE_BYTES + 4 * BN * 4 + 2 * (8192 + 2 * BIAS_PAD) * 4;
-    static bool attr_set = false;
-    if (!attr_set) {
-        AB_CUDA_CHECK(cudaFuncSetAttribute(attn_bwd_dq2_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_MAX));
-        AB_CUDA_CHECK(cudaFuncSetAttribute(attn_bwd_dq2_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_MAX));
-        AB_CUDA_CHECK(cudaFuncSetAttribute(attn_bwd_dkv2_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_MAX));
-        AB_CUDA_CHECK(cudaFuncSetAttribute(attn_bwd_dkv2_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_MAX));
-        attr_set = true;
-    }
     abh::prof_begin(s, abh::PROF_ATTENTION_BWD);
-    if (is_bf16) {
-        attn_bwd_dq2_kernel<true><<<static_cast<unsigned>(nq_ctas), THREADS, smem_dq, s>>>(p);
-        attn_bwd_dkv2_kernel<true><<<static_cast<unsigned>(nk_ctas), THREADS, smem_dkv, s>>>(p);
-    } else {
-        attn_bwd_dq2_kernel<false><<<static_cast<unsigned>(nq_ctas), THREADS, smem_dq, s>>>(p);
-        attn_bwd_dkv2_kernel<false><<<static_cast<unsigned>(nk_ctas), THREADS, smem_dkv, s>>>(p);
-    }
+    const int lrc = launch_bwd(p, nq_ctas, nk_ctas, is_bf16, s);
+    if (lrc) return lrc;
     abh::prof_end(s, abh::PROF_ATTENTION_BWD, 16.0 * B * H * static_cast<double>(Lq) * Lk * D);
+    abh::count_launch(2);
+    AB_CUDA_CHECK(cudaGetLastError());
+    return ATLAS_B200_OK;
+}
+
+// Backward of atlas_b200_attention_packed with lse_out (self-attention on the packed rows of the padding-compacted encoder):
+// qkv / dqkv hold q | k | v and dq | dk | dv at columns 0, 64 H and 128 H of [rows, >= 192 H] buffers; out / dout [rows, 64 H].
+// lse and dsum are [B, H, L] in the padded layout; dbias_delta [H, 2L - 1] is incremented.
+int atlas_b200_attention_packed_bwd(const void* qkv, int64_t ld, const void* out, int64_t ldo, const void* dout, int64_t lddo,
+                                    void* dqkv, int64_t ldd, const float* add_mask, const float* bias_delta, float* dbias_delta,
+                                    const float* lse, float* dsum, const uint8_t* keep, const int32_t* tile_off, int32_t B,
+                                    int32_t H, int32_t L, float scale, float dropout_p, uint64_t seed, uint64_t offset,
+                                    int32_t is_bf16, void* stream) {
+    using namespace attnb;
+    AB_REQUIRE(B > 0 && H > 0 && L > 0 && L % 64 == 0 && L <= 576 && keep != nullptr && tile_off != nullptr,
+               "attention_packed_bwd: 0 < L <= 576, L %% 64 == 0 and the segment tables are required (got L=%d)", L);
+    AB_REQUIRE(lse != nullptr && dsum != nullptr,
+               "attention_packed_bwd: lse (the forward's log-sum-exp) and dsum ([B, H, L] fp32 each) are required");
+    AB_REQUIRE(dropout_p >= 0.f && dropout_p < 1.f, "attention_packed_bwd: need 0 <= dropout_p < 1 (got %f)", dropout_p);
+    AB_REQUIRE(ld % 8 == 0 && ldo % 8 == 0 && lddo % 8 == 0 && ldd % 8 == 0,
+               "attention_packed_bwd: strides must be multiples of 8 elements");
+    AB_REQUIRE(dbias_delta == nullptr || bias_delta != nullptr, "attention_packed_bwd: dbias_delta without bias_delta");
+    AB_REQUIRE(static_cast<int64_t>(B) * L < (1ll << 31) && static_cast<int64_t>(B) * H * (L / 64) < (1ll << 31),
+               "attention_packed_bwd: more than 2^31 rows");
+    const int nb = L / 64;
+    Params p;
+    p.q = p.k = p.v = static_cast<const uint16_t*>(qkv);
+    p.o = static_cast<const uint16_t*>(out);
+    p.dout = static_cast<const uint16_t*>(dout);
+    p.ldq = p.ldk = p.ldv = ld;
+    p.ldo = ldo;
+    p.lddo = lddo;
+    p.q_col0 = 0, p.k_col0 = H * D, p.v_col0 = 2 * H * D;
+    p.dq = p.dk = p.dv = static_cast<uint16_t*>(dqkv);
+    p.lddq = p.lddk = p.lddv = ldd;
+    p.dq_col0 = 0, p.dk_col0 = H * D, p.dv_col0 = 2 * H * D;
+    p.add_mask = add_mask;
+    p.bias_delta = bias_delta;
+    p.dbias = dbias_delta;
+    p.lse = const_cast<float*>(lse);
+    p.dsum = dsum;
+    p.dq_accum = nullptr;
+    p.key_chunks = 1;
+    p.B = B, p.H = H, p.Lq = L, p.Lk = L;
+    p.scale = scale;
+    p.causal_value = 0.f;
+    p.drop = abdrop::make_key(dropout_p, seed, offset);
+    p.blk_live = keep;
+    p.tile_off = tile_off;
+    cudaStream_t s = static_cast<cudaStream_t>(stream);
+    const int64_t ctas = static_cast<int64_t>(B) * H * nb;     // per kernel; the CTAs of dropped tiles return at once
+    abh::prof_begin(s, abh::PROF_ATTENTION_BWD);
+    const int lrc = launch_bwd(p, ctas, ctas, is_bf16, s);
+    if (lrc) return lrc;
+    abh::prof_end_tile_pairs(s, abh::PROF_ATTENTION_BWD, 16.0 * H * 64.0 * 64.0 * D, keep, B, nb);
     abh::count_launch(2);
     AB_CUDA_CHECK(cudaGetLastError());
     return ATLAS_B200_OK;

@@ -19,15 +19,18 @@ __device__ __forceinline__ float f32(uint32_t h) {
 template <bool kBF16>
 __global__ void __launch_bounds__(256)
 dropout_kernel(const uint16_t* __restrict__ x, int64_t ldx, const uint16_t* __restrict__ res, int64_t ldr,
-               uint16_t* __restrict__ out, int64_t ldo, int64_t M, int N, abdrop::Key key) {
+               uint16_t* __restrict__ out, int64_t ldo, int64_t M, int N, const int32_t* __restrict__ row_tiles,
+               abdrop::Key key) {
     const int vec_per_row = N / 8;
     const int64_t nvec = M * vec_per_row;
     for (int64_t v = blockIdx.x * 256ll + threadIdx.x; v < nvec; v += gridDim.x * 256ll) {
         const int64_t m = v / vec_per_row;
         const int c = static_cast<int>(v % vec_per_row) * 8;
         const uint4 xv = __ldg(reinterpret_cast<const uint4*>(x + m * ldx + c));
+        // the mask of row m, or of padded row 64 row_tiles[m / 64] + m % 64 on the packed rows of the compacted encoder
+        const int64_t mk = row_tiles != nullptr ? 64ll * __ldg(row_tiles + m / 64) + m % 64 : m;
         uint32_t w[4];
-        abdrop::elem_words(key, static_cast<uint64_t>(v), w);
+        abdrop::elem_words(key, static_cast<uint64_t>(mk * vec_per_row + c / 8), w);
         const uint32_t xs[4] = {xv.x, xv.y, xv.z, xv.w};
         uint32_t o[4];
         uint4 rv = make_uint4(0, 0, 0, 0);
@@ -92,17 +95,21 @@ inline int grid_for(int64_t work) {
 extern "C" {
 
 int atlas_b200_dropout(const void* x, int64_t ldx, const void* residual, int64_t ldr, void* out, int64_t ldo, int64_t M,
-                       int32_t N, float p, uint64_t seed, uint64_t offset, int32_t is_bf16, void* stream) {
+                       int32_t N, float p, uint64_t seed, uint64_t offset, const int32_t* row_tiles, int32_t is_bf16,
+                       void* stream) {
     AB_REQUIRE(M >= 0 && N > 0 && N % 8 == 0 && ldx % 8 == 0 && ldo % 8 == 0 && (residual == nullptr || ldr % 8 == 0),
                "dropout: N and the strides must be multiples of 8 elements");
+    AB_REQUIRE(row_tiles == nullptr || M % 64 == 0, "dropout: row_tiles needs whole 64-row tiles (got M=%lld)",
+               static_cast<long long>(M));
     AB_REQUIRE(p >= 0.f && p < 1.f, "dropout: need 0 <= p < 1 (got %f)", p);
     if (M == 0) return ATLAS_B200_OK;
     const abdrop::Key key = abdrop::make_key(p, seed, offset);
     cudaStream_t s = static_cast<cudaStream_t>(stream);
     const int grid = dr::grid_for(M * (N / 8));
     const uint16_t *xp = static_cast<const uint16_t*>(x), *rp = static_cast<const uint16_t*>(residual);
-    if (is_bf16) dr::dropout_kernel<true><<<grid, 256, 0, s>>>(xp, ldx, rp, ldr, static_cast<uint16_t*>(out), ldo, M, N, key);
-    else dr::dropout_kernel<false><<<grid, 256, 0, s>>>(xp, ldx, rp, ldr, static_cast<uint16_t*>(out), ldo, M, N, key);
+    uint16_t* op = static_cast<uint16_t*>(out);
+    if (is_bf16) dr::dropout_kernel<true><<<grid, 256, 0, s>>>(xp, ldx, rp, ldr, op, ldo, M, N, row_tiles, key);
+    else dr::dropout_kernel<false><<<grid, 256, 0, s>>>(xp, ldx, rp, ldr, op, ldo, M, N, row_tiles, key);
     abh::count_launch();
     AB_CUDA_CHECK(cudaGetLastError());
     return ATLAS_B200_OK;

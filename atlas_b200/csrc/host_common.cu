@@ -130,10 +130,8 @@ void prof_end(cudaStream_t s, int kind, double work) {
     g_prof_launch.push_back({work, -1});
 }
 
-void prof_end_dyn(cudaStream_t s, int kind, double work_per_row, const int32_t* m_dev, int32_t m_max) {
-    if (g_prof_on != kind || g_prof_used >= g_prof_events.size()) return;
-    cudaEventRecord(g_prof_events[g_prof_used].second, s);
-    ++g_prof_used;
+// the work of the launch just bracketed: work_per_row * *m_dev, copied to a pinned host slot in stream order
+static void dyn_work(cudaStream_t s, double work_per_row, const int32_t* m_dev, int32_t m_max) {
     if (g_prof_rows == nullptr && cudaMallocHost(reinterpret_cast<void**>(&g_prof_rows), PROF_ROW_SLOTS * sizeof(int32_t)) != cudaSuccess)
         g_prof_rows = nullptr;
     const int slot = static_cast<int>(g_prof_dyn.size());
@@ -147,6 +145,39 @@ void prof_end_dyn(cudaStream_t s, int kind, double work_per_row, const int32_t* 
     }
     g_prof_work += work_per_row * m_max;          // no slot: counted at full height
     g_prof_launch.push_back({work_per_row * m_max, -1});
+}
+
+void prof_end_dyn(cudaStream_t s, int kind, double work_per_row, const int32_t* m_dev, int32_t m_max) {
+    if (g_prof_on != kind || g_prof_used >= g_prof_events.size()) return;
+    cudaEventRecord(g_prof_events[g_prof_used].second, s);
+    ++g_prof_used;
+    dyn_work(s, work_per_row, m_dev, m_max);
+}
+
+// sum over the segments of popcount(keep[b, :])^2: the (query tile, key tile) pairs of the packed encoder's attention
+__global__ void tile_pairs_kernel(const uint8_t* __restrict__ keep, int S, int nb, int32_t* __restrict__ pairs) {
+    for (int b = blockIdx.x * blockDim.x + threadIdx.x; b < S; b += gridDim.x * blockDim.x) {
+        int n = 0;
+        for (int t = 0; t < nb; ++t) n += keep[static_cast<size_t>(b) * nb + t] != 0;
+        atomicAdd(pairs, n * n);
+    }
+}
+
+void prof_end_tile_pairs(cudaStream_t s, int kind, double work_per_pair, const uint8_t* keep, int32_t S, int32_t nb) {
+    if (g_prof_on != kind || g_prof_used >= g_prof_events.size()) return;
+    cudaEventRecord(g_prof_events[g_prof_used].second, s);
+    ++g_prof_used;
+    static int32_t* pairs = nullptr;               // one counter, reused in stream order (each count is copied out behind it)
+    if (pairs == nullptr && cudaMalloc(reinterpret_cast<void**>(&pairs), sizeof(int32_t)) != cudaSuccess) pairs = nullptr;
+    if (pairs != nullptr && cudaMemsetAsync(pairs, 0, sizeof(int32_t), s) == cudaSuccess) {
+        tile_pairs_kernel<<<(S + 255) / 256, 256, 0, s>>>(keep, S, nb, pairs);
+        if (cudaGetLastError() == cudaSuccess) {
+            dyn_work(s, work_per_pair, pairs, S * nb * nb);
+            return;
+        }
+    }
+    g_prof_work += work_per_pair * S * nb * nb;    // no count: every tile pair
+    g_prof_launch.push_back({work_per_pair * S * nb * nb, -1});
 }
 
 }  // namespace abh

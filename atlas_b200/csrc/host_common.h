@@ -62,6 +62,9 @@ void prof_begin(cudaStream_t s, int kind);
 void prof_end(cudaStream_t s, int kind, double work);   // work = algorithmic bytes (scan) or FLOPs of this launch
 // ... of a launch whose row count lives in device memory: work = work_per_row * min(m_max, *m_dev), resolved when read
 void prof_end_dyn(cudaStream_t s, int kind, double work_per_row, const int32_t* m_dev, int32_t m_max);
+// ... of a launch over the packed encoder rows (atlas_b200_segment_tile_scan's keep [S, nb]): work = work_per_pair times the
+// (query tile, key tile) pairs of the kept tiles, counted on the device only while `kind` is being measured
+void prof_end_tile_pairs(cudaStream_t s, int kind, double work_per_pair, const uint8_t* keep, int32_t S, int32_t nb);
 
 inline size_t align_up(size_t x, size_t a) { return (x + a - 1) / a * a; }
 

@@ -691,7 +691,10 @@ class FiD(nn.Module):
         return fn(*args)
 
     def _encode_train(self, WG, input_ids, attention_mask):
-        """`encode` with autograd (same kernels forward, un-fused norms; backward = grad_ops)."""
+        """`encode` with autograd (same kernels forward, un-fused norms; backward = grad_ops).  Where the padding-compacted
+        encoder takes the shape (ops.encoder_packs, ops._ENC_PACKED), the stack runs on the packed rows like _encode_rows'
+        and is expanded to the padded layout at the end: the loss and the gradients are the padded step's up to summation
+        order (same dropout masks and draws of dropout keys), the fp16 overflow clamp sees the kept rows only."""
         g = grad_ops
         c = self.config
         W, G, dt = WG
@@ -703,34 +706,54 @@ class FiD(nn.Module):
         d, H = c.d_model, c.num_heads
         eps = c.layer_norm_epsilon
         pdrop = self._dropout_p()
-        h = g.dropout(self._embed_train(W, dt, ids), pdrop)
         add_mask = (1.0 - mask.to(torch.float32)) * -10000.0
-        add_mask._atlas_block_live = ops.key_block_live(add_mask)     # read by grad_ops._SelfAttention (all layers share it)
+        live = ops.key_block_live(add_mask)
+        add_mask._atlas_block_live = live     # read by grad_ops._SelfAttention (all layers share it)
+        bias = bias_by_delta(W["encoder.block.0.layer.0.SelfAttention.relative_attention_bias.weight"], L, L, True,
+                             c.relative_attention_num_buckets)
+        packed = ops._ENC_PACKED and ops.encoder_packs(live, L)
+        row_tiles = None
+        if packed:
+            # the tables once per forward; the row count read to the host once (the step is eager and synchronises for the
+            # loss anyway), so every GEMM, norm and weight gradient runs unchanged on [rows, d]
+            keep, tile_off, tile_src, count = ops.segment_tile_scan(live)
+            rows = int(count.item())
+            row_tiles = tile_src[: rows // 64]                        # padded tile of every packed tile: dropout masks
+            src = (row_tiles.long()[:, None] * 64 + torch.arange(64, device=ids.device)).reshape(-1)
+            h = g.dropout(self._embed_train(W, dt, ids.reshape(-1)[src]), pdrop, row_tiles=row_tiles)
+
+            def attention(qkv, bias):
+                return g.packed_self_attention(qkv, keep, tile_off, S, H, L, add_mask, bias_delta=bias, scale=1.0,
+                                               dropout_p=pdrop)
+        else:
+            h = g.dropout(self._embed_train(W, dt, ids), pdrop)
+
+            def attention(qkv, bias):
+                return g.self_attention(qkv, S, H, L, add_mask=add_mask, bias_delta=bias, scale=1.0, dropout_p=pdrop,
+                                        long_segments=True)
 
         def lin_res(x, w, res):
             # h + dropout(linear(x)) (T5LayerSelfAttention / T5LayerFF); without dropout the add is the GEMM's epilogue;
             # then the fp16 overflow clamp of the block (a no-op for bf16)
             if pdrop:
-                return g.clamp_inf(g.dropout(g.linear(x, w), pdrop, residual=res))
+                return g.clamp_inf(g.dropout(g.linear(x, w), pdrop, residual=res, row_tiles=row_tiles))
             return g.clamp_inf(g.linear(x, w, None, residual=res))
-
-        bias = bias_by_delta(W["encoder.block.0.layer.0.SelfAttention.relative_attention_bias.weight"], L, L, True,
-                             c.relative_attention_num_buckets)
 
         def block(i, h, bias):
             p = f"encoder.block.{i}.layer.0."
             n = g.layernorm(h, W[p + "layer_norm.weight"], None, eps, kind=1)
             qkv = g.linear(n, G[p + "SelfAttention.qkv"])
-            ctx = g.self_attention(qkv, S, H, L, add_mask=add_mask, bias_delta=bias, scale=1.0, dropout_p=pdrop,
-                                   long_segments=True)
-            h = lin_res(ctx, W[p + "SelfAttention.o.weight"], h)
+            h = lin_res(attention(qkv, bias), W[p + "SelfAttention.o.weight"], h)
             p = f"encoder.block.{i}.layer.1."
             n = g.layernorm(h, W[p + "layer_norm.weight"], None, eps, kind=1)
-            return lin_res(g.dropout(self._ff_train(W, G, p, n), pdrop), W[p + "DenseReluDense.wo.weight"], h)
+            return lin_res(g.dropout(self._ff_train(W, G, p, n), pdrop, row_tiles=row_tiles), W[p + "DenseReluDense.wo.weight"],
+                           h)
 
         for i in range(c.num_layers):
             h = self._maybe_ckpt(block, i, h, bias)
-        h = g.dropout(g.layernorm(h, W["encoder.final_layer_norm.weight"], None, eps, kind=1), pdrop)
+        h = g.dropout(g.layernorm(h, W["encoder.final_layer_norm.weight"], None, eps, kind=1), pdrop, row_tiles=row_tiles)
+        if packed:
+            h = g.expand_packed(h, keep, tile_off)       # zeros at the dropped tiles, which the cross-attention masks
         return h.view(bsz, -1, d)
 
     def _decode_train(self, WG, decoder_input_ids, enc, enc_mask):

@@ -112,6 +112,55 @@ def self_attention(qkv, B, H, L, add_mask=None, bias_delta=None, scale=1.0, caus
                                 long_segments)
 
 
+class _PackedSelfAttention(torch.autograd.Function):
+    """qkv [rows, 3*H*64] on the packed rows of the padding-compacted encoder (ops.segment_tile_scan) -> ctx [rows, H*64]."""
+
+    @staticmethod
+    def forward(ctx, qkv, bias_delta, add_mask, keep, tile_off, S, H, L, scale, dropout_p):
+        ctx.drop = (dropout_p,) + next_dropout_key(qkv.device) if dropout_p else None
+        out, lse = ops.attention_packed(qkv, keep, tile_off, S, H, L, add_mask, bias_delta, scale=scale, lse=True,
+                                        dropout=ctx.drop)
+        ctx.save_for_backward(qkv, out, bias_delta, add_mask, keep, tile_off, lse)
+        ctx.dims = (S, H, L, scale)
+        return out
+
+    @staticmethod
+    def backward(ctx, dout):
+        qkv, out, bias_delta, add_mask, keep, tile_off, lse = ctx.saved_tensors
+        S, H, L, scale = ctx.dims
+        dqkv, dbias = ops.attention_packed_bwd(qkv, out, dout.contiguous(), keep, tile_off, S, H, L, add_mask, bias_delta, lse,
+                                               scale=scale, need_dbias=bias_delta is not None and _need(ctx, 1),
+                                               dropout=ctx.drop)
+        return dqkv, dbias, None, None, None, None, None, None, None, None
+
+
+def packed_self_attention(qkv, keep, tile_off, S, H, L, add_mask, bias_delta=None, scale=1.0, dropout_p=0.0):
+    """`self_attention` of segments of L tokens on their packed rows (keep / tile_off: ops.segment_tile_scan); the same
+    dropout masks, draw of the dropout key and gradients on the kept rows as the padded layout's."""
+    return _PackedSelfAttention.apply(qkv, bias_delta, add_mask, keep, tile_off, S, H, L, scale, float(dropout_p or 0.0))
+
+
+class _ExpandPacked(torch.autograd.Function):
+    """Packed rows [rows, d] -> the padded layout [n_tiles * 64, d], zeros at the dropped tiles; backward: the gradient rows of
+    the kept tiles, packed again (ops.compact_live_tiles over keep, the same tile order)."""
+
+    @staticmethod
+    def forward(ctx, x, keep, tile_off):
+        ctx.save_for_backward(keep)
+        ctx.rows = x.shape[0]
+        return ops.expand_packed_tiles(x, tile_off)
+
+    @staticmethod
+    def backward(ctx, dy):
+        (keep,) = ctx.saved_tensors
+        dx, _, _ = ops.compact_live_tiles(dy.contiguous(), keep)
+        return dx[: ctx.rows], None, None
+
+
+def expand_packed(x, keep, tile_off):
+    return _ExpandPacked.apply(x, keep, tile_off)
+
+
 class _CrossAttention(torch.autograd.Function):
     """q [B*T, H*64], kv [B*Lk, 2*H*64] (k | v) -> ctx [B*T, H*64]; forward = split-KV kernel + combine."""
 
@@ -157,24 +206,26 @@ class _Dropout(torch.autograd.Function):
     """y = (residual +) dropout(x) (nn.Dropout on hidden states, training mode); masks re-derived in the backward."""
 
     @staticmethod
-    def forward(ctx, x, residual, p):
+    def forward(ctx, x, residual, p, row_tiles):
         ctx.key = next_dropout_key(x.device)
         ctx.p = p
         ctx.has_res = residual is not None
-        return ops.dropout(x, p, ctx.key[0], ctx.key[1], residual=residual)
+        ctx.row_tiles = row_tiles
+        return ops.dropout(x, p, ctx.key[0], ctx.key[1], residual=residual, row_tiles=row_tiles)
 
     @staticmethod
     def backward(ctx, dy):
         dy = dy.contiguous()
-        dx = ops.dropout(dy, ctx.p, ctx.key[0], ctx.key[1]) if _need(ctx, 0) else None
-        return dx, (dy if (ctx.has_res and _need(ctx, 1)) else None), None
+        dx = ops.dropout(dy, ctx.p, ctx.key[0], ctx.key[1], row_tiles=ctx.row_tiles) if _need(ctx, 0) else None
+        return dx, (dy if (ctx.has_res and _need(ctx, 1)) else None), None, None
 
 
-def dropout(x, p, residual=None):
-    """(residual +) dropout(x) with rate p; p == 0 is the identity (plus the residual add)."""
+def dropout(x, p, residual=None, row_tiles=None):
+    """(residual +) dropout(x) with rate p; p == 0 is the identity (plus the residual add).  row_tiles: x holds packed rows
+    (ops.dropout), which take the masks of their padded rows."""
     if not p:
         return x if residual is None else x + residual
-    return _Dropout.apply(x, residual, float(p))
+    return _Dropout.apply(x, residual, float(p), row_tiles)
 
 
 class _ClampInf(torch.autograd.Function):

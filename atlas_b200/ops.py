@@ -822,10 +822,14 @@ _ENC_PACKED = os.environ.get("ATLAS_B200_ENC_PACKED", "1") != "0"          # A/B
 _BERT_PACKED = os.environ.get("ATLAS_B200_BERT_PACKED", "1") != "0"        # ... of the Contriever encoder (needs _ENC_PACKED too)
 
 
+PACKED_MAX_L = ATTENTION_MAX_LK     # segment length limit of the padding-compacted encoder (attention_packed)
+
+
 def encoder_packs(live, L):
-    """Whether the padding-compacted encoder takes segments of L tokens with the live 64-key blocks `live`
-    (key_block_live): there is a mask, the segments are whole 64-row tiles, and at most 384 tokens long."""
-    return live is not None and L % 64 == 0 and 64 <= L <= 384
+    """Whether the padding-compacted encoder (no-grad and training) takes segments of L tokens with the live 64-key blocks
+    `live` (key_block_live): there is a mask, the segments are whole 64-row tiles, and at most PACKED_MAX_L tokens long.
+    Longer segments run padded, on attention_long."""
+    return live is not None and L % 64 == 0 and 64 <= L <= PACKED_MAX_L
 
 
 def segment_tile_scan(live):
@@ -861,17 +865,44 @@ def embed_packed_tiles(ids, table, tile_src):
     return out
 
 
-def attention_packed(qkv, keep, tile_off, S, H, L, add_mask, bias_delta, scale=1.0, out=None):
-    """Encoder self-attention on the packed rows (segment s = its kept tiles, back to back): atlas_b200_attention_packed."""
+def attention_packed(qkv, keep, tile_off, S, H, L, add_mask, bias_delta, scale=1.0, out=None, lse=False, dropout=None):
+    """Encoder self-attention on the packed rows (segment s = its kept tiles, back to back): atlas_b200_attention_packed.
+    lse: also return the row log-sum-exp [S, H, L] fp32 in the padded layout (kept rows written), for attention_packed_bwd.
+    dropout = (p, seed, offset): dropout on the probabilities with the padded layout's masks."""
     require_cuda(qkv, "qkv")
     if out is None:
         out = torch.empty((qkv.shape[0], H * 64), dtype=qkv.dtype, device=qkv.device)
     am = add_mask.float().contiguous()
     bd = bias_delta.float().contiguous() if bias_delta is not None else None
+    lse_t = torch.empty((S, H, L), dtype=torch.float32, device=qkv.device) if lse else None
+    dp, dseed, doff = dropout if dropout is not None else (0.0, 0, 0)
     check(lib().atlas_b200_attention_packed(_ptr(qkv), qkv.stride(0), 0, H * 64, 2 * H * 64, _ptr(out), out.stride(0), _ptr(am),
                                             _ptr(bd) if bd is not None else None, _ptr(keep), _ptr(tile_off), S, H, L,
-                                            float(scale), _bf(qkv), current_stream_ptr()))
-    return out
+                                            float(scale), _ptr(lse_t) if lse else None, float(dp), int(dseed), int(doff),
+                                            _bf(qkv), current_stream_ptr()))
+    return (out, lse_t) if lse else out
+
+
+def attention_packed_bwd(qkv, out, dout, keep, tile_off, S, H, L, add_mask, bias_delta, lse, scale=1.0, need_dbias=False,
+                         dropout=None):
+    """Backward of `attention_packed(..., lse=True)` (atlas_b200_attention_packed_bwd) -> (dqkv like qkv: dq | dk | dv at the
+    columns of q | k | v, dbias_delta fp32 [H, 2L - 1] or None)."""
+    require_cuda(qkv, "qkv")
+    if lse is None:
+        raise AtlasB200Error("attention_packed_bwd: needs the forward's log-sum-exp (lse, from lse=True)")
+    am = add_mask.float().contiguous()
+    bd = bias_delta.float().contiguous() if bias_delta is not None else None
+    dbias = torch.zeros((H, 2 * L - 1), dtype=torch.float32, device=qkv.device) if (need_dbias and bd is not None) else None
+    dsum = torch.empty((S, H, L), dtype=torch.float32, device=qkv.device)
+    dqkv = torch.empty_like(qkv)
+    o2, do2 = _rows2d(out), _rows2d(dout)
+    dp, dseed, doff = dropout if dropout is not None else (0.0, 0, 0)
+    check(lib().atlas_b200_attention_packed_bwd(_ptr(qkv), qkv.stride(0), _ptr(o2), o2.stride(0), _ptr(do2), do2.stride(0),
+                                                _ptr(dqkv), dqkv.stride(0), _ptr(am), _ptr(bd) if bd is not None else None,
+                                                _ptr(dbias) if dbias is not None else None, _ptr(lse.contiguous()), _ptr(dsum),
+                                                _ptr(keep), _ptr(tile_off), S, H, L, float(scale), float(dp), int(dseed),
+                                                int(doff), _bf(qkv), current_stream_ptr()))
+    return dqkv, dbias
 
 
 def expand_packed_tiles(x, tile_off):
@@ -1065,16 +1096,23 @@ def gelu_erf(z, dy=None):
     return out.reshape(z.shape)
 
 
-def dropout(x, p, seed, offset, residual=None):
+def dropout(x, p, seed, offset, residual=None, row_tiles=None):
     """out = (residual +) dropout(x): keep decisions are a pure function of (seed, offset, position), so calling this on
-    dy with the same (seed, offset) is the backward of the forward call (csrc/dropout.cu)."""
+    dy with the same (seed, offset) is the backward of the forward call (csrc/dropout.cu).  row_tiles (int32, one entry per
+    64 rows): x holds the packed rows of the padding-compacted encoder, row r takes the mask of padded row
+    64 row_tiles[r // 64] + r % 64 (segment_tile_scan's tile_src)."""
     require_cuda(x, "x")
     x2 = _rows2d(x)
     r2 = _rows2d(residual) if residual is not None else None
+    if row_tiles is not None and (row_tiles.dtype != torch.int32 or row_tiles.device != x.device
+                                  or x2.shape[0] % 64 or row_tiles.numel() < x2.shape[0] // 64):
+        raise AtlasB200Error(f"dropout: row_tiles must be int32 on {x.device} with one entry per 64 of the {x2.shape[0]} rows")
+    rt = row_tiles.contiguous() if row_tiles is not None else None
     out = torch.empty_like(x2)
     check(lib().atlas_b200_dropout(_ptr(x2), x2.stride(0), _ptr(r2) if r2 is not None else None,
                                    r2.stride(0) if r2 is not None else 0, _ptr(out), out.stride(0), x2.shape[0],
-                                   x2.shape[1], float(p), int(seed), int(offset), _bf(x), current_stream_ptr()))
+                                   x2.shape[1], float(p), int(seed), int(offset), _ptr(rt) if rt is not None else None,
+                                   _bf(x), current_stream_ptr()))
     return out.reshape(x.shape)
 
 

@@ -630,12 +630,15 @@ int atlas_b200_cross_entropy_bwd(const void* logits, int64_t ld, const int64_t* 
 /* nn.Dropout on 16-bit hidden states in the TRAINING path (src/modeling_t5.py:266,286,310,561,960,1070;
  * src/modeling_bert.py:222,378,459):  out = (residual +) r16(keep ? x / (1 - p) : 0).  The keep decisions are a pure
  * function of (seed, offset, element position) - Philox4x32-7, 16-bit uniforms, realised drop rate round(p * 65536) / 65536
- * (csrc/dropout.cuh) - so the backward of y = dropout(x) is the same call on dy with the same (seed, offset).
+ * (csrc/dropout.cuh) - so the backward of y = dropout(x) is the same call on dy with the same (seed, offset).  row_tiles
+ * (NULL: row r is row r): the rows are the packed rows of the padding-compacted encoder, row r is keyed as the padded row
+ * 64 row_tiles[r / 64] + r % 64 (atlas_b200_segment_tile_scan's tile_src; M must be a multiple of 64).
  * atlas_b200_dropout_mask / atlas_b200_attention_dropout_mask export the keep masks (1 byte per element) of the
  * elementwise layout ([M, N]) and of the attention-probability layout ([B * H * Lq, Lk], see atlas_b200_attention_train)
  * for the parity tests. */
 int atlas_b200_dropout(const void* x, int64_t ldx, const void* residual, int64_t ldr, void* out, int64_t ldo, int64_t M,
-                       int32_t N, float p, uint64_t seed, uint64_t offset, int32_t is_bf16, void* stream);
+                       int32_t N, float p, uint64_t seed, uint64_t offset, const int32_t* row_tiles, int32_t is_bf16,
+                       void* stream);
 int atlas_b200_dropout_mask(uint8_t* out, int64_t M, int32_t N, float p, uint64_t seed, uint64_t offset, void* stream);
 int atlas_b200_attention_dropout_mask(uint8_t* out, int64_t rows, int32_t Lk, float p, uint64_t seed, uint64_t offset,
                                       void* stream);
@@ -712,11 +715,12 @@ int atlas_b200_cross_attention_stream_compact(const void* q, int64_t ldq, int32_
                                               int32_t chunk, float scale, float* o_partial, float* ml_partial, int32_t is_bf16,
                                               void* stream);
 
-/* Padding-compacted FiD encoder (inference forward, fid.py: FiD.encode_packed).  The reference encodes every passage padded to
- * text_maxlength (src/atlas.py:261-270, src/fid.py:32-78) and masks the padding keys; a padded position never influences a live
- * one (its softmax weight is exactly 0, every other encoder op is row-wise) and the decoder's cross-attention masks it too, so
- * the encoder runs on the 64-row tiles up to each segment's last live key only, packed back to back.  Static launch shapes:
- * the packed row count lives in device memory.
+/* Padding-compacted FiD encoder (no-grad forward: fid.py FiD._encode_rows; training step: FiD._encode_train), for
+ * text_maxlength L a multiple of 64 up to 576.  The reference encodes every passage padded to text_maxlength (src/atlas.py:261-270,
+ * src/fid.py:32-78) and masks the padding keys; a padded position never influences a live one (its softmax weight is exactly 0,
+ * every other encoder op is row-wise) and the decoder's cross-attention masks it too (so its gradients are exactly 0), so the
+ * encoder runs on the 64-row tiles up to each segment's last live key only, packed back to back.  Static launch shapes: the
+ * packed row count lives in device memory (the training step reads it to the host once per forward).
  *   atlas_b200_segment_tile_scan: live uint8 [S, nb] (key_block_live) -> keep [S, nb] (tiles 0 .. last live tile of the segment;
  *     all nb if none is live), tile_off int32 [S * nb] (packed index of a kept tile, -1 = dropped), tile_src int32 [S * nb] (source
  *     tile of packed tile o, -1 past the end), *count_rows = 64 x #kept.
@@ -725,7 +729,14 @@ int atlas_b200_cross_attention_stream_compact(const void* q, int64_t ldq, int32_
  *   The projections run on atlas_b200_linear_rows with m_dev = count_rows.
  *   atlas_b200_attention_packed: T5Attention.forward (src/modeling_t5.py:478-524) of the encoder on the packed rows: segment b =
  *     rows [64 tile_off[b * nb], + 64 popcount(keep[b, :])) of qkv / out; add_mask [B, L] and bias_delta [H, 2L - 1] as in
- *     atlas_b200_attention_train (positions are those of the padded layout: kept tiles are a prefix of the segment).
+ *     atlas_b200_attention_train (positions are those of the padded layout: kept tiles are a prefix of the segment).  lse_out
+ *     (or NULL): the row log-sum-exp [B, H, L] in the padded layout, written for the kept rows; dropout_p / seed / offset: dropout
+ *     on the probabilities with the masks of atlas_b200_attention_train on the padded layout (row (b H + h) L + i, key j).
+ *     L <= 384 without lse_out and dropout runs a persistent kernel; otherwise the resident kernel of atlas_b200_attention_train.
+ *   atlas_b200_attention_packed_bwd: its backward, the contract of atlas_b200_attention_bwd_train for self-attention: lse
+ *     (required, only read) and dsum scratch [B, H, L] in the padded layout, dbias_delta [H, 2L - 1] incremented (or NULL), the
+ *     dropout masks re-derived, dropped tiles never touched.  qkv / dqkv hold q | k | v and dq | dk | dv at columns 0, 64 H and
+ *     128 H; out / dout are the forward's output and its gradient.
  *   atlas_b200_expand_packed_tiles: back to the padded layout [S * nb * 64, d] (zeros at dropped tiles - the positions the
  *     reference fills with values nothing reads).
  * embed_packed_tiles, expand_packed_tiles and compact_live_tiles move 16-byte vectors: d and the row strides are multiples of 8
@@ -736,7 +747,13 @@ int atlas_b200_embed_packed_tiles(const int64_t* ids, const void* table, int64_t
                                   int32_t n_tiles, void* dst, int64_t ldd, int32_t d, void* stream);
 int atlas_b200_attention_packed(const void* qkv, int64_t ld, int32_t q_col0, int32_t k_col0, int32_t v_col0, void* out, int64_t ldo,
                                 const float* add_mask, const float* bias_delta, const uint8_t* keep, const int32_t* tile_off,
-                                int32_t B, int32_t H, int32_t L, float scale, int32_t is_bf16, void* stream);
+                                int32_t B, int32_t H, int32_t L, float scale, float* lse_out, float dropout_p, uint64_t seed,
+                                uint64_t offset, int32_t is_bf16, void* stream);
+int atlas_b200_attention_packed_bwd(const void* qkv, int64_t ld, const void* out, int64_t ldo, const void* dout, int64_t lddo,
+                                    void* dqkv, int64_t ldd, const float* add_mask, const float* bias_delta, float* dbias_delta,
+                                    const float* lse, float* dsum, const uint8_t* keep, const int32_t* tile_off, int32_t B,
+                                    int32_t H, int32_t L, float scale, float dropout_p, uint64_t seed, uint64_t offset,
+                                    int32_t is_bf16, void* stream);
 int atlas_b200_expand_packed_tiles(const void* src, int64_t lds, const int32_t* tile_off, int32_t n_tiles, void* dst, int64_t ldd,
                                    int32_t d, void* stream);
 
